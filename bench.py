@@ -4,6 +4,7 @@
     python bench.py [--gpus N --steps K --warmup W]            the headline line (below)
     python bench.py --impl reference ...                        the reference arm: CPU oracle on all host cores
     python bench.py --workload clip|c4|c5 ...                   the other BASELINE.json configs as their own line
+    python bench.py ... --dump-outputs DIR                      also write what the last timed step computed, DIR/<name>.npy
 
 Headline workload at N GPUs: YOLOv9-c, 32 synthetic 640x640x3 uint8 BGR frames per GPU per step (BASELINE.json
 configs[1], weak scaling: frames shard by batch, no data-path collective), whole path = stem(/255,BGR flip) -> 144 convs
@@ -12,7 +13,7 @@ configs[1], weak scaling: frames shard by batch, no data-path collective), whole
   value     : frames/s with the uint8 frames already resident in HBM (rotating through > L2-size worth of inputs)
   e2e       : frames/s through the public API (YOLOv9.detect_pipelined) from PINNED HOST frames, H2D and the D2H read
               of the (B,300,6) result inside the timed region
-  roofline  : conv_gemm_kernel (tcgen05) = algorithmic conv FLOPs per step / summed device time of its launches inside a
+  roofline  : conv_gemm_kernel (wgmma) = algorithmic conv FLOPs per step / summed device time of its launches inside a
               plain forward (the kernels' own globaltimer stamps, cc_yolo_trace: no events between launches, PDL overlap as
               in the timed region), against MEASURED_PEAKS.json sustained bf16 peak; `frac_events` is the same with every
               launch bracketed by CUDA events (cc_yolo_profile: serialised, launch latency exposed)
@@ -59,7 +60,8 @@ def peaks():
         return {"tflops": p["bf16_tflops"], "tflops_sustained": p.get("bf16_tflops_sustained", p["bf16_tflops"]),
                 "hbm": p["hbm_gbs"], "src": "measured"}
     except Exception:
-        return {"tflops": 1590.0, "tflops_sustained": 1400.0, "hbm": 6650.0, "src": "fallback"}
+        # NVIDIA's H100 SXM data sheet (dense bf16, HBM3), a card allowed 700 W: an upper bound, never a measured rate
+        return {"tflops": 989.0, "tflops_sustained": 989.0, "hbm": 3350.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -104,6 +106,18 @@ class ClockSampler:
                     reasons.add(n)
         sm.sort()
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def dump_outputs(args, name, t):
+    """--dump-outputs: one array the timed path returned, as DIR/<name>.npy (float32, or float64 when computed so)."""
+    if not args.dump_outputs:
+        return
+    import numpy as np
+    t = torch.as_tensor(getattr(t, "tensor", t))
+    t = t.detach().cpu()
+    t = t.double() if t.dtype == torch.float64 else t.float()
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    np.save(os.path.join(args.dump_outputs, name + ".npy"), t.numpy())
 
 
 def make_weights(size=SIZE, hw=HW):
@@ -337,7 +351,7 @@ def yolo_section(cx, with_cpu):
     B, W, K = args.batch, max(args.warmup, 3), args.steps
     P = make_weights()
     model = YOLOv9(SIZE, RES, weights=P)
-    # > L2 (126 MB) worth of distinct device-resident input batches, rotated between steps
+    # > L2 (50 MB) worth of distinct device-resident input batches, rotated between steps
     nbuf = max(2, int(160e6 // (B * HW * HW * 3)) + 1)
     base = o.synthetic_frames(4, HW, HW, seed=100 + rank)
     g = torch.Generator(device="cuda").manual_seed(rank)
@@ -356,8 +370,11 @@ def yolo_section(cx, with_cpu):
     sampler = ClockSampler(cx.local)
     if rank == 0:
         sampler.start()
-    ms_total = cx.timed(lambda i: model.detect_batch(dev_batches[i % nbuf]), K)
+    last = {}
+    ms_total = cx.timed(lambda i: last.__setitem__("det", model.detect_batch(dev_batches[i % nbuf])), K)
     clocks = sampler.stop() if rank == 0 else None
+    if rank == 0:
+        dump_outputs(args, "yolo_detections", last["det"])          # (B, 300, 6) of the last timed step
     value = world * B * K / (ms_total / 1000.0)
 
     # ---- end to end through the public API from pinned host memory
@@ -419,11 +436,11 @@ def yolo_section(cx, with_cpu):
         # launches), read from globaltimer stamps the kernels write: per launch, last CTA exit - grid dependency released.  That
         # is what ncu's gpu__time_duration measures per launch, but warm and overlapped as in the timed region.
         # `frac_events` is the older figure: every launch bracketed by its own CUDA events, which serialises the stream and adds
-        # the ~8 us launch latency to each of the 125 launches.
+        # a launch latency to each launch.
         roof = {"bound": "tensor", "kernel": "conv_gemm_kernel", "achieved": in_situ_tf, "peak": pk["tflops_sustained"],
                 "unit": "TFLOP/s", "frac": in_situ_tf / pk["tflops_sustained"], "peak_src": pk["src"] + " (sustained bf16)",
                 "how": "in-situ: globaltimer stamps written by the conv kernels (dependency released -> last CTA exit) during a plain forward, summed over the launches of a step",
-                # DRAM bytes are not measurable without a profiler: see profiles/ for the ncu launch list of this command
+                # DRAM bytes are not measurable without a hardware profiler
                 "traffic": None, "algorithmic_bytes": sum(r["bytes"] for r in prof if r["kind"] == "conv_gemm") / max(gm["n"], 1),
                 "launches": gm["n"], "share_of_step": work_ms / (ms_total / K),
                 "in_situ": {"conv_work_ms": work_ms, "first_conv_to_last_conv_ms": span_ms},
@@ -443,7 +460,7 @@ def yolo_section(cx, with_cpu):
                 "dtype": "bf16", "data": "synthetic",
                 "config": {"workload": YOLO_WORKLOAD if B == BATCH else YOLO_WORKLOAD.replace(f"{BATCH} uint8", f"{B} uint8"),
                            "global_batch": world * B, "res": RES, "weights": "seeded synthetic",
-                           "l2": f"{nbuf} rotating input batches ({nbuf * B * HW * HW * 3 / 1e6:.0f} MB) + {info['act_bytes'] / 1e9:.1f} GB activations per step (> 126 MB L2)",
+                           "l2": f"{nbuf} rotating input batches ({nbuf * B * HW * HW * 3 / 1e6:.0f} MB) + {info['act_bytes'] / 1e9:.1f} GB activations per step (> 50 MB L2)",
                            "parallelism": f"dp{world} (frames sharded by batch, no collective)"},
                 "clocks": clocks,
                 "e2e": {"value": e2e, "unit": "frames/s", "h2d_bytes_per_step": B * HW * HW * 3, "d2h_bytes_per_step": B * 300 * 6 * 4},
@@ -475,8 +492,12 @@ def clip_section(cx, with_cpu, archs=(("ViT-B/32", 256), ("ViT-L/14", 256))):
         xs = [oc.synthetic_images(8, cfg.image_size, seed=10 + i)[torch.arange(cb) % 8].cuda() for i in range(3)]
         for i in range(3):
             cm.precompute_embedding(xs[i % 3], gather=world > 1)
-        steps_c = max(3, min(K, 10))
-        ms = cx.timed(lambda i: cm.precompute_embedding(xs[i % 3], gather=world > 1), steps_c)
+        steps_c = K
+        last = {}
+        ms = cx.timed(lambda i: last.__setitem__("img", cm.precompute_embedding(xs[i % 3], gather=world > 1)), steps_c)
+        tag = arch.replace("/", "").replace("-", "_")
+        if rank == 0:
+            dump_outputs(cx.args, f"clip_{tag}_image_embeddings", last["img"])
         ips = world * cb * steps_c / (ms / 1000.0)
         r = {"batch_per_gpu": cb, "value": ips, "unit": "images/s", "ms_per_step": ms / steps_c,
              "tflops": ips * oc.flops_image(cfg) / 1e12, "gflop_per_image": oc.flops_image(cfg) / 1e9, "all_gather": world > 1}
@@ -509,7 +530,9 @@ def clip_section(cx, with_cpu, archs=(("ViT-B/32", 256), ("ViT-L/14", 256))):
         ids = oc.pad_tokens([torch.randint(1000, 40000, (int(n),), generator=g).tolist() for n in torch.randint(3, 20, (qb,), generator=g)]).int().cuda()
         for _ in range(2):
             cm.encode_token_ids(ids)
-        ms = cx.timed(lambda i: cm.encode_token_ids(ids), steps_c)
+        ms = cx.timed(lambda i: last.__setitem__("txt", cm.encode_token_ids(ids)), steps_c)
+        if rank == 0:
+            dump_outputs(cx.args, f"clip_{tag}_text_embeddings", last["txt"])
         r["text"] = {"batch_per_gpu": qb, "queries_per_s": world * qb * steps_c / (ms / 1000.0),
                      "tflops": world * qb * steps_c / (ms / 1000.0) * oc.flops_text(cfg) / 1e12}
         if rank == 0:
@@ -569,11 +592,13 @@ def c4_section(cx):
     emb_local = torch.zeros(max(1, len(mine)) * MAXC, fin.model.embed_dim, device="cuda")
     emb_all = torch.zeros(world * emb_local.shape[0], fin.model.embed_dim, device="cuda") if world > 1 else None
     counts = {"frames": 0, "crops": 0}
+    last = {}
 
     def step(t):
         for j, c in enumerate(mine):
             boxes[c].fill(io.BytesIO(feeds[j][t % 3]))                      # the ingest thread's job: bytes -> pinned slot
         res = cb.step_mailboxes(boxes)
+        last["res"] = res
         emb_local.zero_()
         row = 0
         for c, r in res.items():
@@ -593,8 +618,12 @@ def c4_section(cx):
     for t in range(3):
         step(t)
     counts["frames"] = counts["crops"] = 0
-    K = max(5, min(cx.args.steps, 20))
+    K = cx.args.steps
     ms = cx.timed(step, K)
+    if rank == 0:       # the last step's tracks per camera of this rank, and the (gathered) crop embeddings
+        for c, r in last["res"].items():
+            dump_outputs(cx.args, f"c4_cam{c}_tracks", r.rows)
+        dump_outputs(cx.args, "c4_embeddings", emb_all if world > 1 else emb_local)
     tot = torch.tensor([counts["frames"], counts["crops"]], device="cuda", dtype=torch.float64)
     if world > 1:
         cx.dist.all_reduce(tot)
@@ -625,17 +654,22 @@ def c5_section(cx):
     rects = [(f, 40 + 10 * f, 60, 40 + 10 * f + 300, 60 + 360) for f in range(B)] + [(f, 200, 100 + 5 * f, 520, 420 + 5 * f) for f in range(B)]
     full = torch.empty(world * 2 * B, fin.model.embed_dim, device="cuda")
 
+    last = {}
+
     def step(i):
         fb = batches[i % len(batches)]
-        model.detect_batch(fb)
+        last["det"] = model.detect_batch(fb)
         x = fin.preprocess_device(fb, rects)
         fin.model.embed_into(x, full, rank * 2 * B)
         if world > 1:
             cx.dist.all_gather_into_tensor(full, full[rank * 2 * B:(rank + 1) * 2 * B])
     for i in range(3):
         step(i)
-    K = max(5, min(cx.args.steps, 20))
+    K = cx.args.steps
     ms = cx.timed(step, K)
+    if rank == 0:
+        dump_outputs(cx.args, "c5_detections", last["det"])
+        dump_outputs(cx.args, "c5_embeddings", full)
     fps = world * B * K / (ms / 1000.0)
     out = {"workload": f"YOLOv9-e, {B} uint8 640x640 frames per GPU per step ({world * B} in total) + ViT-B/32 embeddings of {2 * B} crops per GPU + all-gather",
            "scaling": "weak", "steps": K, "ms_per_step": ms / K, "frames_per_s": fps, "crops_per_s": 2 * fps,
@@ -656,6 +690,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline legs")
     ap.add_argument("--no-clip", action="store_true", help="headline line without the clip object")
     ap.add_argument("--extras", action="store_true", help="add the c4 and c5 objects to the headline line (default when N > 1)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write the arrays the last timed step returned as DIR/<name>.npy")
     ap.add_argument("--cpu-worker", default=None, help=argparse.SUPPRESS)
     ap.add_argument("--threads", type=int, default=16, help=argparse.SUPPRESS)
     ap.add_argument("--sync-dir", default="", help=argparse.SUPPRESS)
@@ -691,13 +727,13 @@ def main():
         if cx.rank == 0:
             b = r["ViT-B/32"]
             line = {"metric": "images/s CLIP ViT-B/32 224px", "value": b["value"], "unit": "images/s", "n_gpus": cx.world,
-                    "steps": max(3, min(args.steps, 10)), "warmup": 3, "ms_per_step": b["ms_per_step"], "higher_is_better": True,
+                    "steps": args.steps, "warmup": 3, "ms_per_step": b["ms_per_step"], "higher_is_better": True,
                     "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
                     "config": {"workload": CLIP_WORKLOAD, "global_batch": cx.world * 256, "weights": "seeded synthetic",
-                               "l2": "3 rotating input batches of 154 MB (> 126 MB L2)",
+                               "l2": "3 rotating input batches of 154 MB (> 50 MB L2)",
                                "parallelism": f"dp{cx.world} (crops sharded by batch; in-place all-gather of the embeddings when N > 1)"},
                     "e2e": b["e2e"], "roofline": b.get("roofline"), "cpu_baseline": b.get("cpu_baseline"), "text": b["text"],
-                    "gpu_launches": b.get("launches_per_step", 0) * max(3, min(args.steps, 10)), "ViT-L/14": r["ViT-L/14"]}
+                    "gpu_launches": b.get("launches_per_step", 0) * args.steps, "ViT-L/14": r["ViT-L/14"]}
     else:
         r = (c4_section if args.workload == "c4" else c5_section)(cx)
         if cx.rank == 0:

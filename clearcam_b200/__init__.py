@@ -1,2 +1,2 @@
-"""clearcam_b200 — B200-native (sm_100a) YOLOv9 + CLIP hot path behind the reference's Python signatures."""
+"""clearcam_b200 — H100-native (sm_90a) YOLOv9 + CLIP hot path behind the reference's Python signatures."""
 from ._lib import CCError, lib, LIB_PATH  # noqa: F401

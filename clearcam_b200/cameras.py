@@ -2,7 +2,7 @@
 
 The reference walks its cameras round-robin and runs the detector on one frame at a time (`VideoCapture.start`,
 clearcam.py:270-271 -> `process_frame` :423-461 -> `run_inference` :580-586: Tensor(frame) -> jit_infer(model) ->
-.numpy() -> tracker.update).  On a B200 a single 1080p frame leaves the GPU mostly idle, so `CameraBatch.step` takes the
+.numpy() -> tracker.update).  On an H100 a single 1080p frame leaves the GPU mostly idle, so `CameraBatch.step` takes the
 latest frame of every camera, groups the frames by shape (cameras differ in resolution; the detector's letterbox plan is
 per input shape), runs ONE `detect_batch` per group with uploads and result reads queued back to back, waits once, and
 then steps every camera's tracker in one library call.  What comes back per camera is what `run_inference` computes up

@@ -1,52 +1,38 @@
-// Multi-head attention on tcgen05 (sm_100a), d_head = 64:  ctx = softmax(Q K^T / 8 [+ causal mask]) V per (image, head).
-// Reference: models/objects.py:108-118 (image tower), :157-168 (text tower, causal).
+// Multi-head attention on Hopper warpgroup MMA (sm_90a), d_head = 64:  ctx = softmax(Q K^T / 8 [+ causal mask]) V per
+// (image, head).  Reference: models/objects.py:108-118 (image tower), :157-168 (text tower, causal).
 //
-// One CTA per (group of G consecutive images, head): the tokens of the G images are one packed sequence of G*L rows (they are
-// consecutive rows of the QKV buffer) with a block-diagonal mask — a query row attends the keys of its own image only.  Short
-// sequences (ViT-B/32: 50 tokens, text: 77) fill the 128-row MMA blocks this way (G = 5 -> 250 of 256 rows, G = 3 -> 231 of
-// 256) and share one TMEM allocation / barrier set-up / K,V load per CTA; the long one (ViT-L/14: 257) runs with G = 1.
-// Softmax work is NOT wasted on the mask: a row reads and exponentiates only its own image's key columns.
-// K and V^T of the group are TMA-loaded once, then the CTA walks the 128-query blocks:
-//   S[128 x Lk]  = Q[128 x 64] . K[Lk x 64]^T      tcgen05.mma, accumulators in TMEM columns [0, Lk)
-//   softmax      : 4 warps, thread == query row, two passes over TMEM (row max, then exp2/sum); P (bf16, unnormalised,
-//                  <= 1) is written straight into the 128B-swizzled K-major layout the second MMA reads as its A operand
-//   O[128 x 64]  = P[128 x Lk] . Vt[64 x Lk]^T     tcgen05.mma, accumulators in the 64 TMEM columns after S
-//   ctx          = O / rowsum  -> bf16
-// V is consumed as a K-major B operand, so a small pre-pass writes V^T per head ([B*H*64, Lk], keys contiguous,
-// zero padded to Lk = ceil(L/64)*64); Q and K are read in place from the fused QKV buffer through one 2-D tensor map.
+// One CTA = one warpgroup = 64 query rows of one (image, head).  Q, the K rows and a V^T copy of the keys it needs are
+// TMA-loaded once (128B-swizzled, K-major), then the warpgroup walks 64-key blocks with an online softmax (flash):
+//   S[64 x 64]  = Q[64 x 64] . K_j[64 x 64]^T     wgmma, both operands from shared memory, fp32 accumulators in registers
+//   softmax     : row max / rescale / exp2 on the accumulator fragments (a row lives in the four lanes of a quad)
+//   O[64 x 64] += P_j[64 x 64] . Vt_j[64 x 64]^T  wgmma with P straight from registers (the S fragment, rounded to bf16)
+//   ctx         = O / rowsum -> bf16
+// V is consumed as a K-major B operand, so a small pre-pass writes V^T per head ([B*H*64, Lk], keys contiguous, zero
+// padded to Lk = ceil(L/64)*64); Q and K are read in place from the fused QKV buffer through one 2-D tensor map.
 #include "ops.cuh"
 #include "cc_common.h"
 #include "cc_ptx.cuh"
+#include <math.h>
 #include <stdlib.h>
 
 namespace cc {
 
-static constexpr int kMaxLk = 384;   // S uses TMEM columns [0, Lk), O the 64 columns after it (Lk + 64 <= 512); shared memory holds K, V^T, P for 384 keys
+static constexpr int kMaxLk = 384;   // shared memory holds K and V^T of up to 384 keys (2 x 48 KB)
 
 struct AttnParams {
   CUtensorMap tmQK;   // qkv viewed as [B*L rows][3W cols], box 64 rows x 64 cols
   CUtensorMap tmVt;   // Vt [B*H*64 rows][Lk cols], box 64 rows x 64 cols
-  const __nv_bfloat16* qkv;
   __nv_bfloat16* ctx;
-  int B, L, Lk, H, W, causal;
-  int nq;          // Q buffers (2 where shared memory allows: both query blocks of a 257-token sequence are loaded up front)
-  int vmajor;      // 1: V is read in place from the QKV buffer ([key][64 d] tiles = an MN-major B operand); 0: from the V^T pre-pass
-  unsigned long long* trace;   // diagnostic (CC_ATTN_TRACE=1): SM-cycle stamps of CTA 0, see attention_tc_launch
-  int tail;        // 1: one image per CTA and L = 128 n + 1 -> the last token runs on CUDA cores (warp 9)
-  int G;           // images per CTA (packed sequence of G*L tokens, Lk = ceil(G*L / 64) * 64 key columns)
-  int tmem_cols;   // power of two >= Lk + 64
+  int L, Lk, H, W, causal;
 };
 
 // ---------------------------------------------------------------- V^T pre-pass
-// (L here = tokens of one group = G * tokens per image; the last group of a batch may hold fewer: Ltot bounds the rows)
-__global__ void __launch_bounds__(256) vt_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ vt, int Lg,
-                                                 long long Ltot, int Lk, int H, int W) {
+__global__ void __launch_bounds__(256) vt_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ vt, int L,
+                                                 int Lk, int H, int W) {
   __shared__ __nv_bfloat16 tile[64][66];
   const int bh = blockIdx.x, b = bh / H, h = bh % H;
   const int t0 = blockIdx.y * 64;
-  const long long rem = Ltot - static_cast<long long>(b) * Lg;
-  const int L = rem < Lg ? static_cast<int>(rem) : Lg;
-  const __nv_bfloat16* src = qkv + static_cast<long long>(b) * Lg * 3 * W + 2 * W + h * 64;
+  const __nv_bfloat16* src = qkv + static_cast<long long>(b) * L * 3 * W + 2 * W + h * 64;
   for (int i = threadIdx.x; i < 64 * 8; i += 256) {   // 64 tokens x 8 chunks of 8 d
     const int t = i >> 3, c = (i & 7) * 8;
     uint4 v = make_uint4(0, 0, 0, 0);
@@ -63,403 +49,138 @@ __global__ void __launch_bounds__(256) vt_kernel(const __nv_bfloat16* __restrict
   }
 }
 
+__device__ __forceinline__ uint32_t attn_pack(float a, float b) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+__device__ __forceinline__ float attn_exp2(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+
 // ---------------------------------------------------------------- main kernel
-// warps: 0 = control (TMA + MMA issue), 1..8 = softmax (two warps per TMEM lane quarter, each taking every other 16-column
-// chunk of a row), 9 = tail row on CUDA cores (sequences of 128 n + 1 tokens, i.e. ViT-L/14's 257: the last token would
-// otherwise cost a whole 128-row block of MMA + softmax work for one row)
-static constexpr int kParts = 2;                       // softmax warps per TMEM lane quarter (each takes every kParts-th 16-column chunk)
-static constexpr int kSoftWarps = 4 * kParts;
-static constexpr int kAttnThreads = 32 * (2 + kSoftWarps);   // control + softmax + tail-row warp
-__global__ void __launch_bounds__(kAttnThreads, 1) attention_tc_kernel(const __grid_constant__ AttnParams p) {
+__global__ void __launch_bounds__(128) attention_tc_kernel(const __grid_constant__ AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 0) p.trace[13] = clock64();   // kernel entry
-  const int nkb = p.Lk >> 6;                       // 64-key blocks
-  uint8_t* sQ = smem;                              // nq x [128][128 B]
-  uint8_t* sK = sQ + p.nq * 128 * 128;             // [Lk][128 B]
-  uint8_t* sV = sK + p.Lk * 128;                   // nkb x [64 d][128 B]
-  uint8_t* sP = sV + nkb * 8192;                   // nkb x [128 rows][128 B]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + nkb * 16384);
-  uint64_t* bar_k = bars;        // K landed
-  uint64_t* bar_v = bars + 1;    // V^T landed
-  uint64_t* bar_q = bars + 2;    // Q block landed, buffer 0 (buffer 1: bars + 7)
-  uint64_t* bar_s = bars + 3;    // S = QK^T complete
-  uint64_t* bar_p = bars + 4;    // P written (8 arrivals: one per softmax warp)
-  uint64_t* bar_o = bars + 5;    // O = PV complete
-  uint64_t* bar_oe = bars + 6;   // O read back (8 arrivals)
-  uint64_t* bar_q1 = bars + 7;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-  float* sRed = reinterpret_cast<float*>(bars + 10);   // [kParts][128] partial row maxima of the column parts
-  float* sSum = sRed + kParts * 128;                   // [kParts][128] partial row sums
-  float* sPt = sSum + kParts * 128;                             // [kMaxLk] tail row probabilities
+  const int qb = blockIdx.x, bh = blockIdx.y, b = bh / p.H, h = bh % p.H;
+  const int L = p.L;
+  const int nkb_all = p.Lk >> 6;
+  // causal: the keys of this query block's rows end at its last row
+  const int nkb = p.causal ? (qb + 1 < nkb_all ? qb + 1 : nkb_all) : nkb_all;
+  uint8_t* sQ = smem;                       // [64 rows][128 B]
+  uint8_t* sK = sQ + 8192;                  // nkb x [64 keys][128 B]
+  uint8_t* sV = sK + nkb_all * 8192;        // nkb x [64 d][128 B] (keys of block j)
+  uint64_t* bar = reinterpret_cast<uint64_t*>(sV + nkb_all * 8192);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int row0 = b * L;                   // first token of this image in the QKV / ctx buffers
 
-  const int bh = blockIdx.x, grp = bh / p.H, h = bh % p.H;
-  const int nimg = (p.B - grp * p.G) < p.G ? (p.B - grp * p.G) : p.G;   // images in this group (the last one may be short)
-  const int Lt = nimg * p.L;                      // tokens of the packed sequence
-  const bool tail = p.tail != 0;                  // the last token is computed by warp 9
-  const int nqb = tail ? (Lt >> 7) : ((Lt + 127) >> 7);
-  const uint32_t kOCol = p.Lk;                    // O accumulator right after S
-  const int row0 = grp * p.G * p.L;               // first row of the packed sequence in the QKV / ctx buffers
-
-  if (warp == 0) {
-    if (lane == 0) {
-      tma_prefetch_desc(&p.tmQK);
-      tma_prefetch_desc(&p.tmVt);
-      mbar_init(bar_k, 1); mbar_init(bar_v, 1); mbar_init(bar_q, 1); mbar_init(bar_q1, 1); mbar_init(bar_s, 1);
-      mbar_init(bar_p, kSoftWarps); mbar_init(bar_o, 1); mbar_init(bar_oe, kSoftWarps);   // one arrival per softmax warp
-      fence_mbar_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_slot, p.tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const bool tr = p.trace != nullptr && blockIdx.x == 0;
-  if (tr && threadIdx.x == 0) p.trace[0] = clock64();          // set-up done
-
-  if (warp == 0) {
-    // ===================== control warp: TMA loads + MMA issue (one elected lane) =====================
-    if (lane == 0) {
-      // order = order of use: Q(0) and K feed the first S, V is needed only by the first P.V (the in-kernel timeline — CC_ATTN_TRACE —
-      // showed the first S waiting ~9000 cycles for all 96 KB, and the second query block waiting for its Q to be fetched)
-      auto load_q = [&](int qb) {
-        uint64_t* bq = (qb & 1) && p.nq == 2 ? bar_q1 : bar_q;
-        uint8_t* dst = sQ + ((qb & 1) && p.nq == 2 ? 128 * 128 : 0);
-        mbar_arrive_expect_tx(bq, 128 * 128);
-        tma_load_2d(dst, &p.tmQK, bq, h * 64, row0 + 128 * qb);
-        tma_load_2d(dst + 8192, &p.tmQK, bq, h * 64, row0 + 128 * qb + 64);
-      };
-      if (nqb > 0) load_q(0);
-      mbar_arrive_expect_tx(bar_k, p.Lk * 128);
-      for (int j = 0; j < nkb; ++j) tma_load_2d(sK + j * 8192, &p.tmQK, bar_k, p.W + h * 64, row0 + 64 * j);
-      if (nqb > 1 && p.nq == 2) load_q(1);
-      mbar_arrive_expect_tx(bar_v, nkb * 8192);
-      for (int j = 0; j < nkb; ++j) {
-        if (p.vmajor) tma_load_2d(sV + j * 8192, &p.tmQK, bar_v, 2 * p.W + h * 64, row0 + 64 * j);   // V rows as they are: [key][64 d]
-        else tma_load_2d(sV + j * 8192, &p.tmVt, bar_v, 64 * j, bh * 64);
-      }
-    }
-    __syncwarp();
-    const int nch = (p.Lk + 255) >> 8;             // N chunks of the first MMA (N <= 256 each)
-    const int chN = p.Lk / nch;
-    const uint32_t idesc_s = umma_idesc_f16(128, chN, 1);
-    // O = P . V: B operand = V.  From the V^T pre-pass it is K-major like every other operand; read in place it is [key][d] =
-    // MN-major (b_major, instruction-descriptor bit 16): rows = K (keys) 128 B apart, 8-row groups SBO = 1024 B apart, the 64 d of
-    // a row are one 128-B swizzle span, a K = 16 step advances 2048 B (cute/atom/mma_traits_sm100.hpp, canonical Major-MN B128)
-    const uint32_t idesc_o = umma_idesc_f16(128, 64, 1) | (p.vmajor ? (1u << 16) : 0u);
-    const uint64_t dconst = (1ull << 16) | (static_cast<uint64_t>(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-    const uint32_t q16_0 = (smem_u32(sQ) & 0x3FFFF) >> 4, k16 = (smem_u32(sK) & 0x3FFFF) >> 4;
-    const uint32_t v16 = (smem_u32(sV) & 0x3FFFF) >> 4, p16 = (smem_u32(sP) & 0x3FFFF) >> 4;
-    mbar_wait(bar_k, 0);
-    if (tr && lane == 0) p.trace[1] = clock64();              // K landed
-    for (int qb = 0; qb < nqb; ++qb) {
-      const uint32_t ph = qb & 1;
-      const bool qodd = (qb & 1) && p.nq == 2;
-      mbar_wait(qodd ? bar_q1 : bar_q, p.nq == 2 ? ((qb >> 1) & 1) : ph);
-      tc_fence_after();
-      const uint32_t q16 = q16_0 + (qodd ? ((128 * 128) >> 4) : 0);
-      if (elect_one()) {
-        for (int c = 0; c < nch; ++c) {
-          const uint64_t bd = dconst | (k16 + ((c * chN * 128) >> 4));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            if (k == 0) umma_f16_c<false>(tmem_base + c * chN, dconst | q16, bd, idesc_s);
-            else umma_f16_c<true>(tmem_base + c * chN, (dconst | q16) + 2 * k, bd + 2 * k, idesc_s);
-          }
-        }
-        umma_commit(bar_s);
-      }
-      __syncwarp();
-      mbar_wait(bar_p, ph);          // P ready (=> S fully read, first MMA long done: Q buffer is free)
-      tc_fence_after();
-      if (qb + p.nq < nqb && lane == 0) {        // the buffer S(qb) read is free: fetch the query block that uses it next
-        const int nx = qb + p.nq;
-        uint64_t* bq = (nx & 1) && p.nq == 2 ? bar_q1 : bar_q;
-        uint8_t* dst = sQ + ((nx & 1) && p.nq == 2 ? 128 * 128 : 0);
-        mbar_arrive_expect_tx(bq, 128 * 128);
-        tma_load_2d(dst, &p.tmQK, bq, h * 64, row0 + 128 * nx);
-        tma_load_2d(dst + 8192, &p.tmQK, bq, h * 64, row0 + 128 * nx + 64);
-      }
-      __syncwarp();
-      if (qb == 0) mbar_wait(bar_v, 0);
-      else mbar_wait(bar_oe, ph ^ 1);   // previous O has been read back
-      tc_fence_after();
-      if (elect_one()) {
-        for (int kb = 0; kb < nkb; ++kb) {
-          const uint64_t ad = dconst | (p16 + kb * (16384 >> 4));
-          const uint64_t bd = dconst | (v16 + kb * (8192 >> 4));
-          const uint32_t bstep = p.vmajor ? (2048 >> 4) : 2;        // per K = 16: 16 key rows (MN-major) or 32 B along the row (K-major)
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            if (kb == 0 && k == 0) umma_f16_c<false>(tmem_base + kOCol, ad, bd, idesc_o);
-            else umma_f16_c<true>(tmem_base + kOCol, ad + 2 * k, bd + bstep * k, idesc_o);
-          }
-        }
-        umma_commit(bar_o);
-      }
-      __syncwarp();
-    }
-  } else if (warp <= kSoftWarps) {
-    // ===================== softmax / epilogue warps (thread pair == query row) =====================
-    const int quarter = warp & 3;
-    const int half = (warp - 1) >> 2;             // which 16-column chunks of a row this warp handles (chunk index mod kParts)
-    const int row = quarter * 32 + lane;
-    const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    const float kScale = 0.125f * 1.4426950408889634f;   // 1/sqrt(64) * log2(e)
-    for (int qb = 0; qb < nqb; ++qb) {
-      const uint32_t ph = qb & 1;
-      const int qi = qb * 128 + row;              // query index inside the packed sequence
-      // keys this row may see: those of its own image, up to itself when causal (rows past the packed sequence: none)
-      int lo = 1 << 28, lim = -1;                 // (sentinel far below INT_MAX: w_lo + 16 must not overflow)
-      if (qi < Lt) {
-        const int img = qi / p.L;
-        lo = img * p.L;
-        lim = p.causal ? qi : lo + p.L - 1;
-      }
-      // tcgen05.ld is .sync.aligned: every lane of the warp must execute the same loads, so the chunk loops run over the
-      // WARP's key range (its 32 consecutive rows touch at most two or three images) and each lane masks to its own keys
-      const int w_lo = __reduce_min_sync(0xffffffffu, lo) & ~15;     // 16-column chunks that intersect the warp's keys
-      const int w_hi = __reduce_max_sync(0xffffffffu, lim);
-      mbar_wait(bar_s, ph);
-      tc_fence_after();
-      const bool trs = tr && warp == 1 && lane == 0 && qb < 2;
-      if (trs) p.trace[2 + 5 * qb] = clock64();                 // S complete
-      float m = -INFINITY;
-      for (int c0 = w_lo + 16 * half; c0 <= w_hi; c0 += 16 * kParts) {
-        uint32_t v[16];
-        tmem_ld16(t_row + c0, v);
-        tmem_ld_wait();
-        if (__all_sync(0xffffffffu, c0 >= lo && c0 + 15 <= lim)) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) m = fmaxf(m, __uint_as_float(v[j]));
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (c0 + j >= lo && c0 + j <= lim) m = fmaxf(m, __uint_as_float(v[j]));
-        }
-      }
-      sRed[half * 128 + row] = m;
-      named_bar_sync(1, 32 * kSoftWarps);         // the column parts of every row exchange their maxima
-#pragma unroll
-      for (int q = 0; q < kParts; ++q) m = fmaxf(m, sRed[q * 128 + row]);
-      if (trs) p.trace[3 + 5 * qb] = clock64();                 // row maxima known
-      const float mc = m * kScale;
-      float sum = 0.f;
-      for (int c0 = 16 * half; c0 < p.Lk; c0 += 16 * kParts) {
-        uint8_t* blk = sP + (c0 >> 6) * 16384 + row * 128;
-        const uint32_t i0 = (c0 & 63) >> 3;
-        if (c0 < w_lo || c0 > w_hi) {            // keys of images no row of this warp belongs to: P = 0, no TMEM read, no exponentials
-          *reinterpret_cast<uint4*>(blk + ((i0 ^ (row & 7)) << 4)) = make_uint4(0, 0, 0, 0);
-          *reinterpret_cast<uint4*>(blk + (((i0 + 1) ^ (row & 7)) << 4)) = make_uint4(0, 0, 0, 0);
-          continue;
-        }
-        uint32_t v[16];
-        tmem_ld16(t_row + c0, v);
-        tmem_ld_wait();
-        float e[16];
-        // chunks that lie inside every row's own key range (all but the edges of an image's keys) skip the per-element mask:
-        // the pass is bound by instruction issue next to the MUFU, and the mask is three of its ~7 instructions per element
-        const bool inner = __all_sync(0xffffffffu, c0 >= lo && c0 + 15 <= lim);
-        if (inner) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e[j]) : "f"(fmaf(__uint_as_float(v[j]), kScale, -mc)));
-            sum += e[j];
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float x;
-            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(x) : "f"(fmaf(__uint_as_float(v[j]), kScale, -mc)));
-            e[j] = (c0 + j >= lo && c0 + j <= lim) ? x : 0.f;
-            sum += e[j];
-          }
-        }
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          uint32_t w[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            __nv_bfloat162 hh = __floats2bfloat162_rn(e[8 * q + 2 * j], e[8 * q + 2 * j + 1]);
-            w[j] = *reinterpret_cast<uint32_t*>(&hh);
-          }
-          *reinterpret_cast<uint4*>(blk + (((i0 + q) ^ (row & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-      }
-      if (trs) p.trace[4 + 5 * qb] = clock64();                 // this warp's P written
-      sSum[half * 128 + row] = sum;               // read by the partner after bar_o (ordered through bar_p -> MMA -> bar_o)
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p);
-      // ---- O -> ctx: each warp of the pair normalises and stores 32 of the 64 output columns
-      mbar_wait(bar_o, ph);
-      tc_fence_after();
-      if (trs) p.trace[5 + 5 * qb] = clock64();                 // O complete
-      float tot = 0.f;
-#pragma unroll
-      for (int q = 0; q < kParts; ++q) tot += sSum[q * 128 + row];      // (own part included: fixed summation order for all warps of a row)
-      const float inv = 1.0f / tot;
-      constexpr int kOC = 64 / kParts;            // output columns per warp (16 with four parts)
-      __nv_bfloat16* out = p.ctx + (static_cast<long long>(row0) + qi) * p.W + h * 64 + kOC * half;
-#pragma unroll
-      for (int c0 = 0; c0 < kOC; c0 += 16) {
-        uint32_t v[16];
-        tmem_ld16(t_row + kOCol + kOC * half + c0, v);
-        tmem_ld_wait();
-        if (qi < Lt) {
-#pragma unroll
-          for (int q = 0; q < 2; ++q) {
-            uint32_t w[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              __nv_bfloat162 hh = __floats2bfloat162_rn(__uint_as_float(v[8 * q + 2 * j]) * inv,
-                                                        __uint_as_float(v[8 * q + 2 * j + 1]) * inv);
-              w[j] = *reinterpret_cast<uint32_t*>(&hh);
-            }
-            *reinterpret_cast<uint4*>(out + c0 + 8 * q) = make_uint4(w[0], w[1], w[2], w[3]);
-          }
-        }
-      }
-      if (trs) p.trace[6 + 5 * qb] = clock64();                 // O stored
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_oe);
-    }
-  } else if (tail) {
-    // ===================== tail row (token Lt - 1) on CUDA cores, from the K and V^T tiles in shared memory ===============
-    const int qi = Lt - 1;
-    float q[64];
-    {
-      const uint4* src = reinterpret_cast<const uint4*>(p.qkv + (static_cast<long long>(row0) + qi) * 3 * p.W + h * 64);
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        const uint4 u = __ldg(src + c);
-        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          q[8 * c + 2 * j] = __uint_as_float(w[j] << 16);
-          q[8 * c + 2 * j + 1] = __uint_as_float(w[j] & 0xFFFF0000u);
-        }
-      }
-    }
-    const float kScale = 0.125f * 1.4426950408889634f;
-    mbar_wait(bar_k, 0);
-    float sc[kMaxLk / 32];
-    float m = -INFINITY;
-#pragma unroll
-    for (int i = 0; i < kMaxLk / 32; ++i) {
-      const int j = lane + 32 * i;
-      float a = -INFINITY;
-      if (j < Lt && j < p.Lk) {                   // the last token sees every key of its image (causal or not)
-        const uint8_t* kr = sK + (j >> 6) * 8192 + (j & 63) * 128;
-        a = 0.f;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const uint4 u = *reinterpret_cast<const uint4*>(kr + ((c ^ (j & 7)) << 4));
-          const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            a = fmaf(q[8 * c + 2 * t], __uint_as_float(w[t] << 16), a);
-            a = fmaf(q[8 * c + 2 * t + 1], __uint_as_float(w[t] & 0xFFFF0000u), a);
-          }
-        }
-        a *= kScale;
-      }
-      sc[i] = a;
-      m = fmaxf(m, a);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    float sum = 0.f;
-#pragma unroll
-    for (int i = 0; i < kMaxLk / 32; ++i) {
-      const int j = lane + 32 * i;
-      float e = 0.f;
-      if (j < Lt && j < p.Lk) {
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(sc[i] - m));
-        e = __bfloat162float(__float2bfloat16_rn(e));    // as the tensor-core rows: P is rounded to bf16 before P.V
-      }
-      if (j < p.Lk) sPt[j] = e;
-      sum += e;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    __syncwarp();
-    mbar_wait(bar_v, 0);
-    float o0 = 0.f, o1 = 0.f;                     // output dims: (lane, lane + 32) from V^T, (2 lane, 2 lane + 1) from V in place
-    if (p.vmajor) {
-      for (int j = 0; j < Lt; ++j) {              // V row j: [64 d] = 128 B, 16-B chunk c at slot c ^ (j & 7); this lane's two d's = one word
-        const uint32_t w = *reinterpret_cast<const uint32_t*>(sV + (j >> 6) * 8192 + (j & 63) * 128 + ((((lane >> 2) ^ (j & 7))) << 4) + (lane & 3) * 4);
-        const float pj = sPt[j];
-        o0 = fmaf(pj, __uint_as_float(w << 16), o0);
-        o1 = fmaf(pj, __uint_as_float(w & 0xFFFF0000u), o1);
-      }
-      const float inv = 1.0f / sum;
-      __nv_bfloat162 r = __floats2bfloat162_rn(o0 * inv, o1 * inv);
-      *reinterpret_cast<__nv_bfloat162*>(p.ctx + (static_cast<long long>(row0) + qi) * p.W + h * 64 + 2 * lane) = r;
-    } else {
-    for (int kb = 0; kb < nkb; ++kb) {
-      const uint8_t* v0 = sV + kb * 8192 + lane * 128;
-      const uint8_t* v1 = v0 + 32 * 128;
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        const float4 pa = *reinterpret_cast<const float4*>(sPt + kb * 64 + c * 8), pb = *reinterpret_cast<const float4*>(sPt + kb * 64 + c * 8 + 4);
-        const float pp[8] = {pa.x, pa.y, pa.z, pa.w, pb.x, pb.y, pb.z, pb.w};
-        const uint4 a = *reinterpret_cast<const uint4*>(v0 + ((c ^ (lane & 7)) << 4));
-        const uint4 b = *reinterpret_cast<const uint4*>(v1 + ((c ^ (lane & 7)) << 4));
-        const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          o0 = fmaf(pp[2 * t], __uint_as_float(aw[t] << 16), o0);
-          o0 = fmaf(pp[2 * t + 1], __uint_as_float(aw[t] & 0xFFFF0000u), o0);
-          o1 = fmaf(pp[2 * t], __uint_as_float(bw[t] << 16), o1);
-          o1 = fmaf(pp[2 * t + 1], __uint_as_float(bw[t] & 0xFFFF0000u), o1);
-        }
-      }
-    }
-    const float inv = 1.0f / sum;
-    __nv_bfloat16* out = p.ctx + (static_cast<long long>(row0) + qi) * p.W + h * 64;
-    out[lane] = __float2bfloat16_rn(o0 * inv);
-    out[lane + 32] = __float2bfloat16_rn(o1 * inv);
+  if (tid == 0) {
+    tma_prefetch_desc(&p.tmQK);
+    tma_prefetch_desc(&p.tmVt);
+    mbar_init(bar, 1);
+    fence_mbar_init();
+    mbar_arrive_expect_tx(bar, 8192 + 2 * nkb * 8192);
+    tma_load_2d(sQ, &p.tmQK, bar, h * 64, row0 + 64 * qb);
+    for (int j = 0; j < nkb; ++j) {
+      tma_load_2d(sK + j * 8192, &p.tmQK, bar, p.W + h * 64, row0 + 64 * j);
+      tma_load_2d(sV + j * 8192, &p.tmVt, bar, 64 * j, bh * 64);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  if (tr && threadIdx.x == 0) p.trace[12] = clock64();         // all roles done
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
+  mbar_wait(bar, 0);
+
+  const uint64_t qdesc = gmma_desc(smem_u32(sQ), 128);
+  const uint64_t kdesc = gmma_desc(smem_u32(sK), 128);
+  const uint64_t vdesc = gmma_desc(smem_u32(sV), 128);
+  const float kScale = 0.125f * 1.4426950408889634f;   // 1/sqrt(64) * log2(e)
+  const int q0 = 64 * qb + 16 * warp + (lane >> 2), q1 = q0 + 8;   // this thread's two query rows
+  const int cq = 2 * (lane & 3);                                   // its first column inside each 8-column group
+
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  for (int j = 0; j < nkb; ++j) {
+    float s[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) Wgmma<64>::mma(s, qdesc + 2 * k, kdesc + j * (8192 >> 4) + 2 * k, k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(s);
+    // mask (keys past the image, or after the query when causal), scale to the log2 domain, row maxima
+    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int key = 64 * j + 8 * i + cq + e;
+        const bool ok0 = key < L && (!p.causal || key <= q0), ok1 = key < L && (!p.causal || key <= q1);
+        s[4 * i + e] = ok0 ? s[4 * i + e] * kScale : -INFINITY;
+        s[4 * i + 2 + e] = ok1 ? s[4 * i + 2 + e] * kScale : -INFINITY;
+        mx0 = fmaxf(mx0, s[4 * i + e]);
+        mx1 = fmaxf(mx1, s[4 * i + 2 + e]);
+      }
+#pragma unroll
+    for (int d = 1; d <= 2; d <<= 1) {
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, d));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, d));
+    }
+    // key 0 is visible to every row, so after the first block the maxima are finite
+    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
+    const float a0 = attn_exp2(m0 - mn0), a1 = attn_exp2(m1 - mn1);
+    m0 = mn0; m1 = mn1;
+    float sum0 = 0.f, sum1 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        s[4 * i + e] = attn_exp2(s[4 * i + e] - mn0);
+        s[4 * i + 2 + e] = attn_exp2(s[4 * i + 2 + e] - mn1);
+        sum0 += s[4 * i + e];
+        sum1 += s[4 * i + 2 + e];
+        o[4 * i + e] *= a0;
+        o[4 * i + 2 + e] *= a1;
+      }
+    l0 = l0 * a0 + sum0;
+    l1 = l1 * a1 + sum1;
+    // P (bf16, unnormalised, <= 1) as the register A operand: K step kk covers keys 16 kk .. 16 kk + 15 of the block
+    uint32_t a[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      a[kk][0] = attn_pack(s[8 * kk + 0], s[8 * kk + 1]);
+      a[kk][1] = attn_pack(s[8 * kk + 2], s[8 * kk + 3]);
+      a[kk][2] = attn_pack(s[8 * kk + 4], s[8 * kk + 5]);
+      a[kk][3] = attn_pack(s[8 * kk + 6], s[8 * kk + 7]);
+    }
+    wgmma_fence_acc(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_rs_m64n64(o, a[kk], vdesc + j * (8192 >> 4) + 2 * kk, 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(o);
+  }
+#pragma unroll
+  for (int d = 1; d <= 2; d <<= 1) {
+    l0 += __shfl_xor_sync(0xffffffffu, l0, d);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, d);
+  }
+  const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+  __nv_bfloat16* out0 = p.ctx + (static_cast<long long>(row0) + q0) * p.W + h * 64 + cq;
+  __nv_bfloat16* out1 = out0 + 8ll * p.W;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    if (q0 < L) *reinterpret_cast<uint32_t*>(out0 + 8 * i) = attn_pack(o[4 * i] * inv0, o[4 * i + 1] * inv0);
+    if (q1 < L) *reinterpret_cast<uint32_t*>(out1 + 8 * i) = attn_pack(o[4 * i + 2] * inv1, o[4 * i + 3] * inv1);
   }
 }
 
 // ---------------------------------------------------------------- host
-// images per CTA: the packing that fills the 128-row query blocks best while the packed key range stays within 256 columns
-// (larger G only adds masked S / PV columns); one image per CTA when a single image already spans more than 256 keys
-static int attention_group(int B, int L) {
-  int best = 1;
-  double best_u = -1;
-  for (int g = 1; g <= B && g <= 16; ++g) {
-    const int rows = g * L, lk = (rows + 63) / 64 * 64;
-    if (g > 1 && lk > 256) break;
-    const double u = double(rows) / (128.0 * ((rows + 127) / 128));
-    if (u > best_u + 1e-9 || (u > best_u - 1e-9 && g > best)) { best_u = u; best = g; }
-  }
-  return best;
-}
-static int attention_lk(int B, int L) { return (attention_group(B, L) * L + 63) / 64 * 64; }
-
 bool attention_tc_supported(int L) {
-  // CC_ATTN_TC: 0 = never (mma.sync kernel of vit.cu), 1 (default) = by measured speed, 2 = wherever it fits.  Read when a plan
-  // is built, so tests can force either path.  Measured on B200 (bench.py --workload clip, per 12- or 24-layer forward, B = 256):
-  // ViT-L/14 image tower (257 tokens) 13.4 ms here vs 17.0 ms on the mma.sync kernel; ViT-B/32 image tower (50 tokens, packed
-  // five images per CTA) 0.82 ms here vs 0.44 ms there, text tower (77 tokens) 12 % slower here: the short sequences are bound
-  // by this kernel's serial per-CTA chain (loads -> S -> softmax -> PV with one CTA per SM), which the mma.sync kernel hides with
-  // several CTAs per SM.  So by default the tcgen05 kernel takes the sequences longer than one 128-row block.
+  // CC_ATTN_TC: 0 = never (mma.sync kernel of vit.cu), 1 (default) = sequences longer than 128 tokens (ViT-L/14's 257),
+  // 2 = wherever it fits.  Read when a plan is built, so tests can force either path.
   const char* e = getenv("CC_ATTN_TC");
   const int mode = e ? atoi(e) : 1;
   const int Lk = (L + 63) / 64 * 64;
@@ -468,24 +189,18 @@ bool attention_tc_supported(int L) {
   return true;
 }
 size_t attention_tc_workspace_bytes(int B, int L, int H) {
-  const int G = attention_group(B, L);
-  return static_cast<size_t>((B + G - 1) / G) * H * 64 * attention_lk(B, L) * 2;
+  return static_cast<size_t>(B) * H * 64 * ((L + 63) / 64 * 64) * 2;
 }
 
 int attention_tc_launch(const __nv_bfloat16* qkv, __nv_bfloat16* ctx, __nv_bfloat16* vt_ws, int B, int L, int H, int causal,
                         cudaStream_t st) {
   if (B == 0) return CC_OK;
-  const int G = attention_group(B, L), NG = (B + G - 1) / G;
-  const int W = H * 64, Lk = attention_lk(B, L), nkb = Lk / 64;
+  const int W = H * 64, Lk = (L + 63) / 64 * 64, nkb = Lk / 64;
   CC_REQUIRE(Lk <= kMaxLk, "attention_tc: sequence length %d too long", L);
   PFN_encodeTiled enc = get_encode_tiled();
   CC_REQUIRE(enc != nullptr, "attention_tc: cuTensorMapEncodeTiled unavailable");
   AttnParams p{};
-  static const int vt_env = getenv("CC_ATTN_VT") ? atoi(getenv("CC_ATTN_VT")) : 0;
-  p.vmajor = vt_env ? 0 : 1;
-  p.qkv = qkv; p.ctx = ctx; p.tail = (G == 1 && L > 128 && (L & 127) == 1) ? 1 : 0; p.B = B; p.L = L; p.Lk = Lk; p.H = H; p.W = W; p.causal = causal; p.G = G;
-  p.tmem_cols = 32;
-  while (p.tmem_cols < Lk + 64) p.tmem_cols <<= 1;
+  p.ctx = ctx; p.L = L; p.Lk = Lk; p.H = H; p.W = W; p.causal = causal;
   {
     cuuint64_t dims[2] = {cuuint64_t(3) * W, cuuint64_t(B) * L};
     cuuint64_t strides[1] = {cuuint64_t(3) * W * 2};
@@ -496,7 +211,7 @@ int attention_tc_launch(const __nv_bfloat16* qkv, __nv_bfloat16* ctx, __nv_bfloa
     CC_REQUIRE(r == CUDA_SUCCESS, "attention_tc: tensor map (QK) failed: %d", int(r));
   }
   {
-    cuuint64_t dims[2] = {cuuint64_t(Lk), cuuint64_t(NG) * H * 64};
+    cuuint64_t dims[2] = {cuuint64_t(Lk), cuuint64_t(B) * H * 64};
     cuuint64_t strides[1] = {cuuint64_t(Lk) * 2};
     cuuint32_t box[2] = {64, 64}, estr[2] = {1, 1};
     CUresult r = enc(&p.tmVt, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, vt_ws, dims, strides, box, estr,
@@ -504,36 +219,15 @@ int attention_tc_launch(const __nv_bfloat16* qkv, __nv_bfloat16* ctx, __nv_bfloa
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     CC_REQUIRE(r == CUDA_SUCCESS, "attention_tc: tensor map (Vt) failed: %d", int(r));
   }
-  if (!p.vmajor) {
-    vt_kernel<<<dim3(NG * H, nkb), 256, 0, st>>>(qkv, vt_ws, G * L, static_cast<long long>(B) * L, Lk, H, W);
-    CC_CHECK_CUDA(cudaGetLastError());
-  }
-  p.nq = (1024 + 2 * 128 * 128 + Lk * 128 + nkb * 8192 + nkb * 16384 + 80 + (2 * kParts * 128 + kMaxLk) * 4 <= 227 * 1024) ? 2 : 1;
-  const int smem = 1024 + p.nq * 128 * 128 + Lk * 128 + nkb * 8192 + nkb * 16384 + 80 + (2 * kParts * 128 + kMaxLk) * 4;
+  vt_kernel<<<dim3(B * H, nkb), 256, 0, st>>>(qkv, vt_ws, L, Lk, H, W);
+  CC_CHECK_CUDA(cudaGetLastError());
+  const int smem = 1024 + 8192 + 2 * nkb * 8192 + 64;
   static bool attr_set = false;
   if (!attr_set) {
-    CC_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    CC_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 1024 + 8192 + 2 * (kMaxLk / 64) * 8192 + 64));
     attr_set = true;
   }
-  static const int trace_env = getenv("CC_ATTN_TRACE") ? atoi(getenv("CC_ATTN_TRACE")) : 0;
-  static int traced = 0;
-  if (trace_env && traced < 2 && L > 128) {       // diagnostic only: synchronises and prints the timeline of CTA 0 (SM cycles)
-    ++traced;
-    unsigned long long* d = nullptr;
-    cudaMalloc(&d, 16 * 8);
-    cudaMemsetAsync(d, 0, 16 * 8, st);
-    p.trace = d;
-    attention_tc_kernel<<<NG * H, kAttnThreads, smem, st>>>(p);
-    unsigned long long h[16];
-    cudaStreamSynchronize(st);
-    cudaMemcpy(h, d, sizeof(h), cudaMemcpyDeviceToHost);
-    cudaFree(d);
-    const unsigned long long t0 = h[13];
-    fprintf(stderr, "attention_tc CTA 0 timeline (SM cycles after kernel entry; B=%d L=%d Lk=%d G=%d): setup %llu | K landed %llu | qb0: S %llu max %llu P %llu O %llu stored %llu | qb1: S %llu max %llu P %llu O %llu stored %llu | done %llu\n",
-            B, L, Lk, G, h[0] - t0, h[1] - t0, h[2] - t0, h[3] - t0, h[4] - t0, h[5] - t0, h[6] - t0, h[7] - t0, h[8] - t0, h[9] - t0, h[10] - t0, h[11] - t0, h[12] - t0);
-    return CC_OK;
-  }
-  attention_tc_kernel<<<NG * H, kAttnThreads, smem, st>>>(p);
+  attention_tc_kernel<<<dim3((L + 63) / 64, B * H), 128, smem, st>>>(p);
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;
 }

@@ -56,7 +56,7 @@ int device_sm_count() {
     cudaDeviceProp prop;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess) {
       n = -1;
-    } else if (prop.major != 10) {
+    } else if (prop.major != 9) {
       n = -1;
     } else {
       n = prop.multiProcessorCount;

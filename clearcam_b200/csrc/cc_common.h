@@ -12,7 +12,7 @@ enum : int {
   CC_OK = 0,
   CC_ERR_INVALID = -1,   // bad argument / unsupported shape
   CC_ERR_CUDA = -2,      // CUDA runtime / driver error
-  CC_ERR_NOGPU = -3,     // no sm_100 device
+  CC_ERR_NOGPU = -3,     // no sm_90 device
   CC_ERR_STATE = -4,     // handle used in the wrong state
 };
 

@@ -1,5 +1,5 @@
-// clearcam_b200 — sm_100a PTX wrappers (mbarrier, TMA, tcgen05/TMEM).
-// Hand-written for B200; no CUTLASS dependency. Every wait is a bounded spin that traps
+// clearcam_b200 — sm_90a PTX wrappers (mbarrier, TMA, wgmma).
+// Hand-written for H100; no CUTLASS dependency. Every wait is a bounded spin that traps
 // instead of hanging the GPU, so a pipeline bug surfaces as a launch failure, not a dead box.
 #pragma once
 #include <cuda_runtime.h>
@@ -17,16 +17,6 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
-}
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
 }
 
 // ---------------------------------------------------------------- explicit shared-space accesses
@@ -104,42 +94,10 @@ __device__ __forceinline__ void tma_load_5d(void* smem_dst, const void* tmap, ui
       : "memory");
 }
 
-// Cluster-multicast variant: the box lands at the same shared-memory offset in every CTA of `cta_mask`, and each of them
-// gets the complete_tx on its own mbarrier at the same offset.
-__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
 // TMA store: smem tile -> global box (bulk async-group completion); out-of-bounds parts of the box are clipped.
-__device__ __forceinline__ void tma_store_5d(const void* tmap, const void* smem_src, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(tmap)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-               : "memory");
-}
 __device__ __forceinline__ void tma_store_2d(const void* tmap, const void* smem_src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(tmap)),
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-// TMA reduce-add store: global[box] += smem tile, performed at the L2 (used for the in-place fp32 residual of the CLIP
-// out-proj / MLP-proj GEMMs: x += GEMM, one fp32 add per element exactly like load-add-store).
-__device__ __forceinline__ void tma_reduce_add_5d(const void* tmap, const void* smem_src, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile("cp.reduce.async.bulk.tensor.5d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(tmap)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
                : "memory");
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
@@ -149,104 +107,88 @@ __device__ __forceinline__ void tma_store_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
+// ---------------------------------------------------------------- wgmma (warpgroup MMA, sm_90a)
+// Shared-memory matrix descriptor, K-major swizzled canonical layout: rows of `row_bytes` (= swizzle span: 128/64/32 B),
+// 8-row groups `sbo_bytes` apart.  Swizzle mode in bits [62,64): 1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B.
+// Advancing the start address by 32 B steps one K = 16 slice inside the swizzle span (the XOR is applied on absolute
+// shared-memory address bits, as TMA writes it).
+__host__ __device__ __forceinline__ uint64_t gmma_desc_const(uint32_t row_bytes, uint32_t sbo_bytes) {
+  const uint64_t layout = row_bytes == 128 ? 1ull : (row_bytes == 64 ? 2ull : 3ull);
+  return (1ull << 16) | (static_cast<uint64_t>(sbo_bytes >> 4) << 32) | (layout << 62);
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr, uint32_t row_bytes) {
+  return gmma_desc_const(row_bytes, 8u * row_bytes) | ((smem_addr & 0x3FFFF) >> 4);
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator registers across an asynchronous wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, kind::f16 (bf16/fp16 in, fp32 accumulate). One thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same with the accumulate predicate fixed at compile time (no setp / predicate plumbing in the hot issue loop).
-template <bool ACC>
-__device__ __forceinline__ void umma_f16_c(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc) {
-  if (ACC)
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc)
-                 : "memory");
-  else
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, 1, 1;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc)
-                 : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// Same, arriving on the mbarrier at this offset in every CTA of `cta_mask` (a smem stage that a peer CTA multicasts into may
-// only be refilled once BOTH CTAs' MMAs have read it).
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, bf16 in, fp32 accumulate, A and B K-major from shared memory.  Thread t of the
+// warpgroup holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) and columns 8 i + 2 (t % 4) (+ 1): d[4 i + {0, 1}] in the first row,
+// d[4 i + {2, 3}] in the second.
+template <int N>
+struct Wgmma;
+template <>
+struct Wgmma<16> {
+  static __device__ __forceinline__ void mma(float (&d)[8], uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <>
+struct Wgmma<32> {
+  static __device__ __forceinline__ void mma(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <>
+struct Wgmma<64> {
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <>
+struct Wgmma<128> {
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
 
-// K-major shared-memory matrix descriptor (sm_100 "version 1"), swizzled canonical layout:
-// rows of `row_bytes` (= swizzle span: 128/64/32 B), 8-row groups `8*row_bytes` apart (SBO).
-// layout_type: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B, 6 = SWIZZLE_32B.
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t smem_addr, uint32_t row_bytes) {
-  const uint64_t layout = row_bytes == 128 ? 2ull : (row_bytes == 64 ? 4ull : 6ull);
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);            // start address   [0,14)
-  d |= static_cast<uint64_t>(1) << 16;                              // LBO (unused for swizzled K-major)
-  d |= static_cast<uint64_t>((8u * row_bytes) >> 4) << 32;          // SBO             [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                              // descriptor version 1 (Blackwell)
-  d |= layout << 61;                                                // swizzle mode    [61,64)
-  return d;
-}
-// Same, for a 128B-swizzled K-major view whose 8-row groups are `sbo_bytes` apart and whose start may be shifted by
-// whole 128-B rows inside the swizzle atom (halo views): base_offset carries (start >> 7) & 7 when requested.
-__device__ __forceinline__ uint64_t umma_smem_desc_halo(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t row_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= (row_bytes == 128 ? 2ull : 4ull) << 61;   // SWIZZLE_128B / SWIZZLE_64B (the XOR is on absolute smem address bits)
-  return d;
-}
-__device__ __forceinline__ uint64_t umma_smem_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t base_offset) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(base_offset & 7) << 49;
-  d |= 2ull << 61;
-  return d;
-}
-// Instruction descriptor for kind::f16: fp32 accumulate, A/B = bf16 (fmt 1) or fp16 (fmt 0), both K-major.
-__host__ __device__ __forceinline__ uint32_t umma_idesc_f16(uint32_t M, uint32_t N, uint32_t ab_fmt) {
-  return (1u << 4) | (ab_fmt << 7) | (ab_fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// Same with A from registers (m64n64k16): a[0..3] = bf16 pairs (row r, k 2q..2q+1), (row r+8, ...), (row r, k 8+2q..),
+// (row r+8, k 8+2q..) with r = 16 (t / 32) + (t % 32) / 4, q = t % 4 — the accumulator layout of a 64 x 16 tile, so an fp32
+// accumulator converted pairwise to bf16 is directly the A operand of the next MMA.
+__device__ __forceinline__ void wgmma_rs_m64n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
+      "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d));
 }
 
 // Programmatic dependent launch: wait for the prerequisite grids' memory / let dependents start their prologue.

@@ -1,4 +1,4 @@
-// CLIP (OpenCLIP ViT) image + text encoders as static op lists over the sm_100a kernels.
+// CLIP (OpenCLIP ViT) image + text encoders as static op lists over the sm_90a kernels.
 //
 // Replaces in the reference: OpenCLIP.precompute_embedding (models/objects.py:94-133), encode_text (:145-186) and the
 // weight container OpenCLIP.__init__ (:22-92).  Parametric in the architecture (the reference hard-codes
@@ -8,7 +8,7 @@
 // depend on bf16 round-off accumulation); every GEMM operand is bf16 (LayerNorm writes bf16, the QKV / MLP-fc
 // epilogues write bf16), the out-proj and MLP-proj GEMMs add the fp32 residual in their epilogue in place.
 // Per block: LN -> QKV GEMM(+bias) -> attention -> out-proj GEMM(+bias,+residual) -> LN -> fc GEMM(+bias,+GELU-tanh)
-// -> proj GEMM(+bias,+residual).  All GEMMs run on the tcgen05 kernel of conv_gemm.cu.
+// -> proj GEMM(+bias,+residual).  All GEMMs run on the wgmma kernel of conv_gemm.cu.
 #include "clearcam_b200.h"
 #include "cc_common.h"
 #include "conv_gemm.cuh"
@@ -241,7 +241,7 @@ int cc_clip_create(const cc_clip_config* cfg, int n_tensors, const char* const* 
                    const int64_t* numels, cc_clip** out) {
   CC_REQUIRE(cfg && out, "cc_clip_create: null argument");
   const int sms = device_sm_count();
-  CC_REQUIRE(sms > 0, "cc_clip_create: no sm_100 (B200) device");
+  CC_REQUIRE(sms > 0, "cc_clip_create: no sm_90 (H100) device");
   CC_REQUIRE(cfg->image_size % cfg->patch == 0 && cfg->v_width % 128 == 0 && cfg->t_width % 128 == 0 &&
                  cfg->v_width == cfg->v_heads * 64 && cfg->t_width == cfg->t_heads * 64 && cfg->embed_dim % 16 == 0 &&
                  cfg->v_mlp % 16 == 0 && cfg->t_mlp % 16 == 0,

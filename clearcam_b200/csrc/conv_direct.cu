@@ -1,4 +1,4 @@
-// Direct (CUDA-core) NHWC convolution: the generic path for shapes the tcgen05 kernel does not take
+// Direct (CUDA-core) NHWC convolution: the generic path for shapes the wgmma kernel does not take
 // (channel counts that are not multiples of 16 — YOLOv9-t/-s/-m widths such as 24/48/90 —, true grouped
 // convs, odd spatial sizes with stride 2) and the stem.  fp32 accumulate, same epilogue semantics as
 // conv_gemm (bias -> act -> +residual).  Reference: detection/yolov9.py:33-38 (Conv), :171-194 (head convs).
@@ -72,7 +72,7 @@ int conv_direct_launch(const DirectConvParams& p, cudaStream_t stream) {
   if (total == 0) return CC_OK;
   const int threads = 128;
   long long blocks = (total + threads - 1) / threads;
-  if (blocks > 148 * 64) blocks = 148 * 64;
+  if (blocks > 132 * 64) blocks = 132 * 64;
   conv_direct_kernel<<<static_cast<int>(blocks), threads, 0, stream>>>(p);
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;

@@ -1,16 +1,17 @@
-// Implicit-GEMM conv / linear on tcgen05 (sm_100a). See conv_gemm.cuh for what it replaces in the reference.
+// Implicit-GEMM conv / linear on Hopper warpgroup MMA (sm_90a). See conv_gemm.cuh for what it replaces in the reference.
 //
 // GEMM view: M = output pixels (N*H*W), N = Cout, K = kh*kw*Cin.
-//   * CTA tile: 128 pixels x BN channels; the 128 pixels are a TW x TH x TN box of the NHWC output
-//     (TW*TH*TN = 128, chosen per layer so 20x20/40x40 maps tile without waste).
+//   * CTA tile: 128 pixels x BN channels (BN in {16, 32, 64, 128}); the 128 pixels are a TW x TH x TN box of the NHWC
+//     output (TW*TH*TN = 128, chosen per layer so 20x20/40x40 maps tile without waste).
 //   * K loop: for each filter tap (r,s) and each BK-channel chunk, ONE TMA box load of the input shifted by
-//     the tap offset (TMA zero-fills out-of-bounds = conv padding) + one TMA box of the weights.
+//     the tap offset (TMA zero-fills out-of-bounds = conv padding) + one TMA box of the weights (or, when the weights of
+//     the layer fit, all of them once per CTA: "resident" weights).
 //     stride 2 uses a 5-D "pixel pair" view (dims: 2*C, W/2, 2, H/2, N) so every tap is again a dense box.
 //   * smem tiles are K-major, 128/64/32-byte swizzled (BK = 64/32/16 channels) exactly as TMA writes them;
-//     tcgen05.mma (M=128, N=BN, K=16) reads them through shared-memory descriptors; accumulators live in TMEM
-//     (2 x 256 columns, double buffered so the epilogue of tile i overlaps the mainloop of tile i+1).
-//   * warp roles: w0 = TMA producer, w1 = MMA issuer, w2 = TMEM allocator, w4..7 = epilogue
-//     (tcgen05.ld -> bias -> SiLU/GELU -> (+residual) -> bf16/fp32 -> padded smem staging -> coalesced 16-B stores).
+//     wgmma.mma_async (M=64, N=BN, K=16) reads them through shared-memory descriptors, accumulators in registers.
+//   * warpgroup roles: wg0 = TMA producer (one thread), wg1 / wg2 = consumers, each owning 64 rows of the tile:
+//     wgmma mainloop -> fp32 accumulators to smem -> thread pair == output row: bias -> SiLU/GELU -> (+residual) ->
+//     bf16/fp32 in place -> coalesced 16-B stores.
 //   * persistent: grid = min(tiles, SMs), static round-robin tile schedule.
 #include "conv_gemm.cuh"
 #include "cc_common.h"
@@ -21,14 +22,11 @@
 
 namespace cc {
 
-#ifndef CC_EPI_WARPS
-#define CC_EPI_WARPS 16
-#endif
-static constexpr int kEpiThreads = 32 * CC_EPI_WARPS;   // epilogue warps (multiple of 4: one per TMEM lane quarter)
-static constexpr int kThreads = 128 + kEpiThreads;      // w0 TMA, w1 MMA, w2 TMEM alloc, w3 idle, w4.. epilogue
-static constexpr int kMaxAcc = 4;                       // TMEM accumulator slots == independent epilogue groups (2 or 4)
+static constexpr int kConsumers = 2;                       // consumer warpgroups (64 rows each)
+static constexpr int kThreads = 128 * (1 + kConsumers);     // wg0 producer + consumers
+static constexpr int kEpiThreads = 128 * kConsumers;
 static constexpr int kTileM = 128;
-static constexpr uint32_t kTmemCols = 512;
+static constexpr int kMaxBN = 128;
 static constexpr int kMaxSmem = 232448;  // 227 KB
 
 __device__ __forceinline__ float tanh_approx(float x) {
@@ -37,10 +35,8 @@ __device__ __forceinline__ float tanh_approx(float x) {
   return t;
 }
 
-// Epilogue activations.  tests/tools/ubench_pipes.cu on B200: tanh.approx / ex2.approx / rcp.approx all issue one warp
-// instruction per 8 cycles per scheduler (16 lanes/clk/SM), fma one per cycle, cvt.rn.bf16x2 one per 2 cycles; the packed
-// tanh.approx.bf16x2 / f16x2 take 16 cycles (no gain).  So an activation that needs two MUFU ops (ex2 + rcp) costs twice the
-// MUFU time of the tanh form, and MUFU time is what bounds a chunk of the epilogue once enough warps run it:
+// Epilogue activations.  tanh.approx / ex2.approx / rcp.approx all run on the multi-function unit, so an activation that
+// needs two of them (ex2 + rcp) costs twice the MUFU time of the tanh form:
 //   ACT_SILU       : x*sigmoid(x) = h + h*tanh(h), h = x/2 : ONE MUFU (tanh.approx.f32, |abs err| <= 2^-11 on tanh, i.e.
 //                    <= |x| * 2.4e-4 on the result, below the bf16 rounding of the stored value for x > -2)
 //   ACT_SILU_EXACT : x / (1 + 2^(-x log2 e)) with ex2.approx + rcp.approx (two MUFU, ~1e-7 relative)
@@ -69,32 +65,16 @@ __device__ __forceinline__ int fdiv(int x, const uint32_t fd[2]) {
 }
 // tile -> n block, tile origin
 struct TileXY { int nb, w0, h0, n0; };
-__device__ __forceinline__ TileXY tile_origin(const GemmParams& p, int tile, int lw) {
+__device__ __forceinline__ TileXY tile_origin(const GemmParams& p, int tile) {
   TileXY t;
   const int m = fdiv(tile, p.fd_nb);
   t.nb = tile - m * p.n_blocks;
   const int mh = fdiv(m, p.fd_tw);                 // m / tiles_w
-  t.w0 = (m - mh * p.tiles_w) << lw;
+  t.w0 = (m - mh * p.tiles_w) << p.lTW;
   const int n = fdiv(m, p.fd_twh);                 // m / (tiles_w * tiles_h)
   t.h0 = (mh - n * p.tiles_h) << p.lTH;
   t.n0 = n << p.lTN;
   return t;
-}
-
-// Static tile schedule.  A CTA walks "slots" first, first+step, ... < limit; a slot is a tile, or — with CTA pairs — a super
-// tile (two adjacent M tiles x one N block) of which the CTA takes the M tile of its cluster rank.  An odd M-tile count leaves
-// the last pair's second CTA a tile past the end: it runs the same protocol on zero-filled loads and fully clipped stores.
-struct Sched { int first, step, limit, rank; };
-__device__ __forceinline__ Sched make_sched(const GemmParams& p) {
-  Sched s;
-  if (p.pair) { s.first = blockIdx.x >> 1; s.step = gridDim.x >> 1; s.limit = p.n_super; s.rank = static_cast<int>(cluster_ctarank()); }
-  else { s.first = blockIdx.x; s.step = gridDim.x; s.limit = p.num_tiles; s.rank = 0; }
-  return s;
-}
-__device__ __forceinline__ int slot_tile(const GemmParams& p, const Sched& s, int slot) {
-  if (!p.pair) return slot;
-  const int mp = fdiv(slot, p.fd_nb);
-  return (2 * mp + s.rank) * p.n_blocks + (slot - mp * p.n_blocks);
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
@@ -102,588 +82,238 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-__device__ __forceinline__ int lane_id() { return static_cast<int>(threadIdx.x & 31); }
-
-// ---- MMA issuer role (warp 1), templated on the number of UMMA_K=16 steps per k-block and on resident weights so the
-// issue sequence is straight-line code.  The WHOLE warp runs the loop with warp-uniform values and one elected lane
-// issues: descriptors and TMEM addresses then live in uniform registers (a single active lane made ptxas wrap every
-// tcgen05.mma in an ELECT/R2UR.BROADCAST loop: ~100 SASS instructions per k-block).  Every elect block costs the warp
-// ~60 dependent instructions (~300 cycles: R2UR moves, constant loads, reconvergence) — more than the tensor time of a
-// k-block at BN <= 128 — so the loops below issue as much as they can per block: with resident weights all nine taps of
-// a halo chunk (plus both commits) go out under ONE elect, otherwise one block per k-block with the commits folded in.
-// (CC_DBG bisection + ncu source view, profiles/round1/r02_issue_loop.md)
-template <int KPB>
-__device__ __forceinline__ void mma_kblock(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  umma_f16(d_tmem, adesc, bdesc, idesc, accumulate);
-#pragma unroll
-  for (int k = 1; k < KPB; ++k) umma_f16_c<true>(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc);
+// One k-block (BK channels = KPB steps of K = 16) of this warpgroup's 64 x BN accumulator.
+template <int BN>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t adesc, uint64_t bdesc, int kpb, bool first) {
+  Wgmma<BN>::mma(acc, adesc, bdesc, first ? 0u : 1u);
+  for (int k = 1; k < kpb; ++k) Wgmma<BN>::mma(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
 }
 
-template <int KPB, bool BRES>
-__device__ __forceinline__ void mma_issuer(const GemmParams& p, uint8_t* sA, uint8_t* sB, uint32_t row_bytes, uint32_t a_bytes,
-                                           uint32_t b_bytes, int S, int num_kb, uint64_t* full_bar, uint64_t* empty_bar,
-                                           uint64_t* tfull_bar, uint64_t* tempty_bar, uint64_t* afull_bar,
-                                           uint64_t* aempty_bar, uint64_t* bres_bar, uint32_t tmem_base) {
-    const uint32_t idesc = umma_idesc_f16(kTileM, p.BN, p.ab_fmt);
-    // constant upper parts of the K-major swizzled descriptors (LBO=1, SBO, version 1, swizzle mode)
-    const uint64_t lay = row_bytes == 128 ? 2ull : (row_bytes == 64 ? 4ull : 6ull);
-    const uint64_t dconst = (1ull << 16) | (1ull << 46) | (lay << 61);
-    const uint64_t d_tile = dconst | (static_cast<uint64_t>((8u * row_bytes) >> 4) << 32);    // dense 128-row tiles
-    const uint64_t d_halo = dconst | (static_cast<uint64_t>((static_cast<uint32_t>(p.halo_pitch) * row_bytes) >> 4) << 32);   // halo views: 8-px groups one halo row apart
-    const uint32_t sA16 = (smem_u32(sA) & 0x3FFFF) >> 4, sB16 = (smem_u32(sB) & 0x3FFFF) >> 4;
-    const uint32_t a16 = a_bytes >> 4, b16 = b_bytes >> 4, h16 = p.halo_bytes >> 4;
-    const Sched sc = make_sched(p);
-    const int cpt = p.chunks_per_tap, hstages = p.halo_stages;
-    const bool pair = p.pair != 0;
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const int n_acc = p.n_acc;
-    const uint32_t acc_cols = kTmemCols / n_acc;
-    if (BRES) { mbar_wait(bres_bar, 0); tc_fence_after(); }
-    bool first = p.trace != nullptr && blockIdx.x == 0;          // timeline of CTA 0 (cc_yolo_trace): first operands landed
-    if (p.halo) {
-      int sa = 0;
-      uint32_t pa = 0;
-      const uint32_t rstep16 = ((static_cast<uint32_t>(p.halo_pitch) << p.lTN) * row_bytes) >> 4;  // one halo row block (TN images x pitch px), in 16-B units
-      const uint32_t sstep16 = row_bytes >> 4;                      // one pixel
-      const uint32_t btap16 = cpt * b16;                            // resident weights: descriptor step between taps
-      for (int slot = sc.first; slot < sc.limit; slot += sc.step) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * acc_cols;
-        for (int ch = 0; ch < cpt; ++ch) {
-          mbar_wait(&afull_bar[sa], pa);
-          tc_fence_after();
-          if (first) { first = false; if (lane_id() == 0) p.trace[3] = globaltimer_ns(); }
-          const uint64_t a_base = d_halo | (sA16 + sa * h16);
-          if (BRES) {
-            if (elect_one()) {
-              const uint64_t b_base = d_tile | (sB16 + ch * b16);
-#pragma unroll
-              for (int t = 0; t < 9; ++t)
-                mma_kblock<KPB>(d_tmem, a_base + ((t / 3) * rstep16 + (t % 3) * sstep16), b_base + t * btap16, idesc,
-                                t == 0 ? static_cast<uint32_t>(ch != 0) : 1u);
-              umma_commit(&aempty_bar[sa]);
-              if (ch == cpt - 1) umma_commit(&tfull_bar[acc]);
-            }
-            __syncwarp();
-          } else {
-#pragma unroll 1
-            for (int t = 0; t < 9; ++t) {
-              mbar_wait(&full_bar[stage], phase);
-              tc_fence_after();
-              if (elect_one()) {
-                const int r = t / 3;
-                mma_kblock<KPB>(d_tmem, a_base + (r * rstep16 + (t - 3 * r) * sstep16), d_tile | (sB16 + stage * b16), idesc,
-                                static_cast<uint32_t>((ch | t) != 0));
-                if (pair) umma_commit_mc(&empty_bar[stage], 3); else umma_commit(&empty_bar[stage]);
-                if (t == 8) {
-                  umma_commit(&aempty_bar[sa]);
-                  if (ch == cpt - 1) umma_commit(&tfull_bar[acc]);
-                }
-              }
-              __syncwarp();
-              if (++stage == S) { stage = 0; phase ^= 1; }
-            }
-          }
-          if (++sa == hstages) { sa = 0; pa ^= 1; }
-        }
-        if (++acc == n_acc) { acc = 0; acc_phase ^= 1; }
-      }
-    } else {
-      const bool whole_tile = BRES && num_kb <= 4 && num_kb <= S && !(p.dbg & 8);
-      for (int slot = sc.first; slot < sc.limit; slot += sc.step) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * acc_cols;
-        if (whole_tile) {
-          // small-K tile with resident weights (1x1 convs, K <= 256): wait for all its activation stages, then issue the
-          // whole tile under ONE elect block (an elect block costs the warp ~300 cycles, more than the MMAs of a k-block)
-          int s2 = stage;
-          uint32_t ph2 = phase;
-          for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait(&full_bar[s2], ph2);
-            if (++s2 == S) { s2 = 0; ph2 ^= 1; }
-          }
-          tc_fence_after();
-          if (first) { first = false; if (lane_id() == 0) p.trace[3] = globaltimer_ns(); }
-          if (elect_one()) {
-            int s3 = stage;
-#pragma unroll
-            for (int kb = 0; kb < 4; ++kb) {
-              if (kb < num_kb) {
-                mma_kblock<KPB>(d_tmem, d_tile | (sA16 + s3 * a16), d_tile | (sB16 + kb * b16), idesc, static_cast<uint32_t>(kb != 0));
-                umma_commit(&empty_bar[s3]);
-                if (++s3 == S) s3 = 0;
-              }
-            }
-            umma_commit(&tfull_bar[acc]);
-          }
-          __syncwarp();
-          stage = s2;
-          phase = ph2;
-        } else {
-          for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            if (first) { first = false; if (lane_id() == 0) p.trace[3] = globaltimer_ns(); }
-            if (elect_one()) {
-              mma_kblock<KPB>(d_tmem, d_tile | (sA16 + stage * a16), d_tile | (sB16 + (BRES ? kb : stage) * b16), idesc,
-                              static_cast<uint32_t>(kb != 0));
-              // frees this smem stage once the MMAs have read it (in both CTAs of a pair: the peer multicasts into it)
-              if (pair) umma_commit_mc(&empty_bar[stage], 3); else umma_commit(&empty_bar[stage]);
-              if (kb == num_kb - 1) umma_commit(&tfull_bar[acc]);     // accumulator complete -> epilogue
-            }
-            __syncwarp();
-            if (++stage == S) { stage = 0; phase ^= 1; }
-          }
-        }
-        if (++acc == n_acc) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-    if (p.trace != nullptr && blockIdx.x == 0 && lane_id() == 0) p.trace[4] = globaltimer_ns();   // all MMAs of CTA 0 issued
-}
-
-template <int ACT, bool F32>
+template <int ACT, bool F32, int BN>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   // 1024-B alignment for the 128B-swizzled tiles
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
+  const int wg = threadIdx.x >> 7;
   const uint32_t row_bytes = p.BK * 2;
   const uint32_t a_bytes = kTileM * row_bytes;
-  const uint32_t b_bytes = p.BN * row_bytes;
+  const uint32_t b_bytes = BN * row_bytes;
   const int S = p.stages;
   constexpr int es = F32 ? 4 : 2;
-  const int NG = p.n_acc;                                              // TMEM accumulator slots (2 or 4)
-  const int NGRP = p.n_grp;                                            // epilogue groups (== NG, or 4 column groups sharing 2 slots)
-  const int CH = p.CH;                                                 // columns per staging pass
-  const uint32_t pitch = p.tma_store ? CH * es : CH * es + 16;
-  const uint32_t stg_bytes = (kTileM * pitch + 15) & ~15u;           // one staging buffer; every epilogue group owns p.stg_nbuf of them
-  const int NBUF = p.stg_nbuf;
+  constexpr uint32_t pitch = BN * 4 + 16;                 // fp32 accumulator row in the staging buffer (+16 B: bank spread)
+  const int num_kb = p.num_taps * p.chunks_per_tap;
 
-  const uint32_t a_region = p.halo ? p.halo_stages * p.halo_bytes : S * a_bytes;   // halo mode: S = B stages
   uint8_t* sA = smem;
-  uint8_t* sB = sA + a_region;
-  const int num_kb_all = p.num_taps * p.chunks_per_tap;
+  uint8_t* sB = sA + S * a_bytes;
   // resident-B mode: sB holds ALL k-blocks of the weights (loaded once); the ring then carries A only
-  uint8_t* sStage = reinterpret_cast<uint8_t*>(
-      (reinterpret_cast<uintptr_t>(sB + (p.b_res ? num_kb_all : S) * b_bytes) + 1023) & ~uintptr_t(1023));
-  float* sBias = reinterpret_cast<float*>(sStage + stg_bytes * NGRP * NBUF);
+  uint8_t* sStage = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(sB + (p.b_res ? num_kb : S) * b_bytes) + 15) & ~uintptr_t(15));
+  float* sBias = reinterpret_cast<float*>(sStage + kTileM * pitch);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + p.cout);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + S;
-  uint64_t* tfull_bar = bars + 2 * S;           // [kMaxAcc]
-  uint64_t* tempty_bar = bars + 2 * S + 4;      // [kMaxAcc]
-  uint64_t* afull_bar = bars + 2 * S + 8;       // halo mode (up to 4 stages)
-  uint64_t* aempty_bar = bars + 2 * S + 12;
-  uint64_t* bres_bar = bars + 2 * S + 16;       // resident-B mode
-  uint64_t* res_bar = bars + 2 * S + 17;        // residual prefetch (one per staging buffer: 2 x kMaxAcc)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 25);
+  uint64_t* bres_bar = bars + 2 * S;
 
   if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[0] = globaltimer_ns();
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmB);
-    if (p.tma_store) tma_prefetch_desc(&p.tmC);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < S; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], p.pair ? 2 : 1);   // pairs: the MMA warps of both CTAs release a stage
-    }
-    for (int i = 0; i < kMaxAcc; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], p.colsplit ? (NGRP << p.lgw) : (1 << p.lgw));   // one arrival per warp that reads the slot
-      mbar_init(&afull_bar[i], 1);
-      mbar_init(&aempty_bar[i], 1);
-      mbar_init(&res_bar[2 * i], 1);
-      mbar_init(&res_bar[2 * i + 1], 1);
+      mbar_init(&empty_bar[i], kConsumers);   // one arrival per consumer warpgroup
     }
     mbar_init(bres_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, kTmemCols);
-    tmem_relinquish();
-  }
-  if (warp >= 4) {  // bias -> smem once per CTA (epilogue reads it as broadcast LDS.128)
+  if (wg > 0) {  // bias -> smem once per CTA (epilogue reads it as broadcast LDS.128)
     for (int i = threadIdx.x - 128; i < p.cout; i += kEpiThreads) sBias[i] = p.bias ? __ldg(p.bias + i) : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  if (p.pair) cluster_sync_all();   // the peer's barriers must exist before anything is multicast into its shared memory
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const Sched sc = make_sched(p);
   // PDL: let the next kernel start its prologue as our CTAs retire; everything that only touches WEIGHTS (bias above,
-  // resident / first weight tiles below) runs before griddepcontrol.wait, i.e. overlaps the previous kernel's tail.
+  // resident weight tiles below) runs before griddepcontrol.wait, i.e. overlaps the previous kernel's tail.
   // Activations of the previous layer are read only by the TMA producer (A operand) and the epilogue (residual):
   // both execute pdl_wait() first.
   pdl_trigger();
 
-  const int num_kb = p.num_taps * p.chunks_per_tap;
-
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (threadIdx.x == 0) {
       // ===================== TMA producer =====================
       int stage = 0;
       uint32_t phase = 0;
       if (p.b_res) {   // weights are not produced by the previous kernel: issued BEFORE the grid dependency wait
-        mbar_arrive_expect_tx(bres_bar, num_kb_all * b_bytes);
-        for (int kb = 0; kb < num_kb_all; ++kb) tma_load_2d(sB + kb * b_bytes, &p.tmB, bres_bar, kb * p.BK, 0);
+        mbar_arrive_expect_tx(bres_bar, num_kb * b_bytes);
+        for (int kb = 0; kb < num_kb; ++kb) tma_load_2d(sB + kb * b_bytes, &p.tmB, bres_bar, kb * p.BK, 0);
       }
       pdl_wait();
       if (p.trace && blockIdx.x == 0) p.trace[1] = globaltimer_ns();
-      if (p.halo) {
-        int sa = 0;
-        uint32_t pa = 0;
-        const int cin = p.chunks_per_tap * p.BK;
-        const uint32_t hb = b_bytes >> 1;
-        for (int slot = sc.first; slot < sc.limit; slot += sc.step) {
-          const TileXY tx = tile_origin(p, slot_tile(p, sc, slot), 3);
-          const int nb = tx.nb, w0 = tx.w0, h0 = tx.h0, n0 = tx.n0;
-          for (int ch = 0; ch < p.chunks_per_tap; ++ch) {
-            mbar_wait(&aempty_bar[sa], pa ^ 1);
-            if (p.dbg & 4) mbar_arrive(&afull_bar[sa]);
-            else {
-              mbar_arrive_expect_tx(&afull_bar[sa], p.halo_tx);
-              tma_load_5d(sA + sa * p.halo_bytes, &p.tmA, &afull_bar[sa], ch * p.BK, w0 - 1, n0, h0 - 1, 0);
-            }
-            if (++sa == p.halo_stages) { sa = 0; pa ^= 1; }
-            if (!p.b_res)
-              for (int t = 0; t < 9; ++t) {
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                mbar_arrive_expect_tx(&full_bar[stage], b_bytes);
-                if (p.pair)   // my half of the weight tile, to both CTAs; the peer sends the other half
-                  tma_load_2d_mc(sB + stage * b_bytes + sc.rank * hb, &p.tmB, &full_bar[stage], t * cin + ch * p.BK,
-                                 nb * p.BN + sc.rank * (p.BN >> 1), 3);
-                else tma_load_2d(sB + stage * b_bytes, &p.tmB, &full_bar[stage], t * cin + ch * p.BK, nb * p.BN);
-                if (++stage == S) { stage = 0; phase ^= 1; }
-              }
-          }
-        }
-      } else
-      for (int slot = sc.first; slot < sc.limit; slot += sc.step) {
-        const TileXY tx = tile_origin(p, slot_tile(p, sc, slot), p.lTW);
-        const int nb = tx.nb, w0 = tx.w0, h0 = tx.h0, n0 = tx.n0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        const TileXY tx = tile_origin(p, tile);
         int kb = 0;
         for (int t = 0; t < p.num_taps; ++t) {
           const int c_base = p.tap[t][0];
-          const int c1 = w0 + p.tap[t][1];
-          const int c2 = p.s2 ? p.tap[t][2] : h0 + p.tap[t][2];
-          const int c3 = p.s2 ? h0 + p.tap[t][3] : n0;
-          const int c4 = p.s2 ? n0 : 0;
+          const int c1 = tx.w0 + p.tap[t][1];
+          const int c2 = p.s2 ? p.tap[t][2] : tx.h0 + p.tap[t][2];
+          const int c3 = p.s2 ? tx.h0 + p.tap[t][3] : tx.n0;
+          const int c4 = p.s2 ? tx.n0 : 0;
           for (int ch = 0; ch < p.chunks_per_tap; ++ch, ++kb) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
-            mbar_arrive_expect_tx(&full_bar[stage], (p.dbg & 4) ? (p.b_res ? 0 : b_bytes) : (p.b_res ? a_bytes : a_bytes + b_bytes));
-            if (!(p.dbg & 4))
-              tma_load_5d(sA + stage * a_bytes, &p.tmA, &full_bar[stage], c_base + ch * p.BK, c1, c2, c3, c4);
-            if (p.pair)
-              tma_load_2d_mc(sB + stage * b_bytes + sc.rank * (b_bytes >> 1), &p.tmB, &full_bar[stage], kb * p.BK,
-                             nb * p.BN + sc.rank * (p.BN >> 1), 3);
-            else if (!p.b_res) tma_load_2d(sB + stage * b_bytes, &p.tmB, &full_bar[stage], kb * p.BK, nb * p.BN);
+            mbar_arrive_expect_tx(&full_bar[stage], p.b_res ? a_bytes : a_bytes + b_bytes);
+            tma_load_5d(sA + stage * a_bytes, &p.tmA, &full_bar[stage], c_base + ch * p.BK, c1, c2, c3, c4);
+            if (!p.b_res) tma_load_2d(sB + stage * b_bytes, &p.tmB, &full_bar[stage], kb * p.BK, tx.nb * BN);
             if (++stage == S) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-#define CC_ISSUE(KPB) \
-    do { if (p.b_res) mma_issuer<KPB, true>(p, sA, sB, row_bytes, a_bytes, b_bytes, S, num_kb, full_bar, empty_bar, tfull_bar, tempty_bar, afull_bar, aempty_bar, bres_bar, tmem_base); \
-         else mma_issuer<KPB, false>(p, sA, sB, row_bytes, a_bytes, b_bytes, S, num_kb, full_bar, empty_bar, tfull_bar, tempty_bar, afull_bar, aempty_bar, bres_bar, tmem_base); } while (0)
-    if (p.BK == 64) CC_ISSUE(4);
-    else if (p.BK == 32) CC_ISSUE(2);
-    else CC_ISSUE(1);
-#undef CC_ISSUE
-  } else if (warp >= 4 && warp < 4 + (NGRP << p.lgw)) {
-    // ===================== epilogue: NG independent groups of 4 or 8 warps.  Group g owns TMEM accumulator slot g, its own
-    // staging buffer, named barrier and residual barrier, and handles every NG-th tile of this CTA, so up to NG tile
-    // epilogues are in flight at once.  (One 16-warp epilogue per tile was a serial chain of ~2500 cycles — tfull wait,
-    // staging-free barrier, tcgen05.ld, activation, st.shared, proxy fence, barrier, TMA store — which set the tile rate of
-    // every small-K layer: 1.3-1.4 us per tile whatever the tile did, profiles/round1/r02_issue_loop.md.)  Inside a group the
-    // warp's TMEM lane quarter is warp & 3; with 8-warp groups (wide tiles) the two warps of a lane quarter split the
-    // 16-column chunks of a pass.  thread == output row in the register phase.
-    // Column split (p.colsplit, tiles wider than 128 columns): the in-kernel timeline showed that ONE group converting a
-    // 128 x 256 tile is a ~11000-cycle serial chain (a lone warp per scheduler issues an instruction every ~4 cycles), which is
-    // the critical path of every layer with three or fewer tiles per CTA.  There the four 4-warp groups all work on EVERY
-    // tile, group g converting columns [g BN/4, (g+1) BN/4) of it; the two accumulator slots alternate by tile. ============
-    const int lgw = p.lgw;                     // log2(warps per group): 2 or 3
-    const int grp = (warp - 4) >> lgw;
-    const int wig = (warp - 4) & ((1 << lgw) - 1);
-    const int gthreads = 32 << lgw;
-    const int gt = static_cast<int>(threadIdx.x) - 128 - grp * gthreads;   // thread within the group
-    const int ew = warp & 3;                   // TMEM lane quarter this warp may access
-    const int half = wig >> 2;                 // which 16-column chunks of a pass this warp converts
-    const int row = ew * 32 + lane;            // row of the 128-pixel tile
-    const int cstep = 16 << (lgw - 2);         // column stride between the chunks one warp converts
-    const uint32_t bar_id = 1 + grp;
-    uint8_t* const sbuf0 = sStage + grp * NBUF * stg_bytes;     // this group's staging buffers (pass k uses buffer k % NBUF)
-    const uint32_t sbias32 = smem_u32(sBias);
-    uint64_t* const rbar0 = &res_bar[2 * grp];
+  } else {
+    // ===================== consumers: warpgroup c owns rows [64 c, 64 c + 64) of every tile =====================
+    const int c = wg - 1;
+    const int et = static_cast<int>(threadIdx.x) - 128;      // 0 .. 255 over both consumers
+    const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+    const int kpb = p.BK >> 4;
+    const uint64_t dconst = gmma_desc_const(row_bytes, 8u * row_bytes);
+    const uint32_t sA16 = ((smem_u32(sA) & 0x3FFFF) >> 4) + ((c * 64 * row_bytes) >> 4), sB16 = (smem_u32(sB) & 0x3FFFF) >> 4;
+    const uint32_t a16 = a_bytes >> 4, b16 = b_bytes >> 4;
+    const uint32_t stg32 = smem_u32(sStage), sbias32 = smem_u32(sBias);
     const int TWm = (1 << p.lTW) - 1, THm = (1 << p.lTH) - 1;
-    const bool colsplit = p.colsplit != 0;
-    const uint32_t acc_cols = kTmemCols / NG;
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(ew * 32) << 16);
-    const int gcols = colsplit ? p.BN / NGRP : p.BN;      // columns of a tile this group converts
-    const int cc_begin = colsplit ? grp * gcols : 0, cc_end = cc_begin + gcols;
-    uint32_t tcount = 0;     // tiles this group has taken -> phase of its accumulator barriers
-    uint32_t pass_ctr = 0;   // staging passes of this group so far
-    const int passes_per_tile = (gcols + CH - 1) / CH;
-    // TMA-store staging: rows of 128 B (SWIZZLE_128B: 16-B chunk j of row r at slot j ^ (r & 7)) or, for tiles whose
-    // pass is an odd multiple of 64 B, rows of 64 B (SWIZZLE_64B: slot j ^ ((r >> 1) & 3)); sub-tiles of 128 rows follow
-    // each other
-    const int lrow = p.stg_lrow, srow = 1 << lrow;
-    const uint32_t swz = lrow == 7 ? (row & 7) : ((row >> 1) & 3);
-    // residual prefetch (in-place residual through tmC): the TMA load of the residual sub-tiles of this group's staging
-    // pass `k` lands in the buffer the pass will overwrite with its result; issued by thread gt == 0 as soon as the
-    // previous store has read the buffer
-    auto issue_res = [&](uint32_t k) {
-      const int jg = static_cast<int>(k) / passes_per_tile;                          // k-th pass of this group
-      const int slot_k = colsplit ? sc.first + jg * sc.step : sc.first + (grp + jg * NG) * sc.step;
-      if (slot_k >= sc.limit) return;
-      const int tile_k = slot_tile(p, sc, slot_k);
-      const int cc0k = cc_begin + (static_cast<int>(k) - jg * passes_per_tile) * CH;
-      const int chnk = (cc_end - cc0k) < CH ? (cc_end - cc0k) : CH;
-      const TileXY tk = tile_origin(p, tile_k, p.lTW);
-      const int nbk = tk.nb, w0k = tk.w0, h0k = tk.h0, n0k = tk.n0;
-      const int nsub = (chnk * es) >> lrow;
-      const uint32_t pbk = NBUF == 2 ? (k & 1u) : 0u;
-      uint8_t* const sbufk = sbuf0 + pbk * stg_bytes;
-      uint64_t* const rbark = rbar0 + pbk;
-      mbar_arrive_expect_tx(rbark, nsub * (kTileM << lrow));
-      for (int j = 0; j < nsub; ++j) {
-        const int cc = nbk * p.BN + cc0k + j * (srow / es);
-        if (p.halo) tma_load_5d(sbufk + j * (kTileM << lrow), &p.tmC, rbark, cc, w0k, n0k, h0k, 0);
-        else tma_load_5d(sbufk + j * (kTileM << lrow), &p.tmC, rbark, cc, w0k, h0k, n0k, 0);
-      }
-    };
+    // register phase: thread pair == output row, the pair's halves take columns [0, BN/2) and [BN/2, BN).  A bf16 result is
+    // written back over the fp32 accumulators it was computed from; the second half's results go after the first half's
+    // fp32 values (byte BN*2 on), so neither thread overwrites values the other has yet to read.
+    // (BN = 16 is one 16-column chunk: the first thread of the pair converts it alone)
+    constexpr bool kSplit = BN >= 32;
+    constexpr int kHalfCols = kSplit ? BN / 2 : BN;
+    const int row = et >> 1, half = et & 1;
+    const uint32_t out_off = F32 ? 0u : static_cast<uint32_t>(half) * BN * 2;    // bf16: where this half's fp32 columns start
+    int stage = 0;
+    uint32_t phase = 0;
+    bool first_tile = true;
+    if (p.b_res) mbar_wait(bres_bar, 0);
     pdl_wait();   // residual reads below depend on the previous kernel's output
-    if (p.res_tma == 1 && gt == 0) issue_res(0);
-    for (int slot = colsplit ? sc.first : sc.first + grp * sc.step; slot < sc.limit; slot += (colsplit ? 1 : NG) * sc.step, ++tcount) {
-      const uint32_t acc = colsplit ? (tcount & static_cast<uint32_t>(NG - 1)) : static_cast<uint32_t>(grp);   // accumulator slot of this tile
-      const uint32_t acc_par = colsplit ? (tcount >> (NG == 4 ? 2 : 1)) & 1u : tcount & 1u;
-      const uint32_t t_row = t_lane + acc * acc_cols;
-      const TileXY tx = tile_origin(p, slot_tile(p, sc, slot), p.lTW);
-      const int nb = tx.nb, w0 = tx.w0, h0 = tx.h0, n0 = tx.n0;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      const TileXY tx = tile_origin(p, tile);
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        if (first_tile && kb == 0 && p.trace && blockIdx.x == 0 && et == 0) p.trace[3] = globaltimer_ns();
+        wgmma_fence_acc(acc);
+        wgmma_fence();
+        mma_kblock<BN>(acc, dconst | (sA16 + stage * a16), dconst | (sB16 + (p.b_res ? kb : stage) * b16), kpb, kb == 0);
+        wgmma_commit();
+        wgmma_fence_acc(acc);
+        wgmma_wait<1>();       // the previous k-block's MMAs are done: release its stage
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == S) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+      if (first_tile && p.trace && blockIdx.x == 0 && et == 0) p.trace[5] = globaltimer_ns();
+      first_tile = false;
 
-      // this thread's pixel (register phase: residual read)
-      int pw, ph, pn;
-      if (p.halo) { pw = w0 + (row & 7); pn = n0 + ((row >> 3) & ((1 << p.lTN) - 1)); ph = h0 + (row >> (3 + p.lTN)); }
-      else { pw = w0 + (row & TWm); ph = h0 + ((row >> p.lTW) & THm); pn = n0 + (row >> (p.lTW + p.lTH)); }
+      // ---- accumulators -> staging (fp32 rows of `pitch` bytes)
+      named_bar_sync(1, kEpiThreads);     // the previous tile's copy-out has read the staging buffer
+      {
+        const int r0 = c * 64 + wq * 16 + (lane >> 2);
+        const uint32_t base = stg32 + r0 * pitch + (lane & 3) * 8;
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i) {
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(base + i * 32), "f"(acc[4 * i]), "f"(acc[4 * i + 1]) : "memory");
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(base + 8 * pitch + i * 32), "f"(acc[4 * i + 2]), "f"(acc[4 * i + 3]) : "memory");
+        }
+      }
+      named_bar_sync(1, kEpiThreads);
+
+      // ---- register phase: this thread's pixel, columns [half BN/2, (half+1) BN/2)
+      const int nb = tx.nb, w0 = tx.w0, h0 = tx.h0, n0 = tx.n0;
+      const int pw = w0 + (row & TWm), ph = h0 + ((row >> p.lTW) & THm), pn = n0 + (row >> (p.lTW + p.lTH));
       const bool pvalid = (pw < p.W) && (ph < p.H) && (pn < p.N);
       const long long ppix = static_cast<long long>(pn) * p.out_ns + ph * p.W + pw;
       // pre-activation addend from a half-resolution fp32 map (nearest x2 upsample by addressing): this pixel's source row
       const float* const pre_row = (p.pre != nullptr && pvalid)
           ? p.pre + ((static_cast<long long>(pn) * p.pre_h + (ph >> 1)) * p.pre_w + (pw >> 1)) * p.cout : nullptr;
-
-      mbar_wait(&tfull_bar[acc], acc_par);
-      tc_fence_after();
-      if (p.trace != nullptr && blockIdx.x == 0 && gt == 0 && grp == 0 && tcount == 0) p.trace[5] = globaltimer_ns();   // first accumulator complete
-      if (p.dbg & 1) {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-        continue;
-      }
-
-      for (int cc0 = cc_begin; cc0 < cc_end; cc0 += CH) {
-        const int chn = (cc_end - cc0) < CH ? (cc_end - cc0) : CH;  // columns in this pass (multiple of 16)
-        const uint32_t pb = NBUF == 2 ? (pass_ctr & 1u) : 0u;      // staging buffer of this pass
-        uint8_t* const sbuf = sbuf0 + pb * stg_bytes;
-        const uint32_t sbuf32 = smem_u32(sbuf);
-        if (p.res_tma == 1) {
-          // the residual tile has landed in the staging buffer (which also proves the buffer was free)
-          mbar_wait(rbar0 + pb, (NBUF == 2 ? (pass_ctr >> 1) : pass_ctr) & 1);
-        } else {
-          // the store that last read this buffer is done with it: the previous one (one buffer), or the one before it (two
-          // buffers: the previous pass's store may still be in flight — a TMA store takes ~0.3 us to issue and its smem read
-          // completes well after that, time a single buffer spent idle every pass)
-          if (p.tma_store && gt == 0) { if (NBUF == 2) tma_store_wait_read<1>(); else tma_store_wait_read<0>(); }
-          named_bar_sync(bar_id, gthreads);                        // staging buffer free
+      const uint32_t srow = stg32 + row * pitch;
+#pragma unroll 1
+      for (int cc = half * kHalfCols; cc < (kSplit || half == 0 ? (half + 1) * kHalfCols : 0); cc += 16) {
+        const int gcol = nb * BN + cc;   // global output channel of column cc
+        float f[16];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const uint4 vu = lds_u4(srow + (cc + 4 * j) * 4);
+          const float4 v = make_float4(__uint_as_float(vu.x), __uint_as_float(vu.y), __uint_as_float(vu.z), __uint_as_float(vu.w));
+          float4 b4 = lds_f4(sbias32 + (gcol + 4 * j) * 4);
+          if (pre_row != nullptr) {
+            const float4 q4 = __ldg(reinterpret_cast<const float4*>(pre_row + gcol) + j);
+            b4.x += q4.x; b4.y += q4.y; b4.z += q4.z; b4.w += q4.w;
+          }
+          f[4 * j] = act_apply<ACT>(v.x + b4.x);
+          f[4 * j + 1] = act_apply<ACT>(v.y + b4.y);
+          f[4 * j + 2] = act_apply<ACT>(v.z + b4.z);
+          f[4 * j + 3] = act_apply<ACT>(v.w + b4.w);
         }
-        const bool tr = p.trace != nullptr && blockIdx.x == 0 && gt == 0 && grp == 0 && tcount == 0 && cc0 == cc_begin;
-        if (tr) p.trace[8] = static_cast<unsigned long long>(clock64());   // first pass, SM cycles: staging free
-        // one 16-column chunk of this thread's row: + bias -> activation -> (+ residual) -> staging
-        auto chunk = [&](const int c, const uint32_t (&v)[16]) {
-          const int gcol = nb * p.BN + cc0 + c;  // global output channel of v[0]
-          float f[16];
+        if (p.res != nullptr && pvalid) {
+          if (F32) {
+            const float4* r4 = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.res) + ppix * p.res_cs + p.res_co + gcol);
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float4 b4 = lds_f4(sbias32 + (gcol + 4 * j) * 4);
-            if (pre_row != nullptr) {
-              const float4 q4 = __ldg(reinterpret_cast<const float4*>(pre_row + gcol) + j);
-              b4.x += q4.x; b4.y += q4.y; b4.z += q4.z; b4.w += q4.w;
-            }
-            f[4 * j] = act_apply<ACT>(__uint_as_float(v[4 * j]) + b4.x);
-            f[4 * j + 1] = act_apply<ACT>(__uint_as_float(v[4 * j + 1]) + b4.y);
-            f[4 * j + 2] = act_apply<ACT>(__uint_as_float(v[4 * j + 2]) + b4.z);
-            f[4 * j + 3] = act_apply<ACT>(__uint_as_float(v[4 * j + 3]) + b4.w);
-          }
-          if (p.res_tma == 2) {
-            // nothing to read: the TMA reduce-add store adds the residual in place
-          } else if (p.res_tma == 1) {
-            const uint32_t boff = c * es;
-            const uint32_t sub = sbuf32 + (boff >> lrow) * (kTileM << lrow) + (row << lrow);
-            const uint32_t ch0 = (boff & (srow - 1)) >> 4;
-            if (F32) {
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const uint4 ru = lds_u4(sub + (((ch0 + j) ^ swz) << 4));
-                const float4 r = make_float4(__uint_as_float(ru.x), __uint_as_float(ru.y), __uint_as_float(ru.z), __uint_as_float(ru.w));
-                f[4 * j + 0] += r.x; f[4 * j + 1] += r.y; f[4 * j + 2] += r.z; f[4 * j + 3] += r.w;
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 2; ++j) {
-                const uint4 r = lds_u4(sub + (((ch0 + j) ^ swz) << 4));
-                const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  f[8 * j + 2 * q + 0] += __uint_as_float(rr[q] << 16);
-                  f[8 * j + 2 * q + 1] += __uint_as_float(rr[q] & 0xFFFF0000u);
-                }
-              }
-            }
-          } else if (p.res != nullptr && pvalid) {
-            if (F32) {
-              const float4* r4 = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.res) +
-                                                                 ppix * p.res_cs + p.res_co + gcol);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const float4 r = __ldg(r4 + j);
-                f[4 * j + 0] += r.x; f[4 * j + 1] += r.y; f[4 * j + 2] += r.z; f[4 * j + 3] += r.w;
-              }
-            } else {
-              const uint4* r4 = reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(p.res) +
-                                                               ppix * p.res_cs + p.res_co + gcol);
-#pragma unroll
-              for (int j = 0; j < 2; ++j) {
-                const uint4 r = __ldg(r4 + j);
-                const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  // bf16 -> fp32 is a 16-bit shift
-                  f[8 * j + 2 * q + 0] += __uint_as_float(rr[q] << 16);
-                  f[8 * j + 2 * q + 1] += __uint_as_float(rr[q] & 0xFFFF0000u);
-                }
-              }
-            }
-          }
-          if (p.tma_store) {
-            const uint32_t boff = c * es;                       // byte offset of this 16-column group in the pass row
-            const uint32_t sub = sbuf32 + (boff >> lrow) * (kTileM << lrow) + (row << lrow);
-            const uint32_t ch0 = (boff & (srow - 1)) >> 4;
-            if (F32) {
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                sts_u4(sub + (((ch0 + j) ^ swz) << 4), __float_as_uint(f[4 * j]), __float_as_uint(f[4 * j + 1]), __float_as_uint(f[4 * j + 2]),
-                       __float_as_uint(f[4 * j + 3]));
-            } else {
-#pragma unroll
-              for (int j = 0; j < 2; ++j)
-                sts_u4(sub + (((ch0 + j) ^ swz) << 4), pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
-                       pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7]));
+            for (int j = 0; j < 4; ++j) {
+              const float4 r = __ldg(r4 + j);
+              f[4 * j + 0] += r.x; f[4 * j + 1] += r.y; f[4 * j + 2] += r.z; f[4 * j + 3] += r.w;
             }
           } else {
-            uint8_t* dst = sbuf + row * pitch + c * es;
-            if (F32) {
+            const uint4* r4 = reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(p.res) + ppix * p.res_cs + p.res_co + gcol);
 #pragma unroll
-              for (int j = 0; j < 4; ++j)
-                *reinterpret_cast<float4*>(dst + 16 * j) = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-            } else {
+            for (int j = 0; j < 2; ++j) {
+              const uint4 r = __ldg(r4 + j);
+              const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
 #pragma unroll
-              for (int j = 0; j < 2; ++j)
-                *reinterpret_cast<uint4*>(dst + 16 * j) =
-                    make_uint4(pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
-                               pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7]));
-            }
-          }
-        };
-        // two chunks' TMEM loads go out before the one tcgen05.wait::ld (the in-kernel timeline puts the TMEM read at ~150 cycles;
-        // the conversion of a chunk at 450-950 cycles depending on how many warps share the scheduler's MUFU pipe)
-        for (int c = half * 16; c < chn; c += 2 * cstep) {
-          const bool two = c + cstep < chn;                        // warp-uniform
-          uint32_t va[16], vb[16];
-          tmem_ld16(t_row + cc0 + c, va);
-          if (two) tmem_ld16(t_row + cc0 + c + cstep, vb);
-          tmem_ld_wait();
-          if (tr && c == half * 16) p.trace[9] = static_cast<unsigned long long>(clock64());     // ... TMEM loads returned
-          chunk(c, va);
-          if (tr && c == half * 16) p.trace[10] = static_cast<unsigned long long>(clock64());    // ... first chunk staged
-          if (two) chunk(c + cstep, vb);
-        }
-        if (cc0 + CH >= cc_end) {
-          // all TMEM reads of this accumulator done -> hand it back to the MMA warp.  ONE arrival per warp: hundreds of
-          // threads arriving on the same mbarrier serialise in the LSU (CC_DBG bisection, profiles/round1/)
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-        }
-        if (tr) p.trace[11] = static_cast<unsigned long long>(clock64());  // ... all of this thread's chunks staged
-        if (p.tma_store) {
-          fence_proxy_async_smem();          // generic-proxy smem writes -> visible to the TMA (async proxy)
-          named_bar_sync(bar_id, gthreads);  // staging filled
-          if (gt == 0) {
-            const int nsub = (chn * es) >> lrow;
-            const int col0 = nb * p.BN + cc0;
-            for (int j = 0; j < nsub; ++j) {
-              const int cc = col0 + j * (srow / es);
-              if (p.res_tma == 2) {   // out += tile (fp32 in-place residual, added at the L2)
-                if (p.halo) tma_reduce_add_5d(&p.tmC, sbuf + j * (kTileM << lrow), cc, w0, n0, h0, 0);
-                else tma_reduce_add_5d(&p.tmC, sbuf + j * (kTileM << lrow), cc, w0, h0, n0, 0);
-              } else if (p.halo) tma_store_5d(&p.tmC, sbuf + j * (kTileM << lrow), cc, w0, n0, h0, 0);
-              else tma_store_5d(&p.tmC, sbuf + j * (kTileM << lrow), cc, w0, h0, n0, 0);
-            }
-            tma_store_commit();
-            if (p.res_tma == 1) {
-              // the next pass's buffer is free once its last store has read it (this one with a single buffer, the
-              // previous one with two)
-              if (NBUF == 2) tma_store_wait_read<1>(); else tma_store_wait_read<0>();
-              issue_res(pass_ctr + 1);
-            }
-          }
-          ++pass_ctr;
-          continue;
-        }
-        named_bar_sync(bar_id, gthreads);  // staging filled
-        // coalesced copy-out, division free: a set of `1 << lg` (power of two >= chunks per row) lanes owns one row
-        const int cpr = (chn * es) >> 4;  // 16-B chunks per row (2..16)
-        const int lg = cpr > 8 ? 4 : (cpr > 4 ? 3 : (cpr > 2 ? 2 : 1));
-        const int chk = gt & ((1 << lg) - 1);
-        const int rstep = gthreads >> lg;
-        if (chk < cpr) {
-          uint8_t* gbase = reinterpret_cast<uint8_t*>(p.out) + static_cast<size_t>(p.out_co + nb * p.BN + cc0) * es + chk * 16;
-          for (int r = gt >> lg; r < kTileM; r += rstep) {
-            int qw, qh, qn;
-            if (p.halo) { qw = w0 + (r & 7); qn = n0 + ((r >> 3) & ((1 << p.lTN) - 1)); qh = h0 + (r >> (3 + p.lTN)); }
-            else { qw = w0 + (r & TWm); qh = h0 + ((r >> p.lTW) & THm); qn = n0 + (r >> (p.lTW + p.lTH)); }
-            if (qw < p.W && qh < p.H && qn < p.N) {
-              const long long pix = static_cast<long long>(qn) * p.out_ns + qh * p.W + qw;
-              const uint4 val = *reinterpret_cast<const uint4*>(sbuf + r * pitch + chk * 16);
-              *reinterpret_cast<uint4*>(gbase + pix * p.out_cs * es) = val;
+              for (int q = 0; q < 4; ++q) {
+                // bf16 -> fp32 is a 16-bit shift
+                f[8 * j + 2 * q + 0] += __uint_as_float(rr[q] << 16);
+                f[8 * j + 2 * q + 1] += __uint_as_float(rr[q] & 0xFFFF0000u);
+              }
             }
           }
         }
-        ++pass_ctr;
+        // in place: fp32 results over their own accumulators; bf16 results of column cc at out_off + 2 (cc - half BN/2), which
+        // only covers fp32 columns of this thread that it has already read
+        const uint32_t dst = F32 ? srow + cc * 4 : srow + out_off + (cc - half * kHalfCols) * 2;
+        if (F32) {
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+            sts_u4(dst + 16 * j, __float_as_uint(f[4 * j]), __float_as_uint(f[4 * j + 1]), __float_as_uint(f[4 * j + 2]), __float_as_uint(f[4 * j + 3]));
+        } else {
+#pragma unroll
+          for (int j = 0; j < 2; ++j)
+            sts_u4(dst + 16 * j, pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
+                   pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7]));
+        }
+      }
+      named_bar_sync(1, kEpiThreads);    // results staged
+
+      // ---- coalesced copy-out, division free: a set of `1 << lg` (power of two >= chunks per row) threads owns one row
+      constexpr int cpr = (BN * es) >> 4;  // 16-B chunks per row (2..32)
+      constexpr int hcpr = cpr / 2;        // chunks of one half
+      constexpr int lg = cpr > 16 ? 5 : (cpr > 8 ? 4 : (cpr > 4 ? 3 : (cpr > 2 ? 2 : 1)));
+      const int chk = et & ((1 << lg) - 1);
+      constexpr int rstep = kEpiThreads >> lg;
+      if (chk < cpr) {
+        // bf16: the second half's results start at byte 2 BN of the staging row (see out_off)
+        const uint32_t soff = (F32 || !kSplit) ? chk * 16 : (chk < hcpr ? chk * 16 : BN * 2 + (chk - hcpr) * 16);
+        uint8_t* gbase = reinterpret_cast<uint8_t*>(p.out) + static_cast<size_t>(p.out_co + nb * BN) * es + chk * 16;
+        for (int r = et >> lg; r < kTileM; r += rstep) {
+          const int qw = w0 + (r & TWm), qh = h0 + ((r >> p.lTW) & THm), qn = n0 + (r >> (p.lTW + p.lTH));
+          if (qw < p.W && qh < p.H && qn < p.N) {
+            const long long pix = static_cast<long long>(qn) * p.out_ns + qh * p.W + qw;
+            const uint4 val = lds_u4(stg32 + r * pitch + soff);
+            *reinterpret_cast<uint4*>(gbase + pix * p.out_cs * es) = val;
+          }
+        }
       }
     }
-    if (p.tma_store && gt == 0) tma_store_wait_read<0>();   // smem must outlive the bulk stores' reads (global completion is tracked by the grid)
-    if (p.trace != nullptr && blockIdx.x == 0 && gt == 0) atomicMax(p.trace + 6, globaltimer_ns());   // last epilogue group of CTA 0 done
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (p.pair) cluster_sync_all();   // the peer may still multicast into / arrive on this CTA's shared memory until it is done too
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
+    if (p.trace != nullptr && blockIdx.x == 0 && et == 0) p.trace[6] = globaltimer_ns();   // last epilogue of CTA 0 done
   }
   if (p.trace && threadIdx.x == 0) {
     atomicMax(p.trace + 2, globaltimer_ns());
@@ -721,45 +351,16 @@ int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
   p.BK = (d.Cin % 64 == 0) ? 64 : (d.Cin % 32 == 0 ? 32 : 16);
   p.num_taps = d.k * d.k;
   p.chunks_per_tap = d.Cin / p.BK;
-  // ---- N blocking
-  int BN = d.bn_override;
-  if (BN == 0) {
-    static const int f32bn_env = getenv("CC_F32_BN") ? atoi(getenv("CC_F32_BN")) : 256;
-    const int maxbn = d.out_f32 ? f32bn_env : 256;   // fp32 output: 64-column staging passes, so 256-wide tiles fit too
-    // largest multiple of 16 that divides Cout and fits the tile limit
-    for (BN = (d.Cout < maxbn ? d.Cout : maxbn) & ~15; BN >= 16; BN -= 16)
-      if (d.Cout % BN == 0) break;
-    const long long mt = (static_cast<long long>(d.N) * Hout * Wout + 127) / 128;
-    static const int bnmodel_env = getenv("CC_BN_MODEL") ? atoi(getenv("CC_BN_MODEL")) : 2;
-    // measured (same-box A/B): the model helps the fp32-output GEMMs of the ViT (+7 % ViT-B/32) and costs the bf16
-    // conv stack 1 %, so by default it is applied to fp32 outputs only (1 = everywhere, 0 = never)
-    if (bnmodel_env == 1 || (bnmodel_env == 2 && d.out_f32)) {
-      // pick the N tile by a small cost model: rounds over the SMs x per-tile time, where a tile costs the larger of its
-      // MMA time (2*BN cycles per 64-deep k-block, ~160-cycle issue floor) and its L2->SM load time, plus the epilogue
-      const int bk = (d.Cin % 64 == 0) ? 64 : (d.Cin % 32 == 0 ? 32 : 16);
-      const double nkb = double(d.k) * d.k * d.Cin / bk;
-      double best_cost = 1e30;
-      int best_bn = BN;
-      for (int bn = (d.Cout < maxbn ? d.Cout : maxbn) & ~15; bn >= 16; bn -= 16) {
-        if (d.Cout % bn) continue;
-        const double tiles = double(mt) * (d.Cout / bn);
-        const double rounds = ceil(tiles / num_sms);
-        const double mma = nkb * (2.0 * bn > 160 ? 2.0 * bn : 160.0) * bk / 64.0;
-        static const double halo_cost = getenv("CC_HALO_COST") ? atof(getenv("CC_HALO_COST")) : 2.25;
-        const double a_bytes = (d.k == 3 && d.stride == 1 && bk >= 32) ? 128.0 * bk * 2 * halo_cost / 9 : 128.0 * bk * 2;  // halo re-use
-        const double load = nkb * (a_bytes + bn * bk * 2.0) / 40.0;
-        const double epi = bn * 10.0 + 600.0;
-        const double tile = (mma > load ? mma : load);
-        const double cost = rounds * (tile > epi ? tile : epi) + epi + 3000.0;
-        if (cost < best_cost * 0.999) { best_cost = cost; best_bn = bn; }
-      }
-      BN = best_bn;
-    } else {
-      // if the machine would be under-filled, halve the N tile (more, smaller tiles)
-      while (BN > 64 && (BN / 2) % 16 == 0 && mt * (d.Cout / BN) < num_sms) BN /= 2;
-    }
-  }
-  CC_REQUIRE(BN % 16 == 0 && BN >= 16 && BN <= 256 && d.Cout % BN == 0, "conv_gemm: bad BN=%d for Cout=%d", BN, d.Cout);
+  // ---- N blocking: a power of two in [16, 128] that divides Cout (the kernel is compiled for those four widths); an
+  // override is taken as an upper bound
+  const long long mt = (static_cast<long long>(d.N) * Hout * Wout + 127) / 128;
+  const int maxbn = d.bn_override > 0 && d.bn_override < kMaxBN ? d.bn_override : kMaxBN;
+  int BN = 16;
+  while (BN * 2 <= maxbn && d.Cout % (BN * 2) == 0) BN *= 2;
+  // if the machine would be under-filled, halve the N tile (more, smaller tiles)
+  if (d.bn_override == 0)
+    while (BN > 64 && mt * (d.Cout / BN) < num_sms) BN /= 2;
+  CC_REQUIRE(BN >= 16 && BN <= kMaxBN && d.Cout % BN == 0, "conv_gemm: bad BN=%d for Cout=%d", BN, d.Cout);
   p.BN = BN;
   p.n_blocks = d.Cout / BN;
   p.cout = d.Cout;
@@ -771,44 +372,17 @@ int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
     for (int lh = 0; lw + lh <= 7; ++lh) {
       const int ln = 7 - lw - lh;
       const int tw = 1 << lw, th = 1 << lh, tn = 1 << ln;
-      if (tw > 256 || th > 256 || tn > 256) continue;
       const double cover = double((Wout + tw - 1) / tw * tw) * ((Hout + th - 1) / th * th) * ((d.N + tn - 1) / tn * tn);
       double eff = double(Wout) * Hout * d.N / cover + 1e-6 * lw - 1e-7 * ln;  // ties: wider rows, fewer images
       if (eff > best_eff) { best_eff = eff; best[0] = lw; best[1] = lh; best[2] = ln; }
     }
   p.lTW = best[0]; p.lTH = best[1]; p.lTN = best[2];
-  // halo mainloop for 3x3 stride-1 convs with 64-channel chunks: tile = 8 px wide x (TH rows x TN images), TH*TN = 16
-  static const int halo_env = getenv("CC_HALO") ? atoi(getenv("CC_HALO")) : 1;
-  static const int halo_bo_env = getenv("CC_HALO_BO") ? atoi(getenv("CC_HALO_BO")) : 0;
-  p.halo = (halo_env && d.k == 3 && d.stride == 1 && d.Cin % 32 == 0) ? 1 : 0;   // BK = 64 (128-B rows) or 32 (64-B rows)
-  p.halo_bo = halo_bo_env;
-  if (p.halo) {
-    double be = -1;
-    for (int lh = 0; lh <= 4; ++lh) {
-      const int th = 1 << lh, tn = 16 >> lh;
-      const double cover = double((Hout + th - 1) / th * th) * ((d.N + tn - 1) / tn * tn);
-      const double eff = double(Hout) * d.N / cover + 1e-6 * lh;   // ties: taller tiles (fewer halo rows per output row)
-      if (eff > be) { be = eff; p.lTH = lh; p.lTN = 4 - lh; }
-    }
-    p.lTW = 3;
-    // Halo row pitch in shared memory.  The taps read pixels w0-1 .. w0+8 of a row: 10 pixels.  Round 1 loaded 16 (a
-    // power-of-two pitch keeps every 8-pixel group on a swizzle-atom boundary), i.e. 2.25x the tile's own bytes from L2 per
-    // chunk; the small-channel 3x3 layers move ~5 TB/s between L2 and the SMs, which is where that fabric saturates, with
-    // both pipes idle.  The swizzle XOR is a function of ABSOLUTE shared-memory address bits for TMA writes and UMMA reads
-    // alike (the tap views already start 128 B off an atom boundary), so a 10-pixel pitch (stride between 8-row groups =
-    // 10 rows, not a multiple of the atom) reads back what was written: 1.41x instead of 2.25x.
-    static const int hpitch_env = getenv("CC_HALO_PITCH") ? atoi(getenv("CC_HALO_PITCH")) : 10;
-    p.halo_pitch = hpitch_env == 16 ? 16 : 10;
-    p.halo_tx = p.BK * p.halo_pitch * (1 << p.lTN) * ((1 << p.lTH) + 2) * 2;
-    p.halo_bytes = (p.halo_tx + 1023) & ~1023;                  // stage stride: buffers stay 1024-B aligned
-  }
   const int TW = 1 << p.lTW, TH = 1 << p.lTH, TN = 1 << p.lTN;
   p.tiles_w = (Wout + TW - 1) / TW;
   p.tiles_h = (Hout + TH - 1) / TH;
   p.tiles_n = (d.N + TN - 1) / TN;
   p.num_tiles = p.tiles_w * p.tiles_h * p.tiles_n * p.n_blocks;
   p.s2 = d.stride == 2;
-  p.ab_fmt = 1;
 
   // ---- taps
   const int pad = d.k / 2;
@@ -834,12 +408,7 @@ int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
     cuuint64_t dims[5], strides[4];
     cuuint32_t box[5], estr[5] = {1, 1, 1, 1, 1};
     const cuuint64_t px = cuuint64_t(d.in_cs) * 2;  // bytes per pixel
-    if (p.halo) {
-      // (C, W, N, H): the box [64 ch][pitch px][TN images][TH+2 rows] lands in smem as [row][image][pixel][128 B]
-      dims[0] = d.Cin; dims[1] = d.Win; dims[2] = d.N; dims[3] = d.Hin; dims[4] = 1;
-      strides[0] = px; strides[1] = px * d.Win * d.Hin; strides[2] = px * d.Win; strides[3] = px * d.Win * d.Hin * d.N;
-      box[0] = p.BK; box[1] = p.halo_pitch; box[2] = TN; box[3] = TH + 2; box[4] = 1;
-    } else if (!p.s2) {
+    if (!p.s2) {
       dims[0] = d.Cin; dims[1] = d.Win; dims[2] = d.Hin; dims[3] = d.N; dims[4] = 1;
       strides[0] = px; strides[1] = px * d.Win; strides[2] = px * d.Win * d.Hin; strides[3] = px * d.Win * d.Hin * d.N;
       box[0] = p.BK; box[1] = TW; box[2] = TH; box[3] = TN; box[4] = 1;
@@ -854,19 +423,17 @@ int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
     CC_REQUIRE(r == CUDA_SUCCESS, "conv_gemm: cuTensorMapEncodeTiled(A) failed: %d (dims %llu,%llu,%llu,%llu,%llu)", int(r),
                dims[0], dims[1], dims[2], dims[3], dims[4]);
   }
-  auto encode_B = [&](int rows) -> int {     // weights [Cout][Ktot] bf16, box = BK x rows
+  {     // weights [Cout][Ktot] bf16, box = BK x BN
     const cuuint64_t Ktot = cuuint64_t(d.k) * d.k * d.Cin;
     cuuint64_t dims[2] = {Ktot, cuuint64_t(d.Cout)};
     cuuint64_t strides[1] = {Ktot * 2};
-    cuuint32_t box[2] = {cuuint32_t(p.BK), cuuint32_t(rows)};
+    cuuint32_t box[2] = {cuuint32_t(p.BK), cuuint32_t(BN)};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(&p.tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(d.w), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     CC_REQUIRE(r == CUDA_SUCCESS, "conv_gemm: cuTensorMapEncodeTiled(B) failed: %d", int(r));
-    return CC_OK;
-  };
-  { int rcb = encode_B(BN); if (rcb) return rcb; }
+  }
 
   // ---- epilogue
   p.out = d.out; p.out_cs = d.out_cs; p.out_co = d.out_co; p.out_f32 = d.out_f32;
@@ -875,82 +442,6 @@ int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
   p.out_ns = d.out_ns > 0 ? d.out_ns : Hout * Wout;
   p.pre = d.pre; p.pre_h = d.pre_h; p.pre_w = d.pre_w;
   if (d.pre) CC_REQUIRE(d.pre_h * 2 == Hout && d.pre_w * 2 == Wout && d.Cout % 4 == 0, "conv_gemm: the pre-activation addend must be a half-resolution map of the output");
-
-  // ---- epilogue groups / staging / smem budget -> pipeline depth
-  // Preferred: 4 groups of 4 warps with 16-KB staging each (BN <= 128: four 128-column TMEM slots), 2 groups of 8 warps
-  // with 32-KB staging each for BN = 256.  When that staging would squeeze the load pipeline (fewer than 3 halo buffers /
-  // 4 stages) the next level halves it: 2 groups of 4 warps (BN <= 128) / 64-column passes (BN = 256).
-  static const int nacc_env = getenv("CC_NACC") ? atoi(getenv("CC_NACC")) : 4;
-  int level = (BN <= 128 && nacc_env == 2) ? 1 : 0;
-  // two staging buffers per epilogue group where the operand pipeline keeps its depth (>= 3 halo buffers / >= 4 stages): a pass
-  // then never waits for the previous pass's TMA store
-  static const int nbuf_env = getenv("CC_STG_NBUF") ? atoi(getenv("CC_STG_NBUF")) : 2;
-  int nbuf = nbuf_env == 1 ? 1 : 2;
-  static const int colsplit_env = getenv("CC_COLSPLIT") ? atoi(getenv("CC_COLSPLIT")) : 1;
-  int cs = colsplit_env;      // column split wanted (dropped again below when its staging squeezes the operand pipeline)
-budget_again:
-  p.stg_nbuf = nbuf;
-  // column split for wide tiles: four 4-warp groups each convert a quarter of every tile's columns (see the kernel)
-  p.colsplit = (cs && BN > 128 && (BN / 4) % (d.out_f32 ? 32 : 64) == 0) ? 1 : 0;
-  // ... and for 128-column tiles of layers with only a few tiles per CTA (the 20x20 / 40x40 maps; every layer of a
-  // single-frame call): with one group per tile the other three idle while one converts 128 columns alone (~2.9 us per tile
-  // in the timeline, the longest link of those layers' chains); split, each converts 32 columns (64-B staging rows)
-  static const int cs128_env = getenv("CC_COLSPLIT128") ? atoi(getenv("CC_COLSPLIT128")) : 3;   // max tiles per CTA; 0 = off
-  const int tiles_per_cta = (p.num_tiles + num_sms - 1) / num_sms;
-  const bool cs_narrow = cs && cs128_env > 0 && BN == 128 && level == 0 && tiles_per_cta <= cs128_env;
-  if (cs_narrow) p.colsplit = 1;
-  if (cs_narrow) { p.n_acc = 4; p.n_grp = 4; p.lgw = 2; }
-  else if (p.colsplit) { p.n_acc = 2; p.n_grp = 4; p.lgw = 2; }
-  else if (BN > 128) { p.n_acc = 2; p.n_grp = 2; p.lgw = 3; }
-  else { p.n_acc = level == 0 ? 4 : 2; p.n_grp = p.n_acc; p.lgw = 2; }
-  int CH = (p.lgw == 2 || level >= 1) ? (d.out_f32 ? 32 : 64) : (d.out_f32 ? 64 : 128);
-  if (CH > BN) CH = BN;
-  if (p.colsplit && CH > BN / 4) CH = BN / 4;
-  p.CH = CH;
-  static const int tmas_env = getenv("CC_TMASTORE") ? atoi(getenv("CC_TMASTORE")) : 1;
-  static const int tmas64_env = getenv("CC_TMASTORE64") ? atoi(getenv("CC_TMASTORE64")) : 1;
-  p.stg_lrow = 7;
-  const int wcols = p.colsplit ? BN / 4 : BN;      // columns one epilogue group stores per tile
-  p.tma_store = (tmas_env && (wcols * es) % 128 == 0) ? 1 : 0;
-  if (!p.tma_store && tmas_env && tmas64_env && (wcols * es) % 64 == 0) {   // narrow tiles (BN = 32 bf16, 16 fp32, ...): 64-B rows
-    p.tma_store = 1;
-    p.stg_lrow = 6;
-  }
-  if (p.tma_store) {
-    void* base = reinterpret_cast<uint8_t*>(d.out) + size_t(d.out_co) * es;
-    cuuint64_t dims[5], strides[4];
-    cuuint32_t box[5], estr[5] = {1, 1, 1, 1, 1};
-    const cuuint64_t px = cuuint64_t(d.out_cs) * es;
-    const cuuint64_t img = px * cuuint64_t(p.out_ns);
-    if (p.halo) {
-      dims[0] = d.Cout; dims[1] = Wout; dims[2] = d.N; dims[3] = Hout; dims[4] = 1;
-      strides[0] = px; strides[1] = img; strides[2] = px * Wout; strides[3] = img * d.N;
-      box[0] = (1 << p.stg_lrow) / es; box[1] = 8; box[2] = TN; box[3] = TH; box[4] = 1;
-    } else {
-      dims[0] = d.Cout; dims[1] = Wout; dims[2] = Hout; dims[3] = d.N; dims[4] = 1;
-      strides[0] = px; strides[1] = px * Wout; strides[2] = img; strides[3] = img * d.N;
-      box[0] = (1 << p.stg_lrow) / es; box[1] = TW; box[2] = TH; box[3] = TN; box[4] = 1;
-    }
-    CUresult r = enc(&p.tmC, d.out_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, base, dims,
-                     strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     p.stg_lrow == 7 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                     CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CC_REQUIRE(r == CUDA_SUCCESS, "conv_gemm: cuTensorMapEncodeTiled(C) failed: %d", int(r));
-  }
-  static const int restma_env = getenv("CC_RES_TMA") ? atoi(getenv("CC_RES_TMA")) : 1;
-  p.res_tma = (restma_env && p.tma_store && d.res != nullptr && d.res == d.out && d.res_cs == d.out_cs && d.res_co == d.out_co) ? 1 : 0;
-  if (p.res_tma && d.out_f32 && restma_env >= 1 && restma_env != 3) p.res_tma = 2;   // fp32: reduce-add store (CC_RES_TMA=3 forces the prefetch variant)
-  const int pitch = p.tma_store ? CH * es : CH * es + 16;
-  const int staging = ((kTileM * pitch + 15) & ~15) * p.n_grp * nbuf;
-  const int stage_bytes = kTileM * p.BK * 2 + BN * p.BK * 2;
-  const int fixed = 1024 /*alignment slack of the smem base*/ + staging + d.Cout * 4 /*bias*/ + 336 /*barriers + TMEM slot*/;
-  // the staging area starts at the next 1024-B boundary after the operand rings (a no-op unless a weight tile is an odd
-  // multiple of 512 B)
-  auto stage_pad = [](int operand_bytes) { return (1024 - operand_bytes % 1024) % 1024; };
-  int S;
-  static const int bres_env = getenv("CC_BRES") ? atoi(getenv("CC_BRES")) : 1;
-  static const int dbg_env = getenv("CC_DBG") ? atoi(getenv("CC_DBG")) : 0;
-  p.dbg = dbg_env;
   {
     auto fast_div = [](uint32_t d, uint32_t fd[2]) {      // q = (umulhi(mul, x) + x) >> shift for x < 2^31
       uint32_t l = 0;
@@ -960,109 +451,35 @@ budget_again:
     };
     fast_div(p.n_blocks, p.fd_nb);
     fast_div(p.tiles_w, p.fd_tw);
-    fast_div(p.tiles_h, p.fd_th);
     fast_div(p.tiles_w * p.tiles_h, p.fd_twh);
   }
-  static const int hst_env = getenv("CC_HALO_STAGES") ? atoi(getenv("CC_HALO_STAGES")) : 0;
-  const int bres_bytes = BN * p.BK * 2 * p.num_taps * p.chunks_per_tap;
-  // resident weights up to 128 KB (a 1x1 conv 256 -> 256): with the halved staging of level 1 four activation stages still fit
-  static const int bres_kb_env = getenv("CC_BRES_KB") ? atoi(getenv("CC_BRES_KB")) : 128;
-  static const int bres_min_stages = getenv("CC_BRES_MIN_STAGES") ? atoi(getenv("CC_BRES_MIN_STAGES")) : 4;
-  p.b_res = (bres_env && p.n_blocks == 1 && bres_bytes <= bres_kb_env * 1024) ? 1 : 0;
-  p.halo_stages = 2;
-  if (p.halo) {
-    const int b_bytes = BN * p.BK * 2;
-    // budget: staging (already in `fixed`), then weights (resident, or a ring of >= 3 taps), then as many halo
-    // buffers as fit (2..4): a halo chunk is only 9 taps of MMA work, so 2 buffers cannot hide the TMA latency
-    int avail = kMaxSmem - fixed;
-    if (p.b_res && avail - bres_bytes < 2 * p.halo_bytes) {
-      if (nbuf == 2) { nbuf = 1; goto budget_again; }   // resident weights beat the second staging buffer
-      p.b_res = 0;
-    }
-    int wbytes;
-    bool deep = false;      // weight ring deep enough to cover the L2 latency
-    if (p.b_res) { wbytes = bres_bytes; S = 2; }
-    else {
-      // Streamed weights: the weight ring must cover the L2 latency — one k-block consumes a b_bytes stage per 2*BN tensor
-      // cycles (64 B/clk whatever BN is), and at ~1200 cycles of latency that is ~80 KB in flight.  With three 16-KB stages
-      // (BN = 128) the 3x3 128->128 convs ran at 57 % of their tensor time, and halving the bytes per CTA (pair multicast) did
-      // not move them: the depth was the limit.  A halo buffer, in contrast, holds nine k-blocks of work, so two of them are
-      // enough to prefetch one chunk ahead: weight stages are bought before the third halo buffer.
-      // (Measured again once the 10-pixel halo pitch had freed shared memory: 112 KB wanted is +0.7 % on the step over 80 KB —
-      // under load the latency is longer than the idle figure.)
-      static const int bdepth_env = getenv("CC_B_INFLIGHT_KB") ? atoi(getenv("CC_B_INFLIGHT_KB")) : 112;
-      const int want = (bdepth_env * 1024 + b_bytes - 1) / b_bytes;
-      S = 3;
-      while (S < 8 && S < want && avail - (S + 1) * b_bytes >= 2 * p.halo_bytes) ++S;
-      while (S < 6 && avail - (S + 1) * b_bytes >= 3 * p.halo_bytes) ++S;   // more of both where there is room
-      wbytes = S * b_bytes;
-      deep = S >= want;
-    }
-    int hs = (avail - wbytes) / p.halo_bytes;
-    if (hs > 4) hs = 4;
-    if (hst_env >= 2 && hst_env <= 4 && hst_env < hs) hs = hst_env;
-    const bool depth_ok = hs >= 3 || (hs >= 2 && deep);
-    if (!depth_ok && nbuf == 2) { nbuf = 1; goto budget_again; }
-    if (!depth_ok && p.colsplit) { cs = 0; nbuf = nbuf_env == 1 ? 1 : 2; goto budget_again; }   // K-heavy 3x3 tiles: the mainloop matters more
-    if (!depth_ok && level == 0) {   // the staging squeezes the operand rings: halve it (an MMA-bound layer does not need more)
-      level = 1;
-      goto budget_again;
-    }
-    if (hs < 2) {   // does not fit: caller falls back
-      set_error("conv_gemm: halo tile does not fit (BN=%d halo=%d B)", BN, p.halo_bytes);
-      return CC_ERR_INVALID;
-    }
-    p.halo_stages = hs;
-    L->smem_bytes = fixed + wbytes + hs * p.halo_bytes + stage_pad(wbytes + hs * p.halo_bytes);
-  } else if (p.b_res && (kMaxSmem - fixed - bres_bytes) / (kTileM * p.BK * 2) >= bres_min_stages) {
-    const int a_bytes = kTileM * p.BK * 2;
-    S = (kMaxSmem - fixed - bres_bytes) / a_bytes;
-    if (S > 8) S = 8;
-    if (fixed + bres_bytes + S * a_bytes + stage_pad(bres_bytes + S * a_bytes) > kMaxSmem) --S;
-    L->smem_bytes = fixed + bres_bytes + S * a_bytes + stage_pad(bres_bytes + S * a_bytes);
-  } else if (p.b_res && nbuf == 2) {   // keep the weights resident rather than the second staging buffer
-    nbuf = 1;
-    goto budget_again;
-  } else {
-    p.b_res = 0;
-    S = (kMaxSmem - fixed) / stage_bytes;
-    if (S > 8) S = 8;
-    if (S < 4 && nbuf == 2) { nbuf = 1; goto budget_again; }
-    if (S < 3 && p.colsplit) { cs = 0; nbuf = nbuf_env == 1 ? 1 : 2; goto budget_again; }
-    if (S < 4 && level == 0 && !p.colsplit) {
-      level = 1;
-      goto budget_again;
-    }
-    if (fixed + S * stage_bytes + stage_pad(S * stage_bytes) > kMaxSmem) --S;
-    CC_REQUIRE(S >= 2, "conv_gemm: tile does not fit shared memory (BN=%d BK=%d)", BN, p.BK);
-    L->smem_bytes = fixed + S * stage_bytes + stage_pad(S * stage_bytes);
-  }
+
+  // ---- smem budget -> pipeline depth.  Fixed part: alignment slack, the fp32 staging tile, bias, barriers.
+  const int a_bytes = kTileM * p.BK * 2, b_bytes = BN * p.BK * 2;
+  const int fixed = 1024 + kTileM * (BN * 4 + 16) + 16 + d.Cout * 4 + 8 * 20;
+  const int num_kb = p.num_taps * p.chunks_per_tap;
+  const int bres_bytes = b_bytes * num_kb;
+  // resident weights (single N block) when they leave room for at least four activation stages: the ring then carries
+  // A only and the weights cross the L2 once per CTA instead of once per tile
+  p.b_res = (p.n_blocks == 1 && (kMaxSmem - fixed - bres_bytes) / a_bytes >= 4) ? 1 : 0;
+  int S = p.b_res ? (kMaxSmem - fixed - bres_bytes) / a_bytes : (kMaxSmem - fixed) / (a_bytes + b_bytes);
+  if (S > 8) S = 8;
+  CC_REQUIRE(S >= 2, "conv_gemm: tile does not fit shared memory (BN=%d BK=%d)", BN, p.BK);
+  CC_REQUIRE(S <= 8, "conv_gemm: too many stages");
   p.stages = S;
+  L->smem_bytes = fixed + (p.b_res ? bres_bytes + S * a_bytes : S * (a_bytes + b_bytes));
   L->grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-  // CTA pairs: wide, streamed (non-resident) weight tiles are what the L2 -> SM fabric spends most of its bandwidth on
-  // (A 16 KB + B 32 KB per 128x256x64 block = 85 FLOP/B); two CTAs on adjacent M tiles of the same N block each load half of
-  // the weight tile and multicast it to both (16 + 16 KB = 128 FLOP/B)
-  static const int pair_env = getenv("CC_PAIR") ? atoi(getenv("CC_PAIR")) : 1;
-  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  p.pair = (pair_env && !p.b_res && BN >= 128 && (BN / 2) % 8 == 0 && m_tiles >= 2 && num_sms >= 2) ? 1 : 0;
-  p.n_super = ((m_tiles + 1) / 2) * p.n_blocks;
-  if (p.pair) {
-    int rcb = encode_B(BN / 2);
-    if (rcb) return rcb;
-    const int cap = num_sms & ~1;
-    L->grid = 2 * p.n_super < cap ? 2 * p.n_super : cap;
-  }
   L->flops = 2.0 * double(d.N) * Hout * Wout * d.Cout * d.k * d.k * d.Cin;
   L->bytes = double(d.N) * d.Hin * d.Win * d.Cin * 2 + double(d.N) * Hout * Wout * d.Cout * es * (d.res ? 2 : 1) +
              double(d.Cout) * d.k * d.k * d.Cin * 2;
   return CC_OK;
 }
 
-template <int ACT, bool F32>
-static int launch_variant(const GemmLaunch& L, cudaStream_t stream) {
+template <int ACT, bool F32, int BN>
+static int launch_bn(const GemmLaunch& L, cudaStream_t stream) {
   static bool attr_set = false;
   if (!attr_set) {
-    CC_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<ACT, F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+    CC_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<ACT, F32, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
     attr_set = true;
   }
   cudaLaunchConfig_t cfg{};
@@ -1070,20 +487,25 @@ static int launch_variant(const GemmLaunch& L, cudaStream_t stream) {
   cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = L.smem_bytes;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  if (L.p.pair) {
-    attr[1].id = cudaLaunchAttributeClusterDimension;
-    attr[1].val.clusterDim.x = 2;
-    attr[1].val.clusterDim.y = 1;
-    attr[1].val.clusterDim.z = 1;
-    cfg.numAttrs = 2;
-  }
-  CC_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<ACT, F32>, L.p));
+  CC_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<ACT, F32, BN>, L.p));
   return CC_OK;
+}
+
+template <int ACT, bool F32>
+static int launch_variant(const GemmLaunch& L, cudaStream_t stream) {
+  switch (L.p.BN) {
+    case 16: return launch_bn<ACT, F32, 16>(L, stream);
+    case 32: return launch_bn<ACT, F32, 32>(L, stream);
+    case 64: return launch_bn<ACT, F32, 64>(L, stream);
+    case 128: return launch_bn<ACT, F32, 128>(L, stream);
+  }
+  set_error("conv_gemm: no kernel for BN=%d", L.p.BN);
+  return CC_ERR_INVALID;
 }
 
 int conv_gemm_launch(const GemmLaunch& L, cudaStream_t stream) {

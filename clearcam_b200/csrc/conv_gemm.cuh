@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution / linear layer on tcgen05 tensor cores (sm_100a), host-side descriptors.
+// Implicit-GEMM convolution / linear layer on Hopper warpgroup MMA (wgmma, sm_90a), host-side descriptors.
 //
 // One kernel serves every GEMM-shaped op on the hot path:
 //   * YOLOv9 `Conv` = nn.Conv2d(bias) -> SiLU          (reference detection/yolov9.py:33-38), k in {1,3}, s in {1,2}
@@ -7,7 +7,7 @@
 //   * CLIP linears: QKV / out-proj / MLP (+tanh-GELU)   (models/objects.py:107-127,157-179)
 // Activations are NHWC bf16 (a channel *slice* of a wider buffer is addressed in place, so Tensor.cat /
 // chunk in the reference cost nothing here); weights are [Cout][kh][kw][Cin] bf16 (K-major); accumulation fp32
-// in TMEM; bias + activation + residual in the epilogue.
+// in registers; bias + activation + residual in the epilogue.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -20,7 +20,6 @@ enum Act : int32_t { ACT_NONE = 0, ACT_SILU = 1, ACT_GELU_TANH = 2, ACT_SILU_EXA
 struct GemmParams {
   CUtensorMap tmA;  // 5-D view of the NHWC activation (see conv_gemm.cu)
   CUtensorMap tmB;  // 2-D [Cout][Ktot] weights
-  CUtensorMap tmC;  // 5-D view of the NHWC output slice (TMA-store epilogue)
   int32_t tap[9][4];  // per filter tap: delta on dims 0..3 of the A view
   int32_t num_taps, chunks_per_tap, BK, BN;
   int32_t n_blocks;                   // Cout / BN
@@ -30,41 +29,22 @@ struct GemmParams {
   int32_t W, H, N;                    // OUTPUT spatial dims / batch
   int32_t stages;
   int32_t num_tiles;
-  int32_t ab_fmt;                     // 1 = bf16
   // epilogue
   void* out;
   int32_t out_cs, out_co, out_f32;    // channel stride of the out buffer, channel offset, fp32 output flag
   const float* bias;                  // [Cout] or nullptr
   int32_t act;
-  const void* res;                    // residual (same dtype as out) or nullptr
+  const void* res;                    // residual (same dtype as out) or nullptr; may be the output slice itself (in place)
   int32_t res_cs, res_co;
   int32_t cout;
   int32_t out_ns;                     // pixels per image in the out/residual buffers (default H*W)
-  // halo mainloop (3x3 stride-1, Cin % 64 == 0): one TMA load of the (TH+2) x 16-pixel halo per 64-channel chunk,
-  // the nine taps are shifted shared-memory descriptor views of it
-  int32_t halo, halo_bytes, halo_bo;  // enabled / bytes per halo stage / descriptor base_offset mode
-  int32_t halo_stages;                // 2..4 halo buffers in flight
-  int32_t halo_pitch, halo_tx;        // pixels per halo row in shared memory (10: exactly the 8 + 2 the taps read; 16: round-1 layout) / bytes one halo load transfers
-  int32_t tma_store;                  // epilogue stores through TMA from swizzled staging (one buffer per epilogue group)
   int32_t b_res;                      // weights of the (single) N block stay resident in smem for the whole kernel
-  int32_t res_tma;                    // in-place residual is prefetched into the staging buffer by TMA (through tmC)
-  // tile index -> (n block, w, h, n) without integer division: q = (umulhi(mul, x) + x) >> shift (per-tile index
-  // math was ~140 of the ~260 instructions every epilogue warp spends per tile; ncu, profiles/round1/)
-  uint32_t fd_nb[2], fd_tw[2], fd_th[2], fd_twh[2];
-  int32_t stg_lrow;                   // log2 of the staging / TMA-store row: 7 (SWIZZLE_128B) or 6 (SWIZZLE_64B, narrow tiles)
-  int32_t dbg;                        // CC_DBG bisection switches (never set in production): 1 no epilogue work, 4 no A loads
-  int32_t n_acc;                      // TMEM accumulator slots == independent epilogue groups: 4 (BN <= 128) or 2
-  int32_t lgw;                        // log2(warps per epilogue group): 2 or 3
-  // CTA pairs (2-CTA clusters): both CTAs of a pair work on the same N block of two adjacent M tiles, each TMA-loads half of
-  // every weight tile and multicasts it to both (halves the weight traffic L2 -> SM of the wide GEMMs, which are bound by it)
-  int32_t pair, n_super;              // enabled / number of (M-tile pair, N block) super tiles
-  int32_t CH;                         // output columns per staging pass of one epilogue group
-  int32_t stg_nbuf;                   // staging buffers per epilogue group (1 or 2)
+  // tile index -> (n block, w, h, n) without integer division: q = (umulhi(mul, x) + x) >> shift
+  uint32_t fd_nb[2], fd_tw[2], fd_twh[2];
   const float* pre;                   // optional fp32 [N][H/2][W/2][Cout]: added BEFORE the activation at (n, h/2, w/2) — a 1x1 conv over
   int32_t pre_h, pre_w;               //   concat(upsample(a), b) is computed as conv_b(b) + upsample(conv_a(a)) (see yolo.cu)
-  int32_t n_grp, colsplit;            // epilogue groups; 1: every group converts its share of the columns of EVERY tile
   unsigned long long* trace;          // optional device timeline slots [8] (globaltimer ns): first CTA entry, dependency released, last CTA exit,
-                                      // and of CTA 0: first operands landed, all MMAs issued, first accumulator complete, last epilogue done, exit
+                                      // and of CTA 0: first operands landed, -, first accumulator complete, last epilogue done, exit
 };
 
 struct ConvDesc {

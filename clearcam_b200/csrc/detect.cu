@@ -87,7 +87,7 @@ int decode_launch(const DecodeParams& p, cudaStream_t s) {
   const long long total = static_cast<long long>(p.B) * p.A;
   if (total == 0) return CC_OK;
   long long blocks = (total + 127) / 128;
-  if (blocks > 148LL * 16) blocks = 148LL * 16;
+  if (blocks > 132LL * 16) blocks = 132LL * 16;
   decode_kernel<<<static_cast<int>(blocks), 128, 0, s>>>(p);
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;
@@ -126,7 +126,7 @@ int pred_from_raw_launch(const float* raw, int B, int A, int nc, float conf_thr,
   const long long total = static_cast<long long>(B) * A;
   if (total == 0) return CC_OK;
   long long blocks = (total + 127) / 128;
-  if (blocks > 148LL * 16) blocks = 148LL * 16;
+  if (blocks > 132LL * 16) blocks = 132LL * 16;
   pred_from_raw_kernel<<<static_cast<int>(blocks), 128, 0, s>>>(raw, B, A, nc, conf_thr, pred);
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;

@@ -93,7 +93,6 @@ struct StemTcParams {
   int B, H, W, Cout;
   long long Mrows;
   int tiles;
-  int tmem_cols;
 };
 int stem_tc_build(int B, int H, int W, const __nv_bfloat16* w32, const float* bias, int Cout, const TSlice& out, StemTcParams* p);
 int stem_tc_launch(const StemTcParams& p, const uint8_t* frames, cudaStream_t s);
@@ -131,7 +130,7 @@ int text_embed_launch(const int* ids, const float* tok, const float* pos, float*
                       int vocab, cudaStream_t st);
 int l2norm_launch(const float* in, float* out, int rows, int D, long long out_stride, float eps, cudaStream_t st);
 int attention_launch(const __nv_bfloat16* qkv, __nv_bfloat16* ctx, int B, int L, int H, int causal, cudaStream_t st);
-// tcgen05 attention (attention_tc.cu); vt_ws: workspace of attention_tc_workspace_bytes() for the per-head V^T copy
+// wgmma attention (attention_tc.cu); vt_ws: workspace of attention_tc_workspace_bytes() for the per-head V^T copy
 bool attention_tc_supported(int L);
 size_t attention_tc_workspace_bytes(int B, int L, int H);
 int attention_tc_launch(const __nv_bfloat16* qkv, __nv_bfloat16* ctx, __nv_bfloat16* vt_ws, int B, int L, int H, int causal,

@@ -71,7 +71,7 @@ __device__ __forceinline__ E* at_w(const TSlice& t, int n, int h, int w, int c) 
 
 static int grid_for(long long total, int threads) {
   long long b = (total + threads - 1) / threads;
-  const long long cap = 148LL * 32;
+  const long long cap = 132LL * 32;
   return static_cast<int>(b < 1 ? 1 : (b > cap ? cap : b));
 }
 
@@ -624,7 +624,7 @@ int stem_launch(const StemParams& p, cudaStream_t s) {
   const long long total = static_cast<long long>(p.B) * (p.H / 2) * (p.W / 2);
   const int smem = (27 + 1) * p.Cout * sizeof(float);
   long long blocks = (total + 127) / 128;
-  if (blocks > 148LL * 16) blocks = 148LL * 16;
+  if (blocks > 132LL * 16) blocks = 132LL * 16;
   if (p.out.f32) {
     if (p.is_f32) stem_kernel<true, float><<<static_cast<int>(blocks), 128, smem, s>>>(p);
     else stem_kernel<false, float><<<static_cast<int>(blocks), 128, smem, s>>>(p);

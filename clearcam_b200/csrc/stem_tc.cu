@@ -1,17 +1,19 @@
-// Stem conv on tcgen05 straight from the uint8 frame (no im2col round trip through HBM).
+// Stem conv on Hopper warpgroup MMA straight from the uint8 frame (no im2col round trip through HBM).
 //
 // What it replaces in the reference: `frame[..., ::-1] / 255` (detection/yolov9.py:378-379) folded into model[0] =
 // Conv(3, c, 3, 2) = conv 3x3 / s2 / p1 + bias + SiLU (:33-38, :303; also model[1] and model[15] of size e).
 //
 // Raw pixel values 0..255 are exact in bf16, the weights are bf16(w / 255) with the 27 taps in (r, s, RGB) order (RGB
 // channel c = frame channel 2 - c), K padded to 32.  GEMM view: M = output pixels (flattened n, oy, ox), N = Cout, K = 32.
-// One CTA = 128 threads = one 128-pixel tile at a time:
+// One CTA = 128 threads = one warpgroup = one 128-pixel tile at a time:
 //   thread == output pixel: 27 byte gathers (L1-resident: neighbouring pixels share two thirds of their window)
 //     -> its 64-B row of the A tile, written in the SWIZZLE_64B K-major layout the MMA reads
-//   one elected thread: two tcgen05.mma (M128 x N=Cout x K16), accumulator in TMEM
-//   thread == accumulator row: tcgen05.ld -> +bias -> SiLU -> bf16 -> swizzled staging -> ONE TMA store of the tile
-// The chain inside a CTA is serial; 6 CTAs are co-resident per SM (28 KB shared memory, 64 TMEM columns each) and hide each
-// other's latencies.  Bound: HBM (frame bytes in, 2*Cout bytes per output pixel out).
+//   the warpgroup: four wgmma (two 64-row halves x two K = 16 steps, N = Cout), accumulators in registers
+//   from the accumulator fragments: +bias -> SiLU -> bf16 -> swizzled staging -> ONE TMA store of the tile
+// The chain inside a CTA is serial; 5 CTAs are co-resident per SM (28 KB shared memory each) and hide each other's
+// latencies; 5 x 128 threads leave each thread up to 102 registers, and the Cout = 64 variant needs 94 to keep its
+// accumulators without serialising the wgmma.
+// Bound: HBM (frame bytes in, 2*Cout bytes per output pixel out).
 #include "ops.cuh"
 #include "cc_common.h"
 #include "cc_ptx.cuh"
@@ -30,48 +32,30 @@ __device__ __forceinline__ uint32_t stem_pack(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-__global__ void __launch_bounds__(128, 6) stem_tc_kernel(const __grid_constant__ StemTcParams p) {
+template <int COUT>
+__global__ void __launch_bounds__(128, 5) stem_tc_kernel(const __grid_constant__ StemTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;                 // 128 rows x 64 B
   uint8_t* sW = sA + 8192;            // Cout rows x 64 B (<= 4 KB)
   uint8_t* sC = sW + 4096;            // 128 rows x 2*Cout B staging (<= 16 KB)
   float* sBias = reinterpret_cast<float*>(sC + 16384);
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sBias + 64);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 1);
 
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int Cout = p.Cout;
-  if (tid == 0) {
-    tma_prefetch_desc(&p.tmC);
-    mbar_init(bar, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) {
-    __syncwarp();
-    tmem_alloc(tmem_slot, p.tmem_cols);
-    tmem_relinquish();
-  }
-  for (int i = tid; i < Cout * 4; i += 128) {      // weights -> SWIZZLE_64B K-major rows
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  if (tid == 0) tma_prefetch_desc(&p.tmC);
+  for (int i = tid; i < COUT * 4; i += 128) {      // weights -> SWIZZLE_64B K-major rows
     const int r = i >> 2, j = i & 3;
     *reinterpret_cast<uint4*>(sW + r * 64 + ((j ^ ((r >> 1) & 3)) << 4)) = __ldg(reinterpret_cast<const uint4*>(p.w + r * 32) + j);
   }
-  if (tid < Cout) sBias[tid] = __ldg(p.bias + tid);
-  fence_proxy_async_smem();
-  tc_fence_before();
+  if (tid < COUT) sBias[tid] = __ldg(p.bias + tid);
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int Ho = p.H >> 1, Wo = p.W >> 1;
-  const uint32_t idesc = umma_idesc_f16(128, Cout, 1);
-  const uint64_t dconst = (1ull << 16) | (static_cast<uint64_t>(512 >> 4) << 32) | (1ull << 46) | (4ull << 61);   // SWIZZLE_64B, SBO = 8 rows x 64 B
+  const uint64_t dconst = gmma_desc_const(64, 512);   // SWIZZLE_64B, SBO = 8 rows x 64 B
   const uint64_t adesc = dconst | ((smem_u32(sA) & 0x3FFFF) >> 4), bdesc = dconst | ((smem_u32(sW) & 0x3FFFF) >> 4);
-  const uint32_t t_row = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
-  const uint32_t rb = Cout * 2, swz_mask = (rb >> 4) - 1;   // staging row bytes (32 / 64 / 128) and its TMA swizzle span
+  constexpr uint32_t rb = COUT * 2, swz_mask = (rb >> 4) - 1;   // staging row bytes (32 / 64 / 128) and its TMA swizzle span
 
-  uint32_t it = 0;
-  for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x, ++it) {
+  for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
     // ---- gather: this thread's output pixel
     const long long idx = static_cast<long long>(tile) * 128 + tid;
     float v[32];
@@ -93,8 +77,8 @@ __global__ void __launch_bounds__(128, 6) stem_tc_kernel(const __grid_constant__
           if (ix < 0 || ix >= p.W) continue;
           const uint8_t* px = rowp + ix * 3;
 #pragma unroll
-          // byte -> float without the conversion unit (I2F shares the 16-lane/clk XU pipe with the 64 MUFU.TANH of this thread's
-          // row; ncu had the kernel at 53 % XU): 0x4B000000 | b is the float 2^23 + b exactly, one subtraction leaves b
+          // byte -> float without the conversion unit (I2F shares its pipe with the MUFU.TANH of the epilogue):
+          // 0x4B000000 | b is the float 2^23 + b exactly, one subtraction leaves b
           for (int c = 0; c < 3; ++c) v[(r * 3 + s) * 3 + c] = __uint_as_float(0x4B000000u | __ldg(px + 2 - c)) - 8388608.0f;
         }
       }
@@ -105,36 +89,36 @@ __global__ void __launch_bounds__(128, 6) stem_tc_kernel(const __grid_constant__
       *reinterpret_cast<uint4*>(sA + tid * 64 + ((j ^ ((tid >> 1) & 3)) << 4)) =
           make_uint4(stem_pack(v[8 * j], v[8 * j + 1]), stem_pack(v[8 * j + 2], v[8 * j + 3]), stem_pack(v[8 * j + 4], v[8 * j + 5]),
                      stem_pack(v[8 * j + 6], v[8 * j + 7]));
-    fence_proxy_async_smem();
+    fence_proxy_async_smem();                   // generic-proxy A tile -> visible to wgmma
     __syncthreads();
-    if (warp == 0) {
-      tc_fence_after();
-      if (elect_one()) {
-        umma_f16_c<false>(tmem_base, adesc, bdesc, idesc);
-        umma_f16_c<true>(tmem_base, adesc + 2, bdesc + 2, idesc);
-        umma_commit(bar);
-      }
-      __syncwarp();
-    }
-    mbar_wait(bar, it & 1);
-    tc_fence_after();
-    // ---- epilogue: thread == accumulator row
-    for (int c = 0; c < Cout; c += 16) {
-      uint32_t a[16];
-      tmem_ld16(t_row + c, a);
-      tmem_ld_wait();
-      float f[16];
+    // ---- the warpgroup: rows 0..63 and 64..127 of the tile, K = 32 in two steps
+    float acc0[COUT / 2], acc1[COUT / 2];
+    wgmma_fence();
+    Wgmma<COUT>::mma(acc0, adesc, bdesc, 0u);
+    Wgmma<COUT>::mma(acc0, adesc + 2, bdesc + 2, 1u);
+    Wgmma<COUT>::mma(acc1, adesc + (4096 >> 4), bdesc, 0u);
+    Wgmma<COUT>::mma(acc1, adesc + (4096 >> 4) + 2, bdesc + 2, 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc0);
+    wgmma_fence_acc(acc1);
+    // ---- epilogue from the fragments: +bias -> SiLU -> bf16 pairs -> swizzled staging
 #pragma unroll
-      for (int j = 0; j < 16; ++j) f[j] = stem_silu(__uint_as_float(a[j]) + sBias[c + j]);
+    for (int h = 0; h < 2; ++h) {
+      const float* acc = h ? acc1 : acc0;
 #pragma unroll
-      for (int q = 0; q < 2; ++q) {
-        const uint32_t off = tid * rb + c * 2 + 16 * q;
-        *reinterpret_cast<uint4*>(sC + (off ^ (((off >> 7) & swz_mask) << 4))) =
-            make_uint4(stem_pack(f[8 * q], f[8 * q + 1]), stem_pack(f[8 * q + 2], f[8 * q + 3]), stem_pack(f[8 * q + 4], f[8 * q + 5]),
-                       stem_pack(f[8 * q + 6], f[8 * q + 7]));
+      for (int i = 0; i < COUT / 8; ++i) {
+        const int col = 8 * i + 2 * (lane & 3);
+        const float b0 = sBias[col], b1 = sBias[col + 1];
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          const int r = 64 * h + 16 * warp + (lane >> 2) + 8 * q;
+          const uint32_t off = r * rb + col * 2;
+          *reinterpret_cast<uint32_t*>(sC + (off ^ (((off >> 7) & swz_mask) << 4))) =
+              stem_pack(stem_silu(acc[4 * i + 2 * q] + b0), stem_silu(acc[4 * i + 2 * q + 1] + b1));
+        }
       }
     }
-    tc_fence_before();
     fence_proxy_async_smem();
     __syncthreads();
     if (tid == 0) {
@@ -143,12 +127,6 @@ __global__ void __launch_bounds__(128, 6) stem_tc_kernel(const __grid_constant__
     }
   }
   if (tid == 0) tma_store_wait_all();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
-  }
 }
 
 int stem_tc_build(int B, int H, int W, const __nv_bfloat16* w32, const float* bias, int Cout, const TSlice& out, StemTcParams* q) {
@@ -163,7 +141,6 @@ int stem_tc_build(int B, int H, int W, const __nv_bfloat16* w32, const float* bi
   p.Mrows = static_cast<long long>(B) * (H / 2) * (W / 2);
   CC_REQUIRE(p.Mrows < (1ll << 31) - 128, "stem_tc: too many output pixels");
   p.tiles = static_cast<int>((p.Mrows + 127) / 128);
-  p.tmem_cols = Cout < 32 ? 32 : Cout;
   cuuint64_t dims[2] = {cuuint64_t(Cout), cuuint64_t(p.Mrows)};
   cuuint64_t strides[1] = {cuuint64_t(out.cs) * 2};
   cuuint32_t box[2] = {cuuint32_t(Cout), 128}, estr[2] = {1, 1};
@@ -174,19 +151,30 @@ int stem_tc_build(int B, int H, int W, const __nv_bfloat16* w32, const float* bi
   return CC_OK;
 }
 
+template <int COUT>
+static cudaError_t stem_launch_cout(const StemTcParams& p, int grid, int smem, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    const cudaError_t e = cudaFuncSetAttribute(stem_tc_kernel<COUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return e;
+    attr_set = true;
+  }
+  stem_tc_kernel<COUT><<<grid, 128, smem, st>>>(p);
+  return cudaSuccess;
+}
+
 int stem_tc_launch(const StemTcParams& q, const uint8_t* frames, cudaStream_t st) {
   StemTcParams p = q;
   p.in = frames;
-  const int smem = 1024 + 8192 + 4096 + 16384 + 256 + 64;
-  static bool attr_set = false;
-  if (!attr_set) {
-    CC_CHECK_CUDA(cudaFuncSetAttribute(stem_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_set = true;
-  }
+  const int smem = 1024 + 8192 + 4096 + 16384 + 256;
   const int sms = device_sm_count();
-  int grid = 6 * (sms > 0 ? sms : 148);
+  int grid = 5 * (sms > 0 ? sms : 132);
   if (grid > p.tiles) grid = p.tiles;
-  stem_tc_kernel<<<grid, 128, smem, st>>>(p);
+  switch (p.Cout) {
+    case 16: CC_CHECK_CUDA(stem_launch_cout<16>(p, grid, smem, st)); break;
+    case 32: CC_CHECK_CUDA(stem_launch_cout<32>(p, grid, smem, st)); break;
+    default: CC_CHECK_CUDA(stem_launch_cout<64>(p, grid, smem, st)); break;
+  }
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;
 }

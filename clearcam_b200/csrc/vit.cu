@@ -1,4 +1,4 @@
-// CLIP ViT encoder kernels other than the GEMMs (those run on conv_gemm.cu's tcgen05 kernel as 1x1 "convs").
+// CLIP ViT encoder kernels other than the GEMMs (those run on conv_gemm.cu's wgmma kernel as 1x1 "convs").
 // Reference: models/objects.py:94-133 (image tower), :145-186 (text tower).
 //   patchify        : NCHW fp32 image -> bf16 patch matrix [B*P, Kpad]  (the 14x14/s14 conv :95 as a GEMM operand)
 //   embed_ln_pre    : class token + positional embedding + ln_pre        (:96-102)  -> fp32 residual stream
@@ -52,7 +52,7 @@ int patchify_launch(const float* x, __nv_bfloat16* out, int B, int S, int p, int
   CC_REQUIRE(S % p == 0 && Kpad % 8 == 0 && Kpad >= 3 * p * p, "patchify: bad shape");
   const long long total = static_cast<long long>(B) * (S / p) * (S / p) * (Kpad / 8);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 32) blocks = 148LL * 32;
+  if (blocks > 132LL * 32) blocks = 132LL * 32;
   patchify_kernel<<<static_cast<int>(blocks < 1 ? 1 : blocks), 256, 0, st>>>(x, out, B, S, p, Kpad);
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;
@@ -160,7 +160,7 @@ static int dispatch_n4(int W, F&& f) {
 int embed_ln_pre_launch(float* x, const float* cls, const float* pos, const float* gamma, const float* beta, int rows, int L,
                         int W, cudaStream_t st) {
   CC_REQUIRE(W % 128 == 0, "embed_ln_pre: width %d not a multiple of 128", W);
-  const int blocks = rows < 148 * 8 ? (rows + 7) / 8 : 148 * 4;
+  const int blocks = rows < 132 * 8 ? (rows + 7) / 8 : 132 * 4;
   return dispatch_n4(W, [&](auto n4) -> int {
     embed_ln_pre_kernel<decltype(n4)::value><<<blocks < 1 ? 1 : blocks, 256, 0, st>>>(x, cls, pos, gamma, beta, rows, L, W);
     CC_CHECK_CUDA(cudaGetLastError());
@@ -172,7 +172,7 @@ int layernorm_bf16_launch(const float* x, __nv_bfloat16* out, const float* gamma
                           long long row_stride, const int* row_idx, cudaStream_t st) {
   CC_REQUIRE(W % 128 == 0, "layernorm: width %d not a multiple of 128", W);
   if (rows == 0) return CC_OK;
-  const int blocks = rows < 148 * 8 ? (rows + 7) / 8 : 148 * 4;
+  const int blocks = rows < 132 * 8 ? (rows + 7) / 8 : 132 * 4;
   return dispatch_n4(W, [&](auto n4) -> int {
     layernorm_bf16_kernel<decltype(n4)::value><<<blocks < 1 ? 1 : blocks, 256, 0, st>>>(x, out, gamma, beta, rows, W, row_stride, row_idx);
     CC_CHECK_CUDA(cudaGetLastError());
@@ -213,7 +213,7 @@ int text_embed_launch(const int* ids, const float* tok, const float* pos, float*
                       int vocab, cudaStream_t st) {
   CC_REQUIRE(W % 4 == 0, "text_embed: bad width");
   const int rows = B * L;
-  const int blocks = rows < 148 * 8 ? (rows + 7) / 8 : 148 * 4;
+  const int blocks = rows < 132 * 8 ? (rows + 7) / 8 : 132 * 4;
   text_embed_kernel<<<blocks < 1 ? 1 : blocks, 256, 0, st>>>(ids, tok, pos, x, eot_row, B, L, W, vocab);
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;
@@ -236,7 +236,7 @@ __global__ void l2norm_kernel(const float* __restrict__ in, float* __restrict__ 
 int l2norm_launch(const float* in, float* out, int rows, int D, long long out_stride, float eps, cudaStream_t st) {
   if (rows == 0) return CC_OK;
   const int blocks = (rows + 7) / 8;
-  l2norm_kernel<<<blocks > 148 * 4 ? 148 * 4 : blocks, 256, 0, st>>>(in, out, rows, D, out_stride, eps);
+  l2norm_kernel<<<blocks > 132 * 4 ? 132 * 4 : blocks, 256, 0, st>>>(in, out, rows, D, out_stride, eps);
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;
 }
@@ -245,7 +245,7 @@ int l2norm_launch(const float* in, float* out, int rows, int D, long long out_st
 // One CTA per (batch, head); K and V of the head live in shared memory ([Lp][72] bf16, 144-B pitch = conflict-free
 // for both the 32-bit B-fragment reads of K and ldmatrix.trans on V); each warp owns 16-query blocks and runs an
 // online-softmax (flash) loop over 16-key blocks with mma.sync m16n8k16 bf16 (fp32 accumulate).
-// NOTE: legacy tensor path (HMMA); attention is 4 % of the encoder FLOPs — a tcgen05 version is listed as next.
+// Serves the short sequences (several CTAs per SM hide the per-CTA chain); the long ones run on attention_tc.cu (wgmma).
 static constexpr int kAttnPitch = 72;  // bf16 elements per smem row
 
 __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -443,7 +443,7 @@ int search_scores_launch(const float* index, const float* q, float* scores, int 
   const int smem = Q * D * 4;
   CC_REQUIRE(smem <= 48 * 1024, "search: %d queries x %d dims exceed the 48 KB query buffer", Q, D);
   int blocks = (N + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   search_scores_kernel<<<blocks, 256, smem, st>>>(index, q, scores, N, D, Q);
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;
@@ -528,7 +528,7 @@ int search_topk_launch(const float* index, const float* q, const int* group, con
   CC_CHECK_CUDA(cudaMemsetAsync(best, 0, static_cast<size_t>(G > 0 ? G : 1) * sizeof(unsigned long long), st));
   if (N > 0) {
     int blocks = (N + 7) / 8;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     search_group_best_kernel<<<blocks, 256, D * 4, st>>>(index, q, group, mask, best, N, D);
     CC_CHECK_CUDA(cudaGetLastError());
   }

@@ -1,13 +1,13 @@
-"""Drop-in for the reference's `detection/yolov9.py` on B200 (same import names and call signatures).
+"""Drop-in for the reference's `detection/yolov9.py` on H100 (same import names and call signatures).
 
     from clearcam_b200.detection.yolov9 import YOLOv9
     model = YOLOv9(size="c", res=640, weights=state_dict_or_path)
     preds = model(frame).numpy()          # (300,6) float32 [x1,y1,x2,y2,conf,class]   (clearcam.py:583)
 
 Mirrors: class YOLOv9 (/root/reference/detection/yolov9.py:298-421), postprocess (:439-458), and the names
-test/run_mot.py:1-2 imports from the module.  All arithmetic runs in libclearcam_b200.so (hand-written sm_100a
+test/run_mot.py:1-2 imports from the module.  All arithmetic runs in libclearcam_b200.so (hand-written sm_90a
 kernels) through ctypes; torch tensors are only device containers.  There is no CPU fallback: without the
-library or without a B200 every call raises CCError.
+library or without an H100 every call raises CCError.
 
 Differences the reference cannot express (additions): `detect_batch(frames[B,H,W,3])`, explicit `weights=`
 (the reference downloads from HuggingFace at construction, :372; there is no network here).
@@ -146,7 +146,7 @@ class YOLOv9:
         L = lib()
         n = L.cc_device_check()
         if n <= 0:
-            raise CCError("clearcam_b200 needs a B200 (sm_100) GPU: " + L.cc_last_error().decode())
+            raise CCError("clearcam_b200 needs an H100 (sm_90) GPU: " + L.cc_last_error().decode())
         sd = {k.replace(".list.", "."): _to_host_fp32(v) for k, v in state_dict.items() if not k.endswith(("anchors", "strides"))}
         lib_size = self.size
         if self.pad and padding.padded_size(self.size):

@@ -1,4 +1,4 @@
-"""Drop-in for the reference's `models/objects.py` CLIP part on B200 (same names and call signatures).
+"""Drop-in for the reference's `models/objects.py` CLIP part on H100 (same names and call signatures).
 
     from clearcam_b200.models.objects import ObjectFinder
     finder = ObjectFinder(); finder.init_clip(weights=..., arch="ViT-L/14")
@@ -68,7 +68,7 @@ class OpenCLIP:
     def load_weights(self, state_dict) -> None:
         L = lib()
         if L.cc_device_check() <= 0:
-            raise CCError("clearcam_b200 needs a B200 (sm_100) GPU: " + L.cc_last_error().decode())
+            raise CCError("clearcam_b200 needs an H100 (sm_90) GPU: " + L.cc_last_error().decode())
         items = [(k, _to_host_fp32(v)) for k, v in state_dict.items() if k != "attn_mask"]
         names = (ctypes.c_char_p * len(items))(*[k.encode() for k, _ in items])
         ptrs = (ctypes.c_void_p * len(items))(*[a.ctypes.data for _, a in items])

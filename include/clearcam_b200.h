@@ -1,4 +1,4 @@
-/* clearcam_b200 — C-ABI of the B200-native per-frame vision hot path of roryclear/clearcam.
+/* clearcam_b200 — C-ABI of the H100-native per-frame vision hot path of roryclear/clearcam.
  *
  * The reference has no FFI: its boundary is Python call signatures (SURVEY.md §8b).  This header is the
  * C-ABI that sits UNDER those signatures; clearcam_b200/detection/yolov9.py and clearcam_b200/models/objects.py
@@ -25,7 +25,7 @@ extern "C" {
 
 int cc_version(void);
 const char* cc_last_error(void);
-/* number of SMs of the current device if it is sm_100 (B200), else <0 */
+/* number of SMs of the current device if it is sm_90 (H100), else <0 */
 int cc_device_check(void);
 
 /* activation codes */
@@ -38,8 +38,8 @@ int cc_device_check(void);
 /* Conv2d(bias) [+act] [+residual], k in {1,3}, stride in {1,2}, pad = k/2, NHWC bf16 in, bf16|fp32 out.
  * Replaces nn.Conv2d + .silu() of detection/yolov9.py:33-38 (and the bare nn.Conv2d of :173,:186,:224).
  * d_w: bf16 [Cout][k][k][Cin/groups]; d_bias: fp32 [Cout] or NULL; d_res: same dtype/shape class as out or NULL.
- * impl: 0 = auto (tcgen05 implicit GEMM when the shape allows, else direct), 1 = force tcgen05, 2 = force direct.
- * bn: tcgen05 N-tile override (0 = heuristic). */
+ * impl: 0 = auto (wgmma implicit GEMM when the shape allows, else direct), 1 = force wgmma, 2 = force direct.
+ * bn: wgmma N-tile upper bound (0 = heuristic). */
 int cc_conv2d(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin,
               const void* d_w, const float* d_bias, int Cout, int k, int stride, int groups,
               void* d_out, int out_cs, int out_co, int out_f32, int act,
@@ -60,7 +60,7 @@ typedef struct cc_yolo cc_yolo;
 int cc_yolo_create(const char* size, int n_tensors, const char* const* names, const float* const* h_data,
                    const int64_t* numels, cc_yolo** out);
 /* Same with options.  CC_YOLO_FP32_ACCURATE: the fp32-accurate mode — activations stored in fp32, every conv as six
- * bf16 plane products of a 3-way split of both operands on the same tcgen05 kernel (fp32 accumulation), exact SiLU.  The
+ * bf16 plane products of a 3-way split of both operands on the same wgmma kernel (fp32 accumulation), exact SiLU.  The
  * reference computes in fp32 end to end (SURVEY.md §2.1); this is the mode whose boxes / scores are compared with the fp32
  * oracle at the north-star tolerance.  Costs ~6x the tensor work and 2x the activation bytes of the default (bf16) mode. */
 #define CC_YOLO_FP32_ACCURATE 1

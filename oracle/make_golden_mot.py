@@ -5,7 +5,9 @@ person tracks with tracklet_len >= 1 and speed >= 2.5 -> the reference asserts 1
 TEST INFRASTRUCTURE.  The reference's detector cannot run here (tinygrad) and its weights are fetched from HuggingFace;
 this script runs the ORACLE detector with the YOLOv9-t weights recovered from the reference's iOS model blob
 (oracle/extract_ios_weights.py -> tests/golden/yolov9t_mot16.npz) on the reference's own video and stores the (1501,300,6)
-detections in tests/golden/mot16_oracle_dets.npz for tests/test_oracle_cpu.py.  bgr_swap=False: the configuration that also
+detections in tests/golden/mot16_oracle_dets.npz for tests/test_oracle_cpu.py, and frame 1 of the video as its uint8
+difference from frame 0 (mod 256; frame 0 is stored in yolov9t_mot16.npz) in tests/golden/mot16_frame1_delta.npz, so the
+test can re-run the oracle on the first two frames.  bgr_swap=False: the configuration that also
 reproduces the detections recorded in test/tracks.pkl (SURVEY.md D10: the reference's fixtures were recorded by a detector
 revision without the BGR->RGB swap of detection/yolov9.py:378; either that, or the blob's first conv is stored in BGR order).
 
@@ -42,11 +44,13 @@ def main():
     g = np.load(ROOT / "tests" / "golden" / "yolov9t_mot16.npz")
     P = {k[2:]: torch.from_numpy(g[k]) for k in g.keys() if k.startswith("w:")}
     cap = cv2.VideoCapture("/root/reference/test/videos/MOT16-03.mp4")
-    dets = []
+    dets, first = [], []
     while True:
         ret, im = cap.read()
         if not ret:
             break
+        if len(first) < 2:
+            first.append(im)
         with torch.no_grad():
             dets.append(o.detect("t", P, torch.from_numpy(im).float()[None], 960, bgr_swap=False)[0].numpy())
     dets = np.stack(dets)
@@ -55,6 +59,8 @@ def main():
     n_ref = count_people(dets, ref_ocsort.OCSort(max_age=60))
     print("frames", len(dets), "people tracks (reference tracker):", n_ref)
     np.savez_compressed(ROOT / "tests" / "golden" / "mot16_oracle_dets.npz", dets=dets, people=n_ref, expected=156)
+    assert np.array_equal(first[0], g["frame"])
+    np.savez_compressed(ROOT / "tests" / "golden" / "mot16_frame1_delta.npz", delta=first[1] - first[0])   # uint8: mod 256
 
 
 if __name__ == "__main__":

@@ -81,6 +81,18 @@ def synthetic_scene(seed, n_frames=240, n_obj=14, W=1280, H=720):
     return np.stack(frames)
 
 
+def random_scene_args(seed):
+    """Constructor arguments, detection threshold and scene of random scene `seed` (tests/golden/ocsort_random_scenes.npz)."""
+    g = np.random.default_rng(seed)
+    kw = dict(max_age=int(g.choice([5, 30, 100])), min_hits=int(g.choice([1, 3])), iou_threshold=float(g.choice([0.2, 0.3, 0.5])),
+              delta_t=int(g.choice([1, 2, 3])), inertia=float(g.choice([0.0, 0.2, 0.4])), use_byte=bool(g.integers(0, 2)))
+    thr = float(g.choice([0.25, 0.4, 0.5]))
+    return kw, thr, synthetic_scene(seed, n_frames=100, n_obj=int(g.integers(3, 25)))
+
+
+RANDOM_SEEDS = range(100, 112)
+
+
 def main():
     OUT.mkdir(parents=True, exist_ok=True)
     sys.path.insert(0, str(REF))
@@ -117,6 +129,14 @@ def main():
         out[f"{name}_args"] = np.array([thr, kw["max_age"], float(kw.get("use_byte", False))])
         print("tracker_inputs", name, rows.shape, "ids up to", rows[:, 6].max())
     np.savez_compressed(OUT / "ocsort_street.npz", **out)
+
+    # random scenes and constructor arguments: rows as float32 (the test compares at rtol 1e-5), offsets as int32
+    rnd = {}
+    for seed in RANDOM_SEEDS:
+        kw, thr, fr = random_scene_args(seed)
+        rows, offs = run_reference(fr, thr, **kw)
+        rnd[f"rows_{seed}"], rnd[f"offs_{seed}"] = np.asarray(rows, np.float32), np.asarray(offs, np.int32)
+    np.savez_compressed(OUT / "ocsort_random_scenes.npz", **rnd)
 
 
 if __name__ == "__main__":

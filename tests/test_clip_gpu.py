@@ -18,7 +18,8 @@ PROMPTS = ["ferrari f40", "text here", "a photo of a cat", "person riding a bicy
 
 @pytest.fixture(params=["0", "2"], ids=["attn-mma.sync", "attn-tcgen05"])
 def attn_mode(request, monkeypatch):
-    """Both attention kernels at every sequence length (CC_ATTN_TC is read when a plan is built; default 1 picks by shape)."""
+    """Both attention kernels at every sequence length (CC_ATTN_TC is read when a plan is built; default 1 picks by shape).
+    The second id names the tensor-core attention variant, attention_tc.cu (warpgroup MMA on Hopper)."""
     monkeypatch.setenv("CC_ATTN_TC", request.param)
     return request.param
 

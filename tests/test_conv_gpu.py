@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit-GEMM conv (and the direct conv) against a plain fp32 torch conv2d
+"""GPU parity of the wgmma implicit-GEMM conv (and the direct conv) against a plain fp32 torch conv2d
 on the same bf16-rounded operands.  Reference op: detection/yolov9.py:33-38 (Conv = Conv2d+bias -> SiLU)."""
 import pytest
 import torch
@@ -25,7 +25,7 @@ CASES = [
     (2, 40, 40, 256, 512, 1, 1, 1, False, False, 256, 0, 512, 0, 256),
     (4, 48, 80, 128, 128, 3, 2, 1, False, False, 256, 128, 128, 0, 0),
     (32, 40, 40, 256, 256, 3, 1, 1, False, False, 256, 0, 256, 0, 0),
-    # narrow tiles: the TMA-store staging uses 64-byte rows (SWIZZLE_64B) and only part of the epilogue warps
+    # narrow tiles (BN = 16: one thread of each pair converts the row alone) and odd channel counts
     (2, 40, 40, 32, 32, 3, 1, 1, True, False, 64, 32, 64, 0, 0),
     (2, 20, 20, 64, 16, 1, 1, 0, False, True, 64, 0, 16, 0, 0),
     (2, 20, 20, 64, 96, 3, 1, 1, False, False, 64, 0, 96, 0, 0),
@@ -79,9 +79,8 @@ def test_conv_matches_torch(case, impl):
 
 @pytest.mark.parametrize("Cout,out_f32,k", [(32, False, 3), (64, False, 3), (128, False, 1), (16, True, 1), (64, True, 3), (96, False, 1)])
 def test_conv_in_place_residual(Cout, out_f32, k):
-    """out = act(conv(x)) + out, the RepNBottleneck / transformer residual form: the residual tile is prefetched into
-    the staging buffer by TMA (bf16) or added by a TMA reduce-add store (fp32) — through the same tensor map as the store,
-    in both staging row widths."""
+    """out = act(conv(x)) + out, the RepNBottleneck / transformer residual form: the epilogue reads each residual element
+    before it writes the same element, in bf16 and fp32 and at every tile width."""
     g = torch.Generator(device="cuda").manual_seed(77 + Cout)
     N, H, W, Cin = 3, 24, 40, 64
     x = torch.randn(N, H, W, Cin, device="cuda", generator=g).to(torch.bfloat16)

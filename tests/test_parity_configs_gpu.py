@@ -22,9 +22,8 @@ from clearcam_b200.models.objects import OpenCLIP
 pytestmark = pytest.mark.gpu
 
 CASES = [("c", 640, 32, 640, 640), ("e", 640, 16, 640, 640), ("c", 640, 8, 1080, 1920)]
-# measured on B200 (tests/tools/diag_precise.py), default mode vs fp32 oracle, head output over ALL anchors:
-#   size c: box |d| p50 ~0.1 px, p99 ~2-3.5 px; class prob |d| p99 ~4e-3, max ~0.06 (synthetic weights are far worse
-#   conditioned than trained ones: real YOLOv9-t weights give p90 0.15 px)
+# default mode vs fp32 oracle, head output over ALL anchors (tests/tools/diag_precise.py prints the quantiles): synthetic
+# weights are far worse conditioned than trained ones, so the absolute bars are loose sanity bounds
 DEFAULT_BARS = {"box_p50": 0.5, "box_p99": 12.0, "prob_p99": 3e-2, "prob_max": 0.2}     # absolute sanity (the relative bars below are the test)
 PRECISE_BARS = {"box_p99": 1e-2, "box_max": 0.25, "prob_max": 1e-3}
 

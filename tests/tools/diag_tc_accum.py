@@ -1,4 +1,4 @@
-"""GPU diagnostic: how accurate is the tcgen05 fp32 accumulation behind the fp32-accurate mode?  One conv through the same
+"""GPU diagnostic: how accurate is the tensor-core fp32 accumulation behind the fp32-accurate mode?  One conv through the same
 six-plane bf16 split the detector uses (yolo.cu / pool.cu split_planes_kernel), built here in torch, against fp64 and fp32
 CPU convs of the same fp32 operands.  Prints the signed mean (bias = truncating accumulation) and the rms of the relative
 error.  usage: diag_tc_accum.py"""
@@ -40,7 +40,7 @@ def run(N, H, W, Cin, Cout, k, positive):
     ref64 = F.conv2d(xn.double(), wn.double(), padding=k // 2).permute(0, 2, 3, 1)
     ref32 = F.conv2d(xn, wn, padding=k // 2).permute(0, 2, 3, 1).double()
     scale = ref64.abs().mean()
-    for tag, t in (("tcgen05 six-plane", got), ("torch fp32 CPU   ", ref32)):
+    for tag, t in (("wgmma six-plane  ", got), ("torch fp32 CPU   ", ref32)):
         e = (t - ref64) / scale
         print(f"  {tag}: signed mean {e.mean():+.3e}  rms {e.pow(2).mean().sqrt():.3e}  max {e.abs().max():.3e}")
 

@@ -1,6 +1,7 @@
 // Dev tool (no GPU needed): run conv_gemm_build's host-side tiling / shared-memory budget over the conv shapes of the
 // detector and the CLIP linears with a stub tensor-map encoder, and print the configuration each one gets.
-//   nvcc -std=c++17 --expt-relaxed-constexpr -I clearcam_b200/csrc -I include -o /tmp/hbc tests/tools/host_budget_check.cu && /tmp/hbc
+//   nvcc -gencode arch=compute_90a,code=sm_90a -std=c++17 --expt-relaxed-constexpr -I clearcam_b200/csrc -I include \
+//        -o /tmp/hbc tests/tools/host_budget_check.cu && /tmp/hbc
 #include "../../clearcam_b200/csrc/conv_gemm.cu"
 #include <stdarg.h>
 namespace cc {
@@ -12,7 +13,7 @@ static CUresult fake_enc(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, c
   return CUDA_SUCCESS;
 }
 PFN_encodeTiled get_encode_tiled() { return fake_enc; }
-int device_sm_count() { return 148; }
+int device_sm_count() { return 132; }   // H100 SXM
 }
 using namespace cc;
 int main() {
@@ -37,7 +38,7 @@ int main() {
       {32, 40, 40, 6144, 512, 1, 1, 1, 0}, {32, 160, 160, 768, 128, 3, 2, 1, 0}};
   static float dummy[64];
   int bad = 0;
-  printf("%-34s %4s %3s %2s %3s %3s %2s %2s %4s %4s %3s %7s %6s %6s\n", "shape", "BN", "BK", "nA", "lgw", "CH", "S", "hs", "halo", "bres", "tma", "smem", "tiles", "grid");
+  printf("%-34s %4s %3s %2s %4s %7s %6s %6s\n", "shape", "BN", "BK", "S", "bres", "smem", "tiles", "grid");
   for (const S& q : shapes) {
     ConvDesc d{};
     d.in = dummy; d.in_cs = q.Cin; d.in_co = 0; d.Cin = q.Cin; d.N = q.N; d.Hin = q.H; d.Win = q.W; d.k = q.k; d.stride = q.s;
@@ -46,12 +47,11 @@ int main() {
     GemmLaunch L;
     char name[96];
     snprintf(name, sizeof(name), "%dx%dx%d %d->%d k%d s%d %s%s", q.N, q.H, q.W, q.Cin, q.Cout, q.k, q.s, q.f32 ? "f32" : "bf16", q.res ? "+res" : "");
-    int rc = conv_gemm_build(d, 148, &L);
+    int rc = conv_gemm_build(d, device_sm_count(), &L);
     if (rc) { printf("%-34s FAILED: %s\n", name, last_error()); ++bad; continue; }
     const GemmParams& p = L.p;
-    printf("%-34s %4d %3d %2d %3d %3d %2d %2d %4d %4d %3d %7d %6d %6d\n", name, p.BN, p.BK, p.n_acc, p.lgw, p.CH, p.stages, p.halo_stages, p.halo, p.b_res,
-           p.tma_store ? p.stg_lrow : 0, L.smem_bytes, p.num_tiles, L.grid);
-    if (L.smem_bytes > 232448) { printf("   ^^^ exceeds shared memory\n"); ++bad; }
+    printf("%-34s %4d %3d %2d %4d %7d %6d %6d\n", name, p.BN, p.BK, p.stages, p.b_res, L.smem_bytes, p.num_tiles, L.grid);
+    if (L.smem_bytes > kMaxSmem) { printf("   ^^^ exceeds shared memory\n"); ++bad; }
   }
   return bad ? 1 : 0;
 }

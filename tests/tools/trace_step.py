@@ -25,7 +25,7 @@ for _ in range(5):
         best = (span, tr)
 span, tr = best
 print(f"span first conv entry -> last conv exit: {span/1e6:.3f} ms (B={B})")
-print(f"{'#':>3} {'kind':12s} {'name':34s} {'t_in_us':>9s} {'t_dep_us':>9s} {'t_out_us':>9s} {'work_us':>8s} {'gap_us':>7s} {'ideal_us':>8s} | CTA 0, us after t_dep: operands landed, MMAs issued, first acc done, epilogue done, exit) | first staging pass, SM cycles after 'staging free': TMEM loads returned, first chunk staged, all chunks staged")
+print(f"{'#':>3} {'kind':12s} {'name':34s} {'t_in_us':>9s} {'t_dep_us':>9s} {'t_out_us':>9s} {'work_us':>8s} {'gap_us':>7s} {'ideal_us':>8s} | CTA 0, us after t_dep: operands landed, MMAs issued, first acc done, epilogue done, exit) | first staging pass, SM cycles after 'staging free': (unused)")
 prev_out = 0
 tw = tg = 0.0
 nonconv = []

@@ -1,5 +1,5 @@
-// Throughput of the epilogue's candidate instructions on one SM sub-partition mix (B200): cycles per warp-instruction with
-// 1, 2, 4, 8 warps per scheduler.  build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench_pipes ubench_pipes.cu
+// Throughput of the epilogue's candidate instructions on one SM sub-partition mix: cycles per warp-instruction with
+// 1, 2, 4, 8 warps per scheduler.  build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench_pipes ubench_pipes.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
