@@ -9,9 +9,11 @@
 //     stride 2 uses a 5-D "pixel pair" view (dims: 2*C, W/2, 2, H/2, N) so every tap is again a dense box.
 //   * smem tiles are K-major, 128/64/32-byte swizzled (BK = 64/32/16 channels) exactly as TMA writes them;
 //     wgmma.mma_async (M=64, N=BN, K=16) reads them through shared-memory descriptors, accumulators in registers.
-//   * warpgroup roles: wg0 = TMA producer (one thread), wg1 / wg2 = consumers, each owning 64 rows of the tile:
-//     wgmma mainloop -> fp32 accumulators to smem -> thread pair == output row: bias -> SiLU/GELU -> (+residual) ->
-//     bf16/fp32 in place -> coalesced 16-B stores.
+//   * warpgroup roles ("ping-pong"): wg0 = TMA producer (one thread), wg1 / wg2 = consumers that take the CTA's tiles
+//     in turn, each owning a whole 128 x BN tile (two m64 wgmmas per k16).
+//     An ordering barrier makes their mainloops alternate, so one warpgroup's epilogue (bias -> SiLU/GELU -> +residual
+//     on the accumulator registers -> bf16/fp32 into its own swizzled staging tile -> TMA tensor store) runs while the
+//     other one's MMAs keep the tensor cores busy.
 //   * persistent: grid = min(tiles, SMs), static round-robin tile schedule.
 #include "conv_gemm.cuh"
 #include "cc_common.h"
@@ -19,15 +21,25 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
+#include <type_traits>
 
 namespace cc {
 
-static constexpr int kConsumers = 2;                       // consumer warpgroups (64 rows each)
+static constexpr int kConsumers = 2;                       // consumer warpgroups (whole tiles, alternating)
 static constexpr int kThreads = 128 * (1 + kConsumers);     // wg0 producer + consumers
 static constexpr int kEpiThreads = 128 * kConsumers;
 static constexpr int kTileM = 128;
 static constexpr int kMaxBN = 128;
 static constexpr int kMaxSmem = 232448;  // 227 KB
+static constexpr int kBarriers = 24;      // full[S <= 8], empty[S], resident weights, turn[2], residual[2]
+
+// Output staging of one consumer warpgroup.  The 128 x BN tile is cut into column boxes of one swizzle span (<= 128 B)
+// x 128 rows, each written with the span's XOR swizzle (conflict-free fragment stores) and stored by one TMA box.  fp32
+// tiles of BN = 128 (the CLIP residual stream, the fp32-accurate mode) go out in two column passes of 32 KB so the operand
+// ring keeps its depth.
+__host__ __device__ constexpr int epi_box_bytes(int bn, int es) { return bn * es < 128 ? bn * es : 128; }
+__host__ __device__ constexpr int epi_passes(int bn, int es) { return es == 4 && bn == 128 ? 2 : 1; }
+__host__ __device__ constexpr int epi_stage_bytes(int bn, int es) { return kTileM * bn * es / epi_passes(bn, es); }
 
 __device__ __forceinline__ float tanh_approx(float x) {
   float t;
@@ -82,11 +94,18 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// One k-block (BK channels = KPB steps of K = 16) of this warpgroup's 64 x BN accumulator.
-template <int BN>
-__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t adesc, uint64_t bdesc, int kpb, bool first) {
-  Wgmma<BN>::mma(acc, adesc, bdesc, first ? 0u : 1u);
-  for (int k = 1; k < kpb; ++k) Wgmma<BN>::mma(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+// One k-block (BK channels = KPB steps of K = 16) of a 128 x BN tile: rows [0, 64) into acc0, rows [64, 128) into acc1
+// (`ahalf` = descriptor offset of row 64).  Each accumulator sees the same k order as a single m64 warpgroup would.
+// KPB is a compile-time constant so the 2 KPB wgmmas go out as one batch: with a runtime trip count ptxas waits for each
+// pair before issuing the next, and only one consumer is in its mainloop at a time to cover such gaps.
+template <int BN, int KPB>
+__device__ __forceinline__ void mma_kblock(float (&acc0)[BN / 2], float (&acc1)[BN / 2], uint64_t adesc, uint64_t bdesc,
+                                           uint32_t ahalf, bool first) {
+#pragma unroll
+  for (int k = 0; k < KPB; ++k) {
+    Wgmma<BN>::mma(acc0, adesc + 2 * k, bdesc + 2 * k, first && k == 0 ? 0u : 1u);
+    Wgmma<BN>::mma(acc1, adesc + ahalf + 2 * k, bdesc + 2 * k, first && k == 0 ? 0u : 1u);
+  }
 }
 
 template <int ACT, bool F32, int BN>
@@ -95,49 +114,64 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
   // 1024-B alignment for the 128B-swizzled tiles
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
+  constexpr int es = F32 ? 4 : 2;
+  constexpr int kBoxBytes = epi_box_bytes(BN, es);
+  constexpr int kBoxCols = kBoxBytes / es;
+  constexpr int kBoxTile = kTileM * kBoxBytes;                  // one column box in smem (a multiple of 4 KB)
+  constexpr int kPasses = epi_passes(BN, es);
+  constexpr int kPassCols = BN / kPasses;
+  constexpr int kPassBoxes = kPassCols / kBoxCols;
+  constexpr int kStageBytes = epi_stage_bytes(BN, es);
+  constexpr uint32_t kSwz = kBoxBytes == 128 ? 0x70 : (kBoxBytes == 64 ? 0x30 : 0x10);   // 16-B chunk bits XORed by row
+
   const int wg = threadIdx.x >> 7;
   const uint32_t row_bytes = p.BK * 2;
   const uint32_t a_bytes = kTileM * row_bytes;
   const uint32_t b_bytes = BN * row_bytes;
   const int S = p.stages;
-  constexpr int es = F32 ? 4 : 2;
-  constexpr uint32_t pitch = BN * 4 + 16;                 // fp32 accumulator row in the staging buffer (+16 B: bank spread)
   const int num_kb = p.num_taps * p.chunks_per_tap;
 
-  uint8_t* sA = smem;
+  uint8_t* sStage = smem;                                     // kConsumers x kStageBytes, 1024-B aligned
+  uint8_t* sA = sStage + kConsumers * kStageBytes;
   uint8_t* sB = sA + S * a_bytes;
   // resident-B mode: sB holds ALL k-blocks of the weights (loaded once); the ring then carries A only
-  uint8_t* sStage = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(sB + (p.b_res ? num_kb : S) * b_bytes) + 15) & ~uintptr_t(15));
-  float* sBias = reinterpret_cast<float*>(sStage + kTileM * pitch);
+  float* sBias = reinterpret_cast<float*>(sB + (p.b_res ? num_kb : S) * b_bytes);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + p.cout);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + S;
   uint64_t* bres_bar = bars + 2 * S;
+  uint64_t* turn_bar = bars + 2 * S + 1;    // [c]: consumer c may start its next mainloop
+  uint64_t* res_bar = bars + 2 * S + 3;     // [c]: residual tile of consumer c landed in its staging
 
   if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[0] = globaltimer_ns();
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmB);
+    tma_prefetch_desc(&p.tmO);
     for (int i = 0; i < S; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], kConsumers);   // one arrival per consumer warpgroup
+      mbar_init(&empty_bar[i], 1);   // released by the one consumer warpgroup that read the stage
     }
     mbar_init(bres_bar, 1);
+    for (int c = 0; c < kConsumers; ++c) {
+      mbar_init(&turn_bar[c], 1);
+      mbar_init(&res_bar[c], 1);
+    }
     fence_mbar_init();
   }
-  if (wg > 0) {  // bias -> smem once per CTA (epilogue reads it as broadcast LDS.128)
+  if (wg > 0) {  // bias -> smem once per CTA
     for (int i = threadIdx.x - 128; i < p.cout; i += kEpiThreads) sBias[i] = p.bias ? __ldg(p.bias + i) : 0.f;
   }
   __syncthreads();
   // PDL: let the next kernel start its prologue as our CTAs retire; everything that only touches WEIGHTS (bias above,
   // resident weight tiles below) runs before griddepcontrol.wait, i.e. overlaps the previous kernel's tail.
-  // Activations of the previous layer are read only by the TMA producer (A operand) and the epilogue (residual):
-  // both execute pdl_wait() first.
+  // Activations of the previous layer are read only by the TMA producer (A operand) and the consumers (residual, pre
+  // addend): both execute pdl_wait() first.
   pdl_trigger();
 
   if (wg == 0) {
     if (threadIdx.x == 0) {
-      // ===================== TMA producer =====================
+      // ===================== TMA producer: every tile of the CTA, in order, into one ring =====================
       int stage = 0;
       uint32_t phase = 0;
       if (p.b_res) {   // weights are not produced by the previous kernel: issued BEFORE the grid dependency wait
@@ -166,154 +200,149 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       }
     }
   } else {
-    // ===================== consumers: warpgroup c owns rows [64 c, 64 c + 64) of every tile =====================
+    // ===================== consumers: warpgroup c owns the CTA's local tiles c, c + 2, c + 4, ... =====================
     const int c = wg - 1;
-    const int et = static_cast<int>(threadIdx.x) - 128;      // 0 .. 255 over both consumers
-    const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
-    const int kpb = p.BK >> 4;
+    const int t = threadIdx.x & 127;
+    const bool lead = t == 0;
+    const int lane = t & 31, wq = t >> 5;
     const uint64_t dconst = gmma_desc_const(row_bytes, 8u * row_bytes);
-    const uint32_t sA16 = ((smem_u32(sA) & 0x3FFFF) >> 4) + ((c * 64 * row_bytes) >> 4), sB16 = (smem_u32(sB) & 0x3FFFF) >> 4;
-    const uint32_t a16 = a_bytes >> 4, b16 = b_bytes >> 4;
-    const uint32_t stg32 = smem_u32(sStage), sbias32 = smem_u32(sBias);
+    const uint32_t sA16 = (smem_u32(sA) & 0x3FFFF) >> 4, sB16 = (smem_u32(sB) & 0x3FFFF) >> 4;
+    const uint32_t a16 = a_bytes >> 4, b16 = b_bytes >> 4, ahalf = (64 * row_bytes) >> 4;
+    const uint32_t stg = smem_u32(sStage + c * kStageBytes), sbias32 = smem_u32(sBias);
     const int TWm = (1 << p.lTW) - 1, THm = (1 << p.lTH) - 1;
-    // register phase: thread pair == output row, the pair's halves take columns [0, BN/2) and [BN/2, BN).  A bf16 result is
-    // written back over the fp32 accumulators it was computed from; the second half's results go after the first half's
-    // fp32 values (byte BN*2 on), so neither thread overwrites values the other has yet to read.
-    // (BN = 16 is one 16-column chunk: the first thread of the pair converts it alone)
-    constexpr bool kSplit = BN >= 32;
-    constexpr int kHalfCols = kSplit ? BN / 2 : BN;
-    const int row = et >> 1, half = et & 1;
-    const uint32_t out_off = F32 ? 0u : static_cast<uint32_t>(half) * BN * 2;    // bf16: where this half's fp32 columns start
-    int stage = 0;
-    uint32_t phase = 0;
-    bool first_tile = true;
+    // the residual of column pass `pass` of the tile at (nb, w0, h0, n0) -> this warpgroup's staging, on res_bar[c]
+    auto load_res = [&](const TileXY& tx, int pass) {
+      mbar_arrive_expect_tx(&res_bar[c], kStageBytes);
+#pragma unroll
+      for (int b = 0; b < kPassBoxes; ++b)
+        tma_load_4d(stg + b * kBoxTile, &p.tmR, &res_bar[c], tx.nb * BN + pass * kPassCols + b * kBoxCols, tx.w0, tx.h0, tx.n0);
+    };
     if (p.b_res) mbar_wait(bres_bar, 0);
-    pdl_wait();   // residual reads below depend on the previous kernel's output
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const TileXY tx = tile_origin(p, tile);
-      float acc[BN / 2];
+    pdl_wait();   // residual / pre reads depend on the previous kernel's output
+    // barrier phases follow from the local tile index j: this consumer's (j / 2)-th tile; consumer 0 runs the CTA's first
+    // mainloop (j = 0) without waiting
+    for (int j = c; blockIdx.x + j * gridDim.x < p.num_tiles; j += kConsumers) {
+      const TileXY tx = tile_origin(p, blockIdx.x + j * gridDim.x);
+      // prefetch the residual while the mainloop runs, once the previous tile's stores have read the staging
+      if (p.res != nullptr && lead) {
+        tma_store_wait_read<0>();
+        load_res(tx, 0);
+      }
+      if (j > 0) mbar_wait(&turn_bar[c], ((j >> 1) + (c == 0)) & 1);
+
+      float acc0[BN / 2], acc1[BN / 2];
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int i = 0; i < BN / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+      // this tile's k-blocks follow those of the CTA's earlier tiles in the ring
+      const int g0 = j * num_kb;
+      int stage = g0 % S;
+      uint32_t phase = (g0 / S) & 1;
       int prev = -1;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        if (first_tile && kb == 0 && p.trace && blockIdx.x == 0 && et == 0) p.trace[3] = globaltimer_ns();
-        wgmma_fence_acc(acc);
-        wgmma_fence();
-        mma_kblock<BN>(acc, dconst | (sA16 + stage * a16), dconst | (sB16 + (p.b_res ? kb : stage) * b16), kpb, kb == 0);
-        wgmma_commit();
-        wgmma_fence_acc(acc);
-        wgmma_wait<1>();       // the previous k-block's MMAs are done: release its stage
-        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
-        prev = stage;
-        if (++stage == S) { stage = 0; phase ^= 1; }
-      }
+      auto mainloop = [&](auto kpb_c) {    // BK = 16 KPB
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          if (j == 0 && kb == 0 && p.trace && blockIdx.x == 0 && lead) p.trace[3] = globaltimer_ns();
+          wgmma_fence_acc(acc0);
+          wgmma_fence_acc(acc1);
+          wgmma_fence();
+          mma_kblock<BN, decltype(kpb_c)::value>(acc0, acc1, dconst | (sA16 + stage * a16),
+                                                 dconst | (sB16 + (p.b_res ? kb : stage) * b16), ahalf, kb == 0);
+          wgmma_commit();
+          wgmma_fence_acc(acc0);
+          wgmma_fence_acc(acc1);
+          wgmma_wait<1>();       // the previous k-block's MMAs are done: release its stage
+          if (prev >= 0 && lead) mbar_arrive(&empty_bar[prev]);
+          prev = stage;
+          if (++stage == S) { stage = 0; phase ^= 1; }
+        }
+      };
+      if (p.BK == 64) mainloop(std::integral_constant<int, 4>{});
+      else if (p.BK == 32) mainloop(std::integral_constant<int, 2>{});
+      else mainloop(std::integral_constant<int, 1>{});
+      if (lead) mbar_arrive(&turn_bar[c ^ 1]);   // every MMA of this tile is issued: the other consumer's mainloop may start
       wgmma_wait<0>();
-      wgmma_fence_acc(acc);
-      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
-      if (first_tile && p.trace && blockIdx.x == 0 && et == 0) p.trace[5] = globaltimer_ns();
-      first_tile = false;
+      wgmma_fence_acc(acc0);
+      wgmma_fence_acc(acc1);
+      if (lead) mbar_arrive(&empty_bar[prev]);
+      if (j == 0 && p.trace && blockIdx.x == 0 && lead) p.trace[5] = globaltimer_ns();
 
-      // ---- accumulators -> staging (fp32 rows of `pitch` bytes)
-      named_bar_sync(1, kEpiThreads);     // the previous tile's copy-out has read the staging buffer
-      {
-        const int r0 = c * 64 + wq * 16 + (lane >> 2);
-        const uint32_t base = stg32 + r0 * pitch + (lane & 3) * 8;
-#pragma unroll
-        for (int i = 0; i < BN / 8; ++i) {
-          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(base + i * 32), "f"(acc[4 * i]), "f"(acc[4 * i + 1]) : "memory");
-          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(base + 8 * pitch + i * 32), "f"(acc[4 * i + 2]), "f"(acc[4 * i + 3]) : "memory");
-        }
-      }
-      named_bar_sync(1, kEpiThreads);
-
-      // ---- register phase: this thread's pixel, columns [half BN/2, (half+1) BN/2)
-      const int nb = tx.nb, w0 = tx.w0, h0 = tx.h0, n0 = tx.n0;
-      const int pw = w0 + (row & TWm), ph = h0 + ((row >> p.lTW) & THm), pn = n0 + (row >> (p.lTW + p.lTH));
-      const bool pvalid = (pw < p.W) && (ph < p.H) && (pn < p.N);
-      const long long ppix = static_cast<long long>(pn) * p.out_ns + ph * p.W + pw;
-      // pre-activation addend from a half-resolution fp32 map (nearest x2 upsample by addressing): this pixel's source row
-      const float* const pre_row = (p.pre != nullptr && pvalid)
-          ? p.pre + ((static_cast<long long>(pn) * p.pre_h + (ph >> 1)) * p.pre_w + (pw >> 1)) * p.cout : nullptr;
-      const uint32_t srow = stg32 + row * pitch;
-#pragma unroll 1
-      for (int cc = half * kHalfCols; cc < (kSplit || half == 0 ? (half + 1) * kHalfCols : 0); cc += 16) {
-        const int gcol = nb * BN + cc;   // global output channel of column cc
-        float f[16];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const uint4 vu = lds_u4(srow + (cc + 4 * j) * 4);
-          const float4 v = make_float4(__uint_as_float(vu.x), __uint_as_float(vu.y), __uint_as_float(vu.z), __uint_as_float(vu.w));
-          float4 b4 = lds_f4(sbias32 + (gcol + 4 * j) * 4);
-          if (pre_row != nullptr) {
-            const float4 q4 = __ldg(reinterpret_cast<const float4*>(pre_row + gcol) + j);
-            b4.x += q4.x; b4.y += q4.y; b4.z += q4.z; b4.w += q4.w;
-          }
-          f[4 * j] = act_apply<ACT>(v.x + b4.x);
-          f[4 * j + 1] = act_apply<ACT>(v.y + b4.y);
-          f[4 * j + 2] = act_apply<ACT>(v.z + b4.z);
-          f[4 * j + 3] = act_apply<ACT>(v.w + b4.w);
-        }
-        if (p.res != nullptr && pvalid) {
-          if (F32) {
-            const float4* r4 = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.res) + ppix * p.res_cs + p.res_co + gcol);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float4 r = __ldg(r4 + j);
-              f[4 * j + 0] += r.x; f[4 * j + 1] += r.y; f[4 * j + 2] += r.z; f[4 * j + 3] += r.w;
-            }
-          } else {
-            const uint4* r4 = reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(p.res) + ppix * p.res_cs + p.res_co + gcol);
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-              const uint4 r = __ldg(r4 + j);
-              const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                // bf16 -> fp32 is a 16-bit shift
-                f[8 * j + 2 * q + 0] += __uint_as_float(rr[q] << 16);
-                f[8 * j + 2 * q + 1] += __uint_as_float(rr[q] & 0xFFFF0000u);
-              }
-            }
-          }
-        }
-        // in place: fp32 results over their own accumulators; bf16 results of column cc at out_off + 2 (cc - half BN/2), which
-        // only covers fp32 columns of this thread that it has already read
-        const uint32_t dst = F32 ? srow + cc * 4 : srow + out_off + (cc - half * kHalfCols) * 2;
-        if (F32) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            sts_u4(dst + 16 * j, __float_as_uint(f[4 * j]), __float_as_uint(f[4 * j + 1]), __float_as_uint(f[4 * j + 2]), __float_as_uint(f[4 * j + 3]));
+      // ---- epilogue on the accumulator fragments.  Thread t holds rows 64 m + 16 (t / 32) + (t % 32) / 4 + 8 r (m, r in
+      // {0, 1}: fragment quarter q = 2 m + r) and columns 8 i + 2 (t % 4) + {0, 1}.
+      const int nb = tx.nb;
+      const uint32_t bias_t = sbias32 + (nb * BN + 2 * (lane & 3)) * 4;   // this thread's first bias pair
+      // one column pass (a compile-time constant, so every accumulator index below is static and stays in registers)
+      auto epilogue_pass = [&](auto pass_c) {
+        constexpr int pass = decltype(pass_c)::value;
+        if (p.res != nullptr) {  // the residual landed in the staging (loaded after the previous stores had read it)
+          mbar_wait(&res_bar[c], ((j >> 1) * kPasses + pass) & 1);
         } else {
-#pragma unroll
-          for (int j = 0; j < 2; ++j)
-            sts_u4(dst + 16 * j, pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
-                   pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7]));
+          if (lead) tma_store_wait_read<0>();   // the previous tile's stores have read the staging
+          named_bar_sync(1 + c, 128);
         }
-      }
-      named_bar_sync(1, kEpiThreads);    // results staged
-
-      // ---- coalesced copy-out, division free: a set of `1 << lg` (power of two >= chunks per row) threads owns one row
-      constexpr int cpr = (BN * es) >> 4;  // 16-B chunks per row (2..32)
-      constexpr int hcpr = cpr / 2;        // chunks of one half
-      constexpr int lg = cpr > 16 ? 5 : (cpr > 8 ? 4 : (cpr > 4 ? 3 : (cpr > 2 ? 2 : 1)));
-      const int chk = et & ((1 << lg) - 1);
-      constexpr int rstep = kEpiThreads >> lg;
-      if (chk < cpr) {
-        // bf16: the second half's results start at byte 2 BN of the staging row (see out_off)
-        const uint32_t soff = (F32 || !kSplit) ? chk * 16 : (chk < hcpr ? chk * 16 : BN * 2 + (chk - hcpr) * 16);
-        uint8_t* gbase = reinterpret_cast<uint8_t*>(p.out) + static_cast<size_t>(p.out_co + nb * BN) * es + chk * 16;
-        for (int r = et >> lg; r < kTileM; r += rstep) {
-          const int qw = w0 + (r & TWm), qh = h0 + ((r >> p.lTW) & THm), qn = n0 + (r >> (p.lTW + p.lTH));
-          if (qw < p.W && qh < p.H && qn < p.N) {
-            const long long pix = static_cast<long long>(qn) * p.out_ns + qh * p.W + qw;
-            const uint4 val = lds_u4(stg32 + r * pitch + soff);
-            *reinterpret_cast<uint4*>(gbase + pix * p.out_cs * es) = val;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int row = 64 * (q >> 1) + 16 * wq + (lane >> 2) + 8 * (q & 1);
+          // pre-activation addend from a half-resolution fp32 map (nearest x2 upsample by addressing): this row's source
+          const float* pre_row = nullptr;
+          if (p.pre != nullptr) {
+            const int pw = tx.w0 + (row & TWm), ph = tx.h0 + ((row >> p.lTW) & THm), pn = tx.n0 + (row >> (p.lTW + p.lTH));
+            if ((pw < p.W) && (ph < p.H) && (pn < p.N))
+              pre_row = p.pre + ((static_cast<long long>(pn) * p.pre_h + (ph >> 1)) * p.pre_w + (pw >> 1)) * p.cout + nb * BN;
+          }
+          // staging address of (row, column): the TMA box swizzle XORs the 16-B chunk index with bits of the row offset
+          const uint32_t roff = static_cast<uint32_t>(row * kBoxBytes), rxor = (roff >> 3) & kSwz;
+          const uint32_t rbase = stg + roff;
+#pragma unroll
+          for (int i = pass * kPassCols / 8; i < (pass + 1) * kPassCols / 8; ++i) {
+            const int col = 8 * i + 2 * (lane & 3);
+            const float2 bb = lds_f2(bias_t + 32 * i);
+            const int pc = col - pass * kPassCols;
+            float b0 = bb.x, b1 = bb.y;
+            if (pre_row != nullptr) {
+              const float2 pq = __ldg(reinterpret_cast<const float2*>(pre_row + col));
+              b0 += pq.x; b1 += pq.y;
+            }
+            const int k = 4 * i + 2 * (q & 1);
+            float f0 = act_apply<ACT>(((q >> 1) ? acc1[k] : acc0[k]) + b0);
+            float f1 = act_apply<ACT>(((q >> 1) ? acc1[k + 1] : acc0[k + 1]) + b1);
+            const uint32_t addr = rbase + (pc / kBoxCols) * kBoxTile + (((pc % kBoxCols) * es) ^ rxor);
+            if (F32) {
+              if (p.res != nullptr) {
+                const float2 r = lds_f2(addr);
+                f0 += r.x; f1 += r.y;
+              }
+              sts_f2(addr, f0, f1);
+            } else {
+              if (p.res != nullptr) {
+                const uint32_t r = lds_u32(addr);   // bf16 -> fp32 is a 16-bit shift
+                f0 += __uint_as_float(r << 16);
+                f1 += __uint_as_float(r & 0xFFFF0000u);
+              }
+              sts_u32(addr, pack_bf16x2(f0, f1));
+            }
           }
         }
-      }
+        fence_proxy_async_smem();      // generic-proxy writes -> visible to the TMA store
+        named_bar_sync(1 + c, 128);
+        if (lead) {
+          // the box is clipped at the edges of the output slice [out_co, out_co + Cout) x W x H x N
+#pragma unroll
+          for (int b = 0; b < kPassBoxes; ++b)
+            tma_store_4d(&p.tmO, stg + b * kBoxTile, nb * BN + pass * kPassCols + b * kBoxCols, tx.w0, tx.h0, tx.n0);
+          tma_store_commit();
+          if (p.res != nullptr && pass + 1 < kPasses) {
+            tma_store_wait_read<0>();
+            load_res(tx, pass + 1);
+          }
+        }
+      };
+      epilogue_pass(std::integral_constant<int, 0>{});
+      if constexpr (kPasses > 1) epilogue_pass(std::integral_constant<int, 1>{});
     }
-    if (p.trace != nullptr && blockIdx.x == 0 && et == 0) p.trace[6] = globaltimer_ns();   // last epilogue of CTA 0 done
+    if (lead) {
+      tma_store_wait_all();    // the output is complete in global memory before the CTA retires (PDL successors read it)
+      if (p.trace != nullptr && blockIdx.x == 0) atomicMax(p.trace + 6, globaltimer_ns());   // last epilogue of CTA 0 done
+    }
   }
   if (p.trace && threadIdx.x == 0) {
     atomicMax(p.trace + 2, globaltimer_ns());
@@ -442,6 +471,25 @@ int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
   p.out_ns = d.out_ns > 0 ? d.out_ns : Hout * Wout;
   p.pre = d.pre; p.pre_h = d.pre_h; p.pre_w = d.pre_w;
   if (d.pre) CC_REQUIRE(d.pre_h * 2 == Hout && d.pre_w * 2 == Wout && d.Cout % 4 == 0, "conv_gemm: the pre-activation addend must be a half-resolution map of the output");
+  {     // output slice (and residual) as [N][H][W][Cout] with the buffer's strides, box = one staging column box x the pixel box
+    const int box_bytes = epi_box_bytes(BN, es);   // one swizzle span: the kernel writes the staging with the same XOR
+    const CUtensorMapSwizzle oswz = box_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                  : box_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
+    auto encode = [&](CUtensorMap* tm, const void* buf, int cs, int co, const char* what) -> int {
+      void* base = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(buf)) + size_t(co) * es;
+      cuuint64_t dims[4] = {cuuint64_t(d.Cout), cuuint64_t(Wout), cuuint64_t(Hout), cuuint64_t(d.N)};
+      const cuuint64_t px = cuuint64_t(cs) * es;     // bytes per pixel
+      cuuint64_t strides[3] = {px, px * Wout, px * p.out_ns};
+      cuuint32_t box[4] = {cuuint32_t(box_bytes / es), cuuint32_t(TW), cuuint32_t(TH), cuuint32_t(TN)};
+      cuuint32_t estr[4] = {1, 1, 1, 1};
+      CUresult r = enc(tm, d.out_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, dims, strides, box,
+                       estr, CU_TENSOR_MAP_INTERLEAVE_NONE, oswz, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      CC_REQUIRE(r == CUDA_SUCCESS, "conv_gemm: cuTensorMapEncodeTiled(%s) failed: %d", what, int(r));
+      return CC_OK;
+    };
+    if (int rc = encode(&p.tmO, d.out, d.out_cs, d.out_co, "out")) return rc;
+    if (d.res) if (int rc = encode(&p.tmR, d.res, d.res_cs, d.res_co, "residual")) return rc;
+  }
   {
     auto fast_div = [](uint32_t d, uint32_t fd[2]) {      // q = (umulhi(mul, x) + x) >> shift for x < 2^31
       uint32_t l = 0;
@@ -454,9 +502,9 @@ int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
     fast_div(p.tiles_w * p.tiles_h, p.fd_twh);
   }
 
-  // ---- smem budget -> pipeline depth.  Fixed part: alignment slack, the fp32 staging tile, bias, barriers.
+  // ---- smem budget -> pipeline depth.  Fixed part: alignment slack, one output staging tile per consumer, bias, barriers.
   const int a_bytes = kTileM * p.BK * 2, b_bytes = BN * p.BK * 2;
-  const int fixed = 1024 + kTileM * (BN * 4 + 16) + 16 + d.Cout * 4 + 8 * 20;
+  const int fixed = 1024 + kConsumers * epi_stage_bytes(BN, es) + d.Cout * 4 + 8 * kBarriers;
   const int num_kb = p.num_taps * p.chunks_per_tap;
   const int bres_bytes = b_bytes * num_kb;
   // resident weights (single N block) when they leave room for at least four activation stages: the ring then carries

@@ -20,6 +20,8 @@ enum Act : int32_t { ACT_NONE = 0, ACT_SILU = 1, ACT_GELU_TANH = 2, ACT_SILU_EXA
 struct GemmParams {
   CUtensorMap tmA;  // 5-D view of the NHWC activation (see conv_gemm.cu)
   CUtensorMap tmB;  // 2-D [Cout][Ktot] weights
+  CUtensorMap tmO;  // 4-D output slice [N][H][W][Cout] (epilogue TMA stores)
+  CUtensorMap tmR;  // 4-D residual slice, same boxes (when res != nullptr)
   int32_t tap[9][4];  // per filter tap: delta on dims 0..3 of the A view
   int32_t num_taps, chunks_per_tap, BK, BN;
   int32_t n_blocks;                   // Cout / BN

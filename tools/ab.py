@@ -1,6 +1,6 @@
 """Same-box A/B of environment toggles (boxes differ by +-5 %, so variants must be compared inside ONE gpurun call).
 
-usage:  python tools/ab.py [--conv 6 2 0] [--bench] [--batch 32] -- "CC_X=0" "CC_X=1 CC_Y=2" ...
+usage:  python tools/ab.py [--conv 6 2 0] [--bench] [--batch 32] [--steps 100] -- "CC_X=0" "CC_X=1 CC_Y=2" ...
 Each variant (a space-separated list of VAR=value, or "base") runs tools/one_conv.py on the given shapes and/or
 bench.py --no-cpu in a fresh process; one table is printed at the end."""
 import json
@@ -16,7 +16,7 @@ def main():
     if "--" not in argv:
         sys.exit(__doc__)
     opts, variants = argv[:argv.index("--")], argv[argv.index("--") + 1:]
-    shapes, bench, batch, i = [], False, None, 0
+    shapes, bench, batch, steps, i = [], False, None, None, 0
     while i < len(opts):
         if opts[i] == "--conv":
             i += 1
@@ -29,6 +29,9 @@ def main():
         elif opts[i] == "--batch":
             i += 1
             batch = opts[i]
+        elif opts[i] == "--steps":     # timed steps per bench run (bench.py's default window is short for an A/B)
+            i += 1
+            steps = opts[i]
         i += 1
     rows = []
     for v in variants:
@@ -43,12 +46,13 @@ def main():
                 shape, rest = line.split(":", 1)
                 row[shape.strip()] = rest.split("ms")[0].strip() + " ms"
         if bench:
-            cmd = [sys.executable, os.path.join(ROOT, "bench.py"), "--no-cpu", "--no-clip"] + (["--batch", batch] if batch else [])
+            cmd = [sys.executable, os.path.join(ROOT, "bench.py"), "--no-cpu", "--no-clip"] + (["--batch", batch] if batch else []) + (["--steps", steps] if steps else [])
             out = subprocess.run(cmd, env=env, capture_output=True, text=True).stdout.strip().splitlines()
             try:
                 d = json.loads(out[-1])
                 row["frames/s"], row["ms/step"], row["e2e"], row["frac"] = (round(d["value"], 1), round(d["ms_per_step"], 3),
                                                                              round(d["e2e"]["value"], 1), round(d["roofline"]["frac"], 4))
+                row["conv TFLOP/s"] = round(d["roofline"]["achieved"], 1)
             except Exception as ex:
                 row["bench"] = f"failed: {ex!r}"
         rows.append(row)
