@@ -7,13 +7,17 @@ latest frame of every camera, groups the frames by shape (cameras differ in reso
 per input shape), runs ONE `detect_batch` per group with uploads and result reads queued back to back, waits once, and
 then steps every camera's tracker in one library call.  What comes back per camera is what `run_inference` computes up
 to clearcam.py:589 — the (300,6) detector rows and the tracker's targets; zones, alerts and clip saving (:590-621) are
-the product's control plane and stay with the caller."""
+the product's control plane and stay with the caller.
+
+Each camera has a pixel format (clearcam_b200/pixfmt.py): "bgr24" [H,W,3] frames (the default) or "yuv420p" [H*3/2,W]
+frames, which the detector converts on the GPU.  Groups are keyed by (H, W, dtype, format)."""
 from typing import Dict, Hashable, List, NamedTuple, Optional
 
 import numpy as np
 import torch
 
 from .ocsort_tracker import ocsort
+from .pixfmt import BGR24, check_pix_fmt, yuv420p_size
 from .utils.helpers import batch_bucket
 from .ocsort_tracker.STrack import STrack
 
@@ -25,24 +29,27 @@ class CameraResult(NamedTuple):
 
 
 class _Camera:
-    def __init__(self, thresh, classes, max_age):
-        self.thresh, self.classes = thresh, classes
+    def __init__(self, thresh, classes, max_age, pix_fmt=BGR24):
+        self.thresh, self.classes, self.pix_fmt = thresh, classes, pix_fmt
         self.tracker = ocsort.OCSort(max_age=max_age)          # clearcam.py:239
 
 
 class CameraBatch:
     def __init__(self, model, max_age: int = 100):
-        """model: a clearcam_b200 YOLOv9 (anything with detect_batch(frames[B,H,W,3]) -> (B,300,6))."""
+        """model: a clearcam_b200 YOLOv9 (anything with detect_batch(frames[B,H,W,3]) -> (B,300,6); for yuv420p cameras
+        also detect_batch(frames[B,H*3/2,W], pix_fmt="yuv420p"))."""
         self.model, self.max_age = model, max_age
         self.cams: Dict[Hashable, _Camera] = {}
-        self._stage: Dict[tuple, tuple] = {}                   # (H,W,dtype,bucket) -> (device frame batch, pinned rows)
+        self._stage: Dict[tuple, tuple] = {}                   # (H,W,dtype,pix_fmt,bucket) -> (device frame batch, pinned rows)
         self._pin = torch.cuda.is_available()
         self._seen: Dict[Hashable, int] = {}                   # last frame_num taken from each camera's mailbox
         self._where: Dict[Hashable, tuple] = {}                # camera -> (device batch, row) of its frame in the last detect()
 
     # -- camera set (clearcam.py:207-240 init_cam; settings threshold :584, class filter :586)
-    def add_camera(self, name, thresh: float = 0.5, classes=None):
-        self.cams[name] = _Camera(thresh or 0.5, None if classes is None else {int(c) for c in classes}, self.max_age)
+    def add_camera(self, name, thresh: float = 0.5, classes=None, pix_fmt: str = BGR24):
+        """pix_fmt: the format of this camera's frames, "bgr24" [H,W,3] or "yuv420p" [H*3/2,W] (clearcam_b200/pixfmt.py)."""
+        self.cams[name] = _Camera(thresh or 0.5, None if classes is None else {int(c) for c in classes}, self.max_age,
+                                  check_pix_fmt(pix_fmt))
 
     def remove_camera(self, name):
         self.cams.pop(name, None)
@@ -57,25 +64,39 @@ class CameraBatch:
 
     # -- one pass over every camera that has a new frame
     @staticmethod
-    def group_by_shape(frames: Dict[Hashable, np.ndarray]) -> Dict[tuple, List[Hashable]]:
+    def group_by_shape(frames: Dict[Hashable, np.ndarray], pix_fmts: Optional[Dict[Hashable, str]] = None
+                       ) -> Dict[tuple, List[Hashable]]:
+        """{camera: frame} -> {(H, W, dtype, pix_fmt): cameras}; H, W in pixels.  pix_fmts: each camera's format (missing
+        cameras are bgr24).  A frame that does not match its camera's format raises ValueError."""
         groups: Dict[tuple, List[Hashable]] = {}
         for name, f in frames.items():
             if f is None:
                 continue
+            fmt = (pix_fmts or {}).get(name, BGR24)
             dt = {torch.uint8: "|u1", torch.float32: "<f4"}.get(f.dtype) if isinstance(f, torch.Tensor) else \
                 (f.dtype.str if f.dtype in (np.uint8, np.float32) else None)
-            if f.ndim != 3 or f.shape[2] != 3 or dt is None:
-                raise ValueError(f"camera {name!r}: frame must be HWC BGR uint8 or float32, got {f.dtype} {tuple(f.shape)}")
-            groups.setdefault((int(f.shape[0]), int(f.shape[1]), dt), []).append(name)
+            if fmt == BGR24:
+                if f.ndim != 3 or f.shape[2] != 3 or dt is None:
+                    raise ValueError(f"camera {name!r}: frame must be HWC BGR uint8 or float32, got {f.dtype} {tuple(f.shape)}")
+                H, W = int(f.shape[0]), int(f.shape[1])
+            else:
+                if f.ndim != 2 or dt != "|u1":
+                    raise ValueError(f"camera {name!r}: a yuv420p frame must be uint8 [H*3/2,W], got {f.dtype} {tuple(f.shape)}")
+                try:
+                    H, W = yuv420p_size(f.shape)
+                except ValueError as ex:
+                    raise ValueError(f"camera {name!r}: {ex}") from None
+            groups.setdefault((H, W, dt, fmt), []).append(name)
         return groups
 
     def _buffers(self, key, n):
         k = key + (self.bucket(n),)
         if k not in self._stage:
-            H, W, dt = key
+            H, W, dt, fmt = key
             tdt = torch.uint8 if np.dtype(dt) == np.uint8 else torch.float32
             dev = "cuda" if self._pin else "cpu"
-            self._stage[k] = (torch.zeros((k[-1], H, W, 3), dtype=tdt, device=dev),
+            shape = (H, W, 3) if fmt == BGR24 else (H * 3 // 2, W)
+            self._stage[k] = (torch.zeros((k[-1],) + shape, dtype=tdt, device=dev),
                               torch.empty((k[-1], 300, 6), dtype=torch.float32, pin_memory=self._pin))
         return self._stage[k]
 
@@ -84,13 +105,15 @@ class CameraBatch:
         Each frame goes host -> its row of the device batch directly (asynchronously when it lives in pinned memory, e.g. a
         FrameMailbox slot): no host-side stacking copy."""
         pending = []
-        for key, names in self.group_by_shape(frames).items():
+        fmts = {name: cam.pix_fmt for name, cam in self.cams.items() if cam.pix_fmt != BGR24}
+        for key, names in self.group_by_shape(frames, fmts).items():
             dev, rows = self._buffers(key, len(names))
             for i, name in enumerate(names):
                 f = frames[name]
                 dev[i].copy_(f if isinstance(f, torch.Tensor) else torch.from_numpy(f), non_blocking=True)
                 self._where[name] = (dev, i)
-            out = self.model.detect_batch(dev)
+            # bgr24 groups call detect_batch exactly as before the format existed (stand-in models need not know it)
+            out = self.model.detect_batch(dev) if key[3] == BGR24 else self.model.detect_batch(dev, pix_fmt=key[3])
             rows.copy_(out, non_blocking=True)
             pending.append((names, rows))
         if self._pin:
@@ -98,18 +121,22 @@ class CameraBatch:
         return {name: rows[i].numpy().copy() for names, rows in pending for i, name in enumerate(names)}
 
     def device_frame(self, name) -> torch.Tensor:
-        """The [H,W,3] device copy of the frame camera `name` contributed to the last detect()/step() — what the object
-        crops for CLIP are cut from (ObjectFinder.embed_crops) without a second upload.  Valid until the next step."""
+        """The device copy of the frame camera `name` contributed to the last detect()/step(), in the camera's own format
+        ([H,W,3] bgr24 or [H*3/2,W] yuv420p) — what the object crops for CLIP are cut from
+        (ObjectFinder.embed_crops(..., pix_fmt=...)) without a second upload.  Valid until the next step."""
         dev, i = self._where[name]
         return dev[i]
 
     def step_mailboxes(self, mailboxes: Dict[Hashable, "FrameMailbox"]) -> Dict[Hashable, CameraResult]:
         """`step` on every camera whose mailbox (clearcam_b200.ingest) holds a frame this object has not seen yet —
-        the reference's `if frame_num == last_frame_num: return` per camera (clearcam.py:446)."""
+        the reference's `if frame_num == last_frame_num: return` per camera (clearcam.py:446).  A camera seen here for
+        the first time is added with its mailbox's pixel format."""
         frames = {}
         for name, mb in mailboxes.items():
             got = mb.latest(self._seen.get(name, -1))
             if got is not None:
+                if name not in self.cams:
+                    self.add_camera(name, pix_fmt=getattr(mb, "pix_fmt", BGR24))
                 self._seen[name], frames[name] = got
         return self.step(frames) if frames else {}
 

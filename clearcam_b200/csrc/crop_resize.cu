@@ -3,7 +3,8 @@
 // Replaces, for objects cut out of frames that are already in HBM for the detector: the crop of
 // `VideoCapture.save_object` (clearcam.py:396), the BGR->RGB swap (models/objects.py:249) and `ObjectFinder.preprocess`
 // (models/objects.py:237-242: cv2.resize(INTER_CUBIC) -> /255 -> (x-0.5)/0.5 -> CHW), skipping the reference's JPEG
-// write/read in between.  Bit-exact with OpenCV's own 8-bit bicubic (see oracle/clip_preprocess.py for the arithmetic
+// write/read in between.  I420 frames (ffmpeg yuv420p) are converted to RGB per tap, exactly as
+// cv2.cvtColor(COLOR_YUV2RGB_I420) converts the whole frame, so a crop equals the crop of the converted frame.  Bit-exact with OpenCV's own 8-bit bicubic (see oracle/clip_preprocess.py for the arithmetic
 // and its pinning against cv2): taps in float32 with one rounding per operation (hence the explicit _rn intrinsics —
 // no fused multiply-add), 11-bit fixed-point taps, exact int32 horizontal pass, float32 vertical pass, round-half-even.
 //
@@ -22,7 +23,7 @@ constexpr int kRectsPerLaunch = 64;
 struct CropParams {
   const uint8_t* frames;
   float* out;
-  int H, W, S, bgr, k0;
+  int H, W, S, swap, k0;            // swap: source channel order is BGR (the crop is RGB)
   int rect[kRectsPerLaunch][5];     // frame, x1, y1, x2, y2 (validated on the host)
 };
 
@@ -45,12 +46,15 @@ __device__ __forceinline__ void cubic_taps(int d, int src, int dst, int& s, int 
   taps[3] = __float2int_rn(__fmul_rn(c3, 2048.f));
 }
 
+// I420: the frames are [n, H*3/2, W] planar YUV 4:2:0, converted per tap (to BGR, then swapped like a BGR frame)
+template <bool I420>
 __global__ void __launch_bounds__(256) crop_resize_kernel(const __grid_constant__ CropParams p) {
   const int dx = blockIdx.x * 32 + threadIdx.x, dy = blockIdx.y * 8 + threadIdx.y, k = blockIdx.z;
   if (dx >= p.S || dy >= p.S) return;
   const int fr = p.rect[k][0], x1 = p.rect[k][1], y1 = p.rect[k][2];
   const int cw = p.rect[k][3] - x1, ch = p.rect[k][4] - y1;
-  const uint8_t* img = p.frames + (static_cast<size_t>(fr) * p.H + y1) * p.W * 3 + static_cast<size_t>(x1) * 3;
+  const uint8_t* img = I420 ? p.frames + static_cast<size_t>(fr) * p.H * p.W * 3 / 2
+                            : p.frames + (static_cast<size_t>(fr) * p.H + y1) * p.W * 3 + static_cast<size_t>(x1) * 3;
   int sx, sy, ax[4], ay[4];
   cubic_taps(dx, cw, p.S, sx, ax);
   cubic_taps(dy, ch, p.S, sy, ay);
@@ -63,8 +67,15 @@ __global__ void __launch_bounds__(256) crop_resize_kernel(const __grid_constant_
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int xx = min(max(sx - 1 + j, 0), cw - 1);
+      if constexpr (I420) {
+        int px[3];
+        i420_bgr(img, p.H, p.W, y1 + yy, x1 + xx, px);       // absolute frame coordinates: the chroma of the full frame
 #pragma unroll
-      for (int c = 0; c < 3; ++c) acc[c] += static_cast<int>(__ldg(row + xx * 3 + c)) * ax[j];
+        for (int c = 0; c < 3; ++c) acc[c] += px[c] * ax[j];
+      } else {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) acc[c] += static_cast<int>(__ldg(row + xx * 3 + c)) * ax[j];
+      }
     }
 #pragma unroll
     for (int c = 0; c < 3; ++c) hor[r][c] = acc[c];
@@ -77,7 +88,7 @@ __global__ void __launch_bounds__(256) crop_resize_kernel(const __grid_constant_
   float* out = p.out + static_cast<size_t>(p.k0 + k) * 3 * p.S * p.S + static_cast<size_t>(dy) * p.S + dx;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {                  // c indexes the crop's channel order after the optional BGR->RGB swap
-    const int sc = p.bgr ? 2 - c : c;
+    const int sc = p.swap ? 2 - c : c;
     int v;
     if (dx * 3 + c < tail) {
       float t = __fmul_rn(static_cast<float>(hor[3][sc]), b[3]);
@@ -100,10 +111,13 @@ __global__ void __launch_bounds__(256) crop_resize_kernel(const __grid_constant_
 }  // namespace cc
 
 extern "C" int cc_clip_preprocess(const uint8_t* d_frames, int n_frames, int H, int W, const int32_t* rects, int K, int size,
-                                  int bgr, float* d_out, void* stream) {
+                                  int src_fmt, float* d_out, void* stream) {
   using namespace cc;
   CC_REQUIRE(d_frames && d_out && (rects || K == 0), "cc_clip_preprocess: null pointer");
   CC_REQUIRE(n_frames > 0 && H > 0 && W > 0 && K >= 0 && size >= 1 && size <= 4096, "cc_clip_preprocess: bad sizes");
+  CC_REQUIRE(src_fmt >= 0 && src_fmt <= 2, "cc_clip_preprocess: unknown source format %d (0 = RGB, 1 = BGR, 2 = I420)", src_fmt);
+  CC_REQUIRE(src_fmt != 2 || (H % 2 == 0 && W % 2 == 0), "cc_clip_preprocess: an I420 frame needs an even height and width, got %dx%d",
+             H, W);
   for (int k = 0; k < K; ++k) {
     const int32_t* r = rects + 5 * k;
     CC_REQUIRE(r[0] >= 0 && r[0] < n_frames && r[1] >= 0 && r[2] >= 0 && r[3] > r[1] && r[4] > r[2] && r[3] <= W && r[4] <= H,
@@ -118,12 +132,14 @@ extern "C" int cc_clip_preprocess(const uint8_t* d_frames, int n_frames, int H, 
     p.H = H;
     p.W = W;
     p.S = size;
-    p.bgr = bgr;
+    p.swap = src_fmt != 0;
     p.k0 = k0;
     const int n = K - k0 < kRectsPerLaunch ? K - k0 : kRectsPerLaunch;
     for (int i = 0; i < n; ++i)
       for (int j = 0; j < 5; ++j) p.rect[i][j] = rects[5 * (k0 + i) + j];
-    crop_resize_kernel<<<dim3((size + 31) / 32, (size + 7) / 8, n), dim3(32, 8), 0, st>>>(p);
+    const dim3 grid((size + 31) / 32, (size + 7) / 8, n);
+    if (src_fmt == 2) crop_resize_kernel<true><<<grid, dim3(32, 8), 0, st>>>(p);
+    else crop_resize_kernel<false><<<grid, dim3(32, 8), 0, st>>>(p);
     CC_CHECK_CUDA(cudaGetLastError());
   }
   return CC_OK;

@@ -62,10 +62,23 @@ int upsample2_launch(const TSlice& in, const TSlice& out, cudaStream_t s);
 struct CBFuseParams { TSlice src[5]; int nsrc; TSlice last; TSlice out; int shift[5]; };   // shift: filled by the launcher (log2 of out/src, -1 = general)
 int cbfuse_launch(const CBFuseParams& p, cudaStream_t s);
 
+// One I420 pixel as BGR, bit-exact with cv2.cvtColor(COLOR_YUV2BGR_I420): BT.601 limited range in 20-bit fixed point,
+// the chroma sample of the 2x2 block holding frame pixel (y, x).  Used per tap by the letterbox and the crop kernels.
+// The products stay within int32; >> is arithmetic on the negative sums.
+__device__ __forceinline__ void i420_bgr(const uint8_t* __restrict__ fr, int H, int W, int y, int x, int bgr[3]) {
+  const int hw = H * W, cw = W >> 1, ci = (y >> 1) * cw + (x >> 1);
+  const int Y = __ldg(fr + y * W + x), u = __ldg(fr + hw + ci) - 128, v = __ldg(fr + hw + (hw >> 2) + ci) - 128;
+  const int yy = max(Y - 16, 0) * 1220542 + (1 << 19);
+  bgr[0] = min(max((yy + 2116026 * u) >> 20, 0), 255);
+  bgr[1] = min(max((yy - 852492 * v - 409993 * u) >> 20, 0), 255);
+  bgr[2] = min(max((yy + 1673527 * v) >> 20, 0), 255);
+}
+
 // Letterbox: bilinear resize (utils/helpers.py:127-131 semantics, W axis first then H, result cast to the
-// input dtype after each axis) + zero pad (detection/yolov9.py:390-404).  HWC, 3 channels, u8 or f32.
+// input dtype after each axis) + zero pad (detection/yolov9.py:390-404).  fmt: a CC_FRAME_* code; out is HWC BGR, float32
+// for CC_FRAME_BGR_F32, else uint8 (I420 taps are converted to BGR before the interpolation).
 struct LetterboxParams {
-  const void* in; void* out; int is_f32;
+  const void* in; void* out; int fmt;
   int B, Hin, Win, Hr, Wr, pad_y, pad_x, Hout, Wout;   // resized extent, pads, final extent
   float sx, sy;                                        // float(Win/Wr), float(Hin/Hr) computed in double on the host
 };

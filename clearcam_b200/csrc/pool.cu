@@ -4,6 +4,7 @@
 // sized to cover the tensor once (grid-stride, capped at a multiple of the 148 SMs).
 #include "ops.cuh"
 #include "cc_common.h"
+#include "clearcam_b200.h"
 #include <stdlib.h>
 
 namespace cc {
@@ -456,6 +457,8 @@ __device__ __forceinline__ int lerp_u8(int a, int b, int wi) {
   int diff = ((b - a + 128) & 255) - 128;     // int8 wrap-around of the reference's uint8 subtraction
   return (a + ((diff * wi + 64) >> 7)) & 255;
 }
+// FMT: CC_FRAME_* code of the source, a template argument so the per-pixel path has no format branch
+template <int FMT>
 __global__ void letterbox_kernel(LetterboxParams p) {
   const long long total = static_cast<long long>(p.B) * p.Hout * p.Wout;
   CC_GRID_STRIDE(idx, total) {
@@ -470,7 +473,7 @@ __global__ void letterbox_kernel(LetterboxParams p) {
       if (p.Wr != p.Win) lerp_idx(rx, p.Win, p.sx, xl, xh, wx); else { xl = xh = rx; }
       if (p.Hr != p.Hin) lerp_idx(ry, p.Hin, p.sy, yl, yh, wy); else { yl = yh = ry; }
     }
-    if (p.is_f32) {
+    if constexpr (FMT == CC_FRAME_BGR_F32) {
       const float* src = static_cast<const float*>(p.in) + static_cast<long long>(n) * p.Hin * p.Win * 3;
       float* dst = static_cast<float*>(p.out) + idx * 3;
       for (int c = 0; c < 3; ++c) {
@@ -485,17 +488,32 @@ __global__ void letterbox_kernel(LetterboxParams p) {
         dst[c] = r;
       }
     } else {
-      const uint8_t* src = static_cast<const uint8_t*>(p.in) + static_cast<long long>(n) * p.Hin * p.Win * 3;
       uint8_t* dst = static_cast<uint8_t*>(p.out) + idx * 3;
       const int wxi = static_cast<int>(static_cast<short>(wx * 128.f + 0.5f));
       const int wyi = static_cast<int>(static_cast<short>(wy * 128.f + 0.5f));
+      // the four taps as BGR: a = (yl,xl), b = (yl,xh), d = (yh,xl), e = (yh,xh)
+      int a[3] = {0, 0, 0}, b[3] = {0, 0, 0}, d[3] = {0, 0, 0}, e[3] = {0, 0, 0};
+      if (inside) {
+        if constexpr (FMT == CC_FRAME_I420_U8) {
+          const uint8_t* src = static_cast<const uint8_t*>(p.in) + static_cast<long long>(n) * p.Hin * p.Win * 3 / 2;
+          i420_bgr(src, p.Hin, p.Win, yl, xl, a);
+          i420_bgr(src, p.Hin, p.Win, yl, xh, b);
+          i420_bgr(src, p.Hin, p.Win, yh, xl, d);
+          i420_bgr(src, p.Hin, p.Win, yh, xh, e);
+        } else {
+          const uint8_t* src = static_cast<const uint8_t*>(p.in) + static_cast<long long>(n) * p.Hin * p.Win * 3;
+          for (int c = 0; c < 3; ++c) {
+            a[c] = src[(static_cast<long long>(yl) * p.Win + xl) * 3 + c]; b[c] = src[(static_cast<long long>(yl) * p.Win + xh) * 3 + c];
+            d[c] = src[(static_cast<long long>(yh) * p.Win + xl) * 3 + c]; e[c] = src[(static_cast<long long>(yh) * p.Win + xh) * 3 + c];
+          }
+        }
+      }
+#pragma unroll
       for (int c = 0; c < 3; ++c) {
         int r = 0;
         if (inside) {
-          const int a = src[(static_cast<long long>(yl) * p.Win + xl) * 3 + c], b = src[(static_cast<long long>(yl) * p.Win + xh) * 3 + c];
-          const int d = src[(static_cast<long long>(yh) * p.Win + xl) * 3 + c], e = src[(static_cast<long long>(yh) * p.Win + xh) * 3 + c];
-          const int top = (p.Wr != p.Win) ? lerp_u8(a, b, wxi) : a;
-          const int bot = (p.Wr != p.Win) ? lerp_u8(d, e, wxi) : d;
+          const int top = (p.Wr != p.Win) ? lerp_u8(a[c], b[c], wxi) : a[c];
+          const int bot = (p.Wr != p.Win) ? lerp_u8(d[c], e[c], wxi) : d[c];
           r = (p.Hr != p.Hin) ? lerp_u8(top, bot, wyi) : top;
         }
         dst[c] = static_cast<uint8_t>(r);
@@ -505,7 +523,16 @@ __global__ void letterbox_kernel(LetterboxParams p) {
 }
 int letterbox_launch(const LetterboxParams& p, cudaStream_t s) {
   const long long total = static_cast<long long>(p.B) * p.Hout * p.Wout;
-  letterbox_kernel<<<grid_for(total, 256), 256, 0, s>>>(p);
+  const int g = grid_for(total, 256);
+  switch (p.fmt) {
+    case CC_FRAME_BGR_U8: letterbox_kernel<CC_FRAME_BGR_U8><<<g, 256, 0, s>>>(p); break;
+    case CC_FRAME_BGR_F32: letterbox_kernel<CC_FRAME_BGR_F32><<<g, 256, 0, s>>>(p); break;
+    case CC_FRAME_I420_U8:
+      CC_REQUIRE(p.Hin % 2 == 0 && p.Win % 2 == 0, "letterbox: I420 frame %dx%d has an odd side", p.Hin, p.Win);
+      letterbox_kernel<CC_FRAME_I420_U8><<<g, 256, 0, s>>>(p);
+      break;
+    default: CC_REQUIRE(false, "letterbox: unknown frame format %d", p.fmt);
+  }
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;
 }

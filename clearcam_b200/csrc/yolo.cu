@@ -178,7 +178,7 @@ struct Op {
 };
 
 struct YoloPlan {
-  int B = 0, Hf = 0, Wf = 0, res = 0, is_f32 = 0, H = 0, W = 0, A = 0;
+  int B = 0, Hf = 0, Wf = 0, res = 0, fmt = 0, H = 0, W = 0, A = 0;    // fmt: CC_FRAME_* of the frames
   int Hr = 0, Wr = 0;          // the reference's letterboxed extent (H, W are it rounded up to a multiple of 32)
   std::vector<Op> ops;
   size_t alloc_bytes = 0;      // bytes of the handle's shared workspace this plan addresses
@@ -186,7 +186,7 @@ struct YoloPlan {
   uint64_t last_use = 0;       // LRU stamp
   float* pred = nullptr;   // [B,A,6]
   float* raw = nullptr;    // [B,84,A] (allocated lazily when a tap is requested)
-  void* lb_out = nullptr;  // letterboxed frames (same dtype as input) or nullptr when identity
+  void* lb_out = nullptr;  // letterboxed BGR frames (float32 for float frames, else uint8) or nullptr when identity
   double conv_flops = 0;
   int n_launch = 0;
   std::vector<T> layer_outs;   // per spec layer (parity taps)
@@ -562,14 +562,16 @@ int Builder::build() {
   CC_REQUIRE(P.H > 0 && P.W > 0 && P.H - Hr <= 1 && P.W - Wr <= 1,
              "yolo: letterboxed input %dx%d is not within one pixel of a multiple of 32 (frame %dx%d, res %d)", Hr, Wr, P.Hf, P.Wf, P.res);
   const void* net_in = nullptr;   // filled per run when identity (frames pointer) -> patched in run()
-  if (!(new_w == P.Wf && new_h == P.Hf && px == 0 && py == 0 && P.H == Hr && P.W == Wr)) {
-    const size_t es = P.is_f32 ? 4 : 1;
+  const bool f32 = P.fmt == CC_FRAME_BGR_F32;
+  // the stems read HWC BGR: I420 frames always go through the letterbox, which converts them (an identity resize included)
+  if (P.fmt == CC_FRAME_I420_U8 || !(new_w == P.Wf && new_h == P.Hf && px == 0 && py == 0 && P.H == Hr && P.W == Wr)) {
+    const size_t es = f32 ? 4 : 1;
     P.lb_out = dalloc(static_cast<size_t>(P.B) * P.H * P.W * 3 * es);
     net_in = P.lb_out;
     if (!bump.dry) {
     Op op; op.kind = Op::LETTERBOX; op.name = "letterbox";
     op.lb = LetterboxParams{};
-    op.lb.in = nullptr; op.lb.out = P.lb_out; op.lb.is_f32 = P.is_f32;
+    op.lb.in = nullptr; op.lb.out = P.lb_out; op.lb.fmt = P.fmt;
     op.lb.B = P.B; op.lb.Hin = P.Hf; op.lb.Win = P.Wf; op.lb.Hr = new_h; op.lb.Wr = new_w;
     op.lb.pad_y = py; op.lb.pad_x = px; op.lb.Hout = P.H; op.lb.Wout = P.W;
     op.lb.sx = float(double(P.Wf) / double(new_w)); op.lb.sy = float(double(P.Hf) / double(new_h));
@@ -599,7 +601,7 @@ int Builder::build() {
           out = out_for(i, l.b, in.H / 2, in.W / 2);
           const ConvW& cw = M.convs[pfx];
           static const int stem_tc_env = getenv("CC_STEM_TC") ? atoi(getenv("CC_STEM_TC")) : 1;
-          if (!P.is_f32 && stem_tc_env && cw.cout % 16 == 0 && !M.precise) {
+          if (!f32 && stem_tc_env && cw.cout % 16 == 0 && !M.precise) {
             // uint8 frames: raw pixel values are exact in bf16, weights bf16(w/255).  Default (CC_STEM_TC=1): stem_tc_kernel
             // gathers the A tile from the frame itself; CC_STEM_TC=2: the earlier im2col to [B*Ho*Wo, 32] + conv_gemm
             const long long Mrows = static_cast<long long>(P.B) * (P.H / 2) * (P.W / 2);
@@ -634,7 +636,7 @@ int Builder::build() {
           if (bump.dry) break;
           Op op; op.kind = Op::STEM; op.name = pfx;
           op.stem = StemParams{};
-          op.stem.in = net_in; op.stem.is_f32 = P.is_f32; op.stem.B = P.B; op.stem.H = P.H; op.stem.W = P.W;
+          op.stem.in = net_in; op.stem.is_f32 = f32; op.stem.B = P.B; op.stem.H = P.H; op.stem.W = P.W;
           op.stem.w = cw.wf32; op.stem.bias = cw.bias; op.stem.Cout = cw.cout; op.stem.out = ts(out);
           P.conv_flops += 2.0 * P.B * (P.H / 2) * (P.W / 2) * cw.cout * 27;
           P.ops.push_back(std::move(op));
@@ -870,7 +872,10 @@ static double op_bytes(const Op& op) {
     case Op::SPP3: return 4.0 * op.s_in.N * op.s_in.H * op.s_in.W * op.s_out.C * 2;
     case Op::CBFUSE: { double b = sl(op.cbf.last) + sl(op.cbf.out); for (int k = 0; k < op.cbf.nsrc; ++k) b += sl(op.cbf.src[k]); return b; }
     case Op::STEM_TC: return double(op.stem_tc.B) * op.stem_tc.H * op.stem_tc.W * 3 + double(op.stem_tc.Mrows) * op.stem_tc.Cout * 2;
-    case Op::LETTERBOX: return double(op.lb.B) * (double(op.lb.Hin) * op.lb.Win + double(op.lb.Hout) * op.lb.Wout) * 3 * (op.lb.is_f32 ? 4 : 1);
+    case Op::LETTERBOX: {
+      const double in_px = op.lb.fmt == CC_FRAME_BGR_F32 ? 12.0 : op.lb.fmt == CC_FRAME_I420_U8 ? 1.5 : 3.0;   // bytes per pixel
+      return double(op.lb.B) * (double(op.lb.Hin) * op.lb.Win * in_px + double(op.lb.Hout) * op.lb.Wout * 3 * (op.lb.fmt == CC_FRAME_BGR_F32 ? 4 : 1));
+    }
     case Op::DECODE: return double(op.dec.B) * op.dec.A * ((64 + 80) * 4 + 6 * 4);
     default: return 0.0;
   }
@@ -1005,15 +1010,24 @@ int cc_yolo_destroy(cc_yolo* h) {
 
 static constexpr size_t kMaxPlans = 16;   // cached plans per handle (host metadata only: plans own no device memory)
 
-static std::string plan_key(int is_f32, int B, int Hf, int Wf, int res) {
+// frame_fmt is a CC_FRAME_* code; I420 needs even sides (4:2:0 chroma covers 2x2 blocks)
+static int check_frame_fmt(const char* who, int fmt, int Hf, int Wf) {
+  CC_REQUIRE(fmt == CC_FRAME_BGR_U8 || fmt == CC_FRAME_BGR_F32 || fmt == CC_FRAME_I420_U8,
+             "%s: unknown frame format %d (0 = BGR uint8, 1 = BGR float32, 2 = I420)", who, fmt);
+  CC_REQUIRE(fmt != CC_FRAME_I420_U8 || (Hf % 2 == 0 && Wf % 2 == 0),
+             "%s: an I420 frame needs an even height and width, got %dx%d", who, Hf, Wf);
+  return CC_OK;
+}
+
+static std::string plan_key(int fmt, int B, int Hf, int Wf, int res) {
   char key[96];
-  snprintf(key, sizeof(key), "%d,%d,%d,%d,%d", is_f32, B, Hf, Wf, res);
+  snprintf(key, sizeof(key), "%d,%d,%d,%d,%d", fmt, B, Hf, Wf, res);
   return key;
 }
 // workspace bytes a plan of this shape addresses (measuring pass of the builder: no device work)
-static int plan_bytes(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, size_t* bytes, size_t* scratch = nullptr, size_t* accb = nullptr) {
+static int plan_bytes(cc_yolo* h, int fmt, int B, int Hf, int Wf, int res, size_t* bytes, size_t* scratch = nullptr, size_t* accb = nullptr) {
   YoloPlan tmp;
-  tmp.B = B; tmp.Hf = Hf; tmp.Wf = Wf; tmp.res = res; tmp.is_f32 = is_f32;
+  tmp.B = B; tmp.Hf = Hf; tmp.Wf = Wf; tmp.res = res; tmp.fmt = fmt;
   Builder dry(h->m, tmp);
   dry.bump.dry = true;
   int rc = dry.build();
@@ -1023,9 +1037,9 @@ static int plan_bytes(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, si
   if (accb) *accb = dry.max_acc;
   return CC_OK;
 }
-static int get_plan(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, YoloPlan** out) {
+static int get_plan(cc_yolo* h, int fmt, int B, int Hf, int Wf, int res, YoloPlan** out) {
   YoloModel& M = h->m;
-  const std::string key = plan_key(is_f32, B, Hf, Wf, res);
+  const std::string key = plan_key(fmt, B, Hf, Wf, res);
   auto it = M.plans.find(key);
   if (it != M.plans.end() && it->second->gen == M.arena.gen) {
     it->second->last_use = ++M.tick;
@@ -1033,14 +1047,14 @@ static int get_plan(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, Yolo
     return CC_OK;
   }
   size_t bytes = 0, scratch = 0, accb = 0;
-  int rc = plan_bytes(h, is_f32, B, Hf, Wf, res, &bytes, &scratch, &accb);
+  int rc = plan_bytes(h, fmt, B, Hf, Wf, res, &bytes, &scratch, &accb);
   if (rc) return rc;
   if ((rc = M.arena.reserve(bytes))) return rc;
   // plans built against an older workspace are stale (they are rebuilt on their next use)
   for (auto p = M.plans.begin(); p != M.plans.end();)
     p = (p->second->gen != M.arena.gen) ? M.plans.erase(p) : std::next(p);
   std::unique_ptr<YoloPlan> P(new YoloPlan());
-  P->B = B; P->Hf = Hf; P->Wf = Wf; P->res = res; P->is_f32 = is_f32;
+  P->B = B; P->Hf = Hf; P->Wf = Wf; P->res = res; P->fmt = fmt;
   Builder bld(M, *P);
   bld.bump.base = static_cast<uint8_t*>(M.arena.base);
   bld.scratch_bytes = scratch;
@@ -1060,9 +1074,10 @@ static int get_plan(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, Yolo
   return CC_OK;
 }
 
-int cc_yolo_workspace_bytes(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, size_t* bytes) {
+int cc_yolo_workspace_bytes(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, size_t* bytes) {
   CC_REQUIRE(h && bytes && B > 0 && Hf > 0 && Wf > 0 && res > 0, "cc_yolo_workspace_bytes: bad argument");
-  return plan_bytes(h, is_f32, B, Hf, Wf, res, bytes);
+  if (int rc = check_frame_fmt("cc_yolo_workspace_bytes", frame_fmt, Hf, Wf)) return rc;
+  return plan_bytes(h, frame_fmt, B, Hf, Wf, res, bytes);
 }
 
 int cc_yolo_set_workspace(cc_yolo* h, void* d_workspace, size_t bytes) {
@@ -1073,11 +1088,12 @@ int cc_yolo_set_workspace(cc_yolo* h, void* d_workspace, size_t bytes) {
   return h->m.arena.adopt(d_workspace, bytes);
 }
 
-int cc_yolo_forward(cc_yolo* h, const void* d_frames, int is_f32, int B, int Hf, int Wf, int res, float* d_out,
+int cc_yolo_forward(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, float* d_out,
                     float* d_raw, void* stream) {
   CC_REQUIRE(h && d_frames && d_out && B > 0 && Hf > 0 && Wf > 0 && res > 0, "cc_yolo_forward: bad argument");
+  if (int rc = check_frame_fmt("cc_yolo_forward", frame_fmt, Hf, Wf)) return rc;
   YoloPlan* P = nullptr;
-  int rc = get_plan(h, is_f32, B, Hf, Wf, res, &P);
+  int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P);
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   static const int graph_env = getenv("CC_GRAPH") ? atoi(getenv("CC_GRAPH")) : 1;
@@ -1112,11 +1128,12 @@ int cc_yolo_forward(cc_yolo* h, const void* d_frames, int is_f32, int B, int Hf,
   return plan_run(*P, d_frames, d_out, d_raw, st);
 }
 
-int cc_yolo_plan_info(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, int* net_h, int* net_w, int* anchors,
+int cc_yolo_plan_info(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int* net_h, int* net_w, int* anchors,
                       int* launches, double* conv_flops, double* act_bytes) {
   CC_REQUIRE(h, "cc_yolo_plan_info: null handle");
   YoloPlan* P = nullptr;
-  int rc = get_plan(h, is_f32, B, Hf, Wf, res, &P);
+  if (int rc = check_frame_fmt("cc_yolo_plan_info", frame_fmt, Hf, Wf)) return rc;
+  int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P);
   if (rc) return rc;
   if (net_h) *net_h = P->H;
   if (net_w) *net_w = P->W;
@@ -1130,11 +1147,12 @@ int cc_yolo_plan_info(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, in
 /* Per-op device timing of one forward (CUDA events between launches on `stream`; synchronises at the end).
  * Fills up to `cap` entries: ms[i], flops[i] (algorithmic, 0 for non-conv ops) and a name pointer valid for the
  * life of the handle.  Returns the op count through n_ops. */
-int cc_yolo_profile(cc_yolo* h, const void* d_frames, int is_f32, int B, int Hf, int Wf, int res, float* d_out, int cap,
+int cc_yolo_profile(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, float* d_out, int cap,
                     float* ms, double* flops, double* bytes, const char** kinds, const char** names, int* n_ops, void* stream) {
   CC_REQUIRE(h && d_frames && d_out, "cc_yolo_profile: bad argument");
   YoloPlan* P = nullptr;
-  int rc = get_plan(h, is_f32, B, Hf, Wf, res, &P);
+  if (int rc = check_frame_fmt("cc_yolo_profile", frame_fmt, Hf, Wf)) return rc;
+  int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P);
   if (rc) return rc;
   const size_t n = P->ops.size();
   std::vector<cudaEvent_t> ev(n + 1);
@@ -1162,11 +1180,12 @@ int cc_yolo_profile(cc_yolo* h, const void* d_frames, int is_f32, int B, int Hf,
  * as in production): for every conv_gemm op, globaltimer ns of (first CTA entered, grid dependency released, last CTA
  * exited, then five stamps of CTA 0: first operands landed, all MMAs issued, first accumulator complete, last epilogue group
  * done, exit); zeros for the other ops.  host_ns: [12 * cap].  Synchronises at the end. */
-int cc_yolo_trace(cc_yolo* h, const void* d_frames, int is_f32, int B, int Hf, int Wf, int res, float* d_out, int cap,
+int cc_yolo_trace(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, float* d_out, int cap,
                   unsigned long long* host_ns, const char** kinds, const char** names, double* flops, int* n_ops, void* stream) {
   CC_REQUIRE(h && d_frames && d_out && host_ns, "cc_yolo_trace: bad argument");
   YoloPlan* P = nullptr;
-  int rc = get_plan(h, is_f32, B, Hf, Wf, res, &P);
+  if (int rc = check_frame_fmt("cc_yolo_trace", frame_fmt, Hf, Wf)) return rc;
+  int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P);
   if (rc) return rc;
   const size_t n = P->ops.size();
   unsigned long long* d_trace = nullptr;
@@ -1203,11 +1222,12 @@ __global__ void tap_kernel(const __nv_bfloat16* src, int f32, int cs, int co, in
   }
 }
 
-int cc_yolo_layer_output(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, int layer, float* d_dst, int* C,
+int cc_yolo_layer_output(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int layer, float* d_dst, int* C,
                          int* H, int* W, void* stream) {
   CC_REQUIRE(h, "cc_yolo_layer_output: null handle");
   YoloPlan* P = nullptr;
-  int rc = get_plan(h, is_f32, B, Hf, Wf, res, &P);
+  if (int rc = check_frame_fmt("cc_yolo_layer_output", frame_fmt, Hf, Wf)) return rc;
+  int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P);
   if (rc) return rc;
   CC_REQUIRE(layer >= 0 && layer < static_cast<int>(P->layer_outs.size()), "cc_yolo_layer_output: bad layer %d", layer);
   const T& t = P->layer_outs[layer];
@@ -1248,8 +1268,9 @@ int cc_detect_decode(const float* const* d_box, const float* const* d_cls, const
   return decode_launch(p, static_cast<cudaStream_t>(stream));
 }
 
-int cc_letterbox(const void* d_in, int is_f32, int B, int Hin, int Win, int res, void* d_out, int* out_h, int* out_w,
+int cc_letterbox(const void* d_in, int frame_fmt, int B, int Hin, int Win, int res, void* d_out, int* out_h, int* out_w,
                  void* stream) {
+  if (int rc = check_frame_fmt("cc_letterbox", frame_fmt, Hin, Win)) return rc;
   const double r = std::min(double(res) / Hin, double(res) / Win);
   const int new_w = int(std::nearbyint(Win * r)), new_h = int(std::nearbyint(Hin * r));
   double dw = double(((res - new_w) % 32 + 32) % 32) / 2, dh = double(((res - new_h) % 32 + 32) % 32) / 2;
@@ -1258,7 +1279,7 @@ int cc_letterbox(const void* d_in, int is_f32, int B, int Hin, int Win, int res,
   if (out_w) *out_w = new_w + 2 * px;
   if (!d_out) return CC_OK;   // size query
   LetterboxParams p{};
-  p.in = d_in; p.out = d_out; p.is_f32 = is_f32; p.B = B; p.Hin = Hin; p.Win = Win; p.Hr = new_h; p.Wr = new_w;
+  p.in = d_in; p.out = d_out; p.fmt = frame_fmt; p.B = B; p.Hin = Hin; p.Win = Win; p.Hr = new_h; p.Wr = new_w;
   p.pad_y = py; p.pad_x = px; p.Hout = new_h + 2 * py; p.Wout = new_w + 2 * px;
   p.sx = float(double(Win) / double(new_w)); p.sy = float(double(Hin) / double(new_h));
   return letterbox_launch(p, static_cast<cudaStream_t>(stream));

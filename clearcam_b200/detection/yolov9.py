@@ -10,7 +10,9 @@ kernels) through ctypes; torch tensors are only device containers.  There is no 
 library or without an H100 every call raises CCError.
 
 Differences the reference cannot express (additions): `detect_batch(frames[B,H,W,3])`, explicit `weights=`
-(the reference downloads from HuggingFace at construction, :372; there is no network here).
+(the reference downloads from HuggingFace at construction, :372; there is no network here), and `pix_fmt="yuv420p"`:
+frames as a camera decodes them, uint8 [H*3/2,W] (a batch [B,H*3/2,W]), converted to BGR on the GPU bit-exactly as
+cv2.cvtColor(COLOR_YUV2BGR_I420) would (clearcam_b200/pixfmt.py).
 """
 from __future__ import annotations
 
@@ -23,6 +25,7 @@ import torch
 
 from . import padding
 from .._lib import CCError, check, lib, ptr, stream_ptr
+from ..pixfmt import BGR24, CC_FRAME_BGR_F32, CC_FRAME_BGR_U8, CC_FRAME_I420_U8, check_pix_fmt, yuv420p_size
 
 
 # ----------------------------------------------------------------------------------------------- helpers
@@ -50,6 +53,30 @@ def _to_host_fp32(v) -> np.ndarray:
     if hasattr(v, "numpy") and not isinstance(v, np.ndarray):
         v = v.numpy()
     return np.ascontiguousarray(np.asarray(v, dtype=np.float32))
+
+
+def _as_tensor(v) -> torch.Tensor:
+    """numpy / torch / tinygrad-like -> torch tensor, dtype and device unchanged."""
+    if isinstance(v, DeviceResult):
+        v = v.tensor
+    if not isinstance(v, torch.Tensor):
+        if hasattr(v, "numpy") and not isinstance(v, np.ndarray):
+            v = v.numpy()
+        v = torch.from_numpy(np.ascontiguousarray(v))
+    return v
+
+
+def _yuv_geometry(t: torch.Tensor):
+    """A yuv420p batch [B,H*3/2,W] uint8 -> (B, H, W); ValueError for anything else."""
+    if t.dtype != torch.uint8 or t.dim() != 3:
+        raise ValueError(f"yuv420p frames must be uint8 [B,H*3/2,W], got {t.dtype} {tuple(t.shape)}")
+    return (int(t.shape[0]),) + yuv420p_size(t.shape)
+
+
+def _frame_code(t: torch.Tensor, pix_fmt: str) -> int:
+    if check_pix_fmt(pix_fmt) == BGR24:
+        return CC_FRAME_BGR_F32 if t.dtype == torch.float32 else CC_FRAME_BGR_U8
+    return CC_FRAME_I420_U8
 
 
 def safe_load(path) -> Dict[str, torch.Tensor]:
@@ -186,23 +213,34 @@ class YOLOv9:
             t = t.to(torch.float32)
         return t.to("cuda", non_blocking=True).contiguous()
 
-    def detect_batch(self, frames, raw: bool = False, stream=None):
-        """frames: [B,H,W,3] BGR uint8|float32 (host or device). Returns device tensor (B,300,6)
-        (and the (B,84,A) head tap when raw=True)."""
-        t = self._as_device_frames(frames)
-        assert t.dim() == 4 and t.shape[-1] == 3, "frames must be [B,H,W,3]"
-        B, Hf, Wf, _ = t.shape
+    def _device_batch(self, frames, pix_fmt: str):
+        """-> (device tensor, frame_fmt code, B, Hf, Wf) of a batch in `pix_fmt`, validated before any library call."""
+        if check_pix_fmt(pix_fmt) == BGR24:
+            t = self._as_device_frames(frames)
+            assert t.dim() == 4 and t.shape[-1] == 3, "frames must be [B,H,W,3]"
+            B, Hf, Wf, _ = t.shape
+        else:
+            t = _as_tensor(frames)
+            B, Hf, Wf = _yuv_geometry(t)
+            t = t.to("cuda", non_blocking=True).contiguous()
+        return t, _frame_code(t, pix_fmt), B, Hf, Wf
+
+    def detect_batch(self, frames, raw: bool = False, stream=None, pix_fmt: str = BGR24):
+        """frames: [B,H,W,3] BGR uint8|float32 (pix_fmt="bgr24"), or [B,H*3/2,W] uint8 (pix_fmt="yuv420p"; H, W even);
+        host or device.  Returns device tensor (B,300,6) in frame pixels (and the (B,84,A) head tap when raw=True)."""
+        t, code, B, Hf, Wf = self._device_batch(frames, pix_fmt)
         out = torch.empty(B, 300, 6, device="cuda", dtype=torch.float32)
         rawt = None
         if raw:
-            A = self.plan_info(B, Hf, Wf, is_f32=t.dtype == torch.float32)["anchors"]
+            A = self.plan_info(B, Hf, Wf, is_f32=code == CC_FRAME_BGR_F32, pix_fmt=pix_fmt)["anchors"]
             rawt = torch.empty(B, 84, A, device="cuda", dtype=torch.float32)
-        check(lib().cc_yolo_forward(self._h, ptr(t), 1 if t.dtype == torch.float32 else 0, B, Hf, Wf, self.res, ptr(out),
-                                    ptr(rawt), stream_ptr(stream)), "cc_yolo_forward")
+        check(lib().cc_yolo_forward(self._h, ptr(t), code, B, Hf, Wf, self.res, ptr(out), ptr(rawt), stream_ptr(stream)),
+              "cc_yolo_forward")
         return (out, rawt) if raw else out
 
-    def detect_pipelined(self, host_batches, depth: int = 2):
-        """Throughput API for host-resident frames: iterates over pinned host batches [B,H,W,3] and yields one
+    def detect_pipelined(self, host_batches, depth: int = 2, pix_fmt: str = BGR24):
+        """Throughput API for host-resident frames: iterates over pinned host batches ([B,H,W,3] bgr24 or [B,H*3/2,W]
+        yuv420p, as `pix_fmt` says) and yields one
         pinned host result (B,300,6) per batch.  The H2D copy of batch i+1 and the D2H read of result i-1 run on a side
         stream while batch i computes (double-buffered device frames / results), so PCIe time hides behind the kernels."""
         main = torch.cuda.current_stream()
@@ -229,7 +267,7 @@ class YOLOv9:
             nxt = next(it, None)
             staged = stage(nxt) if nxt is not None else None          # H2D of the next batch overlaps this compute
             main.wait_event(ev)
-            out = self.detect_batch(dev)
+            out = self.detect_batch(dev, pix_fmt=pix_fmt)
             done = torch.cuda.Event()
             done.record(main)
             dev.record_stream(main)
@@ -249,51 +287,55 @@ class YOLOv9:
             f.synchronize()
             yield h
 
-    def __call__(self, frame):
-        """frame: HWC BGR image (uint8 or float32; numpy / torch / anything with .numpy()).  -> (300,6)
+    def __call__(self, frame, pix_fmt: str = BGR24):
+        """frame: HWC BGR image (uint8 or float32; numpy / torch / anything with .numpy()), or with pix_fmt="yuv420p" a
+        uint8 [H*3/2,W] planar frame.  -> (300,6)
         The single-frame call of the reference's camera loop (clearcam.py:580-583).  A host frame is copied into a device
-        buffer this object keeps per frame shape and the result is produced in a kept buffer too, so the library sees the same
-        pointers call after call and replays its captured CUDA graph of the plan instead of re-launching ~140 kernels."""
+        buffer this object keeps per frame shape and format, and the result is produced in a kept buffer too, so the library
+        sees the same pointers call after call and replays its captured CUDA graph of the plan instead of re-launching ~140
+        kernels."""
+        single_dim = 3 if check_pix_fmt(pix_fmt) == BGR24 else 2
         t = frame
         if isinstance(t, DeviceResult):
             t = t.tensor
         if isinstance(t, torch.Tensor) and t.is_cuda:
-            t = self._as_device_frames(t)
-            if t.dim() == 3:
+            if pix_fmt == BGR24:
+                t = self._as_device_frames(t)
+            if t.dim() == single_dim:
                 t = t.unsqueeze(0)
-            return DeviceResult(self.detect_batch(t)[0])
-        if not isinstance(t, torch.Tensor):
-            if hasattr(t, "numpy") and not isinstance(t, np.ndarray):
-                t = t.numpy()
-            t = torch.from_numpy(np.ascontiguousarray(t))
-        if t.dtype not in (torch.uint8, torch.float32):
+            return DeviceResult(self.detect_batch(t, pix_fmt=pix_fmt)[0])
+        t = _as_tensor(t)
+        if pix_fmt == BGR24 and t.dtype not in (torch.uint8, torch.float32):
             t = t.to(torch.float32)
-        if t.dim() == 3:
+        if t.dim() == single_dim:
             t = t.unsqueeze(0)
-        key = (tuple(t.shape), t.dtype)
+        if pix_fmt != BGR24:
+            _yuv_geometry(t)
+        key = (tuple(t.shape), t.dtype, pix_fmt)
         bufs = getattr(self, "_single", None)
         if bufs is None or bufs[0] != key:
             bufs = self._single = (key, torch.empty(t.shape, dtype=t.dtype, device="cuda"),
                                    torch.empty(t.shape[0], 300, 6, device="cuda", dtype=torch.float32))
         _, dev, out = bufs
         dev.copy_(t, non_blocking=True)
-        B, Hf, Wf, _c = dev.shape
-        check(lib().cc_yolo_forward(self._h, ptr(dev), 1 if dev.dtype == torch.float32 else 0, B, Hf, Wf, self.res, ptr(out),
-                                    None, stream_ptr()), "cc_yolo_forward")
+        B, Hf, Wf = _yuv_geometry(dev) if pix_fmt != BGR24 else dev.shape[:3]
+        check(lib().cc_yolo_forward(self._h, ptr(dev), _frame_code(dev, pix_fmt), B, Hf, Wf, self.res, ptr(out), None,
+                                    stream_ptr()), "cc_yolo_forward")
         return DeviceResult(out[0].clone())
 
-    def plan_info(self, B, Hf, Wf, is_f32=False) -> dict:
+    def plan_info(self, B, Hf, Wf, is_f32=False, pix_fmt: str = BGR24) -> dict:
+        """Facts of the plan for B frames of Hf x Wf pixels (is_f32: float32 bgr24 frames)."""
+        code = (CC_FRAME_BGR_F32 if is_f32 else CC_FRAME_BGR_U8) if check_pix_fmt(pix_fmt) == BGR24 else CC_FRAME_I420_U8
         i = [ctypes.c_int() for _ in range(4)]
         d = [ctypes.c_double() for _ in range(2)]
-        check(lib().cc_yolo_plan_info(self._h, 1 if is_f32 else 0, B, Hf, Wf, self.res, *[ctypes.byref(x) for x in i],
+        check(lib().cc_yolo_plan_info(self._h, code, B, Hf, Wf, self.res, *[ctypes.byref(x) for x in i],
                                       *[ctypes.byref(x) for x in d]), "cc_yolo_plan_info")
         return {"net_h": i[0].value, "net_w": i[1].value, "anchors": i[2].value, "launches": i[3].value,
                 "conv_flops": d[0].value, "act_bytes": d[1].value}
 
-    def profile(self, frames):
+    def profile(self, frames, pix_fmt: str = BGR24):
         """Per-op device times of one forward: list of dicts {kind, name, ms, flops}."""
-        t = self._as_device_frames(frames)
-        B, Hf, Wf, _ = t.shape
+        t, code, B, Hf, Wf = self._device_batch(frames, pix_fmt)
         out = torch.empty(B, 300, 6, device="cuda", dtype=torch.float32)
         cap = 1024
         ms = (ctypes.c_float * cap)()
@@ -302,7 +344,7 @@ class YOLOv9:
         kinds = (ctypes.c_char_p * cap)()
         names = (ctypes.c_char_p * cap)()
         n = ctypes.c_int()
-        check(lib().cc_yolo_profile(self._h, ptr(t), 1 if t.dtype == torch.float32 else 0, B, Hf, Wf, self.res, ptr(out), cap,
+        check(lib().cc_yolo_profile(self._h, ptr(t), code, B, Hf, Wf, self.res, ptr(out), cap,
                                     ms, fl, by, kinds, names, ctypes.byref(n), stream_ptr()), "cc_yolo_profile")
         return [{"kind": kinds[i].decode(), "name": names[i].decode(), "ms": ms[i], "flops": fl[i], "bytes": by[i]}
                 for i in range(n.value)]
@@ -352,18 +394,27 @@ class YOLOv9:
         return out.permute(0, 3, 1, 2)
 
     # -- host-side helpers kept for API parity
-    def preprocess(self, image, new_shape=None):
-        """YOLOv9.preprocess (:390-404) on device; returns DeviceResult HWC (same dtype)."""
-        t = self._as_device_frames(image)
-        squeeze = t.dim() == 3
-        if squeeze:
-            t = t.unsqueeze(0)
-        B, Hf, Wf, _ = t.shape
+    def preprocess(self, image, new_shape=None, pix_fmt: str = BGR24):
+        """YOLOv9.preprocess (:390-404) on device; returns DeviceResult HWC BGR (same dtype; uint8 for yuv420p frames,
+        [H*3/2,W] or [B,H*3/2,W])."""
+        if check_pix_fmt(pix_fmt) == BGR24:
+            t = self._as_device_frames(image)
+            squeeze = t.dim() == 3
+            if squeeze:
+                t = t.unsqueeze(0)
+            B, Hf, Wf, _ = t.shape
+        else:
+            t = _as_tensor(image)
+            squeeze = t.dim() == 2
+            if squeeze:
+                t = t.unsqueeze(0)
+            B, Hf, Wf = _yuv_geometry(t)
+            t = t.to("cuda", non_blocking=True).contiguous()
         res = self.res if new_shape is None else int(new_shape)
         oh, ow = ctypes.c_int(), ctypes.c_int()
-        f32 = 1 if t.dtype == torch.float32 else 0
-        check(lib().cc_letterbox(None, f32, B, Hf, Wf, res, None, ctypes.byref(oh), ctypes.byref(ow), None), "cc_letterbox")
+        code = _frame_code(t, pix_fmt)
+        check(lib().cc_letterbox(None, code, B, Hf, Wf, res, None, ctypes.byref(oh), ctypes.byref(ow), None), "cc_letterbox")
         out = torch.empty(B, oh.value, ow.value, 3, device="cuda", dtype=t.dtype)
-        check(lib().cc_letterbox(ptr(t), f32, B, Hf, Wf, res, ptr(out), ctypes.byref(oh), ctypes.byref(ow), stream_ptr()),
+        check(lib().cc_letterbox(ptr(t), code, B, Hf, Wf, res, ptr(out), ctypes.byref(oh), ctypes.byref(ow), stream_ptr()),
               "cc_letterbox")
         return DeviceResult(out[0] if squeeze else out)

@@ -1,4 +1,4 @@
-"""Frame ingest for the batched detector (SURVEY.md §8f N4): raw bgr24 frames from a pipe into pinned host memory.
+"""Frame ingest for the batched detector (SURVEY.md §8f N4): raw frames from a pipe into pinned host memory.
 
 The reference reads `width*height*3` bytes per frame from an ffmpeg `-f rawvideo -pix_fmt bgr24` pipe into a fresh
 bytes object, wraps it in numpy, and the consumer copies it again before use (`frame_loop`, clearcam.py:401-421;
@@ -10,6 +10,10 @@ bytes object, wraps it in numpy, and the consumer copies it again before use (`f
                      after more than five in a row (clearcam.py:407-412)
   * `CameraBatch.step_mailboxes` (cameras.py) takes every camera's unseen frame straight from its mailbox
 
+Frames are bgr24 (`-pix_fmt bgr24`, H*W*3 bytes) or, with `FrameMailbox(h, w, pix_fmt="yuv420p")`, yuv420p
+(`-pix_fmt yuv420p`, H*W*3/2 bytes: half the pipe, pinned-memory and PCIe bytes, and no swscale conversion on the host;
+the GPU converts them, see clearcam_b200/pixfmt.py).
+
 Spawning ffmpeg (and HLS recording, clearcam.py:310-371) stays with the caller: `PipeReader` takes any callable that
 returns a readable binary stream, e.g. `lambda: subprocess.Popen(cmd, stdout=subprocess.PIPE).stdout`."""
 import threading
@@ -18,13 +22,18 @@ from typing import Callable, Optional, Tuple
 
 import torch
 
+from .pixfmt import BGR24, check_pix_fmt, yuv420p_rows
+
 
 class FrameMailbox:
-    def __init__(self, height: int, width: int, pin: Optional[bool] = None):
-        self.height, self.width = int(height), int(width)
-        self.frame_bytes = self.height * self.width * 3                      # clearcam.py:403
+    def __init__(self, height: int, width: int, pin: Optional[bool] = None, pix_fmt: str = BGR24):
+        """height, width: the picture size in pixels; pix_fmt: "bgr24" (slots [H,W,3]) or "yuv420p" (slots [H*3/2,W],
+        H and W even)."""
+        self.height, self.width, self.pix_fmt = int(height), int(width), check_pix_fmt(pix_fmt)
+        shape = (self.height, self.width, 3) if pix_fmt == BGR24 else (yuv420p_rows(self.height, self.width), self.width)
+        self.frame_bytes = shape[0] * shape[1] * (shape[2] if len(shape) == 3 else 1)        # clearcam.py:403 for bgr24
         pin = torch.cuda.is_available() if pin is None else pin
-        self._slots = torch.empty((3, self.height, self.width, 3), dtype=torch.uint8, pin_memory=pin)
+        self._slots = torch.empty((3,) + shape, dtype=torch.uint8, pin_memory=pin)
         self._views = [memoryview(self._slots[i].numpy()).cast("B") for i in range(3)]
         self._lock = threading.Lock()
         self._latest = -1          # slot of the newest complete frame
@@ -48,7 +57,7 @@ class FrameMailbox:
         return True
 
     def latest(self, last_seen: int = -1) -> Optional[Tuple[int, torch.Tensor]]:
-        """(frame_num, pinned uint8 [H,W,3] BGR view) of the newest frame, or None when there is none newer than `last_seen`
+        """(frame_num, pinned uint8 view: [H,W,3] bgr24 or [H*3/2,W] yuv420p) of the newest frame, or None when there is none newer than `last_seen`
         (clearcam.py:446 `if frame_num == last_frame_num: return`).  The view stays intact until `latest` is called again."""
         with self._lock:
             if self._latest < 0 or self.frame_num == last_seen:

@@ -26,6 +26,7 @@ import torch
 
 from .._lib import CCError, check, lib, ptr, stream_ptr
 from ..detection.yolov9 import DeviceResult, _to_host_fp32, fetch, safe_load
+from ..pixfmt import BGR24, check_pix_fmt, yuv420p_size
 from ..utils.clip_tokenizer import SimpleTokenizer
 from ..utils.helpers import batch_bucket
 
@@ -241,17 +242,28 @@ class ObjectFinder:
             return None
         return nx1, ny1, nx2, ny2
 
-    def preprocess_device(self, frames, rects, bgr: bool = True, size: Optional[int] = None, rows: Optional[int] = None):
+    def preprocess_device(self, frames, rects, bgr: bool = True, size: Optional[int] = None, rows: Optional[int] = None,
+                          pix_fmt: str = BGR24):
         """frames: uint8 [n,H,W,3] or [H,W,3] (host or device; BGR as the cameras deliver them), rects: K rows of
         (frame, x1, y1, x2, y2) or (x1, y1, x2, y2) -> DeviceResult (K,3,S,S) float32, bit-identical to
-        `preprocess(cv2.cvtColor(frame[y1:y2, x1:x2], BGR2RGB))` with OpenCV's own bicubic — without leaving the GPU."""
+        `preprocess(cv2.cvtColor(frame[y1:y2, x1:x2], BGR2RGB))` with OpenCV's own bicubic — without leaving the GPU.
+        pix_fmt="yuv420p": frames are uint8 [n,H*3/2,W] or [H*3/2,W] (H, W even; rects in pixels), and the result is
+        bit-identical to the same crop of `cv2.cvtColor(frame, COLOR_YUV2RGB_I420)` (`bgr` does not apply)."""
         t = frames.tensor if isinstance(frames, DeviceResult) else frames
         if not isinstance(t, torch.Tensor):
             t = torch.from_numpy(np.ascontiguousarray(t))
-        if t.dim() == 3:
-            t = t.unsqueeze(0)
-        if t.dtype != torch.uint8 or t.dim() != 4 or t.shape[-1] != 3:
-            raise ValueError("frames must be uint8 [n,H,W,3]")
+        if check_pix_fmt(pix_fmt) == BGR24:
+            if t.dim() == 3:
+                t = t.unsqueeze(0)
+            if t.dtype != torch.uint8 or t.dim() != 4 or t.shape[-1] != 3:
+                raise ValueError("frames must be uint8 [n,H,W,3]")
+            H, W, src_fmt = t.shape[1], t.shape[2], 1 if bgr else 0
+        else:
+            if t.dim() == 2:
+                t = t.unsqueeze(0)
+            if t.dtype != torch.uint8 or t.dim() != 3:
+                raise ValueError(f"yuv420p frames must be uint8 [n,H*3/2,W], got {t.dtype} {tuple(t.shape)}")
+            (H, W), src_fmt = yuv420p_size(t.shape), 2
         t = t.to("cuda", non_blocking=True).contiguous()
         r = np.asarray(rects, np.int32).reshape(-1, np.shape(rects)[-1] if len(rects) else 5)
         if r.shape[1] == 4:
@@ -261,19 +273,20 @@ class ObjectFinder:
         # rows > K: the result is allocated with `rows` images, the first K filled and the rest zero (batch padding)
         out = torch.empty(len(r), 3, s, s, device="cuda", dtype=torch.float32) if not rows or rows <= len(r) else \
             torch.zeros(rows, 3, s, s, device="cuda", dtype=torch.float32)
-        check(lib().cc_clip_preprocess(ptr(t), t.shape[0], t.shape[1], t.shape[2], r.ctypes.data, len(r), s, int(bgr), ptr(out),
-                                       stream_ptr(None)), "cc_clip_preprocess")
+        check(lib().cc_clip_preprocess(ptr(t), t.shape[0], H, W, r.ctypes.data, len(r), s, src_fmt, ptr(out), stream_ptr(None)),
+              "cc_clip_preprocess")
         return DeviceResult(out)
 
-    def embed_crops(self, frames, rects, bgr: bool = True):
+    def embed_crops(self, frames, rects, bgr: bool = True, pix_fmt: str = BGR24):
         """Detector frame -> embeddings of its objects in one device pass: crop + preprocess + `precompute_embedding`
-        (the reference goes through cv2.imwrite / cv2.imread and the host, clearcam.py:398, 274-276)."""
+        (the reference goes through cv2.imwrite / cv2.imread and the host, clearcam.py:398, 274-276).  `pix_fmt` as in
+        `preprocess_device` (CameraBatch.device_frame returns a camera's frame in its own format)."""
         k = len(rects)
         if k == 0:
             return DeviceResult(torch.empty(0, self.model.embed_dim, device="cuda", dtype=torch.float32))
         # the number of objects differs from frame to frame: pad the batch to a bucket size so the encoder keeps a small,
         # bounded set of plans; the padded rows are dropped
-        x = self.preprocess_device(frames, rects, bgr, rows=batch_bucket(k))
+        x = self.preprocess_device(frames, rects, bgr, rows=batch_bucket(k), pix_fmt=pix_fmt)
         return DeviceResult(self.model.precompute_embedding(x).tensor[:k])
 
     def _device_index(self):

@@ -68,17 +68,28 @@ int cc_yolo_create_ex(const char* size, int flags, int n_tensors, const char* co
                       const int64_t* numels, cc_yolo** out);
 int cc_yolo_destroy(cc_yolo* h);
 
+/* Frame formats (the frame_fmt argument of the detector entry points and cc_letterbox):
+ *   CC_FRAME_BGR_U8  [B,Hf,Wf,3] HWC BGR uint8 (clearcam.py:582, ffmpeg -pix_fmt bgr24);
+ *   CC_FRAME_BGR_F32 [B,Hf,Wf,3] HWC BGR float32 (test/run_mot.py:33);
+ *   CC_FRAME_I420_U8 [B,Hf*3/2,Wf] uint8 planar YUV 4:2:0 (ffmpeg -pix_fmt yuv420p, OpenCV I420): the Y plane Hf x Wf, then
+ *                    U and V, each (Hf/2) x (Wf/2); Hf and Wf must be even.  Converted to BGR on the device exactly as
+ *                    cv2.cvtColor(yuv, COLOR_YUV2BGR_I420) does (BT.601 limited range, 20-bit fixed point, nearest chroma).
+ * Any other code, or an odd Hf / Wf with I420, fails with CC_ERR_INVALID before anything is launched. */
+#define CC_FRAME_BGR_U8 0
+#define CC_FRAME_BGR_F32 1
+#define CC_FRAME_I420_U8 2
+
 /* YOLOv9.__call__ (detection/yolov9.py:375-388) for a batch of same-shape frames.
- * d_frames: [B,Hf,Wf,3] HWC **BGR**, uint8 (is_f32=0, clearcam.py:582) or float32 (is_f32=1, test/run_mot.py:33).
+ * d_frames: B frames of format frame_fmt, Hf x Wf pixels each.
  * d_out: [B,300,6] fp32 rows [x1,y1,x2,y2,conf,class] in frame pixels, descending conf, suppressed rows all-zero.
  * d_raw: optional [B,84,A] fp32 tap of the head output (xc,yc,w,h,80 class probs) for parity tests, or NULL.
  * A plan (buffers, TMA descriptors) is built and cached on the first call for each (dtype,B,Hf,Wf,res) — the
  * analogue of jit_infer's per-shape TinyJit cache (utils/helpers.py:214-221); later calls only launch kernels. */
-int cc_yolo_forward(cc_yolo* h, const void* d_frames, int is_f32, int B, int Hf, int Wf, int res, float* d_out,
+int cc_yolo_forward(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, float* d_out,
                     float* d_raw, void* stream);
 /* plan facts: letterboxed net input size, anchors, kernel launches per forward, algorithmic conv FLOPs,
  * bytes of activation workspace */
-int cc_yolo_plan_info(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, int* net_h, int* net_w, int* anchors,
+int cc_yolo_plan_info(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int* net_h, int* net_w, int* anchors,
                       int* launches, double* conv_flops, double* act_bytes);
 
 /* Workspace.  Every cached plan of a handle carves its activations out of ONE device workspace (size of the largest plan;
@@ -89,25 +100,25 @@ int cc_yolo_plan_info(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, in
  * cc_yolo_set_workspace (256-byte aligned device memory, owned by the caller; d_workspace = NULL returns to the
  * library-owned one); a plan that does not fit a caller-owned workspace fails with CC_ERR_INVALID.  The plans of one
  * handle share the memory: run them in stream order (one stream per handle). */
-int cc_yolo_workspace_bytes(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, size_t* bytes);
+int cc_yolo_workspace_bytes(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, size_t* bytes);
 int cc_yolo_set_workspace(cc_yolo* h, void* d_workspace, size_t bytes);
 
 /* measurement: per-op device time of one forward (CUDA events between launches on `stream`; synchronises).
  * Up to `cap` entries of ms / algorithmic conv FLOPs / algorithmic HBM bytes / kernel kind / op name (pointers valid
  * while h lives). */
-int cc_yolo_profile(cc_yolo* h, const void* d_frames, int is_f32, int B, int Hf, int Wf, int res, float* d_out, int cap,
+int cc_yolo_profile(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, float* d_out, int cap,
                     float* ms, double* flops, double* bytes, const char** kinds, const char** names, int* n_ops, void* stream);
 
 /* measurement: in-situ device timeline of one forward, no events between the launches (so programmatic dependent launch
  * overlaps exactly as in production).  For op i, host_ns[12i..12i+11] = globaltimer ns of (first CTA entered, grid
  * dependency released, last CTA exited; then of CTA 0: first operands landed, all MMAs issued, first accumulator complete,
  * last epilogue group done, exit; then four stamps inside the first staging pass of its first tile) for the tensor-core conv launches, zeros for the other kernels.  Synchronises. */
-int cc_yolo_trace(cc_yolo* h, const void* d_frames, int is_f32, int B, int Hf, int Wf, int res, float* d_out, int cap,
+int cc_yolo_trace(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, float* d_out, int cap,
                   unsigned long long* host_ns, const char** kinds, const char** names, double* flops, int* n_ops, void* stream);
 
 /* parity tap: after a forward, copy the output of graph layer `layer` (index into the reference's self.model list,
  * detection/yolov9.py:303-371) to dense fp32 [B,H,W,C].  d_dst == NULL only queries C/H/W (C = 0: no tensor). */
-int cc_yolo_layer_output(cc_yolo* h, int is_f32, int B, int Hf, int Wf, int res, int layer, float* d_dst, int* C,
+int cc_yolo_layer_output(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int layer, float* d_dst, int* C,
                          int* H, int* W, void* stream);
 
 /* kernel-level taps (parity tests) */
@@ -122,9 +133,10 @@ int cc_detect_pred_from_raw(const float* d_raw, int B, int n_classes, int A, flo
  * d_box[i] [B,h,w,64], d_cls[i] [B,h,w,80] (strides 8,16,32) -> d_pred [B,A,6], optional d_raw [B,84,A] */
 int cc_detect_decode(const float* const* d_box, const float* const* d_cls, const int* hs, const int* ws, int B,
                      float conf_thr, float* d_pred, float* d_raw, void* stream);
-/* YOLOv9.preprocess (detection/yolov9.py:390-404) + resize (utils/helpers.py:127-131): [B,Hin,Win,3] -> letterboxed
- * [B,out_h,out_w,3], same dtype.  d_out == NULL only queries the output size. */
-int cc_letterbox(const void* d_in, int is_f32, int B, int Hin, int Win, int res, void* d_out, int* out_h, int* out_w,
+/* YOLOv9.preprocess (detection/yolov9.py:390-404) + resize (utils/helpers.py:127-131): B frames of format frame_fmt,
+ * Hin x Win pixels -> letterboxed BGR [B,out_h,out_w,3], float32 for CC_FRAME_BGR_F32, else uint8 (an I420 frame is
+ * converted to BGR at each bilinear tap).  d_out == NULL only queries the output size. */
+int cc_letterbox(const void* d_in, int frame_fmt, int B, int Hin, int Win, int res, void* d_out, int* out_h, int* out_w,
                  void* stream);
 
 /* ---- CLIP image/text encoder (replaces class OpenCLIP, models/objects.py:21-186) ---- */
@@ -168,12 +180,14 @@ int cc_search_topk(const float* d_index, int N, int D, const float* d_q, const i
                    void* d_workspace, int32_t* d_rows, float* d_scores, void* stream);
 
 /* Crop + ObjectFinder.preprocess on the device, for objects cut out of frames already resident for the detector:
- * frame[y1:y2, x1:x2] (clearcam.py:396) -> BGR->RGB when bgr != 0 (models/objects.py:249) -> cv2.resize((size,size),
- * INTER_CUBIC) -> /255 -> (x-0.5)/0.5 -> CHW (models/objects.py:237-242).  d_frames: device uint8 [n_frames,H,W,3];
- * rects: HOST int32 [K,5] = frame, x1, y1, x2, y2 (validated, passed as kernel arguments: no copy, no sync);
- * d_out: device float32 [K,3,size,size] — the tensor cc_clip_encode_image takes. */
-int cc_clip_preprocess(const uint8_t* d_frames, int n_frames, int H, int W, const int32_t* rects, int K, int size, int bgr,
-                       float* d_out, void* stream);
+ * frame[y1:y2, x1:x2] (clearcam.py:396) -> RGB (models/objects.py:249) -> cv2.resize((size,size), INTER_CUBIC) -> /255 ->
+ * (x-0.5)/0.5 -> CHW (models/objects.py:237-242).  src_fmt: 0 = d_frames is uint8 RGB [n_frames,H,W,3], taken as is;
+ * 1 = uint8 BGR [n_frames,H,W,3], channels swapped; 2 = I420 [n_frames,H*3/2,W] (H, W even), converted as
+ * cv2.cvtColor(frame, COLOR_YUV2RGB_I420) and then cropped.  rects: HOST int32 [K,5] = frame, x1, y1, x2, y2 in pixels
+ * (validated, passed as kernel arguments: no copy, no sync); d_out: device float32 [K,3,size,size] — the tensor
+ * cc_clip_encode_image takes. */
+int cc_clip_preprocess(const uint8_t* d_frames, int n_frames, int H, int W, const int32_t* rects, int K, int size,
+                       int src_fmt, float* d_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Tracker that consumes the detector rows (host code, no GPU): ocsort_tracker/ocsort.py:163-308 `OCSort`, with
