@@ -63,6 +63,7 @@ _SIGS = {
     "cc_ocsort_update_batch": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _vp]),
     "cc_ocsort_num_tracks": (_i, [_vp]),
     "cc_letterbox": (_i, [_vp, _i, _i, _i, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
+    "cc_attention": (_i, [_vp, _i, _i, _i, _i, _i, _vp, ctypes.c_size_t, _vp, ctypes.POINTER(ctypes.c_size_t), _vp]),
 }
 
 

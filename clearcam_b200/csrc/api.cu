@@ -47,4 +47,28 @@ int cc_conv2d(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, i
   return conv_direct_launch(p, static_cast<cudaStream_t>(stream));
 }
 
+int cc_attention(const void* d_qkv, int B, int L, int H, int causal, int impl, void* d_ws, size_t ws_bytes, void* d_ctx,
+                 size_t* ws_needed, void* stream) {
+  CC_REQUIRE(impl == 1 || impl == 2, "cc_attention: unknown impl %d (1 = mma.sync, 2 = wgmma)", impl);
+  CC_REQUIRE(B >= 0 && L >= 1 && H >= 1, "cc_attention: bad shape B=%d L=%d H=%d", B, L, H);
+  const int max_len = impl == 1 ? attention_max_len() : attention_tc_max_len();
+  CC_REQUIRE(L <= max_len, "cc_attention: sequence length %d too long for impl %d (at most %d)", L, impl, max_len);
+  // one CTA row per (image, head): gridDim.x for the mma.sync kernel, gridDim.y (at most 65535) for the wgmma kernel
+  CC_REQUIRE(static_cast<long long>(B) * H <= (impl == 1 ? 0x7fffffffLL : 65535LL),
+             "cc_attention: B*H = %lld (image, head) pairs exceed the grid of impl %d", static_cast<long long>(B) * H, impl);
+  const size_t need = impl == 2 ? attention_tc_workspace_bytes(B, L, H) : 0;
+  if (ws_needed) *ws_needed = need;
+  if (!d_ctx) return CC_OK;   // workspace size query
+  CC_REQUIRE(d_qkv != nullptr, "cc_attention: d_qkv is NULL");
+  CC_REQUIRE(ws_bytes >= need && (need == 0 || d_ws != nullptr), "cc_attention: workspace of %zu bytes too small (%zu needed)",
+             d_ws ? ws_bytes : size_t(0), need);
+  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(d_ws) & 15) == 0,
+             "cc_attention: d_qkv and d_ws must be 16-byte aligned");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const __nv_bfloat16* qkv = static_cast<const __nv_bfloat16*>(d_qkv);
+  __nv_bfloat16* ctx = static_cast<__nv_bfloat16*>(d_ctx);
+  return impl == 1 ? attention_launch(qkv, ctx, B, L, H, causal ? 1 : 0, st)
+                   : attention_tc_launch(qkv, ctx, static_cast<__nv_bfloat16*>(d_ws), B, L, H, causal ? 1 : 0, st);
+}
+
 }  // extern "C"

@@ -188,6 +188,7 @@ bool attention_tc_supported(int L) {
   if (mode == 1) return L > 128;
   return true;
 }
+int attention_tc_max_len() { return kMaxLk; }
 size_t attention_tc_workspace_bytes(int B, int L, int H) {
   return static_cast<size_t>(B) * H * 64 * ((L + 63) / 64 * 64) * 2;
 }

@@ -143,8 +143,10 @@ int text_embed_launch(const int* ids, const float* tok, const float* pos, float*
                       int vocab, cudaStream_t st);
 int l2norm_launch(const float* in, float* out, int rows, int D, long long out_stride, float eps, cudaStream_t st);
 int attention_launch(const __nv_bfloat16* qkv, __nv_bfloat16* ctx, int B, int L, int H, int causal, cudaStream_t st);
+int attention_max_len();      // longest sequence whose K and V fit the mma.sync kernel's shared memory
 // wgmma attention (attention_tc.cu); vt_ws: workspace of attention_tc_workspace_bytes() for the per-head V^T copy
 bool attention_tc_supported(int L);
+int attention_tc_max_len();
 size_t attention_tc_workspace_bytes(int B, int L, int H);
 int attention_tc_launch(const __nv_bfloat16* qkv, __nv_bfloat16* ctx, __nv_bfloat16* vt_ws, int B, int L, int H, int causal,
                         cudaStream_t st);

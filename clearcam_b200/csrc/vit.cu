@@ -392,15 +392,19 @@ __global__ void __launch_bounds__(32 * kAttnWarps) attention_kernel(const __nv_b
   }
 }
 
+static constexpr int kAttnSmemMax = 200 * 1024;   // K and V of one head, [Lp][kAttnPitch] bf16 each
+
+int attention_max_len() { return (kAttnSmemMax / (2 * kAttnPitch * 2)) & ~15; }
+
 int attention_launch(const __nv_bfloat16* qkv, __nv_bfloat16* ctx, int B, int L, int H, int causal, cudaStream_t st) {
   if (B == 0) return CC_OK;
   const int Lp = (L + 15) & ~15;
   const int smem = 2 * Lp * kAttnPitch * 2;
-  CC_REQUIRE(smem <= 200 * 1024, "attention: sequence length %d too long for the single-CTA kernel", L);
+  CC_REQUIRE(smem <= kAttnSmemMax, "attention: sequence length %d too long for the single-CTA kernel", L);
   static bool attr_set = false;
   if (!attr_set) {
-    CC_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    CC_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    CC_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemMax));
+    CC_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemMax));
     attr_set = true;
   }
   const dim3 grid(B * H, ((L + 15) / 16 > 2 * kAttnWarps) ? kAttnSplitMax : 1);   // short sequences: one CTA stages K/V once

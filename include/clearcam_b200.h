@@ -138,6 +138,14 @@ int cc_detect_decode(const float* const* d_box, const float* const* d_cls, const
  * converted to BGR at each bilinear tap).  d_out == NULL only queries the output size. */
 int cc_letterbox(const void* d_in, int frame_fmt, int B, int Hin, int Win, int res, void* d_out, int* out_h, int* out_w,
                  void* stream);
+/* CLIP multi-head attention (models/objects.py:108-118, :157-168), d_head = 64: per (image, head)
+ * ctx = softmax(Q K^T / 8 [+ causal mask when causal != 0]) V.  d_qkv: bf16 [B*L, 3*H*64], the fused Q | K | V rows the
+ * encoder plans pass; d_ctx: bf16 [B*L, H*64].  impl: 1 = the mma.sync kernel (vit.cu, L <= 704), 2 = the wgmma kernel
+ * (attention_tc.cu, L <= 384); there is no automatic choice here.  d_ws: device scratch of *ws_needed bytes (the wgmma
+ * kernel's V^T copy; 0 bytes for impl 1), 16-byte aligned.  d_ctx == NULL only writes *ws_needed.  An unknown impl, a bad
+ * shape, a sequence the kernel cannot hold or a short workspace fails with CC_ERR_INVALID before anything is launched. */
+int cc_attention(const void* d_qkv, int B, int L, int H, int causal, int impl, void* d_ws, size_t ws_bytes, void* d_ctx,
+                 size_t* ws_needed, void* stream);
 
 /* ---- CLIP image/text encoder (replaces class OpenCLIP, models/objects.py:21-186) ---- */
 typedef struct cc_clip cc_clip;
