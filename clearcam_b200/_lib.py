@@ -64,6 +64,17 @@ _SIGS = {
     "cc_ocsort_num_tracks": (_i, [_vp]),
     "cc_letterbox": (_i, [_vp, _i, _i, _i, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
     "cc_attention": (_i, [_vp, _i, _i, _i, _i, _i, _vp, ctypes.c_size_t, _vp, ctypes.POINTER(ctypes.c_size_t), _vp]),
+    "cc_pool": (_i, [_i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
+    "cc_spp3": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "cc_cbfuse": (_i, [_i, _i, ctypes.POINTER(_vp), ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i),
+                       _vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "cc_split_planes": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
+    "cc_finish_f32": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp]),
+    "cc_stem": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, ctypes.c_size_t,
+                     ctypes.POINTER(ctypes.c_size_t), _vp]),
+    "cc_conv2d_pre": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _i, _vp]),
+    "cc_conv2d_fp32_accurate": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp,
+                                     ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t), _vp]),
 }
 
 

@@ -72,3 +72,111 @@ int cc_attention(const void* d_qkv, int B, int L, int H, int causal, int impl, v
 }
 
 }  // extern "C"
+
+// An NHWC slice argument of the detector taps: non-NULL, 16-byte aligned, cs / co / C in whole vectors of `vec` channels
+// and the slice inside the row.
+static int slice_arg(const char* who, const char* what, const void* p, int N, int H, int W, int cs, int co, int C, int f32, int vec,
+                     TSlice* t) {
+  CC_REQUIRE(p != nullptr, "%s: %s is NULL", who, what);
+  CC_REQUIRE((reinterpret_cast<uintptr_t>(p) & 15) == 0, "%s: %s must be 16-byte aligned", who, what);
+  CC_REQUIRE(N >= 1 && H >= 1 && W >= 1 && C >= 1, "%s: %s has a bad shape N=%d H=%d W=%d C=%d", who, what, N, H, W, C);
+  CC_REQUIRE(C % vec == 0 && co % vec == 0 && cs % vec == 0 && co >= 0 && co + C <= cs,
+             "%s: %s slice cs=%d co=%d C=%d must be whole vectors of %d channels inside the row", who, what, cs, co, C, vec);
+  *t = TSlice{};
+  t->p = static_cast<__nv_bfloat16*>(const_cast<void*>(p)); t->cs = cs; t->co = co; t->C = C; t->N = N; t->H = H; t->W = W; t->f32 = f32;
+  return CC_OK;
+}
+
+extern "C" {
+
+int cc_pool(int op, int f32, const void* d_in, int N, int H, int W, int in_cs, int in_co, int C, void* d_out, int out_cs, int out_co,
+            void* stream) {
+  CC_REQUIRE(op >= CC_POOL_AVG2_PAD && op <= CC_POOL_UPSAMPLE2, "cc_pool: unknown op %d", op);
+  CC_REQUIRE(f32 == 0 || f32 == 1, "cc_pool: f32 is 0 (bf16) or 1 (fp32), got %d", f32);
+  CC_REQUIRE(op == CC_POOL_MAX5 || op == CC_POOL_UPSAMPLE2 || (H >= 2 && W >= 2), "cc_pool: op %d needs a map of at least 2x2", op);
+  CC_REQUIRE(op != CC_POOL_AVGMAX || (H % 2 == 0 && W % 2 == 0), "cc_pool: avgmax needs even sides, got %dx%d", H, W);
+  const int Ho = op == CC_POOL_AVGMAX ? H / 2 : op == CC_POOL_UPSAMPLE2 ? 2 * H : H;
+  const int Wo = op == CC_POOL_AVGMAX ? W / 2 : op == CC_POOL_UPSAMPLE2 ? 2 * W : W;
+  TSlice in, out;
+  if (int rc = slice_arg("cc_pool", "input", d_in, N, H, W, in_cs, in_co, C, f32, 8, &in)) return rc;
+  if (int rc = slice_arg("cc_pool", "output", d_out, N, Ho, Wo, out_cs, out_co, C, f32, 8, &out)) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  switch (op) {
+    case CC_POOL_AVG2_PAD: return avgpool2_pad_launch(in, out, st);
+    case CC_POOL_AVGMAX: return avgmax_pool_launch(in, out, st);
+    case CC_POOL_MAX5: return maxpool5_launch(in, out, st);
+    default: return upsample2_launch(in, out, st);
+  }
+}
+
+int cc_spp3(void* d_cat, int N, int H, int W, int cs, int co, int c1, void* stream) {
+  CC_REQUIRE(c1 >= 1, "cc_spp3: c1=%d", c1);
+  TSlice cat;
+  if (int rc = slice_arg("cc_spp3", "concat buffer", d_cat, N, H, W, cs, co, 4 * c1, 0, 8, &cat)) return rc;
+  CC_REQUIRE(N <= 65535, "cc_spp3: N=%d exceeds the grid", N);
+  CC_REQUIRE(spp3_supported(cat, c1), "cc_spp3: not supported for H*W=%d, c1=%d (c1 a multiple of 64, at most 800 pixels)", H * W, c1);
+  return spp3_launch(cat, c1, static_cast<cudaStream_t>(stream));
+}
+
+int cc_cbfuse(int f32, int nsrc, const void* const* d_src, const int* src_h, const int* src_w, const int* src_cs, const int* src_co,
+              const void* d_last, int last_cs, int last_co, void* d_out, int out_cs, int out_co, int N, int H, int W, int C,
+              void* stream) {
+  CC_REQUIRE(f32 == 0 || f32 == 1, "cc_cbfuse: f32 is 0 (bf16) or 1 (fp32), got %d", f32);
+  CC_REQUIRE(nsrc >= 1 && nsrc <= 5, "cc_cbfuse: nsrc=%d (1 to 5 sources)", nsrc);
+  CC_REQUIRE(d_src && src_h && src_w && src_cs && src_co, "cc_cbfuse: a NULL source array");
+  CBFuseParams p{};
+  p.nsrc = nsrc;
+  for (int k = 0; k < nsrc; ++k)
+    if (int rc = slice_arg("cc_cbfuse", "a source", d_src[k], N, src_h[k], src_w[k], src_cs[k], src_co[k], C, f32, 8, &p.src[k])) return rc;
+  if (int rc = slice_arg("cc_cbfuse", "last", d_last, N, H, W, last_cs, last_co, C, f32, 8, &p.last)) return rc;
+  if (int rc = slice_arg("cc_cbfuse", "output", d_out, N, H, W, out_cs, out_co, C, f32, 8, &p.out)) return rc;
+  return cbfuse_launch(p, static_cast<cudaStream_t>(stream));
+}
+
+int cc_split_planes(const float* d_in, int npix, int cs, int co, int C, void* d_out, void* stream) {
+  TSlice in;
+  if (int rc = slice_arg("cc_split_planes", "input", d_in, npix, 1, 1, cs, co, C, 1, 4, &in)) return rc;
+  CC_REQUIRE(d_out != nullptr && (reinterpret_cast<uintptr_t>(d_out) & 7) == 0, "cc_split_planes: d_out must be 8-byte aligned");
+  return split_planes_launch(in, static_cast<__nv_bfloat16*>(d_out), static_cast<cudaStream_t>(stream));
+}
+
+int cc_finish_f32(const float* d_acc, const float* d_bias, int act, int npix, int C, float* d_out, int out_cs, int out_co,
+                  const float* d_res, int res_cs, int res_co, void* stream) {
+  CC_REQUIRE(act == CC_ACT_NONE || act == CC_ACT_SILU, "cc_finish_f32: act %d (0 none, 1 SiLU)", act);
+  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_bias) & 15) == 0, "cc_finish_f32: d_bias must be 16-byte aligned");
+  FinishParams p{};
+  TSlice t;
+  if (int rc = slice_arg("cc_finish_f32", "acc", d_acc, npix, 1, 1, C, 0, C, 1, 4, &t)) return rc;
+  if (int rc = slice_arg("cc_finish_f32", "output", d_out, npix, 1, 1, out_cs, out_co, C, 1, 4, &t)) return rc;
+  if (d_res)
+    if (int rc = slice_arg("cc_finish_f32", "residual", d_res, npix, 1, 1, res_cs, res_co, C, 1, 4, &t)) return rc;
+  p.acc = d_acc; p.bias = d_bias; p.act = act; p.npix = npix; p.C = C;
+  p.out = d_out; p.out_cs = out_cs; p.out_co = out_co;
+  p.res = d_res; p.res_cs = res_cs; p.res_co = res_co;
+  return finish_f32_launch(p, static_cast<cudaStream_t>(stream));
+}
+
+int cc_conv2d_pre(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const void* d_w, const float* d_bias,
+                  int Cout, int k, int stride, void* d_out, int out_cs, int out_co, int out_f32, int act, const float* d_pre, int bn,
+                  void* stream) {
+  CC_REQUIRE(d_in && d_w && d_out && d_pre, "cc_conv2d_pre: d_in, d_w, d_out and d_pre must not be NULL");
+  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_pre) & 15) == 0, "cc_conv2d_pre: d_pre must be 16-byte aligned");
+  CC_REQUIRE(N >= 1 && Hin >= 1 && Win >= 1 && (stride == 1 || stride == 2), "cc_conv2d_pre: bad shape N=%d Hin=%d Win=%d stride=%d", N, Hin, Win, stride);
+  const int Ho = stride == 2 ? Hin / 2 : Hin, Wo = stride == 2 ? Win / 2 : Win;
+  CC_REQUIRE(Ho % 2 == 0 && Wo % 2 == 0, "cc_conv2d_pre: the output %dx%d must have even sides (pre is its half-resolution map)", Ho, Wo);
+  ConvDesc d{};
+  d.in = d_in; d.in_cs = in_cs; d.in_co = in_co; d.Cin = Cin;
+  d.N = N; d.Hin = Hin; d.Win = Win; d.k = k; d.stride = stride;
+  d.w = d_w; d.bias = d_bias;
+  d.out = d_out; d.out_cs = out_cs; d.out_co = out_co; d.Cout = Cout; d.out_f32 = out_f32;
+  d.act = act; d.bn_override = bn;
+  d.pre = d_pre; d.pre_h = Ho / 2; d.pre_w = Wo / 2;
+  CC_REQUIRE(conv_gemm_supported(d), "cc_conv2d_pre: shape not supported by the wgmma conv (Cin=%d Cout=%d k=%d stride=%d)", Cin, Cout, k, stride);
+  const int sms = device_sm_count();
+  CC_REQUIRE(sms > 0, "cc_conv2d_pre: no sm_90 (H100) device");
+  GemmLaunch L;
+  if (int rc = conv_gemm_build(d, sms, &L)) return rc;
+  return conv_gemm_launch(L, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

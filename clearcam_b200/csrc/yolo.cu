@@ -148,8 +148,7 @@ struct ConvW {           // device-resident, kernel layout
   // fp32-accurate mode: the fp32 weight is split w = hi + mid + lo (three bf16).  w5: [Cout][k][k][5][Cin] = planes
   // hi|mid|lo|hi|mid (the five cross products below 2^-8 of the result, against the activation planes lo|mid|hi|mid|hi);
   // whi[i]: [Cout][k][k][seg_c[i]] = the hi plane of input-channel segment i (the hi x hi products, one GEMM per segment so
-  // that no tensor-core accumulator takes more than ~48 MMA steps: the tensor core's fp32 accumulation truncates, and its bias
-  // grows with the number of steps into one accumulator — tests/tools/diag_tc_accum.py)
+  // that no tensor-core accumulator takes more than 48 MMA steps: hi_segments)
   __nv_bfloat16* w5 = nullptr;
   std::vector<__nv_bfloat16*> whi;
   std::vector<int> seg_off, seg_c;
@@ -158,6 +157,64 @@ struct ConvW {           // device-resident, kernel layout
 };
 
 static __nv_bfloat16 f2bf(float x) { return __float2bfloat16_rn(x); }
+
+// ---- weight packing, shared by the plan builder and the kernel-level taps (cc_stem, cc_conv2d_fp32_accurate)
+// stem: PyTorch [Cout][3][3][3] fp32 -> wf [Cout][27] fp32 with the taps in (r, s, RGB) order (stem_kernel)
+static void stem_weights_rsc(const float* w, int cout, float* wf) {
+  for (int co = 0; co < cout; ++co)
+    for (int ci = 0; ci < 3; ++ci)
+      for (int r = 0; r < 3; ++r)
+        for (int s = 0; s < 3; ++s) wf[(static_cast<size_t>(co) * 9 + r * 3 + s) * 3 + ci] = w[((static_cast<size_t>(co) * 3 + ci) * 3 + r) * 3 + s];
+}
+// ... and the tensor-core stem's operand: bf16(w / 255) [Cout][32], K = 27 taps zero padded to 32 (raw pixels are exact in bf16)
+static std::vector<__nv_bfloat16> stem_tc_weights(const float* wf, int cout) {
+  std::vector<__nv_bfloat16> wt(static_cast<size_t>(cout) * 32, f2bf(0.f));
+  for (int co = 0; co < cout; ++co)
+    for (int kk = 0; kk < 27; ++kk) wt[static_cast<size_t>(co) * 32 + kk] = f2bf(wf[static_cast<size_t>(co) * 27 + kk] / 255.0f);
+  return wt;
+}
+
+// fp32-accurate mode: the input-channel segments of the hi x hi products, one GEMM each.  The tensor core's fp32 accumulation
+// truncates and its bias grows with the number of MMA steps into one accumulator (tests/tools/diag_tc_accum.py), so no segment
+// takes more than 48 k16 steps (seg_c * k * k / 16 <= 48).  Widths are multiples of 64 when Cin allows (the kernel's widest
+// k-block), else of 16, and as even as that allows.
+static constexpr int kMaxHiSteps = 48;
+static void hi_segments(int cin, int k, std::vector<int>* seg_off, std::vector<int>* seg_c) {
+  const int unit = cin % 64 == 0 ? 64 : 16;
+  int max_c = kMaxHiSteps * 16 / (k * k) / unit * unit;
+  if (max_c < unit) max_c = unit;
+  const int nseg = (cin + max_c - 1) / max_c;
+  const int sc = ((cin + nseg - 1) / nseg + unit - 1) / unit * unit;
+  seg_off->clear(); seg_c->clear();
+  for (int off = 0; off < cin; off += sc) { seg_off->push_back(off); seg_c->push_back(std::min(sc, cin - off)); }
+}
+// Split fp32 weights wf [rows = Cout*k*k][cin] into w = hi + mid + lo (three bf16).  w5: [rows][5][cin] = planes hi|mid|lo|hi|mid
+// (the five cross products below 2^-8 of the result, against the activation planes lo|mid|hi|mid|hi); whi[i]: [rows][seg_c[i]] =
+// the hi plane of input-channel segment i.
+static void split_weight_planes(const float* wf, size_t rows, int cin, const std::vector<int>& seg_off, const std::vector<int>& seg_c,
+                                std::vector<__nv_bfloat16>* w5, std::vector<std::vector<__nv_bfloat16>>* whi) {
+  w5->assign(rows * 5 * cin, f2bf(0.f));
+  std::vector<__nv_bfloat16> hi_plane(rows * cin);
+  for (size_t row = 0; row < rows; ++row)
+    for (int ci = 0; ci < cin; ++ci) {
+      const float v = wf[row * cin + ci];
+      const __nv_bfloat16 hi = f2bf(v);
+      const float r1 = v - __bfloat162float(hi);
+      const __nv_bfloat16 mid = f2bf(r1);
+      const __nv_bfloat16 lo = f2bf(r1 - __bfloat162float(mid));
+      __nv_bfloat16* d5 = w5->data() + row * 5 * cin + ci;
+      d5[0] = hi; d5[cin] = mid; d5[2 * cin] = lo; d5[3 * cin] = hi; d5[4 * cin] = mid;
+      hi_plane[row * cin + ci] = hi;
+    }
+  whi->assign(seg_off.size(), {});
+  for (size_t sgi = 0; sgi < seg_off.size(); ++sgi) {
+    const int off = seg_off[sgi], sc = seg_c[sgi];
+    std::vector<__nv_bfloat16>& ws = (*whi)[sgi];
+    ws.resize(rows * sc);
+    for (size_t row = 0; row < rows; ++row)
+      for (int c = 0; c < sc; ++c) ws[row * sc + c] = hi_plane[row * cin + off + c];
+  }
+}
 
 struct T { __nv_bfloat16* p = nullptr; int cs = 0, co = 0, C = 0, H = 0, W = 0; bool image = false; bool f32 = false; };   // f32: p is really float*
 
@@ -238,6 +295,7 @@ struct YoloModel {
     std::vector<__nv_bfloat16> w(static_cast<size_t>(cout_total) * k * k * cin_eff, f2bf(0.f));
     std::vector<float> wf, bias(cout_total);
     if (stem) wf.resize(static_cast<size_t>(cout_total) * 27);
+    else if (precise) wf.assign(w.size(), 0.f);   // fp32-accurate mode: w's layout in fp32 (split into bf16 planes below)
     int co_base = 0;
     for (size_t t = 0; t < names.size(); ++t) {
       auto iw = host.find(names[t] + ".weight"), ib = host.find(names[t] + ".bias");
@@ -250,15 +308,20 @@ struct YoloModel {
       CC_REQUIRE(ci_total == cin || groups == 1, "yolo: '%s': an input-channel sub-range of a grouped conv", names[t].c_str());
       const float* src = iw->second.p;
       const int cpg_out = cout / groups;
+      if (stem) {
+        CC_REQUIRE(k == 3 && cin == 3 && groups == 1 && ci_total == 3, "yolo: stem '%s' is not a 3x3 conv over 3 channels", names[t].c_str());
+        stem_weights_rsc(src, cout, &wf[static_cast<size_t>(co_base) * 27]);
+      }
       for (int co = 0; co < cout; ++co) {
         const int g = co / cpg_out;
-        for (int ci = 0; ci < cin_g; ++ci)
+        for (int ci = 0; ci < cin_g && !stem; ++ci)
           for (int r = 0; r < k; ++r)
             for (int s = 0; s < k; ++s) {
               const float v = src[((static_cast<size_t>(co) * src_cin_g + ci_begin + ci) * k + r) * k + s];
               const int ci_eff = dense ? g * cin_g + ci : ci;
-              if (stem) wf[(static_cast<size_t>(co_base + co) * 9 + r * 3 + s) * 3 + ci] = v;
-              else w[((static_cast<size_t>(co_base + co) * k + r) * k + s) * cin_eff + ci_eff] = f2bf(v);
+              const size_t o = ((static_cast<size_t>(co_base + co) * k + r) * k + s) * cin_eff + ci_eff;
+              w[o] = f2bf(v);
+              if (precise) wf[o] = v;
             }
         bias[co_base + co] = with_bias ? ib->second.p[co] : 0.f;
       }
@@ -269,49 +332,17 @@ struct YoloModel {
     int rc;
     if (stem) {
       if ((rc = upload(wf.data(), wf.size() * 4, reinterpret_cast<void**>(&cw.wf32)))) return rc;
-      std::vector<__nv_bfloat16> wt(static_cast<size_t>(cout_total) * 32, f2bf(0.f));
-      for (int co = 0; co < cout_total; ++co)
-        for (int kk = 0; kk < 27; ++kk) wt[static_cast<size_t>(co) * 32 + kk] = f2bf(wf[static_cast<size_t>(co) * 27 + kk] / 255.0f);
+      const std::vector<__nv_bfloat16> wt = stem_tc_weights(wf.data(), cout_total);
       if ((rc = upload(wt.data(), wt.size() * 2, reinterpret_cast<void**>(&cw.wtc)))) return rc;
     }
     else if (!precise) { if ((rc = upload(w.data(), w.size() * 2, reinterpret_cast<void**>(&cw.w)))) return rc; }
     else {
-      // the fp32 weights again (w above is already rounded = the hi plane)
-      {
-        const int steps = cin_eff * k * k / 16;
-        const int nseg = (steps + 47) / 48;
-        const int unit = cin_eff % 64 == 0 ? 64 : 16;
-        int sc = ((cin_eff + nseg - 1) / nseg + unit - 1) / unit * unit;
-        for (int off = 0; off < cin_eff; off += sc) { cw.seg_off.push_back(off); cw.seg_c.push_back(std::min(sc, cin_eff - off)); }
-      }
-      std::vector<__nv_bfloat16> w5(w.size() * 5, f2bf(0.f));
-      int cb = 0;
-      for (size_t t = 0; t < names.size(); ++t) {
-        const float* src = host.find(names[t] + ".weight")->second.p;
-        const int cout = couts[t], cpg_out = cout / groups;
-        for (int co = 0; co < cout; ++co) {
-          const int g = co / cpg_out;
-          for (int ci = 0; ci < cin_g; ++ci)
-            for (int r = 0; r < k; ++r)
-              for (int s2 = 0; s2 < k; ++s2) {
-                const float v = src[((static_cast<size_t>(co) * cin_g + ci) * k + r) * k + s2];
-                const __nv_bfloat16 hi = f2bf(v);
-                const float r1 = v - __bfloat162float(hi);
-                const __nv_bfloat16 mid = f2bf(r1);
-                const __nv_bfloat16 lo = f2bf(r1 - __bfloat162float(mid));
-                const int ci_eff = dense ? g * cin_g + ci : ci;
-                __nv_bfloat16* d5 = &w5[(((static_cast<size_t>(cb + co) * k + r) * k + s2) * 5) * cin_eff + ci_eff];
-                d5[0] = hi; d5[cin_eff] = mid; d5[2 * cin_eff] = lo; d5[3 * cin_eff] = hi; d5[4 * cin_eff] = mid;
-              }
-        }
-        cb += cout;
-      }
+      hi_segments(cin_eff, k, &cw.seg_off, &cw.seg_c);
+      std::vector<__nv_bfloat16> w5;
+      std::vector<std::vector<__nv_bfloat16>> whi;
+      split_weight_planes(wf.data(), static_cast<size_t>(cout_total) * k * k, cin_eff, cw.seg_off, cw.seg_c, &w5, &whi);
       if ((rc = upload(w5.data(), w5.size() * 2, reinterpret_cast<void**>(&cw.w5)))) return rc;
-      for (size_t sgi = 0; sgi < cw.seg_off.size(); ++sgi) {
-        const int off = cw.seg_off[sgi], sc = cw.seg_c[sgi];
-        std::vector<__nv_bfloat16> ws(static_cast<size_t>(cout_total) * k * k * sc);
-        for (size_t row = 0; row < static_cast<size_t>(cout_total) * k * k; ++row)
-          for (int c = 0; c < sc; ++c) ws[row * sc + c] = w[row * cin_eff + off + c];
+      for (const std::vector<__nv_bfloat16>& ws : whi) {
         __nv_bfloat16* dptr = nullptr;
         if ((rc = upload(ws.data(), ws.size() * 2, reinterpret_cast<void**>(&dptr)))) return rc;
         cw.whi.push_back(dptr);
@@ -324,6 +355,44 @@ struct YoloModel {
 };
 
 static bool tc_ok(int cin, int cout) { return cin % 16 == 0 && cout % 16 == 0; }
+
+// The fp32-accurate conv as ops, shared by the plan builder and cc_conv2d_fp32_accurate: fp32 slice -> six bf16 planes
+// [lo|mid|hi|mid|hi|hi] in `scratch`; then on the same wgmma conv kernel, all with fp32 output into the dense partial-sum buffer
+// `accbuf`: one GEMM per input-channel segment of the hi x hi products (hi plane at channel offset 5C), accumulated with the
+// in-place fp32 residual of the epilogue (one round-to-nearest add), one GEMM for the five cross products (planes 0..4 against
+// the weight planes hi|mid|lo|hi|mid); a last pass applies bias, the exact SiLU and the residual and writes the output slice.
+static int precise_conv_ops(const std::string& key, const ConvW& cw, const TSlice& in, int stride, int act, __nv_bfloat16* scratch,
+                            float* accbuf, float* out, int out_cs, int out_co, const float* res, int res_cs, int res_co, int sms,
+                            std::vector<Op>* ops, double* conv_flops) {
+  Op sp; sp.kind = Op::SPLIT; sp.name = key + ".split"; sp.s_in = in; sp.s_out = TSlice{}; sp.s_out.p = scratch;
+  ops->push_back(std::move(sp));
+  const int Ho = stride == 2 ? in.H / 2 : in.H, Wo = stride == 2 ? in.W / 2 : in.W;
+  const int nseg = static_cast<int>(cw.seg_off.size());
+  for (int g = 0; g <= nseg; ++g) {
+    ConvDesc d{};
+    d.in = scratch; d.in_cs = 6 * in.C;
+    if (g < nseg) { d.in_co = 5 * in.C + cw.seg_off[g]; d.Cin = cw.seg_c[g]; d.w = cw.whi[g]; }
+    else { d.in_co = 0; d.Cin = 5 * in.C; d.w = cw.w5; }
+    d.N = in.N; d.Hin = in.H; d.Win = in.W; d.k = cw.k; d.stride = stride;
+    d.bias = nullptr;
+    d.out = accbuf; d.out_cs = cw.cout; d.out_co = 0; d.out_f32 = 1;
+    d.Cout = cw.cout; d.act = CC_ACT_NONE;
+    if (g > 0) { d.res = accbuf; d.res_cs = cw.cout; d.res_co = 0; }
+    Op gop; gop.kind = Op::GEMM; gop.name = key + (g < nseg ? ".hi" + std::to_string(g) : ".cross");
+    if (int rc = conv_gemm_build(d, sms, &gop.gemm)) return rc;
+    gop.gemm.flops = g == 0 ? 2.0 * in.N * Ho * Wo * double(cw.cout) * cw.k * cw.k * cw.cin : 0.0;   // algorithmic FLOPs once
+    *conv_flops += gop.gemm.flops;
+    ops->push_back(std::move(gop));
+  }
+  Op op; op.kind = Op::FINISH; op.name = key;
+  FinishParams& f = op.fin;
+  f = FinishParams{};
+  f.acc = accbuf; f.bias = cw.bias; f.act = act; f.npix = static_cast<long long>(in.N) * Ho * Wo; f.C = cw.cout;
+  f.out = out; f.out_cs = out_cs; f.out_co = out_co;
+  if (res) { f.res = res; f.res_cs = res_cs; f.res_co = res_co; }
+  ops->push_back(std::move(op));
+  return CC_OK;
+}
 // The two first convs of a detect-head scale read the same input and are fused into one conv of 64 + d output channels —
 // unless that sum only tiles in narrow blocks (the conv kernel tiles Cout by its largest divisor that is a multiple of 16
 // and at most 256: 64 + 240 = 304 = 16 x 19 would run 19 blocks of 16, measured 7 ms of a 14 ms YOLOv9-m step).
@@ -389,43 +458,16 @@ struct Builder {
       if (need_acc > max_acc) max_acc = need_acc;
     }
     if (bump.dry) return;
+    if (M.precise) {
+      float* o = out_f32 ? out_f32 : reinterpret_cast<float*>(out.p);
+      rc = precise_conv_ops(key, cw, ts(in), stride, act, scratch, accbuf, o, out_f32 ? cw.cout : out.cs, out_f32 ? 0 : out.co,
+                            res ? reinterpret_cast<const float*>(res->p) : nullptr, res ? res->cs : 0, res ? res->co : 0, M.sms,
+                            &P.ops, &P.conv_flops);
+      return;
+    }
     Op op;
     op.name = key;
-    if (M.precise) {
-      // fp32 slice -> six bf16 planes [lo|mid|hi|mid|hi|hi] in the scratch; then on the same wgmma conv kernel, all with fp32
-      // output into one dense partial-sum buffer: one GEMM per input-channel segment of the hi x hi products (hi plane at
-      // channel offset 5C), accumulated with the in-place fp32 residual of the epilogue (one round-to-nearest add), one GEMM
-      // for the five cross products (planes 0..4 against the weight planes hi|mid|lo|hi|mid); a last pass applies bias, the
-      // exact SiLU and the residual and writes the output slice.
-      Op sp; sp.kind = Op::SPLIT; sp.name = key + ".split"; sp.s_in = ts(in); sp.s_out = TSlice{}; sp.s_out.p = scratch;
-      P.ops.push_back(std::move(sp));
-      const int Ho = stride == 2 ? in.H / 2 : in.H, Wo = stride == 2 ? in.W / 2 : in.W;
-      const int nseg = static_cast<int>(cw.seg_off.size());
-      for (int g = 0; g <= nseg; ++g) {
-        ConvDesc d{};
-        d.in = scratch; d.in_cs = 6 * in.C;
-        if (g < nseg) { d.in_co = 5 * in.C + cw.seg_off[g]; d.Cin = cw.seg_c[g]; d.w = cw.whi[g]; }
-        else { d.in_co = 0; d.Cin = 5 * in.C; d.w = cw.w5; }
-        d.N = P.B; d.Hin = in.H; d.Win = in.W; d.k = cw.k; d.stride = stride;
-        d.bias = nullptr;
-        d.out = accbuf; d.out_cs = cw.cout; d.out_co = 0; d.out_f32 = 1;
-        d.Cout = cw.cout; d.act = CC_ACT_NONE;
-        if (g > 0) { d.res = accbuf; d.res_cs = cw.cout; d.res_co = 0; }
-        Op gop; gop.kind = Op::GEMM; gop.name = key + (g < nseg ? ".hi" + std::to_string(g) : ".cross");
-        rc = conv_gemm_build(d, M.sms, &gop.gemm);
-        if (rc) return;
-        gop.gemm.flops = g == 0 ? 2.0 * P.B * Ho * Wo * double(cw.cout) * cw.k * cw.k * cw.cin : 0.0;   // algorithmic FLOPs once
-        P.conv_flops += gop.gemm.flops;
-        P.ops.push_back(std::move(gop));
-      }
-      op.kind = Op::FINISH;
-      FinishParams& f = op.fin;
-      f = FinishParams{};
-      f.acc = accbuf; f.bias = cw.bias; f.act = act; f.npix = static_cast<long long>(P.B) * Ho * Wo; f.C = cw.cout;
-      if (out_f32) { f.out = out_f32; f.out_cs = cw.cout; f.out_co = 0; }
-      else { f.out = reinterpret_cast<float*>(out.p); f.out_cs = out.cs; f.out_co = out.co; }
-      if (res) { f.res = reinterpret_cast<const float*>(res->p); f.res_cs = res->cs; f.res_co = res->co; }
-    } else if (cw.groups == 1 && tc_ok(cw.cin, cw.cout)) {
+    if (cw.groups == 1 && tc_ok(cw.cin, cw.cout)) {
       ConvDesc d{};
       d.in = in.p; d.in_cs = in.cs; d.in_co = in.co; d.Cin = in.C;
       d.N = P.B; d.Hin = in.H; d.Win = in.W; d.k = cw.k; d.stride = stride;
@@ -1283,6 +1325,109 @@ int cc_letterbox(const void* d_in, int frame_fmt, int B, int Hin, int Win, int r
   p.pad_y = py; p.pad_x = px; p.Hout = new_h + 2 * py; p.Wout = new_w + 2 * px;
   p.sx = float(double(Win) / double(new_w)); p.sy = float(double(Hin) / double(new_h));
   return letterbox_launch(p, static_cast<cudaStream_t>(stream));
+}
+
+static size_t al256(size_t b) { return (b + 255) & ~size_t(255); }
+static bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+int cc_stem(const void* d_frames, int frame_f32, int B, int H, int W, const float* h_w, const float* h_bias, int Cout, void* d_out,
+            int out_cs, int out_co, int out_f32, int impl, void* d_ws, size_t ws_bytes, size_t* ws_needed, void* stream) {
+  CC_REQUIRE(impl == 1 || impl == 2, "cc_stem: unknown impl %d (1 = stem_tc, 2 = stem_kernel)", impl);
+  CC_REQUIRE((frame_f32 == 0 || frame_f32 == 1) && (out_f32 == 0 || out_f32 == 1), "cc_stem: frame_f32 and out_f32 are 0 or 1");
+  CC_REQUIRE(B >= 1 && H >= 2 && W >= 2 && H % 2 == 0 && W % 2 == 0 && Cout >= 8 && Cout % 8 == 0,
+             "cc_stem: bad shape B=%d H=%d W=%d Cout=%d (even frame sides, Cout a multiple of 8)", B, H, W, Cout);
+  CC_REQUIRE(impl == 2 || (!frame_f32 && !out_f32 && (Cout == 16 || Cout == 32 || Cout == 64)),
+             "cc_stem: stem_tc takes uint8 frames and writes bf16, Cout 16, 32 or 64");
+  CC_REQUIRE(out_co >= 0 && out_co % 8 == 0 && out_cs % 8 == 0 && out_co + Cout <= out_cs,
+             "cc_stem: bad output slice cs=%d co=%d for Cout=%d (multiples of 8 channels)", out_cs, out_co, Cout);
+  const size_t need = al256(size_t(Cout) * 27 * 4) + al256(size_t(Cout) * 32 * 2) + al256(size_t(Cout) * 4);
+  if (ws_needed) *ws_needed = need;
+  if (!d_out) return CC_OK;   // workspace size query
+  CC_REQUIRE(d_frames && h_w && h_bias, "cc_stem: d_frames, h_w and h_bias must not be NULL");
+  CC_REQUIRE(ws_bytes >= need && d_ws, "cc_stem: workspace of %zu bytes too small (%zu needed)", d_ws ? ws_bytes : size_t(0), need);
+  CC_REQUIRE(al16(d_out) && al16(d_ws) && (!frame_f32 || (reinterpret_cast<uintptr_t>(d_frames) & 3) == 0),
+             "cc_stem: d_out and d_ws must be 16-byte aligned, float frames 4-byte aligned");
+  std::vector<float> wf(static_cast<size_t>(Cout) * 27);
+  stem_weights_rsc(h_w, Cout, wf.data());
+  const std::vector<__nv_bfloat16> wt = stem_tc_weights(wf.data(), Cout);
+  uint8_t* ws = static_cast<uint8_t*>(d_ws);
+  float* dwf = reinterpret_cast<float*>(ws);
+  __nv_bfloat16* dwt = reinterpret_cast<__nv_bfloat16*>(ws + al256(wf.size() * 4));
+  float* db = reinterpret_cast<float*>(ws + al256(wf.size() * 4) + al256(wt.size() * 2));
+  TSlice out{};
+  out.p = static_cast<__nv_bfloat16*>(d_out); out.cs = out_cs; out.co = out_co; out.C = Cout; out.N = B; out.H = H / 2; out.W = W / 2;
+  out.f32 = out_f32;
+  StemTcParams tc{};
+  if (impl == 1)
+    if (int rc = stem_tc_build(B, H, W, dwt, db, Cout, out, &tc)) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CC_CHECK_CUDA(cudaMemcpyAsync(dwf, wf.data(), wf.size() * 4, cudaMemcpyHostToDevice, st));
+  CC_CHECK_CUDA(cudaMemcpyAsync(dwt, wt.data(), wt.size() * 2, cudaMemcpyHostToDevice, st));
+  CC_CHECK_CUDA(cudaMemcpyAsync(db, h_bias, size_t(Cout) * 4, cudaMemcpyHostToDevice, st));
+  if (impl == 1) return stem_tc_launch(tc, static_cast<const uint8_t*>(d_frames), st);
+  StemParams p{};
+  p.in = d_frames; p.is_f32 = frame_f32; p.B = B; p.H = H; p.W = W; p.w = dwf; p.bias = db; p.Cout = Cout; p.out = out;
+  return stem_launch(p, st);
+}
+
+int cc_conv2d_fp32_accurate(const float* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const float* h_w,
+                            const float* h_bias, int Cout, int k, int stride, int act, const float* d_res, int res_cs, int res_co,
+                            float* d_out, int out_cs, int out_co, void* d_ws, size_t ws_bytes, size_t* ws_needed, void* stream) {
+  CC_REQUIRE((k == 1 && stride == 1) || (k == 3 && (stride == 1 || stride == 2)),
+             "cc_conv2d_fp32_accurate: k=%d stride=%d (k 1 with stride 1, or k 3 with stride 1 or 2)", k, stride);
+  CC_REQUIRE(act == CC_ACT_NONE || act == CC_ACT_SILU, "cc_conv2d_fp32_accurate: act %d (0 none, 1 SiLU)", act);
+  CC_REQUIRE(N >= 1 && Hin >= 1 && Win >= 1 && (stride == 1 || (Hin % 2 == 0 && Win % 2 == 0)),
+             "cc_conv2d_fp32_accurate: bad shape N=%d Hin=%d Win=%d (even sides for stride 2)", N, Hin, Win);
+  CC_REQUIRE(Cin >= 16 && Cin % 16 == 0 && Cout >= 16 && Cout % 16 == 0,
+             "cc_conv2d_fp32_accurate: Cin=%d Cout=%d (multiples of 16)", Cin, Cout);
+  CC_REQUIRE(in_co >= 0 && in_co % 4 == 0 && in_cs % 4 == 0 && in_co + Cin <= in_cs && out_co >= 0 && out_co % 4 == 0 &&
+                 out_cs % 4 == 0 && out_co + Cout <= out_cs && (!d_res || (res_co >= 0 && res_co % 4 == 0 && res_cs % 4 == 0 && res_co + Cout <= res_cs)),
+             "cc_conv2d_fp32_accurate: bad slice (cs, co multiples of 4 channels, the slice inside the row)");
+  const int Ho = stride == 2 ? Hin / 2 : Hin, Wo = stride == 2 ? Win / 2 : Win;
+  std::vector<int> seg_off, seg_c;
+  hi_segments(Cin, k, &seg_off, &seg_c);
+  const size_t rows = static_cast<size_t>(Cout) * k * k;
+  const size_t planes_b = al256(static_cast<size_t>(N) * Hin * Win * 6 * Cin * 2), acc_b = al256(static_cast<size_t>(N) * Ho * Wo * Cout * 4);
+  const size_t w5_b = al256(rows * 5 * Cin * 2), bias_b = al256(size_t(Cout) * 4);
+  size_t need = planes_b + acc_b + w5_b + bias_b;
+  for (int c : seg_c) need += al256(rows * c * 2);
+  if (ws_needed) *ws_needed = need;
+  if (!d_out) return CC_OK;   // workspace size query
+  CC_REQUIRE(d_in && h_w, "cc_conv2d_fp32_accurate: d_in and h_w must not be NULL");
+  CC_REQUIRE(ws_bytes >= need && d_ws, "cc_conv2d_fp32_accurate: workspace of %zu bytes too small (%zu needed)", d_ws ? ws_bytes : size_t(0), need);
+  CC_REQUIRE(al16(d_in) && al16(d_out) && al16(d_res) && al16(d_ws), "cc_conv2d_fp32_accurate: device pointers must be 16-byte aligned");
+  const int sms = device_sm_count();
+  CC_REQUIRE(sms > 0, "cc_conv2d_fp32_accurate: no sm_90 (H100) device");
+  // PyTorch [Cout][Cin][k][k] -> the kernel layout [Cout][k][k][Cin], then the planes exactly as the plan's weights
+  std::vector<float> wf(rows * Cin);
+  for (int co = 0; co < Cout; ++co)
+    for (int ci = 0; ci < Cin; ++ci)
+      for (int r = 0; r < k; ++r)
+        for (int s = 0; s < k; ++s) wf[((static_cast<size_t>(co) * k + r) * k + s) * Cin + ci] = h_w[((static_cast<size_t>(co) * Cin + ci) * k + r) * k + s];
+  std::vector<__nv_bfloat16> w5;
+  std::vector<std::vector<__nv_bfloat16>> whi;
+  split_weight_planes(wf.data(), rows, Cin, seg_off, seg_c, &w5, &whi);
+  uint8_t* ws = static_cast<uint8_t*>(d_ws);
+  __nv_bfloat16* planes = reinterpret_cast<__nv_bfloat16*>(ws);  ws += planes_b;
+  float* acc = reinterpret_cast<float*>(ws);                     ws += acc_b;
+  ConvW cw;
+  cw.cin = Cin; cw.cout = Cout; cw.k = k; cw.groups = 1; cw.seg_off = seg_off; cw.seg_c = seg_c;
+  cw.w5 = reinterpret_cast<__nv_bfloat16*>(ws);                  ws += w5_b;
+  cw.bias = h_bias ? reinterpret_cast<float*>(ws) : nullptr;     ws += bias_b;
+  for (size_t i = 0; i < seg_c.size(); ++i) { cw.whi.push_back(reinterpret_cast<__nv_bfloat16*>(ws)); ws += al256(rows * seg_c[i] * 2); }
+  TSlice in{};
+  in.p = reinterpret_cast<__nv_bfloat16*>(const_cast<float*>(d_in)); in.cs = in_cs; in.co = in_co; in.C = Cin;
+  in.N = N; in.H = Hin; in.W = Win; in.f32 = 1;
+  YoloPlan run;
+  double flops = 0;
+  if (int rc = precise_conv_ops("conv", cw, in, stride, act, planes, acc, d_out, out_cs, out_co, d_res, res_cs, res_co, sms, &run.ops, &flops))
+    return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CC_CHECK_CUDA(cudaMemcpyAsync(cw.w5, w5.data(), w5.size() * 2, cudaMemcpyHostToDevice, st));
+  if (h_bias) CC_CHECK_CUDA(cudaMemcpyAsync(cw.bias, h_bias, size_t(Cout) * 4, cudaMemcpyHostToDevice, st));
+  for (size_t i = 0; i < whi.size(); ++i)
+    CC_CHECK_CUDA(cudaMemcpyAsync(cw.whi[i], whi[i].data(), whi[i].size() * 2, cudaMemcpyHostToDevice, st));
+  return plan_run(run, nullptr, nullptr, nullptr, st);
 }
 
 }  // extern "C"

@@ -37,3 +37,106 @@ def attention(qkv, L, H, causal, impl, ctx=None, stream=None):
     check(lib().cc_attention(ptr(qkv), B, L, H, causal, impl, ptr(ws), need.value, ptr(ctx), None, stream_ptr(stream)),
           "cc_attention")
     return ctx
+
+
+# ---- the detector's non-GEMM kernels and its two special conv forms, as the plan runs them (include/clearcam_b200.h)
+POOL_OPS = {"avg2_pad": 0, "avgmax": 1, "max5": 2, "upsample2": 3}
+
+
+def _nhwc(t):
+    assert t.is_cuda and t.dtype in (torch.bfloat16, torch.float32) and t.is_contiguous() and t.dim() == 4
+    return t.shape
+
+
+def pool(op, xbuf, in_co, C, obuf, out_co, stream=None):
+    """op in POOL_OPS on channels [in_co, in_co + C) of xbuf [N,H,W,in_cs] into [out_co, out_co + C) of obuf
+    [N,Ho,Wo,out_cs]; both bf16 or both fp32."""
+    N, H, W, in_cs = _nhwc(xbuf)
+    _nhwc(obuf)
+    assert obuf.dtype == xbuf.dtype
+    check(lib().cc_pool(POOL_OPS[op], int(xbuf.dtype == torch.float32), ptr(xbuf), N, H, W, in_cs, in_co, C, ptr(obuf),
+                        obuf.shape[-1], out_co, stream_ptr(stream)), "cc_pool")
+    return obuf
+
+
+def spp3(cat, co, c1, stream=None):
+    """The three cascaded 5x5 max pools of SPPELAN in place in the bf16 concat buffer cat [N,H,W,cs]."""
+    N, H, W, cs = _nhwc(cat)
+    check(lib().cc_spp3(ptr(cat), N, H, W, cs, co, c1, stream_ptr(stream)), "cc_spp3")
+    return cat
+
+
+def cbfuse(srcs, last, out, C, stream=None):
+    """srcs: list of (buf [N,h,w,cs], co); last, out: (buf [N,H,W,cs], co).  out = sum of nearest-resized sources + last."""
+    n = len(srcs)
+    bufs = [s for s, _ in srcs]
+    for b in bufs + [last[0], out[0]]:
+        _nhwc(b)
+    N, H, W, _ = out[0].shape
+    arr = lambda vals, t=ctypes.c_int: (t * max(n, 1))(*vals)
+    check(lib().cc_cbfuse(int(out[0].dtype == torch.float32), n, arr([b.data_ptr() for b in bufs], ctypes.c_void_p),
+                          arr([b.shape[1] for b in bufs]), arr([b.shape[2] for b in bufs]), arr([b.shape[3] for b in bufs]),
+                          arr([co for _, co in srcs]), ptr(last[0]), last[0].shape[-1], last[1], ptr(out[0]), out[0].shape[-1],
+                          out[1], N, H, W, C, stream_ptr(stream)), "cc_cbfuse")
+    return out[0]
+
+
+def split_planes(x, co, C, stream=None):
+    """x: fp32 [npix, cs] CUDA -> bf16 [npix, 6C] planes lo | mid | hi | mid | hi | hi of channels [co, co + C)."""
+    assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 2
+    out = torch.empty(x.shape[0], 6 * C, dtype=torch.bfloat16, device=x.device)
+    check(lib().cc_split_planes(ptr(x), x.shape[0], x.shape[1], co, C, ptr(out), stream_ptr(stream)), "cc_split_planes")
+    return out
+
+
+def finish_f32(acc, bias, act, out, out_co, res=None, res_co=0, stream=None):
+    """out[:, out_co:out_co+C] = [res[:, res_co:res_co+C] +] act(acc + bias); acc fp32 [npix, C], out / res fp32 [npix, cs]."""
+    npix, C = acc.shape
+    check(lib().cc_finish_f32(ptr(acc), ptr(bias), act, npix, C, ptr(out), out.shape[-1], out_co, ptr(res),
+                              0 if res is None else res.shape[-1], res_co, stream_ptr(stream)), "cc_finish_f32")
+    return out
+
+
+def stem(frames, w, b, obuf, out_co, impl, stream=None):
+    """frames: [B,H,W,3] BGR uint8 | float32 CUDA; w: fp32 [Cout,3,3,3] and b: fp32 [Cout] on the host (PyTorch layout);
+    obuf: [B,H/2,W/2,cs] bf16 | fp32.  impl 1 = stem_tc, 2 = stem_kernel."""
+    B, H, W, _ = frames.shape
+    assert frames.is_cuda and frames.is_contiguous() and frames.dtype in (torch.uint8, torch.float32)
+    w, b = w.detach().float().contiguous().cpu(), b.detach().float().contiguous().cpu()
+    Cout = w.shape[0]
+    args = (ptr(frames), int(frames.dtype == torch.float32), B, H, W, ptr(w), ptr(b), Cout)
+    need = ctypes.c_size_t(0)
+    check(lib().cc_stem(*args, None, obuf.shape[-1], out_co, int(obuf.dtype == torch.float32), impl, None, 0,
+                        ctypes.byref(need), None), "cc_stem")
+    ws = torch.empty(need.value, dtype=torch.uint8, device=frames.device)
+    check(lib().cc_stem(*args, ptr(obuf), obuf.shape[-1], out_co, int(obuf.dtype == torch.float32), impl, ptr(ws), need.value,
+                        None, stream_ptr(stream)), "cc_stem")
+    return obuf
+
+
+def conv2d_pre(xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, Cout, act, pre, bn=0, stream=None):
+    """conv2d on the wgmma kernel plus the half-resolution addend pre (fp32 [N,Ho/2,Wo/2,Cout]) before the activation."""
+    N, H, W, in_cs = _nhwc(xbuf)
+    assert w.dtype == torch.bfloat16 and w.is_contiguous() and pre.dtype == torch.float32 and pre.is_contiguous()
+    check(lib().cc_conv2d_pre(ptr(xbuf), N, H, W, in_cs, in_co, Cin, ptr(w), ptr(bias), Cout, k, stride, ptr(obuf),
+                              obuf.shape[-1], out_co, int(obuf.dtype == torch.float32), act, ptr(pre), bn, stream_ptr(stream)),
+          "cc_conv2d_pre")
+    return obuf
+
+
+def conv2d_fp32_accurate(xbuf, in_co, Cin, w, bias, stride, act, obuf, out_co, res=None, res_co=0, stream=None):
+    """One conv of the detector's fp32-accurate mode.  xbuf / obuf / res: fp32 NHWC CUDA; w: fp32 [Cout,Cin,k,k] and bias
+    fp32 [Cout] (or None) on the host, split into bf16 planes exactly as the detector splits its weights."""
+    N, H, W, in_cs = _nhwc(xbuf)
+    w = w.detach().float().contiguous().cpu()
+    bias = None if bias is None else bias.detach().float().contiguous().cpu()
+    Cout, k = w.shape[0], w.shape[-1]
+    args = (ptr(xbuf), N, H, W, in_cs, in_co, Cin, ptr(w), ptr(bias), Cout, k, stride, act, ptr(res),
+            0 if res is None else res.shape[-1], res_co)
+    need = ctypes.c_size_t(0)
+    check(lib().cc_conv2d_fp32_accurate(*args, None, obuf.shape[-1], out_co, None, 0, ctypes.byref(need), None),
+          "cc_conv2d_fp32_accurate")
+    ws = torch.empty(need.value, dtype=torch.uint8, device=xbuf.device)
+    check(lib().cc_conv2d_fp32_accurate(*args, ptr(obuf), obuf.shape[-1], out_co, ptr(ws), need.value, None,
+                                        stream_ptr(stream)), "cc_conv2d_fp32_accurate")
+    return obuf

@@ -147,6 +147,57 @@ int cc_letterbox(const void* d_in, int frame_fmt, int B, int Hin, int Win, int r
 int cc_attention(const void* d_qkv, int B, int L, int H, int causal, int impl, void* d_ws, size_t ws_bytes, void* d_ctx,
                  size_t* ws_needed, void* stream);
 
+/* The detector's memory-bound kernels as the plan runs them, on caller-owned NHWC slices (ptr, cs, co, C) of N x H x W maps.
+ * f32: 0 = bf16 elements, 1 = fp32 (the fp32-accurate mode's activations).  Slices are 16-byte aligned with cs, co and C
+ * multiples of 8 channels (of 4 for cc_split_planes / cc_finish_f32).  A bad argument fails with CC_ERR_INVALID before
+ * anything is launched.
+ * cc_pool op codes, output extent:
+ *   CC_POOL_AVG2_PAD  avg_pool2d(2, 1) into an H x W map whose last row and column are zero (ADown / AConv), H, W >= 2;
+ *   CC_POOL_AVGMAX    max_pool2d(3, 2, 1) of the stored avg_pool2d(2, 1) map (ADown), H and W even, output H/2 x W/2;
+ *   CC_POOL_MAX5      max_pool2d(5, 1, 2) (SPPELAN), H x W;
+ *   CC_POOL_UPSAMPLE2 nearest x2 (Upsample), output 2H x 2W. */
+#define CC_POOL_AVG2_PAD 0
+#define CC_POOL_AVGMAX 1
+#define CC_POOL_MAX5 2
+#define CC_POOL_UPSAMPLE2 3
+int cc_pool(int op, int f32, const void* d_in, int N, int H, int W, int in_cs, int in_co, int C, void* d_out, int out_cs, int out_co,
+            void* stream);
+/* SPPELAN's three cascaded max_pool2d(5, 1, 2) in one launch, in place in the bf16 concat buffer: channels [co, co + c1)
+ * are pooled into [co + c1, co + 2c1), then [co + 2c1, co + 3c1), then [co + 3c1, co + 4c1).  Only where the map fits shared
+ * memory (H * W <= 800) and c1 is a multiple of 64; otherwise CC_ERR_INVALID. */
+int cc_spp3(void* d_cat, int N, int H, int W, int cs, int co, int c1, void* stream);
+/* CBFuse: out = sum_i nearest_resize(src_i, H x W) + last, summed in source order; 1 to 5 sources of C channels each,
+ * source i of extent src_h[i] x src_w[i] at (d_src[i], src_cs[i], src_co[i]). */
+int cc_cbfuse(int f32, int nsrc, const void* const* d_src, const int* src_h, const int* src_w, const int* src_cs, const int* src_co,
+              const void* d_last, int last_cs, int last_co, void* d_out, int out_cs, int out_co, int N, int H, int W, int C,
+              void* stream);
+/* fp32-accurate mode: an fp32 slice of npix pixels -> dense bf16 [npix][6C] planes [lo | mid | hi | mid | hi | hi], x = hi + mid + lo. */
+int cc_split_planes(const float* d_in, int npix, int cs, int co, int C, void* d_out, void* stream);
+/* fp32-accurate mode, last pass of a conv: out = [res +] act(acc + bias), act 0 or 1 (exact SiLU); d_acc dense [npix][C];
+ * d_bias [C] or NULL; d_res NULL or an fp32 slice. */
+int cc_finish_f32(const float* d_acc, const float* d_bias, int act, int npix, int C, float* d_out, int out_cs, int out_co,
+                  const float* d_res, int res_cs, int res_co, void* stream);
+/* The detector's stem: frame[..., ::-1] / 255 -> conv 3x3 s2 p1 (Cin 3) -> bias -> SiLU.  d_frames [B,H,W,3] BGR, uint8 or
+ * float32 (frame_f32); h_w: HOST fp32 [Cout][3][3][3] (PyTorch layout), h_bias: HOST fp32 [Cout], packed exactly as the
+ * detector packs them; output slice [B,H/2,W/2] of bf16 or fp32 (out_f32).  impl 1 = the tensor-core stem (stem_tc: uint8 frames,
+ * bf16 output, Cout 16, 32 or 64), 2 = the CUDA-core stem_kernel.  d_ws: *ws_needed bytes of device scratch for the packed
+ * weights (16-byte aligned); d_out == NULL only writes *ws_needed. */
+int cc_stem(const void* d_frames, int frame_f32, int B, int H, int W, const float* h_w, const float* h_bias, int Cout, void* d_out,
+            int out_cs, int out_co, int out_f32, int impl, void* d_ws, size_t ws_bytes, size_t* ws_needed, void* stream);
+/* cc_conv2d on the wgmma kernel with the fused Upsample -> Concat addend: out = act(conv(x) + bias + pre[n, h/2, w/2, :]) [the
+ * first conv of a RepNCSPELAN4 after an upsample].  d_pre: dense fp32 [N][Ho/2][Wo/2][Cout]; Ho and Wo even. */
+int cc_conv2d_pre(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const void* d_w, const float* d_bias,
+                  int Cout, int k, int stride, void* d_out, int out_cs, int out_co, int out_f32, int act, const float* d_pre, int bn,
+                  void* stream);
+/* One conv of the fp32-accurate mode, as the detector runs it: the six-plane split of the fp32 input slice, one GEMM per hi x hi
+ * input-channel segment (at most 48 k16 steps each) accumulated in fp32, the cross-product GEMM, then [res +] act(acc + bias).
+ * h_w: HOST fp32 [Cout][Cin][k][k], h_bias: HOST fp32 [Cout] or NULL; k 1 (stride 1) or 3 (stride 1 or 2); act 0 or 1; Cin and Cout
+ * multiples of 16; d_in / d_res / d_out fp32 slices (cs, co multiples of 4).  d_ws: *ws_needed bytes of device scratch (planes,
+ * partial sums, packed weights; 16-byte aligned); d_out == NULL only writes *ws_needed. */
+int cc_conv2d_fp32_accurate(const float* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const float* h_w,
+                            const float* h_bias, int Cout, int k, int stride, int act, const float* d_res, int res_cs, int res_co,
+                            float* d_out, int out_cs, int out_co, void* d_ws, size_t ws_bytes, size_t* ws_needed, void* stream);
+
 /* ---- CLIP image/text encoder (replaces class OpenCLIP, models/objects.py:21-186) ---- */
 typedef struct cc_clip cc_clip;
 typedef struct cc_clip_config {

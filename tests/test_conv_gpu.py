@@ -31,12 +31,18 @@ CASES = [
     (2, 20, 20, 64, 96, 3, 1, 1, False, False, 64, 0, 96, 0, 0),
     (3, 33, 21, 48, 16, 3, 1, 1, False, False, 48, 0, 48, 16, 0),
 ]
+# grouped convs (a 16th field: groups) on the direct kernel at the literal-t widths 24 and 48: the t head's g = 4 convs
+GROUPED_CASES = [(2, 20, 20, 24, 24, 3, 1, 1, False, False, 24, 0, 24, 0, 0, 4),
+                 (1, 40, 40, 48, 48, 3, 1, 1, False, False, 48, 0, 48, 0, 0, 4),
+                 (3, 20, 20, 48, 48, 1, 1, 0, False, True, 48, 0, 48, 0, 0, 4),
+                 (1, 80, 80, 24, 24, 3, 2, 1, True, False, 48, 24, 48, 24, 0, 4)]
 # the CLIP GEMMs as the encoders run them, N = H = 1 and W = token rows (6 x 50, 7 x 77, 3 x 257) at the tower widths:
 # QKV (W -> 3W, bf16 out) and mlp fc (W -> 4W, tanh-GELU); out-proj and fc2 are in test_conv_in_place_residual
 CLIP_ROWS = (300, 539, 771)
 CLIP_WIDTHS = (512, 768, 1024)
 CASES += [(1, 1, rows, W, m * W, 1, 1, act, False, False, W, 0, m * W, 0, 0)
           for rows in CLIP_ROWS for W in CLIP_WIDTHS for m, act in ((3, 0), (4, 2))]
+CASES += GROUPED_CASES
 
 # fp32 outputs against the float64 reference: |got - ref| <= F32_BAR * (sum_k |x_k w_k| + |bias| + |res|) per element,
 # the magnitude the fp32 accumulator and the epilogue's fp32 roundings carry.  Measured on an H100: at most 0.045 x 2^-16
@@ -44,8 +50,8 @@ CASES += [(1, 1, rows, W, m * W, 1, 1, act, False, False, W, 0, m * W, 0, 0)
 F32_BAR = 2.0 ** -18
 
 
-def _ref(x, w, b, k, s, act, res):
-    y = F.conv2d(x.permute(0, 3, 1, 2), w.permute(0, 3, 1, 2), b, stride=s, padding=k // 2)
+def _ref(x, w, b, k, s, act, res, groups=1):
+    y = F.conv2d(x.permute(0, 3, 1, 2), w.permute(0, 3, 1, 2), b, stride=s, padding=k // 2, groups=groups)
     if act == 1:
         y = F.silu(y)
     elif act == 2:
@@ -56,11 +62,11 @@ def _ref(x, w, b, k, s, act, res):
     return y
 
 
-def _check_f32(got, x, w, b, k, s, act, res, what=""):
+def _check_f32(got, x, w, b, k, s, act, res, what="", groups=1):
     """fp32 output vs the float64 reference: the Sum|x.w| bar, and the relative 2e-3 bar where that is tighter."""
     res64 = None if res is None else res.double()
-    ref = _ref(x.double(), w.double(), b.double(), k, s, act, res64)
-    mag = _ref(x.double().abs(), w.double().abs(), b.double().abs(), k, s, 0, None if res is None else res64.abs())
+    ref = _ref(x.double(), w.double(), b.double(), k, s, act, res64, groups)
+    mag = _ref(x.double().abs(), w.double().abs(), b.double().abs(), k, s, 0, None if res is None else res64.abs(), groups)
     err = (got.double() - ref).abs()
     ratio = (err / (F32_BAR * mag)).max().item()
     print(f"{what}: fp32 worst |err|/bar {ratio:.3f}, max rel err {(err / ref.abs().clamp(min=1.0)).max().item():.2e}")
@@ -72,26 +78,29 @@ def _check_f32(got, x, w, b, k, s, act, res, what=""):
 @pytest.mark.parametrize("impl", [1, 2])
 @pytest.mark.parametrize("case", CASES)
 def test_conv_matches_torch(case, impl):
-    N, H, W, Cin, Cout, k, s, act, use_res, out_f32, in_cs, in_co, out_cs, out_co, bn = case
+    N, H, W, Cin, Cout, k, s, act, use_res, out_f32, in_cs, in_co, out_cs, out_co, bn = case[:15]
+    groups = case[15] if len(case) > 15 else 1
     if impl == 2 and N * H * W * Cout * Cin * k * k > 3e10:
         pytest.skip("direct kernel: skip the biggest case")
+    if impl == 1 and groups > 1:
+        pytest.skip("grouped convs run on the direct kernel only")
     g = torch.Generator(device="cuda").manual_seed(1234 + N + H + Cin)
     dev = "cuda"
     xbuf = torch.randn(N, H, W, in_cs, device=dev, generator=g).to(torch.bfloat16)
-    w = (torch.randn(Cout, k, k, Cin, device=dev, generator=g) * (2.0 / (k * k * Cin)) ** 0.5).to(torch.bfloat16)
+    w = (torch.randn(Cout, k, k, Cin // groups, device=dev, generator=g) * (2.0 / (k * k * Cin // groups)) ** 0.5).to(torch.bfloat16)
     b = torch.randn(Cout, device=dev, generator=g) * 0.1
     Ho, Wo = (H // 2, W // 2) if s == 2 else (H, W)
     odt = torch.float32 if out_f32 else torch.bfloat16
     obuf = torch.full((N, Ho, Wo, out_cs), -7.0, device=dev, dtype=odt)
     res = torch.randn(N, Ho, Wo, Cout, device=dev, generator=g).to(odt) if use_res else None
-    ops.conv2d(xbuf, in_co, Cin, w, b, k, s, obuf, out_co, Cout, act=act, res=res, res_co=0, impl=impl, bn=bn)
+    ops.conv2d(xbuf, in_co, Cin, w, b, k, s, obuf, out_co, Cout, act=act, res=res, res_co=0, groups=groups, impl=impl, bn=bn)
     torch.cuda.synchronize()
     x = xbuf[..., in_co:in_co + Cin].float()
     got = obuf[..., out_co:out_co + Cout].float()
     if out_f32:
-        _check_f32(got, x, w.float(), b, k, s, act, res, f"{case} impl {impl}")
+        _check_f32(got, x, w.float(), b, k, s, act, res, f"{case} impl {impl}", groups)
     else:
-        ref = _ref(x, w.float(), b, k, s, act, None if res is None else res.float())
+        ref = _ref(x, w.float(), b, k, s, act, None if res is None else res.float(), groups)
         err = (got - ref).abs()
         scale = ref.abs().clamp(min=1.0)
         assert torch.isfinite(got).all()
