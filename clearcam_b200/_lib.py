@@ -75,6 +75,10 @@ _SIGS = {
     "cc_conv2d_pre": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _i, _vp]),
     "cc_conv2d_fp32_accurate": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp,
                                      ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t), _vp]),
+    "cc_jpeg_bound": (_i, [_i, _i, ctypes.POINTER(ctypes.c_int64)]),
+    "cc_jpeg_encode_crops": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, ctypes.c_int64, _vp, _vp, _vp, ctypes.c_size_t,
+                                  ctypes.POINTER(ctypes.c_size_t), _vp]),
+    "cc_jpeg_coeffs": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, ctypes.POINTER(ctypes.c_int64), _vp]),
 }
 
 

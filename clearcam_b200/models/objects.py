@@ -177,6 +177,32 @@ def search_scores(index, queries) -> torch.Tensor:
     return out
 
 
+def _device_crops(frames, rects, bgr: bool, pix_fmt: str):
+    """The frame / rect conventions of `ObjectFinder.preprocess_device` and `encode_crops`: frames uint8 [n,H,W,3] / [H,W,3]
+    (bgr24) or [n,H*3/2,W] / [H*3/2,W] (yuv420p), host or device; rects K rows of (frame, x1, y1, x2, y2) or (x1, y1, x2,
+    y2).  -> (contiguous device frames [n,...], H, W, the C-ABI src_fmt (0 RGB, 1 BGR, 2 I420), int32 rects [K,5])."""
+    t = frames.tensor if isinstance(frames, DeviceResult) else frames
+    if not isinstance(t, torch.Tensor):
+        t = torch.from_numpy(np.ascontiguousarray(t))
+    if check_pix_fmt(pix_fmt) == BGR24:
+        if t.dim() == 3:
+            t = t.unsqueeze(0)
+        if t.dtype != torch.uint8 or t.dim() != 4 or t.shape[-1] != 3:
+            raise ValueError("frames must be uint8 [n,H,W,3]")
+        H, W, src_fmt = t.shape[1], t.shape[2], 1 if bgr else 0
+    else:
+        if t.dim() == 2:
+            t = t.unsqueeze(0)
+        if t.dtype != torch.uint8 or t.dim() != 3:
+            raise ValueError(f"yuv420p frames must be uint8 [n,H*3/2,W], got {t.dtype} {tuple(t.shape)}")
+        (H, W), src_fmt = yuv420p_size(t.shape), 2
+    t = t.to("cuda", non_blocking=True).contiguous()
+    r = np.asarray(rects, np.int32).reshape(-1, np.shape(rects)[-1] if len(rects) else 5)
+    if r.shape[1] == 4:
+        r = np.concatenate([np.zeros((len(r), 1), np.int32), r], 1)
+    return t, H, W, src_fmt, np.ascontiguousarray(r, np.int32)
+
+
 class ObjectFinder:
     """CLIP half of the reference's ObjectFinder (models/objects.py:188-206, 237-251, 356-421)."""
 
@@ -249,26 +275,7 @@ class ObjectFinder:
         `preprocess(cv2.cvtColor(frame[y1:y2, x1:x2], BGR2RGB))` with OpenCV's own bicubic — without leaving the GPU.
         pix_fmt="yuv420p": frames are uint8 [n,H*3/2,W] or [H*3/2,W] (H, W even; rects in pixels), and the result is
         bit-identical to the same crop of `cv2.cvtColor(frame, COLOR_YUV2RGB_I420)` (`bgr` does not apply)."""
-        t = frames.tensor if isinstance(frames, DeviceResult) else frames
-        if not isinstance(t, torch.Tensor):
-            t = torch.from_numpy(np.ascontiguousarray(t))
-        if check_pix_fmt(pix_fmt) == BGR24:
-            if t.dim() == 3:
-                t = t.unsqueeze(0)
-            if t.dtype != torch.uint8 or t.dim() != 4 or t.shape[-1] != 3:
-                raise ValueError("frames must be uint8 [n,H,W,3]")
-            H, W, src_fmt = t.shape[1], t.shape[2], 1 if bgr else 0
-        else:
-            if t.dim() == 2:
-                t = t.unsqueeze(0)
-            if t.dtype != torch.uint8 or t.dim() != 3:
-                raise ValueError(f"yuv420p frames must be uint8 [n,H*3/2,W], got {t.dtype} {tuple(t.shape)}")
-            (H, W), src_fmt = yuv420p_size(t.shape), 2
-        t = t.to("cuda", non_blocking=True).contiguous()
-        r = np.asarray(rects, np.int32).reshape(-1, np.shape(rects)[-1] if len(rects) else 5)
-        if r.shape[1] == 4:
-            r = np.concatenate([np.zeros((len(r), 1), np.int32), r], 1)
-        r = np.ascontiguousarray(r, np.int32)
+        t, H, W, src_fmt, r = _device_crops(frames, rects, bgr, pix_fmt)
         s = size or (self.model.image_size if self.model is not None else 224)
         # rows > K: the result is allocated with `rows` images, the first K filled and the rest zero (batch padding)
         out = torch.empty(len(r), 3, s, s, device="cuda", dtype=torch.float32) if not rows or rows <= len(r) else \
@@ -288,6 +295,17 @@ class ObjectFinder:
         # bounded set of plans; the padded rows are dropped
         x = self.preprocess_device(frames, rects, bgr, rows=batch_bucket(k), pix_fmt=pix_fmt)
         return DeviceResult(self.model.precompute_embedding(x).tensor[:k])
+
+    def encode_crops(self, frames, rects, quality: int = 95, bgr: bool = True, pix_fmt: str = BGR24) -> List[bytes]:
+        """Detector frame -> the JPEG file of each object crop, encoded on the device: element k is byte for byte what
+        `cv2.imwrite(path, frame[y1:y2, x1:x2])` writes at IMWRITE_JPEG_QUALITY `quality` (`save_object`,
+        clearcam.py:373-399).  frames / rects / bgr / pix_fmt as in `preprocess_device`; a yuv420p frame gives the file of
+        the same crop of `cv2.cvtColor(frame, COLOR_YUV2BGR_I420)`.  Only the encoded bytes cross PCIe."""
+        from .. import ops
+        if not 0 <= int(quality) <= 100:
+            raise ValueError(f"quality must be in 0..100 (cv2's range), got {quality}")
+        t, _, _, src_fmt, r = _device_crops(frames, rects, bgr, pix_fmt)
+        return ops.jpeg_encode_crops(t, r, quality, src_fmt)
 
     def _device_index(self):
         """Contiguous device copy of `image_embeddings` plus, per row, what `search` filters and groups on — rebuilt

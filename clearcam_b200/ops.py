@@ -140,3 +140,73 @@ def conv2d_fp32_accurate(xbuf, in_co, Cin, w, bias, stride, act, obuf, out_co, r
     check(lib().cc_conv2d_fp32_accurate(*args, ptr(obuf), obuf.shape[-1], out_co, ptr(ws), need.value, None,
                                         stream_ptr(stream)), "cc_conv2d_fp32_accurate")
     return obuf
+
+
+# ---- JPEG of frame crops (object thumbnails), byte-identical to cv2.imwrite
+JPEG_SRC_FMTS = {"rgb": 0, "bgr": 1, "i420": 2}
+
+
+def jpeg_bound(w, h):
+    """Worst-case bytes of one encoded w x h crop."""
+    b = ctypes.c_int64(0)
+    check(lib().cc_jpeg_bound(int(w), int(h), ctypes.byref(b)), "cc_jpeg_bound")
+    return b.value
+
+
+def _jpeg_frames(frames, src_fmt):
+    assert frames.is_cuda and frames.dtype == torch.uint8 and frames.is_contiguous()
+    if src_fmt == 2:
+        n, rows, W = frames.shape
+        return n, rows * 2 // 3, W
+    n, H, W, _ = frames.shape
+    return n, H, W
+
+
+def _rects_i32(rects):
+    import numpy as np
+    return np.ascontiguousarray(np.asarray(rects, np.int32).reshape(-1, 5))
+
+
+def jpeg_encode_crops(frames, rects, quality=95, src_fmt=1, stream=None):
+    """frames: uint8 CUDA [n,H,W,3] (src_fmt 0 RGB, 1 BGR) or [n,H*3/2,W] (2 I420); rects: K rows (frame, x1, y1, x2, y2)
+    -> list of K `bytes`, each the file cv2.imwrite writes for that crop at `quality`.  The crops go into one device buffer
+    at offsets given by the prefix sum of their bounds; only the lengths and then the used bytes come back to the host."""
+    import numpy as np
+    n, H, W = _jpeg_frames(frames, src_fmt)
+    r = _rects_i32(rects)
+    K = len(r)
+    if K == 0:
+        return []
+    bounds = np.array([jpeg_bound(x2 - x1, y2 - y1) if x2 > x1 and y2 > y1 else 0 for _, x1, y1, x2, y2 in r], np.int64)
+    offsets = np.ascontiguousarray(np.concatenate([[0], np.cumsum(bounds)[:-1]]).astype(np.int64))
+    need = ctypes.c_size_t(0)
+    args = (ptr(frames), n, H, W, src_fmt, r.ctypes.data, K, int(quality))
+    check(lib().cc_jpeg_encode_crops(*args, None, 0, None, None, None, 0, ctypes.byref(need), None), "cc_jpeg_encode_crops")
+    dev = frames.device
+    out = torch.empty(int(bounds.sum()), dtype=torch.uint8, device=dev)
+    lengths = torch.empty(K, dtype=torch.int64, device=dev)
+    ws = torch.empty(max(need.value, 1), dtype=torch.uint8, device=dev)
+    check(lib().cc_jpeg_encode_crops(*args, ptr(out), out.numel(), offsets.ctypes.data, ptr(lengths), ptr(ws), need.value, None,
+                                     stream_ptr(stream)), "cc_jpeg_encode_crops")
+    lens = lengths.cpu().numpy()
+    # gather the used bytes of every crop into one contiguous device run, then one copy to the host
+    total = int(lens.sum())
+    starts = torch.cumsum(lengths, 0) - lengths
+    idx = torch.arange(total, device=dev) + torch.repeat_interleave(torch.from_numpy(offsets).to(dev) - starts, lengths,
+                                                                     output_size=total)
+    flat = out[idx].cpu().numpy().tobytes()
+    ends = np.cumsum(lens)
+    return [flat[e - l:e] for e, l in zip(ends, lens)]
+
+
+def jpeg_coeffs(frames, rects, quality=95, src_fmt=1, stream=None):
+    """The quantised coefficients of every block of every crop: int16 CUDA [n_blocks, 64], zigzag order, crop by crop, MCU
+    by MCU (Y0 Y1 Y2 Y3 Cb Cr), dummy blocks included (oracle.jpeg.blocks of each crop, concatenated)."""
+    n, H, W = _jpeg_frames(frames, src_fmt)
+    r = _rects_i32(rects)
+    nb = ctypes.c_int64(0)
+    args = (ptr(frames), n, H, W, src_fmt, r.ctypes.data, len(r), int(quality))
+    check(lib().cc_jpeg_coeffs(*args, None, ctypes.byref(nb), None), "cc_jpeg_coeffs")
+    coef = torch.empty(nb.value, 64, dtype=torch.int16, device=frames.device)
+    check(lib().cc_jpeg_coeffs(*args, ptr(coef), ctypes.byref(nb), stream_ptr(stream)), "cc_jpeg_coeffs")
+    return coef

@@ -248,6 +248,26 @@ int cc_search_topk(const float* d_index, int N, int D, const float* d_q, const i
 int cc_clip_preprocess(const uint8_t* d_frames, int n_frames, int H, int W, const int32_t* rects, int K, int size,
                        int src_fmt, float* d_out, void* stream);
 
+/* Object thumbnails on the device: baseline JPEG of frame crops, byte for byte the file cv2.imwrite(path, crop) writes at
+ * IMWRITE_JPEG_QUALITY `quality` (`VideoCapture.save_object`, clearcam.py:373-399): 4:2:0, integer DCT, Annex K tables,
+ * JFIF 1.01 header; oracle/jpeg.py states the arithmetic.  d_frames, n_frames, H, W, src_fmt and the HOST rects [K,5]
+ * (frame, x1, y1, x2, y2) are as in cc_clip_preprocess; the crop is encoded as the BGR image cv2 would see (RGB frames are
+ * swapped, I420 frames converted as cv2.cvtColor(COLOR_YUV2BGR_I420) and then cropped).  quality: 0..100 (0 acts as 1).
+ * cc_jpeg_bound: worst-case bytes of one encoded w x h crop (every code at its longest, every byte stuffed, headers, EOI).
+ * cc_jpeg_encode_crops: crop k is written to d_out + out_offsets[k] (HOST int64 [K]; each region [offset, offset +
+ * cc_jpeg_bound) inside the out_bytes of d_out, none overlapping: the prefix sum of the bounds needs no sync) and its
+ * length to d_lengths[k] (device int64 [K]).  d_workspace: *ws_needed bytes of device scratch, 256-byte aligned.
+ * d_out == NULL only writes *ws_needed.  Nothing is allocated and nothing synchronises; a bad argument fails with
+ * CC_ERR_INVALID before anything is launched.
+ * cc_jpeg_coeffs (parity tap): the quantised coefficients of every 8x8 block of every crop, int16 [n_blocks][64] in zigzag
+ * order: crop by crop, MCU by MCU (Y0 Y1 Y2 Y3 Cb Cr), dummy blocks included.  d_coef == NULL only writes *n_blocks. */
+int cc_jpeg_bound(int w, int h, int64_t* bytes);
+int cc_jpeg_encode_crops(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K, int quality,
+                         uint8_t* d_out, int64_t out_bytes, const int64_t* out_offsets, int64_t* d_lengths, void* d_workspace,
+                         size_t ws_bytes, size_t* ws_needed, void* stream);
+int cc_jpeg_coeffs(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K, int quality,
+                   int16_t* d_coef, int64_t* n_blocks, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Tracker that consumes the detector rows (host code, no GPU): ocsort_tracker/ocsort.py:163-308 `OCSort`, with
  * association.py and kalmanfilter.py.  One handle per camera (clearcam.py:239 `ocsort.OCSort(max_age=100)`).
