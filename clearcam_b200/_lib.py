@@ -79,6 +79,11 @@ _SIGS = {
     "cc_jpeg_encode_crops": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, ctypes.c_int64, _vp, _vp, _vp, ctypes.c_size_t,
                                   ctypes.POINTER(ctypes.c_size_t), _vp]),
     "cc_jpeg_coeffs": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, ctypes.POINTER(ctypes.c_int64), _vp]),
+    "cc_jpeg_table_bytes": (ctypes.c_size_t, []),
+    "cc_jpeg_parse": (_i, [_vp, ctypes.c_int64, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "cc_jpeg_decode": (_i, [_vp, _vp, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t), _vp]),
+    "cc_jpeg_crops_decoded": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, ctypes.c_size_t,
+                                   ctypes.POINTER(ctypes.c_size_t), _vp]),
 }
 
 

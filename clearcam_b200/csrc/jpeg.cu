@@ -700,6 +700,15 @@ int launch_transform(const JpegParams& p, int src_fmt, cudaStream_t st) {
 }
 
 }  // namespace
+
+// the quantisation tables the encoder writes for `quality` (natural order): what a decoder of its files dequantises with
+void jpeg_quant_tables(int quality, uint16_t qt[2][64]) {
+  static thread_local JpegParams p;
+  fill_tables(quality, p);
+  for (int t = 0; t < 2; ++t)
+    for (int i = 0; i < 64; ++i) qt[t][i] = static_cast<uint16_t>(p.qdiv[t][i] / 8);
+}
+
 }  // namespace cc
 
 using namespace cc;

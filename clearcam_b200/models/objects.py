@@ -307,6 +307,74 @@ class ObjectFinder:
         t, _, _, src_fmt, r = _device_crops(frames, rects, bgr, pix_fmt)
         return ops.jpeg_encode_crops(t, r, quality, src_fmt)
 
+    def embed_images(self, items):
+        """The batched device form of `run_clip`'s `preprocess_clip` + `precompute_embedding` (clearcam.py:671-678,
+        models/objects.py:244-251): items are `bytes` (an uploaded file) or the reference's paths relative to data/cameras
+        (stored thumbnails) -> DeviceResult (K, embed_dim).  The files are decoded on the device (ops.jpeg_decode), then
+        cropped, resized and normalised by cc_clip_preprocess and embedded in one batch.  A file the device reports as
+        unsupported or corrupt is decoded by cv2 on the host and joins the same batch; where cv2 returns None this raises as
+        the reference's cvtColor does."""
+        import cv2
+        from .. import ops
+        k = len(items)
+        if k == 0:
+            return DeviceResult(torch.empty(0, self.model.embed_dim, device="cuda", dtype=torch.float32))
+        files = []
+        for it in items:
+            if type(it) == bytes:
+                files.append(it)
+            else:
+                try:
+                    with open(f"data/cameras{it}", "rb") as f:
+                        files.append(f.read())
+                except OSError:
+                    files.append(b"")                   # cv2.imread gives None: raised below
+        batch = ops.JpegBatch(files)
+        host = {}
+
+        def host_decode(i):
+            img = cv2.imdecode(np.frombuffer(files[i], np.uint8), cv2.IMREAD_COLOR) if files[i] else None
+            cv2.cvtColor(img, cv2.COLOR_BGR2RGB)        # raises on None exactly as preprocess_clip does
+            host[i] = img
+
+        for i in np.flatnonzero(batch.status != ops.JPEG_OK):
+            host_decode(int(i))
+        sizes = [(int(w), int(h)) for w, h in batch.sizes]
+        for i, img in host.items():
+            sizes[i] = (img.shape[1], img.shape[0])
+        hmax, wmax = max(h for _, h in sizes), max(w for w, _ in sizes)
+        out, status = batch.decode(hmax=hmax, wmax=wmax)
+        late = [i for i in np.flatnonzero(status.cpu().numpy() != ops.JPEG_OK) if int(i) not in host]
+        for i in late:
+            host_decode(int(i))
+        for i, img in host.items():
+            out[i, :img.shape[0], :img.shape[1]] = torch.from_numpy(img).to(out.device)
+        rects = [(i, 0, 0, w, h) for i, (w, h) in enumerate(sizes)]
+        x = self.preprocess_device(out, rects, bgr=True, rows=batch_bucket(k))
+        return DeviceResult(self.model.precompute_embedding(x).tensor[:k])
+
+    def encode_embed_crops(self, frames, rects, quality: int = 95, bgr: bool = True, pix_fmt: str = BGR24):
+        """Detector frame -> (the JPEG file of each object crop, exactly as `encode_crops` returns them, and DeviceResult
+        (K, embed_dim): the embeddings `clip_latest_img` stores for those files).  The reference writes the crop with
+        cv2.imwrite, reads the file back and embeds the decoded pixels (clearcam.py:272-279, 1278-1287); here the decoded
+        pixels come from the encoder's quantised coefficients on the device (ops.jpeg_crops_decoded), with no host round
+        trip, and are embedded in one batch (a crop whose coefficients the device leaves to cv2 is decoded from its file on
+        the host)."""
+        from .. import ops
+        files = self.encode_crops(frames, rects, quality, bgr, pix_fmt)
+        k = len(files)
+        if k == 0:
+            return files, DeviceResult(torch.empty(0, self.model.embed_dim, device="cuda", dtype=torch.float32))
+        t, _, _, src_fmt, r = _device_crops(frames, rects, bgr, pix_fmt)
+        pix, status = ops.jpeg_crops_decoded(t, r, quality, src_fmt)
+        for i in np.flatnonzero(status.cpu().numpy() != ops.JPEG_OK):
+            import cv2                                  # coefficients outside the range every libjpeg-turbo IDCT agrees on
+            img = cv2.imdecode(np.frombuffer(files[i], np.uint8), cv2.IMREAD_COLOR)
+            pix[i, :img.shape[0], :img.shape[1]] = torch.from_numpy(img).to(pix.device)
+        crops = [(i, 0, 0, int(x2 - x1), int(y2 - y1)) for i, (_, x1, y1, x2, y2) in enumerate(r)]
+        x = self.preprocess_device(pix, crops, bgr=True, rows=batch_bucket(k))
+        return files, DeviceResult(self.model.precompute_embedding(x).tensor[:k])
+
     def _device_index(self):
         """Contiguous device copy of `image_embeddings` plus, per row, what `search` filters and groups on — rebuilt
         whenever a key OR the array stored under a key changes (the fingerprint holds the identity of every value, so an

@@ -210,3 +210,98 @@ def jpeg_coeffs(frames, rects, quality=95, src_fmt=1, stream=None):
     coef = torch.empty(nb.value, 64, dtype=torch.int16, device=frames.device)
     check(lib().cc_jpeg_coeffs(*args, ptr(coef), ctypes.byref(nb), stream_ptr(stream)), "cc_jpeg_coeffs")
     return coef
+
+
+# ---- JPEG files -> BGR pixels, pixel for pixel cv2.imdecode(buf, IMREAD_COLOR)
+JPEG_OK, JPEG_UNSUPPORTED, JPEG_CORRUPT = 0, 1, 2
+
+
+class JpegBatch:
+    """K files parsed on the host and copied to the device once: the files' bytes and the parse table share one pinned
+    buffer and one host-to-device copy."""
+
+    def __init__(self, files, device="cuda"):
+        import numpy as np
+        files = [bytes(f) for f in files]
+        self.K = K = len(files)
+        lengths = np.array([len(f) for f in files], np.int64)
+        offsets = np.concatenate([[0], np.cumsum(lengths)[:-1]]).astype(np.int64) if K else np.zeros(0, np.int64)
+        nbytes = int(lengths.sum())
+        tb = int(lib().cc_jpeg_table_bytes())
+        self.table_off = (nbytes + 255) & ~255
+        host = torch.empty(self.table_off + K * tb, dtype=torch.uint8, pin_memory=torch.cuda.is_available())
+        h = host.numpy()
+        if K:
+            h[:nbytes] = np.frombuffer(b"".join(files), np.uint8)
+        self.sizes = np.zeros((K, 2), np.int32)
+        self.status = np.zeros(K, np.int32)
+        self.blocks = np.zeros(K, np.int64)
+        base = host.data_ptr()
+        check(lib().cc_jpeg_parse(ctypes.c_void_p(base), nbytes, offsets.ctypes.data, lengths.ctypes.data, K,
+                                  ctypes.c_void_p(base + self.table_off), self.sizes.ctypes.data, self.status.ctypes.data,
+                                  self.blocks.ctypes.data), "cc_jpeg_parse")
+        self.host = host
+        self.dev = host.to(device, non_blocking=True)
+
+    def _ptrs(self):
+        return (ctypes.c_void_p(self.dev.data_ptr()), ctypes.c_void_p(self.host.data_ptr() + self.table_off),
+                ctypes.c_void_p(self.dev.data_ptr() + self.table_off))
+
+    def decode(self, out=None, hmax=None, wmax=None, coef=None, stream=None):
+        """-> (out uint8 CUDA [K, Hmax, Wmax, 3], device int32 status [K]).  Image k fills out[k, :h, :w] when its status
+        is JPEG_OK; nothing else of `out` is written."""
+        ok = self.status == JPEG_OK
+        if out is None:
+            hmax = hmax or max([int(v) for v in self.sizes[ok, 1]] + [1])
+            wmax = wmax or max([int(v) for v in self.sizes[ok, 0]] + [1])
+            out = torch.zeros(self.K, hmax, wmax, 3, dtype=torch.uint8, device=self.dev.device)
+        assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.dim() == 4 and out.shape[0] >= self.K
+        status = torch.empty(max(self.K, 1), dtype=torch.int32, device=self.dev.device)
+        d_data, h_table, d_table = self._ptrs()
+        need = ctypes.c_size_t(0)
+        check(lib().cc_jpeg_decode(d_data, h_table, d_table, self.K, None, 0, 0, None, ptr(coef), None, 0, ctypes.byref(need),
+                                   None), "cc_jpeg_decode")
+        ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=self.dev.device)
+        check(lib().cc_jpeg_decode(d_data, h_table, d_table, self.K, ptr(out), out.shape[1], out.shape[2], ptr(status), ptr(coef),
+                                   ptr(ws), ws.numel(), None, stream_ptr(stream)), "cc_jpeg_decode")
+        return out, status[:self.K]
+
+
+def jpeg_decode(files, out=None, stream=None):
+    """files: list of `bytes` -> (out uint8 CUDA [K, Hmax, Wmax, 3] BGR, sizes int32 numpy [K, 2] (width, height), device int32
+    status [K]).  Where status is JPEG_OK, out[k, :h, :w] is exactly cv2.imdecode(file, IMREAD_COLOR); JPEG_UNSUPPORTED and
+    JPEG_CORRUPT images are not written (the caller decodes those with cv2)."""
+    b = JpegBatch(files)
+    o, st = b.decode(out, stream=stream)
+    return o, b.sizes, st
+
+
+def jpeg_decode_coeffs(files, stream=None):
+    """The dequantisation input of every file the host parse accepts: int16 CUDA [n_blocks, 64], zigzag order, block by
+    block in scan order, file after file (the coefficient tap), and the device status."""
+    b = JpegBatch(files)
+    coef = torch.zeros(max(int(b.blocks.sum()), 1), 64, dtype=torch.int16, device=b.dev.device)
+    _, st = b.decode(coef=coef, stream=stream)
+    return coef[:int(b.blocks.sum())], st
+
+
+def jpeg_crops_decoded(frames, rects, quality=95, src_fmt=1, out=None, stream=None):
+    """frames / rects / quality / src_fmt as in jpeg_encode_crops -> (uint8 CUDA [K, Hmax, Wmax, 3], device int32 status [K]):
+    where the status is JPEG_OK, crop k's slot holds, in its h x w corner, the pixels cv2.imdecode gives for the file
+    jpeg_encode_crops writes for it; JPEG_UNSUPPORTED (coefficients outside the range where every libjpeg-turbo IDCT agrees)
+    leaves the slot unwritten, for the caller to decode that file with cv2."""
+    n, H, W = _jpeg_frames(frames, src_fmt)
+    r = _rects_i32(rects)
+    K = len(r)
+    if out is None:
+        hmax = max([int(y2 - y1) for _, _, y1, _, y2 in r] + [1])
+        wmax = max([int(x2 - x1) for _, x1, _, x2, _ in r] + [1])
+        out = torch.zeros(K, hmax, wmax, 3, dtype=torch.uint8, device=frames.device)
+    args = (ptr(frames), n, H, W, src_fmt, r.ctypes.data, K, int(quality))
+    need = ctypes.c_size_t(0)
+    check(lib().cc_jpeg_crops_decoded(*args, None, 0, 0, None, None, 0, ctypes.byref(need), None), "cc_jpeg_crops_decoded")
+    ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=frames.device)
+    status = torch.empty(max(K, 1), dtype=torch.int32, device=frames.device)
+    check(lib().cc_jpeg_crops_decoded(*args, ptr(out), out.shape[1], out.shape[2], ptr(status), ptr(ws), ws.numel(), None,
+                                      stream_ptr(stream)), "cc_jpeg_crops_decoded")
+    return out, status[:K]

@@ -268,6 +268,47 @@ int cc_jpeg_encode_crops(const uint8_t* d_frames, int n_frames, int H, int W, in
 int cc_jpeg_coeffs(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K, int quality,
                    int16_t* d_coef, int64_t* n_blocks, void* stream);
 
+/* JPEG files -> BGR uint8 on the device, pixel for pixel what cv2.imdecode(buf, IMREAD_COLOR) returns (libjpeg-turbo 3.1:
+ * islow IDCT, fancy upsampling, table-driven YCbCr -> BGR); oracle/jpeg_decode.py states the arithmetic.  Replaces the host
+ * decodes of stored thumbnails (clearcam.py:272-279) and of search-by-image uploads (models/objects.py:244-251).
+ * Decoded on the device: baseline and extended sequential Huffman (SOF0 / SOF1), 8-bit, one scan holding every component,
+ * 1 component (grey, replicated to B, G and R) or 3 with luma sampling 1x1, 2x1, 1x2 or 2x2 and chroma 1x1 (4:4:4, 4:2:2,
+ * 4:4:0, 4:2:0), any DQT / DHT tables, restart intervals, APPn / COM skipped.  Every other file gets a status and is left to
+ * the caller (cv2 on the host): CC_JPEG_UNSUPPORTED for progressive, arithmetic, lossless, 12-bit, 4:1:1, CMYK / Adobe RGB,
+ * several scans, an Exif orientation other than 1, a missing Huffman table, or coefficients outside the range where every
+ * libjpeg-turbo IDCT agrees; CC_JPEG_CORRUPT for a malformed header (a marker libjpeg does not know included), an invalid
+ * Huffman code, wrong RSTn markers or a scan that ends before its last MCU.
+ * cc_jpeg_table_bytes: bytes of one image's entry in the parse table.
+ * cc_jpeg_parse (host only): K files at h_data + offsets[k], lengths[k] bytes (all HOST int64 [K], inside data_bytes) ->
+ * h_table (K entries, 16-byte aligned), h_sizes [K,2] = width, height (0 where the header did not say), h_status [K] and
+ * h_blocks [K] (8x8 blocks of each decoded image, 0 for the others).  A file never makes it fail; the entries also place
+ * each image's intermediates in the workspace, so a table belongs to its own set of K files.
+ * cc_jpeg_decode: d_data holds the same bytes as h_data and d_table the same bytes as h_table.  Image k (status OK) is
+ * written to d_out [K, Hmax, Wmax, 3] rows 0..h-1, columns 0..w-1 of slot k; no other byte of d_out is written.  d_status
+ * [K] (device int32) receives the final status: the parse status, or CC_JPEG_CORRUPT / CC_JPEG_UNSUPPORTED found on the
+ * device, in which case that image's region is left as it was and the other images are unaffected.  d_coef: NULL, or
+ * device int16 [sum of h_blocks][64] that receives the dequantisation input (zigzag order, block by block in scan order,
+ * image after image): the coefficient tap.  d_workspace: *ws_needed bytes of device scratch, 256-byte aligned; d_out ==
+ * NULL only writes *ws_needed.  Nothing is allocated and nothing synchronises; a bad argument fails with CC_ERR_INVALID
+ * before anything is launched.
+ * cc_jpeg_crops_decoded: for the crops of cc_jpeg_encode_crops (same frames, rects and quality), the pixels
+ * cv2.imdecode(cv2.imencode(".jpg", crop, quality)) gives: the encoder's transform, then the decoder's reconstruction, with
+ * no entropy coding between them (the coefficients are the file's content).  Crop k goes to slot k of d_out [K, Hmax,
+ * Wmax, 3] as above, and d_status [K] (device int32) gets CC_JPEG_OK, or CC_JPEG_UNSUPPORTED where the coefficients leave
+ * the range in which every libjpeg-turbo IDCT agrees (that slot is then not written; decode the file with cv2).
+ * Workspace as above. */
+#define CC_JPEG_OK 0
+#define CC_JPEG_UNSUPPORTED 1
+#define CC_JPEG_CORRUPT 2
+size_t cc_jpeg_table_bytes(void);
+int cc_jpeg_parse(const uint8_t* h_data, int64_t data_bytes, const int64_t* offsets, const int64_t* lengths, int K, void* h_table,
+                  int32_t* h_sizes, int32_t* h_status, int64_t* h_blocks);
+int cc_jpeg_decode(const uint8_t* d_data, const void* h_table, const void* d_table, int K, uint8_t* d_out, int Hmax, int Wmax,
+                   int32_t* d_status, int16_t* d_coef, void* d_workspace, size_t ws_bytes, size_t* ws_needed, void* stream);
+int cc_jpeg_crops_decoded(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K, int quality,
+                          uint8_t* d_out, int Hmax, int Wmax, int32_t* d_status, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
+                          void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Tracker that consumes the detector rows (host code, no GPU): ocsort_tracker/ocsort.py:163-308 `OCSort`, with
  * association.py and kalmanfilter.py.  One handle per camera (clearcam.py:239 `ocsort.OCSort(max_age=100)`).
