@@ -15,6 +15,15 @@ class CCError(RuntimeError):
     pass
 
 
+# frames per cc_yolo_forward_frames / cc_letterbox_frames call (CC_MAX_FRAMES in include/clearcam_b200.h)
+CC_MAX_FRAMES = 128
+
+
+class cc_frame(ctypes.Structure):
+    """One row of a frame table: device pointer (None = padding row), CC_FRAME_* code, height, width in pixels."""
+    _fields_ = [("data", ctypes.c_void_p), ("fmt", ctypes.c_int), ("h", ctypes.c_int), ("w", ctypes.c_int)]
+
+
 _lib = None
 
 _vp = ctypes.c_void_p
@@ -63,6 +72,10 @@ _SIGS = {
     "cc_ocsort_update_batch": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _vp]),
     "cc_ocsort_num_tracks": (_i, [_vp]),
     "cc_letterbox": (_i, [_vp, _i, _i, _i, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
+    "cc_yolo_net_shape": (_i, [_i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i)]),
+    "cc_yolo_forward_frames": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "cc_yolo_workspace_bytes_frames": (_i, [_vp, _vp, _i, _i, ctypes.POINTER(ctypes.c_size_t)]),
+    "cc_letterbox_frames": (_i, [_vp, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
     "cc_attention": (_i, [_vp, _i, _i, _i, _i, _i, _vp, ctypes.c_size_t, _vp, ctypes.POINTER(ctypes.c_size_t), _vp]),
     "cc_pool": (_i, [_i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
     "cc_spp3": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp]),

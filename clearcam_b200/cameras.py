@@ -10,12 +10,20 @@ to clearcam.py:589 — the (300,6) detector rows and the tracker's targets; zone
 the product's control plane and stay with the caller.
 
 Each camera has a pixel format (clearcam_b200/pixfmt.py): "bgr24" [H,W,3] frames (the default) or "yuv420p" [H*3/2,W]
-frames, which the detector converts on the GPU.  Groups are keyed by (H, W, dtype, format)."""
+frames, which the detector converts on the GPU.  Groups are keyed by (H, W, dtype, format).
+
+With the detector's frame tables (a model with `net_shape` and `detect_frames`), uint8 groups whose frames letterbox to
+the same net input are merged: a fleet of 720p, 1080p, 1440p and 2160p cameras, bgr24 and yuv420p alike, runs as ONE
+batch at res 640 (all of them give a 384 x 640 net input).  A merged group copies each frame into its camera's own
+device buffer and makes one `detect_frames` call per CC_MAX_FRAMES cameras, padded to the batch bucket with None rows.
+A group with a single source shape and format still calls `detect_batch`, as do float32 frames and models without
+frame tables."""
 from typing import Dict, Hashable, List, NamedTuple, Optional
 
 import numpy as np
 import torch
 
+from ._lib import CC_MAX_FRAMES
 from .ocsort_tracker import ocsort
 from .pixfmt import BGR24, check_pix_fmt, yuv420p_size
 from .utils.helpers import batch_bucket
@@ -37,13 +45,18 @@ class _Camera:
 class CameraBatch:
     def __init__(self, model, max_age: int = 100):
         """model: a clearcam_b200 YOLOv9 (anything with detect_batch(frames[B,H,W,3]) -> (B,300,6); for yuv420p cameras
-        also detect_batch(frames[B,H*3/2,W], pix_fmt="yuv420p"))."""
+        also detect_batch(frames[B,H*3/2,W], pix_fmt="yuv420p")).  When it also has net_shape(H, W, pix_fmt=...) and
+        detect_frames(frames, pix_fmts=...), uint8 cameras of different shapes and formats share calls (module doc)."""
         self.model, self.max_age = model, max_age
         self.cams: Dict[Hashable, _Camera] = {}
         self._stage: Dict[tuple, tuple] = {}                   # (H,W,dtype,pix_fmt,bucket) -> (device frame batch, pinned rows)
         self._pin = torch.cuda.is_available()
         self._seen: Dict[Hashable, int] = {}                   # last frame_num taken from each camera's mailbox
         self._where: Dict[Hashable, tuple] = {}                # camera -> (device batch, row) of its frame in the last detect()
+        self._tables = hasattr(model, "net_shape") and hasattr(model, "detect_frames")
+        self._net: Dict[tuple, tuple] = {}                     # (H,W,dtype,pix_fmt) -> (net_h, net_w)
+        self._cam_dev: Dict[Hashable, torch.Tensor] = {}       # camera -> its device frame buffer (merged groups)
+        self._table_rows: Dict[tuple, torch.Tensor] = {}       # (net_h, net_w, chunk, bucket) -> pinned rows
 
     # -- camera set (clearcam.py:207-240 init_cam; settings threshold :584, class filter :586)
     def add_camera(self, name, thresh: float = 0.5, classes=None, pix_fmt: str = BGR24):
@@ -54,6 +67,7 @@ class CameraBatch:
     def remove_camera(self, name):
         self.cams.pop(name, None)
         self._where.pop(name, None)
+        self._cam_dev.pop(name, None)
         self._seen.pop(name, None)             # a re-added camera starts a new mailbox whose frame_num restarts at 0
 
     def reset_tracker(self, name):
@@ -100,13 +114,41 @@ class CameraBatch:
                               torch.empty((k[-1], 300, 6), dtype=torch.float32, pin_memory=self._pin))
         return self._stage[k]
 
+    def merge_groups(self, groups: Dict[tuple, List[Hashable]]) -> List[tuple]:
+        """Shape groups -> [(net shape or None, [shape keys])]: with frame tables, the uint8 groups of one net shape go
+        together; float32 groups (and every group without frame tables) stay alone with net shape None."""
+        merged: Dict[tuple, tuple] = {}
+        for key in groups:
+            H, W, dt, fmt = key
+            if not self._tables or dt != "|u1":
+                merged[("shape",) + key] = (None, [key])
+                continue
+            if key not in self._net:
+                self._net[key] = tuple(self.model.net_shape(H, W, pix_fmt=fmt))
+            net = self._net[key]
+            merged.setdefault(("net",) + net, (net, []))[1].append(key)
+        return list(merged.values())
+
+    def _camera_buffer(self, name, f) -> torch.Tensor:
+        buf = self._cam_dev.get(name)
+        if buf is None or tuple(buf.shape) != tuple(f.shape):
+            buf = self._cam_dev[name] = torch.empty(tuple(f.shape), dtype=torch.uint8, device="cuda" if self._pin else "cpu")
+        return buf
+
     def detect(self, frames: Dict[Hashable, np.ndarray]) -> Dict[Hashable, np.ndarray]:
-        """Detector only: {camera: HWC frame} -> {camera: (300,6) rows}.  One batched call per distinct frame shape.
-        Each frame goes host -> its row of the device batch directly (asynchronously when it lives in pinned memory, e.g. a
-        FrameMailbox slot): no host-side stacking copy."""
+        """Detector only: {camera: HWC frame} -> {camera: (300,6) rows}.  One batched call per distinct frame shape, or
+        with frame tables per distinct net shape (module doc).
+        Each frame goes host -> its row of the device batch (or its camera's device buffer) directly (asynchronously when it
+        lives in pinned memory, e.g. a FrameMailbox slot): no host-side stacking copy."""
         pending = []
         fmts = {name: cam.pix_fmt for name, cam in self.cams.items() if cam.pix_fmt != BGR24}
-        for key, names in self.group_by_shape(frames, fmts).items():
+        groups = self.group_by_shape(frames, fmts)
+        for net, keys in self.merge_groups(groups):
+            if len(keys) > 1:
+                pending += self._detect_table(net, [(name, key[3]) for key in keys for name in groups[key]], frames)
+                continue
+            key = keys[0]
+            names = groups[key]
             dev, rows = self._buffers(key, len(names))
             for i, name in enumerate(names):
                 f = frames[name]
@@ -119,6 +161,29 @@ class CameraBatch:
         if self._pin:
             torch.cuda.current_stream().synchronize()
         return {name: rows[i].numpy().copy() for names, rows in pending for i, name in enumerate(names)}
+
+    def _detect_table(self, net, cams, frames) -> list:
+        """One detect_frames call per CC_MAX_FRAMES cameras of one net shape; cams: [(camera, pix_fmt)]."""
+        pending = []
+        for c0 in range(0, len(cams), CC_MAX_FRAMES):
+            chunk = cams[c0:c0 + CC_MAX_FRAMES]
+            devs = []
+            for name, _ in chunk:
+                f = frames[name]
+                buf = self._camera_buffer(name, f)
+                buf.copy_(f if isinstance(f, torch.Tensor) else torch.from_numpy(f), non_blocking=True)
+                self._where[name] = (buf.unsqueeze(0), 0)
+                devs.append(buf)
+            b = self.bucket(len(chunk))
+            out = self.model.detect_frames(devs + [None] * (b - len(chunk)),
+                                           pix_fmts=[fmt for _, fmt in chunk] + [BGR24] * (b - len(chunk)))
+            k = tuple(net) + (c0 // CC_MAX_FRAMES, b)
+            if k not in self._table_rows:
+                self._table_rows[k] = torch.empty((b, 300, 6), dtype=torch.float32, pin_memory=self._pin)
+            rows = self._table_rows[k]
+            rows.copy_(out, non_blocking=True)
+            pending.append(([name for name, _ in chunk], rows))
+        return pending
 
     def device_frame(self, name) -> torch.Tensor:
         """The device copy of the frame camera `name` contributed to the last detect()/step(), in the camera's own format

@@ -142,7 +142,10 @@ __device__ __forceinline__ unsigned long long make_key(float prob, int idx) {
          static_cast<unsigned long long>(0xFFFFFFFFu - static_cast<unsigned>(idx));
 }
 
-__global__ void __launch_bounds__(kPostThreads) postprocess_kernel(PostParams p) {
+// scale_boxes of image b: s[b * stride] (stride 0: one entry for the whole batch)
+struct PostScales { PostScale s[CC_MAX_FRAMES]; int stride; };
+
+__global__ void __launch_bounds__(kPostThreads) postprocess_kernel(PostParams p, const __grid_constant__ PostScales sc) {
   __shared__ unsigned int hist[256];
   __shared__ unsigned long long sel[kMaxDet];
   __shared__ float rows[kMaxDet][6];
@@ -240,10 +243,11 @@ __global__ void __launch_bounds__(kPostThreads) postprocess_kernel(PostParams p)
     const float k = keep ? 1.f : 0.f;
     float x1 = __fmul_rn(jx1, k), y1 = __fmul_rn(jy1, k), x2 = __fmul_rn(jx2, k), y2 = __fmul_rn(jy2, k);
     if (p.do_scale) {
-      x1 = fminf(fmaxf(__fdiv_rn(__fsub_rn(x1, p.pad_x), p.gain), 0.f), p.clip_w);
-      x2 = fminf(fmaxf(__fdiv_rn(__fsub_rn(x2, p.pad_x), p.gain), 0.f), p.clip_w);
-      y1 = fminf(fmaxf(__fdiv_rn(__fsub_rn(y1, p.pad_y), p.gain), 0.f), p.clip_h);
-      y2 = fminf(fmaxf(__fdiv_rn(__fsub_rn(y2, p.pad_y), p.gain), 0.f), p.clip_h);
+      const PostScale& g = sc.s[b * sc.stride];
+      x1 = fminf(fmaxf(__fdiv_rn(__fsub_rn(x1, g.pad_x), g.gain), 0.f), g.clip_w);
+      x2 = fminf(fmaxf(__fdiv_rn(__fsub_rn(x2, g.pad_x), g.gain), 0.f), g.clip_w);
+      y1 = fminf(fmaxf(__fdiv_rn(__fsub_rn(y1, g.pad_y), g.gain), 0.f), g.clip_h);
+      y2 = fminf(fmaxf(__fdiv_rn(__fsub_rn(y2, g.pad_y), g.gain), 0.f), g.clip_h);
     }
     o[0] = x1; o[1] = y1; o[2] = x2; o[3] = y2;
     o[4] = __fmul_rn(rows[j][4], k);
@@ -251,10 +255,19 @@ __global__ void __launch_bounds__(kPostThreads) postprocess_kernel(PostParams p)
   }
 }
 
-int postprocess_launch(const PostParams& p, cudaStream_t s) {
+int postprocess_launch(const PostParams& p, cudaStream_t s, const PostScale* per_image) {
   CC_REQUIRE(p.max_det >= 1 && p.max_det <= kMaxDet, "postprocess: max_det must be in [1,%d]", kMaxDet);
+  CC_REQUIRE(!per_image || p.B <= CC_MAX_FRAMES, "postprocess: %d per-image scales (at most %d)", p.B, CC_MAX_FRAMES);
   if (p.B == 0) return CC_OK;
-  postprocess_kernel<<<p.B, kPostThreads, 0, s>>>(p);
+  PostScales sc{};
+  if (per_image) {
+    for (int b = 0; b < p.B; ++b) sc.s[b] = per_image[b];
+    sc.stride = 1;
+  } else {
+    sc.s[0] = p.scale;
+    sc.stride = 0;
+  }
+  postprocess_kernel<<<p.B, kPostThreads, 0, s>>>(p, sc);
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;
 }

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+#include "clearcam_b200.h"
 
 namespace cc {
 
@@ -82,7 +83,20 @@ struct LetterboxParams {
   int B, Hin, Win, Hr, Wr, pad_y, pad_x, Hout, Wout;   // resized extent, pads, final extent
   float sx, sy;                                        // float(Win/Wr), float(Hin/Hr) computed in double on the host
 };
+// B frames of one shape and format (in = the first, the others follow contiguously) -> [B,Hout,Wout,3]
 int letterbox_launch(const LetterboxParams& p, cudaStream_t s);
+// The same kernel driven by a per-image table (frames of different shapes and formats into one [B,Hout,Wout,3] batch).  The
+// table travels as the kernel parameter: no copy, no allocation, no sync.
+struct LetterboxFrame {
+  const void* in;                                      // the frame, or nullptr: a padding image, written as zeros
+  int fmt, Hin, Win, Hr, Wr, pad_y, pad_x;
+  float sx, sy;
+};
+struct LetterboxTable {
+  void* out; int B, Hout, Wout, out_f32;               // out: float32 when out_f32 (CC_FRAME_BGR_F32 frames), else uint8
+  LetterboxFrame f[CC_MAX_FRAMES];
+};
+int letterbox_frames_launch(const LetterboxTable& t, cudaStream_t s);
 
 // Stem: frame[..., ::-1]/255 -> Conv 3x3 s2 p1 (Cin=3) -> bias -> SiLU -> NHWC bf16
 // (detection/yolov9.py:378-379 fused into model[0] / model[1],model[15] of size e).  fp32 weights [Cout][3][3][3] (RGB order).
@@ -126,12 +140,15 @@ int decode_launch(const DecodeParams& p, cudaStream_t s);
 int pred_from_raw_launch(const float* raw, int B, int A, int nc, float conf_thr, float* pred, cudaStream_t s);
 
 // postprocess tail (detection/yolov9.py:449-458) + scale_boxes/clip_boxes (:406-421), one CTA per image.
+struct PostScale { float pad_x, pad_y, gain, clip_w, clip_h; };   // scale_boxes of one image
 struct PostParams {
   const float* pred; int B, A; int max_det; float iou_thr;
-  float pad_x, pad_y, gain, clip_w, clip_h; int do_scale;
+  PostScale scale; int do_scale;              // one scale_boxes for the whole batch
   float* out;                                 // [B,max_det,6]
 };
-int postprocess_launch(const PostParams& p, cudaStream_t s);
+// per_image: NULL (every image takes p.scale), or B <= CC_MAX_FRAMES entries, image b taking per_image[b]; either way the
+// scales reach the kernel as a parameter table
+int postprocess_launch(const PostParams& p, cudaStream_t s, const PostScale* per_image = nullptr);
 
 // ---- CLIP ViT kernels (vit.cu) ----
 int patchify_launch(const float* x, __nv_bfloat16* out, int B, int S, int p, int Kpad, cudaStream_t st);

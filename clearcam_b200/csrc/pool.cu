@@ -457,14 +457,14 @@ __device__ __forceinline__ int lerp_u8(int a, int b, int wi) {
   int diff = ((b - a + 128) & 255) - 128;     // int8 wrap-around of the reference's uint8 subtraction
   return (a + ((diff * wi + 64) >> 7)) & 255;
 }
-// FMT: CC_FRAME_* code of the source, a template argument so the per-pixel path has no format branch
+// One image of the batch.  FMT: CC_FRAME_* code of its frame, a template argument so the per-pixel path has no format
+// branch (the kernel picks the instance once per CTA: a CTA covers one image).  out: the image's [Hout,Wout,3] slot.
 template <int FMT>
-__global__ void letterbox_kernel(LetterboxParams p) {
-  const long long total = static_cast<long long>(p.B) * p.Hout * p.Wout;
+__device__ __forceinline__ void letterbox_image(const LetterboxFrame& p, int Hout, int Wout, void* out) {
+  const long long total = static_cast<long long>(Hout) * Wout;
   CC_GRID_STRIDE(idx, total) {
-    const int x = static_cast<int>(idx % p.Wout);
-    const int y = static_cast<int>((idx / p.Wout) % p.Hout);
-    const int n = static_cast<int>(idx / (static_cast<long long>(p.Wout) * p.Hout));
+    const int x = static_cast<int>(idx % Wout);
+    const int y = static_cast<int>(idx / Wout);
     const int ry = y - p.pad_y, rx = x - p.pad_x;
     const bool inside = ry >= 0 && ry < p.Hr && rx >= 0 && rx < p.Wr;
     int xl = 0, xh = 0, yl = 0, yh = 0;
@@ -474,8 +474,8 @@ __global__ void letterbox_kernel(LetterboxParams p) {
       if (p.Hr != p.Hin) lerp_idx(ry, p.Hin, p.sy, yl, yh, wy); else { yl = yh = ry; }
     }
     if constexpr (FMT == CC_FRAME_BGR_F32) {
-      const float* src = static_cast<const float*>(p.in) + static_cast<long long>(n) * p.Hin * p.Win * 3;
-      float* dst = static_cast<float*>(p.out) + idx * 3;
+      const float* src = static_cast<const float*>(p.in);
+      float* dst = static_cast<float*>(out) + idx * 3;
       for (int c = 0; c < 3; ++c) {
         float r = 0.f;
         if (inside) {
@@ -488,20 +488,20 @@ __global__ void letterbox_kernel(LetterboxParams p) {
         dst[c] = r;
       }
     } else {
-      uint8_t* dst = static_cast<uint8_t*>(p.out) + idx * 3;
+      uint8_t* dst = static_cast<uint8_t*>(out) + idx * 3;
       const int wxi = static_cast<int>(static_cast<short>(wx * 128.f + 0.5f));
       const int wyi = static_cast<int>(static_cast<short>(wy * 128.f + 0.5f));
       // the four taps as BGR: a = (yl,xl), b = (yl,xh), d = (yh,xl), e = (yh,xh)
       int a[3] = {0, 0, 0}, b[3] = {0, 0, 0}, d[3] = {0, 0, 0}, e[3] = {0, 0, 0};
       if (inside) {
         if constexpr (FMT == CC_FRAME_I420_U8) {
-          const uint8_t* src = static_cast<const uint8_t*>(p.in) + static_cast<long long>(n) * p.Hin * p.Win * 3 / 2;
+          const uint8_t* src = static_cast<const uint8_t*>(p.in);
           i420_bgr(src, p.Hin, p.Win, yl, xl, a);
           i420_bgr(src, p.Hin, p.Win, yl, xh, b);
           i420_bgr(src, p.Hin, p.Win, yh, xl, d);
           i420_bgr(src, p.Hin, p.Win, yh, xh, e);
         } else {
-          const uint8_t* src = static_cast<const uint8_t*>(p.in) + static_cast<long long>(n) * p.Hin * p.Win * 3;
+          const uint8_t* src = static_cast<const uint8_t*>(p.in);
           for (int c = 0; c < 3; ++c) {
             a[c] = src[(static_cast<long long>(yl) * p.Win + xl) * 3 + c]; b[c] = src[(static_cast<long long>(yl) * p.Win + xh) * 3 + c];
             d[c] = src[(static_cast<long long>(yh) * p.Win + xl) * 3 + c]; e[c] = src[(static_cast<long long>(yh) * p.Win + xh) * 3 + c];
@@ -521,19 +521,62 @@ __global__ void letterbox_kernel(LetterboxParams p) {
     }
   }
 }
-int letterbox_launch(const LetterboxParams& p, cudaStream_t s) {
-  const long long total = static_cast<long long>(p.B) * p.Hout * p.Wout;
-  const int g = grid_for(total, 256);
-  switch (p.fmt) {
-    case CC_FRAME_BGR_U8: letterbox_kernel<CC_FRAME_BGR_U8><<<g, 256, 0, s>>>(p); break;
-    case CC_FRAME_BGR_F32: letterbox_kernel<CC_FRAME_BGR_F32><<<g, 256, 0, s>>>(p); break;
-    case CC_FRAME_I420_U8:
-      CC_REQUIRE(p.Hin % 2 == 0 && p.Win % 2 == 0, "letterbox: I420 frame %dx%d has an odd side", p.Hin, p.Win);
-      letterbox_kernel<CC_FRAME_I420_U8><<<g, 256, 0, s>>>(p);
-      break;
-    default: CC_REQUIRE(false, "letterbox: unknown frame format %d", p.fmt);
+// blockIdx.y = image of the table; x covers its pixels
+__global__ void __launch_bounds__(256) letterbox_kernel(const __grid_constant__ LetterboxTable t) {
+  const LetterboxFrame& f = t.f[blockIdx.y];
+  const long long img = static_cast<long long>(t.Hout) * t.Wout * 3;
+  void* out = t.out_f32 ? static_cast<void*>(static_cast<float*>(t.out) + blockIdx.y * img)
+                        : static_cast<void*>(static_cast<uint8_t*>(t.out) + blockIdx.y * img);
+  if (!f.in) {                                   // padding image
+    if (t.out_f32) { float* o = static_cast<float*>(out); CC_GRID_STRIDE(i, img) o[i] = 0.f; }
+    else { uint8_t* o = static_cast<uint8_t*>(out); CC_GRID_STRIDE(i, img) o[i] = 0; }
+    return;
   }
+  switch (f.fmt) {
+    case CC_FRAME_BGR_F32: letterbox_image<CC_FRAME_BGR_F32>(f, t.Hout, t.Wout, out); break;
+    case CC_FRAME_I420_U8: letterbox_image<CC_FRAME_I420_U8>(f, t.Hout, t.Wout, out); break;
+    default: letterbox_image<CC_FRAME_BGR_U8>(f, t.Hout, t.Wout, out); break;
+  }
+}
+int letterbox_frames_launch(const LetterboxTable& t, cudaStream_t s) {
+  CC_REQUIRE(t.B >= 1 && t.B <= CC_MAX_FRAMES && t.Hout > 0 && t.Wout > 0 && t.out, "letterbox: bad table (B=%d, %dx%d)", t.B, t.Hout, t.Wout);
+  for (int i = 0; i < t.B; ++i) {
+    const LetterboxFrame& f = t.f[i];
+    if (!f.in) continue;
+    CC_REQUIRE((f.fmt == CC_FRAME_BGR_F32) == (t.out_f32 != 0) && (f.fmt == CC_FRAME_BGR_U8 || f.fmt == CC_FRAME_BGR_F32 || f.fmt == CC_FRAME_I420_U8),
+               "letterbox: image %d has frame format %d (out_f32 %d)", i, f.fmt, t.out_f32);
+    CC_REQUIRE(f.fmt != CC_FRAME_I420_U8 || (f.Hin % 2 == 0 && f.Win % 2 == 0), "letterbox: I420 frame %dx%d has an odd side", f.Hin, f.Win);
+    CC_REQUIRE(f.pad_y >= 0 && f.pad_x >= 0 && f.Hr >= 0 && f.Wr >= 0 &&f.pad_y + f.Hr <= t.Hout && f.pad_x + f.Wr <= t.Wout,
+               "letterbox: image %d (%dx%d at %d,%d) does not fit %dx%d", i, f.Hr, f.Wr, f.pad_y, f.pad_x, t.Hout, t.Wout);
+  }
+  // as many CTAs in all as the batch-wide grid-stride launch it replaces (grid_for's cap), at least one per image
+  const long long per_img = (static_cast<long long>(t.Hout) * t.Wout + 255) / 256;
+  long long gx = 132LL * 32 / t.B;
+  gx = gx < 1 ? 1 : (gx > per_img ? per_img : gx);
+  letterbox_kernel<<<dim3(static_cast<unsigned>(gx), t.B), 256, 0, s>>>(t);
   CC_CHECK_CUDA(cudaGetLastError());
+  return CC_OK;
+}
+int letterbox_launch(const LetterboxParams& p, cudaStream_t s) {
+  CC_REQUIRE(p.fmt == CC_FRAME_BGR_U8 || p.fmt == CC_FRAME_BGR_F32 || p.fmt == CC_FRAME_I420_U8, "letterbox: unknown frame format %d", p.fmt);
+  CC_REQUIRE(p.fmt != CC_FRAME_I420_U8 || (p.Hin % 2 == 0 && p.Win % 2 == 0), "letterbox: I420 frame %dx%d has an odd side", p.Hin, p.Win);
+  const bool f32 = p.fmt == CC_FRAME_BGR_F32;
+  const long long hw = static_cast<long long>(p.Hin) * p.Win;
+  const long long in_bytes = f32 ? hw * 12 : p.fmt == CC_FRAME_I420_U8 ? hw * 3 / 2 : hw * 3;
+  const long long out_bytes = static_cast<long long>(p.Hout) * p.Wout * 3 * (f32 ? 4 : 1);
+  LetterboxTable t;
+  t.Hout = p.Hout; t.Wout = p.Wout; t.out_f32 = f32 ? 1 : 0;
+  for (int b0 = 0; b0 < p.B; b0 += CC_MAX_FRAMES) {          // the table holds CC_MAX_FRAMES images per launch
+    t.B = p.B - b0 < CC_MAX_FRAMES ? p.B - b0 : CC_MAX_FRAMES;
+    t.out = static_cast<uint8_t*>(p.out) + b0 * out_bytes;
+    for (int i = 0; i < t.B; ++i) {
+      LetterboxFrame& f = t.f[i];
+      f.in = static_cast<const uint8_t*>(p.in) + (b0 + i) * in_bytes;
+      f.fmt = p.fmt; f.Hin = p.Hin; f.Win = p.Win; f.Hr = p.Hr; f.Wr = p.Wr; f.pad_y = p.pad_y; f.pad_x = p.pad_x;
+      f.sx = p.sx; f.sy = p.sy;
+    }
+    if (int rc = letterbox_frames_launch(t, s)) return rc;
+  }
   return CC_OK;
 }
 

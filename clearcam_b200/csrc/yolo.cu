@@ -216,6 +216,42 @@ static void split_weight_planes(const float* wf, size_t rows, int cin, const std
   }
 }
 
+// ---- letterbox geometry of one Hf x Wf frame at `res` (detection/yolov9.py:390-404, scale_boxes :406-421), shared by the plan
+// builder, cc_letterbox, the frame-table path and cc_yolo_net_shape
+struct LbGeom {
+  int new_h = 0, new_w = 0, py = 0, px = 0;   // resized extent, pads
+  int Hr = 0, Wr = 0;                         // the reference's letterboxed extent
+  int H = 0, W = 0;                           // the net input: Hr x Wr rounded up to a multiple of 32
+  float sx = 0.f, sy = 0.f;                   // float(Wf / new_w), float(Hf / new_h), computed in double
+  PostScale scale{};                          // scale_boxes back to the frame
+};
+static LbGeom letterbox_geom(int Hf, int Wf, int res) {
+  LbGeom g;
+  const double r = std::min(double(res) / Hf, double(res) / Wf);
+  g.new_w = int(std::nearbyint(Wf * r)); g.new_h = int(std::nearbyint(Hf * r));
+  const double dw = double(((res - g.new_w) % 32 + 32) % 32) / 2, dh = double(((res - g.new_h) % 32 + 32) % 32) / 2;
+  g.px = int(std::nearbyint(dw - 0.1)); g.py = int(std::nearbyint(dh - 0.1));
+  // The reference pads int(round(d - 0.1)) on BOTH sides, so when (res - new) % 32 is odd its net input is one pixel short of
+  // a multiple of 32 (SURVEY App. A5) — and it keeps going: a 3x3/s2/p1 conv over 2k-1 rows gives the same k output rows as
+  // over 2k rows whose last row is zero.  So the net input buffer is rounded up to the multiple of 32 with that zero row /
+  // column (the letterbox kernel pads with zeros anyway): identical arithmetic, even dims for the TMA views.  scale_boxes
+  // still sees the reference's odd extent (Hr, Wr).
+  g.Hr = g.new_h + 2 * g.py; g.Wr = g.new_w + 2 * g.px;
+  g.H = (g.Hr + 31) / 32 * 32; g.W = (g.Wr + 31) / 32 * 32;
+  g.sx = float(double(Wf) / double(g.new_w)); g.sy = float(double(Hf) / double(g.new_h));
+  const double gain = std::min(double(g.Hr) / Hf, double(g.Wr) / Wf);   // the reference's img1_shape (detection/yolov9.py:406-416)
+  g.scale.gain = float(gain);
+  g.scale.pad_x = float((g.Wr - Wf * gain) / 2); g.scale.pad_y = float((g.Hr - Hf * gain) / 2);
+  g.scale.clip_w = float(Wf); g.scale.clip_h = float(Hf);
+  return g;
+}
+// the detector runs a frame only when its letterboxed extent is within one pixel of a multiple of 32 (res a multiple of 32)
+static int require_net(const LbGeom& g, int Hf, int Wf, int res) {
+  CC_REQUIRE(g.H > 0 && g.W > 0 && g.H - g.Hr <= 1 && g.W - g.Wr <= 1,
+             "yolo: letterboxed input %dx%d is not within one pixel of a multiple of 32 (frame %dx%d, res %d)", g.Hr, g.Wr, Hf, Wf, res);
+  return CC_OK;
+}
+
 struct T { __nv_bfloat16* p = nullptr; int cs = 0, co = 0, C = 0, H = 0, W = 0; bool image = false; bool f32 = false; };   // f32: p is really float*
 
 struct Op {
@@ -237,6 +273,10 @@ struct Op {
 struct YoloPlan {
   int B = 0, Hf = 0, Wf = 0, res = 0, fmt = 0, H = 0, W = 0, A = 0;    // fmt: CC_FRAME_* of the frames
   int Hr = 0, Wr = 0;          // the reference's letterboxed extent (H, W are it rounded up to a multiple of 32)
+  // frame-table plan (cc_yolo_forward_frames): Hf x Wf is the net shape itself, the frames come with every call.  Its op list
+  // has no letterbox (launched by the caller with the call's table into lb_out) and ends with the postprocess (launched with
+  // the call's per-image scales); in between it is the op list of a uniform plan of the net shape.
+  bool table = false;
   std::vector<Op> ops;
   size_t alloc_bytes = 0;      // bytes of the handle's shared workspace this plan addresses
   uint64_t gen = 0;            // workspace generation the pointers / TMA descriptors were built against
@@ -253,6 +293,7 @@ struct YoloPlan {
   cudaGraphExec_t gexec = nullptr;
   const void* g_frames = nullptr; float* g_out = nullptr; float* g_raw = nullptr;      // pointers the graph was captured with
   const void* l_frames = nullptr; float* l_out = nullptr; float* l_raw = nullptr;      // pointers of the previous call
+  bool ran = false;            // a previous call exists (a frame-table plan passes null frames / out pointers every time)
   ~YoloPlan() { if (gexec) cudaGraphExecDestroy(gexec); }
 };
 
@@ -586,37 +627,30 @@ int Builder::build() {
     }
 
   // ---- preprocess (detection/yolov9.py:390-404)
-  const double r = std::min(double(P.res) / P.Hf, double(P.res) / P.Wf);
-  const int new_w = int(std::nearbyint(P.Wf * r)), new_h = int(std::nearbyint(P.Hf * r));
-  double dw = double((P.res - new_w) % 32), dh = double((P.res - new_h) % 32);
-  if (dw < 0) dw += 32;
-  if (dh < 0) dh += 32;
-  dw /= 2; dh /= 2;
-  const int px = int(std::nearbyint(dw - 0.1)), py = int(std::nearbyint(dh - 0.1));
-  // The reference pads int(round(d - 0.1)) on BOTH sides, so when (res - new) % 32 is odd its net input is one pixel short of
-  // a multiple of 32 (SURVEY App. A5) — and it keeps going: a 3x3/s2/p1 conv over 2k-1 rows gives the same k output rows as
-  // over 2k rows whose last row is zero.  So the net input buffer is rounded up to the multiple of 32 with that zero row /
-  // column (the letterbox kernel pads with zeros anyway): identical arithmetic, even dims for the TMA views.  scale_boxes
-  // still sees the reference's odd extent (Hr, Wr below).
-  const int Hr = new_h + 2 * py, Wr = new_w + 2 * px;
-  P.H = (Hr + 31) / 32 * 32; P.W = (Wr + 31) / 32 * 32;
-  P.Hr = Hr; P.Wr = Wr;
-  CC_REQUIRE(P.H > 0 && P.W > 0 && P.H - Hr <= 1 && P.W - Wr <= 1,
-             "yolo: letterboxed input %dx%d is not within one pixel of a multiple of 32 (frame %dx%d, res %d)", Hr, Wr, P.Hf, P.Wf, P.res);
+  LbGeom g;                       // a frame-table plan has no frame geometry of its own (the postprocess gets it per call)
+  if (P.table) {
+    P.H = P.Hr = P.Hf; P.W = P.Wr = P.Wf;
+  } else {
+    g = letterbox_geom(P.Hf, P.Wf, P.res);
+    if (int e = require_net(g, P.Hf, P.Wf, P.res)) return e;
+    P.H = g.H; P.W = g.W; P.Hr = g.Hr; P.Wr = g.Wr;
+  }
   const void* net_in = nullptr;   // filled per run when identity (frames pointer) -> patched in run()
   const bool f32 = P.fmt == CC_FRAME_BGR_F32;
-  // the stems read HWC BGR: I420 frames always go through the letterbox, which converts them (an identity resize included)
-  if (P.fmt == CC_FRAME_I420_U8 || !(new_w == P.Wf && new_h == P.Hf && px == 0 && py == 0 && P.H == Hr && P.W == Wr)) {
+  // the stems read HWC BGR: I420 frames always go through the letterbox, which converts them (an identity resize included);
+  // a frame-table plan always letterboxes into lb_out (its frames are not one tensor)
+  const bool identity = g.new_w == P.Wf && g.new_h == P.Hf && g.px == 0 && g.py == 0 && P.H == g.Hr && P.W == g.Wr;
+  if (P.table || P.fmt == CC_FRAME_I420_U8 || !identity) {
     const size_t es = f32 ? 4 : 1;
     P.lb_out = dalloc(static_cast<size_t>(P.B) * P.H * P.W * 3 * es);
     net_in = P.lb_out;
-    if (!bump.dry) {
+    if (!bump.dry && !P.table) {
     Op op; op.kind = Op::LETTERBOX; op.name = "letterbox";
     op.lb = LetterboxParams{};
     op.lb.in = nullptr; op.lb.out = P.lb_out; op.lb.fmt = P.fmt;
-    op.lb.B = P.B; op.lb.Hin = P.Hf; op.lb.Win = P.Wf; op.lb.Hr = new_h; op.lb.Wr = new_w;
-    op.lb.pad_y = py; op.lb.pad_x = px; op.lb.Hout = P.H; op.lb.Wout = P.W;
-    op.lb.sx = float(double(P.Wf) / double(new_w)); op.lb.sy = float(double(P.Hf) / double(new_h));
+    op.lb.B = P.B; op.lb.Hin = P.Hf; op.lb.Win = P.Wf; op.lb.Hr = g.new_h; op.lb.Wr = g.new_w;
+    op.lb.pad_y = g.py; op.lb.pad_x = g.px; op.lb.Hout = P.H; op.lb.Wout = P.W;
+    op.lb.sx = g.sx; op.lb.sy = g.sy;
     P.ops.push_back(std::move(op));
     }
   }
@@ -850,11 +884,7 @@ int Builder::build() {
         Op po; po.kind = Op::POST; po.name = "postprocess";
         po.post = PostParams{};
         po.post.pred = P.pred; po.post.B = P.B; po.post.A = A; po.post.max_det = 300; po.post.iou_thr = 0.45f;
-        const int Hr = P.Hr, Wr = P.Wr;               // the reference's img1_shape (detection/yolov9.py:406-416)
-        const double gain = std::min(double(Hr) / P.Hf, double(Wr) / P.Wf);
-        po.post.gain = float(gain);
-        po.post.pad_x = float((Wr - P.Wf * gain) / 2); po.post.pad_y = float((Hr - P.Hf * gain) / 2);
-        po.post.clip_w = float(P.Wf); po.post.clip_h = float(P.Hf); po.post.do_scale = 1;
+        po.post.scale = g.scale; po.post.do_scale = 1;
         po.post.out = nullptr;
         P.ops.push_back(std::move(po));
         break;
@@ -867,10 +897,14 @@ int Builder::build() {
   return rc;
 }
 
+// ops [first, last) of the plan (all of them by default)
 static int plan_run(YoloPlan& P, const void* d_frames, float* d_out, float* d_raw, cudaStream_t st,
-                    std::vector<cudaEvent_t>* ev = nullptr, unsigned long long* d_trace = nullptr) {
+                    std::vector<cudaEvent_t>* ev = nullptr, unsigned long long* d_trace = nullptr, size_t first = 0,
+                    size_t last = SIZE_MAX) {
   size_t oi = 0, ti = 0;
-  for (Op& op : P.ops) {
+  if (last > P.ops.size()) last = P.ops.size();
+  for (size_t k = first; k < last; ++k) {
+    Op& op = P.ops[k];
     int rc = CC_OK;
     if (ev) cudaEventRecord((*ev)[oi++], st);
     switch (op.kind) {
@@ -1061,15 +1095,17 @@ static int check_frame_fmt(const char* who, int fmt, int Hf, int Wf) {
   return CC_OK;
 }
 
-static std::string plan_key(int fmt, int B, int Hf, int Wf, int res) {
+// table: a frame-table plan (Hf x Wf = the net shape, fmt = CC_FRAME_BGR_U8: what its letterbox writes)
+static std::string plan_key(int fmt, int B, int Hf, int Wf, int res, bool table) {
   char key[96];
-  snprintf(key, sizeof(key), "%d,%d,%d,%d,%d", fmt, B, Hf, Wf, res);
+  snprintf(key, sizeof(key), "%s%d,%d,%d,%d,%d", table ? "table:" : "", fmt, B, Hf, Wf, res);
   return key;
 }
 // workspace bytes a plan of this shape addresses (measuring pass of the builder: no device work)
-static int plan_bytes(cc_yolo* h, int fmt, int B, int Hf, int Wf, int res, size_t* bytes, size_t* scratch = nullptr, size_t* accb = nullptr) {
+static int plan_bytes(cc_yolo* h, int fmt, int B, int Hf, int Wf, int res, size_t* bytes, size_t* scratch = nullptr, size_t* accb = nullptr,
+                      bool table = false) {
   YoloPlan tmp;
-  tmp.B = B; tmp.Hf = Hf; tmp.Wf = Wf; tmp.res = res; tmp.fmt = fmt;
+  tmp.B = B; tmp.Hf = Hf; tmp.Wf = Wf; tmp.res = res; tmp.fmt = fmt; tmp.table = table;
   Builder dry(h->m, tmp);
   dry.bump.dry = true;
   int rc = dry.build();
@@ -1079,9 +1115,9 @@ static int plan_bytes(cc_yolo* h, int fmt, int B, int Hf, int Wf, int res, size_
   if (accb) *accb = dry.max_acc;
   return CC_OK;
 }
-static int get_plan(cc_yolo* h, int fmt, int B, int Hf, int Wf, int res, YoloPlan** out) {
+static int get_plan(cc_yolo* h, int fmt, int B, int Hf, int Wf, int res, YoloPlan** out, bool table = false) {
   YoloModel& M = h->m;
-  const std::string key = plan_key(fmt, B, Hf, Wf, res);
+  const std::string key = plan_key(fmt, B, Hf, Wf, res, table);
   auto it = M.plans.find(key);
   if (it != M.plans.end() && it->second->gen == M.arena.gen) {
     it->second->last_use = ++M.tick;
@@ -1089,14 +1125,14 @@ static int get_plan(cc_yolo* h, int fmt, int B, int Hf, int Wf, int res, YoloPla
     return CC_OK;
   }
   size_t bytes = 0, scratch = 0, accb = 0;
-  int rc = plan_bytes(h, fmt, B, Hf, Wf, res, &bytes, &scratch, &accb);
+  int rc = plan_bytes(h, fmt, B, Hf, Wf, res, &bytes, &scratch, &accb, table);
   if (rc) return rc;
   if ((rc = M.arena.reserve(bytes))) return rc;
   // plans built against an older workspace are stale (they are rebuilt on their next use)
   for (auto p = M.plans.begin(); p != M.plans.end();)
     p = (p->second->gen != M.arena.gen) ? M.plans.erase(p) : std::next(p);
   std::unique_ptr<YoloPlan> P(new YoloPlan());
-  P->B = B; P->Hf = Hf; P->Wf = Wf; P->res = res; P->fmt = fmt;
+  P->B = B; P->Hf = Hf; P->Wf = Wf; P->res = res; P->fmt = fmt; P->table = table;
   Builder bld(M, *P);
   bld.bump.base = static_cast<uint8_t*>(M.arena.base);
   bld.scratch_bytes = scratch;
@@ -1130,22 +1166,19 @@ int cc_yolo_set_workspace(cc_yolo* h, void* d_workspace, size_t bytes) {
   return h->m.arena.adopt(d_workspace, bytes);
 }
 
-int cc_yolo_forward(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, float* d_out,
-                    float* d_raw, void* stream) {
-  CC_REQUIRE(h && d_frames && d_out && B > 0 && Hf > 0 && Wf > 0 && res > 0, "cc_yolo_forward: bad argument");
-  if (int rc = check_frame_fmt("cc_yolo_forward", frame_fmt, Hf, Wf)) return rc;
-  YoloPlan* P = nullptr;
-  int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P);
-  if (rc) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+// Runs ops [first, last) of the plan on `st`: from its CUDA graph once the caller has passed the same (frames, out, raw)
+// pointers twice in a row, else launch by launch.
+static int run_graphed(cc_yolo* h, YoloPlan* P, const void* d_frames, float* d_out, float* d_raw, cudaStream_t st, size_t first = 0,
+                       size_t last = SIZE_MAX) {
+  int rc = CC_OK;
   static const int graph_env = getenv("CC_GRAPH") ? atoi(getenv("CC_GRAPH")) : 1;
   if (graph_env) {
     if (P->gexec && P->g_frames == d_frames && P->g_out == d_out && P->g_raw == d_raw) {
       CC_CHECK_CUDA(cudaGraphLaunch(P->gexec, st));
       return CC_OK;
     }
-    const bool stable = P->l_frames == d_frames && P->l_out == d_out && P->l_raw == d_raw;
-    P->l_frames = d_frames; P->l_out = d_out; P->l_raw = d_raw;
+    const bool stable = P->ran && P->l_frames == d_frames && P->l_out == d_out && P->l_raw == d_raw;
+    P->l_frames = d_frames; P->l_out = d_out; P->l_raw = d_raw; P->ran = true;
     if (stable) {
       // second call in a row with these pointers: capture the launch list (on a private stream: nothing executes) and replay
       if (!h->m.cap_stream) CC_CHECK_CUDA(cudaStreamCreateWithFlags(&h->m.cap_stream, cudaStreamNonBlocking));
@@ -1153,7 +1186,7 @@ int cc_yolo_forward(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int 
       cudaGraph_t g = nullptr;
       bool ok = cudaStreamBeginCapture(h->m.cap_stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
       if (ok) {
-        rc = plan_run(*P, d_frames, d_out, d_raw, h->m.cap_stream);
+        rc = plan_run(*P, d_frames, d_out, d_raw, h->m.cap_stream, nullptr, nullptr, first, last);
         ok = cudaStreamEndCapture(h->m.cap_stream, &g) == cudaSuccess && rc == CC_OK && g != nullptr;
       }
       if (ok) ok = cudaGraphInstantiate(&P->gexec, g, 0) == cudaSuccess;
@@ -1167,7 +1200,95 @@ int cc_yolo_forward(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int 
       P->gexec = nullptr;
     }
   }
-  return plan_run(*P, d_frames, d_out, d_raw, st);
+  return plan_run(*P, d_frames, d_out, d_raw, st, nullptr, nullptr, first, last);
+}
+
+int cc_yolo_forward(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, float* d_out,
+                    float* d_raw, void* stream) {
+  CC_REQUIRE(h && d_frames && d_out && B > 0 && Hf > 0 && Wf > 0 && res > 0, "cc_yolo_forward: bad argument");
+  if (int rc = check_frame_fmt("cc_yolo_forward", frame_fmt, Hf, Wf)) return rc;
+  YoloPlan* P = nullptr;
+  int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P);
+  if (rc) return rc;
+  return run_graphed(h, P, d_frames, d_out, d_raw, static_cast<cudaStream_t>(stream));
+}
+
+// ---- frame tables: every frame's geometry, the shared net shape, and the letterbox table of a call
+static int table_geometry(const char* who, const cc_frame* frames, int B, int res, std::vector<LbGeom>* geo, int* net_h, int* net_w) {
+  CC_REQUIRE(frames && B >= 1 && B <= CC_MAX_FRAMES && res > 0, "%s: bad argument (B=%d must be in [1, %d], res %d)", who, B,
+             CC_MAX_FRAMES, res);
+  geo->assign(B, LbGeom{});
+  int H = 0, W = 0, first = -1;
+  for (int b = 0; b < B; ++b) {
+    const cc_frame& f = frames[b];
+    if (!f.data) continue;
+    CC_REQUIRE(f.fmt == CC_FRAME_BGR_U8 || f.fmt == CC_FRAME_I420_U8,
+               "%s: frame %d has format %d; a frame table takes CC_FRAME_BGR_U8 (0) or CC_FRAME_I420_U8 (2) frames", who, b, f.fmt);
+    CC_REQUIRE(f.h > 0 && f.w > 0, "%s: frame %d is %dx%d", who, b, f.h, f.w);
+    if (int rc = check_frame_fmt(who, f.fmt, f.h, f.w)) return rc;
+    const LbGeom g = letterbox_geom(f.h, f.w, res);
+    if (int rc = require_net(g, f.h, f.w, res)) return rc;
+    if (first < 0) { first = b; H = g.H; W = g.W; }
+    CC_REQUIRE(g.H == H && g.W == W, "%s: frame %d (%dx%d) has net shape %dx%d, frame %d has %dx%d: one call takes one net shape",
+               who, b, f.h, f.w, g.H, g.W, first, H, W);
+    (*geo)[b] = g;
+  }
+  CC_REQUIRE(first >= 0, "%s: every one of the %d frames is a padding row", who, B);
+  *net_h = H; *net_w = W;
+  return CC_OK;
+}
+static void table_letterbox(const cc_frame* frames, int B, const std::vector<LbGeom>& geo, int H, int W, void* out, LetterboxTable* t) {
+  t->out = out; t->B = B; t->Hout = H; t->Wout = W; t->out_f32 = 0;
+  for (int b = 0; b < B; ++b) {
+    const LbGeom& g = geo[b];
+    LetterboxFrame& f = t->f[b];
+    f = LetterboxFrame{};
+    f.in = frames[b].data;
+    if (!f.in) continue;
+    f.fmt = frames[b].fmt; f.Hin = frames[b].h; f.Win = frames[b].w; f.Hr = g.new_h; f.Wr = g.new_w;
+    f.pad_y = g.py; f.pad_x = g.px; f.sx = g.sx; f.sy = g.sy;
+  }
+}
+
+int cc_yolo_net_shape(int frame_fmt, int Hf, int Wf, int res, int* net_h, int* net_w) {
+  CC_REQUIRE(Hf > 0 && Wf > 0 && res > 0 && net_h && net_w, "cc_yolo_net_shape: bad argument (%dx%d, res %d)", Hf, Wf, res);
+  if (int rc = check_frame_fmt("cc_yolo_net_shape", frame_fmt, Hf, Wf)) return rc;
+  const LbGeom g = letterbox_geom(Hf, Wf, res);
+  if (int rc = require_net(g, Hf, Wf, res)) return rc;
+  *net_h = g.H; *net_w = g.W;
+  return CC_OK;
+}
+
+int cc_yolo_workspace_bytes_frames(cc_yolo* h, const cc_frame* frames, int B, int res, size_t* bytes) {
+  CC_REQUIRE(h && bytes, "cc_yolo_workspace_bytes_frames: bad argument");
+  std::vector<LbGeom> geo;
+  int H = 0, W = 0;
+  if (int rc = table_geometry("cc_yolo_workspace_bytes_frames", frames, B, res, &geo, &H, &W)) return rc;
+  return plan_bytes(h, CC_FRAME_BGR_U8, B, H, W, res, bytes, nullptr, nullptr, true);
+}
+
+int cc_yolo_forward_frames(cc_yolo* h, const cc_frame* frames, int B, int res, float* d_out, float* d_raw, void* stream) {
+  CC_REQUIRE(h && d_out, "cc_yolo_forward_frames: bad argument");
+  std::vector<LbGeom> geo;
+  int H = 0, W = 0;
+  if (int rc = table_geometry("cc_yolo_forward_frames", frames, B, res, &geo, &H, &W)) return rc;
+  YoloPlan* P = nullptr;
+  if (int rc = get_plan(h, CC_FRAME_BGR_U8, B, H, W, res, &P, true)) return rc;
+  CC_REQUIRE(!P->ops.empty() && P->ops.back().kind == Op::POST && P->lb_out, "cc_yolo_forward_frames: plan without postprocess");
+  LetterboxTable t;
+  table_letterbox(frames, B, geo, H, W, P->lb_out, &t);
+  std::vector<PostScale> scales(B);
+  for (int b = 0; b < B; ++b)
+    if (frames[b].data) scales[b] = geo[b].scale;
+    else scales[b] = PostScale{0.f, 0.f, 1.f, 0.f, 0.f};     // a padding row: boxes clipped to 0
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // the letterbox and the postprocess take this call's tables as kernel parameters; the ops between them read and write only
+  // the workspace (and d_raw), so their graph does not depend on the table
+  if (int rc = letterbox_frames_launch(t, st)) return rc;
+  if (int rc = run_graphed(h, P, nullptr, nullptr, d_raw, st, 0, P->ops.size() - 1)) return rc;
+  PostParams q = P->ops.back().post;
+  q.out = d_out;
+  return postprocess_launch(q, st, scales.data());
 }
 
 int cc_yolo_plan_info(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int* net_h, int* net_w, int* anchors,
@@ -1288,7 +1409,7 @@ int cc_detect_postprocess(const float* d_pred, int B, int A, int max_det, float 
                           float pad_y, float gain, float clip_w, float clip_h, float* d_out, void* stream) {
   PostParams p{};
   p.pred = d_pred; p.B = B; p.A = A; p.max_det = max_det; p.iou_thr = iou_thr;
-  p.do_scale = do_scale; p.pad_x = pad_x; p.pad_y = pad_y; p.gain = gain; p.clip_w = clip_w; p.clip_h = clip_h;
+  p.do_scale = do_scale; p.scale = PostScale{pad_x, pad_y, gain, clip_w, clip_h};
   p.out = d_out;
   return postprocess_launch(p, static_cast<cudaStream_t>(stream));
 }
@@ -1313,18 +1434,27 @@ int cc_detect_decode(const float* const* d_box, const float* const* d_cls, const
 int cc_letterbox(const void* d_in, int frame_fmt, int B, int Hin, int Win, int res, void* d_out, int* out_h, int* out_w,
                  void* stream) {
   if (int rc = check_frame_fmt("cc_letterbox", frame_fmt, Hin, Win)) return rc;
-  const double r = std::min(double(res) / Hin, double(res) / Win);
-  const int new_w = int(std::nearbyint(Win * r)), new_h = int(std::nearbyint(Hin * r));
-  double dw = double(((res - new_w) % 32 + 32) % 32) / 2, dh = double(((res - new_h) % 32 + 32) % 32) / 2;
-  const int px = int(std::nearbyint(dw - 0.1)), py = int(std::nearbyint(dh - 0.1));
-  if (out_h) *out_h = new_h + 2 * py;
-  if (out_w) *out_w = new_w + 2 * px;
+  const LbGeom g = letterbox_geom(Hin, Win, res);
+  if (out_h) *out_h = g.Hr;
+  if (out_w) *out_w = g.Wr;
   if (!d_out) return CC_OK;   // size query
   LetterboxParams p{};
-  p.in = d_in; p.out = d_out; p.fmt = frame_fmt; p.B = B; p.Hin = Hin; p.Win = Win; p.Hr = new_h; p.Wr = new_w;
-  p.pad_y = py; p.pad_x = px; p.Hout = new_h + 2 * py; p.Wout = new_w + 2 * px;
-  p.sx = float(double(Win) / double(new_w)); p.sy = float(double(Hin) / double(new_h));
+  p.in = d_in; p.out = d_out; p.fmt = frame_fmt; p.B = B; p.Hin = Hin; p.Win = Win; p.Hr = g.new_h; p.Wr = g.new_w;
+  p.pad_y = g.py; p.pad_x = g.px; p.Hout = g.Hr; p.Wout = g.Wr;
+  p.sx = g.sx; p.sy = g.sy;
   return letterbox_launch(p, static_cast<cudaStream_t>(stream));
+}
+
+int cc_letterbox_frames(const cc_frame* frames, int B, int res, void* d_out, int* net_h, int* net_w, void* stream) {
+  std::vector<LbGeom> geo;
+  int H = 0, W = 0;
+  if (int rc = table_geometry("cc_letterbox_frames", frames, B, res, &geo, &H, &W)) return rc;
+  if (net_h) *net_h = H;
+  if (net_w) *net_w = W;
+  if (!d_out) return CC_OK;   // size query
+  LetterboxTable t;
+  table_letterbox(frames, B, geo, H, W, d_out, &t);
+  return letterbox_frames_launch(t, static_cast<cudaStream_t>(stream));
 }
 
 static size_t al256(size_t b) { return (b + 255) & ~size_t(255); }

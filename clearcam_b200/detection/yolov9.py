@@ -10,22 +10,23 @@ kernels) through ctypes; torch tensors are only device containers.  There is no 
 library or without an H100 every call raises CCError.
 
 Differences the reference cannot express (additions): `detect_batch(frames[B,H,W,3])`, explicit `weights=`
-(the reference downloads from HuggingFace at construction, :372; there is no network here), and `pix_fmt="yuv420p"`:
+(the reference downloads from HuggingFace at construction, :372; there is no network here), `pix_fmt="yuv420p"`:
 frames as a camera decodes them, uint8 [H*3/2,W] (a batch [B,H*3/2,W]), converted to BGR on the GPU bit-exactly as
-cv2.cvtColor(COLOR_YUV2BGR_I420) would (clearcam_b200/pixfmt.py).
+cv2.cvtColor(COLOR_YUV2BGR_I420) would (clearcam_b200/pixfmt.py), and `detect_frames([...])`: frames of different
+shapes and formats in one batch, as long as they letterbox to the same net input (`net_shape`).
 """
 from __future__ import annotations
 
 import ctypes
 import os
-from typing import Dict, Optional
+from typing import Dict, Optional, Tuple
 
 import numpy as np
 import torch
 
 from . import padding
-from .._lib import CCError, check, lib, ptr, stream_ptr
-from ..pixfmt import BGR24, CC_FRAME_BGR_F32, CC_FRAME_BGR_U8, CC_FRAME_I420_U8, check_pix_fmt, yuv420p_size
+from .._lib import CC_MAX_FRAMES, CCError, cc_frame, check, lib, ptr, stream_ptr
+from ..pixfmt import BGR24, CC_FRAME_BGR_F32, CC_FRAME_BGR_U8, CC_FRAME_I420_U8, check_pix_fmt, yuv420p_rows, yuv420p_size
 
 
 # ----------------------------------------------------------------------------------------------- helpers
@@ -77,6 +78,56 @@ def _frame_code(t: torch.Tensor, pix_fmt: str) -> int:
     if check_pix_fmt(pix_fmt) == BGR24:
         return CC_FRAME_BGR_F32 if t.dtype == torch.float32 else CC_FRAME_BGR_U8
     return CC_FRAME_I420_U8
+
+
+def net_shape(H: int, W: int, res: int, pix_fmt: str = BGR24) -> Tuple[int, int]:
+    """(net_h, net_w): the detector's input extent for an H x W frame at `res` — the letterboxed extent of
+    YOLOv9.preprocess rounded up to a multiple of 32.  Frames with the same net shape can share one `detect_frames`
+    batch (720p, 1080p, 1440p and 2160p all give (384, 640) at res 640).  Host only, needs no GPU."""
+    if check_pix_fmt(pix_fmt) != BGR24:
+        yuv420p_rows(int(H), int(W))                # ValueError for odd sides
+    code = CC_FRAME_BGR_U8 if pix_fmt == BGR24 else CC_FRAME_I420_U8
+    nh, nw = ctypes.c_int(), ctypes.c_int()
+    check(lib().cc_yolo_net_shape(code, int(H), int(W), int(res), ctypes.byref(nh), ctypes.byref(nw)), "cc_yolo_net_shape")
+    return nh.value, nw.value
+
+
+def frame_table(frames, pix_fmts, res: int):
+    """Validate a list of device frames for one frame-table call -> (ctypes cc_frame array, (net_h, net_w)).
+    frames: uint8 CUDA tensors, [H,W,3] for "bgr24" or [H*3/2,W] for "yuv420p", or None for a padding row; pix_fmts: one
+    format for all, or one per frame.  Raises ValueError before any library call that launches work."""
+    frames = list(frames)
+    B = len(frames)
+    fmts = [pix_fmts] * B if isinstance(pix_fmts, str) else list(pix_fmts)
+    if len(fmts) != B:
+        raise ValueError(f"{B} frames but {len(fmts)} pixel formats")
+    if not 1 <= B <= CC_MAX_FRAMES:
+        raise ValueError(f"a frame table holds 1 to {CC_MAX_FRAMES} frames, got {B}")
+    table = (cc_frame * B)()
+    net = None
+    for i, (f, fmt) in enumerate(zip(frames, fmts)):
+        check_pix_fmt(fmt)
+        if f is None:
+            continue
+        if not isinstance(f, torch.Tensor) or not f.is_cuda or f.dtype != torch.uint8 or not f.is_contiguous():
+            raise ValueError(f"frame {i}: expected a contiguous uint8 CUDA tensor, got "
+                             f"{type(f).__name__} {getattr(f, 'dtype', '')} {tuple(getattr(f, 'shape', ()))}")
+        if fmt == BGR24:
+            if f.dim() != 3 or f.shape[2] != 3:
+                raise ValueError(f"frame {i}: a bgr24 frame is [H,W,3], got {tuple(f.shape)}")
+            H, W = int(f.shape[0]), int(f.shape[1])
+        else:
+            if f.dim() != 2:
+                raise ValueError(f"frame {i}: a yuv420p frame is [H*3/2,W], got {tuple(f.shape)}")
+            H, W = yuv420p_size(f.shape)
+        ns = net_shape(H, W, res, fmt)
+        if net is not None and ns != net:
+            raise ValueError(f"frame {i} ({H}x{W}) has net shape {ns}, an earlier frame {net}: one call takes one net shape")
+        net = ns
+        table[i] = cc_frame(f.data_ptr(), CC_FRAME_BGR_U8 if fmt == BGR24 else CC_FRAME_I420_U8, H, W)
+    if net is None:
+        raise ValueError("every frame of the table is a padding row (None)")
+    return table, net
 
 
 def safe_load(path) -> Dict[str, torch.Tensor]:
@@ -236,6 +287,28 @@ class YOLOv9:
             rawt = torch.empty(B, 84, A, device="cuda", dtype=torch.float32)
         check(lib().cc_yolo_forward(self._h, ptr(t), code, B, Hf, Wf, self.res, ptr(out), ptr(rawt), stream_ptr(stream)),
               "cc_yolo_forward")
+        return (out, rawt) if raw else out
+
+    def net_shape(self, H: int, W: int, pix_fmt: str = BGR24) -> Tuple[int, int]:
+        """(net_h, net_w) of an H x W frame at this model's res: frames with equal net shapes can share a
+        `detect_frames` call."""
+        return net_shape(H, W, self.res, pix_fmt)
+
+    def detect_frames(self, frames, pix_fmts=BGR24, raw: bool = False, stream=None):
+        """Frames of different shapes and formats in one batch.  frames: a list of B <= CC_MAX_FRAMES (128) device uint8
+        tensors, [H,W,3] bgr24 or [H*3/2,W] yuv420p as `pix_fmts` says (one format, or one per frame), None for a padding
+        row; every frame must have the same `net_shape`.  Returns the device tensor (B,300,6): row b is frame b's
+        detections in its own pixels, what `detect_batch` of B frames of its shape and format gives at row b (and the
+        (B,84,A) head tap when raw=True).  Shapes and formats are checked before the library is called (ValueError)."""
+        table, (nh, nw) = frame_table(frames, pix_fmts, self.res)
+        B = len(table)
+        out = torch.empty(B, 300, 6, device="cuda", dtype=torch.float32)
+        rawt = None
+        if raw:
+            A = sum((nh // s) * (nw // s) for s in (8, 16, 32))
+            rawt = torch.empty(B, 84, A, device="cuda", dtype=torch.float32)
+        check(lib().cc_yolo_forward_frames(self._h, ctypes.cast(table, ctypes.c_void_p), B, self.res, ptr(out), ptr(rawt),
+                                           stream_ptr(stream)), "cc_yolo_forward_frames")
         return (out, rawt) if raw else out
 
     def detect_pipelined(self, host_batches, depth: int = 2, pix_fmt: str = BGR24):

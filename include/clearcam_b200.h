@@ -87,6 +87,25 @@ int cc_yolo_destroy(cc_yolo* h);
  * analogue of jit_infer's per-shape TinyJit cache (utils/helpers.py:214-221); later calls only launch kernels. */
 int cc_yolo_forward(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, float* d_out,
                     float* d_raw, void* stream);
+/* Frames of different shapes and formats in one forward.  Every camera whose frames letterbox to the same net input
+ * (720p, 1080p, 1440p and 2160p all give 384 x 640 at res 640) runs in one batch: the letterbox reads a per-frame table,
+ * the conv stack is that of a uniform batch of the net shape, and scale_boxes takes each frame's own geometry.
+ * cc_frame: data = device pointer to one frame (CC_FRAME_BGR_U8 [h,w,3] or CC_FRAME_I420_U8 [h*3/2,w], h and w even), or
+ * NULL for a padding row (letterboxed as zeros; its output rows mean nothing).  At most CC_MAX_FRAMES frames per call. */
+#define CC_MAX_FRAMES 128
+typedef struct { const void* data; int fmt; int h; int w; } cc_frame;
+/* The net input extent (the letterboxed extent rounded up to a multiple of 32) of an Hf x Wf frame at `res`: the key under
+ * which frames can share a batch.  Host only: needs no GPU. */
+int cc_yolo_net_shape(int frame_fmt, int Hf, int Wf, int res, int* net_h, int* net_w);
+/* cc_yolo_forward over a table of B frames (HOST array, read during the call only) that share one net shape; row b of
+ * d_out [B,300,6] is frame b's detections in its own pixels, as cc_yolo_forward of a batch of frames of its shape and
+ * format would give it at that row.  d_raw: optional [B,84,A] head tap.  Mixed net shapes, CC_FRAME_BGR_F32 frames, odd
+ * I420 sides, no frame at all or B > CC_MAX_FRAMES fail with CC_ERR_INVALID before anything is launched.  Plans are
+ * cached per (B, net shape, res); the letterbox and the postprocess take the table as a kernel parameter on every call and
+ * the CUDA graph covers the launches between them, so a different table every call still replays the graph. */
+int cc_yolo_forward_frames(cc_yolo* h, const cc_frame* frames, int B, int res, float* d_out, float* d_raw, void* stream);
+int cc_yolo_workspace_bytes_frames(cc_yolo* h, const cc_frame* frames, int B, int res, size_t* bytes);
+
 /* plan facts: letterboxed net input size, anchors, kernel launches per forward, algorithmic conv FLOPs,
  * bytes of activation workspace */
 int cc_yolo_plan_info(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int* net_h, int* net_w, int* anchors,
@@ -138,6 +157,10 @@ int cc_detect_decode(const float* const* d_box, const float* const* d_cls, const
  * converted to BGR at each bilinear tap).  d_out == NULL only queries the output size. */
 int cc_letterbox(const void* d_in, int frame_fmt, int B, int Hin, int Win, int res, void* d_out, int* out_h, int* out_w,
                  void* stream);
+/* The same for a table of B frames sharing one net shape (cc_yolo_forward_frames' rules): frame b is letterboxed into row b
+ * of d_out uint8 [B,net_h,net_w,3], its cc_letterbox extent at the top left and zeros past it; a NULL frame gives a zero
+ * row.  d_out == NULL only queries net_h / net_w. */
+int cc_letterbox_frames(const cc_frame* frames, int B, int res, void* d_out, int* net_h, int* net_w, void* stream);
 /* CLIP multi-head attention (models/objects.py:108-118, :157-168), d_head = 64: per (image, head)
  * ctx = softmax(Q K^T / 8 [+ causal mask when causal != 0]) V.  d_qkv: bf16 [B*L, 3*H*64], the fused Q | K | V rows the
  * encoder plans pass; d_ctx: bf16 [B*L, H*64].  impl: 1 = the mma.sync kernel (vit.cu, L <= 704), 2 = the wgmma kernel
