@@ -24,6 +24,15 @@ class cc_frame(ctypes.Structure):
     _fields_ = [("data", ctypes.c_void_p), ("fmt", ctypes.c_int), ("h", ctypes.c_int), ("w", ctypes.c_int)]
 
 
+class cc_track_job(ctypes.Structure):
+    """One row of a tracker job table (cc_ocsort_gpu_update): device rows [n,6], their count, slot, threshold."""
+    _fields_ = [("rows", ctypes.c_void_p), ("n", ctypes.c_int), ("slot", ctypes.c_int), ("det_thresh", ctypes.c_float),
+                ("reserved", ctypes.c_int)]
+
+
+# cc_ocsort_gpu_update statuses (CC_TRACK_* in include/clearcam_b200.h)
+CC_TRACK_OK, CC_TRACK_NEEDS_ROOM, CC_TRACK_BAD_CLASS, CC_TRACK_OVERFLOW = 0, 1, 2, 3
+
 _lib = None
 
 _vp = ctypes.c_void_p
@@ -71,6 +80,14 @@ _SIGS = {
     "cc_ocsort_update": (_i, [_vp, _vp, _i, _f, _vp, _i, ctypes.POINTER(_i)]),
     "cc_ocsort_update_batch": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _vp]),
     "cc_ocsort_num_tracks": (_i, [_vp]),
+    "cc_ocsort_gpu_create": (_i, [_i, _i, ctypes.POINTER(_vp)]),
+    "cc_ocsort_gpu_destroy": (_i, [_vp]),
+    "cc_ocsort_gpu_configure": (_i, [_vp, _i, _i, _i, ctypes.c_double, _i, ctypes.c_double, _i, _i, _vp]),
+    "cc_ocsort_gpu_free": (_i, [_vp, _i, _vp]),
+    "cc_ocsort_gpu_grow": (_i, [_vp, _i, _i, _vp]),
+    "cc_ocsort_gpu_capacity": (_i, [_vp, _i, ctypes.POINTER(_i)]),
+    "cc_ocsort_gpu_num_tracks": (_i, [_vp, _i, ctypes.POINTER(_i), _vp]),
+    "cc_ocsort_gpu_update": (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
     "cc_letterbox": (_i, [_vp, _i, _i, _i, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
     "cc_yolo_net_shape": (_i, [_i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i)]),
     "cc_yolo_forward_frames": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),

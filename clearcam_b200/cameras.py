@@ -5,7 +5,10 @@ clearcam.py:270-271 -> `process_frame` :423-461 -> `run_inference` :580-586: Ten
 .numpy() -> tracker.update).  On an H100 a single 1080p frame leaves the GPU mostly idle, so `CameraBatch.step` takes the
 latest frame of every camera, groups the frames by shape (cameras differ in resolution; the detector's letterbox plan is
 per input shape), runs ONE `detect_batch` per group with uploads and result reads queued back to back, waits once, and
-then steps every camera's tracker in one library call.  What comes back per camera is what `run_inference` computes up
+then steps every camera's tracker in one library call.  When the detector's rows are on the GPU, the trackers run there
+too (`ocsort.DeviceTrackers`): one launch over every group of the step, queued right after the detector calls and
+before that single wait, bit for bit what the host trackers give.  Rows on the host (stand-in models) keep the host
+trackers.  What comes back per camera is what `run_inference` computes up
 to clearcam.py:589 — the (300,6) detector rows and the tracker's targets; zones, alerts and clip saving (:590-621) are
 the product's control plane and stay with the caller.
 
@@ -57,6 +60,7 @@ class CameraBatch:
         self._net: Dict[tuple, tuple] = {}                     # (H,W,dtype,pix_fmt) -> (net_h, net_w)
         self._cam_dev: Dict[Hashable, torch.Tensor] = {}       # camera -> its device frame buffer (merged groups)
         self._table_rows: Dict[tuple, torch.Tensor] = {}       # (net_h, net_w, chunk, bucket) -> pinned rows
+        self._dev_trk: Optional[ocsort.DeviceTrackers] = None  # device trackers, made on the first step with device rows
 
     # -- camera set (clearcam.py:207-240 init_cam; settings threshold :584, class filter :586)
     def add_camera(self, name, thresh: float = 0.5, classes=None, pix_fmt: str = BGR24):
@@ -66,12 +70,16 @@ class CameraBatch:
 
     def remove_camera(self, name):
         self.cams.pop(name, None)
+        if self._dev_trk is not None:
+            self._dev_trk.remove(name)
         self._where.pop(name, None)
         self._cam_dev.pop(name, None)
         self._seen.pop(name, None)             # a re-added camera starts a new mailbox whose frame_num restarts at 0
 
     def reset_tracker(self, name):
         self.cams[name].tracker = ocsort.OCSort(max_age=self.max_age)
+        if self._dev_trk is not None and name in self._dev_trk:
+            self._dev_trk.reset(name)
         self._seen.pop(name, None)
 
     bucket = staticmethod(batch_bucket)   # group sizes are padded to a small set of batch sizes (bounded plan count)
@@ -140,6 +148,14 @@ class CameraBatch:
         with frame tables per distinct net shape (module doc).
         Each frame goes host -> its row of the device batch (or its camera's device buffer) directly (asynchronously when it
         lives in pinned memory, e.g. a FrameMailbox slot): no host-side stacking copy."""
+        pending = self._launch(frames)
+        if self._pin:
+            torch.cuda.current_stream().synchronize()
+        return {name: rows[i].numpy().copy() for names, rows, _ in pending for i, name in enumerate(names)}
+
+    def _launch(self, frames) -> list:
+        """Queue every detector call of `detect` and the copies of its rows to the host: [(cameras, host rows, detector
+        output)]."""
         pending = []
         fmts = {name: cam.pix_fmt for name, cam in self.cams.items() if cam.pix_fmt != BGR24}
         groups = self.group_by_shape(frames, fmts)
@@ -157,10 +173,8 @@ class CameraBatch:
             # bgr24 groups call detect_batch exactly as before the format existed (stand-in models need not know it)
             out = self.model.detect_batch(dev) if key[3] == BGR24 else self.model.detect_batch(dev, pix_fmt=key[3])
             rows.copy_(out, non_blocking=True)
-            pending.append((names, rows))
-        if self._pin:
-            torch.cuda.current_stream().synchronize()
-        return {name: rows[i].numpy().copy() for names, rows in pending for i, name in enumerate(names)}
+            pending.append((names, rows, out))
+        return pending
 
     def _detect_table(self, net, cams, frames) -> list:
         """One detect_frames call per CC_MAX_FRAMES cameras of one net shape; cams: [(camera, pix_fmt)]."""
@@ -182,7 +196,7 @@ class CameraBatch:
                 self._table_rows[k] = torch.empty((b, 300, 6), dtype=torch.float32, pin_memory=self._pin)
             rows = self._table_rows[k]
             rows.copy_(out, non_blocking=True)
-            pending.append(([name for name, _ in chunk], rows))
+            pending.append(([name for name, _ in chunk], rows, out))
         return pending
 
     def device_frame(self, name) -> torch.Tensor:
@@ -209,12 +223,28 @@ class CameraBatch:
         for name in frames:
             if name not in self.cams:
                 self.add_camera(name)
-        det = self.detect(frames)
+        pending = self._launch(frames)
+        on_device = bool(pending) and all(isinstance(out, torch.Tensor) and out.is_cuda for _, _, out in pending)
+        if on_device:                          # track on the GPU, queued before the one wait below
+            if self._dev_trk is None:
+                self._dev_trk = ocsort.DeviceTrackers()
+            for names, _, _ in pending:
+                for n in names:
+                    if n not in self._dev_trk:
+                        self._dev_trk.add(n, max_age=self.max_age)
+            launched = self._dev_trk.launch([(n, out[i], self.cams[n].thresh)
+                                             for names, _, out in pending for i, n in enumerate(names)])
+        if self._pin:
+            torch.cuda.current_stream().synchronize()
+        det = {name: rows[i].numpy().copy() for names, rows, _ in pending for i, name in enumerate(names)}
         names = list(det)
         if not names:
             return {}
-        targets = ocsort.update_many([self.cams[n].tracker for n in names], np.stack([det[n] for n in names]),
-                                     [self.cams[n].thresh for n in names])
+        if on_device:
+            targets = self._dev_trk.finish(launched)
+        else:
+            targets = ocsort.update_many([self.cams[n].tracker for n in names], np.stack([det[n] for n in names]),
+                                         [self.cams[n].thresh for n in names])
         res = {}
         for name, tg in zip(names, targets):
             cam = self.cams[name]

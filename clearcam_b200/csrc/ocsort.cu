@@ -4,7 +4,9 @@
 // in numpy at ~6 ms/frame (ocsort_tracker/ocsort.py:163-308, association.py, kalmanfilter.py); behind a detector that
 // delivers thousands of frames/s that is the bottleneck, so it is rebuilt here as flat-array C++ (a few microseconds
 // per frame) behind cc_ocsort_* and checked against golden vectors produced by the reference itself
-// (tests/golden/ocsort_*.npz, oracle/make_golden_ocsort.py).
+// (tests/golden/ocsort_*.npz, oracle/make_golden_ocsort.py).  The per-track arithmetic (filter, boxes, IoU, direction,
+// angle cost) lives in ocsort_math.cuh, shared with the device tracker of ocsort_gpu.cu, which is held to this one bit
+// for bit; this file keeps the control flow.
 //
 // Arithmetic follows the reference's dtypes where they reach the state: detector rows are float32 and the reference
 // converts a box to the filter measurement, the track direction and the mean speed in float32 before anything is
@@ -22,189 +24,18 @@
 
 #include "cc_common.h"
 #include "clearcam_b200.h"
+#include "ocsort_math.cuh"
 
 using cc::CC_ERR_INVALID;
 using cc::CC_OK;
 
 namespace {
 
-// ------------------------------------------------------------------------------------------------- Kalman filter
-// 7-state constant-velocity filter on z = [cx, cy, area, aspect] (ocsort.py:69-80): F = I + shift(4), H = [I4 0],
-// R = diag(1,1,10,10), P0 = diag(10,10,10,10,1e4,1e4,1e4), Q = diag(1,1,1,1,.01,.01,1e-4).
-struct Meas {
-  bool some = false;   // false = "no observation this frame"
-  bool f32 = false;    // the four numbers were produced by float32 arithmetic (a real detection) rather than float64
-  double v[4] = {0, 0, 0, 0};
-};
-
-static const double kR[4] = {1., 1., 10., 10.};
-static const double kQ[7] = {1., 1., 1., 1., 0.01, 0.01, 0.0001};
-
-static bool invert4(const double S[16], double inv[16]) {
-  double a[4][8];
-  for (int i = 0; i < 4; ++i)
-    for (int j = 0; j < 4; ++j) {
-      a[i][j] = S[i * 4 + j];
-      a[i][4 + j] = i == j ? 1. : 0.;
-    }
-  for (int c = 0; c < 4; ++c) {
-    int piv = c;
-    for (int r = c + 1; r < 4; ++r)
-      if (std::fabs(a[r][c]) > std::fabs(a[piv][c])) piv = r;
-    if (a[piv][c] == 0.) return false;
-    if (piv != c)
-      for (int j = 0; j < 8; ++j) std::swap(a[piv][j], a[c][j]);
-    const double d = 1. / a[c][c];
-    for (int j = 0; j < 8; ++j) a[c][j] *= d;
-    for (int r = 0; r < 4; ++r) {
-      if (r == c) continue;
-      const double f = a[r][c];
-      if (f != 0.)
-        for (int j = 0; j < 8; ++j) a[r][j] -= f * a[c][j];
-    }
-  }
-  for (int i = 0; i < 4; ++i)
-    for (int j = 0; j < 4; ++j) inv[i * 4 + j] = a[i][4 + j];
-  return true;
-}
-
-// The reference appends every measurement (or None) to a list that only ever answers one question: where are the last two
-// real entries (kalmanfilter.py:57, 70-74).  Keeping just those and the length is equivalent and does not grow.
-struct History {
-  int len = 0;
-  int idx[2] = {-1, -1};     // [0] = last real entry, [1] = the one before
-  Meas m[2];
-  void push(const Meas& z) {
-    if (z.some) {
-      idx[1] = idx[0];
-      m[1] = m[0];
-      idx[0] = len;
-      m[0] = z;
-    }
-    ++len;
-  }
-};
-
-struct Kalman {
-  double x[7];
-  double P[49];
-  History hist;
-  bool observed = false;
-  // state frozen when the track was last seen (kalmanfilter.py:112-114); restored by the re-update on re-acquisition
-  bool has_saved = false;
-  double sx[7];
-  double sP[49];
-  History shist;
-
-  Kalman() {
-    std::memset(x, 0, sizeof x);
-    std::memset(P, 0, sizeof P);
-    for (int i = 0; i < 7; ++i) P[i * 7 + i] = i < 4 ? 10. : 10000.;
-  }
-
-  void predict() {            // kalmanfilter.py:65-67
-    double FP[49];
-    for (int i = 0; i < 7; ++i)
-      for (int j = 0; j < 7; ++j) FP[i * 7 + j] = i < 3 ? P[i * 7 + j] + P[(i + 4) * 7 + j] : P[i * 7 + j];
-    for (int i = 0; i < 7; ++i)
-      for (int j = 0; j < 7; ++j) P[i * 7 + j] = (j < 3 ? FP[i * 7 + j] + FP[i * 7 + j + 4] : FP[i * 7 + j]) + (i == j ? kQ[i] : 0.);
-    x[0] += x[4];
-    x[1] += x[5];
-    x[2] += x[6];
-  }
-
-  void correct(const double z[4]) {   // kalmanfilter.py:121-131 (Joseph form)
-    double y[4], S[16], SI[16], K[28];
-    for (int i = 0; i < 4; ++i) y[i] = z[i] - x[i];
-    for (int i = 0; i < 4; ++i)
-      for (int j = 0; j < 4; ++j) S[i * 4 + j] = P[i * 7 + j] + (i == j ? kR[i] : 0.);
-    if (!invert4(S, SI)) return;
-    for (int i = 0; i < 7; ++i)
-      for (int j = 0; j < 4; ++j) {
-        double s = 0.;
-        for (int k = 0; k < 4; ++k) s += P[i * 7 + k] * SI[k * 4 + j];
-        K[i * 4 + j] = s;
-      }
-    for (int i = 0; i < 7; ++i) {
-      double s = 0.;
-      for (int k = 0; k < 4; ++k) s += K[i * 4 + k] * y[k];
-      x[i] += s;
-    }
-    double A[49], AP[49], Pn[49];       // A = I - K H
-    for (int i = 0; i < 7; ++i)
-      for (int j = 0; j < 7; ++j) A[i * 7 + j] = (i == j ? 1. : 0.) - (j < 4 ? K[i * 4 + j] : 0.);
-    for (int i = 0; i < 7; ++i)
-      for (int j = 0; j < 7; ++j) {
-        double s = 0.;
-        for (int k = 0; k < 7; ++k) s += A[i * 7 + k] * P[k * 7 + j];
-        AP[i * 7 + j] = s;
-      }
-    for (int i = 0; i < 7; ++i)
-      for (int j = 0; j < 7; ++j) {
-        double s = 0.;
-        for (int k = 0; k < 7; ++k) s += AP[i * 7 + k] * A[j * 7 + k];
-        double krk = 0.;
-        for (int k = 0; k < 4; ++k) krk += K[i * 4 + k] * kR[k] * K[j * 4 + k];
-        Pn[i * 7 + j] = s + krk;
-      }
-    std::memcpy(P, Pn, sizeof P);
-  }
-
-  void update_none() {        // kalmanfilter.py:109-117
-    hist.push(Meas{});
-    if (observed) {
-      has_saved = true;
-      std::memcpy(sx, x, sizeof x);
-      std::memcpy(sP, P, sizeof P);
-      shist = hist;
-    }
-    observed = false;
-  }
-
-  // Observation-centric re-update (kalmanfilter.py:69-105): roll back to the frozen state and replay a straight-line
-  // virtual trajectory from the last observation before the gap to the new one.
-  void unfreeze() {
-    const int i2 = hist.idx[0], i1 = hist.idx[1];
-    if (i1 < 0) return;
-    const Meas a = hist.m[1], b = hist.m[0];
-    // float32 where the reference's operands are both float32 (two real detections), float64 otherwise
-    auto mul = [](double p, double q, bool f) { return f ? double(float(p) * float(q)) : p * q; };
-    auto dvd = [](double p, double q, bool f) { return f ? double(float(p) / float(q)) : p / q; };
-    auto sqr = [](double p, bool f) { return f ? double(std::sqrt(float(p))) : std::sqrt(p); };
-    auto sub = [](double p, double q, bool f) { return f ? double(float(p) - float(q)) : p - q; };
-    const double w1 = sqr(mul(a.v[2], a.v[3], a.f32), a.f32), h1 = sqr(dvd(a.v[2], a.v[3], a.f32), a.f32);
-    const double w2 = sqr(mul(b.v[2], b.v[3], b.f32), b.f32), h2 = sqr(dvd(b.v[2], b.v[3], b.f32), b.f32);
-    const bool ff = a.f32 && b.f32;
-    const double gap = double(i2 - i1);
-    const double dx = sub(b.v[0], a.v[0], ff) / gap, dy = sub(b.v[1], a.v[1], ff) / gap;
-    const double dw = sub(w2, w1, ff) / gap, dh = sub(h2, h1, ff) / gap;
-    std::memcpy(x, sx, sizeof x);
-    std::memcpy(P, sP, sizeof P);
-    hist = shist;
-    observed = true;
-    const int n = i2 - i1;
-    for (int i = 0; i < n; ++i) {
-      const double w = w1 + (i + 1) * dw, h = h1 + (i + 1) * dh;
-      Meas m;
-      m.some = true;
-      m.f32 = false;
-      m.v[0] = a.v[0] + (i + 1) * dx;
-      m.v[1] = a.v[1] + (i + 1) * dy;
-      m.v[2] = w * h;
-      m.v[3] = w / h;
-      hist.push(m);
-      correct(m.v);
-      if (i != n - 1) predict();
-    }
-  }
-
-  void update(const Meas& z) {      // kalmanfilter.py:107-131, z present
-    hist.push(z);
-    if (!observed && has_saved) unfreeze();
-    observed = true;
-    correct(z.v);
-  }
-};
+using ocs::Kalman;
+using ocs::Meas;
+using ocs::box_to_z;
+using ocs::iou;
+using ocs::state_to_box;
 
 // ------------------------------------------------------------------------------------------------- one track
 struct Obs { float b[5]; };
@@ -224,10 +55,7 @@ struct Track {
 
   // `last_observation.sum() >= 0` (ocsort.py:113, 281): a real box whose five numbers sum below zero reads as "none"
   bool last_nonneg() const {
-    if (!has_last) return false;
-    float s = last.b[0];
-    for (int i = 1; i < 5; ++i) s += last.b[i];
-    return s >= 0.f;
+    return has_last && ocs::box_sum_nonneg(last.b);
   }
   const Obs* find_obs(int a) const {
     for (auto it = obs.rbegin(); it != obs.rend(); ++it)
@@ -235,33 +63,6 @@ struct Track {
     return nullptr;
   }
 };
-
-static Meas box_to_z(const float* b) {    // ocsort.py:21-33, float32 arithmetic
-  const float w = b[2] - b[0], h = b[3] - b[1];
-  Meas m;
-  m.some = true;
-  m.f32 = true;
-  m.v[0] = b[0] + w / 2.f;
-  m.v[1] = b[1] + h / 2.f;
-  m.v[2] = w * h;
-  m.v[3] = w / (h + 1e-6f);
-  return m;
-}
-
-static void state_to_box(const double* x, double out[4]) {   // ocsort.py:36-45
-  const double w = std::sqrt(x[2] * x[3]), h = x[2] / w;
-  out[0] = x[0] - w / 2.;
-  out[1] = x[1] - h / 2.;
-  out[2] = x[0] + w / 2.;
-  out[3] = x[1] + h / 2.;
-}
-
-static double iou(const double* a, const double* b) {   // association.py:3-20
-  const double xx1 = std::max(a[0], b[0]), yy1 = std::max(a[1], b[1]);
-  const double xx2 = std::min(a[2], b[2]), yy2 = std::min(a[3], b[3]);
-  const double w = std::max(0., xx2 - xx1), h = std::max(0., yy2 - yy1), wh = w * h;
-  return wh / ((a[2] - a[0]) * (a[3] - a[1]) + (b[2] - b[0]) * (b[3] - b[1]) - wh);
-}
 
 // association.py:34-54: walk the pairs by ascending cost, take a pair when its row and column are both free, stop when
 // every row or every column is used.  Ties are broken by flat index (the reference's argsort leaves them unspecified).
@@ -329,16 +130,7 @@ struct cc_ocsort {
       const Obs* prev = nullptr;
       for (int i = 0; i < delta_t && !prev; ++i) prev = t.find_obs(t.age - (delta_t - i));
       if (!prev) prev = &t.last;
-      const float cx1 = (prev->b[0] + prev->b[2]) / 2.f, cy1 = (prev->b[1] + prev->b[3]) / 2.f;   // ocsort.py:48-53
-      const float cx2 = (b[0] + b[2]) / 2.f, cy2 = (b[1] + b[3]) / 2.f;
-      const float dy = cy2 - cy1, dx = cx2 - cx1;
-      const float norm = std::sqrt(dy * dy + dx * dx) + 1e-6f;
-      t.vel[0] = dy / norm;
-      t.vel[1] = dx / norm;
-      const float a = static_cast<float>(t.age);
-      t.avg_vel[0] += static_cast<double>(dy / a);
-      t.avg_vel[1] += static_cast<double>(dx / a);
-      t.speed = std::fabs(t.avg_vel[0]) + std::fabs(t.avg_vel[1]);
+      ocs::velocity_update(prev->b, b, t.age, t.vel, t.avg_vel, &t.speed);
     }
     std::memcpy(t.last.b, b, sizeof t.last.b);
     t.has_last = true;
@@ -407,19 +199,10 @@ struct cc_ocsort {
               if (!ko) ko = &tr.obs.back().second;
             }
             const double pb[5] = {ko ? ko->b[0] : -1., ko ? ko->b[1] : -1., ko ? ko->b[2] : -1., ko ? ko->b[3] : -1., ko ? ko->b[4] : -1.};
-            const double valid = pb[4] < 0. ? 0. : 1.;
-            const double cx2 = (pb[0] + pb[2]) / 2., cy2 = (pb[1] + pb[3]) / 2.;
+            double valid, cx2, cy2;
+            ocs::angle_anchor(pb, &valid, &cx2, &cy2);
             for (int d = 0; d < D; ++d) {
-              const double cx1 = (dbox[d][0] + dbox[d][2]) / 2., cy1 = (dbox[d][1] + dbox[d][3]) / 2.;
-              double dx = cx1 - cx2, dy = cy1 - cy2;
-              const double norm = std::sqrt(dx * dx + dy * dy) + 1e-6;
-              dx /= norm;
-              dy /= norm;
-              double c = tr.vel[1] * dx + tr.vel[0] * dy;
-              c = std::min(1., std::max(-1., c));
-              // c == 0 (tracks that have no direction yet) gives acos = pi/2 and an angle term of exactly 0: skip the call
-              const double ang = c == 0. ? 0. : (M_PI / 2.0 - std::fabs(std::acos(c))) / M_PI;
-              const double adc = (valid * ang) * inertia * static_cast<double>(dets[d].b[4]);
+              const double adc = ocs::angle_term(valid, cx2, cy2, tr.vel, dbox[d].data(), dets[d].b[4], inertia);
               cost[static_cast<size_t>(d) * T + t] = -(iou_m[static_cast<size_t>(d) * T + t] + adc);
             }
           }

@@ -4,16 +4,18 @@ C++ tracker of libclearcam_b200 (csrc/ocsort.cu) instead of per-frame numpy.
     tracker = ocsort.OCSort(max_age=100)                 # clearcam.py:239
     online_targets = tracker.update(preds, thresh)       # clearcam.py:585, preds = the detector's (300,6) array
 
-`update_many` steps the trackers of several cameras on one batched detector result in a single library call."""
+`update_many` steps the trackers of several cameras on one batched detector result in a single library call;
+`DeviceTrackers` does the same on the GPU for rows that stay on the device."""
 import ctypes
 from typing import List, Optional, Sequence
 
 import numpy as np
 
-from .._lib import check, lib
+from .._lib import CC_TRACK_BAD_CLASS, CC_TRACK_NEEDS_ROOM, CC_TRACK_OVERFLOW, CCError, check, lib
 from .STrack import STrack
 
 _CAP = 1024          # rows of the result buffer (the detector emits at most 300 boxes per frame)
+_HEAD = 128          # DeviceTrackers: rows per camera copied to the host with every launch; longer results are read after
 
 
 def _rows(output_results) -> np.ndarray:
@@ -81,3 +83,167 @@ def update_many(trackers: Sequence[Optional[OCSort]], results, det_thresh) -> Li
         if t is not None:
             t.frame_count += 1
     return [_tracks(out[b], int(n[b])) if trackers[b] is not None else [] for b in range(B)]
+
+
+class DeviceTrackers:
+    """One `OCSort` per camera, all on the GPU (csrc/ocsort_gpu.cu): `update` steps every camera of a list of jobs in one
+    launch per CC_MAX_FRAMES cameras, on detector rows that never leave the device, and returns what `update_many` returns
+    for the same rows, bit for bit (track ids included).
+
+        trk = DeviceTrackers()
+        trk.add("cam0", max_age=100)                         # OCSort.__init__'s arguments
+        [targets] = trk.update([("cam0", rows, 0.5)])       # rows: CUDA float32 (n,6), e.g. one row of detect_batch's output
+
+    `launch` / `finish` split `update` around a synchronisation the caller does anyway (CameraBatch.step)."""
+
+    def __init__(self, slots: int = 1024, max_delta_t: int = 8, capacity: int = 64):
+        import torch
+        from .._lib import CC_MAX_FRAMES
+        self._torch, self._B = torch, CC_MAX_FRAMES
+        self._h = ctypes.c_void_p()
+        check(lib().cc_ocsort_gpu_create(int(slots), int(max_delta_t), ctypes.byref(self._h)), "cc_ocsort_gpu_create")
+        self._free = list(range(slots - 1, -1, -1))
+        self._slot, self._args, self._cap = {}, {}, {}
+        self._capacity = int(capacity)
+        self._bufs = []                                        # per launch of one update: device and pinned results
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().cc_ocsort_gpu_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def __contains__(self, cam):
+        return cam in self._slot
+
+    def _stream(self):
+        return ctypes.c_void_p(self._torch.cuda.current_stream().cuda_stream)
+
+    def _configure(self, cam):
+        a = self._args[cam]
+        check(lib().cc_ocsort_gpu_configure(self._h, self._slot[cam], a["max_age"], a["min_hits"], a["iou_threshold"], a["delta_t"],
+                                            a["inertia"], a["use_byte"], self._cap[cam], self._stream()),
+              f"cc_ocsort_gpu_configure (camera {cam!r})")
+
+    def add(self, cam, det_thresh=0.25, max_age=30, min_hits=3, iou_threshold=0.3, delta_t=3, asso_func="iou", inertia=0.2,
+            use_byte=False):
+        """A tracker for camera `cam` with OCSort.__init__'s arguments (an existing one is replaced)."""
+        if asso_func != "iou":
+            raise ValueError("only the IoU association the reference uses is implemented")
+        if cam not in self._slot:
+            if not self._free:
+                raise ValueError("every tracker slot is in use")
+            self._slot[cam] = self._free.pop()
+            self._cap[cam] = self._capacity
+        self._args[cam] = dict(max_age=int(max_age), min_hits=int(min_hits), iou_threshold=float(iou_threshold),
+                               delta_t=int(delta_t), inertia=float(inertia), use_byte=int(bool(use_byte)))
+        try:
+            self._configure(cam)
+        except Exception:
+            self._free.append(self._slot.pop(cam))
+            del self._args[cam], self._cap[cam]
+            raise
+
+    def reset(self, cam):
+        """Start camera `cam`'s tracker afresh (as a new OCSort with the same arguments)."""
+        self._configure(cam)
+
+    def remove(self, cam):
+        slot = self._slot.pop(cam, None)
+        if slot is None:
+            return
+        del self._args[cam], self._cap[cam]
+        check(lib().cc_ocsort_gpu_free(self._h, slot, self._stream()), "cc_ocsort_gpu_free")
+        self._free.append(slot)
+
+    def num_tracks(self, cam) -> int:
+        n = ctypes.c_int()
+        check(lib().cc_ocsort_gpu_num_tracks(self._h, self._slot[cam], ctypes.byref(n), self._stream()), "cc_ocsort_gpu_num_tracks")
+        return n.value
+
+    def _buffers(self, i):
+        """Buffer set i: device results [B,_CAP,9], counts and statuses, their first _HEAD rows packed on the device, and
+        pinned host copies of those (only the head crosses PCIe with every launch)."""
+        torch = self._torch
+        while len(self._bufs) <= i:
+            self._bufs.append((torch.empty((self._B, _CAP, 9), dtype=torch.float64, device="cuda"),
+                               torch.empty((2, self._B), dtype=torch.int32, device="cuda"),
+                               torch.empty((self._B, _HEAD, 9), dtype=torch.float64, device="cuda"),
+                               torch.empty((self._B, _HEAD, 9), dtype=torch.float64, pin_memory=True),
+                               torch.empty((2, self._B), dtype=torch.int32, pin_memory=True)))
+        return self._bufs[i]
+
+    def _launch(self, jobs, i):
+        """Enqueue one launch for <= CC_MAX_FRAMES jobs into buffer set i and the copy of its results to the host."""
+        from .._lib import cc_track_job
+        table = (cc_track_job * len(jobs))()
+        for b, (cam, rows, thr) in enumerate(jobs):
+            if cam not in self._slot:
+                raise KeyError(f"camera {cam!r} has no tracker: add() it first")
+            if rows.dtype != self._torch.float32 or not rows.is_cuda or rows.dim() != 2 or rows.shape[1] != 6 or not rows.is_contiguous():
+                raise ValueError(f"camera {cam!r}: rows must be a contiguous CUDA float32 (n, 6) tensor")
+            table[b] = cc_track_job(rows.data_ptr() if rows.shape[0] else None, rows.shape[0], self._slot[cam], float(thr), 0)
+        out, cs, head, hout, hcs = self._buffers(i)
+        B = len(jobs)
+        check(lib().cc_ocsort_gpu_update(self._h, table, B, out.data_ptr(), _CAP, cs[0].data_ptr(), cs[1].data_ptr(),
+                                         self._stream()), "cc_ocsort_gpu_update")
+        head[:B].copy_(out[:B, :_HEAD])
+        hcs.copy_(cs, non_blocking=True)
+        hout[:B].copy_(head[:B], non_blocking=True)
+
+    def launch(self, jobs):
+        """Enqueue `update(jobs)` without waiting; pass the result to `finish` after the stream is synchronised."""
+        jobs = list(jobs)
+        for i, c0 in enumerate(range(0, len(jobs), self._B)):
+            self._launch(jobs[c0:c0 + self._B], i)
+        return jobs
+
+    def finish(self, jobs) -> List[List[STrack]]:
+        """The targets of `launch(jobs)` once the stream has been synchronised.  A camera whose tracker lacked room is
+        grown and stepped again here (one more launch and wait).  Every other camera's frame is complete before anything
+        is raised: if cameras failed (a class id that is not an integer in 0..79: that tracker is unchanged; more than
+        _CAP tracks: the frame was applied), one CCError names them all, and its `results` holds every camera's targets,
+        None for the failed ones."""
+        res = [None] * len(jobs)
+        errors = []
+        idx = list(range(len(jobs)))                           # the job behind each launched row, in launch order
+        while idx:
+            grow = []
+            for i, c0 in enumerate(range(0, len(idx), self._B)):
+                out, _, _, hout, hcs = self._bufs[i]
+                for b, k in enumerate(idx[c0:c0 + self._B]):
+                    cam, n, st = jobs[k][0], int(hcs[0, b]), int(hcs[1, b])
+                    if st == CC_TRACK_NEEDS_ROOM:
+                        grow.append((k, n))
+                    elif st == CC_TRACK_BAD_CLASS:
+                        errors.append(f"camera {cam!r}: a detection's class id is not an integer in 0..79 (its tracker is unchanged)")
+                    elif st == CC_TRACK_OVERFLOW:
+                        errors.append(f"camera {cam!r}: {n} tracks do not fit the output capacity {_CAP}")
+                    elif n <= _HEAD:                           # copies: the buffers are reused by the next launch
+                        res[k] = _tracks(hout[b, :n].numpy().copy(), n)
+                    else:
+                        res[k] = _tracks(out[b, :n].cpu().numpy(), n)
+            for k, need in grow:
+                cam = jobs[k][0]
+                cap = max(2 * self._cap[cam], need)
+                check(lib().cc_ocsort_gpu_grow(self._h, self._slot[cam], cap, self._stream()), f"cc_ocsort_gpu_grow (camera {cam!r})")
+                self._cap[cam] = cap
+            idx = [k for k, _ in grow]
+            if idx:
+                self.launch([jobs[k] for k in idx])
+                self._torch.cuda.current_stream().synchronize()
+        if errors:
+            e = CCError("; ".join(errors))
+            e.results = res
+            raise e
+        return res
+
+    def update(self, jobs) -> List[List[STrack]]:
+        """jobs: [(camera, rows, det_thresh)] with rows a CUDA float32 (n,6) tensor; one camera at most once.  Returns each
+        camera's targets, as OCSort.update / update_many would."""
+        p = self.launch(jobs)
+        self._torch.cuda.current_stream().synchronize()
+        return self.finish(p)
+

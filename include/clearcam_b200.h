@@ -351,6 +351,47 @@ int cc_ocsort_update_batch(cc_ocsort_t* hs, int B, const float* rows, int n, con
                            int* n_out);
 int cc_ocsort_num_tracks(cc_ocsort_t h);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * The same tracker on the GPU, bit for bit (track ids included): a handle owns `slots` camera trackers on the current
+ * device, and one cc_ocsort_gpu_update launch steps up to CC_MAX_FRAMES of them, one CTA per camera, on rows that stay
+ * on the device.  Slot calls are stream-ordered on the stream given (use one stream per handle); nothing synchronises
+ * except cc_ocsort_gpu_num_tracks (which waits for `stream`, then reads the count) and cc_ocsort_gpu_destroy.
+ *
+ * cc_ocsort_gpu_configure: (re)starts slot `slot` as cc_ocsort_create(max_age, ...) would, with room for `capacity`
+ * tracks (storage is reused when the capacity is unchanged); delta_t may not exceed the handle's max_delta_t.
+ * cc_ocsort_gpu_grow: keeps the slot's tracks and raises its room to `capacity` (a smaller value does nothing).
+ *
+ * cc_ocsort_gpu_update: job b steps slot jobs[b].slot on the device rows d_rows [n,6] (as cc_ocsort_update's rows) at
+ * det_thresh; each slot at most once per call.  Per job b: d_out [B,cap,9] float64 rows as cc_ocsort_update writes them,
+ * d_count[b], d_status[b] = CC_TRACK_*:
+ *   OK         the frame was applied, d_count[b] rows written;
+ *   NEEDS_ROOM the slot lacks room for the tracks this frame may add: nothing changed, d_count[b] = the capacity needed
+ *              (cc_ocsort_gpu_grow, then step the camera again);
+ *   BAD_CLASS  a detection inside the score gates has a class id that is not an integer in 0..CC_OCSORT_CLASSES-1:
+ *              nothing changed, d_count[b] = 0;
+ *   OVERFLOW   more than cap rows: the frame was applied (as cc_ocsort_update does), d_count[b] = the row count, only
+ *              cap rows written.
+ * Nothing is written in d_out past a job's rows.  Bad arguments (unconfigured or repeated slot, n outside
+ * 0..CC_OCSORT_MAX_ROWS, NULL rows, B outside 1..CC_MAX_FRAMES) fail with CC_ERR_INVALID before the launch. */
+typedef struct cc_ocsort_gpu cc_ocsort_gpu;
+typedef struct { const float* d_rows; int n; int slot; float det_thresh; int reserved; } cc_track_job;
+#define CC_OCSORT_CLASSES 80
+#define CC_OCSORT_MAX_ROWS 1024
+#define CC_TRACK_OK 0
+#define CC_TRACK_NEEDS_ROOM 1
+#define CC_TRACK_BAD_CLASS 2
+#define CC_TRACK_OVERFLOW 3
+int cc_ocsort_gpu_create(int slots, int max_delta_t, cc_ocsort_gpu** out);
+int cc_ocsort_gpu_destroy(cc_ocsort_gpu* h);
+int cc_ocsort_gpu_configure(cc_ocsort_gpu* h, int slot, int max_age, int min_hits, double iou_threshold, int delta_t,
+                            double inertia, int use_byte, int capacity, void* stream);
+int cc_ocsort_gpu_free(cc_ocsort_gpu* h, int slot, void* stream);
+int cc_ocsort_gpu_grow(cc_ocsort_gpu* h, int slot, int capacity, void* stream);
+int cc_ocsort_gpu_capacity(cc_ocsort_gpu* h, int slot, int* capacity);
+int cc_ocsort_gpu_num_tracks(cc_ocsort_gpu* h, int slot, int* n, void* stream);
+int cc_ocsort_gpu_update(cc_ocsort_gpu* h, const cc_track_job* jobs, int B, double* d_out, int cap, int* d_count,
+                         int* d_status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
