@@ -32,6 +32,9 @@ class cc_track_job(ctypes.Structure):
 
 # cc_ocsort_gpu_update statuses (CC_TRACK_* in include/clearcam_b200.h)
 CC_TRACK_OK, CC_TRACK_NEEDS_ROOM, CC_TRACK_BAD_CLASS, CC_TRACK_OVERFLOW = 0, 1, 2, 3
+# cc_ocsort_gpu_events statuses (CC_EVENT_* in include/clearcam_b200.h)
+CC_EVENT_OK, CC_EVENT_NEEDS_ROOM, CC_EVENT_BAD_BOX, CC_EVENT_NOT_RUN, CC_EVENT_BAD_ORDER = 0, 1, 2, 3, 4
+CC_EVENT_MAX_VERTICES = 256
 
 _lib = None
 
@@ -88,6 +91,9 @@ _SIGS = {
     "cc_ocsort_gpu_capacity": (_i, [_vp, _i, ctypes.POINTER(_i)]),
     "cc_ocsort_gpu_num_tracks": (_i, [_vp, _i, ctypes.POINTER(_i), _vp]),
     "cc_ocsort_gpu_update": (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
+    "cc_ocsort_gpu_events_configure": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _i, _vp]),
+    "cc_ocsort_gpu_events_grow": (_i, [_vp, _i, _i, _vp]),
+    "cc_ocsort_gpu_events": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     "cc_letterbox": (_i, [_vp, _i, _i, _i, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
     "cc_yolo_net_shape": (_i, [_i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i)]),
     "cc_yolo_forward_frames": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),

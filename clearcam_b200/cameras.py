@@ -8,9 +8,11 @@ per input shape), runs ONE `detect_batch` per group with uploads and result read
 then steps every camera's tracker in one library call.  When the detector's rows are on the GPU, the trackers run there
 too (`ocsort.DeviceTrackers`): one launch over every group of the step, queued right after the detector calls and
 before that single wait, bit for bit what the host trackers give.  Rows on the host (stand-in models) keep the host
-trackers.  What comes back per camera is what `run_inference` computes up
-to clearcam.py:589 — the (300,6) detector rows and the tracker's targets; zones, alerts and clip saving (:590-621) are
-the product's control plane and stay with the caller.
+trackers.  What `step` returns per camera is what `run_inference` computes up to clearcam.py:589 — the (300,6)
+detector rows and the tracker's targets.  `step_events` goes on to :621: each camera's zone, motion gate, object-save
+picks and new-object flags (clearcam_b200/events.py), on the GPU right after the trackers (csrc/events_gpu.cu) for
+device rows and by `ObjectEvents` for host rows, and returns run_inference's preds; the alerts' counters and the saving
+of the picked crops stay with the caller.
 
 Each camera has a pixel format (clearcam_b200/pixfmt.py): "bgr24" [H,W,3] frames (the default) or "yuv420p" [H*3/2,W]
 frames, which the detector converts on the GPU.  Groups are keyed by (H, W, dtype, format).
@@ -21,12 +23,14 @@ batch at res 640 (all of them give a 384 x 640 net input).  A merged group copie
 device buffer and makes one `detect_frames` call per CC_MAX_FRAMES cameras, padded to the batch bucket with None rows.
 A group with a single source shape and format still calls `detect_batch`, as do float32 frames and models without
 frame tables."""
+import time
 from typing import Dict, Hashable, List, NamedTuple, Optional
 
 import numpy as np
 import torch
 
 from ._lib import CC_MAX_FRAMES
+from .events import ObjectEvents
 from .ocsort_tracker import ocsort
 from .pixfmt import BGR24, check_pix_fmt, yuv420p_size
 from .utils.helpers import batch_bucket
@@ -39,10 +43,22 @@ class CameraResult(NamedTuple):
     preds: np.ndarray           # (k,7) x1,y1,x2,y2,score,class,track_id of targets seen for more than one frame
 
 
+class CameraEvents(NamedTuple):
+    rows: np.ndarray            # (300,6) float32 detector output in this camera's frame coordinates
+    preds: np.ndarray           # (k,7) float64: run_inference's return value (clearcam.py:611, 622)
+    flags: np.ndarray           # (k,) uint8 per preds row: bit 0 new (object_set), bit 1 new in the zone (object_set_zone)
+    saves: np.ndarray           # (m,6) int64 track_id, class_id, x1, y1, x2, y2: the crops save_object writes
+
+
 class _Camera:
     def __init__(self, thresh, classes, max_age, pix_fmt=BGR24):
         self.thresh, self.classes, self.pix_fmt = thresh, classes, pix_fmt
         self.tracker = ocsort.OCSort(max_age=max_age)          # clearcam.py:239
+        self.zone = (None, False, False)                       # settings["coords"], settings["outside"], non-zone alert
+        self.events = ObjectEvents(classes=classes)            # host rows' events (pred_occs, object_set, object_set_zone)
+
+    def fresh_events(self):
+        self.events = ObjectEvents(*self.zone, classes=self.classes)
 
 
 class CameraBatch:
@@ -77,10 +93,22 @@ class CameraBatch:
         self._seen.pop(name, None)             # a re-added camera starts a new mailbox whose frame_num restarts at 0
 
     def reset_tracker(self, name):
+        """A fresh tracker and fresh events for camera `name`, as init_cam makes them."""
         self.cams[name].tracker = ocsort.OCSort(max_age=self.max_age)
+        self.cams[name].fresh_events()
         if self._dev_trk is not None and name in self._dev_trk:
             self._dev_trk.reset(name)
         self._seen.pop(name, None)
+
+    def set_zone(self, name, zone=None, outside: bool = False, non_zone_alert: bool = False):
+        """Camera `name`'s zone for `step_events`: settings["coords"] (fractions of the frame; None for no zone),
+        settings["outside"] and whether any of its alerts has no zone (clearcam.py:599-610).  Its event state (which ids
+        were saved, counted and alerted on) starts afresh."""
+        cam = self.cams[name]
+        cam.zone = (zone, outside, non_zone_alert)
+        cam.fresh_events()                                     # checks the arguments
+        if self._dev_trk is not None and name in self._dev_trk:
+            self._dev_trk.events(name, zone, outside, non_zone_alert, cam.classes)
 
     bucket = staticmethod(batch_bucket)   # group sizes are padded to a small set of batch sizes (bounded plan count)
 
@@ -210,6 +238,16 @@ class CameraBatch:
         """`step` on every camera whose mailbox (clearcam_b200.ingest) holds a frame this object has not seen yet —
         the reference's `if frame_num == last_frame_num: return` per camera (clearcam.py:446).  A camera seen here for
         the first time is added with its mailbox's pixel format."""
+        frames = self._from_mailboxes(mailboxes)
+        return self.step(frames) if frames else {}
+
+    def step_events_mailboxes(self, mailboxes: Dict[Hashable, "FrameMailbox"], now: Optional[float] = None
+                              ) -> Dict[Hashable, CameraEvents]:
+        """`step_events` on the cameras whose mailboxes hold a new frame (as `step_mailboxes`)."""
+        frames = self._from_mailboxes(mailboxes)
+        return self.step_events(frames, now) if frames else {}
+
+    def _from_mailboxes(self, mailboxes):
         frames = {}
         for name, mb in mailboxes.items():
             got = mb.latest(self._seen.get(name, -1))
@@ -217,9 +255,25 @@ class CameraBatch:
                 if name not in self.cams:
                     self.add_camera(name, pix_fmt=getattr(mb, "pix_fmt", BGR24))
                 self._seen[name], frames[name] = got
-        return self.step(frames) if frames else {}
+        return frames
 
     def step(self, frames: Dict[Hashable, np.ndarray]) -> Dict[Hashable, CameraResult]:
+        return self._step(frames, None)
+
+    def step_events(self, frames: Dict[Hashable, np.ndarray], now: Optional[float] = None) -> Dict[Hashable, CameraEvents]:
+        """`step`, then each camera's object events (clearcam.py:586-621, clearcam_b200/events.py) at clock `now`
+        (time.time() when None; one reading for the whole step) -> {camera: CameraEvents}.  Device rows run the events on
+        the GPU right after the trackers, before the step's one wait; host rows run `ObjectEvents`.  A camera's frame
+        size is its picture's (a yuv420p frame [H*3/2,W] is W x H)."""
+        return self._step(frames, time.time() if now is None else float(now))
+
+    def _picture_size(self, name, f):
+        if self.cams[name].pix_fmt == BGR24:
+            return int(f.shape[1]), int(f.shape[0])
+        H, W = yuv420p_size(f.shape)
+        return W, H
+
+    def _step(self, frames, now):
         for name in frames:
             if name not in self.cams:
                 self.add_camera(name)
@@ -232,8 +286,11 @@ class CameraBatch:
                 for n in names:
                     if n not in self._dev_trk:
                         self._dev_trk.add(n, max_age=self.max_age)
-            launched = self._dev_trk.launch([(n, out[i], self.cams[n].thresh)
-                                             for names, _, out in pending for i, n in enumerate(names)])
+                    if now is not None and not self._dev_trk.has_events(n):
+                        self._dev_trk.events(n, *self.cams[n].zone, self.cams[n].classes)
+            jobs = [(n, out[i], self.cams[n].thresh) for names, _, out in pending for i, n in enumerate(names)]
+            launched = self._dev_trk.launch(jobs, None if now is None else
+                                            [self._picture_size(n, frames[n]) + (now,) for n, _, _ in jobs])
         if self._pin:
             torch.cuda.current_stream().synchronize()
         det = {name: rows[i].numpy().copy() for names, rows, _ in pending for i, name in enumerate(names)}
@@ -241,6 +298,8 @@ class CameraBatch:
         if not names:
             return {}
         if on_device:
+            if now is not None:
+                return {name: CameraEvents(det[name], *e) for name, e in zip(names, self._dev_trk.finish_events(launched))}
             targets = self._dev_trk.finish(launched)
         else:
             targets = ocsort.update_many([self.cams[n].tracker for n in names], np.stack([det[n] for n in names]),
@@ -248,6 +307,9 @@ class CameraBatch:
         res = {}
         for name, tg in zip(names, targets):
             cam = self.cams[name]
+            if now is not None:
+                res[name] = CameraEvents(det[name], *cam.events.update(tg, *self._picture_size(name, frames[name]), now))
+                continue
             if cam.classes is not None:
                 tg = [t for t in tg if int(t.class_id) in cam.classes]                       # clearcam.py:586
             keep = [t for t in tg if t.tracklet_len >= 1]                                     # clearcam.py:589

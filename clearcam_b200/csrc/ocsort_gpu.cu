@@ -24,6 +24,7 @@
 
 #include "cc_common.h"
 #include "clearcam_b200.h"
+#include "ocsort_gpu.cuh"
 #include "ocsort_math.cuh"
 
 using cc::CC_ERR_INVALID;
@@ -55,14 +56,9 @@ __host__ __device__ inline int lane_count(int rb) { return lane_keep(rb) + 4; }
 enum : int { S_COLUSED = 0, S_UTRK = 1, S_FLAGS = 2, S_POS = 3 };
 enum : int { F_MATCHED = 1, F_INUT = 2, F_REMOVED = 4 };
 
-struct SlotCfg {
-  double* dl;
-  int32_t* il;
-  int cap, active;
-  int max_age, min_hits, delta_t, use_byte;
-  double iou_threshold, inertia;
-};
-struct SlotCnt { int T, frame_count, next_id, pad; };
+using ocsg::SlotCfg;
+using ocsg::SlotCnt;
+static_assert(I_ID == ocsg::kLaneId, "events_gpu.cu reads the id lane");
 
 struct JobTable { cc_track_job j[CC_MAX_FRAMES]; };
 
@@ -670,19 +666,13 @@ __global__ void __launch_bounds__(kThreads) ocsort_step_kernel(const __grid_cons
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------- host side
-struct cc_ocsort_gpu {
-  int S = 0, rb = 0;                 // slots; ring entries per track (max delta_t + 2)
-  std::vector<SlotCfg> cfg;          // host copy of every slot's configuration
-  SlotCfg* d_cfg = nullptr;
-  SlotCnt* d_cnt = nullptr;
-  size_t track_bytes() const { return ND * sizeof(double) + static_cast<size_t>(lane_count(rb)) * 4; }
-};
-
 namespace {
+
+size_t track_bytes(const cc_ocsort_gpu* h) { return ND * sizeof(double) + static_cast<size_t>(lane_count(h->rb)) * 4; }
 
 int alloc_slot(cc_ocsort_gpu* h, int cap, cudaStream_t st, SlotCfg& c) {
   void* p = nullptr;
-  CC_CHECK_CUDA(cudaMallocAsync(&p, static_cast<size_t>(cap) * h->track_bytes(), st));
+  CC_CHECK_CUDA(cudaMallocAsync(&p, static_cast<size_t>(cap) * track_bytes(h), st));
   c.dl = static_cast<double*>(p);
   c.il = reinterpret_cast<int32_t*>(static_cast<char*>(p) + static_cast<size_t>(cap) * ND * sizeof(double));
   c.cap = cap;
@@ -723,6 +713,7 @@ int cc_ocsort_gpu_create(int slots, int max_delta_t, cc_ocsort_gpu** out) {
 int cc_ocsort_gpu_destroy(cc_ocsort_gpu* h) {
   if (!h) return CC_OK;
   cudaDeviceSynchronize();            // slot storage is freed stream-ordered elsewhere; here nothing may still use it
+  cc_events_destroy(h);
   for (auto& c : h->cfg)
     if (c.active) cudaFree(c.dl);
   cudaFree(h->d_cfg);
@@ -755,6 +746,8 @@ int cc_ocsort_gpu_configure(cc_ocsort_gpu* h, int slot, int max_age, int min_hit
   c.iou_threshold = iou_threshold;
   c.inertia = inertia;
   CC_CHECK_CUDA(cudaMemsetAsync(h->d_cnt + slot, 0, sizeof(SlotCnt), st));
+  const int r = cc_events_slot_clear(h, slot, st);   // a restarted tracker reuses ids: its events start afresh too
+  if (r != CC_OK) return r;
   return push_cfg(h, slot, st);
 }
 
@@ -763,6 +756,8 @@ int cc_ocsort_gpu_free(cc_ocsort_gpu* h, int slot, void* stream) {
   SlotCfg& c = h->cfg[slot];
   if (!c.active) return CC_OK;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int r = cc_events_slot_free(h, slot, st);
+  if (r != CC_OK) return r;
   CC_CHECK_CUDA(cudaFreeAsync(c.dl, st));
   c = SlotCfg{};
   return push_cfg(h, slot, st);

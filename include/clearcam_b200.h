@@ -392,6 +392,46 @@ int cc_ocsort_gpu_num_tracks(cc_ocsort_gpu* h, int slot, int* n, void* stream);
 int cc_ocsort_gpu_update(cc_ocsort_gpu* h, const cc_track_job* jobs, int B, double* d_out, int cap, int* d_count,
                          int* d_status, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Object events on the tracker handle: what run_inference does with the targets (clearcam.py:586-621), per camera on the
+ * device — the class filter, tracklet_len < 1, the pred_occs clock and save_object's rectangle with its 100-px gate, the
+ * motion gate speed < 2.5, the zone test (point_not_in_polygon in float64, exactly as written there) with `outside` and
+ * the non-zone-alert rule, the (k,7) preds rows and the new / new-in-zone bookkeeping.  clearcam_b200/events.py is the
+ * host form and documents the choices (one clock reading per camera-step; non-finite boxes are errors).
+ *
+ * cc_ocsort_gpu_events_configure: the events of tracker slot `slot` (configured with cc_ocsort_gpu_configure): zone_xy
+ * [n_vertices,2] float64 fractions of the frame (n_vertices 0 = no zone, at most CC_EVENT_MAX_VERTICES, finite),
+ * outside / non_zone_alert as 0/1, class_mask 3 words of bits for class ids 0..79 (NULL = every class), room for
+ * `capacity` track ids.  Clears the slot's event state (pred_occs, object_set, object_set_zone), as does
+ * cc_ocsort_gpu_configure; cc_ocsort_gpu_free frees it.  cc_ocsort_gpu_events_grow keeps the state and raises the room.
+ *
+ * cc_ocsort_gpu_events: job b (a cc_ocsort_gpu_update job table; only .slot is read) runs the events of jobs[b].slot on
+ * row b of that call's outputs d_trk_out [B,trk_cap,9], d_trk_count, d_trk_status, queued after it on the same stream,
+ * for a frame of frame_wh[2b] x frame_wh[2b+1] pixels at clock now[b] (seconds).  Outputs per job b: d_preds [B,cap,7]
+ * float64, d_flags [B,cap] uint8 (bit 0 new, bit 1 new_in_zone), d_saves [B,cap,6] int64 (track_id, class_id, x1, y1,
+ * x2, y2), d_counts[b] preds rows and d_counts[B+b] save rows, d_status[b] = CC_EVENT_*:
+ *   OK         the step was applied;
+ *   NEEDS_ROOM the slot's event storage lacks room: nothing changed, d_counts[b] = the capacity needed
+ *              (cc_ocsort_gpu_events_grow, then run the events of that camera again on the same tracker rows);
+ *   BAD_BOX    a target past the class filter and tracklet_len has a box that is not finite or beyond 2^60: nothing changed;
+ *   NOT_RUN    the tracker's status for the job was not CC_TRACK_OK: nothing changed;
+ *   BAD_ORDER  the tracker's ids are not in the strictly ascending slot order the state relies on: nothing changed.
+ * Nothing is written past a job's rows.  Bad arguments (a slot without tracker or events, a repeated slot, B outside
+ * 1..CC_MAX_FRAMES, cap < trk_cap, a frame side < 1, a non-finite clock, NULL pointers) fail with CC_ERR_INVALID before
+ * the launch. */
+#define CC_EVENT_MAX_VERTICES 256
+#define CC_EVENT_OK 0
+#define CC_EVENT_NEEDS_ROOM 1
+#define CC_EVENT_BAD_BOX 2
+#define CC_EVENT_NOT_RUN 3
+#define CC_EVENT_BAD_ORDER 4
+int cc_ocsort_gpu_events_configure(cc_ocsort_gpu* h, int slot, const double* zone_xy, int n_vertices, int outside,
+                                   int non_zone_alert, const uint32_t* class_mask, int capacity, void* stream);
+int cc_ocsort_gpu_events_grow(cc_ocsort_gpu* h, int slot, int capacity, void* stream);
+int cc_ocsort_gpu_events(cc_ocsort_gpu* h, const cc_track_job* jobs, int B, const int* frame_wh, const double* now,
+                         const double* d_trk_out, int trk_cap, const int* d_trk_count, const int* d_trk_status, double* d_preds,
+                         uint8_t* d_flags, int64_t* d_saves, int cap, int* d_counts, int* d_status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
