@@ -234,6 +234,30 @@ class CameraBatch:
         dev, i = self._where[name]
         return dev[i]
 
+    def save_objects(self, results: Dict[Hashable, CameraEvents], finder, quality: int = 95) -> Dict[Hashable, tuple]:
+        """The thumbnails and embeddings of every camera's object saves of the last step in ONE call (`save_object` and
+        `clip_latest_img`, clearcam.py:373-399, 272-279, 1278-1287): results is what `step_events` /
+        `step_events_mailboxes` returned; every camera's saves[:, 2:6] are cut from its `device_frame` in its own pixel
+        format by one `finder.encode_embed_frames` call -> {camera: (saves, files, embeddings)}, files and embedding rows
+        in saves order (embeddings None when CLIP is not initialised, or when the camera has no saves).  A step without
+        saves makes no library call.  Reads `device_frame`, so it is valid until the next step."""
+        cams = [name for name, ev in results.items() if len(ev.saves)]
+        out = {name: (ev.saves, [], None) for name, ev in results.items()}
+        if not cams:
+            return out
+        frames = [self.device_frame(name) for name in cams]
+        rects = np.concatenate([np.concatenate([np.full((len(results[name].saves), 1), j, np.int64),
+                                                np.asarray(results[name].saves, np.int64)[:, 2:6]], 1)
+                                for j, name in enumerate(cams)]).astype(np.int32)
+        files, emb = finder.encode_embed_frames(frames, [self.cams[name].pix_fmt for name in cams], rects, quality)
+        from .detection.yolov9 import DeviceResult
+        k = 0
+        for name in cams:
+            n = len(results[name].saves)
+            out[name] = (results[name].saves, files[k:k + n], None if emb is None else DeviceResult(emb.tensor[k:k + n]))
+            k += n
+        return out
+
     def step_mailboxes(self, mailboxes: Dict[Hashable, "FrameMailbox"]) -> Dict[Hashable, CameraResult]:
         """`step` on every camera whose mailbox (clearcam_b200.ingest) holds a frame this object has not seen yet —
         the reference's `if frame_num == last_frame_num: return` per camera (clearcam.py:446).  A camera seen here for

@@ -9,8 +9,11 @@
 // no fused multiply-add), 11-bit fixed-point taps, exact int32 horizontal pass, float32 vertical pass, round-half-even.
 //
 // HBM-bound and tiny next to the encoder (K x 224 x 224 outputs, 48 byte reads each, served from L1/L2): one thread per
-// output pixel, three channels, coalesced plane writes.
+// output pixel, three channels, coalesced plane writes.  Each rect carries its own source (frame pointer, extent, format),
+// so one call takes crops of frames of any shapes and formats (cc_clip_preprocess_frames); cc_clip_preprocess fills the
+// same table from one frame batch.
 #include <cstdint>
+#include <vector>
 
 #include "cc_common.h"
 #include "clearcam_b200.h"
@@ -20,11 +23,14 @@ namespace cc {
 namespace {
 
 constexpr int kRectsPerLaunch = 64;
+struct CropRect {
+  CropSource src;                   // the rect's frame, its extent and format (RGB / BGR / I420)
+  int x1, y1, x2, y2;               // validated on the host
+};
 struct CropParams {
-  const uint8_t* frames;
   float* out;
-  int H, W, S, swap, k0;            // swap: source channel order is BGR (the crop is RGB)
-  int rect[kRectsPerLaunch][5];     // frame, x1, y1, x2, y2 (validated on the host)
+  int S, k0;
+  CropRect rect[kRectsPerLaunch];
 };
 
 // source index of the first tap (+1) and the four fixed-point taps for destination index d (resize.cpp, a = -0.75)
@@ -46,15 +52,14 @@ __device__ __forceinline__ void cubic_taps(int d, int src, int dst, int& s, int 
   taps[3] = __float2int_rn(__fmul_rn(c3, 2048.f));
 }
 
-// I420: the frames are [n, H*3/2, W] planar YUV 4:2:0, converted per tap (to BGR, then swapped like a BGR frame)
+// One output pixel of rect k.  I420: the frame is [H*3/2, W] planar YUV 4:2:0, converted per tap (to BGR, then swapped
+// like a BGR frame); otherwise packed RGB / BGR, swapped unless RGB.
 template <bool I420>
-__global__ void __launch_bounds__(256) crop_resize_kernel(const __grid_constant__ CropParams p) {
-  const int dx = blockIdx.x * 32 + threadIdx.x, dy = blockIdx.y * 8 + threadIdx.y, k = blockIdx.z;
-  if (dx >= p.S || dy >= p.S) return;
-  const int fr = p.rect[k][0], x1 = p.rect[k][1], y1 = p.rect[k][2];
-  const int cw = p.rect[k][3] - x1, ch = p.rect[k][4] - y1;
-  const uint8_t* img = I420 ? p.frames + static_cast<size_t>(fr) * p.H * p.W * 3 / 2
-                            : p.frames + (static_cast<size_t>(fr) * p.H + y1) * p.W * 3 + static_cast<size_t>(x1) * 3;
+__device__ __forceinline__ void crop_resize_pixel(const CropParams& p, const CropRect& rc, int k, int dx, int dy) {
+  const CropSource& f = rc.src;
+  const int x1 = rc.x1, y1 = rc.y1;
+  const int cw = rc.x2 - x1, ch = rc.y2 - y1;
+  const uint8_t* img = I420 ? f.frame : f.frame + static_cast<size_t>(y1) * f.W * 3 + static_cast<size_t>(x1) * 3;
   int sx, sy, ax[4], ay[4];
   cubic_taps(dx, cw, p.S, sx, ax);
   cubic_taps(dy, ch, p.S, sy, ay);
@@ -62,14 +67,14 @@ __global__ void __launch_bounds__(256) crop_resize_kernel(const __grid_constant_
 #pragma unroll
   for (int r = 0; r < 4; ++r) {
     const int yy = min(max(sy - 1 + r, 0), ch - 1);
-    const uint8_t* row = img + static_cast<size_t>(yy) * p.W * 3;
+    const uint8_t* row = img + static_cast<size_t>(yy) * f.W * 3;
     int acc[3] = {0, 0, 0};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int xx = min(max(sx - 1 + j, 0), cw - 1);
       if constexpr (I420) {
         int px[3];
-        i420_bgr(img, p.H, p.W, y1 + yy, x1 + xx, px);       // absolute frame coordinates: the chroma of the full frame
+        i420_bgr(img, f.H, f.W, y1 + yy, x1 + xx, px);       // absolute frame coordinates: the chroma of the full frame
 #pragma unroll
         for (int c = 0; c < 3; ++c) acc[c] += px[c] * ax[j];
       } else {
@@ -85,10 +90,11 @@ __global__ void __launch_bounds__(256) crop_resize_kernel(const __grid_constant_
 #pragma unroll
   for (int r = 0; r < 4; ++r) b[r] = __fmul_rn(static_cast<float>(ay[r]), kInv);
   const int tail = (p.S * 3) / 8 * 8;            // interleaved elements past the last group of 8 take the integer form
+  const int swap = f.fmt != 0;                   // source channel order is BGR (the crop is RGB)
   float* out = p.out + static_cast<size_t>(p.k0 + k) * 3 * p.S * p.S + static_cast<size_t>(dy) * p.S + dx;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {                  // c indexes the crop's channel order after the optional BGR->RGB swap
-    const int sc = p.swap ? 2 - c : c;
+    const int sc = swap ? 2 - c : c;
     int v;
     if (dx * 3 + c < tail) {
       float t = __fmul_rn(static_cast<float>(hor[3][sc]), b[3]);
@@ -105,6 +111,34 @@ __global__ void __launch_bounds__(256) crop_resize_kernel(const __grid_constant_
     const float n = __fdiv_rn(__fsub_rn(__fdiv_rn(static_cast<float>(v), 255.f), 0.5f), 0.5f);     // models/objects.py:239-240
     out[static_cast<size_t>(c) * p.S * p.S] = n;
   }
+}
+
+// one CTA row of one rect (blockIdx.z): the source format is read per rect, so the branch is uniform per CTA
+__global__ void __launch_bounds__(256) crop_resize_kernel(const __grid_constant__ CropParams p) {
+  const int dx = blockIdx.x * 32 + threadIdx.x, dy = blockIdx.y * 8 + threadIdx.y, k = blockIdx.z;
+  if (dx >= p.S || dy >= p.S) return;
+  const CropRect& rc = p.rect[k];
+  if (rc.src.fmt == 2) crop_resize_pixel<true>(p, rc, k, dx, dy);
+  else crop_resize_pixel<false>(p, rc, k, dx, dy);
+}
+
+// the launches of one call over crops whose sources and rects are checked
+int crop_resize_sources(const CropSource* src, const int32_t* rects, int K, int size, float* d_out, cudaStream_t st) {
+  for (int k0 = 0; k0 < K; k0 += kRectsPerLaunch) {
+    CropParams p;
+    p.out = d_out;
+    p.S = size;
+    p.k0 = k0;
+    const int n = K - k0 < kRectsPerLaunch ? K - k0 : kRectsPerLaunch;
+    for (int i = 0; i < n; ++i) {
+      const int32_t* r = rects + 5 * (k0 + i);
+      p.rect[i] = CropRect{src[k0 + i], r[1], r[2], r[3], r[4]};
+    }
+    const dim3 grid((size + 31) / 32, (size + 7) / 8, n);
+    crop_resize_kernel<<<grid, dim3(32, 8), 0, st>>>(p);
+    CC_CHECK_CUDA(cudaGetLastError());
+  }
+  return CC_OK;
 }
 
 }  // namespace
@@ -124,23 +158,18 @@ extern "C" int cc_clip_preprocess(const uint8_t* d_frames, int n_frames, int H, 
                "cc_clip_preprocess: rect %d (frame %d, %d,%d-%d,%d) is empty or outside the %dx%d frame", k, r[0], r[1], r[2],
                r[3], r[4], W, H);
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  for (int k0 = 0; k0 < K; k0 += kRectsPerLaunch) {
-    CropParams p;
-    p.frames = d_frames;
-    p.out = d_out;
-    p.H = H;
-    p.W = W;
-    p.S = size;
-    p.swap = src_fmt != 0;
-    p.k0 = k0;
-    const int n = K - k0 < kRectsPerLaunch ? K - k0 : kRectsPerLaunch;
-    for (int i = 0; i < n; ++i)
-      for (int j = 0; j < 5; ++j) p.rect[i][j] = rects[5 * (k0 + i) + j];
-    const dim3 grid((size + 31) / 32, (size + 7) / 8, n);
-    if (src_fmt == 2) crop_resize_kernel<true><<<grid, dim3(32, 8), 0, st>>>(p);
-    else crop_resize_kernel<false><<<grid, dim3(32, 8), 0, st>>>(p);
-    CC_CHECK_CUDA(cudaGetLastError());
-  }
-  return CC_OK;
+  std::vector<CropSource> src(K);
+  uniform_crop_sources(d_frames, H, W, src_fmt, rects, K, src.data());
+  return crop_resize_sources(src.data(), rects, K, size, d_out, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int cc_clip_preprocess_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int size, float* d_out,
+                                         void* stream) {
+  using namespace cc;
+  const char* who = "cc_clip_preprocess_frames";
+  CC_REQUIRE(d_out, "%s: null pointer", who);
+  CC_REQUIRE(size >= 1 && size <= 4096, "%s: bad size %d", who, size);
+  std::vector<CropSource> src(K > 0 ? K : 0);
+  if (int rc = table_crop_sources(who, frames, n_frames, rects, K, src.data())) return rc;
+  return crop_resize_sources(src.data(), rects, K, size, d_out, static_cast<cudaStream_t>(stream));
 }

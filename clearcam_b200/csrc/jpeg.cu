@@ -6,7 +6,10 @@
 // frame) for frames that are already in HBM for the detector: only the compressed bytes cross PCIe.
 //
 // One call, per group of up to kCropsPerLaunch crops (the crop table travels as a kernel parameter, so there is no copy,
-// no allocation and no host sync), runs eight stream-ordered launches over all of its crops:
+// no allocation and no host sync), runs eight stream-ordered launches over all of its crops.  In the transform's table
+// every crop carries its own source (frame pointer, extent, RGB / BGR / I420), so the crops of one call may come from
+// frames of any shapes and formats (cc_jpeg_encode_crops_frames); the uniform entry points fill the same table from one
+// frame batch.
 //   1. transform  one CTA per MCU (16x16 pixels): gather with libjpeg's edge replication, YCbCr, h2v2 downsampling,
 //                 8x8 integer DCT, quantisation -> int16 zigzag coefficients of the 6 blocks, dummy blocks included
 //   2. lengths    one CTA per tile of kTileMcus MCUs, a warp per block: the bit length of every block's Huffman codes
@@ -39,7 +42,7 @@ constexpr int kZeroWords = 4096;                    // scratch words cleared per
 constexpr int kMaxSide = 65535;                     // a JPEG frame header holds 16-bit sizes
 
 struct JpegCrop {
-  int frame, x1, y1, w, h;
+  int x1, y1, w, h;
   int mw, nmcu;           // MCUs per row, MCUs
   int mcu0, tile0, ntile; // first MCU / tile of the crop in the launch group
   int zero0;              // first CTA of the crop in the zero kernel
@@ -53,8 +56,6 @@ struct HuffTables {
 };
 
 struct JpegParams {
-  const uint8_t* frames;
-  int H, W;
   int K, n_mcu, n_tile;
   int16_t* coef;                   // [n_mcu * 6][64], zigzag order
   uint32_t* blen;                  // [n_mcu * 6] bits per block
@@ -69,12 +70,29 @@ struct JpegParams {
   uint8_t header[kHeaderBytes];
   JpegCrop crop[kCropsPerLaunch];
 };
+// the largest launch (the scan kernel) passes two ints beside the table; 32,764 bytes is the kernel parameter limit
+static_assert(sizeof(JpegParams) + 2 * sizeof(int) <= 32764, "the crop table no longer fits the kernel parameters");
+
+// The transform's own, smaller table: only it reads the pixels, so only it carries each crop's source (the seven entropy
+// launches keep the table above and pay nothing for the sources).
+struct TransformCrop {
+  CropSource src;         // the crop's frame, its extent and format
+  int x1, y1, w, h;
+  int mw, mcu0;           // MCUs per row, first MCU of the crop in the launch group
+};
+struct TransformParams {
+  int K;
+  int16_t* coef;                   // [n_mcu * 6][64], zigzag order
+  uint16_t qdiv[2][64];            // 8 x quantisation table, natural order
+  TransformCrop crop[kCropsPerLaunch];
+};
+static_assert(sizeof(TransformParams) <= 32764, "the transform's crop table no longer fits the kernel parameters");
 
 __constant__ uint8_t kZigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
                                     41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
                                     30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
 
-__device__ __forceinline__ int find_crop_by_mcu(const JpegParams& p, int m) {
+__device__ __forceinline__ int find_crop_by_mcu(const TransformParams& p, int m) {
   int lo = 0, hi = p.K - 1;
   while (lo < hi) {
     const int mid = (lo + hi + 1) >> 1;
@@ -130,27 +148,27 @@ __device__ __forceinline__ void fdct8(int* d, int s) {
   d[s] = (tmp7 * kC1_501 + z1 + z4 + kHalf) >> kSh;
 }
 
-// FMT: 0 RGB, 1 BGR (packed [n,H,W,3]), 2 I420 ([n,H*3/2,W])
-template <int FMT>
-__global__ void __launch_bounds__(256) jpeg_transform_kernel(const __grid_constant__ JpegParams p) {
+// the crop's source format (CropSource::fmt) is read per CTA: one MCU belongs to one crop, so the branch is uniform
+__global__ void __launch_bounds__(256) jpeg_transform_kernel(const __grid_constant__ TransformParams p) {
   __shared__ int cb[16][16], cr[16][16];
   __shared__ int blk[6][64];
   __shared__ int dc[4];
   const int m = blockIdx.x, t = threadIdx.x;
-  const JpegCrop& c = p.crop[find_crop_by_mcu(p, m)];
+  const TransformCrop& c = p.crop[find_crop_by_mcu(p, m)];
   const int mi = m - c.mcu0, my = mi / c.mw, mx = mi - my * c.mw;
   const int py = t >> 4, px = t & 15;
   // columns replicated before downsampling, rows to the 2-row group (and, for luma, on to the MCU: same pixel)
   const int yy = c.y1 + min(my * 16 + py, c.h - 1), xx = c.x1 + min(mx * 16 + px, c.w - 1);
   int r, g, b;
-  if constexpr (FMT == 2) {
+  if (c.src.fmt == 2) {
     int bgr[3];
-    i420_bgr(p.frames + static_cast<size_t>(c.frame) * p.H * p.W * 3 / 2, p.H, p.W, yy, xx, bgr);
+    i420_bgr(c.src.frame, c.src.H, c.src.W, yy, xx, bgr);
     b = bgr[0]; g = bgr[1]; r = bgr[2];
   } else {
-    const uint8_t* px3 = p.frames + ((static_cast<size_t>(c.frame) * p.H + yy) * p.W + xx) * 3;
+    const uint8_t* px3 = c.src.frame + (static_cast<size_t>(yy) * c.src.W + xx) * 3;
     const int c0 = __ldg(px3), c1 = __ldg(px3 + 1), c2 = __ldg(px3 + 2);
-    r = FMT == 0 ? c0 : c2; g = c1; b = FMT == 0 ? c2 : c0;
+    const bool rgb = c.src.fmt == 0;
+    r = rgb ? c0 : c2; g = c1; b = rgb ? c2 : c0;
   }
   constexpr int kHalf = 1 << 15, kCbCrOff = (128 << 16) + kHalf - 1;
   const int Y = (fix16(0.299) * r + fix16(0.587) * g + fix16(0.114) * b + kHalf) >> 16;
@@ -657,9 +675,9 @@ int check_common(const char* who, const uint8_t* d_frames, int n_frames, int H, 
 }
 
 // the crop table of crops [k0, k0 + n); with_coef: coefficients at d_coef (the tap) instead of the workspace
-void fill_params(JpegParams& p, const uint8_t* d_frames, int H, int W, const int32_t* rects, int k0, int n, uint8_t* ws,
+void fill_params(JpegParams& p, TransformParams& t, const CropSource* src, const int32_t* rects, int k0, int n, uint8_t* ws,
                  const Layout& L, int16_t* d_coef, uint8_t* d_out, const int64_t* out_offsets, int64_t* d_lengths) {
-  p.frames = d_frames; p.H = H; p.W = W; p.K = n;
+  p.K = n;
   p.n_mcu = static_cast<int>(L.n_mcu); p.n_tile = static_cast<int>(L.n_tile);
   p.coef = d_coef ? d_coef : reinterpret_cast<int16_t*>(ws + L.coef);
   p.blen = reinterpret_cast<uint32_t*>(ws + L.blen);
@@ -669,17 +687,20 @@ void fill_params(JpegParams& p, const uint8_t* d_frames, int H, int W, const int
   p.words = reinterpret_cast<uint32_t*>(ws + L.wordsb);
   p.out = d_out;
   p.lengths = reinterpret_cast<long long*>(d_lengths);
+  t.K = n; t.coef = p.coef;
+  std::memcpy(t.qdiv, p.qdiv, sizeof(t.qdiv));
   int mcu = 0, tile = 0, zero = 0;
   long long word = 0;
   for (int i = 0; i < n; ++i) {
     const int32_t* r = rects + 5 * (k0 + i);
     JpegCrop& c = p.crop[i];
-    c.frame = r[0]; c.x1 = r[1]; c.y1 = r[2]; c.w = r[3] - r[1]; c.h = r[4] - r[2];
+    c.x1 = r[1]; c.y1 = r[2]; c.w = r[3] - r[1]; c.h = r[4] - r[2];
     const Geo g = geo(c.w, c.h);
     c.mw = g.mw; c.nmcu = static_cast<int>(g.nmcu());
     c.mcu0 = mcu; c.tile0 = tile; c.ntile = (c.nmcu + kTileMcus - 1) / kTileMcus; c.zero0 = zero;
     c.word0 = word;
     c.out = out_offsets ? out_offsets[k0 + i] : 0;
+    t.crop[i] = TransformCrop{src[k0 + i], c.x1, c.y1, c.w, c.h, c.mw, c.mcu0};
     mcu += c.nmcu; tile += c.ntile; word += g.words();
     zero += static_cast<int>((g.words() + kZeroWords - 1) / kZeroWords);
   }
@@ -691,40 +712,10 @@ int total_zero_ctas(const JpegParams& p) {
   return c.zero0 + static_cast<int>((w + kZeroWords - 1) / kZeroWords);
 }
 
-int launch_transform(const JpegParams& p, int src_fmt, cudaStream_t st) {
-  if (src_fmt == 0) jpeg_transform_kernel<0><<<p.n_mcu, 256, 0, st>>>(p);
-  else if (src_fmt == 1) jpeg_transform_kernel<1><<<p.n_mcu, 256, 0, st>>>(p);
-  else jpeg_transform_kernel<2><<<p.n_mcu, 256, 0, st>>>(p);
-  CC_CHECK_CUDA(cudaGetLastError());
-  return CC_OK;
-}
-
-}  // namespace
-
-// the quantisation tables the encoder writes for `quality` (natural order): what a decoder of its files dequantises with
-void jpeg_quant_tables(int quality, uint16_t qt[2][64]) {
-  static thread_local JpegParams p;
-  fill_tables(quality, p);
-  for (int t = 0; t < 2; ++t)
-    for (int i = 0; i < 64; ++i) qt[t][i] = static_cast<uint16_t>(p.qdiv[t][i] / 8);
-}
-
-}  // namespace cc
-
-using namespace cc;
-
-extern "C" int cc_jpeg_bound(int w, int h, int64_t* bytes) {
-  CC_REQUIRE(bytes != nullptr, "cc_jpeg_bound: bytes is NULL");
-  CC_REQUIRE(w >= 1 && h >= 1 && w <= kMaxSide && h <= kMaxSide, "cc_jpeg_bound: bad size %dx%d (1..%d)", w, h, kMaxSide);
-  *bytes = geo(w, h).bound();
-  return CC_OK;
-}
-
-extern "C" int cc_jpeg_encode_crops(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K,
-                                    int quality, uint8_t* d_out, int64_t out_bytes, const int64_t* out_offsets, int64_t* d_lengths,
-                                    void* d_workspace, size_t ws_bytes, size_t* ws_needed, void* stream) {
-  const char* who = "cc_jpeg_encode_crops";
-  if (int rc = check_common(who, d_frames, n_frames, H, W, src_fmt, rects, K, quality)) return rc;
+// cc_jpeg_encode_crops from the point where the crops' sources and rects are checked
+int encode_sources(const char* who, const CropSource* src, const int32_t* rects, int K, int quality, uint8_t* d_out,
+                   int64_t out_bytes, const int64_t* out_offsets, int64_t* d_lengths, void* d_workspace, size_t ws_bytes,
+                   size_t* ws_needed, void* stream) {
   size_t need = 0;
   for (int k0 = 0; k0 < K; k0 += kCropsPerLaunch)
     need = std::max(need, layout(rects, k0, std::min(K - k0, kCropsPerLaunch), true).total);
@@ -753,12 +744,13 @@ extern "C" int cc_jpeg_encode_crops(const uint8_t* d_frames, int n_frames, int H
                "%s: the output regions of crops %d and %d overlap (offset + cc_jpeg_bound)", who, order[i - 1], order[i]);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   static thread_local JpegParams p;              // ~17 KB of kernel parameters, kept off the stack
+  static thread_local TransformParams t;         // ~12 KB
   fill_tables(quality, p);
   for (int k0 = 0; k0 < K; k0 += kCropsPerLaunch) {
     const int n = std::min(K - k0, kCropsPerLaunch);
     const Layout L = layout(rects, k0, n, true);
-    fill_params(p, d_frames, H, W, rects, k0, n, static_cast<uint8_t*>(d_workspace), L, nullptr, d_out, out_offsets, d_lengths);
-    if (int rc = launch_transform(p, src_fmt, st)) return rc;
+    fill_params(p, t, src, rects, k0, n, static_cast<uint8_t*>(d_workspace), L, nullptr, d_out, out_offsets, d_lengths);
+    jpeg_transform_kernel<<<p.n_mcu, 256, 0, st>>>(t);
     jpeg_lengths_kernel<<<p.n_tile, 256, 0, st>>>(p);
     jpeg_scan_kernel<<<1, 1024, 0, st>>>(p, 0, k0);
     jpeg_zero_kernel<<<total_zero_ctas(p), 256, 0, st>>>(p);
@@ -771,25 +763,115 @@ extern "C" int cc_jpeg_encode_crops(const uint8_t* d_frames, int n_frames, int H
   return CC_OK;
 }
 
-extern "C" int cc_jpeg_coeffs(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K,
-                              int quality, int16_t* d_coef, int64_t* n_blocks, void* stream) {
-  const char* who = "cc_jpeg_coeffs";
-  if (int rc = check_common(who, d_frames, n_frames, H, W, src_fmt, rects, K, quality)) return rc;
+}  // namespace
+
+void uniform_crop_sources(const uint8_t* d_frames, int H, int W, int src_fmt, const int32_t* rects, int K, CropSource* src) {
+  const size_t frame_bytes = src_fmt == 2 ? static_cast<size_t>(H) * W * 3 / 2 : static_cast<size_t>(H) * W * 3;
+  for (int k = 0; k < K; ++k) src[k] = CropSource{d_frames + static_cast<size_t>(rects[5 * k]) * frame_bytes, H, W, src_fmt};
+}
+
+int table_crop_sources(const char* who, const cc_frame* frames, int n_frames, const int32_t* rects, int K, CropSource* src) {
+  CC_REQUIRE(frames && (rects || K == 0), "%s: null pointer", who);
+  CC_REQUIRE(n_frames > 0 && K >= 0, "%s: bad sizes n_frames=%d K=%d", who, n_frames, K);
+  for (int i = 0; i < n_frames; ++i) {
+    const cc_frame& f = frames[i];
+    CC_REQUIRE(f.data, "%s: frame %d is NULL", who, i);
+    CC_REQUIRE(f.fmt == CC_FRAME_BGR_U8 || f.fmt == CC_FRAME_I420_U8,
+               "%s: frame %d has format %d; crops take CC_FRAME_BGR_U8 (0) or CC_FRAME_I420_U8 (2) frames", who, i, f.fmt);
+    CC_REQUIRE(f.h > 0 && f.w > 0, "%s: frame %d has a bad size %dx%d", who, i, f.w, f.h);
+    CC_REQUIRE(f.fmt != CC_FRAME_I420_U8 || (f.h % 2 == 0 && f.w % 2 == 0),
+               "%s: frame %d: an I420 frame needs an even height and width, got %dx%d", who, i, f.w, f.h);
+  }
+  for (int k = 0; k < K; ++k) {
+    const int32_t* r = rects + 5 * k;
+    CC_REQUIRE(r[0] >= 0 && r[0] < n_frames, "%s: rect %d names frame %d of a %d-frame table", who, k, r[0], n_frames);
+    const cc_frame& f = frames[r[0]];
+    CC_REQUIRE(r[1] >= 0 && r[2] >= 0 && r[3] > r[1] && r[4] > r[2] && r[3] <= f.w && r[4] <= f.h,
+               "%s: rect %d (frame %d, %d,%d-%d,%d) is empty or outside its %dx%d frame", who, k, r[0], r[1], r[2], r[3], r[4],
+               f.w, f.h);
+    src[k] = CropSource{static_cast<const uint8_t*>(f.data), f.h, f.w, f.fmt == CC_FRAME_BGR_U8 ? 1 : 2};
+  }
+  return CC_OK;
+}
+
+int check_table_jpeg(const char* who, const int32_t* rects, int K, int quality) {
+  CC_REQUIRE(quality >= 0 && quality <= 100, "%s: quality %d outside 0..100", who, quality);
+  for (int k = 0; k < K; ++k)
+    CC_REQUIRE(rects[5 * k + 3] - rects[5 * k + 1] <= kMaxSide && rects[5 * k + 4] - rects[5 * k + 2] <= kMaxSide,
+               "%s: rect %d is larger than %d pixels", who, k, kMaxSide);
+  return CC_OK;
+}
+
+int jpeg_coeffs_sources(const CropSource* src, const int32_t* rects, int K, int quality, int16_t* d_coef, int64_t* n_blocks,
+                        cudaStream_t st) {
   long long blocks = 0;
   for (int k = 0; k < K; ++k) blocks += geo(rects[5 * k + 3] - rects[5 * k + 1], rects[5 * k + 4] - rects[5 * k + 2]).nmcu() * 6;
   if (n_blocks) *n_blocks = blocks;
   if (!d_coef) return CC_OK;                     // size query
-  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_coef) & 3) == 0, "%s: d_coef must be 4-byte aligned", who);
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   static thread_local JpegParams p;
+  static thread_local TransformParams t;
   fill_tables(quality, p);
   long long done = 0;
   for (int k0 = 0; k0 < K; k0 += kCropsPerLaunch) {
     const int n = std::min(K - k0, kCropsPerLaunch);
     const Layout L = layout(rects, k0, n, false);
-    fill_params(p, d_frames, H, W, rects, k0, n, nullptr, L, d_coef + done * 64, nullptr, nullptr, nullptr);
-    if (int rc = launch_transform(p, src_fmt, st)) return rc;
+    fill_params(p, t, src, rects, k0, n, nullptr, L, d_coef + done * 64, nullptr, nullptr, nullptr);
+    jpeg_transform_kernel<<<p.n_mcu, 256, 0, st>>>(t);
+    CC_CHECK_CUDA(cudaGetLastError());
     done += L.n_mcu * 6;
   }
   return CC_OK;
+}
+
+// the quantisation tables the encoder writes for `quality` (natural order): what a decoder of its files dequantises with
+void jpeg_quant_tables(int quality, uint16_t qt[2][64]) {
+  static thread_local JpegParams p;
+  fill_tables(quality, p);
+  for (int t = 0; t < 2; ++t)
+    for (int i = 0; i < 64; ++i) qt[t][i] = static_cast<uint16_t>(p.qdiv[t][i] / 8);
+}
+
+}  // namespace cc
+
+using namespace cc;
+
+extern "C" int cc_jpeg_bound(int w, int h, int64_t* bytes) {
+  CC_REQUIRE(bytes != nullptr, "cc_jpeg_bound: bytes is NULL");
+  CC_REQUIRE(w >= 1 && h >= 1 && w <= kMaxSide && h <= kMaxSide, "cc_jpeg_bound: bad size %dx%d (1..%d)", w, h, kMaxSide);
+  *bytes = geo(w, h).bound();
+  return CC_OK;
+}
+
+extern "C" int cc_jpeg_encode_crops(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K,
+                                    int quality, uint8_t* d_out, int64_t out_bytes, const int64_t* out_offsets, int64_t* d_lengths,
+                                    void* d_workspace, size_t ws_bytes, size_t* ws_needed, void* stream) {
+  const char* who = "cc_jpeg_encode_crops";
+  if (int rc = check_common(who, d_frames, n_frames, H, W, src_fmt, rects, K, quality)) return rc;
+  std::vector<CropSource> src(K);
+  uniform_crop_sources(d_frames, H, W, src_fmt, rects, K, src.data());
+  return encode_sources(who, src.data(), rects, K, quality, d_out, out_bytes, out_offsets, d_lengths, d_workspace, ws_bytes,
+                        ws_needed, stream);
+}
+
+extern "C" int cc_jpeg_encode_crops_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int quality,
+                                           uint8_t* d_out, int64_t out_bytes, const int64_t* out_offsets, int64_t* d_lengths,
+                                           void* d_workspace, size_t ws_bytes, size_t* ws_needed, void* stream) {
+  const char* who = "cc_jpeg_encode_crops_frames";
+  std::vector<CropSource> src(std::max(K, 0));
+  if (int rc = table_crop_sources(who, frames, n_frames, rects, K, src.data())) return rc;
+  if (int rc = check_table_jpeg(who, rects, K, quality)) return rc;
+  return encode_sources(who, src.data(), rects, K, quality, d_out, out_bytes, out_offsets, d_lengths, d_workspace, ws_bytes,
+                        ws_needed, stream);
+}
+
+extern "C" int cc_jpeg_coeffs(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K,
+                              int quality, int16_t* d_coef, int64_t* n_blocks, void* stream) {
+  const char* who = "cc_jpeg_coeffs";
+  if (int rc = check_common(who, d_frames, n_frames, H, W, src_fmt, rects, K, quality)) return rc;
+  std::vector<CropSource> src(K);
+  uniform_crop_sources(d_frames, H, W, src_fmt, rects, K, src.data());
+  jpeg_coeffs_sources(src.data(), rects, K, quality, nullptr, n_blocks, nullptr);
+  if (!d_coef) return CC_OK;                     // size query
+  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_coef) & 3) == 0, "%s: d_coef must be 4-byte aligned", who);
+  return jpeg_coeffs_sources(src.data(), rects, K, quality, d_coef, nullptr, static_cast<cudaStream_t>(stream));
 }

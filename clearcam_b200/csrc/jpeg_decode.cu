@@ -1061,13 +1061,12 @@ extern "C" int cc_jpeg_decode(const uint8_t* d_data, const void* h_table, const 
   return launch_recon(rp, imgs, st);
 }
 
-extern "C" int cc_jpeg_crops_decoded(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K,
-                                     int quality, uint8_t* d_out, int Hmax, int Wmax, int32_t* d_status, void* d_workspace,
-                                     size_t ws_bytes, size_t* ws_needed, void* stream) {
-  const char* who = "cc_jpeg_crops_decoded";
+// cc_jpeg_crops_decoded from the point where the crops' sources, rects and quality are checked
+static int crops_decoded_sources(const char* who, const CropSource* src, const int32_t* rects, int K, int quality, uint8_t* d_out,
+                                 int Hmax, int Wmax, int32_t* d_status, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
+                                 void* stream) {
   int64_t nb = 0;
-  // validates the frames, rects and quality exactly as the encoder does, and counts the blocks
-  if (int rc = cc_jpeg_coeffs(d_frames, n_frames, H, W, src_fmt, rects, K, quality, nullptr, &nb, nullptr)) return rc;
+  jpeg_coeffs_sources(src, rects, K, quality, nullptr, &nb, nullptr);     // counts the blocks
   std::vector<ReconImg> imgs(K);
   long long plane = 0, blk = 0;
   for (int k = 0; k < K; ++k) {
@@ -1098,7 +1097,7 @@ extern "C" int cc_jpeg_crops_decoded(const uint8_t* d_frames, int n_frames, int 
   uint16_t qt[2][64];
   jpeg_quant_tables(quality, qt);
   int16_t* coef = reinterpret_cast<int16_t*>(ws + 256);
-  if (int rc = cc_jpeg_coeffs(d_frames, n_frames, H, W, src_fmt, rects, K, quality, coef, &nb, stream)) return rc;
+  if (int rc = jpeg_coeffs_sources(src, rects, K, quality, coef, nullptr, st)) return rc;
   jdec_ok_kernel<<<(K + 255) / 256, 256, 0, st>>>(d_status, K);
   rp.coef = coef; rp.planes = ws + 256 + coef_bytes; rp.out = d_out; rp.status = d_status;
   rp.qbase = reinterpret_cast<const uint16_t*>(ws); rp.Hmax = Hmax; rp.Wmax = Wmax;
@@ -1106,4 +1105,26 @@ extern "C" int cc_jpeg_crops_decoded(const uint8_t* d_frames, int n_frames, int 
   std::memcpy(qa.q, qt, sizeof(qt));
   jdec_put_qt_kernel<<<1, 128, 0, st>>>(qa, reinterpret_cast<uint16_t*>(ws));
   return launch_recon(rp, imgs, st);
+}
+
+extern "C" int cc_jpeg_crops_decoded(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K,
+                                     int quality, uint8_t* d_out, int Hmax, int Wmax, int32_t* d_status, void* d_workspace,
+                                     size_t ws_bytes, size_t* ws_needed, void* stream) {
+  // validates the frames, rects and quality exactly as the encoder does
+  if (int rc = cc_jpeg_coeffs(d_frames, n_frames, H, W, src_fmt, rects, K, quality, nullptr, nullptr, nullptr)) return rc;
+  std::vector<CropSource> src(K);
+  uniform_crop_sources(d_frames, H, W, src_fmt, rects, K, src.data());
+  return crops_decoded_sources("cc_jpeg_crops_decoded", src.data(), rects, K, quality, d_out, Hmax, Wmax, d_status, d_workspace,
+                               ws_bytes, ws_needed, stream);
+}
+
+extern "C" int cc_jpeg_crops_decoded_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int quality,
+                                            uint8_t* d_out, int Hmax, int Wmax, int32_t* d_status, void* d_workspace,
+                                            size_t ws_bytes, size_t* ws_needed, void* stream) {
+  const char* who = "cc_jpeg_crops_decoded_frames";
+  std::vector<CropSource> src(K > 0 ? K : 0);
+  if (int rc = table_crop_sources(who, frames, n_frames, rects, K, src.data())) return rc;
+  if (int rc = check_table_jpeg(who, rects, K, quality)) return rc;
+  return crops_decoded_sources(who, src.data(), rects, K, quality, d_out, Hmax, Wmax, d_status, d_workspace, ws_bytes, ws_needed,
+                               stream);
 }

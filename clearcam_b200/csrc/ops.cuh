@@ -75,6 +75,21 @@ __device__ __forceinline__ void i420_bgr(const uint8_t* __restrict__ fr, int H, 
   bgr[2] = min(max((yy + 1673527 * v) >> 20, 0), 255);
 }
 
+// Where the crop kernels (JPEG transform, CLIP crop-resize) read one crop: its frame and that frame's extent and format.
+// Every crop carries its own source, so one launch cuts crops out of frames of different shapes and formats; the format
+// branch is uniform per CTA.  fmt: 0 RGB or 1 BGR (packed [H,W,3]), 2 I420 ([H*3/2,W], H and W even).
+struct CropSource { const uint8_t* frame; int H, W, fmt; };
+// The sources of a uniform call whose arguments are already checked: crop k reads frame rects[5k] of d_frames.
+void uniform_crop_sources(const uint8_t* d_frames, int H, int W, int src_fmt, const int32_t* rects, int K, CropSource* src);
+// The sources of a frame-table call (CC_FRAME_BGR_U8 -> BGR, CC_FRAME_I420_U8 -> I420), after checking the table and
+// that every rect (frame, x1, y1, x2, y2) is non-empty and inside its own frame; CC_ERR_INVALID names the first bad entry.
+int table_crop_sources(const char* who, const cc_frame* frames, int n_frames, const int32_t* rects, int K, CropSource* src);
+// What a frame-table JPEG call checks beyond table_crop_sources (jpeg.cu): the quality and the 16-bit header sizes.
+int check_table_jpeg(const char* who, const int32_t* rects, int K, int quality);
+// The JPEG transform of crops whose sources and rects are checked (jpeg.cu): the cc_jpeg_coeffs tap for any sources.
+int jpeg_coeffs_sources(const CropSource* src, const int32_t* rects, int K, int quality, int16_t* d_coef, int64_t* n_blocks,
+                        cudaStream_t st);
+
 // Letterbox: bilinear resize (utils/helpers.py:127-131 semantics, W axis first then H, result cast to the
 // input dtype after each axis) + zero pad (detection/yolov9.py:390-404).  fmt: a CC_FRAME_* code; out is HWC BGR, float32
 // for CC_FRAME_BGR_F32, else uint8 (I420 taps are converted to BGR before the interpolation).

@@ -25,7 +25,7 @@ import numpy as np
 import torch
 
 from . import padding
-from .._lib import CC_MAX_FRAMES, CCError, cc_frame, check, lib, ptr, stream_ptr
+from .._lib import CC_MAX_FRAMES, CCError, check, lib, ptr, stream_ptr
 from ..pixfmt import BGR24, CC_FRAME_BGR_F32, CC_FRAME_BGR_U8, CC_FRAME_I420_U8, check_pix_fmt, yuv420p_rows, yuv420p_size
 
 
@@ -96,6 +96,7 @@ def frame_table(frames, pix_fmts, res: int):
     """Validate a list of device frames for one frame-table call -> (ctypes cc_frame array, (net_h, net_w)).
     frames: uint8 CUDA tensors, [H,W,3] for "bgr24" or [H*3/2,W] for "yuv420p", or None for a padding row; pix_fmts: one
     format for all, or one per frame.  Raises ValueError before any library call that launches work."""
+    from ..ops import frame_table as check_frames
     frames = list(frames)
     B = len(frames)
     fmts = [pix_fmts] * B if isinstance(pix_fmts, str) else list(pix_fmts)
@@ -103,28 +104,15 @@ def frame_table(frames, pix_fmts, res: int):
         raise ValueError(f"{B} frames but {len(fmts)} pixel formats")
     if not 1 <= B <= CC_MAX_FRAMES:
         raise ValueError(f"a frame table holds 1 to {CC_MAX_FRAMES} frames, got {B}")
-    table = (cc_frame * B)()
+    table, sizes = check_frames(frames, fmts, padding=True)
     net = None
-    for i, (f, fmt) in enumerate(zip(frames, fmts)):
-        check_pix_fmt(fmt)
-        if f is None:
+    for i, (hw, fmt) in enumerate(zip(sizes, fmts)):
+        if hw is None:
             continue
-        if not isinstance(f, torch.Tensor) or not f.is_cuda or f.dtype != torch.uint8 or not f.is_contiguous():
-            raise ValueError(f"frame {i}: expected a contiguous uint8 CUDA tensor, got "
-                             f"{type(f).__name__} {getattr(f, 'dtype', '')} {tuple(getattr(f, 'shape', ()))}")
-        if fmt == BGR24:
-            if f.dim() != 3 or f.shape[2] != 3:
-                raise ValueError(f"frame {i}: a bgr24 frame is [H,W,3], got {tuple(f.shape)}")
-            H, W = int(f.shape[0]), int(f.shape[1])
-        else:
-            if f.dim() != 2:
-                raise ValueError(f"frame {i}: a yuv420p frame is [H*3/2,W], got {tuple(f.shape)}")
-            H, W = yuv420p_size(f.shape)
-        ns = net_shape(H, W, res, fmt)
+        ns = net_shape(*hw, res, fmt)
         if net is not None and ns != net:
-            raise ValueError(f"frame {i} ({H}x{W}) has net shape {ns}, an earlier frame {net}: one call takes one net shape")
+            raise ValueError(f"frame {i} ({hw[0]}x{hw[1]}) has net shape {ns}, an earlier frame {net}: one call takes one net shape")
         net = ns
-        table[i] = cc_frame(f.data_ptr(), CC_FRAME_BGR_U8 if fmt == BGR24 else CC_FRAME_I420_U8, H, W)
     if net is None:
         raise ValueError("every frame of the table is a padding row (None)")
     return table, net

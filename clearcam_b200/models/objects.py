@@ -375,6 +375,48 @@ class ObjectFinder:
         x = self.preprocess_device(pix, crops, bgr=True, rows=batch_bucket(k))
         return files, DeviceResult(self.model.precompute_embedding(x).tensor[:k])
 
+    def encode_embed_frames(self, frames, pix_fmts, rects, quality: int = 95):
+        """`encode_embed_crops` for the objects of many frames of different shapes and formats in one call (the saves of
+        every camera of a step): frames is a list of device frames, each [H,W,3] bgr24 or [H*3/2,W] yuv420p as its
+        pix_fmts entry says (one format for all, or one per frame); rects: K rows (frame index into `frames`, x1, y1, x2,
+        y2) -> (files, DeviceResult (K, embed_dim) or None).  File k is exactly what `encode_crops` writes for crop k of
+        its frame alone, and embedding k what `encode_embed_crops` stores for it, in a batch padded to batch_bucket(K).
+        Embeddings are None when CLIP is not initialised (the reference writes the thumbnails either way); then only the
+        encoder runs, and the host waits twice, for the lengths and for the bytes.
+        With CLIP, one encoder call, one crops-decoded call, one preprocess and one CLIP forward over all K crops are queued before
+        anything is read; then the host waits twice, whatever the number of frames or crops: once for the files' lengths
+        and the decoded crops' statuses together, once for the files' bytes.  A crop whose coefficients the device leaves
+        to cv2 (CC_JPEG_UNSUPPORTED, which only very low qualities reach) is decoded from its file on the host; the
+        preprocess then runs again over those crops only, and the CLIP forward is repeated on the same padded batch."""
+        from .. import ops
+        if not 0 <= int(quality) <= 100:
+            raise ValueError(f"quality must be in 0..100 (cv2's range), got {quality}")
+        frames = list(frames)
+        table, sizes = ops.frame_table(frames, pix_fmts)
+        r = ops.table_rects(rects, sizes)
+        K = len(r)
+        if K == 0:
+            return [], (None if self.model is None else
+                        DeviceResult(torch.empty(0, self.model.embed_dim, device="cuda", dtype=torch.float32)))
+        out, lengths, offsets = ops.jpeg_encode_launch_frames(table, len(frames), r, quality, frames[0].device)
+        if self.model is None:
+            return ops.jpeg_collect(out, lengths, lengths.cpu().numpy(), offsets), None
+        pix, status = ops.jpeg_crops_decoded_frames(frames, pix_fmts, r, quality, table=(table, r))
+        crops = [(i, 0, 0, int(x2 - x1), int(y2 - y1)) for i, (_, x1, y1, x2, y2) in enumerate(r)]
+        x = self.preprocess_device(pix, crops, bgr=True, rows=batch_bucket(K)).tensor
+        emb = self.model.precompute_embedding(x).tensor
+        got = torch.cat([lengths, status.long()]).cpu().numpy()                 # host wait 1
+        files = ops.jpeg_collect(out, lengths, got[:K], offsets)                # host wait 2
+        bad = [int(i) for i in np.flatnonzero(got[K:] != ops.JPEG_OK)]
+        if bad:
+            import cv2                                  # coefficients outside the range every libjpeg-turbo IDCT agrees on
+            for i in bad:
+                img = cv2.imdecode(np.frombuffer(files[i], np.uint8), cv2.IMREAD_COLOR)
+                pix[i, :img.shape[0], :img.shape[1]] = torch.from_numpy(img).to(pix.device)
+            x[torch.tensor(bad, device=x.device)] = self.preprocess_device(pix, [crops[i] for i in bad], bgr=True).tensor
+            emb = self.model.precompute_embedding(x).tensor
+        return files, DeviceResult(emb[:K])
+
     def _device_index(self):
         """Contiguous device copy of `image_embeddings` plus, per row, what `search` filters and groups on — rebuilt
         whenever a key OR the array stored under a key changes (the fingerprint holds the identity of every value, so an

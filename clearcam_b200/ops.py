@@ -167,29 +167,76 @@ def _rects_i32(rects):
     return np.ascontiguousarray(np.asarray(rects, np.int32).reshape(-1, 5))
 
 
-def jpeg_encode_crops(frames, rects, quality=95, src_fmt=1, stream=None):
-    """frames: uint8 CUDA [n,H,W,3] (src_fmt 0 RGB, 1 BGR) or [n,H*3/2,W] (2 I420); rects: K rows (frame, x1, y1, x2, y2)
-    -> list of K `bytes`, each the file cv2.imwrite writes for that crop at `quality`.  The crops go into one device buffer
-    at offsets given by the prefix sum of their bounds; only the lengths and then the used bytes come back to the host."""
+# ---- frame tables: device frames of different shapes and formats in one call
+def frame_table(frames, pix_fmts, padding=False):
+    """Validate a list of device frames with per-frame formats -> (ctypes cc_frame array, [(H, W) or None per frame]).
+    frames: contiguous uint8 CUDA tensors, [H,W,3] for "bgr24" or [H*3/2,W] for "yuv420p" (H, W even); with `padding`, None
+    is a padding row.  pix_fmts: one format for all, or one per frame.  Raises ValueError; calls nothing in the library."""
+    from ._lib import cc_frame
+    from .pixfmt import BGR24, CC_FRAME_BGR_U8, CC_FRAME_I420_U8, check_pix_fmt, yuv420p_size
+    frames = list(frames)
+    B = len(frames)
+    fmts = [pix_fmts] * B if isinstance(pix_fmts, str) else list(pix_fmts)
+    if len(fmts) != B:
+        raise ValueError(f"{B} frames but {len(fmts)} pixel formats")
+    table = (cc_frame * max(B, 1))()
+    sizes = []
+    for i, (f, fmt) in enumerate(zip(frames, fmts)):
+        check_pix_fmt(fmt)
+        if f is None and padding:
+            sizes.append(None)
+            continue
+        if not isinstance(f, torch.Tensor) or not f.is_cuda or f.dtype != torch.uint8 or not f.is_contiguous():
+            raise ValueError(f"frame {i}: expected a contiguous uint8 CUDA tensor, got "
+                             f"{type(f).__name__} {getattr(f, 'dtype', '')} {tuple(getattr(f, 'shape', ()))}")
+        if fmt == BGR24:
+            if f.dim() != 3 or f.shape[2] != 3:
+                raise ValueError(f"frame {i}: a bgr24 frame is [H,W,3], got {tuple(f.shape)}")
+            H, W = int(f.shape[0]), int(f.shape[1])
+        else:
+            if f.dim() != 2:
+                raise ValueError(f"frame {i}: a yuv420p frame is [H*3/2,W], got {tuple(f.shape)}")
+            H, W = yuv420p_size(f.shape)
+        sizes.append((H, W))
+        table[i] = cc_frame(f.data_ptr(), CC_FRAME_BGR_U8 if fmt == BGR24 else CC_FRAME_I420_U8, H, W)
+    return table, sizes
+
+
+def table_rects(rects, sizes):
+    """rects: K rows (frame, x1, y1, x2, y2) against a frame table's sizes -> contiguous int32 [K,5]; ValueError for a
+    frame index outside the table or a rect that is empty or leaves its own frame."""
     import numpy as np
-    n, H, W = _jpeg_frames(frames, src_fmt)
     r = _rects_i32(rects)
+    for k, (f, x1, y1, x2, y2) in enumerate(r.tolist()):
+        if not 0 <= f < len(sizes) or sizes[f] is None:
+            raise ValueError(f"rect {k} names frame {f} of a {len(sizes)}-frame table")
+        H, W = sizes[f]
+        if not (0 <= x1 < x2 <= W and 0 <= y1 < y2 <= H):
+            raise ValueError(f"rect {k} ({x1},{y1}-{x2},{y2}) is empty or outside its frame {f} ({W}x{H})")
+    return np.ascontiguousarray(r)
+
+
+def _jpeg_encode_launch(fn, args, r, dev, stream):
+    """Queue one encoder call (uniform or table form: fn(*args, d_out, ...)) -> (out, device lengths, offsets)."""
+    import numpy as np
     K = len(r)
-    if K == 0:
-        return []
     bounds = np.array([jpeg_bound(x2 - x1, y2 - y1) if x2 > x1 and y2 > y1 else 0 for _, x1, y1, x2, y2 in r], np.int64)
     offsets = np.ascontiguousarray(np.concatenate([[0], np.cumsum(bounds)[:-1]]).astype(np.int64))
     need = ctypes.c_size_t(0)
-    args = (ptr(frames), n, H, W, src_fmt, r.ctypes.data, K, int(quality))
-    check(lib().cc_jpeg_encode_crops(*args, None, 0, None, None, None, 0, ctypes.byref(need), None), "cc_jpeg_encode_crops")
-    dev = frames.device
+    check(getattr(lib(), fn)(*args, None, 0, None, None, None, 0, ctypes.byref(need), None), fn)
     out = torch.empty(int(bounds.sum()), dtype=torch.uint8, device=dev)
     lengths = torch.empty(K, dtype=torch.int64, device=dev)
     ws = torch.empty(max(need.value, 1), dtype=torch.uint8, device=dev)
-    check(lib().cc_jpeg_encode_crops(*args, ptr(out), out.numel(), offsets.ctypes.data, ptr(lengths), ptr(ws), need.value, None,
-                                     stream_ptr(stream)), "cc_jpeg_encode_crops")
-    lens = lengths.cpu().numpy()
-    # gather the used bytes of every crop into one contiguous device run, then one copy to the host
+    check(getattr(lib(), fn)(*args, ptr(out), out.numel(), offsets.ctypes.data, ptr(lengths), ptr(ws), need.value, None,
+                             stream_ptr(stream)), fn)
+    return out, lengths, offsets
+
+
+def jpeg_collect(out, lengths, lens, offsets):
+    """The encoded files: the used bytes of every crop gathered into one device run, one copy to the host (one wait).
+    lens: the lengths already on the host."""
+    import numpy as np
+    dev = out.device
     total = int(lens.sum())
     starts = torch.cumsum(lengths, 0) - lengths
     idx = torch.arange(total, device=dev) + torch.repeat_interleave(torch.from_numpy(offsets).to(dev) - starts, lengths,
@@ -197,6 +244,68 @@ def jpeg_encode_crops(frames, rects, quality=95, src_fmt=1, stream=None):
     flat = out[idx].cpu().numpy().tobytes()
     ends = np.cumsum(lens)
     return [flat[e - l:e] for e, l in zip(ends, lens)]
+
+
+def jpeg_encode_crops_frames(frames, pix_fmts, rects, quality=95, stream=None):
+    """jpeg_encode_crops over frames of different shapes and formats in one call: frames / pix_fmts as in `frame_table`,
+    rects: K rows (frame index into `frames`, x1, y1, x2, y2) -> list of K `bytes`, file k being exactly what
+    jpeg_encode_crops gives for that crop of its frame alone.  Two host waits: the lengths, then the bytes."""
+    table, sizes = frame_table(frames, pix_fmts)
+    if not sizes:
+        raise ValueError("a frame table needs at least one frame")
+    r = table_rects(rects, sizes)
+    if len(r) == 0:
+        return []
+    out, lengths, offsets = jpeg_encode_launch_frames(table, len(sizes), r, quality, frames[0].device, stream)
+    return jpeg_collect(out, lengths, lengths.cpu().numpy(), offsets)
+
+
+def jpeg_encode_launch_frames(table, n_frames, r, quality, dev, stream=None):
+    """Queue cc_jpeg_encode_crops_frames for a checked table and rects -> (out, device lengths, offsets); nothing waits."""
+    return _jpeg_encode_launch("cc_jpeg_encode_crops_frames", (table, n_frames, r.ctypes.data, len(r), int(quality)), r, dev,
+                               stream)
+
+
+def jpeg_crops_decoded_frames(frames, pix_fmts, rects, quality=95, out=None, stream=None, table=None):
+    """jpeg_crops_decoded over frames of different shapes and formats in one call (frames / pix_fmts / rects as in
+    jpeg_encode_crops_frames) -> (uint8 CUDA [K, Hmax, Wmax, 3], device int32 status [K]); crop k's slot and status are what
+    jpeg_crops_decoded gives for that crop of its frame alone.  Nothing waits.  table: a checked (frame_table, rects) pair
+    to reuse instead of checking again."""
+    if table is None:
+        t, sizes = frame_table(frames, pix_fmts)
+        if not sizes:
+            raise ValueError("a frame table needs at least one frame")
+        table = (t, table_rects(rects, sizes))
+    t, r = table
+    K = len(r)
+    dev = frames[0].device
+    if out is None:
+        hmax = max([int(y2 - y1) for _, _, y1, _, y2 in r] + [1])
+        wmax = max([int(x2 - x1) for _, x1, _, x2, _ in r] + [1])
+        out = torch.zeros(K, hmax, wmax, 3, dtype=torch.uint8, device=dev)
+    args = (t, len(frames), r.ctypes.data, K, int(quality))
+    need = ctypes.c_size_t(0)
+    check(lib().cc_jpeg_crops_decoded_frames(*args, None, 0, 0, None, None, 0, ctypes.byref(need), None),
+          "cc_jpeg_crops_decoded_frames")
+    ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=dev)
+    status = torch.empty(max(K, 1), dtype=torch.int32, device=dev)
+    check(lib().cc_jpeg_crops_decoded_frames(*args, ptr(out), out.shape[1], out.shape[2], ptr(status), ptr(ws), ws.numel(), None,
+                                             stream_ptr(stream)), "cc_jpeg_crops_decoded_frames")
+    return out, status[:K]
+
+
+def jpeg_encode_crops(frames, rects, quality=95, src_fmt=1, stream=None):
+    """frames: uint8 CUDA [n,H,W,3] (src_fmt 0 RGB, 1 BGR) or [n,H*3/2,W] (2 I420); rects: K rows (frame, x1, y1, x2, y2)
+    -> list of K `bytes`, each the file cv2.imwrite writes for that crop at `quality`.  The crops go into one device buffer
+    at offsets given by the prefix sum of their bounds; only the lengths and then the used bytes come back to the host."""
+    n, H, W = _jpeg_frames(frames, src_fmt)
+    r = _rects_i32(rects)
+    K = len(r)
+    if K == 0:
+        return []
+    out, lengths, offsets = _jpeg_encode_launch("cc_jpeg_encode_crops", (ptr(frames), n, H, W, src_fmt, r.ctypes.data, K,
+                                                                         int(quality)), r, frames.device, stream)
+    return jpeg_collect(out, lengths, lengths.cpu().numpy(), offsets)
 
 
 def jpeg_coeffs(frames, rects, quality=95, src_fmt=1, stream=None):

@@ -270,6 +270,12 @@ int cc_search_topk(const float* d_index, int N, int D, const float* d_q, const i
  * cc_clip_encode_image takes. */
 int cc_clip_preprocess(const uint8_t* d_frames, int n_frames, int H, int W, const int32_t* rects, int K, int size,
                        int src_fmt, float* d_out, void* stream);
+/* The same over a frame table: frames (HOST array of n_frames cc_frame rows, read during the call only) of any shapes,
+ * CC_FRAME_BGR_U8 or CC_FRAME_I420_U8 (h, w even); rect r[0] indexes the table and must lie inside its own frame.  Crop k
+ * of the output is what cc_clip_preprocess gives for that crop called on its frame alone.  A NULL frame, another format,
+ * an odd I420 side or a rect outside its own frame fails with CC_ERR_INVALID before anything is launched. */
+int cc_clip_preprocess_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int size, float* d_out,
+                              void* stream);
 
 /* Object thumbnails on the device: baseline JPEG of frame crops, byte for byte the file cv2.imwrite(path, crop) writes at
  * IMWRITE_JPEG_QUALITY `quality` (`VideoCapture.save_object`, clearcam.py:373-399): 4:2:0, integer DCT, Annex K tables,
@@ -290,6 +296,12 @@ int cc_jpeg_encode_crops(const uint8_t* d_frames, int n_frames, int H, int W, in
                          size_t ws_bytes, size_t* ws_needed, void* stream);
 int cc_jpeg_coeffs(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K, int quality,
                    int16_t* d_coef, int64_t* n_blocks, void* stream);
+/* cc_jpeg_encode_crops over a frame table (cc_clip_preprocess_frames' rules for frames and rects): one call encodes the
+ * crops of frames of different shapes and formats, crop k's bytes and length being what cc_jpeg_encode_crops gives for
+ * that crop called on its frame alone. */
+int cc_jpeg_encode_crops_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int quality, uint8_t* d_out,
+                                int64_t out_bytes, const int64_t* out_offsets, int64_t* d_lengths, void* d_workspace,
+                                size_t ws_bytes, size_t* ws_needed, void* stream);
 
 /* JPEG files -> BGR uint8 on the device, pixel for pixel what cv2.imdecode(buf, IMREAD_COLOR) returns (libjpeg-turbo 3.1:
  * islow IDCT, fancy upsampling, table-driven YCbCr -> BGR); oracle/jpeg_decode.py states the arithmetic.  Replaces the host
@@ -331,6 +343,11 @@ int cc_jpeg_decode(const uint8_t* d_data, const void* h_table, const void* d_tab
 int cc_jpeg_crops_decoded(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K, int quality,
                           uint8_t* d_out, int Hmax, int Wmax, int32_t* d_status, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
                           void* stream);
+/* cc_jpeg_crops_decoded over a frame table (cc_clip_preprocess_frames' rules): crop k's pixels and status are what
+ * cc_jpeg_crops_decoded gives for that crop called on its frame alone. */
+int cc_jpeg_crops_decoded_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int quality, uint8_t* d_out,
+                                 int Hmax, int Wmax, int32_t* d_status, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
+                                 void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Tracker that consumes the detector rows (host code, no GPU): ocsort_tracker/ocsort.py:163-308 `OCSort`, with
