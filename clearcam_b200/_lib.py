@@ -113,6 +113,11 @@ _SIGS = {
     "cc_conv2d_pre": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _i, _vp]),
     "cc_conv2d_fp32_accurate": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp,
                                      ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t), _vp]),
+    "cc_patchify": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
+    "cc_clip_embed_ln": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "cc_layernorm_bf16": (_i, [_vp, _i, _i, ctypes.c_longlong, _vp, _vp, _vp, _vp, _vp]),
+    "cc_text_embed": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "cc_l2norm": (_i, [_vp, _i, _i, _f, _vp, ctypes.c_longlong, _vp]),
     "cc_jpeg_bound": (_i, [_i, _i, ctypes.POINTER(ctypes.c_int64)]),
     "cc_jpeg_encode_crops": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, ctypes.c_int64, _vp, _vp, _vp, ctypes.c_size_t,
                                   ctypes.POINTER(ctypes.c_size_t), _vp]),

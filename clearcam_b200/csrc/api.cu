@@ -180,3 +180,66 @@ int cc_conv2d_pre(const void* d_in, int N, int Hin, int Win, int in_cs, int in_c
 }
 
 }  // extern "C"
+
+// ---- the CLIP encoders' row kernels (vit.cu) as the plans run them
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+static int ln_width_arg(const char* who, int W) {
+  CC_REQUIRE(layernorm_width_supported(W), "%s: width %d not supported (128 x 1, 2, 3, 4, 5, 6, 8, 10 or 12)", who, W);
+  return CC_OK;
+}
+
+extern "C" {
+
+int cc_patchify(const float* d_x, int B, int S, int p, int Kpad, void* d_out, void* stream) {
+  CC_REQUIRE(d_x && d_out, "cc_patchify: d_x and d_out must not be NULL");
+  CC_REQUIRE(aligned16(d_out), "cc_patchify: d_out must be 16-byte aligned");
+  CC_REQUIRE(B >= 0 && S >= 1 && p >= 1, "cc_patchify: bad shape B=%d S=%d p=%d", B, S, p);
+  CC_REQUIRE(S % p == 0, "cc_patchify: image side %d is not a multiple of the patch %d", S, p);
+  CC_REQUIRE(Kpad % 8 == 0 && Kpad >= 3 * p * p, "cc_patchify: Kpad=%d must be a multiple of 8 and at least 3p^2 = %d", Kpad,
+             3 * p * p);
+  if (B == 0) return CC_OK;
+  return patchify_launch(d_x, static_cast<__nv_bfloat16*>(d_out), B, S, p, Kpad, static_cast<cudaStream_t>(stream));
+}
+
+int cc_clip_embed_ln(float* d_x, const float* d_cls, const float* d_pos, const float* d_gamma, const float* d_beta, int B, int L, int W,
+                     void* stream) {
+  CC_REQUIRE(d_x && d_cls && d_pos && d_gamma && d_beta, "cc_clip_embed_ln: a NULL pointer");
+  CC_REQUIRE(aligned16(d_x) && aligned16(d_cls) && aligned16(d_pos) && aligned16(d_gamma) && aligned16(d_beta),
+             "cc_clip_embed_ln: every pointer must be 16-byte aligned");
+  CC_REQUIRE(B >= 0 && L >= 1 && static_cast<long long>(B) * L <= 0x7fffffffLL, "cc_clip_embed_ln: bad shape B=%d L=%d", B, L);
+  if (int rc = ln_width_arg("cc_clip_embed_ln", W)) return rc;
+  if (B == 0) return CC_OK;
+  return embed_ln_pre_launch(d_x, d_cls, d_pos, d_gamma, d_beta, B * L, L, W, static_cast<cudaStream_t>(stream));
+}
+
+int cc_layernorm_bf16(const float* d_x, int rows, int W, long long row_stride, const int32_t* d_row_idx, const float* d_gamma,
+                      const float* d_beta, void* d_out, void* stream) {
+  CC_REQUIRE(d_x && d_gamma && d_beta && d_out, "cc_layernorm_bf16: d_x, d_gamma, d_beta and d_out must not be NULL");
+  CC_REQUIRE(aligned16(d_x) && aligned16(d_gamma) && aligned16(d_beta), "cc_layernorm_bf16: d_x, d_gamma and d_beta must be 16-byte aligned");
+  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_out) & 7) == 0, "cc_layernorm_bf16: d_out must be 8-byte aligned");
+  CC_REQUIRE(rows >= 0 && row_stride >= 0, "cc_layernorm_bf16: bad shape rows=%d row_stride=%lld", rows, row_stride);
+  if (int rc = ln_width_arg("cc_layernorm_bf16", W)) return rc;
+  return layernorm_bf16_launch(d_x, static_cast<__nv_bfloat16*>(d_out), d_gamma, d_beta, rows, W, row_stride, d_row_idx,
+                               static_cast<cudaStream_t>(stream));
+}
+
+int cc_text_embed(const int32_t* d_ids, const float* d_tok, const float* d_pos, int B, int L, int W, int vocab, float* d_x,
+                  int32_t* d_eot_row, void* stream) {
+  CC_REQUIRE(d_ids && d_tok && d_pos && d_x && d_eot_row, "cc_text_embed: a NULL pointer");
+  CC_REQUIRE(aligned16(d_tok) && aligned16(d_pos) && aligned16(d_x), "cc_text_embed: d_tok, d_pos and d_x must be 16-byte aligned");
+  CC_REQUIRE(B >= 0 && L >= 1 && W >= 4 && W % 4 == 0 && vocab >= 1 && static_cast<long long>(B) * L <= 0x7fffffffLL,
+             "cc_text_embed: bad shape B=%d L=%d W=%d vocab=%d (W a multiple of 4)", B, L, W, vocab);
+  if (B == 0) return CC_OK;
+  return text_embed_launch(d_ids, d_tok, d_pos, d_x, d_eot_row, B, L, W, vocab, static_cast<cudaStream_t>(stream));
+}
+
+int cc_l2norm(const float* d_in, int rows, int D, float eps, float* d_out, long long out_stride, void* stream) {
+  CC_REQUIRE(d_in && d_out, "cc_l2norm: d_in and d_out must not be NULL");
+  CC_REQUIRE(rows >= 0 && D >= 1, "cc_l2norm: bad shape rows=%d D=%d", rows, D);
+  CC_REQUIRE(out_stride >= D, "cc_l2norm: out_stride %lld is shorter than a row of %d", out_stride, D);
+  CC_REQUIRE(eps >= 0.f, "cc_l2norm: eps must be >= 0");
+  return l2norm_launch(d_in, d_out, rows, D, out_stride, eps, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

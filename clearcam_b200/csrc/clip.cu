@@ -240,12 +240,17 @@ extern "C" {
 int cc_clip_create(const cc_clip_config* cfg, int n_tensors, const char* const* names, const float* const* h_data,
                    const int64_t* numels, cc_clip** out) {
   CC_REQUIRE(cfg && out, "cc_clip_create: null argument");
+  // the configuration first: a CPU-only caller sees the same refusal
+  CC_REQUIRE(cfg->patch >= 1 && cfg->image_size >= cfg->patch && cfg->image_size % cfg->patch == 0 && cfg->v_layers >= 0 &&
+                 cfg->t_layers >= 0 && cfg->v_width == cfg->v_heads * 64 && cfg->t_width == cfg->t_heads * 64 &&
+                 cfg->embed_dim >= 16 && cfg->embed_dim % 16 == 0 && cfg->v_mlp >= 16 && cfg->v_mlp % 16 == 0 &&
+                 cfg->t_mlp >= 16 && cfg->t_mlp % 16 == 0 && cfg->vocab >= 1 && cfg->ctx >= 1,
+             "cc_clip_create: unsupported architecture (need width = 64*heads, image size a multiple of the patch)");
+  CC_REQUIRE(layernorm_width_supported(cfg->v_width) && layernorm_width_supported(cfg->t_width),
+             "cc_clip_create: widths %d / %d not supported by the LayerNorm kernels (128 x 1, 2, 3, 4, 5, 6, 8, 10 or 12)",
+             cfg->v_width, cfg->t_width);
   const int sms = device_sm_count();
   CC_REQUIRE(sms > 0, "cc_clip_create: no sm_90 (H100) device");
-  CC_REQUIRE(cfg->image_size % cfg->patch == 0 && cfg->v_width % 128 == 0 && cfg->t_width % 128 == 0 &&
-                 cfg->v_width == cfg->v_heads * 64 && cfg->t_width == cfg->t_heads * 64 && cfg->embed_dim % 16 == 0 &&
-                 cfg->v_mlp % 16 == 0 && cfg->t_mlp % 16 == 0,
-             "cc_clip_create: unsupported architecture (need width = 64*heads, widths multiple of 128)");
   std::unique_ptr<cc_clip> h(new cc_clip());
   ClipModel& M = h->m;
   M.cfg = *cfg; M.sms = sms;

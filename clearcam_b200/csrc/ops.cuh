@@ -174,6 +174,7 @@ int layernorm_bf16_launch(const float* x, __nv_bfloat16* out, const float* gamma
 int text_embed_launch(const int* ids, const float* tok, const float* pos, float* x, int* eot_row, int B, int L, int W,
                       int vocab, cudaStream_t st);
 int l2norm_launch(const float* in, float* out, int rows, int D, long long out_stride, float eps, cudaStream_t st);
+bool layernorm_width_supported(int W);   // the widths the LayerNorm kernels are instantiated for: 128 x {1..6, 8, 10, 12}
 int attention_launch(const __nv_bfloat16* qkv, __nv_bfloat16* ctx, int B, int L, int H, int causal, cudaStream_t st);
 int attention_max_len();      // longest sequence whose K and V fit the mma.sync kernel's shared memory
 // wgmma attention (attention_tc.cu); vt_ws: workspace of attention_tc_workspace_bytes() for the per-head V^T copy

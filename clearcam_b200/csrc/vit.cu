@@ -157,6 +157,13 @@ static int dispatch_n4(int W, F&& f) {
   return CC_ERR_INVALID;
 }
 
+// the cases of dispatch_n4
+bool layernorm_width_supported(int W) {
+  if (W <= 0 || W % 128 != 0) return false;
+  const int n4 = W / 128;
+  return n4 <= 6 || n4 == 8 || n4 == 10 || n4 == 12;
+}
+
 int embed_ln_pre_launch(float* x, const float* cls, const float* pos, const float* gamma, const float* beta, int rows, int L,
                         int W, cudaStream_t st) {
   CC_REQUIRE(W % 128 == 0, "embed_ln_pre: width %d not a multiple of 128", W);

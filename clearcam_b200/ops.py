@@ -142,6 +142,76 @@ def conv2d_fp32_accurate(xbuf, in_co, Cin, w, bias, stride, act, obuf, out_co, r
     return obuf
 
 
+# ---- the CLIP encoders' row kernels, as the plans run them (include/clearcam_b200.h)
+def _f32_cuda(*ts):
+    for t in ts:
+        assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()
+
+
+def patchify(x, p, kpad, out=None, stream=None):
+    """x: fp32 [B,3,S,S] CUDA -> bf16 [B*(S/p)^2, kpad] patch matrix (zeros past 3p^2)."""
+    _f32_cuda(x)
+    B, _, S, _ = x.shape
+    if out is None:
+        out = torch.empty(B * (S // p) ** 2, kpad, dtype=torch.bfloat16, device=x.device)
+    assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.shape[-1] == kpad
+    check(lib().cc_patchify(ptr(x), B, S, p, kpad, ptr(out), stream_ptr(stream)), "cc_patchify")
+    return out
+
+
+def clip_embed_ln(x, cls, pos, gamma, beta, L, stream=None):
+    """In place on x fp32 [B*L, W]: token 0 := cls, + pos[t], then ln_pre with gamma / beta."""
+    _f32_cuda(x, cls, pos, gamma, beta)
+    W = x.shape[-1]
+    assert x.shape[0] % L == 0 and pos.numel() == L * W
+    check(lib().cc_clip_embed_ln(ptr(x), ptr(cls), ptr(pos), ptr(gamma), ptr(beta), x.shape[0] // L, L, W, stream_ptr(stream)),
+          "cc_clip_embed_ln")
+    return x
+
+
+def layernorm_bf16(x, gamma, beta, rows=None, row_stride=1, row_idx=None, out=None, stream=None):
+    """x fp32 [n, W] -> bf16 [rows, W]: LayerNorm of rows r * row_stride, or of rows row_idx[r] (int32 CUDA) when given."""
+    _f32_cuda(x, gamma, beta)
+    W = x.shape[-1]
+    if rows is None:
+        rows = row_idx.numel() if row_idx is not None else (x.shape[0] + row_stride - 1) // max(row_stride, 1)
+    if row_idx is not None:
+        assert row_idx.is_cuda and row_idx.dtype == torch.int32 and row_idx.numel() >= rows
+    if out is None:
+        out = torch.empty(rows, W, dtype=torch.bfloat16, device=x.device)
+    assert out.dtype == torch.bfloat16 and out.is_contiguous()
+    check(lib().cc_layernorm_bf16(ptr(x), rows, W, row_stride, ptr(row_idx), ptr(gamma), ptr(beta), ptr(out), stream_ptr(stream)),
+          "cc_layernorm_bf16")
+    return out
+
+
+def text_embed(ids, tok, pos, x=None, eot_row=None, stream=None):
+    """ids int32 [B, L] CUDA -> (x fp32 [B*L, W] = tok[clamp(id)] + pos[t], eot_row int32 [B] = b*L + first argmax of ids)."""
+    assert ids.is_cuda and ids.dtype == torch.int32 and ids.is_contiguous()
+    _f32_cuda(tok, pos)
+    B, L = ids.shape
+    vocab, W = tok.shape
+    if x is None:
+        x = torch.empty(B * L, W, device=ids.device)
+    if eot_row is None:
+        eot_row = torch.empty(B, dtype=torch.int32, device=ids.device)
+    _f32_cuda(x)
+    check(lib().cc_text_embed(ptr(ids), ptr(tok), ptr(pos), B, L, W, vocab, ptr(x), ptr(eot_row), stream_ptr(stream)),
+          "cc_text_embed")
+    return x, eot_row
+
+
+def l2norm(x, eps, out=None, out_stride=None, stream=None):
+    """x fp32 [rows, D] -> out rows r * out_stride .. + D: x / (||x|| + eps)."""
+    _f32_cuda(x)
+    rows, D = x.shape
+    if out is None:
+        out = torch.empty(rows, D, device=x.device)
+    out_stride = out.stride(0) if out_stride is None else out_stride
+    check(lib().cc_l2norm(ptr(x), rows, D, eps, ptr(out), out_stride, stream_ptr(stream)), "cc_l2norm")
+    return out
+
+
 # ---- JPEG of frame crops (object thumbnails), byte-identical to cv2.imwrite
 JPEG_SRC_FMTS = {"rgb": 0, "bgr": 1, "i420": 2}
 

@@ -221,6 +221,30 @@ int cc_conv2d_fp32_accurate(const float* d_in, int N, int Hin, int Win, int in_c
                             const float* h_bias, int Cout, int k, int stride, int act, const float* d_res, int res_cs, int res_co,
                             float* d_out, int out_cs, int out_co, void* d_ws, size_t ws_bytes, size_t* ws_needed, void* stream);
 
+/* The CLIP encoders' row kernels as the plans run them (one warp per row, fp32 statistics).  LayerNorm uses eps 1e-5 and takes
+ * the widths W = 128 x {1, 2, 3, 4, 5, 6, 8, 10, 12}.  A bad argument fails with CC_ERR_INVALID before anything is launched.
+ * cc_patchify: d_x fp32 [B,3,S,S] -> d_out bf16 [B*(S/p)^2][Kpad] (16-byte aligned), row b*(S/p)^2 + gy*(S/p) + gx holding
+ *   x[b, c, gy*p + r, gx*p + s] in column c*p^2 + r*p + s and zeros in [3p^2, Kpad); S a multiple of p, Kpad a multiple of 8
+ *   and >= 3p^2. */
+int cc_patchify(const float* d_x, int B, int S, int p, int Kpad, void* d_out, void* stream);
+/* In place on the fp32 stream d_x [B*L][W]: token 0 of every image becomes cls, every token t gets pos[t] added, then each row
+ *   is LayerNorm'ed with d_gamma / d_beta (ln_pre).  Token 0's input rows are not read.  All pointers 16-byte aligned. */
+int cc_clip_embed_ln(float* d_x, const float* d_cls, const float* d_pos, const float* d_gamma, const float* d_beta, int B, int L, int W,
+                     void* stream);
+/* d_out bf16 [rows][W] (dense, 8-byte aligned): row r = LayerNorm(x row src) * gamma + beta, with src = d_row_idx[r] when
+ *   d_row_idx is not NULL (ln_final at the EOT rows; the indices must be rows of d_x) and r * row_stride otherwise (1: every row,
+ *   L: token 0 of each image for ln_post).  d_x, d_gamma, d_beta 16-byte aligned. */
+int cc_layernorm_bf16(const float* d_x, int rows, int W, long long row_stride, const int32_t* d_row_idx, const float* d_gamma,
+                      const float* d_beta, void* d_out, void* stream);
+/* d_x fp32 [B*L][W] = tok[id][:] + pos[t][:] for id = d_ids[b*L + t] clamped to [0, vocab) (an id below 0 reads row 0, one at or
+ *   above vocab reads row vocab - 1); d_eot_row[b] = b*L + the first position of the largest raw id of row b (the EOT token).
+ *   W a multiple of 4; d_tok, d_pos, d_x 16-byte aligned. */
+int cc_text_embed(const int32_t* d_ids, const float* d_tok, const float* d_pos, int B, int L, int W, int vocab, float* d_x,
+                  int32_t* d_eot_row, void* stream);
+/* d_out[r*out_stride + c] = d_in[r*D + c] / (||d_in row r|| + eps), out_stride >= D, eps >= 0 (the image tower uses 1e-8, the
+ *   text tower 0, which gives NaN for a zero row as the reference does). */
+int cc_l2norm(const float* d_in, int rows, int D, float eps, float* d_out, long long out_stride, void* stream);
+
 /* ---- CLIP image/text encoder (replaces class OpenCLIP, models/objects.py:21-186) ---- */
 typedef struct cc_clip cc_clip;
 typedef struct cc_clip_config {
