@@ -47,6 +47,8 @@ _SIGS = {
     "cc_last_error": (ctypes.c_char_p, []),
     "cc_device_check": (_i, []),
     "cc_conv2d": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp]),
+    "cc_conv2d_chain": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _i, _i, _i,
+                             _vp, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "cc_yolo_create": (_i, [ctypes.c_char_p, _i, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_vp),
                             ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(_vp)]),
     "cc_yolo_create_ex": (_i, [ctypes.c_char_p, _i, _i, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_vp),

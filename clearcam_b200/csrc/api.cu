@@ -47,6 +47,31 @@ int cc_conv2d(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, i
   return conv_direct_launch(p, static_cast<cudaStream_t>(stream));
 }
 
+int cc_conv2d_chain(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const void* d_w, const float* d_bias,
+                    int Cout, int k, int stride, void* d_out, int out_cs, int out_co, int store1, const void* d_res, int res_cs,
+                    int res_co, const void* d_w2, const float* d_bias2, int Cout2, int act2, int k0, const void* d_part, int part_cs,
+                    int part_co, int part_C, void* d_out2, int out2_cs, int out2_co, int out2_f32, void* stream) {
+  const int sms = device_sm_count();
+  CC_REQUIRE(sms > 0, "cc_conv2d_chain: no sm_90 (H100) device");
+  CC_REQUIRE(d_in && (d_out || !store1) && d_w2 && d_out2 && (!d_part || part_C > 0), "cc_conv2d_chain: NULL argument");
+  CC_REQUIRE(!d_part || (part_co >= 0 && part_co + part_C <= part_cs), "cc_conv2d_chain: partner slice outside its row");
+  ConvDesc d{};
+  d.in = d_in; d.in_cs = in_cs; d.in_co = in_co; d.Cin = Cin;
+  d.N = N; d.Hin = Hin; d.Win = Win; d.k = k; d.stride = stride;
+  d.w = d_w; d.bias = d_bias;
+  d.out = d_out; d.out_cs = out_cs; d.out_co = out_co; d.Cout = Cout; d.out_f32 = 0;
+  d.act = CC_ACT_SILU; d.res = d_res; d.res_cs = res_cs; d.res_co = res_co;
+  ChainDesc c{};
+  c.w = d_w2; c.bias = d_bias2; c.Cout = Cout2; c.act = act2; c.k0 = k0;
+  c.part = d_part; c.part_cs = part_cs; c.part_co = part_co; c.part_C = d_part ? part_C : 0;
+  c.out = d_out2; c.out_cs = out2_cs; c.out_co = out2_co; c.out_f32 = out2_f32;
+  c.store1 = store1 != 0;
+  CC_REQUIRE(out2_co >= 0 && out2_co + Cout2 <= out2_cs, "cc_conv2d_chain: second output slice outside its row");
+  GemmLaunch L;
+  if (int rc = conv_gemm_chain_build(d, c, sms, &L)) return rc;
+  return conv_gemm_launch(L, static_cast<cudaStream_t>(stream));
+}
+
 int cc_attention(const void* d_qkv, int B, int L, int H, int causal, int impl, void* d_ws, size_t ws_bytes, void* d_ctx,
                  size_t* ws_needed, void* stream) {
   CC_REQUIRE(impl == 1 || impl == 2, "cc_attention: unknown impl %d (1 = mma.sync, 2 = wgmma)", impl);

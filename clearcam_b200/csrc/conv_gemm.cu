@@ -108,7 +108,10 @@ __device__ __forceinline__ void mma_kblock(float (&acc0)[BN / 2], float (&acc1)[
   }
 }
 
-template <int ACT, bool F32, int BN>
+// N2 > 0: the chained mode (conv_gemm_chain_build).  After a tile of n block p.ch_nb is in the staging (and stored, if
+// p.ch_store1), its consumer runs the N2 x N2 1x1 conv over [staging run | partner box] with wgmma A read straight from the
+// staging, then a second bias -> ACT2 -> bf16 / fp32 (F2) epilogue into the same region and a TMA store to tmO2.
+template <int ACT, bool F32, int BN, int N2 = 0, int ACT2 = ACT_NONE, bool F2 = false>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   // 1024-B alignment for the 128B-swizzled tiles
@@ -123,6 +126,12 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
   constexpr int kPassBoxes = kPassCols / kBoxCols;
   constexpr int kStageBytes = epi_stage_bytes(BN, es);
   constexpr uint32_t kSwz = kBoxBytes == 128 ? 0x70 : (kBoxBytes == 64 ? 0x30 : 0x10);   // 16-B chunk bits XORed by row
+  constexpr bool CHAIN = N2 > 0;
+  static_assert(!CHAIN || !F32, "a chained 1x1 reads a bf16 staging tile");
+  constexpr int kW2Bytes = (N2 * N2 * 2 + 1023) & ~1023;     // the 1x1's weights, resident for the whole kernel
+  // a chained launch takes no pre-activation addend, and one with a 128-channel tile no residual: next to 128 accumulator
+  // registers their epilogue code would spill (conv_gemm_chain_build refuses them)
+  constexpr bool kPre = !CHAIN, kRes = !(CHAIN && BN == 128);
 
   const int wg = threadIdx.x >> 7;
   const uint32_t row_bytes = p.BK * 2;
@@ -131,17 +140,21 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
   const int S = p.stages;
   const int num_kb = p.num_taps * p.chunks_per_tap;
 
-  uint8_t* sStage = smem;                                     // kConsumers x kStageBytes, 1024-B aligned
-  uint8_t* sA = sStage + kConsumers * kStageBytes;
+  const int region = CHAIN ? p.ch_stage : kStageBytes;      // one consumer's staging region
+  uint8_t* sStage = smem;                                     // kConsumers x region, 1024-B aligned
+  uint8_t* sW2 = sStage + kConsumers * region;
+  uint8_t* sA = sW2 + kW2Bytes;
   uint8_t* sB = sA + S * a_bytes;
   // resident-B mode: sB holds ALL k-blocks of the weights (loaded once); the ring then carries A only
   float* sBias = reinterpret_cast<float*>(sB + (p.b_res ? num_kb : S) * b_bytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + p.cout);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + p.cout + N2);   // chained: the 1x1's bias follows
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + S;
   uint64_t* bres_bar = bars + 2 * S;
   uint64_t* turn_bar = bars + 2 * S + 1;    // [c]: consumer c may start its next mainloop
   uint64_t* res_bar = bars + 2 * S + 3;     // [c]: residual tile of consumer c landed in its staging
+  uint64_t* w2_bar = bars + 2 * S + 5;      // chained: the 1x1's weights landed
+  uint64_t* par_bar = bars + 2 * S + 6;     // chained, [c]: partner box of consumer c landed
 
   if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[0] = globaltimer_ns();
   if (threadIdx.x == 0) {
@@ -157,10 +170,16 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       mbar_init(&turn_bar[c], 1);
       mbar_init(&res_bar[c], 1);
     }
+    if constexpr (CHAIN) {
+      mbar_init(w2_bar, 1);
+      for (int c = 0; c < kConsumers; ++c) mbar_init(&par_bar[c], 1);
+    }
     fence_mbar_init();
   }
   if (wg > 0) {  // bias -> smem once per CTA
     for (int i = threadIdx.x - 128; i < p.cout; i += kEpiThreads) sBias[i] = p.bias ? __ldg(p.bias + i) : 0.f;
+    if constexpr (CHAIN)
+      for (int i = threadIdx.x - 128; i < N2; i += kEpiThreads) sBias[p.cout + i] = p.bias2 ? __ldg(p.bias2 + i) : 0.f;
   }
   __syncthreads();
   // PDL: let the next kernel start its prologue as our CTAs retire; everything that only touches WEIGHTS (bias above,
@@ -177,6 +196,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       if (p.b_res) {   // weights are not produced by the previous kernel: issued BEFORE the grid dependency wait
         mbar_arrive_expect_tx(bres_bar, num_kb * b_bytes);
         for (int kb = 0; kb < num_kb; ++kb) tma_load_2d(sB + kb * b_bytes, &p.tmB, bres_bar, kb * p.BK, 0);
+      }
+      if constexpr (CHAIN) {   // the 1x1's weights: K blocks of ch_bk2 channels x N2 rows, as the standalone launch loads them
+        mbar_arrive_expect_tx(w2_bar, N2 * N2 * 2);
+        for (int kb = 0; kb < N2 / p.ch_bk2; ++kb) tma_load_2d(sW2 + kb * N2 * p.ch_bk2 * 2, &p.tmW2, w2_bar, kb * p.ch_bk2, 0);
       }
       pdl_wait();
       if (p.trace && blockIdx.x == 0) p.trace[1] = globaltimer_ns();
@@ -208,7 +231,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     const uint64_t dconst = gmma_desc_const(row_bytes, 8u * row_bytes);
     const uint32_t sA16 = (smem_u32(sA) & 0x3FFFF) >> 4, sB16 = (smem_u32(sB) & 0x3FFFF) >> 4;
     const uint32_t a16 = a_bytes >> 4, b16 = b_bytes >> 4, ahalf = (64 * row_bytes) >> 4;
-    const uint32_t stg = smem_u32(sStage + c * kStageBytes), sbias32 = smem_u32(sBias);
+    const uint32_t stg = smem_u32(sStage + c * region), sbias32 = smem_u32(sBias);
     const int TWm = (1 << p.lTW) - 1, THm = (1 << p.lTH) - 1;
     // the residual of column pass `pass` of the tile at (nb, w0, h0, n0) -> this warpgroup's staging, on res_bar[c]
     auto load_res = [&](const TileXY& tx, int pass) {
@@ -218,15 +241,21 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         tma_load_4d(stg + b * kBoxTile, &p.tmR, &res_bar[c], tx.nb * BN + pass * kPassCols + b * kBoxCols, tx.w0, tx.h0, tx.n0);
     };
     if (p.b_res) mbar_wait(bres_bar, 0);
+    if constexpr (CHAIN) mbar_wait(w2_bar, 0);
     pdl_wait();   // residual / pre reads depend on the previous kernel's output
     // barrier phases follow from the local tile index j: this consumer's (j / 2)-th tile; consumer 0 runs the CTA's first
     // mainloop (j = 0) without waiting
     for (int j = c; blockIdx.x + j * gridDim.x < p.num_tiles; j += kConsumers) {
       const TileXY tx = tile_origin(p, blockIdx.x + j * gridDim.x);
       // prefetch the residual while the mainloop runs, once the previous tile's stores have read the staging
-      if (p.res != nullptr && lead) {
+      if (kRes && p.res != nullptr && lead) {
         tma_store_wait_read<0>();
         load_res(tx, 0);
+      }
+      if (CHAIN && p.ch_part && lead) {   // (one n block) the partner box goes right after the staging tile
+        tma_store_wait_read<0>();
+        mbar_arrive_expect_tx(&par_bar[c], kBoxTile);
+        tma_load_4d(stg + kStageBytes, &p.tmP, &par_bar[c], 0, tx.w0, tx.h0, tx.n0);
       }
       if (j > 0) mbar_wait(&turn_bar[c], ((j >> 1) + (c == 0)) & 1);
 
@@ -273,7 +302,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       // one column pass (a compile-time constant, so every accumulator index below is static and stays in registers)
       auto epilogue_pass = [&](auto pass_c) {
         constexpr int pass = decltype(pass_c)::value;
-        if (p.res != nullptr) {  // the residual landed in the staging (loaded after the previous stores had read it)
+        if (kRes && p.res != nullptr) {  // the residual landed in the staging (loaded after the previous stores had read it)
           mbar_wait(&res_bar[c], ((j >> 1) * kPasses + pass) & 1);
         } else {
           if (lead) tma_store_wait_read<0>();   // the previous tile's stores have read the staging
@@ -284,7 +313,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
           const int row = 64 * (q >> 1) + 16 * wq + (lane >> 2) + 8 * (q & 1);
           // pre-activation addend from a half-resolution fp32 map (nearest x2 upsample by addressing): this row's source
           const float* pre_row = nullptr;
-          if (p.pre != nullptr) {
+          if (kPre && p.pre != nullptr) {
             const int pw = tx.w0 + (row & TWm), ph = tx.h0 + ((row >> p.lTW) & THm), pn = tx.n0 + (row >> (p.lTW + p.lTH));
             if ((pw < p.W) && (ph < p.H) && (pn < p.N))
               pre_row = p.pre + ((static_cast<long long>(pn) * p.pre_h + (ph >> 1)) * p.pre_w + (pw >> 1)) * p.cout + nb * BN;
@@ -307,13 +336,13 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             float f1 = act_apply<ACT>(((q >> 1) ? acc1[k + 1] : acc0[k + 1]) + b1);
             const uint32_t addr = rbase + (pc / kBoxCols) * kBoxTile + (((pc % kBoxCols) * es) ^ rxor);
             if (F32) {
-              if (p.res != nullptr) {
+              if (kRes && p.res != nullptr) {
                 const float2 r = lds_f2(addr);
                 f0 += r.x; f1 += r.y;
               }
               sts_f2(addr, f0, f1);
             } else {
-              if (p.res != nullptr) {
+              if (kRes && p.res != nullptr) {
                 const uint32_t r = lds_u32(addr);   // bf16 -> fp32 is a 16-bit shift
                 f0 += __uint_as_float(r << 16);
                 f1 += __uint_as_float(r & 0xFFFF0000u);
@@ -324,13 +353,15 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         }
         fence_proxy_async_smem();      // generic-proxy writes -> visible to the TMA store
         named_bar_sync(1 + c, 128);
-        if (lead) {
+        if (lead && (!CHAIN || p.ch_store1)) {
           // the box is clipped at the edges of the output slice [out_co, out_co + Cout) x W x H x N
 #pragma unroll
           for (int b = 0; b < kPassBoxes; ++b)
             tma_store_4d(&p.tmO, stg + b * kBoxTile, nb * BN + pass * kPassCols + b * kBoxCols, tx.w0, tx.h0, tx.n0);
           tma_store_commit();
-          if (p.res != nullptr && pass + 1 < kPasses) {
+        }
+        if (lead) {
+          if (kRes && p.res != nullptr && pass + 1 < kPasses) {
             tma_store_wait_read<0>();
             load_res(tx, pass + 1);
           }
@@ -338,6 +369,92 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       };
       epilogue_pass(std::integral_constant<int, 0>{});
       if constexpr (kPasses > 1) epilogue_pass(std::integral_constant<int, 1>{});
+      if constexpr (CHAIN) {
+        if (tx.nb == p.ch_nb) {
+          // ---- the chained 1x1.  A operand: the staging boxes (K-major, swizzled as a ring stage of BK = kBoxCols), then the
+          // partner box; k16 step k reads input channel 16 k of the 1x1 as the standalone launch does, with its instruction
+          // N (= N2) and its weight blocks, so each accumulator sees the same sequence of MMAs
+          constexpr int es2 = F2 ? 4 : 2;
+          constexpr int kBox2 = epi_box_bytes(N2, es2), kBoxCols2 = kBox2 / es2, kBoxTile2 = kTileM * kBox2;
+          constexpr uint32_t kSwz2 = kBox2 == 128 ? 0x70 : (kBox2 == 64 ? 0x30 : 0x10);
+          if (p.ch_part) mbar_wait(&par_bar[c], (j >> 1) & 1);
+          // every value below is pinned after the mainloop (the empty asm), so that none is hoisted out of the tile loop and
+          // kept live next to the mainloop's accumulators
+          uint32_t stg_c = stg, bk2 = p.ch_bk2, k0 = p.ch_k0, part = p.ch_part;
+          asm volatile("" : "+r"(stg_c), "+r"(bk2), "+r"(k0), "+r"(part));
+          const uint64_t adc = gmma_desc_const(kBoxBytes, 8u * kBoxBytes);
+          const uint64_t bdc = gmma_desc_const(bk2 * 2, 16u * bk2);
+          const uint32_t stg16 = (stg_c & 0x3FFFF) >> 4, w16 = ((stg_c + (kConsumers - c) * region) & 0x3FFFF) >> 4;
+          const uint32_t ahalf2 = (64 * kBoxBytes) >> 4, wblk16 = (N2 * bk2 * 2) >> 4;
+          const int run16 = N2 / 16 - (part ? kBoxCols / 16 : 0);
+          // rows [0, 64) and then [64, 128), one m64 accumulator at a time (each sees the same MMAs as in the standalone
+          // launch).  When the 1x1's output boxes have the staging boxes' 128-B span, output rows [0, 64) overwrite only A rows
+          // [0, 64) of every box, so each half is written as soon as its MMAs are done (kDirect); otherwise the first half's
+          // outputs wait in registers, packed, until the second half's MMAs have read the whole staging.
+          constexpr bool kDirect = kBox2 == kBoxBytes;
+          constexpr int kHeld = kDirect ? 1 : (F2 ? N2 / 2 : N2 / 4);
+          uint32_t held[kHeld];
+          float d[N2 / 2];
+          const uint32_t bias2_t = sbias32 + (p.cout + 2 * (lane & 3)) * 4;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int i = 0; i < N2 / 2; ++i) d[i] = 0.f;
+            wgmma_fence_acc(d);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < N2 / 16; ++k) {
+              const int ach = k < run16 ? k0 + 16 * k : BN + 16 * (k - run16);   // staging channel (the partner box follows)
+              const uint64_t ad = adc | (stg16 + (ach / kBoxCols) * (kBoxTile >> 4) + 2 * ((ach % kBoxCols) / 16) + h * ahalf2);
+              const uint64_t bd = bdc | (w16 + (16 * k / bk2) * wblk16 + 2 * ((16 * k % bk2) / 16));
+              Wgmma<N2>::mma(d, ad, bd, k == 0 ? 0u : 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_acc(d);
+            if (kDirect || h == 1) {
+              if (lead && p.ch_store1 && h == (kDirect ? 0 : 1)) tma_store_wait_read<0>();   // the first output's store has read it
+              named_bar_sync(1 + c, 128);                  // every warp's MMAs of this half have read the staging
+            }
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+              const int row = 64 * h + 16 * wq + (lane >> 2) + 8 * r;
+              const uint32_t roff = static_cast<uint32_t>(row * kBox2), rxor = (roff >> 3) & kSwz2;
+              const uint32_t rbase = stg_c + roff;
+              const uint32_t row0 = static_cast<uint32_t>((row - 64) * kBox2), rxor0 = (row0 >> 3) & kSwz2;   // its first-half row
+#pragma unroll
+              for (int i = 0; i < N2 / 8; ++i) {
+                const int col = 8 * i + 2 * (lane & 3);
+                const float2 bb = lds_f2(bias2_t + 32 * i);
+                const int k = 4 * i + 2 * r;
+                const float f0 = act_apply<ACT2>(d[k] + bb.x);
+                const float f1 = act_apply<ACT2>(d[k + 1] + bb.y);
+                const int hi = kDirect ? 0 : r * (N2 / 8) + i;
+                const uint32_t cb = (col / kBoxCols2) * kBoxTile2, cc = (col % kBoxCols2) * es2;
+                if (kDirect || h == 1) {
+                  if (F2) sts_f2(rbase + cb + (cc ^ rxor), f0, f1);
+                  else sts_u32(rbase + cb + (cc ^ rxor), pack_bf16x2(f0, f1));
+                }
+                if (!kDirect && h == 0) {
+                  if (F2) { held[2 * hi] = __float_as_uint(f0); held[2 * hi + 1] = __float_as_uint(f1); }
+                  else held[hi] = pack_bf16x2(f0, f1);
+                }
+                if (!kDirect && h == 1) {
+                  if (F2) sts_f2(stg_c + row0 + cb + (cc ^ rxor0), __uint_as_float(held[2 * hi]), __uint_as_float(held[2 * hi + 1]));
+                  else sts_u32(stg_c + row0 + cb + (cc ^ rxor0), held[hi]);
+                }
+              }
+            }
+          }
+          fence_proxy_async_smem();
+          named_bar_sync(1 + c, 128);
+          if (lead) {
+#pragma unroll
+            for (int b = 0; b < N2 / kBoxCols2; ++b) tma_store_4d(&p.tmO2, stg + b * kBoxTile2, b * kBoxCols2, tx.w0, tx.h0, tx.n0);
+            tma_store_commit();
+          }
+        }
+      }
     }
     if (lead) {
       tma_store_wait_all();    // the output is complete in global memory before the CTA retires (PDL successors read it)
@@ -361,7 +478,20 @@ bool conv_gemm_supported(const ConvDesc& d) {
   return true;
 }
 
-int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
+// N tile: a power of two in [16, 128] that divides Cout (the kernel is compiled for those four widths); an override is taken
+// as an upper bound.  If the machine would be under-filled, the tile is halved (more, smaller tiles).
+static int pick_bn(int cout, long long m_tiles, int bn_override, int num_sms) {
+  const int maxbn = bn_override > 0 && bn_override < kMaxBN ? bn_override : kMaxBN;
+  int BN = 16;
+  while (BN * 2 <= maxbn && cout % (BN * 2) == 0) BN *= 2;
+  if (bn_override == 0)
+    while (BN > 64 && m_tiles * (cout / BN) < num_sms) BN /= 2;
+  return BN;
+}
+static int pick_bk(int cin) { return (cin % 64 == 0) ? 64 : (cin % 32 == 0 ? 32 : 16); }
+
+// with_out = false: no first output (a chained launch that drops it; tmO stays unset)
+static int gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L, bool with_out) {
   CC_REQUIRE(conv_gemm_supported(d), "conv_gemm: unsupported shape Cin=%d Cout=%d k=%d s=%d Hin=%d Win=%d", d.Cin, d.Cout,
              d.k, d.stride, d.Hin, d.Win);
   PFN_encodeTiled enc = get_encode_tiled();
@@ -377,18 +507,12 @@ int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
   p.W = Wout; p.H = Hout; p.N = d.N;
 
   // ---- K blocking
-  p.BK = (d.Cin % 64 == 0) ? 64 : (d.Cin % 32 == 0 ? 32 : 16);
+  p.BK = pick_bk(d.Cin);
   p.num_taps = d.k * d.k;
   p.chunks_per_tap = d.Cin / p.BK;
-  // ---- N blocking: a power of two in [16, 128] that divides Cout (the kernel is compiled for those four widths); an
-  // override is taken as an upper bound
+  // ---- N blocking
   const long long mt = (static_cast<long long>(d.N) * Hout * Wout + 127) / 128;
-  const int maxbn = d.bn_override > 0 && d.bn_override < kMaxBN ? d.bn_override : kMaxBN;
-  int BN = 16;
-  while (BN * 2 <= maxbn && d.Cout % (BN * 2) == 0) BN *= 2;
-  // if the machine would be under-filled, halve the N tile (more, smaller tiles)
-  if (d.bn_override == 0)
-    while (BN > 64 && mt * (d.Cout / BN) < num_sms) BN /= 2;
+  const int BN = pick_bn(d.Cout, mt, d.bn_override, num_sms);
   CC_REQUIRE(BN >= 16 && BN <= kMaxBN && d.Cout % BN == 0, "conv_gemm: bad BN=%d for Cout=%d", BN, d.Cout);
   p.BN = BN;
   p.n_blocks = d.Cout / BN;
@@ -487,7 +611,8 @@ int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
       CC_REQUIRE(r == CUDA_SUCCESS, "conv_gemm: cuTensorMapEncodeTiled(%s) failed: %d", what, int(r));
       return CC_OK;
     };
-    if (int rc = encode(&p.tmO, d.out, d.out_cs, d.out_co, "out")) return rc;
+    if (with_out)
+      if (int rc = encode(&p.tmO, d.out, d.out_cs, d.out_co, "out")) return rc;
     if (d.res) if (int rc = encode(&p.tmR, d.res, d.res_cs, d.res_co, "residual")) return rc;
   }
   {
@@ -518,16 +643,119 @@ int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
   L->smem_bytes = fixed + (p.b_res ? bres_bytes + S * a_bytes : S * (a_bytes + b_bytes));
   L->grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
   L->flops = 2.0 * double(d.N) * Hout * Wout * d.Cout * d.k * d.k * d.Cin;
-  L->bytes = double(d.N) * d.Hin * d.Win * d.Cin * 2 + double(d.N) * Hout * Wout * d.Cout * es * (d.res ? 2 : 1) +
+  L->bytes = double(d.N) * d.Hin * d.Win * d.Cin * 2 + double(d.N) * Hout * Wout * d.Cout * es * ((with_out ? 1 : 0) + (d.res ? 1 : 0)) +
              double(d.Cout) * d.k * d.k * d.Cin * 2;
   return CC_OK;
 }
 
-template <int ACT, bool F32, int BN>
+int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
+  CC_REQUIRE(d.out != nullptr, "conv_gemm: no output");
+  return gemm_build(d, num_sms, L, true);
+}
+
+static bool silu_exact_env() {
+  static const int v = getenv("CC_SILU_EXACT") ? atoi(getenv("CC_SILU_EXACT")) : 0;
+  return v != 0;
+}
+static int chain_launch(const GemmLaunch& L, cudaStream_t stream, bool dry);
+
+// The 1x1 c chains onto the conv d when
+//   * d is a SiLU conv with a bf16 output and c is square, Cout2 <= 128 channels (so <= 32 KB of weights), SiLU into bf16 or
+//     no activation into fp32 (at most 64 channels: one 128 x 256-B tile), and the standalone launch of c would tile it as
+//     one n block (its instruction N is then Cout2);
+//   * c's input is a run of d's output channels [k0, k0 + run) inside one n block, starting on a k16 step, optionally
+//     followed by a partner slice exactly one staging box wide;
+//   * d's first output may be dropped only when d has one n block, and the operand ring keeps at least 4 stages.
+int conv_gemm_chain_build(const ConvDesc& d, const ChainDesc& c, int num_sms, GemmLaunch* L) {
+  CC_REQUIRE(c.w && c.out && (d.out || !c.store1), "conv_gemm chain: NULL weights or output");
+  CC_REQUIRE(d.act == ACT_SILU && !d.out_f32 && !silu_exact_env(), "conv_gemm chain: the first conv must be SiLU into bf16");
+  CC_REQUIRE(!d.pre, "conv_gemm chain: the first conv takes no pre-activation addend");
+  CC_REQUIRE(c.Cout >= 16 && c.Cout <= kMaxBN && c.Cout % 16 == 0, "conv_gemm chain: the 1x1 has %d channels (16..128)", c.Cout);
+  CC_REQUIRE((c.act == ACT_SILU && !c.out_f32) || (c.act == ACT_NONE && c.out_f32 && c.Cout <= 64),
+             "conv_gemm chain: the 1x1 is SiLU into bf16 or no activation into fp32 (<= 64 channels)");
+  const int Hout = d.stride == 2 ? d.Hin / 2 : d.Hin, Wout = d.stride == 2 ? d.Win / 2 : d.Win;
+  const long long mt = (static_cast<long long>(d.N) * Hout * Wout + 127) / 128;
+  CC_REQUIRE(pick_bn(c.Cout, mt, 0, num_sms) == c.Cout, "conv_gemm chain: the standalone 1x1 would tile its %d channels in blocks", c.Cout);
+  if (int rc = gemm_build(d, num_sms, L, c.store1)) return rc;
+  GemmParams& p = L->p;
+  const int BN = p.BN;
+  const int box_bytes = epi_box_bytes(BN, 2), box_cols = box_bytes / 2, box_tile = kTileM * box_bytes;
+  const int run = c.Cout - (c.part ? c.part_C : 0);
+  CC_REQUIRE(!c.part || c.part_C == box_cols, "conv_gemm chain: the partner slice must be one staging box (%d channels)", box_cols);
+  CC_REQUIRE(run > 0 && c.k0 >= 0 && c.k0 % 16 == 0 && c.k0 / BN == (c.k0 + run - 1) / BN && c.k0 + run <= d.Cout,
+             "conv_gemm chain: input run [%d, %d) is not inside one %d-channel n block", c.k0, c.k0 + run, BN);
+  CC_REQUIRE(!(d.res && BN == 128), "conv_gemm chain: a 128-channel tile takes no residual");
+  CC_REQUIRE((c.store1 && !c.part) || p.n_blocks == 1, "conv_gemm chain: a dropped first output or a partner needs one n block");
+  p.ch_n2 = c.Cout;
+  p.ch_nb = c.k0 / BN;
+  p.ch_k0 = c.k0 - p.ch_nb * BN;
+  p.ch_part = c.part ? 1 : 0;
+  p.ch_store1 = c.store1 ? 1 : 0;
+  p.ch_bk2 = pick_bk(c.Cout);
+  p.act2 = c.act;
+  p.out2_f32 = c.out_f32;
+  p.bias2 = c.bias;
+  const int es2 = c.out_f32 ? 4 : 2;
+  PFN_encodeTiled enc = get_encode_tiled();
+  CC_REQUIRE(enc != nullptr, "conv_gemm: cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
+  auto swz_of = [](int span) {
+    return span == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : span == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
+  };
+  {     // 1x1 weights [Cout2][Cin2 = Cout2], box = BK2 x Cout2
+    cuuint64_t dims[2] = {cuuint64_t(c.Cout), cuuint64_t(c.Cout)};
+    cuuint64_t strides[1] = {cuuint64_t(c.Cout) * 2};
+    cuuint32_t box[2] = {cuuint32_t(p.ch_bk2), cuuint32_t(c.Cout)};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = enc(&p.tmW2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(c.w), dims, strides, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz_of(p.ch_bk2 * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    CC_REQUIRE(r == CUDA_SUCCESS, "conv_gemm chain: cuTensorMapEncodeTiled(W2) failed: %d", int(r));
+  }
+  const int TW = 1 << p.lTW, TH = 1 << p.lTH, TN = 1 << p.lTN;
+  // an NHWC slice [co, co + C) of a buffer of cs channels at the output's pixels, box = `cols` channels x the pixel box
+  auto encode = [&](CUtensorMap* tm, const void* buf, int cs, int co, int C, int es, int cols, const char* what) -> int {
+    CC_REQUIRE((size_t(cs) * es) % 16 == 0 && (size_t(co) * es) % 16 == 0, "conv_gemm chain: %s slice not 16-B aligned", what);
+    void* base = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(buf)) + size_t(co) * es;
+    cuuint64_t dims[4] = {cuuint64_t(C), cuuint64_t(Wout), cuuint64_t(Hout), cuuint64_t(d.N)};
+    const cuuint64_t px = cuuint64_t(cs) * es;
+    cuuint64_t strides[3] = {px, px * Wout, px * Wout * Hout};
+    cuuint32_t box[4] = {cuuint32_t(cols), cuuint32_t(TW), cuuint32_t(TH), cuuint32_t(TN)};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = enc(tm, es == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, dims, strides, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz_of(cols * es), CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    CC_REQUIRE(r == CUDA_SUCCESS, "conv_gemm chain: cuTensorMapEncodeTiled(%s) failed: %d", what, int(r));
+    return CC_OK;
+  };
+  if (c.part)
+    if (int rc = encode(&p.tmP, c.part, c.part_cs, c.part_co, c.part_C, 2, box_cols, "partner")) return rc;
+  if (int rc = encode(&p.tmO2, c.out, c.out_cs, c.out_co, c.Cout, es2, epi_box_bytes(c.Cout, es2) / es2, "out2")) return rc;
+
+  // ---- smem: each consumer's region holds its staging tile and the partner box, then the 1x1's output tile
+  const int stage1 = epi_stage_bytes(BN, 2) + (c.part ? box_tile : 0), stage2 = kTileM * c.Cout * es2;
+  p.ch_stage = ((stage1 > stage2 ? stage1 : stage2) + 1023) & ~1023;
+  const int w2_bytes = (c.Cout * c.Cout * 2 + 1023) & ~1023;
+  const int a_bytes = kTileM * p.BK * 2, b_bytes = BN * p.BK * 2;
+  const int fixed = 1024 + kConsumers * p.ch_stage + w2_bytes + (d.Cout + c.Cout) * 4 + 8 * kBarriers;
+  const int num_kb = p.num_taps * p.chunks_per_tap;
+  const int bres_bytes = b_bytes * num_kb;
+  p.b_res = (p.n_blocks == 1 && (kMaxSmem - fixed - bres_bytes) / a_bytes >= 4) ? 1 : 0;
+  int S = p.b_res ? (kMaxSmem - fixed - bres_bytes) / a_bytes : (kMaxSmem - fixed) / (a_bytes + b_bytes);
+  if (S > 8) S = 8;
+  CC_REQUIRE(S >= 4, "conv_gemm chain: the operand ring would keep %d stages (at least 4)", S);
+  p.stages = S;
+  L->smem_bytes = fixed + (p.b_res ? bres_bytes + S * a_bytes : S * (a_bytes + b_bytes));
+  const double px = double(d.N) * Hout * Wout;
+  L->flops += 2.0 * px * c.Cout * c.Cout;
+  L->bytes += px * ((c.part ? c.part_C * 2 : 0) + c.Cout * es2) + double(c.Cout) * c.Cout * 2;
+  CC_REQUIRE(chain_launch(*L, nullptr, true) == CC_OK, "conv_gemm chain: no chained kernel for BN=%d and a %d-channel 1x1 (act %d, fp32 %d)",
+             BN, c.Cout, c.act, c.out_f32);
+  return CC_OK;
+}
+
+template <int ACT, bool F32, int BN, int N2 = 0, int ACT2 = ACT_NONE, bool F2 = false>
 static int launch_bn(const GemmLaunch& L, cudaStream_t stream) {
   static bool attr_set = false;
   if (!attr_set) {
-    CC_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<ACT, F32, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+    CC_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<ACT, F32, BN, N2, ACT2, F2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
     attr_set = true;
   }
   cudaLaunchConfig_t cfg{};
@@ -540,7 +768,7 @@ static int launch_bn(const GemmLaunch& L, cudaStream_t stream) {
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  CC_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<ACT, F32, BN>, L.p));
+  CC_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<ACT, F32, BN, N2, ACT2, F2>, L.p));
   return CC_OK;
 }
 
@@ -556,7 +784,31 @@ static int launch_variant(const GemmLaunch& L, cudaStream_t stream) {
   return CC_ERR_INVALID;
 }
 
+// The chained instances: (producer BN, 1x1 channels) of the detector's chains (yolo.cu), SiLU into bf16, and the head's
+// 64 -> 64 logits (no activation, fp32).  dry: only report whether the instance exists.
+static int chain_launch(const GemmLaunch& L, cudaStream_t stream, bool dry) {
+  const GemmParams& p = L.p;
+  const int key = p.BN * 1000 + p.ch_n2;
+  if (p.act2 == ACT_NONE && p.out2_f32) {
+    if (key == 64064) return dry ? CC_OK : launch_bn<ACT_SILU, false, 64, 64, ACT_NONE, true>(L, stream);
+  } else if (p.act2 == ACT_SILU && !p.out2_f32) {
+    switch (key) {
+      case 16032: return dry ? CC_OK : launch_bn<ACT_SILU, false, 16, 32, ACT_SILU, false>(L, stream);
+      case 32032: return dry ? CC_OK : launch_bn<ACT_SILU, false, 32, 32, ACT_SILU, false>(L, stream);
+      case 32064: return dry ? CC_OK : launch_bn<ACT_SILU, false, 32, 64, ACT_SILU, false>(L, stream);
+      case 64032: return dry ? CC_OK : launch_bn<ACT_SILU, false, 64, 32, ACT_SILU, false>(L, stream);
+      case 64064: return dry ? CC_OK : launch_bn<ACT_SILU, false, 64, 64, ACT_SILU, false>(L, stream);
+      case 64128: return dry ? CC_OK : launch_bn<ACT_SILU, false, 64, 128, ACT_SILU, false>(L, stream);
+      case 128064: return dry ? CC_OK : launch_bn<ACT_SILU, false, 128, 64, ACT_SILU, false>(L, stream);
+      case 128128: return dry ? CC_OK : launch_bn<ACT_SILU, false, 128, 128, ACT_SILU, false>(L, stream);
+    }
+  }
+  set_error("conv_gemm: no chained kernel for BN=%d, 1x1 of %d channels, act %d, fp32 %d", p.BN, p.ch_n2, p.act2, p.out2_f32);
+  return CC_ERR_INVALID;
+}
+
 int conv_gemm_launch(const GemmLaunch& L, cudaStream_t stream) {
+  if (L.p.ch_n2 > 0) return chain_launch(L, stream, false);
   const bool f32 = L.p.out_f32 != 0;
   static const int exact_env = getenv("CC_SILU_EXACT") ? atoi(getenv("CC_SILU_EXACT")) : 0;
   int act = L.p.act;

@@ -47,6 +47,17 @@ struct GemmParams {
   int32_t pre_h, pre_w;               //   concat(upsample(a), b) is computed as conv_b(b) + upsample(conv_a(a)) (see yolo.cu)
   unsigned long long* trace;          // optional device timeline slots [8] (globaltimer ns): first CTA entry, dependency released, last CTA exit,
                                       // and of CTA 0: first operands landed, -, first accumulator complete, last epilogue done, exit
+  // chained 1x1 conv (conv_gemm_chain_build; ch_n2 == 0: none): the bf16 tiles of n block ch_nb, once in the consumer's
+  // staging, are the A operand of a square 1x1 conv of ch_n2 channels whose output goes to tmO2
+  CUtensorMap tmW2;                   // 2-D [Cout2][Cin2] weights of the 1x1, box = its standalone BK x Cout2
+  CUtensorMap tmP;                    // 4-D partner slice appended to the 1x1's input (one staging box wide; ch_part)
+  CUtensorMap tmO2;                   // 4-D output slice of the 1x1
+  int32_t ch_n2, ch_nb, ch_k0;        // 1x1 channels, chaining n block, first staging channel of the 1x1's input run
+  int32_t ch_part, ch_store1;         // partner box present; the first output is still stored
+  int32_t ch_bk2;                     // K block of the 1x1's weights in smem (the standalone launch's BK)
+  int32_t ch_stage;                   // bytes of one consumer's staging region (staging + partner box, or the 1x1's output tile)
+  int32_t act2, out2_f32;
+  const float* bias2;                 // [Cout2] or nullptr
 };
 
 struct ConvDesc {
@@ -63,6 +74,17 @@ struct ConvDesc {
   const float* pre; int pre_h, pre_w;      // optional half-resolution fp32 pre-activation addend (see GemmParams::pre)
 };
 
+// A square 1x1 conv run in the epilogue of the conv it reads (conv_gemm_chain_build): its input is the channel run
+// [k0, k0 + Cout - part_C) of that conv's output, followed by an optional partner slice of part_C channels
+struct ChainDesc {
+  const void* w;                           // bf16 [Cout][Cout]
+  const float* bias;
+  int Cout, act, k0;
+  const void* part; int part_cs, part_co, part_C;    // partner slice (bf16, same pixels as the output) or nullptr
+  void* out; int out_cs, out_co, out_f32;
+  bool store1;                             // also store the first conv's output (ConvDesc::out)
+};
+
 struct GemmLaunch {
   GemmParams p;
   int grid, smem_bytes;
@@ -72,6 +94,9 @@ struct GemmLaunch {
 
 // Returns 0 on success; <0 and sets cc_last_error otherwise.
 int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* out);
+// The conv d with the 1x1 c in its epilogue: bit-identical to two conv_gemm_build launches.  Fails with CC_ERR_INVALID
+// (nothing built) when the pair does not chain: see the conditions in conv_gemm.cu.
+int conv_gemm_chain_build(const ConvDesc& d, const ChainDesc& c, int num_sms, GemmLaunch* out);
 int conv_gemm_launch(const GemmLaunch& L, cudaStream_t stream);
 bool conv_gemm_supported(const ConvDesc& d);
 

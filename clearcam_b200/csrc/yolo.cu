@@ -455,6 +455,9 @@ struct Builder {
   std::map<int, Place> place;               // layer -> slice of a concat buffer
   std::map<int, T> concat_buf;              // concat layer -> buffer
   std::vector<int> outC;                    // inferred channels per layer
+  // a Conv layer whose only reader is the next layer's ELAN cv1: its conv is queued there, chained with that cv1
+  struct Deferred { std::string key; T in, out; int stride = 1, layer = -1; } deferred;
+  std::vector<int> folded;                  // layers whose output a chained launch never stored
 
   Bump bump;                                // workspace carving; bump.dry = measuring pass (no launches are built)
   size_t scratch_bytes = 0;                 // fp32-accurate mode: size of the plane-split scratch (from the measuring pass)
@@ -540,6 +543,46 @@ struct Builder {
     }
     P.ops.push_back(std::move(op));
   }
+  // conv key1 (in -> out1) followed by the 1x1 conv key2 over in2, a slice of out1's buffer that starts inside out1 and may
+  // run past its end (the partner: channels another conv wrote), into out2 (or the dense fp32 map out2_f32).  One chained
+  // launch (conv_gemm_chain_build) when the pair chains, and then out1 is written only when keep1; else the two convs.
+  // Returns whether the pair was chained.
+  bool conv_pair(const std::string& key1, const T& in, const T& out1, int stride, const T* res, const std::string& key2, const T& in2,
+                 const T& out2, int act2, float* out2_f32, bool keep1) {
+    if (rc) return false;
+    auto i1 = M.convs.find(key1), i2 = M.convs.find(key2);
+    if (!bump.dry && !M.precise && i1 != M.convs.end() && i2 != M.convs.end()) {
+      const ConvW& c1 = i1->second;
+      const ConvW& c2 = i2->second;
+      const int part_c = in2.co + in2.C - (out1.co + out1.C);
+      if (c1.groups == 1 && tc_ok(c1.cin, c1.cout) && c1.cin == in.C && c2.groups == 1 && c2.k == 1 && c2.cin == in2.C &&
+          c2.cout == c2.cin && in2.p == out1.p && in2.cs == out1.cs && in2.co >= out1.co && in2.co < out1.co + out1.C) {
+        ConvDesc d{};
+        d.in = in.p; d.in_cs = in.cs; d.in_co = in.co; d.Cin = in.C;
+        d.N = P.B; d.Hin = in.H; d.Win = in.W; d.k = c1.k; d.stride = stride;
+        d.w = c1.w; d.bias = c1.bias;
+        d.out = out1.p; d.out_cs = out1.cs; d.out_co = out1.co; d.Cout = c1.cout; d.out_f32 = 0; d.act = CC_ACT_SILU;
+        if (res) { d.res = res->p; d.res_cs = res->cs; d.res_co = res->co; }
+        ChainDesc c{};
+        c.w = c2.w; c.bias = c2.bias; c.Cout = c2.cout; c.act = act2; c.k0 = in2.co - out1.co;
+        if (part_c > 0) { c.part = in2.p; c.part_cs = in2.cs; c.part_co = out1.co + out1.C; c.part_C = part_c; }
+        if (out2_f32) { c.out = out2_f32; c.out_cs = c2.cout; c.out_co = 0; c.out_f32 = 1; }
+        else { c.out = out2.p; c.out_cs = out2.cs; c.out_co = out2.co; c.out_f32 = 0; }
+        c.store1 = keep1;
+        Op op;
+        op.kind = Op::GEMM;
+        op.name = key1 + "+" + key2;
+        if (conv_gemm_chain_build(d, c, M.sms, &op.gemm) == CC_OK) {
+          P.conv_flops += op.gemm.flops;
+          P.ops.push_back(std::move(op));
+          return true;
+        }
+      }
+    }
+    conv(key1, in, out1, stride, CC_ACT_SILU, res);   // the pair does not chain here (shape, tile width, smem, fp32 mode)
+    conv(key2, in2, out2, 1, act2, nullptr, out2_f32);
+    return false;
+  }
   void simple(Op::Kind kind, const T& in, const T& out, const char* name) {
     if (rc || bump.dry) return;
     Op op; op.kind = kind; op.s_in = ts(in); op.s_out = ts(out); op.name = name;
@@ -555,20 +598,24 @@ struct Builder {
     return slice(concat_buf[ci], it->second.co, C);
   }
 
-  // RepNCSP (detection/yolov9.py:92-105) on `x` (2b channels) -> fresh 2b-channel tensor
-  T repncsp(const std::string& pfx, const T& x, int b, int n) {
-    T t1 = talloc(2 * b, x.H, x.W);                         // [x1 | x3]
-    conv(pfx + ".cv1+cv2", x, t1, 1, CC_ACT_SILU);
+  // RepNCSP (detection/yolov9.py:92-105) on `x` (2b channels) -> fresh 2b-channel tensor.  t1 = [x1 | x3] = cv1+cv2(x); the
+  // caller may already have queued that conv (chained onto x's producer) into `t1_done`.  The last bottleneck's cv2 and cv3
+  // over [x1 | x3] run as one chained launch where they can (x1's final value is then never stored).
+  T repncsp(const std::string& pfx, const T& x, int b, int n, const T* t1_done = nullptr) {
+    T t1 = t1_done ? *t1_done : talloc(2 * b, x.H, x.W);    // [x1 | x3]
+    if (!t1_done) conv(pfx + ".cv1+cv2", x, t1, 1, CC_ACT_SILU);
     T x1 = slice(t1, 0, b);
+    T o = talloc(2 * b, x.H, x.W);
+    if (n == 0) conv(pfx + ".cv3", t1, o, 1, CC_ACT_SILU);
     for (int i = 0; i < n; ++i) {
       T t2 = talloc(b, x.H, x.W);
       conv(pfx + ".m." + std::to_string(i) + ".cv1", x1, t2, 1, CC_ACT_SILU);
-      conv(pfx + ".m." + std::to_string(i) + ".cv2", t2, x1, 1, CC_ACT_SILU, &x1);   // x + cv2(cv1(x)), in place
+      if (i + 1 < n) conv(pfx + ".m." + std::to_string(i) + ".cv2", t2, x1, 1, CC_ACT_SILU, &x1);   // x + cv2(cv1(x)), in place
+      else conv_pair(pfx + ".m." + std::to_string(i) + ".cv2", t2, x1, 1, &x1, pfx + ".cv3", t1, o, CC_ACT_SILU, nullptr, false);
     }
-    T o = talloc(2 * b, x.H, x.W);
-    conv(pfx + ".cv3", t1, o, 1, CC_ACT_SILU);
     return o;
   }
+
 
   int build();
 };
@@ -607,6 +654,18 @@ static bool fuse_up_concat(const std::vector<Layer>& S, const std::vector<int>& 
   const int cu = outC[i - 2], cskip = outC[i - 1] - cu;
   if (cu % 16 || cskip % 16 || cu <= 0 || cskip <= 0 || (4 * e.b) % 16) return false;
   if (c_up) *c_up = cu;
+  return true;
+}
+
+// Conv layer i feeds only the next layer, an ELAN4 whose cv1 reads it whole (not the fused Upsample -> Concat form): the conv
+// can run with that cv1 chained in its epilogue and its own output never stored.
+static bool conv_feeds_only_elan(const std::vector<Layer>& S, const std::vector<int>& outC, int i, bool precise) {
+  const int nl = static_cast<int>(S.size());
+  if (i + 1 >= nl || S[i + 1].op != L_ELAN4 || S[i + 1].f.size() != 1 || S[i + 1].f[0] != -1) return false;
+  if (fuse_up_concat(S, outC, i + 1, precise)) return false;
+  for (int j = 0; j < nl; ++j)
+    for (int f : S[j].f)
+      if (j != i + 1 && (f == -1 ? j - 1 : f) == i) return false;
   return true;
 }
 
@@ -718,7 +777,8 @@ int Builder::build() {
           P.ops.push_back(std::move(op));
         } else {
           out = out_for(i, l.b, l.s == 2 ? in.H / 2 : in.H, l.s == 2 ? in.W / 2 : in.W);
-          conv(pfx, in, out, l.s, CC_ACT_SILU);
+          if (!place.count(i) && conv_feeds_only_elan(S, outC, i, M.precise)) deferred = {pfx, in, out, l.s, i};
+          else conv(pfx, in, out, l.s, CC_ACT_SILU);
         }
         break;
       }
@@ -737,6 +797,7 @@ int Builder::build() {
         // detection/yolov9.py:107-125
         const int b = l.b;
         T cat = talloc(8 * b, in.H, in.W);
+        T t1 = talloc(2 * b, in.H, in.W);                  // RepNCSP cv2.0's [x1 | x3]
         if (fuse_up_concat(S, outC, i, M.precise)) {
           const T& lo = outs[i - 3];                       // the Upsample layer's source
           const T& hi = src(S[i - 1].f[1]);                // the Concat's second source
@@ -754,12 +815,23 @@ int Builder::build() {
             g_hi.flops = full;
             g_lo.flops = 0.0;
           }
-        } else {
-          conv(pfx + ".cv1", in, slice(cat, 0, 4 * b), 1, CC_ACT_SILU);
+          conv(pfx + ".cv2.0.cv1+cv2", slice(cat, 2 * b, 2 * b), t1, 1, CC_ACT_SILU);
+        } else if (deferred.layer == i - 1) {   // the previous Conv with cv1 chained in its epilogue; its output is not stored
+          if (conv_pair(deferred.key, deferred.in, deferred.out, deferred.stride, nullptr, pfx + ".cv1", in, slice(cat, 0, 4 * b),
+                        CC_ACT_SILU, nullptr, false))
+            folded.push_back(i - 1);
+          deferred.layer = -1;
+          conv(pfx + ".cv2.0.cv1+cv2", slice(cat, 2 * b, 2 * b), t1, 1, CC_ACT_SILU);
+        } else {   // cv1 -> cat[0, 4b) (kept: cv4 reads it) chained with cv2.0's cv1+cv2 on y1 = cat[2b, 4b)
+          conv_pair(pfx + ".cv1", in, slice(cat, 0, 4 * b), 1, nullptr, pfx + ".cv2.0.cv1+cv2", slice(cat, 2 * b, 2 * b), t1, CC_ACT_SILU,
+                    nullptr, true);
         }
-        T r1 = repncsp(pfx + ".cv2.0", slice(cat, 2 * b, 2 * b), b, l.n);
-        conv(pfx + ".cv2.1", r1, slice(cat, 4 * b, 2 * b), 1, CC_ACT_SILU);
-        T r2 = repncsp(pfx + ".cv3.0", slice(cat, 4 * b, 2 * b), b, l.n);
+        T r1 = repncsp(pfx + ".cv2.0", slice(cat, 2 * b, 2 * b), b, l.n, &t1);
+        // cv2.1 -> y2 = cat[4b, 6b) (kept) chained with cv3.0's cv1+cv2 on y2
+        T t1b = talloc(2 * b, in.H, in.W);
+        conv_pair(pfx + ".cv2.1", r1, slice(cat, 4 * b, 2 * b), 1, nullptr, pfx + ".cv3.0.cv1+cv2", slice(cat, 4 * b, 2 * b), t1b,
+                  CC_ACT_SILU, nullptr, true);
+        T r2 = repncsp(pfx + ".cv3.0", slice(cat, 4 * b, 2 * b), b, l.n, &t1b);
         conv(pfx + ".cv3.1", r2, slice(cat, 6 * b, 2 * b), 1, CC_ACT_SILU);
         out = out_for(i, l.c, in.H, in.W);
         conv(pfx + ".cv4", cat, out, 1, CC_ACT_SILU);
@@ -865,12 +937,12 @@ int Builder::build() {
             conv(hp + ".cv3." + sq + ".0", x, slice(t0, 64, d), 1, CC_ACT_SILU);
           }
           T tb = talloc(64, x.H, x.W), tc = talloc(d, x.H, x.W);
-          conv(hp + ".cv2." + sq + ".1", slice(t0, 0, 64), tb, 1, CC_ACT_SILU);
-          conv(hp + ".cv3." + sq + ".1", slice(t0, 64, d), tc, 1, CC_ACT_SILU);
           float* bl = static_cast<float*>(dalloc(static_cast<size_t>(P.B) * x.H * x.W * 64 * 4));
           float* cl = static_cast<float*>(dalloc(static_cast<size_t>(P.B) * x.H * x.W * 80 * 4));
           T dummy;
-          conv(hp + ".cv2." + sq + ".2", tb, dummy, 1, CC_ACT_NONE, nullptr, bl);
+          // box branch: cv2.j.1 chained with its 1x1 logits cv2.j.2 (tb is then never stored)
+          conv_pair(hp + ".cv2." + sq + ".1", slice(t0, 0, 64), tb, 1, nullptr, hp + ".cv2." + sq + ".2", tb, dummy, CC_ACT_NONE, bl, false);
+          conv(hp + ".cv3." + sq + ".1", slice(t0, 64, d), tc, 1, CC_ACT_SILU);
           conv(hp + ".cv3." + sq + ".2", tc, dummy, 1, CC_ACT_NONE, nullptr, cl);
           dec.dec.box[q] = bl; dec.dec.cls[q] = cl; dec.dec.h[q] = x.H; dec.dec.w[q] = x.W;
           dec.dec.stride[q] = float(P.H / x.H);
@@ -894,6 +966,7 @@ int Builder::build() {
   }
   P.n_launch = static_cast<int>(P.ops.size());
   P.layer_outs = outs;
+  for (int f : folded) P.layer_outs[f].p = nullptr;   // reported as a folded layer (a shape, no tensor)
   return rc;
 }
 

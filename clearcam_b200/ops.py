@@ -21,6 +21,23 @@ def conv2d(xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, Cout, act=0, res=
     return obuf
 
 
+def conv2d_chain(xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, w2, bias2, k0, o2buf, out2_co, act2=1, part=None,
+                 part_co=0, part_C=0, res=None, res_co=0, store1=True, stream=None):
+    """A SiLU conv of w (bf16 [Cout,k,k,Cin]) into obuf[..., out_co:] and, in its epilogue, the square 1x1 conv w2 (bf16
+    [Cout2,1,1,Cout2]) over [its output channels k0.. | part[..., part_co:part_co + part_C]] into o2buf[..., out2_co:] (bf16 with
+    act2 = 1 SiLU, or fp32 with act2 = 0).  store1=False drops the first output (obuf may be None)."""
+    assert xbuf.is_cuda and xbuf.dtype == torch.bfloat16 and xbuf.is_contiguous() and w.is_contiguous() and w2.is_contiguous()
+    N, H, W, in_cs = xbuf.shape
+    Cout, Cout2 = w.shape[0], w2.shape[0]
+    rc = lib().cc_conv2d_chain(ptr(xbuf), N, H, W, in_cs, in_co, Cin, ptr(w), ptr(bias), Cout, k, stride, ptr(obuf),
+                               0 if obuf is None else obuf.shape[-1], out_co, int(store1), ptr(res),
+                               0 if res is None else res.shape[-1], res_co, ptr(w2), ptr(bias2), Cout2, act2, k0, ptr(part),
+                               0 if part is None else part.shape[-1], part_co, part_C, ptr(o2buf), o2buf.shape[-1], out2_co,
+                               int(o2buf.dtype == torch.float32), stream_ptr(stream))
+    check(rc, "cc_conv2d_chain")
+    return o2buf
+
+
 def attention(qkv, L, H, causal, impl, ctx=None, stream=None):
     """qkv: [B*L, 3*H*64] bf16 CUDA (Q | K | V rows of B sequences of L tokens) -> ctx [B*L, H*64] bf16, the attention of
     each (sequence, head).  impl: 1 = mma.sync kernel, 2 = wgmma kernel.  ctx may have more rows than B*L; only the first

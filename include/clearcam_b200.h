@@ -45,6 +45,19 @@ int cc_conv2d(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, i
               void* d_out, int out_cs, int out_co, int out_f32, int act,
               const void* d_res, int res_cs, int res_co, int impl, int bn, void* stream);
 
+/* One launch of two convs: a SiLU conv as cc_conv2d (wgmma, bf16 out) and a square 1x1 conv (d_w2: bf16 [Cout2][Cout2]) whose
+ * input is the channel run [k0, k0 + Cout2 - part_C) of the first conv's output followed by the partner slice (d_part, part_C
+ * channels at part_co of a buffer of part_cs channels, same pixels; or NULL), run in the first conv's epilogue.  act2 is
+ * CC_ACT_SILU with a bf16 second output or CC_ACT_NONE with fp32 (out2_f32).  store1 = 0 drops the first output (d_out may
+ * be NULL).  The results equal two cc_conv2d calls bit for bit.  A pair the kernel cannot chain (see conv_gemm.cu
+ * conv_gemm_chain_build) fails with CC_ERR_INVALID before anything is launched. */
+int cc_conv2d_chain(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin,
+                    const void* d_w, const float* d_bias, int Cout, int k, int stride,
+                    void* d_out, int out_cs, int out_co, int store1, const void* d_res, int res_cs, int res_co,
+                    const void* d_w2, const float* d_bias2, int Cout2, int act2, int k0,
+                    const void* d_part, int part_cs, int part_co, int part_C,
+                    void* d_out2, int out2_cs, int out2_co, int out2_f32, void* stream);
+
 /* ---- YOLOv9 detector (replaces detection/yolov9.py: class YOLOv9, :298-458) ---- */
 typedef struct cc_yolo cc_yolo;
 
