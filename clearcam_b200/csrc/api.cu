@@ -21,12 +21,10 @@ int cc_conv2d(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, i
               int out_f32, int act, const void* d_res, int res_cs, int res_co, int impl, int bn, void* stream) {
   const int sms = device_sm_count();
   CC_REQUIRE(sms > 0, "cc_conv2d: no sm_90 (H100) device");
-  ConvDesc d{};
-  d.in = d_in; d.in_cs = in_cs; d.in_co = in_co; d.Cin = Cin;
-  d.N = N; d.Hin = Hin; d.Win = Win; d.k = k; d.stride = stride;
-  d.w = d_w; d.bias = d_bias;
-  d.out = d_out; d.out_cs = out_cs; d.out_co = out_co; d.Cout = Cout; d.out_f32 = out_f32;
-  d.act = act; d.res = d_res; d.res_cs = res_cs; d.res_co = res_co; d.bn_override = bn;
+  const TSlice res = nhwc_slice(d_res, res_cs, res_co, Cout, out_f32);
+  ConvDesc d = conv_desc(nhwc_slice(d_in, in_cs, in_co, Cin, 0, N, Hin, Win), d_w, d_bias, k, stride,
+                         nhwc_slice(d_out, out_cs, out_co, Cout, out_f32), act, d_res ? &res : nullptr);
+  d.bn_override = bn;
   const bool gemm_ok = groups == 1 && conv_gemm_supported(d);
   CC_REQUIRE(impl != 1 || gemm_ok, "cc_conv2d: shape not supported by the wgmma path");
   if (impl != 2 && gemm_ok) {
@@ -35,16 +33,7 @@ int cc_conv2d(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, i
     if (rc) return rc;
     return conv_gemm_launch(L, static_cast<cudaStream_t>(stream));
   }
-  DirectConvParams p{};
-  p.in = static_cast<const __nv_bfloat16*>(d_in); p.in_cs = in_cs; p.in_co = in_co; p.Cin = Cin;
-  p.N = N; p.Hin = Hin; p.Win = Win; p.Hbuf = Hin; p.Wbuf = Win;
-  p.k = k; p.stride = stride; p.pad = k / 2; p.groups = groups;
-  p.w = static_cast<const __nv_bfloat16*>(d_w); p.bias = d_bias;
-  p.out = d_out; p.out_cs = out_cs; p.out_co = out_co; p.Cout = Cout; p.out_f32 = out_f32;
-  p.Hout = (Hin + 2 * p.pad - k) / stride + 1;
-  p.Wout = (Win + 2 * p.pad - k) / stride + 1;
-  p.act = act; p.res = d_res; p.res_cs = res_cs; p.res_co = res_co;
-  return conv_direct_launch(p, static_cast<cudaStream_t>(stream));
+  return conv_direct_launch(direct_conv_params(d, groups), static_cast<cudaStream_t>(stream));
 }
 
 int cc_conv2d_chain(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const void* d_w, const float* d_bias,
@@ -55,16 +44,13 @@ int cc_conv2d_chain(const void* d_in, int N, int Hin, int Win, int in_cs, int in
   CC_REQUIRE(sms > 0, "cc_conv2d_chain: no sm_90 (H100) device");
   CC_REQUIRE(d_in && (d_out || !store1) && d_w2 && d_out2 && (!d_part || part_C > 0), "cc_conv2d_chain: NULL argument");
   CC_REQUIRE(!d_part || (part_co >= 0 && part_co + part_C <= part_cs), "cc_conv2d_chain: partner slice outside its row");
-  ConvDesc d{};
-  d.in = d_in; d.in_cs = in_cs; d.in_co = in_co; d.Cin = Cin;
-  d.N = N; d.Hin = Hin; d.Win = Win; d.k = k; d.stride = stride;
-  d.w = d_w; d.bias = d_bias;
-  d.out = d_out; d.out_cs = out_cs; d.out_co = out_co; d.Cout = Cout; d.out_f32 = 0;
-  d.act = CC_ACT_SILU; d.res = d_res; d.res_cs = res_cs; d.res_co = res_co;
+  const TSlice res = nhwc_slice(d_res, res_cs, res_co, Cout);
+  const ConvDesc d = conv_desc(nhwc_slice(d_in, in_cs, in_co, Cin, 0, N, Hin, Win), d_w, d_bias, k, stride,
+                               nhwc_slice(d_out, out_cs, out_co, Cout), CC_ACT_SILU, d_res ? &res : nullptr);
   ChainDesc c{};
-  c.w = d_w2; c.bias = d_bias2; c.Cout = Cout2; c.act = act2; c.k0 = k0;
-  c.part = d_part; c.part_cs = part_cs; c.part_co = part_co; c.part_C = d_part ? part_C : 0;
-  c.out = d_out2; c.out_cs = out2_cs; c.out_co = out2_co; c.out_f32 = out2_f32;
+  c.w = d_w2; c.bias = d_bias2; c.act = act2; c.k0 = k0;
+  if (d_part) c.part = nhwc_slice(d_part, part_cs, part_co, part_C);
+  c.out = nhwc_slice(d_out2, out2_cs, out2_co, Cout2, out2_f32);
   c.store1 = store1 != 0;
   CC_REQUIRE(out2_co >= 0 && out2_co + Cout2 <= out2_cs, "cc_conv2d_chain: second output slice outside its row");
   GemmLaunch L;
@@ -107,8 +93,7 @@ static int slice_arg(const char* who, const char* what, const void* p, int N, in
   CC_REQUIRE(N >= 1 && H >= 1 && W >= 1 && C >= 1, "%s: %s has a bad shape N=%d H=%d W=%d C=%d", who, what, N, H, W, C);
   CC_REQUIRE(C % vec == 0 && co % vec == 0 && cs % vec == 0 && co >= 0 && co + C <= cs,
              "%s: %s slice cs=%d co=%d C=%d must be whole vectors of %d channels inside the row", who, what, cs, co, C, vec);
-  *t = TSlice{};
-  t->p = static_cast<__nv_bfloat16*>(const_cast<void*>(p)); t->cs = cs; t->co = co; t->C = C; t->N = N; t->H = H; t->W = W; t->f32 = f32;
+  *t = nhwc_slice(p, cs, co, C, f32, N, H, W);
   return CC_OK;
 }
 
@@ -187,14 +172,11 @@ int cc_conv2d_pre(const void* d_in, int N, int Hin, int Win, int in_cs, int in_c
   CC_REQUIRE(d_in && d_w && d_out && d_pre, "cc_conv2d_pre: d_in, d_w, d_out and d_pre must not be NULL");
   CC_REQUIRE((reinterpret_cast<uintptr_t>(d_pre) & 15) == 0, "cc_conv2d_pre: d_pre must be 16-byte aligned");
   CC_REQUIRE(N >= 1 && Hin >= 1 && Win >= 1 && (stride == 1 || stride == 2), "cc_conv2d_pre: bad shape N=%d Hin=%d Win=%d stride=%d", N, Hin, Win, stride);
-  const int Ho = stride == 2 ? Hin / 2 : Hin, Wo = stride == 2 ? Win / 2 : Win;
+  const int Ho = conv_out(Hin, stride), Wo = conv_out(Win, stride);
   CC_REQUIRE(Ho % 2 == 0 && Wo % 2 == 0, "cc_conv2d_pre: the output %dx%d must have even sides (pre is its half-resolution map)", Ho, Wo);
-  ConvDesc d{};
-  d.in = d_in; d.in_cs = in_cs; d.in_co = in_co; d.Cin = Cin;
-  d.N = N; d.Hin = Hin; d.Win = Win; d.k = k; d.stride = stride;
-  d.w = d_w; d.bias = d_bias;
-  d.out = d_out; d.out_cs = out_cs; d.out_co = out_co; d.Cout = Cout; d.out_f32 = out_f32;
-  d.act = act; d.bn_override = bn;
+  ConvDesc d = conv_desc(nhwc_slice(d_in, in_cs, in_co, Cin, 0, N, Hin, Win), d_w, d_bias, k, stride,
+                         nhwc_slice(d_out, out_cs, out_co, Cout, out_f32), act);
+  d.bn_override = bn;
   d.pre = d_pre; d.pre_h = Ho / 2; d.pre_w = Wo / 2;
   CC_REQUIRE(conv_gemm_supported(d), "cc_conv2d_pre: shape not supported by the wgmma conv (Cin=%d Cout=%d k=%d stride=%d)", Cin, Cout, k, stride);
   const int sms = device_sm_count();

@@ -138,13 +138,10 @@ struct PlanBuilder {
   void gemm(const char* name, const __nv_bfloat16* A, int lda, int Mrows, int K, const __nv_bfloat16* Wt, const float* bias,
             int N, void* out, int ldc, bool f32, int act, const void* res, int n_img = 1, int rows_per_img = 0, int out_ns = 0) {
     if (rc) return;
-    ConvDesc d{};
-    d.in = A; d.in_cs = lda; d.in_co = 0; d.Cin = K;
-    d.N = n_img; d.Hin = 1; d.Win = rows_per_img ? rows_per_img : Mrows;
-    d.k = 1; d.stride = 1; d.w = Wt; d.bias = bias;
-    d.out = out; d.out_cs = ldc; d.out_co = 0; d.Cout = N; d.out_f32 = f32 ? 1 : 0; d.act = act;
-    d.res = res; d.res_cs = ldc; d.res_co = 0; d.out_ns = out_ns;
     if (bump.dry) return;
+    const TSlice o = nhwc_slice(out, ldc, 0, N, f32 ? 1 : 0), r = nhwc_slice(res, ldc, 0, N, f32 ? 1 : 0);
+    ConvDesc d = conv_desc(nhwc_slice(A, lda, 0, K, 0, n_img, 1, rows_per_img ? rows_per_img : Mrows), Wt, bias, 1, 1, o, act, res ? &r : nullptr);
+    d.out_ns = out_ns;
     VOp op; op.kind = VOp::GEMM; op.name = name;
     rc = conv_gemm_build(d, M.sms, &op.gemm);
     if (rc) return;

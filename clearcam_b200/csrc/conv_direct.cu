@@ -3,6 +3,7 @@
 // convs, odd spatial sizes with stride 2) and the stem.  fp32 accumulate, same epilogue semantics as
 // conv_gemm (bias -> act -> +residual).  Reference: detection/yolov9.py:33-38 (Conv), :171-194 (head convs).
 #include "ops.cuh"
+#include "conv_gemm.cuh"
 #include "cc_common.h"
 #include <cuda_bf16.h>
 
@@ -64,6 +65,19 @@ __global__ void conv_direct_kernel(DirectConvParams p) {
       else reinterpret_cast<__nv_bfloat16*>(p.out)[opix * p.out_cs + p.out_co + co] = __float2bfloat16_rn(x);
     }
   }
+}
+
+DirectConvParams direct_conv_params(const ConvDesc& d, int groups) {
+  DirectConvParams p{};
+  p.in = d.in.p; p.in_cs = d.in.cs; p.in_co = d.in.co; p.Cin = d.in.C;
+  p.N = d.in.N; p.Hin = d.in.H; p.Win = d.in.W; p.Hbuf = d.in.H; p.Wbuf = d.in.W;
+  p.k = d.k; p.stride = d.stride; p.pad = d.k / 2; p.groups = groups;
+  p.w = static_cast<const __nv_bfloat16*>(d.w); p.bias = d.bias;
+  p.out = d.out.p; p.out_cs = d.out.cs; p.out_co = d.out.co; p.Cout = d.out.C; p.out_f32 = d.out.f32;
+  p.Hout = (p.Hin + 2 * p.pad - p.k) / p.stride + 1;   // the general form: conv_out() only holds for the GEMM kernel's shapes
+  p.Wout = (p.Win + 2 * p.pad - p.k) / p.stride + 1;
+  p.act = d.act; p.res = d.res.p; p.res_cs = d.res.cs; p.res_co = d.res.co;
+  return p;
 }
 
 int conv_direct_launch(const DirectConvParams& p, cudaStream_t stream) {

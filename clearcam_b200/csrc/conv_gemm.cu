@@ -470,11 +470,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
 // ------------------------------------------------------------------------------------------------ host
 
 bool conv_gemm_supported(const ConvDesc& d) {
-  if (d.Cin % 16 != 0 || d.Cout % 16 != 0) return false;
+  if (d.in.C % 16 != 0 || d.out.C % 16 != 0) return false;
   if (!(d.k == 1 || d.k == 3)) return false;
   if (!(d.stride == 1 || d.stride == 2)) return false;
-  if (d.stride == 2 && (d.k != 3 || (d.Hin & 1) || (d.Win & 1))) return false;
-  if (d.in_co % 8 != 0 || d.in_cs % 8 != 0) return false;
+  if (d.stride == 2 && (d.k != 3 || (d.in.H & 1) || (d.in.W & 1))) return false;
+  if (d.in.co % 8 != 0 || d.in.cs % 8 != 0) return false;
   return true;
 }
 
@@ -490,33 +490,69 @@ static int pick_bn(int cout, long long m_tiles, int bn_override, int num_sms) {
 }
 static int pick_bk(int cin) { return (cin % 64 == 0) ? 64 : (cin % 32 == 0 ? 32 : 16); }
 
+// the swizzle whose span is one box row: the kernel reads / writes the shared-memory tile with the same XOR
+static CUtensorMapSwizzle swizzle_of(int span_bytes) {
+  return span_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : span_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
+}
+
+// The slice s (elements of es bytes) as [N][H][W][C] at the launch's output pixels with the buffer's strides, ns pixels from
+// one image to the next; box = `cols` channels x the 128-pixel tile box.  For the epilogue's TMA stores and loads.
+static int encode_slice(const GemmParams& p, CUtensorMap* tm, const TSlice& s, int es, int cols, int ns, const char* who, const char* what) {
+  CC_REQUIRE((size_t(s.cs) * es) % 16 == 0 && (size_t(s.co) * es) % 16 == 0, "%s: %s slice not 16-B aligned", who, what);
+  void* base = reinterpret_cast<uint8_t*>(s.p) + size_t(s.co) * es;
+  cuuint64_t dims[4] = {cuuint64_t(s.C), cuuint64_t(p.W), cuuint64_t(p.H), cuuint64_t(p.N)};
+  const cuuint64_t px = cuuint64_t(s.cs) * es;     // bytes per pixel
+  cuuint64_t strides[3] = {px, px * p.W, px * ns};
+  cuuint32_t box[4] = {cuuint32_t(cols), cuuint32_t(1 << p.lTW), cuuint32_t(1 << p.lTH), cuuint32_t(1 << p.lTN)};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = get_encode_tiled()(tm, es == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, dims, strides,
+                                  box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_of(cols * es), CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CC_REQUIRE(r == CUDA_SUCCESS, "%s: cuTensorMapEncodeTiled(%s) failed: %d", who, what, int(r));
+  return CC_OK;
+}
+
+// Shared-memory budget -> pipeline depth of a launch whose tiling is set: the arithmetic the kernel's carve-up follows.
+// `fixed`: everything but the operands (alignment slack, the consumers' staging, bias, barriers, a chained 1x1's weights).
+// The weights of a single N block stay resident when they leave room for at least four activation stages: the ring then
+// carries A only and the weights cross the L2 once per CTA instead of once per tile.  Returns the stage count (at most 8).
+static int set_smem_budget(GemmLaunch* L, int fixed) {
+  GemmParams& p = L->p;
+  const int a_bytes = kTileM * p.BK * 2, b_bytes = p.BN * p.BK * 2;
+  const int bres_bytes = b_bytes * p.num_taps * p.chunks_per_tap;
+  p.b_res = (p.n_blocks == 1 && (kMaxSmem - fixed - bres_bytes) / a_bytes >= 4) ? 1 : 0;
+  int S = p.b_res ? (kMaxSmem - fixed - bres_bytes) / a_bytes : (kMaxSmem - fixed) / (a_bytes + b_bytes);
+  if (S > 8) S = 8;
+  p.stages = S;
+  L->smem_bytes = fixed + (p.b_res ? bres_bytes + S * a_bytes : S * (a_bytes + b_bytes));
+  return S;
+}
+
 // with_out = false: no first output (a chained launch that drops it; tmO stays unset)
 static int gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L, bool with_out) {
-  CC_REQUIRE(conv_gemm_supported(d), "conv_gemm: unsupported shape Cin=%d Cout=%d k=%d s=%d Hin=%d Win=%d", d.Cin, d.Cout,
-             d.k, d.stride, d.Hin, d.Win);
+  const int Cin = d.in.C, Cout = d.out.C, N = d.in.N;
+  CC_REQUIRE(conv_gemm_supported(d), "conv_gemm: unsupported shape Cin=%d Cout=%d k=%d s=%d Hin=%d Win=%d", Cin, Cout,
+             d.k, d.stride, d.in.H, d.in.W);
   PFN_encodeTiled enc = get_encode_tiled();
   CC_REQUIRE(enc != nullptr, "conv_gemm: cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
-  const int es = d.out_f32 ? 4 : 2;
-  CC_REQUIRE((d.out_cs * es) % 16 == 0 && (d.out_co * es) % 16 == 0, "conv_gemm: output slice not 16-B aligned");
-  if (d.res) CC_REQUIRE((d.res_cs * es) % 16 == 0 && (d.res_co * es) % 16 == 0, "conv_gemm: residual slice not 16-B aligned");
+  const int es = d.out.f32 ? 4 : 2;
 
   GemmParams& p = L->p;
   memset(&p, 0, sizeof(p));
-  const int Hout = d.stride == 2 ? d.Hin / 2 : d.Hin;
-  const int Wout = d.stride == 2 ? d.Win / 2 : d.Win;
-  p.W = Wout; p.H = Hout; p.N = d.N;
+  const int Hout = conv_out(d.in.H, d.stride), Wout = conv_out(d.in.W, d.stride);
+  p.W = Wout; p.H = Hout; p.N = N;
 
   // ---- K blocking
-  p.BK = pick_bk(d.Cin);
+  p.BK = pick_bk(Cin);
   p.num_taps = d.k * d.k;
-  p.chunks_per_tap = d.Cin / p.BK;
+  p.chunks_per_tap = Cin / p.BK;
   // ---- N blocking
-  const long long mt = (static_cast<long long>(d.N) * Hout * Wout + 127) / 128;
-  const int BN = pick_bn(d.Cout, mt, d.bn_override, num_sms);
-  CC_REQUIRE(BN >= 16 && BN <= kMaxBN && d.Cout % BN == 0, "conv_gemm: bad BN=%d for Cout=%d", BN, d.Cout);
+  const long long mt = (static_cast<long long>(N) * Hout * Wout + 127) / 128;
+  const int BN = pick_bn(Cout, mt, d.bn_override, num_sms);
+  CC_REQUIRE(BN >= 16 && BN <= kMaxBN && Cout % BN == 0, "conv_gemm: bad BN=%d for Cout=%d", BN, Cout);
   p.BN = BN;
-  p.n_blocks = d.Cout / BN;
-  p.cout = d.Cout;
+  p.n_blocks = Cout / BN;
+  p.cout = Cout;
 
   // ---- M tile box: maximise useful pixels per 128-row tile
   int best[3] = {7, 0, 0};
@@ -525,15 +561,15 @@ static int gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L, bool with_o
     for (int lh = 0; lw + lh <= 7; ++lh) {
       const int ln = 7 - lw - lh;
       const int tw = 1 << lw, th = 1 << lh, tn = 1 << ln;
-      const double cover = double((Wout + tw - 1) / tw * tw) * ((Hout + th - 1) / th * th) * ((d.N + tn - 1) / tn * tn);
-      double eff = double(Wout) * Hout * d.N / cover + 1e-6 * lw - 1e-7 * ln;  // ties: wider rows, fewer images
+      const double cover = double((Wout + tw - 1) / tw * tw) * ((Hout + th - 1) / th * th) * ((N + tn - 1) / tn * tn);
+      double eff = double(Wout) * Hout * N / cover + 1e-6 * lw - 1e-7 * ln;  // ties: wider rows, fewer images
       if (eff > best_eff) { best_eff = eff; best[0] = lw; best[1] = lh; best[2] = ln; }
     }
   p.lTW = best[0]; p.lTH = best[1]; p.lTN = best[2];
   const int TW = 1 << p.lTW, TH = 1 << p.lTH, TN = 1 << p.lTN;
   p.tiles_w = (Wout + TW - 1) / TW;
   p.tiles_h = (Hout + TH - 1) / TH;
-  p.tiles_n = (d.N + TN - 1) / TN;
+  p.tiles_n = (N + TN - 1) / TN;
   p.num_tiles = p.tiles_w * p.tiles_h * p.tiles_n * p.n_blocks;
   p.s2 = d.stride == 2;
 
@@ -548,26 +584,26 @@ static int gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L, bool with_o
         // input col 2x+s-1: s=0 -> (pair x-1, odd), s=1 -> (pair x, even), s=2 -> (pair x, odd); same for rows
         const int wp = (s == 1) ? 0 : 1, dw = (s == 0) ? -1 : 0;
         const int hp = (r == 1) ? 0 : 1, dh = (r == 0) ? -1 : 0;
-        t[0] = wp * d.in_cs; t[1] = dw; t[2] = hp; t[3] = dh;
+        t[0] = wp * d.in.cs; t[1] = dw; t[2] = hp; t[3] = dh;
       }
     }
 
   // ---- tensor maps
-  const CUtensorMapSwizzle swz = p.BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
-                               : p.BK == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
+  const CUtensorMapSwizzle swz = swizzle_of(p.BK * 2);
   {
-    void* base = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(d.in)) + size_t(d.in_co) * 2;
+    const int Hin = d.in.H, Win = d.in.W;
+    void* base = reinterpret_cast<uint8_t*>(d.in.p) + size_t(d.in.co) * 2;
     CC_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "conv_gemm: input slice not 16-B aligned");
     cuuint64_t dims[5], strides[4];
     cuuint32_t box[5], estr[5] = {1, 1, 1, 1, 1};
-    const cuuint64_t px = cuuint64_t(d.in_cs) * 2;  // bytes per pixel
+    const cuuint64_t px = cuuint64_t(d.in.cs) * 2;  // bytes per pixel
     if (!p.s2) {
-      dims[0] = d.Cin; dims[1] = d.Win; dims[2] = d.Hin; dims[3] = d.N; dims[4] = 1;
-      strides[0] = px; strides[1] = px * d.Win; strides[2] = px * d.Win * d.Hin; strides[3] = px * d.Win * d.Hin * d.N;
+      dims[0] = Cin; dims[1] = Win; dims[2] = Hin; dims[3] = N; dims[4] = 1;
+      strides[0] = px; strides[1] = px * Win; strides[2] = px * Win * Hin; strides[3] = px * Win * Hin * N;
       box[0] = p.BK; box[1] = TW; box[2] = TH; box[3] = TN; box[4] = 1;
     } else {
-      dims[0] = d.in_cs + d.Cin; dims[1] = d.Win / 2; dims[2] = 2; dims[3] = d.Hin / 2; dims[4] = d.N;
-      strides[0] = 2 * px; strides[1] = px * d.Win; strides[2] = 2 * px * d.Win; strides[3] = px * d.Win * d.Hin;
+      dims[0] = d.in.cs + Cin; dims[1] = Win / 2; dims[2] = 2; dims[3] = Hin / 2; dims[4] = N;
+      strides[0] = 2 * px; strides[1] = px * Win; strides[2] = 2 * px * Win; strides[3] = px * Win * Hin;
       box[0] = p.BK; box[1] = TW; box[2] = 1; box[3] = TH; box[4] = TN;
     }
     CUresult r = enc(&p.tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, base, dims, strides, box, estr,
@@ -577,8 +613,8 @@ static int gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L, bool with_o
                dims[0], dims[1], dims[2], dims[3], dims[4]);
   }
   {     // weights [Cout][Ktot] bf16, box = BK x BN
-    const cuuint64_t Ktot = cuuint64_t(d.k) * d.k * d.Cin;
-    cuuint64_t dims[2] = {Ktot, cuuint64_t(d.Cout)};
+    const cuuint64_t Ktot = cuuint64_t(d.k) * d.k * Cin;
+    cuuint64_t dims[2] = {Ktot, cuuint64_t(Cout)};
     cuuint64_t strides[1] = {Ktot * 2};
     cuuint32_t box[2] = {cuuint32_t(p.BK), cuuint32_t(BN)};
     cuuint32_t estr[2] = {1, 1};
@@ -589,32 +625,18 @@ static int gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L, bool with_o
   }
 
   // ---- epilogue
-  p.out = d.out; p.out_cs = d.out_cs; p.out_co = d.out_co; p.out_f32 = d.out_f32;
+  p.out = d.out.p; p.out_cs = d.out.cs; p.out_co = d.out.co; p.out_f32 = d.out.f32;
   p.bias = d.bias; p.act = d.act;
-  p.res = d.res; p.res_cs = d.res_cs; p.res_co = d.res_co;
+  p.res = d.res.p; p.res_cs = d.res.cs; p.res_co = d.res.co;
   p.out_ns = d.out_ns > 0 ? d.out_ns : Hout * Wout;
   p.pre = d.pre; p.pre_h = d.pre_h; p.pre_w = d.pre_w;
-  if (d.pre) CC_REQUIRE(d.pre_h * 2 == Hout && d.pre_w * 2 == Wout && d.Cout % 4 == 0, "conv_gemm: the pre-activation addend must be a half-resolution map of the output");
-  {     // output slice (and residual) as [N][H][W][Cout] with the buffer's strides, box = one staging column box x the pixel box
-    const int box_bytes = epi_box_bytes(BN, es);   // one swizzle span: the kernel writes the staging with the same XOR
-    const CUtensorMapSwizzle oswz = box_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                                  : box_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
-    auto encode = [&](CUtensorMap* tm, const void* buf, int cs, int co, const char* what) -> int {
-      void* base = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(buf)) + size_t(co) * es;
-      cuuint64_t dims[4] = {cuuint64_t(d.Cout), cuuint64_t(Wout), cuuint64_t(Hout), cuuint64_t(d.N)};
-      const cuuint64_t px = cuuint64_t(cs) * es;     // bytes per pixel
-      cuuint64_t strides[3] = {px, px * Wout, px * p.out_ns};
-      cuuint32_t box[4] = {cuuint32_t(box_bytes / es), cuuint32_t(TW), cuuint32_t(TH), cuuint32_t(TN)};
-      cuuint32_t estr[4] = {1, 1, 1, 1};
-      CUresult r = enc(tm, d.out_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, dims, strides, box,
-                       estr, CU_TENSOR_MAP_INTERLEAVE_NONE, oswz, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      CC_REQUIRE(r == CUDA_SUCCESS, "conv_gemm: cuTensorMapEncodeTiled(%s) failed: %d", what, int(r));
-      return CC_OK;
-    };
-    if (with_out)
-      if (int rc = encode(&p.tmO, d.out, d.out_cs, d.out_co, "out")) return rc;
-    if (d.res) if (int rc = encode(&p.tmR, d.res, d.res_cs, d.res_co, "residual")) return rc;
-  }
+  if (d.pre) CC_REQUIRE(d.pre_h * 2 == Hout && d.pre_w * 2 == Wout && Cout % 4 == 0, "conv_gemm: the pre-activation addend must be a half-resolution map of the output");
+  // output slice (and residual): box = one staging column box (one swizzle span) x the pixel box
+  const int box_cols = epi_box_bytes(BN, es) / es;
+  if (with_out)
+    if (int rc = encode_slice(p, &p.tmO, d.out, es, box_cols, p.out_ns, "conv_gemm", "output")) return rc;
+  if (d.res.p)
+    if (int rc = encode_slice(p, &p.tmR, d.res, es, box_cols, p.out_ns, "conv_gemm", "residual")) return rc;
   {
     auto fast_div = [](uint32_t d, uint32_t fd[2]) {      // q = (umulhi(mul, x) + x) >> shift for x < 2^31
       uint32_t l = 0;
@@ -628,28 +650,17 @@ static int gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L, bool with_o
   }
 
   // ---- smem budget -> pipeline depth.  Fixed part: alignment slack, one output staging tile per consumer, bias, barriers.
-  const int a_bytes = kTileM * p.BK * 2, b_bytes = BN * p.BK * 2;
-  const int fixed = 1024 + kConsumers * epi_stage_bytes(BN, es) + d.Cout * 4 + 8 * kBarriers;
-  const int num_kb = p.num_taps * p.chunks_per_tap;
-  const int bres_bytes = b_bytes * num_kb;
-  // resident weights (single N block) when they leave room for at least four activation stages: the ring then carries
-  // A only and the weights cross the L2 once per CTA instead of once per tile
-  p.b_res = (p.n_blocks == 1 && (kMaxSmem - fixed - bres_bytes) / a_bytes >= 4) ? 1 : 0;
-  int S = p.b_res ? (kMaxSmem - fixed - bres_bytes) / a_bytes : (kMaxSmem - fixed) / (a_bytes + b_bytes);
-  if (S > 8) S = 8;
+  const int S = set_smem_budget(L, 1024 + kConsumers * epi_stage_bytes(BN, es) + Cout * 4 + 8 * kBarriers);
   CC_REQUIRE(S >= 2, "conv_gemm: tile does not fit shared memory (BN=%d BK=%d)", BN, p.BK);
-  CC_REQUIRE(S <= 8, "conv_gemm: too many stages");
-  p.stages = S;
-  L->smem_bytes = fixed + (p.b_res ? bres_bytes + S * a_bytes : S * (a_bytes + b_bytes));
   L->grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-  L->flops = 2.0 * double(d.N) * Hout * Wout * d.Cout * d.k * d.k * d.Cin;
-  L->bytes = double(d.N) * d.Hin * d.Win * d.Cin * 2 + double(d.N) * Hout * Wout * d.Cout * es * ((with_out ? 1 : 0) + (d.res ? 1 : 0)) +
-             double(d.Cout) * d.k * d.k * d.Cin * 2;
+  L->flops = 2.0 * double(N) * Hout * Wout * Cout * d.k * d.k * Cin;
+  L->bytes = double(N) * d.in.H * d.in.W * Cin * 2 + double(N) * Hout * Wout * Cout * es * ((with_out ? 1 : 0) + (d.res.p ? 1 : 0)) +
+             double(Cout) * d.k * d.k * Cin * 2;
   return CC_OK;
 }
 
 int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
-  CC_REQUIRE(d.out != nullptr, "conv_gemm: no output");
+  CC_REQUIRE(d.out.p != nullptr, "conv_gemm: no output");
   return gemm_build(d, num_sms, L, true);
 }
 
@@ -667,87 +678,61 @@ static int chain_launch(const GemmLaunch& L, cudaStream_t stream, bool dry);
 //     followed by a partner slice exactly one staging box wide;
 //   * d's first output may be dropped only when d has one n block, and the operand ring keeps at least 4 stages.
 int conv_gemm_chain_build(const ConvDesc& d, const ChainDesc& c, int num_sms, GemmLaunch* L) {
-  CC_REQUIRE(c.w && c.out && (d.out || !c.store1), "conv_gemm chain: NULL weights or output");
-  CC_REQUIRE(d.act == ACT_SILU && !d.out_f32 && !silu_exact_env(), "conv_gemm chain: the first conv must be SiLU into bf16");
+  const int N2 = c.out.C, part_C = c.part.p ? c.part.C : 0;
+  CC_REQUIRE(c.w && c.out.p && (d.out.p || !c.store1), "conv_gemm chain: NULL weights or output");
+  CC_REQUIRE(d.act == ACT_SILU && !d.out.f32 && !silu_exact_env(), "conv_gemm chain: the first conv must be SiLU into bf16");
   CC_REQUIRE(!d.pre, "conv_gemm chain: the first conv takes no pre-activation addend");
-  CC_REQUIRE(c.Cout >= 16 && c.Cout <= kMaxBN && c.Cout % 16 == 0, "conv_gemm chain: the 1x1 has %d channels (16..128)", c.Cout);
-  CC_REQUIRE((c.act == ACT_SILU && !c.out_f32) || (c.act == ACT_NONE && c.out_f32 && c.Cout <= 64),
+  CC_REQUIRE(N2 >= 16 && N2 <= kMaxBN && N2 % 16 == 0, "conv_gemm chain: the 1x1 has %d channels (16..128)", N2);
+  CC_REQUIRE((c.act == ACT_SILU && !c.out.f32) || (c.act == ACT_NONE && c.out.f32 && N2 <= 64),
              "conv_gemm chain: the 1x1 is SiLU into bf16 or no activation into fp32 (<= 64 channels)");
-  const int Hout = d.stride == 2 ? d.Hin / 2 : d.Hin, Wout = d.stride == 2 ? d.Win / 2 : d.Win;
-  const long long mt = (static_cast<long long>(d.N) * Hout * Wout + 127) / 128;
-  CC_REQUIRE(pick_bn(c.Cout, mt, 0, num_sms) == c.Cout, "conv_gemm chain: the standalone 1x1 would tile its %d channels in blocks", c.Cout);
+  const int Hout = conv_out(d.in.H, d.stride), Wout = conv_out(d.in.W, d.stride);
+  const long long mt = (static_cast<long long>(d.in.N) * Hout * Wout + 127) / 128;
+  CC_REQUIRE(pick_bn(N2, mt, 0, num_sms) == N2, "conv_gemm chain: the standalone 1x1 would tile its %d channels in blocks", N2);
   if (int rc = gemm_build(d, num_sms, L, c.store1)) return rc;
   GemmParams& p = L->p;
   const int BN = p.BN;
   const int box_bytes = epi_box_bytes(BN, 2), box_cols = box_bytes / 2, box_tile = kTileM * box_bytes;
-  const int run = c.Cout - (c.part ? c.part_C : 0);
-  CC_REQUIRE(!c.part || c.part_C == box_cols, "conv_gemm chain: the partner slice must be one staging box (%d channels)", box_cols);
-  CC_REQUIRE(run > 0 && c.k0 >= 0 && c.k0 % 16 == 0 && c.k0 / BN == (c.k0 + run - 1) / BN && c.k0 + run <= d.Cout,
+  const int run = N2 - part_C;
+  CC_REQUIRE(!c.part.p || part_C == box_cols, "conv_gemm chain: the partner slice must be one staging box (%d channels)", box_cols);
+  CC_REQUIRE(run > 0 && c.k0 >= 0 && c.k0 % 16 == 0 && c.k0 / BN == (c.k0 + run - 1) / BN && c.k0 + run <= d.out.C,
              "conv_gemm chain: input run [%d, %d) is not inside one %d-channel n block", c.k0, c.k0 + run, BN);
-  CC_REQUIRE(!(d.res && BN == 128), "conv_gemm chain: a 128-channel tile takes no residual");
-  CC_REQUIRE((c.store1 && !c.part) || p.n_blocks == 1, "conv_gemm chain: a dropped first output or a partner needs one n block");
-  p.ch_n2 = c.Cout;
+  CC_REQUIRE(!(d.res.p && BN == 128), "conv_gemm chain: a 128-channel tile takes no residual");
+  CC_REQUIRE((c.store1 && !c.part.p) || p.n_blocks == 1, "conv_gemm chain: a dropped first output or a partner needs one n block");
+  p.ch_n2 = N2;
   p.ch_nb = c.k0 / BN;
   p.ch_k0 = c.k0 - p.ch_nb * BN;
-  p.ch_part = c.part ? 1 : 0;
+  p.ch_part = c.part.p ? 1 : 0;
   p.ch_store1 = c.store1 ? 1 : 0;
-  p.ch_bk2 = pick_bk(c.Cout);
+  p.ch_bk2 = pick_bk(N2);
   p.act2 = c.act;
-  p.out2_f32 = c.out_f32;
+  p.out2_f32 = c.out.f32;
   p.bias2 = c.bias;
-  const int es2 = c.out_f32 ? 4 : 2;
-  PFN_encodeTiled enc = get_encode_tiled();
-  CC_REQUIRE(enc != nullptr, "conv_gemm: cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
-  auto swz_of = [](int span) {
-    return span == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : span == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
-  };
+  const int es2 = c.out.f32 ? 4 : 2;
   {     // 1x1 weights [Cout2][Cin2 = Cout2], box = BK2 x Cout2
-    cuuint64_t dims[2] = {cuuint64_t(c.Cout), cuuint64_t(c.Cout)};
-    cuuint64_t strides[1] = {cuuint64_t(c.Cout) * 2};
-    cuuint32_t box[2] = {cuuint32_t(p.ch_bk2), cuuint32_t(c.Cout)};
+    cuuint64_t dims[2] = {cuuint64_t(N2), cuuint64_t(N2)};
+    cuuint64_t strides[1] = {cuuint64_t(N2) * 2};
+    cuuint32_t box[2] = {cuuint32_t(p.ch_bk2), cuuint32_t(N2)};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(&p.tmW2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(c.w), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz_of(p.ch_bk2 * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    CUresult r = get_encode_tiled()(&p.tmW2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(c.w), dims, strides, box, estr,
+                                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_of(p.ch_bk2 * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     CC_REQUIRE(r == CUDA_SUCCESS, "conv_gemm chain: cuTensorMapEncodeTiled(W2) failed: %d", int(r));
   }
-  const int TW = 1 << p.lTW, TH = 1 << p.lTH, TN = 1 << p.lTN;
-  // an NHWC slice [co, co + C) of a buffer of cs channels at the output's pixels, box = `cols` channels x the pixel box
-  auto encode = [&](CUtensorMap* tm, const void* buf, int cs, int co, int C, int es, int cols, const char* what) -> int {
-    CC_REQUIRE((size_t(cs) * es) % 16 == 0 && (size_t(co) * es) % 16 == 0, "conv_gemm chain: %s slice not 16-B aligned", what);
-    void* base = const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(buf)) + size_t(co) * es;
-    cuuint64_t dims[4] = {cuuint64_t(C), cuuint64_t(Wout), cuuint64_t(Hout), cuuint64_t(d.N)};
-    const cuuint64_t px = cuuint64_t(cs) * es;
-    cuuint64_t strides[3] = {px, px * Wout, px * Wout * Hout};
-    cuuint32_t box[4] = {cuuint32_t(cols), cuuint32_t(TW), cuuint32_t(TH), cuuint32_t(TN)};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(tm, es == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz_of(cols * es), CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CC_REQUIRE(r == CUDA_SUCCESS, "conv_gemm chain: cuTensorMapEncodeTiled(%s) failed: %d", what, int(r));
-    return CC_OK;
-  };
-  if (c.part)
-    if (int rc = encode(&p.tmP, c.part, c.part_cs, c.part_co, c.part_C, 2, box_cols, "partner")) return rc;
-  if (int rc = encode(&p.tmO2, c.out, c.out_cs, c.out_co, c.Cout, es2, epi_box_bytes(c.Cout, es2) / es2, "out2")) return rc;
+  if (c.part.p)
+    if (int rc = encode_slice(p, &p.tmP, c.part, 2, box_cols, Hout * Wout, "conv_gemm chain", "partner")) return rc;
+  if (int rc = encode_slice(p, &p.tmO2, c.out, es2, epi_box_bytes(N2, es2) / es2, Hout * Wout, "conv_gemm chain", "out2")) return rc;
 
   // ---- smem: each consumer's region holds its staging tile and the partner box, then the 1x1's output tile
-  const int stage1 = epi_stage_bytes(BN, 2) + (c.part ? box_tile : 0), stage2 = kTileM * c.Cout * es2;
+  const int stage1 = epi_stage_bytes(BN, 2) + (c.part.p ? box_tile : 0), stage2 = kTileM * N2 * es2;
   p.ch_stage = ((stage1 > stage2 ? stage1 : stage2) + 1023) & ~1023;
-  const int w2_bytes = (c.Cout * c.Cout * 2 + 1023) & ~1023;
-  const int a_bytes = kTileM * p.BK * 2, b_bytes = BN * p.BK * 2;
-  const int fixed = 1024 + kConsumers * p.ch_stage + w2_bytes + (d.Cout + c.Cout) * 4 + 8 * kBarriers;
-  const int num_kb = p.num_taps * p.chunks_per_tap;
-  const int bres_bytes = b_bytes * num_kb;
-  p.b_res = (p.n_blocks == 1 && (kMaxSmem - fixed - bres_bytes) / a_bytes >= 4) ? 1 : 0;
-  int S = p.b_res ? (kMaxSmem - fixed - bres_bytes) / a_bytes : (kMaxSmem - fixed) / (a_bytes + b_bytes);
-  if (S > 8) S = 8;
+  const int w2_bytes = (N2 * N2 * 2 + 1023) & ~1023;
+  const int S = set_smem_budget(L, 1024 + kConsumers * p.ch_stage + w2_bytes + (d.out.C + N2) * 4 + 8 * kBarriers);
   CC_REQUIRE(S >= 4, "conv_gemm chain: the operand ring would keep %d stages (at least 4)", S);
-  p.stages = S;
-  L->smem_bytes = fixed + (p.b_res ? bres_bytes + S * a_bytes : S * (a_bytes + b_bytes));
-  const double px = double(d.N) * Hout * Wout;
-  L->flops += 2.0 * px * c.Cout * c.Cout;
-  L->bytes += px * ((c.part ? c.part_C * 2 : 0) + c.Cout * es2) + double(c.Cout) * c.Cout * 2;
+  const double px = double(d.in.N) * Hout * Wout;
+  L->flops += 2.0 * px * N2 * N2;
+  L->bytes += px * (part_C * 2 + N2 * es2) + double(N2) * N2 * 2;
   CC_REQUIRE(chain_launch(*L, nullptr, true) == CC_OK, "conv_gemm chain: no chained kernel for BN=%d and a %d-channel 1x1 (act %d, fp32 %d)",
-             BN, c.Cout, c.act, c.out_f32);
+             BN, N2, c.act, c.out.f32);
   return CC_OK;
 }
 
@@ -810,9 +795,8 @@ static int chain_launch(const GemmLaunch& L, cudaStream_t stream, bool dry) {
 int conv_gemm_launch(const GemmLaunch& L, cudaStream_t stream) {
   if (L.p.ch_n2 > 0) return chain_launch(L, stream, false);
   const bool f32 = L.p.out_f32 != 0;
-  static const int exact_env = getenv("CC_SILU_EXACT") ? atoi(getenv("CC_SILU_EXACT")) : 0;
   int act = L.p.act;
-  if (act == ACT_SILU && exact_env) act = ACT_SILU_EXACT;
+  if (act == ACT_SILU && silu_exact_env()) act = ACT_SILU_EXACT;
   switch (act) {
     case ACT_NONE: return f32 ? launch_variant<ACT_NONE, true>(L, stream) : launch_variant<ACT_NONE, false>(L, stream);
     case ACT_SILU: return f32 ? launch_variant<ACT_SILU, true>(L, stream) : launch_variant<ACT_SILU, false>(L, stream);

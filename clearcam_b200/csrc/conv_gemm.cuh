@@ -12,6 +12,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "ops.cuh"
 
 namespace cc {
 
@@ -60,28 +61,41 @@ struct GemmParams {
   const float* bias2;                 // [Cout2] or nullptr
 };
 
+// One conv / linear as the host describes it.  The slices carry pointer, row pitch, channel offset and width; the output
+// extent follows from the input's and the stride (conv_out), so the N / H / W of `out` and `res` are not read.
 struct ConvDesc {
-  const void* in; int in_cs, in_co, Cin;   // input buffer: channels per pixel, slice offset, slice width
-  int N, Hin, Win;                         // stored input dims (even for stride 2)
-  int k, stride;                           // k in {1,3}; pad = k/2; stride in {1,2}
+  TSlice in;                               // bf16 input slice; N, H, W: stored input dims (even for stride 2)
   const void* w;                           // bf16 [Cout][k*k*Cin]
   const float* bias;
-  void* out; int out_cs, out_co, Cout, out_f32;
+  int k, stride;                           // k in {1,3}; pad = k/2; stride in {1,2}
+  TSlice out;                              // output slice, C = Cout, bf16 or fp32 (f32); p == nullptr: none (a chain that drops it)
   int act;
-  const void* res; int res_cs, res_co;
+  TSlice res;                              // residual slice (same dtype as out), p == nullptr: none
   int bn_override;                         // 0 = heuristic
   int out_ns;                              // 0 = Hout*Wout; else pixels per image in the out/residual buffers
   const float* pre; int pre_h, pre_w;      // optional half-resolution fp32 pre-activation addend (see GemmParams::pre)
 };
+// The one place a ConvDesc is made; bn_override, out_ns and pre start at 0 and are set by the few callers that use them.
+inline ConvDesc conv_desc(const TSlice& in, const void* w, const float* bias, int k, int stride, const TSlice& out, int act,
+                          const TSlice* res = nullptr) {
+  ConvDesc d{};
+  d.in = in; d.w = w; d.bias = bias; d.k = k; d.stride = stride; d.out = out; d.act = act;
+  if (res) d.res = *res;
+  return d;
+}
+// Output extent of the convs the GEMM kernel runs (pad = k/2, even input sides for stride 2)
+inline int conv_out(int n, int stride) { return stride == 2 ? n / 2 : n; }
+// The same conv for the direct kernel (conv_direct.cu), which also takes grouped convs and odd extents
+DirectConvParams direct_conv_params(const ConvDesc& d, int groups);
 
 // A square 1x1 conv run in the epilogue of the conv it reads (conv_gemm_chain_build): its input is the channel run
-// [k0, k0 + Cout - part_C) of that conv's output, followed by an optional partner slice of part_C channels
+// [k0, k0 + out.C - part.C) of that conv's output, followed by an optional partner slice of part.C channels
 struct ChainDesc {
-  const void* w;                           // bf16 [Cout][Cout]
+  const void* w;                           // bf16 [Cout][Cout], Cout = out.C
   const float* bias;
-  int Cout, act, k0;
-  const void* part; int part_cs, part_co, part_C;    // partner slice (bf16, same pixels as the output) or nullptr
-  void* out; int out_cs, out_co, out_f32;
+  int act, k0;
+  TSlice part;                             // partner slice (bf16, same pixels as the output), p == nullptr: none
+  TSlice out;                              // bf16 or fp32 (f32) output slice
   bool store1;                             // also store the first conv's output (ConvDesc::out)
 };
 

@@ -31,6 +31,13 @@ struct TSlice {
   int N, H, W;
   int f32;
 };
+// Channels [co, co + C) of a buffer of cs channels per pixel.  The pixel extent may stay 0 where the reader fixes it: a conv's
+// output and residual slices take the extent that follows from its input and stride (ConvDesc).
+inline TSlice nhwc_slice(const void* p, int cs, int co, int C, int f32 = 0, int N = 0, int H = 0, int W = 0) {
+  return TSlice{static_cast<__nv_bfloat16*>(const_cast<void*>(p)), cs, co, C, N, H, W, f32};
+}
+// A dense fp32 map of C channels per pixel (the head logits, the fused-upsample addend, the fp32-accurate partial sums)
+inline TSlice dense_f32(const float* p, int C) { return nhwc_slice(p, C, 0, C, 1); }
 
 // fp32-accurate mode: fp32 activation slice -> six bf16 planes per pixel [lo | mid | hi | mid | hi | hi] (x = hi + mid + lo
 // exactly, each a bf16), the A operand of a tensor-core conv whose weights are laid out [hi | mid | lo | hi | mid | hi]:

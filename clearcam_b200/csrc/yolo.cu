@@ -252,7 +252,8 @@ static int require_net(const LbGeom& g, int Hf, int Wf, int res) {
   return CC_OK;
 }
 
-struct T { __nv_bfloat16* p = nullptr; int cs = 0, co = 0, C = 0, H = 0, W = 0; bool image = false; bool f32 = false; };   // f32: p is really float*
+// A tensor of the plan: a slice, or the input frames (`image`, no buffer of the plan's own)
+struct T : TSlice { bool image = false; T() : TSlice{} {} };
 
 struct Op {
   enum Kind { GEMM, DIRECT, AVGPAD, AVGMAX, MAXPOOL5, UPSAMPLE, CBFUSE, LETTERBOX, STEM, STEM_IM2COL, STEM_TC, DECODE, POST, SPLIT, FINISH, SPP3 } kind;
@@ -403,22 +404,16 @@ static bool tc_ok(int cin, int cout) { return cin % 16 == 0 && cout % 16 == 0; }
 // in-place fp32 residual of the epilogue (one round-to-nearest add), one GEMM for the five cross products (planes 0..4 against
 // the weight planes hi|mid|lo|hi|mid); a last pass applies bias, the exact SiLU and the residual and writes the output slice.
 static int precise_conv_ops(const std::string& key, const ConvW& cw, const TSlice& in, int stride, int act, __nv_bfloat16* scratch,
-                            float* accbuf, float* out, int out_cs, int out_co, const float* res, int res_cs, int res_co, int sms,
-                            std::vector<Op>* ops, double* conv_flops) {
+                            float* accbuf, const TSlice& out, const TSlice* res, int sms, std::vector<Op>* ops, double* conv_flops) {
   Op sp; sp.kind = Op::SPLIT; sp.name = key + ".split"; sp.s_in = in; sp.s_out = TSlice{}; sp.s_out.p = scratch;
   ops->push_back(std::move(sp));
-  const int Ho = stride == 2 ? in.H / 2 : in.H, Wo = stride == 2 ? in.W / 2 : in.W;
+  const int Ho = conv_out(in.H, stride), Wo = conv_out(in.W, stride);
   const int nseg = static_cast<int>(cw.seg_off.size());
+  const TSlice acc = dense_f32(accbuf, cw.cout);
   for (int g = 0; g <= nseg; ++g) {
-    ConvDesc d{};
-    d.in = scratch; d.in_cs = 6 * in.C;
-    if (g < nseg) { d.in_co = 5 * in.C + cw.seg_off[g]; d.Cin = cw.seg_c[g]; d.w = cw.whi[g]; }
-    else { d.in_co = 0; d.Cin = 5 * in.C; d.w = cw.w5; }
-    d.N = in.N; d.Hin = in.H; d.Win = in.W; d.k = cw.k; d.stride = stride;
-    d.bias = nullptr;
-    d.out = accbuf; d.out_cs = cw.cout; d.out_co = 0; d.out_f32 = 1;
-    d.Cout = cw.cout; d.act = CC_ACT_NONE;
-    if (g > 0) { d.res = accbuf; d.res_cs = cw.cout; d.res_co = 0; }
+    const TSlice planes = g < nseg ? nhwc_slice(scratch, 6 * in.C, 5 * in.C + cw.seg_off[g], cw.seg_c[g], 0, in.N, in.H, in.W)
+                                   : nhwc_slice(scratch, 6 * in.C, 0, 5 * in.C, 0, in.N, in.H, in.W);
+    const ConvDesc d = conv_desc(planes, g < nseg ? cw.whi[g] : cw.w5, nullptr, cw.k, stride, acc, CC_ACT_NONE, g > 0 ? &acc : nullptr);
     Op gop; gop.kind = Op::GEMM; gop.name = key + (g < nseg ? ".hi" + std::to_string(g) : ".cross");
     if (int rc = conv_gemm_build(d, sms, &gop.gemm)) return rc;
     gop.gemm.flops = g == 0 ? 2.0 * in.N * Ho * Wo * double(cw.cout) * cw.k * cw.k * cw.cin : 0.0;   // algorithmic FLOPs once
@@ -429,8 +424,8 @@ static int precise_conv_ops(const std::string& key, const ConvW& cw, const TSlic
   FinishParams& f = op.fin;
   f = FinishParams{};
   f.acc = accbuf; f.bias = cw.bias; f.act = act; f.npix = static_cast<long long>(in.N) * Ho * Wo; f.C = cw.cout;
-  f.out = out; f.out_cs = out_cs; f.out_co = out_co;
-  if (res) { f.res = res; f.res_cs = res_cs; f.res_co = res_co; }
+  f.out = reinterpret_cast<float*>(out.p); f.out_cs = out.cs; f.out_co = out.co;
+  if (res) { f.res = reinterpret_cast<const float*>(res->p); f.res_cs = res->cs; f.res_co = res->co; }
   ops->push_back(std::move(op));
   return CC_OK;
 }
@@ -475,21 +470,21 @@ struct Builder {
     return d;
   }
   T talloc(int C, int H, int W) {
-    T t; t.cs = C; t.co = 0; t.C = C; t.H = H; t.W = W; t.f32 = M.precise;
+    T t; t.cs = C; t.co = 0; t.C = C; t.N = P.B; t.H = H; t.W = W; t.f32 = M.precise;
     t.p = static_cast<__nv_bfloat16*>(dalloc(static_cast<size_t>(P.B) * H * W * C * (M.precise ? 4 : 2)));
     return t;
   }
   static T slice(const T& t, int co, int C) { T s = t; s.co = t.co + co; s.C = C; return s; }
-  TSlice ts(const T& t) const { TSlice s; s.p = t.p; s.cs = t.cs; s.co = t.co; s.C = t.C; s.N = P.B; s.H = t.H; s.W = t.W; s.f32 = t.f32 ? 1 : 0; return s; }
 
-  // conv: in -> out slice (out.H/W must already be the conv's output extent)
-  void conv(const std::string& key, const T& in, const T& out, int stride, int act, const T* res = nullptr,
-            float* out_f32 = nullptr, const float* pre = nullptr, int pre_h = 0, int pre_w = 0) {
+  // conv: in -> out slice, a tensor of the plan or a dense fp32 map (dense_f32)
+  void conv(const std::string& key, const TSlice& in, const TSlice& out, int stride, int act, const TSlice* res = nullptr,
+            const float* pre = nullptr, int pre_h = 0, int pre_w = 0) {
     if (rc) return;
     auto it = M.convs.find(key);
     if (it == M.convs.end()) { set_error("yolo plan: conv '%s' not loaded", key.c_str()); rc = CC_ERR_STATE; return; }
     const ConvW& cw = it->second;
     if (cw.cin != in.C) { set_error("yolo plan: conv '%s' expects Cin=%d, got %d", key.c_str(), cw.cin, in.C); rc = CC_ERR_INVALID; return; }
+    if (cw.cout != out.C) { set_error("yolo plan: conv '%s' writes Cout=%d, its output has %d", key.c_str(), cw.cout, out.C); rc = CC_ERR_INVALID; return; }
     if (M.precise) {
       if (!(cw.groups == 1 && tc_ok(cw.cin, cw.cout))) {
         set_error("yolo plan: conv '%s' (%d->%d, groups %d) has no tensor-core form; the fp32-accurate mode needs one", key.c_str(), cw.cin, cw.cout, cw.groups);
@@ -498,76 +493,50 @@ struct Builder {
       }
       const size_t need = static_cast<size_t>(P.B) * in.H * in.W * 6 * in.C * 2;
       if (need > max_scratch) max_scratch = need;
-      const size_t need_acc = static_cast<size_t>(P.B) * (stride == 2 ? in.H / 2 : in.H) * (stride == 2 ? in.W / 2 : in.W) * cw.cout * 4;
+      const size_t need_acc = static_cast<size_t>(P.B) * conv_out(in.H, stride) * conv_out(in.W, stride) * cw.cout * 4;
       if (need_acc > max_acc) max_acc = need_acc;
     }
     if (bump.dry) return;
     if (M.precise) {
-      float* o = out_f32 ? out_f32 : reinterpret_cast<float*>(out.p);
-      rc = precise_conv_ops(key, cw, ts(in), stride, act, scratch, accbuf, o, out_f32 ? cw.cout : out.cs, out_f32 ? 0 : out.co,
-                            res ? reinterpret_cast<const float*>(res->p) : nullptr, res ? res->cs : 0, res ? res->co : 0, M.sms,
-                            &P.ops, &P.conv_flops);
+      rc = precise_conv_ops(key, cw, in, stride, act, scratch, accbuf, out, res, M.sms, &P.ops, &P.conv_flops);
       return;
     }
+    ConvDesc d = conv_desc(in, cw.w, cw.bias, cw.k, stride, out, act, res);
+    d.pre = pre; d.pre_h = pre_h; d.pre_w = pre_w;
     Op op;
     op.name = key;
     if (cw.groups == 1 && tc_ok(cw.cin, cw.cout)) {
-      ConvDesc d{};
-      d.in = in.p; d.in_cs = in.cs; d.in_co = in.co; d.Cin = in.C;
-      d.N = P.B; d.Hin = in.H; d.Win = in.W; d.k = cw.k; d.stride = stride;
-      d.w = cw.w; d.bias = cw.bias;
-      if (out_f32) { d.out = out_f32; d.out_cs = cw.cout; d.out_co = 0; d.out_f32 = 1; }
-      else { d.out = out.p; d.out_cs = out.cs; d.out_co = out.co; d.out_f32 = 0; }
-      d.Cout = cw.cout; d.act = act;
-      if (res) { d.res = res->p; d.res_cs = res->cs; d.res_co = res->co; }
-      d.pre = pre; d.pre_h = pre_h; d.pre_w = pre_w;
       op.kind = Op::GEMM;
       rc = conv_gemm_build(d, M.sms, &op.gemm);
       if (rc) return;
       P.conv_flops += op.gemm.flops;
     } else {
-      DirectConvParams& q = op.direct;
-      q = DirectConvParams{};
-      q.in = in.p; q.in_cs = in.cs; q.in_co = in.co; q.Cin = in.C;
-      q.N = P.B; q.Hin = in.H; q.Win = in.W; q.Hbuf = in.H; q.Wbuf = in.W;
-      q.k = cw.k; q.stride = stride; q.pad = cw.k / 2; q.groups = cw.groups;
-      q.w = cw.w; q.bias = cw.bias;
-      if (out_f32) { q.out = out_f32; q.out_cs = cw.cout; q.out_co = 0; q.out_f32 = 1; }
-      else { q.out = out.p; q.out_cs = out.cs; q.out_co = out.co; q.out_f32 = 0; }
-      q.Cout = cw.cout;
-      q.Hout = stride == 2 ? in.H / 2 : in.H; q.Wout = stride == 2 ? in.W / 2 : in.W;
-      q.act = act;
-      if (res) { q.res = res->p; q.res_cs = res->cs; q.res_co = res->co; }
       op.kind = Op::DIRECT;
-      P.conv_flops += 2.0 * P.B * q.Hout * q.Wout * cw.cout * (cw.cin / cw.groups) * cw.k * cw.k;
+      op.direct = direct_conv_params(d, cw.groups);
+      P.conv_flops += 2.0 * P.B * op.direct.Hout * op.direct.Wout * cw.cout * (cw.cin / cw.groups) * cw.k * cw.k;
     }
     P.ops.push_back(std::move(op));
   }
   // conv key1 (in -> out1) followed by the 1x1 conv key2 over in2, a slice of out1's buffer that starts inside out1 and may
-  // run past its end (the partner: channels another conv wrote), into out2 (or the dense fp32 map out2_f32).  One chained
+  // run past its end (the partner: channels another conv wrote), into out2 (a tensor or a dense fp32 map).  One chained
   // launch (conv_gemm_chain_build) when the pair chains, and then out1 is written only when keep1; else the two convs.
   // Returns whether the pair was chained.
-  bool conv_pair(const std::string& key1, const T& in, const T& out1, int stride, const T* res, const std::string& key2, const T& in2,
-                 const T& out2, int act2, float* out2_f32, bool keep1) {
+  bool conv_pair(const std::string& key1, const TSlice& in, const TSlice& out1, int stride, const TSlice* res, const std::string& key2,
+                 const TSlice& in2, const TSlice& out2, int act2, bool keep1) {
     if (rc) return false;
     auto i1 = M.convs.find(key1), i2 = M.convs.find(key2);
     if (!bump.dry && !M.precise && i1 != M.convs.end() && i2 != M.convs.end()) {
       const ConvW& c1 = i1->second;
       const ConvW& c2 = i2->second;
       const int part_c = in2.co + in2.C - (out1.co + out1.C);
-      if (c1.groups == 1 && tc_ok(c1.cin, c1.cout) && c1.cin == in.C && c2.groups == 1 && c2.k == 1 && c2.cin == in2.C &&
-          c2.cout == c2.cin && in2.p == out1.p && in2.cs == out1.cs && in2.co >= out1.co && in2.co < out1.co + out1.C) {
-        ConvDesc d{};
-        d.in = in.p; d.in_cs = in.cs; d.in_co = in.co; d.Cin = in.C;
-        d.N = P.B; d.Hin = in.H; d.Win = in.W; d.k = c1.k; d.stride = stride;
-        d.w = c1.w; d.bias = c1.bias;
-        d.out = out1.p; d.out_cs = out1.cs; d.out_co = out1.co; d.Cout = c1.cout; d.out_f32 = 0; d.act = CC_ACT_SILU;
-        if (res) { d.res = res->p; d.res_cs = res->cs; d.res_co = res->co; }
+      if (c1.groups == 1 && tc_ok(c1.cin, c1.cout) && c1.cin == in.C && c1.cout == out1.C && c2.groups == 1 && c2.k == 1 &&
+          c2.cin == in2.C && c2.cout == c2.cin && c2.cout == out2.C && in2.p == out1.p && in2.cs == out1.cs && in2.co >= out1.co &&
+          in2.co < out1.co + out1.C) {
+        const ConvDesc d = conv_desc(in, c1.w, c1.bias, c1.k, stride, out1, CC_ACT_SILU, res);
         ChainDesc c{};
-        c.w = c2.w; c.bias = c2.bias; c.Cout = c2.cout; c.act = act2; c.k0 = in2.co - out1.co;
-        if (part_c > 0) { c.part = in2.p; c.part_cs = in2.cs; c.part_co = out1.co + out1.C; c.part_C = part_c; }
-        if (out2_f32) { c.out = out2_f32; c.out_cs = c2.cout; c.out_co = 0; c.out_f32 = 1; }
-        else { c.out = out2.p; c.out_cs = out2.cs; c.out_co = out2.co; c.out_f32 = 0; }
+        c.w = c2.w; c.bias = c2.bias; c.act = act2; c.k0 = in2.co - out1.co;
+        if (part_c > 0) c.part = nhwc_slice(in2.p, in2.cs, out1.co + out1.C, part_c);
+        c.out = out2;
         c.store1 = keep1;
         Op op;
         op.kind = Op::GEMM;
@@ -580,12 +549,12 @@ struct Builder {
       }
     }
     conv(key1, in, out1, stride, CC_ACT_SILU, res);   // the pair does not chain here (shape, tile width, smem, fp32 mode)
-    conv(key2, in2, out2, 1, act2, nullptr, out2_f32);
+    conv(key2, in2, out2, 1, act2);
     return false;
   }
   void simple(Op::Kind kind, const T& in, const T& out, const char* name) {
     if (rc || bump.dry) return;
-    Op op; op.kind = kind; op.s_in = ts(in); op.s_out = ts(out); op.name = name;
+    Op op; op.kind = kind; op.s_in = in; op.s_out = out; op.name = name;
     P.ops.push_back(std::move(op));
   }
 
@@ -611,7 +580,7 @@ struct Builder {
       T t2 = talloc(b, x.H, x.W);
       conv(pfx + ".m." + std::to_string(i) + ".cv1", x1, t2, 1, CC_ACT_SILU);
       if (i + 1 < n) conv(pfx + ".m." + std::to_string(i) + ".cv2", t2, x1, 1, CC_ACT_SILU, &x1);   // x + cv2(cv1(x)), in place
-      else conv_pair(pfx + ".m." + std::to_string(i) + ".cv2", t2, x1, 1, &x1, pfx + ".cv3", t1, o, CC_ACT_SILU, nullptr, false);
+      else conv_pair(pfx + ".m." + std::to_string(i) + ".cv2", t2, x1, 1, &x1, pfx + ".cv3", t1, o, CC_ACT_SILU, false);
     }
     return o;
   }
@@ -743,7 +712,7 @@ int Builder::build() {
             if (stem_tc_env == 1 && (cw.cout == 16 || cw.cout == 32 || cw.cout == 64)) {
               if (bump.dry) break;
               Op op; op.kind = Op::STEM_TC; op.name = pfx; op.stem = StemParams{}; op.stem.in = net_in;
-              rc = stem_tc_build(P.B, P.H, P.W, cw.wtc, cw.bias, cw.cout, ts(out), &op.stem_tc);
+              rc = stem_tc_build(P.B, P.H, P.W, cw.wtc, cw.bias, cw.cout, out, &op.stem_tc);
               if (rc) break;
               op.flops = 2.0 * Mrows * cw.cout * 27;
               P.conv_flops += op.flops;
@@ -755,13 +724,9 @@ int Builder::build() {
             { Op op; op.kind = Op::STEM_IM2COL; op.name = pfx + ".im2col"; op.stem = StemParams{};
               op.stem.in = net_in; op.stem.B = P.B; op.stem.H = P.H; op.stem.W = P.W;
               op.s_out.p = cols; P.ops.push_back(std::move(op)); }
-            ConvDesc d{};
-            d.in = cols; d.in_cs = 32; d.in_co = 0; d.Cin = 32;
-            d.N = 1; d.Hin = 1; d.Win = static_cast<int>(Mrows); d.k = 1; d.stride = 1;
-            d.w = cw.wtc; d.bias = cw.bias;
-            d.out = out.p; d.out_cs = out.cs; d.out_co = out.co; d.Cout = cw.cout; d.out_f32 = 0; d.act = CC_ACT_SILU;
             Op op; op.kind = Op::GEMM; op.name = pfx;
-            rc = conv_gemm_build(d, M.sms, &op.gemm);
+            rc = conv_gemm_build(conv_desc(nhwc_slice(cols, 32, 0, 32, 0, 1, 1, static_cast<int>(Mrows)), cw.wtc, cw.bias, 1, 1, out, CC_ACT_SILU),
+                                 M.sms, &op.gemm);
             if (rc) break;
             op.gemm.flops = 2.0 * Mrows * cw.cout * 27;
             P.conv_flops += op.gemm.flops;
@@ -772,11 +737,11 @@ int Builder::build() {
           Op op; op.kind = Op::STEM; op.name = pfx;
           op.stem = StemParams{};
           op.stem.in = net_in; op.stem.is_f32 = f32; op.stem.B = P.B; op.stem.H = P.H; op.stem.W = P.W;
-          op.stem.w = cw.wf32; op.stem.bias = cw.bias; op.stem.Cout = cw.cout; op.stem.out = ts(out);
+          op.stem.w = cw.wf32; op.stem.bias = cw.bias; op.stem.Cout = cw.cout; op.stem.out = out;
           P.conv_flops += 2.0 * P.B * (P.H / 2) * (P.W / 2) * cw.cout * 27;
           P.ops.push_back(std::move(op));
         } else {
-          out = out_for(i, l.b, l.s == 2 ? in.H / 2 : in.H, l.s == 2 ? in.W / 2 : in.W);
+          out = out_for(i, l.b, conv_out(in.H, l.s), conv_out(in.W, l.s));
           if (!place.count(i) && conv_feeds_only_elan(S, outC, i, M.precise)) deferred = {pfx, in, out, l.s, i};
           else conv(pfx, in, out, l.s, CC_ACT_SILU);
         }
@@ -802,9 +767,8 @@ int Builder::build() {
           const T& lo = outs[i - 3];                       // the Upsample layer's source
           const T& hi = src(S[i - 1].f[1]);                // the Concat's second source
           float* part = static_cast<float*>(dalloc(static_cast<size_t>(P.B) * lo.H * lo.W * 4 * b * 4));
-          T dummy;
-          conv(pfx + ".cv1.lo", lo, dummy, 1, CC_ACT_NONE, nullptr, part);
-          conv(pfx + ".cv1.hi", hi, slice(cat, 0, 4 * b), 1, CC_ACT_SILU, nullptr, nullptr, part, lo.H, lo.W);
+          conv(pfx + ".cv1.lo", lo, dense_f32(part, 4 * b), 1, CC_ACT_NONE);
+          conv(pfx + ".cv1.hi", hi, slice(cat, 0, 4 * b), 1, CC_ACT_SILU, nullptr, part, lo.H, lo.W);
           if (!rc && !bump.dry && P.ops.size() >= 2) {
             // algorithmic FLOPs: the pair replaces ONE 1x1 conv over all input channels at full resolution (what the reference
             // computes and SURVEY 8(d) counts); booked on the full-resolution launch, the half-resolution one carries none
@@ -818,19 +782,19 @@ int Builder::build() {
           conv(pfx + ".cv2.0.cv1+cv2", slice(cat, 2 * b, 2 * b), t1, 1, CC_ACT_SILU);
         } else if (deferred.layer == i - 1) {   // the previous Conv with cv1 chained in its epilogue; its output is not stored
           if (conv_pair(deferred.key, deferred.in, deferred.out, deferred.stride, nullptr, pfx + ".cv1", in, slice(cat, 0, 4 * b),
-                        CC_ACT_SILU, nullptr, false))
+                        CC_ACT_SILU, false))
             folded.push_back(i - 1);
           deferred.layer = -1;
           conv(pfx + ".cv2.0.cv1+cv2", slice(cat, 2 * b, 2 * b), t1, 1, CC_ACT_SILU);
         } else {   // cv1 -> cat[0, 4b) (kept: cv4 reads it) chained with cv2.0's cv1+cv2 on y1 = cat[2b, 4b)
           conv_pair(pfx + ".cv1", in, slice(cat, 0, 4 * b), 1, nullptr, pfx + ".cv2.0.cv1+cv2", slice(cat, 2 * b, 2 * b), t1, CC_ACT_SILU,
-                    nullptr, true);
+                    true);
         }
         T r1 = repncsp(pfx + ".cv2.0", slice(cat, 2 * b, 2 * b), b, l.n, &t1);
         // cv2.1 -> y2 = cat[4b, 6b) (kept) chained with cv3.0's cv1+cv2 on y2
         T t1b = talloc(2 * b, in.H, in.W);
         conv_pair(pfx + ".cv2.1", r1, slice(cat, 4 * b, 2 * b), 1, nullptr, pfx + ".cv3.0.cv1+cv2", slice(cat, 4 * b, 2 * b), t1b,
-                  CC_ACT_SILU, nullptr, true);
+                  CC_ACT_SILU, true);
         T r2 = repncsp(pfx + ".cv3.0", slice(cat, 4 * b, 2 * b), b, l.n, &t1b);
         conv(pfx + ".cv3.1", r2, slice(cat, 6 * b, 2 * b), 1, CC_ACT_SILU);
         out = out_for(i, l.c, in.H, in.W);
@@ -864,8 +828,8 @@ int Builder::build() {
         T cat = talloc(4 * c1, in.H, in.W);
         conv(pfx + ".cv1", in, slice(cat, 0, c1), 1, CC_ACT_SILU);
         static const int spp3_env = getenv("CC_SPP3") ? atoi(getenv("CC_SPP3")) : 1;
-        if (spp3_env && spp3_supported(ts(cat), c1)) {
-          if (!rc && !bump.dry) { Op op; op.kind = Op::SPP3; op.s_in = ts(cat); op.s_out = ts(cat); op.s_out.C = c1; op.name = "spp.max5x3"; P.ops.push_back(std::move(op)); }
+        if (spp3_env && spp3_supported(cat, c1)) {
+          if (!rc && !bump.dry) { Op op; op.kind = Op::SPP3; op.s_in = cat; op.s_out = cat; op.s_out.C = c1; op.name = "spp.max5x3"; P.ops.push_back(std::move(op)); }
         } else {
           for (int q = 0; q < 3; ++q) simple(Op::MAXPOOL5, slice(cat, q * c1, c1), slice(cat, (q + 1) * c1, c1), "spp.max5");
         }
@@ -913,9 +877,9 @@ int Builder::build() {
         for (int q = 0; q < op.cbf.nsrc; ++q) {
           const T& ch = cbl_chunks[l.f[q]][l.list[q]];
           CC_REQUIRE(ch.C == last.C, "yolo: CBFuse chunk has %d channels, target %d", ch.C, last.C);
-          op.cbf.src[q] = ts(ch);
+          op.cbf.src[q] = ch;
         }
-        op.cbf.last = ts(last); op.cbf.out = ts(out);
+        op.cbf.last = last; op.cbf.out = out;
         P.ops.push_back(std::move(op));
         break;
       }
@@ -939,11 +903,10 @@ int Builder::build() {
           T tb = talloc(64, x.H, x.W), tc = talloc(d, x.H, x.W);
           float* bl = static_cast<float*>(dalloc(static_cast<size_t>(P.B) * x.H * x.W * 64 * 4));
           float* cl = static_cast<float*>(dalloc(static_cast<size_t>(P.B) * x.H * x.W * 80 * 4));
-          T dummy;
           // box branch: cv2.j.1 chained with its 1x1 logits cv2.j.2 (tb is then never stored)
-          conv_pair(hp + ".cv2." + sq + ".1", slice(t0, 0, 64), tb, 1, nullptr, hp + ".cv2." + sq + ".2", tb, dummy, CC_ACT_NONE, bl, false);
+          conv_pair(hp + ".cv2." + sq + ".1", slice(t0, 0, 64), tb, 1, nullptr, hp + ".cv2." + sq + ".2", tb, dense_f32(bl, 64), CC_ACT_NONE, false);
           conv(hp + ".cv3." + sq + ".1", slice(t0, 64, d), tc, 1, CC_ACT_SILU);
-          conv(hp + ".cv3." + sq + ".2", tc, dummy, 1, CC_ACT_NONE, nullptr, cl);
+          conv(hp + ".cv3." + sq + ".2", tc, dense_f32(cl, 80), 1, CC_ACT_NONE);
           dec.dec.box[q] = bl; dec.dec.cls[q] = cl; dec.dec.h[q] = x.H; dec.dec.w[q] = x.W;
           dec.dec.stride[q] = float(P.H / x.H);
           A += x.H * x.W;
@@ -1557,9 +1520,7 @@ int cc_stem(const void* d_frames, int frame_f32, int B, int H, int W, const floa
   float* dwf = reinterpret_cast<float*>(ws);
   __nv_bfloat16* dwt = reinterpret_cast<__nv_bfloat16*>(ws + al256(wf.size() * 4));
   float* db = reinterpret_cast<float*>(ws + al256(wf.size() * 4) + al256(wt.size() * 2));
-  TSlice out{};
-  out.p = static_cast<__nv_bfloat16*>(d_out); out.cs = out_cs; out.co = out_co; out.C = Cout; out.N = B; out.H = H / 2; out.W = W / 2;
-  out.f32 = out_f32;
+  const TSlice out = nhwc_slice(d_out, out_cs, out_co, Cout, out_f32, B, H / 2, W / 2);
   StemTcParams tc{};
   if (impl == 1)
     if (int rc = stem_tc_build(B, H, W, dwt, db, Cout, out, &tc)) return rc;
@@ -1586,7 +1547,7 @@ int cc_conv2d_fp32_accurate(const float* d_in, int N, int Hin, int Win, int in_c
   CC_REQUIRE(in_co >= 0 && in_co % 4 == 0 && in_cs % 4 == 0 && in_co + Cin <= in_cs && out_co >= 0 && out_co % 4 == 0 &&
                  out_cs % 4 == 0 && out_co + Cout <= out_cs && (!d_res || (res_co >= 0 && res_co % 4 == 0 && res_cs % 4 == 0 && res_co + Cout <= res_cs)),
              "cc_conv2d_fp32_accurate: bad slice (cs, co multiples of 4 channels, the slice inside the row)");
-  const int Ho = stride == 2 ? Hin / 2 : Hin, Wo = stride == 2 ? Win / 2 : Win;
+  const int Ho = conv_out(Hin, stride), Wo = conv_out(Win, stride);
   std::vector<int> seg_off, seg_c;
   hi_segments(Cin, k, &seg_off, &seg_c);
   const size_t rows = static_cast<size_t>(Cout) * k * k;
@@ -1618,12 +1579,11 @@ int cc_conv2d_fp32_accurate(const float* d_in, int N, int Hin, int Win, int in_c
   cw.w5 = reinterpret_cast<__nv_bfloat16*>(ws);                  ws += w5_b;
   cw.bias = h_bias ? reinterpret_cast<float*>(ws) : nullptr;     ws += bias_b;
   for (size_t i = 0; i < seg_c.size(); ++i) { cw.whi.push_back(reinterpret_cast<__nv_bfloat16*>(ws)); ws += al256(rows * seg_c[i] * 2); }
-  TSlice in{};
-  in.p = reinterpret_cast<__nv_bfloat16*>(const_cast<float*>(d_in)); in.cs = in_cs; in.co = in_co; in.C = Cin;
-  in.N = N; in.H = Hin; in.W = Win; in.f32 = 1;
+  const TSlice in = nhwc_slice(d_in, in_cs, in_co, Cin, 1, N, Hin, Win), res = nhwc_slice(d_res, res_cs, res_co, Cout, 1);
   YoloPlan run;
   double flops = 0;
-  if (int rc = precise_conv_ops("conv", cw, in, stride, act, planes, acc, d_out, out_cs, out_co, d_res, res_cs, res_co, sms, &run.ops, &flops))
+  if (int rc = precise_conv_ops("conv", cw, in, stride, act, planes, acc, nhwc_slice(d_out, out_cs, out_co, Cout, 1), d_res ? &res : nullptr, sms,
+                                &run.ops, &flops))
     return rc;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   CC_CHECK_CUDA(cudaMemcpyAsync(cw.w5, w5.data(), w5.size() * 2, cudaMemcpyHostToDevice, st));

@@ -40,10 +40,8 @@ int main() {
   int bad = 0;
   printf("%-34s %4s %3s %2s %4s %7s %6s %6s\n", "shape", "BN", "BK", "S", "bres", "smem", "tiles", "grid");
   for (const S& q : shapes) {
-    ConvDesc d{};
-    d.in = dummy; d.in_cs = q.Cin; d.in_co = 0; d.Cin = q.Cin; d.N = q.N; d.Hin = q.H; d.Win = q.W; d.k = q.k; d.stride = q.s;
-    d.w = dummy; d.bias = dummy; d.out = dummy; d.out_cs = q.Cout; d.out_co = 0; d.Cout = q.Cout; d.out_f32 = q.f32; d.act = 1;
-    if (q.res) { d.res = d.out; d.res_cs = d.out_cs; d.res_co = 0; }
+    const TSlice out = nhwc_slice(dummy, q.Cout, 0, q.Cout, q.f32);
+    const ConvDesc d = conv_desc(nhwc_slice(dummy, q.Cin, 0, q.Cin, 0, q.N, q.H, q.W), dummy, dummy, q.k, q.s, out, 1, q.res ? &out : nullptr);
     GemmLaunch L;
     char name[96];
     snprintf(name, sizeof(name), "%dx%dx%d %d->%d k%d s%d %s%s", q.N, q.H, q.W, q.Cin, q.Cout, q.k, q.s, q.f32 ? "f32" : "bf16", q.res ? "+res" : "");
