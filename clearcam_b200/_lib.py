@@ -31,6 +31,25 @@ class cc_track_job(ctypes.Structure):
                 ("reserved", ctypes.c_int)]
 
 
+class cc_slice(ctypes.Structure):
+    """An NHWC slice as cc_yolo_op_conv reports it: device pointer, channels per pixel, first channel, channels, N, H, W, fp32."""
+    _fields_ = [("p", ctypes.c_void_p)] + [(n, ctypes.c_int) for n in ("cs", "co", "C", "N", "H", "W", "f32")]
+
+
+class cc_conv_op(ctypes.Structure):
+    """One op of a detector plan as cc_yolo_op_conv describes it (include/clearcam_b200.h); `in_` is the header's `in`."""
+    _fields_ = ([("kind", ctypes.c_int), ("name", ctypes.c_char * 128), ("in_", cc_slice), ("out", cc_slice), ("res", cc_slice),
+                 ("w", ctypes.c_void_p), ("bias", ctypes.c_void_p)]
+                + [(n, ctypes.c_int) for n in ("k", "stride", "groups", "act")]
+                + [("pre", ctypes.c_void_p), ("pre_h", ctypes.c_int), ("pre_w", ctypes.c_int), ("w2", ctypes.c_void_p),
+                   ("bias2", ctypes.c_void_p), ("act2", ctypes.c_int), ("k0", ctypes.c_int), ("part", cc_slice), ("out2", cc_slice),
+                   ("store1", ctypes.c_int)]
+                + [(n, ctypes.c_int) for n in ("BN", "BK", "lTW", "lTH", "lTN", "s2", "stages", "b_res", "grid", "num_tiles")])
+
+
+# cc_conv_op kinds (CC_CONV_OP_* in include/clearcam_b200.h)
+CC_CONV_OP_NONE, CC_CONV_OP_GEMM, CC_CONV_OP_CHAIN, CC_CONV_OP_DIRECT = 0, 1, 2, 3
+
 # cc_ocsort_gpu_update statuses (CC_TRACK_* in include/clearcam_b200.h)
 CC_TRACK_OK, CC_TRACK_NEEDS_ROOM, CC_TRACK_BAD_CLASS, CC_TRACK_OVERFLOW = 0, 1, 2, 3
 # cc_ocsort_gpu_events statuses (CC_EVENT_* in include/clearcam_b200.h)
@@ -65,6 +84,8 @@ _SIGS = {
                              ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_i), _vp]),
     "cc_yolo_trace": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _i, ctypes.POINTER(ctypes.c_ulonglong), ctypes.POINTER(ctypes.c_char_p),
                            ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_double), ctypes.POINTER(_i), _vp]),
+    "cc_yolo_op_conv": (_i, [_vp, _i, _i, _i, _i, _i, _i, ctypes.POINTER(cc_conv_op)]),
+    "cc_yolo_run_ops": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "cc_yolo_layer_output": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i),
                                   ctypes.POINTER(_i), _vp]),
     "cc_detect_postprocess": (_i, [_vp, _i, _i, _i, _f, _i, _f, _f, _f, _f, _f, _vp, _vp]),

@@ -258,6 +258,8 @@ struct T : TSlice { bool image = false; T() : TSlice{} {} };
 struct Op {
   enum Kind { GEMM, DIRECT, AVGPAD, AVGMAX, MAXPOOL5, UPSAMPLE, CBFUSE, LETTERBOX, STEM, STEM_IM2COL, STEM_TC, DECODE, POST, SPLIT, FINISH, SPP3 } kind;
   GemmLaunch gemm;
+  ConvDesc conv{};           // GEMM: the conv its launch was built from (cc_yolo_op_conv reports it; the launch never reads it)
+  ChainDesc chain{};         //   ... and the 1x1 chained in its epilogue (chain.out.p != nullptr)
   DirectConvParams direct;
   TSlice s_in, s_out;
   CBFuseParams cbf;
@@ -415,6 +417,7 @@ static int precise_conv_ops(const std::string& key, const ConvW& cw, const TSlic
                                    : nhwc_slice(scratch, 6 * in.C, 0, 5 * in.C, 0, in.N, in.H, in.W);
     const ConvDesc d = conv_desc(planes, g < nseg ? cw.whi[g] : cw.w5, nullptr, cw.k, stride, acc, CC_ACT_NONE, g > 0 ? &acc : nullptr);
     Op gop; gop.kind = Op::GEMM; gop.name = key + (g < nseg ? ".hi" + std::to_string(g) : ".cross");
+    gop.conv = d;
     if (int rc = conv_gemm_build(d, sms, &gop.gemm)) return rc;
     gop.gemm.flops = g == 0 ? 2.0 * in.N * Ho * Wo * double(cw.cout) * cw.k * cw.k * cw.cin : 0.0;   // algorithmic FLOPs once
     *conv_flops += gop.gemm.flops;
@@ -507,6 +510,7 @@ struct Builder {
     op.name = key;
     if (cw.groups == 1 && tc_ok(cw.cin, cw.cout)) {
       op.kind = Op::GEMM;
+      op.conv = d;
       rc = conv_gemm_build(d, M.sms, &op.gemm);
       if (rc) return;
       P.conv_flops += op.gemm.flops;
@@ -541,6 +545,8 @@ struct Builder {
         Op op;
         op.kind = Op::GEMM;
         op.name = key1 + "+" + key2;
+        op.conv = d;
+        op.chain = c;
         if (conv_gemm_chain_build(d, c, M.sms, &op.gemm) == CC_OK) {
           P.conv_flops += op.gemm.flops;
           P.ops.push_back(std::move(op));
@@ -725,8 +731,8 @@ int Builder::build() {
               op.stem.in = net_in; op.stem.B = P.B; op.stem.H = P.H; op.stem.W = P.W;
               op.s_out.p = cols; P.ops.push_back(std::move(op)); }
             Op op; op.kind = Op::GEMM; op.name = pfx;
-            rc = conv_gemm_build(conv_desc(nhwc_slice(cols, 32, 0, 32, 0, 1, 1, static_cast<int>(Mrows)), cw.wtc, cw.bias, 1, 1, out, CC_ACT_SILU),
-                                 M.sms, &op.gemm);
+            op.conv = conv_desc(nhwc_slice(cols, 32, 0, 32, 0, 1, 1, static_cast<int>(Mrows)), cw.wtc, cw.bias, 1, 1, out, CC_ACT_SILU);
+            rc = conv_gemm_build(op.conv, M.sms, &op.gemm);
             if (rc) break;
             op.gemm.flops = 2.0 * Mrows * cw.cout * 27;
             P.conv_flops += op.gemm.flops;
@@ -1408,6 +1414,67 @@ int cc_yolo_trace(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf
   cudaFree(d_trace);
   if (n_ops) *n_ops = static_cast<int>(n);
   return rc;
+}
+
+// conv op taps: what each conv launch of the cached plan computes, and the plan run one range of ops at a time
+static cc_slice op_slice(const TSlice& t, int N, int H, int W) {
+  cc_slice s{};
+  s.p = t.p; s.cs = t.cs; s.co = t.co; s.C = t.C; s.N = N; s.H = H; s.W = W; s.f32 = t.f32;
+  return s;
+}
+
+int cc_yolo_op_conv(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int i, cc_conv_op* out) {
+  CC_REQUIRE(h, "cc_yolo_op_conv: null handle");
+  if (int rc = check_frame_fmt("cc_yolo_op_conv", frame_fmt, Hf, Wf)) return rc;
+  YoloPlan* P = nullptr;
+  if (int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P)) return rc;
+  const int n = static_cast<int>(P->ops.size());
+  if (!out) return n;
+  CC_REQUIRE(i >= 0 && i < n, "cc_yolo_op_conv: op %d of a plan of %d ops", i, n);
+  const Op& op = P->ops[i];
+  cc_conv_op& o = *out;
+  o = cc_conv_op{};
+  snprintf(o.name, sizeof(o.name), "%s", op.name.c_str());
+  if (op.kind == Op::DIRECT) {
+    const DirectConvParams& p = op.direct;
+    o.kind = CC_CONV_OP_DIRECT;
+    o.in = op_slice(nhwc_slice(p.in, p.in_cs, p.in_co, p.Cin), p.N, p.Hin, p.Win);
+    o.out = op_slice(nhwc_slice(p.out, p.out_cs, p.out_co, p.Cout, p.out_f32), p.N, p.Hout, p.Wout);
+    if (p.res) o.res = op_slice(nhwc_slice(p.res, p.res_cs, p.res_co, p.Cout, p.out_f32), p.N, p.Hout, p.Wout);
+    o.w = p.w; o.bias = p.bias; o.k = p.k; o.stride = p.stride; o.groups = p.groups; o.act = p.act;
+    return n;
+  }
+  if (op.kind != Op::GEMM) return n;
+  const ConvDesc& d = op.conv;
+  const GemmParams& g = op.gemm.p;
+  const int N = d.in.N, Ho = conv_out(d.in.H, d.stride), Wo = conv_out(d.in.W, d.stride);
+  o.kind = op.chain.out.p ? CC_CONV_OP_CHAIN : CC_CONV_OP_GEMM;
+  o.in = op_slice(d.in, N, d.in.H, d.in.W);
+  o.out = op_slice(d.out, N, Ho, Wo);
+  if (d.res.p) o.res = op_slice(d.res, N, Ho, Wo);
+  o.w = d.w; o.bias = d.bias; o.k = d.k; o.stride = d.stride; o.groups = 1; o.act = d.act;
+  o.pre = d.pre; o.pre_h = d.pre_h; o.pre_w = d.pre_w;
+  if (op.chain.out.p) {
+    const ChainDesc& c = op.chain;
+    o.w2 = c.w; o.bias2 = c.bias; o.act2 = c.act; o.k0 = c.k0;
+    if (c.part.p) o.part = op_slice(c.part, N, Ho, Wo);
+    o.out2 = op_slice(c.out, N, Ho, Wo);
+    o.store1 = c.store1 ? 1 : 0;
+  }
+  o.BN = g.BN; o.BK = g.BK; o.lTW = g.lTW; o.lTH = g.lTH; o.lTN = g.lTN; o.s2 = g.s2; o.stages = g.stages; o.b_res = g.b_res;
+  o.grid = op.gemm.grid; o.num_tiles = g.num_tiles;
+  return n;
+}
+
+int cc_yolo_run_ops(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, int first, int last,
+                    float* d_out, float* d_raw, void* stream) {
+  CC_REQUIRE(h && d_frames && d_out, "cc_yolo_run_ops: bad argument");
+  if (int rc = check_frame_fmt("cc_yolo_run_ops", frame_fmt, Hf, Wf)) return rc;
+  YoloPlan* P = nullptr;
+  if (int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P)) return rc;
+  const int n = static_cast<int>(P->ops.size());
+  CC_REQUIRE(0 <= first && first <= last && last <= n, "cc_yolo_run_ops: ops [%d, %d) of a plan of %d ops", first, last, n);
+  return plan_run(*P, d_frames, d_out, d_raw, static_cast<cudaStream_t>(stream), nullptr, nullptr, first, last);
 }
 
 // parity tap: copy the output of spec layer `layer` of the cached plan (after a forward) to dense fp32 NHWC

@@ -148,6 +148,37 @@ int cc_yolo_profile(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int 
 int cc_yolo_trace(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, float* d_out, int cap,
                   unsigned long long* host_ns, const char** kinds, const char** names, double* flops, int* n_ops, void* stream);
 
+/* Conv op taps, for tests that check every conv launch of a plan in place, one op at a time.
+ * cc_yolo_op_conv describes op i of the cached plan of this shape (built on first use, as cc_yolo_forward would) and returns
+ * the plan's op count; out == NULL only returns the count, an i outside [0, count) fails with CC_ERR_INVALID.  out->name is
+ * the op's name (the names cc_yolo_profile reports); out->kind is CC_CONV_OP_NONE for an op that is not a conv (the rest is
+ * then zero).  For a conv: the input, output and residual slices (res.p == NULL: none) with the extents the launch covers;
+ * bf16 weights w [Cout][k][k][Cin/groups], bias [Cout] or NULL, act; the half-resolution fp32 pre-activation addend pre
+ * ([N][pre_h][pre_w][Cout] dense, or NULL).  CC_CONV_OP_CHAIN: the square 1x1 run in the conv's epilogue, w2 [Cout2][Cout2],
+ * bias2, act2, over output channels [k0, k0 + Cout2 - part.C) followed by the partner slice `part`, into out2; store1 = 0:
+ * the first output is not written.  For the tensor-core launches, the tiling as built: N tile BN, K block BK, the 128-pixel
+ * tile box 2^lTW x 2^lTH x 2^lTN (w, h, images), the stride-2 pair view s2, the pipeline stages, resident weights b_res,
+ * the persistent grid and the tile count.
+ * cc_yolo_run_ops launches ops [first, last) of that plan on `stream` exactly as a forward launches them, without a CUDA
+ * graph; d_frames, d_out and d_raw are a cc_yolo_forward call's.  Nothing synchronises. */
+#define CC_CONV_OP_NONE 0
+#define CC_CONV_OP_GEMM 1
+#define CC_CONV_OP_CHAIN 2
+#define CC_CONV_OP_DIRECT 3
+typedef struct { void* p; int cs, co, C, N, H, W, f32; } cc_slice;   /* NHWC slice; f32: float elements, else bf16 */
+typedef struct {
+  int kind;
+  char name[128];
+  cc_slice in, out, res;
+  const void* w; const float* bias; int k, stride, groups, act;
+  const float* pre; int pre_h, pre_w;
+  const void* w2; const float* bias2; int act2, k0; cc_slice part, out2; int store1;
+  int BN, BK, lTW, lTH, lTN, s2, stages, b_res, grid, num_tiles;
+} cc_conv_op;
+int cc_yolo_op_conv(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int i, cc_conv_op* out);
+int cc_yolo_run_ops(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, int first, int last,
+                    float* d_out, float* d_raw, void* stream);
+
 /* parity tap: after a forward, copy the output of graph layer `layer` (index into the reference's self.model list,
  * detection/yolov9.py:303-371) to dense fp32 [B,H,W,C].  d_dst == NULL only queries C/H/W (C = 0: no tensor). */
 int cc_yolo_layer_output(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int layer, float* d_dst, int* C,

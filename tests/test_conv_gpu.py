@@ -47,14 +47,28 @@ GROUPED_CASES = [(2, 20, 20, 24, 24, 3, 1, 1, False, False, 24, 0, 24, 0, 0, 4),
 # QKV (W -> 3W, bf16 out) and mlp fc (W -> 4W, tanh-GELU); out-proj and fc2 are in test_conv_in_place_residual
 CLIP_ROWS = (300, 539, 771)
 CLIP_WIDTHS = (512, 768, 1024)
-CASES += [(1, 1, rows, W, m * W, 1, 1, act, False, False, W, 0, m * W, 0, 0)
-          for rows in CLIP_ROWS for W in CLIP_WIDTHS for m, act in ((3, 0), (4, 2))]
-CASES += GROUPED_CASES
+# ... and at the row counts of the benchmark's batches, at their own widths: ViT-B/32 images (256 x 50), ViT-L/14 images
+# (64 x 257) and 256 text queries (256 x 77) of both towers' text widths
+CLIP_BENCH = ((12800, 768), (16448, 1024), (19712, 512), (19712, 768))
+CLIP_SHAPES = [(rows, W) for rows in CLIP_ROWS for W in CLIP_WIDTHS] + list(CLIP_BENCH)
+
+
+def _clip_cases(shapes):
+    return [(1, 1, rows, W, m * W, 1, 1, act, False, False, W, 0, m * W, 0, 0) for rows, W in shapes for m, act in ((3, 0), (4, 2))]
+
+
+# the bench row counts go last, so that the earlier cases keep their positions
+CASES += _clip_cases(CLIP_SHAPES[:-len(CLIP_BENCH)]) + GROUPED_CASES + _clip_cases(CLIP_BENCH)
 
 # fp32 outputs against the float64 reference: |got - ref| <= F32_BAR * (sum_k |x_k w_k| + |bias| + |res|) per element,
 # the magnitude the fp32 accumulator and the epilogue's fp32 roundings carry.  Measured on an H100: at most 0.045 x 2^-16
 # on the CLIP shapes (K up to 4096) and 0.1 x 2^-16 on the K = 64 SiLU convs, so 2^-18 leaves 2.5x headroom.
+# The tensor core's fp32 accumulator truncates, so its error grows in proportion to the k16 steps into one accumulator:
+# the bar holds per F32_STEPS steps (K = 4096).  Every case here stays within that; a longer K takes
+# F32_BAR x steps / F32_STEPS (tests/test_plan_convs_gpu.py: the fp32-accurate mode's cross-product GEMMs, up to 1440 steps).
 F32_BAR = 2.0 ** -18
+F32_STEPS = 256
+F32_REL = 2e-3           # and |got - ref| / max(|ref|, 1): the tighter bar where the sum cancels heavily
 TANH_Z = 2.0 ** -12      # tanh.approx.f32 errs by <= 2^-11, so SiLU and tanh-GELU (z/2 (1 + tanh)) err by <= 2^-12 |z|
 RN_WINDOW = 0.02         # |mean (got - y) sign(y) / ulp_bf16(y)| of a round-to-nearest store over >= 10^4 outputs
 _WORST = {}
@@ -146,7 +160,7 @@ def _check_f32(got, x, w, b, k, s, act, res, what="", groups=1):
     print(f"{what}: fp32 worst |err|/bar {ratio:.3f}, max rel err {(err / ref.abs().clamp(min=1.0)).max().item():.2e}")
     assert torch.isfinite(got).all()
     assert ratio <= 1.0, f"worst |err|/(F32_BAR * sum|x.w|) {ratio:.3f} (abs {err.max().item()})"
-    assert (err / ref.abs().clamp(min=1.0)).max().item() < 2e-3
+    assert (err / ref.abs().clamp(min=1.0)).max().item() < F32_REL
 
 
 @pytest.mark.parametrize("impl", [1, 2])
@@ -185,7 +199,7 @@ def test_conv_matches_torch(case, impl):
 RESIDUAL_CASES = [pytest.param(3, 24, 40, 64, Cout, k, 1, f32, 0, 2 * Cout, id=f"{Cout}-{f32}-{k}")
                   for Cout, f32, k in [(32, False, 3), (64, False, 3), (128, False, 1), (16, True, 1), (64, True, 3), (96, False, 1)]]
 RESIDUAL_CASES += [pytest.param(1, 1, rows, m * W, W, 1, 0, True, 128, W, id=f"clip-{name}-{rows}x{W}")
-                   for m, name in ((1, "out_proj"), (4, "fc2")) for rows in CLIP_ROWS for W in CLIP_WIDTHS]
+                   for m, name in ((1, "out_proj"), (4, "fc2")) for rows, W in CLIP_SHAPES]
 
 
 def residual_inputs(N, H, W, Cin, Cout, k, out_f32, out_cs):
