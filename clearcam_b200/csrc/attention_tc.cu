@@ -13,7 +13,6 @@
 #include "cc_common.h"
 #include "cc_ptx.cuh"
 #include <math.h>
-#include <stdlib.h>
 
 namespace cc {
 
@@ -179,14 +178,8 @@ __global__ void __launch_bounds__(128) attention_tc_kernel(const __grid_constant
 
 // ---------------------------------------------------------------- host
 bool attention_tc_supported(int L) {
-  // CC_ATTN_TC: 0 = never (mma.sync kernel of vit.cu), 1 (default) = sequences longer than 128 tokens (ViT-L/14's 257),
-  // 2 = wherever it fits.  Read when a plan is built, so tests can force either path.
-  const char* e = getenv("CC_ATTN_TC");
-  const int mode = e ? atoi(e) : 1;
-  const int Lk = (L + 63) / 64 * 64;
-  if (mode == 0 || Lk > kMaxLk) return false;
-  if (mode == 1) return L > 128;
-  return true;
+  // sequences longer than 128 tokens (ViT-L/14's 257) that fit; shorter ones run the mma.sync kernel of vit.cu
+  return L > 128 && (L + 63) / 64 * 64 <= kMaxLk;
 }
 int attention_tc_max_len() { return kMaxLk; }
 size_t attention_tc_workspace_bytes(int B, int L, int H) {

@@ -19,7 +19,6 @@
 #include "cc_common.h"
 #include "cc_ptx.cuh"
 #include <math.h>
-#include <stdlib.h>
 #include <string.h>
 #include <type_traits>
 
@@ -47,22 +46,15 @@ __device__ __forceinline__ float tanh_approx(float x) {
   return t;
 }
 
-// Epilogue activations.  tanh.approx / ex2.approx / rcp.approx all run on the multi-function unit, so an activation that
-// needs two of them (ex2 + rcp) costs twice the MUFU time of the tanh form:
-//   ACT_SILU       : x*sigmoid(x) = h + h*tanh(h), h = x/2 : ONE MUFU (tanh.approx.f32, |abs err| <= 2^-11 on tanh, i.e.
-//                    <= |x| * 2.4e-4 on the result, below the bf16 rounding of the stored value for x > -2)
-//   ACT_SILU_EXACT : x / (1 + 2^(-x log2 e)) with ex2.approx + rcp.approx (two MUFU, ~1e-7 relative)
-//   ACT_GELU_TANH  : 0.5x(1+tanh(sqrt(2/pi)(x+0.044715x^3)))  (models/objects.py:125 gelu()), one MUFU
+// Epilogue activations, each ONE multi-function-unit op (tanh.approx.f32); x / (1 + exp(-x)) would take two (ex2 + rcp):
+//   ACT_SILU       : x*sigmoid(x) = h + h*tanh(h), h = x/2 (|abs err| <= 2^-11 on tanh, i.e. <= |x| * 2.4e-4 on the
+//                    result, below the bf16 rounding of the stored value for x > -2)
+//   ACT_GELU_TANH  : 0.5x(1+tanh(sqrt(2/pi)(x+0.044715x^3)))  (models/objects.py:125 gelu())
 template <int ACT>
 __device__ __forceinline__ float act_apply(float x) {
   if (ACT == ACT_SILU) {
     const float h = 0.5f * x;
     return fmaf(h, tanh_approx(h), h);
-  } else if (ACT == ACT_SILU_EXACT) {
-    float e, r;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(fminf(x * -1.4426950408889634f, 126.0f)));
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
-    return x * r;
   } else if (ACT == ACT_GELU_TANH) {
     const float u = 0.7978845608028654f * fmaf(0.044715f * x * x, x, x);
     const float h = 0.5f * x;
@@ -664,10 +656,6 @@ int conv_gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L) {
   return gemm_build(d, num_sms, L, true);
 }
 
-static bool silu_exact_env() {
-  static const int v = getenv("CC_SILU_EXACT") ? atoi(getenv("CC_SILU_EXACT")) : 0;
-  return v != 0;
-}
 static int chain_launch(const GemmLaunch& L, cudaStream_t stream, bool dry);
 
 // The 1x1 c chains onto the conv d when
@@ -680,7 +668,7 @@ static int chain_launch(const GemmLaunch& L, cudaStream_t stream, bool dry);
 int conv_gemm_chain_build(const ConvDesc& d, const ChainDesc& c, int num_sms, GemmLaunch* L) {
   const int N2 = c.out.C, part_C = c.part.p ? c.part.C : 0;
   CC_REQUIRE(c.w && c.out.p && (d.out.p || !c.store1), "conv_gemm chain: NULL weights or output");
-  CC_REQUIRE(d.act == ACT_SILU && !d.out.f32 && !silu_exact_env(), "conv_gemm chain: the first conv must be SiLU into bf16");
+  CC_REQUIRE(d.act == ACT_SILU && !d.out.f32, "conv_gemm chain: the first conv must be SiLU into bf16");
   CC_REQUIRE(!d.pre, "conv_gemm chain: the first conv takes no pre-activation addend");
   CC_REQUIRE(N2 >= 16 && N2 <= kMaxBN && N2 % 16 == 0, "conv_gemm chain: the 1x1 has %d channels (16..128)", N2);
   CC_REQUIRE((c.act == ACT_SILU && !c.out.f32) || (c.act == ACT_NONE && c.out.f32 && N2 <= 64),
@@ -795,15 +783,11 @@ static int chain_launch(const GemmLaunch& L, cudaStream_t stream, bool dry) {
 int conv_gemm_launch(const GemmLaunch& L, cudaStream_t stream) {
   if (L.p.ch_n2 > 0) return chain_launch(L, stream, false);
   const bool f32 = L.p.out_f32 != 0;
-  int act = L.p.act;
-  if (act == ACT_SILU && silu_exact_env()) act = ACT_SILU_EXACT;
-  switch (act) {
+  switch (L.p.act) {
     case ACT_NONE: return f32 ? launch_variant<ACT_NONE, true>(L, stream) : launch_variant<ACT_NONE, false>(L, stream);
     case ACT_SILU: return f32 ? launch_variant<ACT_SILU, true>(L, stream) : launch_variant<ACT_SILU, false>(L, stream);
     case ACT_GELU_TANH:
       return f32 ? launch_variant<ACT_GELU_TANH, true>(L, stream) : launch_variant<ACT_GELU_TANH, false>(L, stream);
-    case ACT_SILU_EXACT:
-      return f32 ? launch_variant<ACT_SILU_EXACT, true>(L, stream) : launch_variant<ACT_SILU_EXACT, false>(L, stream);
   }
   set_error("conv_gemm: unknown activation %d", L.p.act);
   return CC_ERR_INVALID;

@@ -16,7 +16,7 @@
 
 namespace cc {
 
-enum Act : int32_t { ACT_NONE = 0, ACT_SILU = 1, ACT_GELU_TANH = 2, ACT_SILU_EXACT = 3 };
+enum Act : int32_t { ACT_NONE = 0, ACT_SILU = 1, ACT_GELU_TANH = 2 };
 
 struct GemmParams {
   CUtensorMap tmA;  // 5-D view of the NHWC activation (see conv_gemm.cu)

@@ -128,12 +128,8 @@ struct StemParams {
   TSlice out;                                  // [B,H/2,W/2,Cout]
 };
 int stem_launch(const StemParams& p, cudaStream_t s);
-// uint8 stem on tensor cores: im2col of the 3x3/s2 taps into a bf16 [B*Ho*Wo, 32] matrix (raw pixel values 0..255 are
-// exact in bf16; taps in (r,s,RGB) order = frame channel 2-c; columns 27..31 zero), consumed by conv_gemm with weights
-// bf16(w/255).
-int stem_im2col_launch(const uint8_t* frames, __nv_bfloat16* out, int B, int H, int W, cudaStream_t s);
-// uint8 stem on tensor cores without the im2col round trip (stem_tc.cu): the A tile is gathered from the frame into shared
-// memory by the CTA itself.  Built once per plan (output tensor map), launched with the frame pointer of the call.
+// uint8 stem on tensor cores (stem_tc.cu): the A tile is gathered from the frame into shared memory by the CTA itself.
+// Built once per plan (output tensor map), launched with the frame pointer of the call.
 struct StemTcParams {
   CUtensorMap tmC;           // 2-D [Mrows][Cout] bf16 view of the output slice (row pitch = cs), box [128][Cout]
   const uint8_t* in;         // [B][H][W][3] BGR

@@ -644,50 +644,6 @@ __global__ void __launch_bounds__(128) stem_kernel(StemParams p) {
     }
   }
 }
-// one thread = one output pixel: 27 byte gathers -> 32 bf16 (64 B, four 16-B stores; consecutive threads -> consecutive rows)
-__global__ void __launch_bounds__(256) stem_im2col_kernel(const uint8_t* __restrict__ in, __nv_bfloat16* __restrict__ out, int B,
-                                                          int H, int W) {
-  const int Ho = H / 2, Wo = W / 2;
-  const long long total = static_cast<long long>(B) * Ho * Wo;
-  CC_GRID_STRIDE(idx, total) {
-    const int ox = static_cast<int>(idx % Wo);
-    const int oy = static_cast<int>((idx / Wo) % Ho);
-    const int n = static_cast<int>(idx / (static_cast<long long>(Wo) * Ho));
-    float v[32];
-#pragma unroll
-    for (int i = 27; i < 32; ++i) v[i] = 0.f;
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-      const int iy = 2 * oy + r - 1;
-#pragma unroll
-      for (int s = 0; s < 3; ++s) {
-        const int ix = 2 * ox + s - 1;
-        const bool ok = iy >= 0 && iy < H && ix >= 0 && ix < W;
-        const uint8_t* px = in + ((static_cast<long long>(n) * H + iy) * W + ix) * 3;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) v[(r * 3 + s) * 3 + c] = ok ? static_cast<float>(__ldg(px + 2 - c)) : 0.f;
-      }
-    }
-    uint4* dst = reinterpret_cast<uint4*>(out + idx * 32);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      uint32_t w[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        __nv_bfloat162 h = __floats2bfloat162_rn(v[8 * q + 2 * j], v[8 * q + 2 * j + 1]);
-        w[j] = *reinterpret_cast<uint32_t*>(&h);
-      }
-      dst[q] = make_uint4(w[0], w[1], w[2], w[3]);
-    }
-  }
-}
-int stem_im2col_launch(const uint8_t* frames, __nv_bfloat16* out, int B, int H, int W, cudaStream_t s) {
-  CC_REQUIRE(H % 2 == 0 && W % 2 == 0, "stem_im2col: odd frame");
-  const long long total = static_cast<long long>(B) * (H / 2) * (W / 2);
-  stem_im2col_kernel<<<grid_for(total, 256), 256, 0, s>>>(frames, out, B, H, W);
-  CC_CHECK_CUDA(cudaGetLastError());
-  return CC_OK;
-}
 
 int stem_launch(const StemParams& p, cudaStream_t s) {
   CC_REQUIRE(p.Cout % 8 == 0 && p.H % 2 == 0 && p.W % 2 == 0 && p.out.cs % 8 == 0 && p.out.co % 8 == 0, "stem: bad shape");

@@ -18,7 +18,6 @@
 #include "conv_gemm.cuh"
 #include "ops.cuh"
 #include <cmath>
-#include <cstdlib>
 #include <map>
 #include <memory>
 #include <string>
@@ -256,7 +255,7 @@ static int require_net(const LbGeom& g, int Hf, int Wf, int res) {
 struct T : TSlice { bool image = false; T() : TSlice{} {} };
 
 struct Op {
-  enum Kind { GEMM, DIRECT, AVGPAD, AVGMAX, MAXPOOL5, UPSAMPLE, CBFUSE, LETTERBOX, STEM, STEM_IM2COL, STEM_TC, DECODE, POST, SPLIT, FINISH, SPP3 } kind;
+  enum Kind { GEMM, DIRECT, AVGPAD, AVGMAX, MAXPOOL5, UPSAMPLE, CBFUSE, LETTERBOX, STEM, STEM_TC, DECODE, POST, SPLIT, FINISH, SPP3 } kind;
   GemmLaunch gemm;
   ConvDesc conv{};           // GEMM: the conv its launch was built from (cc_yolo_op_conv reports it; the launch never reads it)
   ChainDesc chain{};         //   ... and the 1x1 chained in its epilogue (chain.out.p != nullptr)
@@ -620,8 +619,7 @@ static int layer_out_channels(const Layer& l, const std::vector<int>& outC, int 
 // addressing (GemmParams::pre): the upsample kernel, the concat buffer and half of the conv's input traffic disappear
 // (detection/yolov9.py:285-292, :107-125; layers 10-12 and 13-15 of t/s/m/c, 30-32 and 33-35 of e).
 static bool fuse_up_concat(const std::vector<Layer>& S, const std::vector<int>& outC, int i, bool precise, int* c_up = nullptr) {
-  static const int env = getenv("CC_FUSE_UP") ? atoi(getenv("CC_FUSE_UP")) : 1;
-  if (!env || precise || i < 3) return false;
+  if (precise || i < 3) return false;
   const Layer& e = S[i];
   if (e.op != L_ELAN4 || e.f.size() != 1 || e.f[0] != -1) return false;
   const Layer& c = S[i - 1];
@@ -710,36 +708,18 @@ int Builder::build() {
           CC_REQUIRE(l.a == 3 && l.k == 3 && l.s == 2, "yolo: unexpected image conv");
           out = out_for(i, l.b, in.H / 2, in.W / 2);
           const ConvW& cw = M.convs[pfx];
-          static const int stem_tc_env = getenv("CC_STEM_TC") ? atoi(getenv("CC_STEM_TC")) : 1;
-          if (!f32 && stem_tc_env && cw.cout % 16 == 0 && !M.precise) {
-            // uint8 frames: raw pixel values are exact in bf16, weights bf16(w/255).  Default (CC_STEM_TC=1): stem_tc_kernel
-            // gathers the A tile from the frame itself; CC_STEM_TC=2: the earlier im2col to [B*Ho*Wo, 32] + conv_gemm
-            const long long Mrows = static_cast<long long>(P.B) * (P.H / 2) * (P.W / 2);
-            if (stem_tc_env == 1 && (cw.cout == 16 || cw.cout == 32 || cw.cout == 64)) {
-              if (bump.dry) break;
-              Op op; op.kind = Op::STEM_TC; op.name = pfx; op.stem = StemParams{}; op.stem.in = net_in;
-              rc = stem_tc_build(P.B, P.H, P.W, cw.wtc, cw.bias, cw.cout, out, &op.stem_tc);
-              if (rc) break;
-              op.flops = 2.0 * Mrows * cw.cout * 27;
-              P.conv_flops += op.flops;
-              P.ops.push_back(std::move(op));
-              break;
-            }
-            __nv_bfloat16* cols = static_cast<__nv_bfloat16*>(dalloc(static_cast<size_t>(Mrows) * 32 * 2));
-            if (bump.dry) break;
-            { Op op; op.kind = Op::STEM_IM2COL; op.name = pfx + ".im2col"; op.stem = StemParams{};
-              op.stem.in = net_in; op.stem.B = P.B; op.stem.H = P.H; op.stem.W = P.W;
-              op.s_out.p = cols; P.ops.push_back(std::move(op)); }
-            Op op; op.kind = Op::GEMM; op.name = pfx;
-            op.conv = conv_desc(nhwc_slice(cols, 32, 0, 32, 0, 1, 1, static_cast<int>(Mrows)), cw.wtc, cw.bias, 1, 1, out, CC_ACT_SILU);
-            rc = conv_gemm_build(op.conv, M.sms, &op.gemm);
+          if (bump.dry) break;
+          if (!f32 && !M.precise && (cw.cout == 16 || cw.cout == 32 || cw.cout == 64)) {
+            // uint8 frames: raw pixel values are exact in bf16, weights bf16(w/255); stem_tc_kernel gathers the A tile from
+            // the frame itself
+            Op op; op.kind = Op::STEM_TC; op.name = pfx; op.stem = StemParams{}; op.stem.in = net_in;
+            rc = stem_tc_build(P.B, P.H, P.W, cw.wtc, cw.bias, cw.cout, out, &op.stem_tc);
             if (rc) break;
-            op.gemm.flops = 2.0 * Mrows * cw.cout * 27;
-            P.conv_flops += op.gemm.flops;
+            op.flops = 2.0 * P.B * (P.H / 2) * (P.W / 2) * cw.cout * 27;
+            P.conv_flops += op.flops;
             P.ops.push_back(std::move(op));
             break;
           }
-          if (bump.dry) break;
           Op op; op.kind = Op::STEM; op.name = pfx;
           op.stem = StemParams{};
           op.stem.in = net_in; op.stem.is_f32 = f32; op.stem.B = P.B; op.stem.H = P.H; op.stem.W = P.W;
@@ -833,8 +813,7 @@ int Builder::build() {
         const int c1 = l.b;
         T cat = talloc(4 * c1, in.H, in.W);
         conv(pfx + ".cv1", in, slice(cat, 0, c1), 1, CC_ACT_SILU);
-        static const int spp3_env = getenv("CC_SPP3") ? atoi(getenv("CC_SPP3")) : 1;
-        if (spp3_env && spp3_supported(cat, c1)) {
+        if (spp3_supported(cat, c1)) {
           if (!rc && !bump.dry) { Op op; op.kind = Op::SPP3; op.s_in = cat; op.s_out = cat; op.s_out.C = c1; op.name = "spp.max5x3"; P.ops.push_back(std::move(op)); }
         } else {
           for (int q = 0; q < 3; ++q) simple(Op::MAXPOOL5, slice(cat, q * c1, c1), slice(cat, (q + 1) * c1, c1), "spp.max5");
@@ -963,10 +942,6 @@ static int plan_run(YoloPlan& P, const void* d_frames, float* d_out, float* d_ra
       case Op::CBFUSE: rc = cbfuse_launch(op.cbf, st); break;
       case Op::LETTERBOX: { LetterboxParams q = op.lb; q.in = d_frames; rc = letterbox_launch(q, st); break; }
       case Op::STEM: { StemParams q = op.stem; if (!q.in) q.in = d_frames; rc = stem_launch(q, st); break; }
-      case Op::STEM_IM2COL:
-        rc = stem_im2col_launch(static_cast<const uint8_t*>(op.stem.in ? op.stem.in : d_frames), op.s_out.p, op.stem.B, op.stem.H,
-                                op.stem.W, st);
-        break;
       case Op::STEM_TC:
         rc = stem_tc_launch(op.stem_tc, static_cast<const uint8_t*>(op.stem.in ? op.stem.in : d_frames), st);
         break;
@@ -1003,7 +978,7 @@ static const char* op_kind_name(Op::Kind k) {
   switch (k) {
     case Op::GEMM: return "conv_gemm"; case Op::DIRECT: return "conv_direct"; case Op::AVGPAD: return "avgpool2_pad";
     case Op::AVGMAX: return "avgmax_pool"; case Op::MAXPOOL5: return "maxpool5"; case Op::UPSAMPLE: return "upsample2";
-    case Op::CBFUSE: return "cbfuse"; case Op::LETTERBOX: return "letterbox"; case Op::STEM: return "stem"; case Op::STEM_IM2COL: return "stem_im2col"; case Op::STEM_TC: return "stem_tc";
+    case Op::CBFUSE: return "cbfuse"; case Op::LETTERBOX: return "letterbox"; case Op::STEM: return "stem"; case Op::STEM_TC: return "stem_tc";
     case Op::DECODE: return "decode"; case Op::POST: return "postprocess"; case Op::SPLIT: return "split_planes"; case Op::FINISH: return "finish_f32"; case Op::SPP3: return "spp3";
   }
   return "?";
@@ -1212,35 +1187,31 @@ int cc_yolo_set_workspace(cc_yolo* h, void* d_workspace, size_t bytes) {
 // pointers twice in a row, else launch by launch.
 static int run_graphed(cc_yolo* h, YoloPlan* P, const void* d_frames, float* d_out, float* d_raw, cudaStream_t st, size_t first = 0,
                        size_t last = SIZE_MAX) {
-  int rc = CC_OK;
-  static const int graph_env = getenv("CC_GRAPH") ? atoi(getenv("CC_GRAPH")) : 1;
-  if (graph_env) {
-    if (P->gexec && P->g_frames == d_frames && P->g_out == d_out && P->g_raw == d_raw) {
+  if (P->gexec && P->g_frames == d_frames && P->g_out == d_out && P->g_raw == d_raw) {
+    CC_CHECK_CUDA(cudaGraphLaunch(P->gexec, st));
+    return CC_OK;
+  }
+  const bool stable = P->ran && P->l_frames == d_frames && P->l_out == d_out && P->l_raw == d_raw;
+  P->l_frames = d_frames; P->l_out = d_out; P->l_raw = d_raw; P->ran = true;
+  if (stable) {
+    // second call in a row with these pointers: capture the launch list (on a private stream: nothing executes) and replay
+    if (!h->m.cap_stream) CC_CHECK_CUDA(cudaStreamCreateWithFlags(&h->m.cap_stream, cudaStreamNonBlocking));
+    if (P->gexec) { cudaGraphExecDestroy(P->gexec); P->gexec = nullptr; }
+    cudaGraph_t g = nullptr;
+    bool ok = cudaStreamBeginCapture(h->m.cap_stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
+    if (ok) {
+      const int rc = plan_run(*P, d_frames, d_out, d_raw, h->m.cap_stream, nullptr, nullptr, first, last);
+      ok = cudaStreamEndCapture(h->m.cap_stream, &g) == cudaSuccess && rc == CC_OK && g != nullptr;
+    }
+    if (ok) ok = cudaGraphInstantiate(&P->gexec, g, 0) == cudaSuccess;
+    if (g) cudaGraphDestroy(g);
+    if (ok) {
+      P->g_frames = d_frames; P->g_out = d_out; P->g_raw = d_raw;
       CC_CHECK_CUDA(cudaGraphLaunch(P->gexec, st));
       return CC_OK;
     }
-    const bool stable = P->ran && P->l_frames == d_frames && P->l_out == d_out && P->l_raw == d_raw;
-    P->l_frames = d_frames; P->l_out = d_out; P->l_raw = d_raw; P->ran = true;
-    if (stable) {
-      // second call in a row with these pointers: capture the launch list (on a private stream: nothing executes) and replay
-      if (!h->m.cap_stream) CC_CHECK_CUDA(cudaStreamCreateWithFlags(&h->m.cap_stream, cudaStreamNonBlocking));
-      if (P->gexec) { cudaGraphExecDestroy(P->gexec); P->gexec = nullptr; }
-      cudaGraph_t g = nullptr;
-      bool ok = cudaStreamBeginCapture(h->m.cap_stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
-      if (ok) {
-        rc = plan_run(*P, d_frames, d_out, d_raw, h->m.cap_stream, nullptr, nullptr, first, last);
-        ok = cudaStreamEndCapture(h->m.cap_stream, &g) == cudaSuccess && rc == CC_OK && g != nullptr;
-      }
-      if (ok) ok = cudaGraphInstantiate(&P->gexec, g, 0) == cudaSuccess;
-      if (g) cudaGraphDestroy(g);
-      if (ok) {
-        P->g_frames = d_frames; P->g_out = d_out; P->g_raw = d_raw;
-        CC_CHECK_CUDA(cudaGraphLaunch(P->gexec, st));
-        return CC_OK;
-      }
-      cudaGetLastError();            // capture is an optimisation: fall through to plain launches
-      P->gexec = nullptr;
-    }
+    cudaGetLastError();            // capture is an optimisation: fall through to plain launches
+    P->gexec = nullptr;
   }
   return plan_run(*P, d_frames, d_out, d_raw, st, nullptr, nullptr, first, last);
 }

@@ -16,14 +16,6 @@ PROMPTS = ["ferrari f40", "text here", "a photo of a cat", "person riding a bicy
            "delivery driver carrying a box", "dog"]
 
 
-@pytest.fixture(params=["0", "2"], ids=["attn-mma.sync", "attn-tcgen05"])
-def attn_mode(request, monkeypatch):
-    """Both attention kernels at every sequence length (CC_ATTN_TC is read when a plan is built; default 1 picks by shape).
-    The second id names the tensor-core attention variant, attention_tc.cu (warpgroup MMA on Hopper)."""
-    monkeypatch.setenv("CC_ATTN_TC", request.param)
-    return request.param
-
-
 def _check(got: torch.Tensor, want: torch.Tensor, pairwise: float = 5e-3):
     cos = (got * want).sum(-1) / (got.norm(dim=-1) * want.norm(dim=-1))
     assert cos.min() >= 0.999, f"cosine {cos.min()}"
@@ -36,7 +28,7 @@ def _check(got: torch.Tensor, want: torch.Tensor, pairwise: float = 5e-3):
 
 
 @pytest.mark.parametrize("arch,B", [("ViT-tiny", 5), ("ViT-B/32", 6), ("ViT-B/32", 1), ("ViT-L/14", 3)])
-def test_image_encoder(arch, B, attn_mode):
+def test_image_encoder(arch, B):
     cfg = oc.CONFIGS[arch]
     P = oc.synthetic_weights(cfg, seed=3)
     x = oc.synthetic_images(B, cfg.image_size, seed=5)
@@ -49,7 +41,7 @@ def test_image_encoder(arch, B, attn_mode):
 
 
 @pytest.mark.parametrize("arch", ["ViT-tiny", "ViT-B/32", "ViT-L/14"])
-def test_text_encoder(arch, attn_mode):
+def test_text_encoder(arch):
     cfg = oc.CONFIGS[arch]
     P = oc.synthetic_weights(cfg, seed=4)
     m = OpenCLIP(weights=P, arch=arch)
@@ -63,7 +55,7 @@ def test_text_encoder(arch, attn_mode):
 
 
 @pytest.mark.parametrize("arch", ["ViT-tiny", "ViT-B/32"])
-def test_text_encoder_at_every_eot_position(arch, attn_mode):
+def test_text_encoder_at_every_eot_position(arch):
     """One row per EOT position 1..76; the last row is a full 77-token prompt with no padding.  Token ids 1000-40000 keep
     the EOT (49407) the row's argmax.  Covers text_embed_kernel's EOT argmax, the ln_final row gather and the causal
     attention rows past 64 (the second 64-row query block) end to end."""

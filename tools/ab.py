@@ -1,8 +1,9 @@
-"""Same-box A/B of environment toggles (boxes differ by +-5 %, so variants must be compared inside ONE gpurun call).
+"""Same-box A/B of library builds (machines differ by +-5 %, so builds must be compared on ONE machine, in one run).
 
-usage:  python tools/ab.py [--conv 6 2 0] [--bench] [--batch 32] [--steps 100] -- "CC_X=0" "CC_X=1 CC_Y=2" ...
-Each variant (a space-separated list of VAR=value, or "base") runs tools/one_conv.py on the given shapes and/or
-bench.py --no-cpu in a fresh process; one table is printed at the end."""
+usage:  python tools/ab.py [--conv 6 2 0] [--bench] [--batch 32] [--steps 100] -- base "CC_LIB=/path/to/other/libclearcam_b200.so" ...
+Each variant ("base" = the in-tree build, or a space-separated list of VAR=value set for its process, normally CC_LIB
+selecting another build) runs tools/one_conv.py on the given shapes and/or bench.py --no-cpu in a fresh process; one
+table is printed at the end."""
 import json
 import os
 import subprocess
