@@ -55,6 +55,17 @@ CC_TRACK_OK, CC_TRACK_NEEDS_ROOM, CC_TRACK_BAD_CLASS, CC_TRACK_OVERFLOW = 0, 1, 
 # cc_ocsort_gpu_events statuses (CC_EVENT_* in include/clearcam_b200.h)
 CC_EVENT_OK, CC_EVENT_NEEDS_ROOM, CC_EVENT_BAD_BOX, CC_EVENT_NOT_RUN, CC_EVENT_BAD_ORDER = 0, 1, 2, 3, 4
 CC_EVENT_MAX_VERTICES = 256
+# cc_ocsort_gpu_alerts: limits, cc_alert flags and statuses (CC_ALERT_* in include/clearcam_b200.h)
+CC_ALERT_MAX_ALERTS, CC_ALERT_MAX_COUNT = 64, 1024
+CC_ALERT_ON, CC_ALERT_ZONE, CC_ALERT_DESC, CC_ALERT_SCHED = 1, 2, 4, 8
+CC_ALERT_OK, CC_ALERT_NOT_RUN = 0, 1
+
+
+class cc_alert(ctypes.Structure):
+    """One alert of cc_ocsort_gpu_alerts_configure: class mask, max, CC_ALERT_* flags, weekday bits (Monday = bit 0),
+    resolved window, schedule start / end (seconds of day), description threshold, last_det."""
+    _fields_ = [("classes", ctypes.c_uint32 * 3), ("max", ctypes.c_int), ("flags", ctypes.c_int), ("days", ctypes.c_int),
+                ("reserved", ctypes.c_int * 2)] + [(n, ctypes.c_double) for n in ("window", "start", "end", "threshold", "last_det")]
 
 _lib = None
 
@@ -119,6 +130,13 @@ _SIGS = {
     "cc_ocsort_gpu_events_configure": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _i, _vp]),
     "cc_ocsort_gpu_events_grow": (_i, [_vp, _i, _i, _vp]),
     "cc_ocsort_gpu_events": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    "cc_ocsort_gpu_events_set_non_zone_alert": (_i, [_vp, _i, _i, _vp]),
+    "cc_ocsort_gpu_alerts_configure": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _vp]),
+    "cc_ocsort_gpu_alerts_set_on": (_i, [_vp, _i, _i, _vp]),
+    "cc_ocsort_gpu_alerts_counts": (_i, [_vp, _i, _vp, _vp]),
+    "cc_ocsort_gpu_alerts_reset_counts": (_i, [_vp, _i, _vp]),
+    "cc_ocsort_gpu_alerts": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    "cc_ocsort_gpu_describe": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     "cc_letterbox": (_i, [_vp, _i, _i, _i, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
     "cc_yolo_net_shape": (_i, [_i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i)]),
     "cc_yolo_forward_frames": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),

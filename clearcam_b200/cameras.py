@@ -11,8 +11,11 @@ before that single wait, bit for bit what the host trackers give.  Rows on the h
 trackers.  What `step` returns per camera is what `run_inference` computes up to clearcam.py:589 — the (300,6)
 detector rows and the tracker's targets.  `step_events` goes on to :621: each camera's zone, motion gate, object-save
 picks and new-object flags (clearcam_b200/events.py), on the GPU right after the trackers (csrc/events_gpu.cu) for
-device rows and by `ObjectEvents` for host rows, and returns run_inference's preds; the alerts' counters and the saving
-of the picked crops stay with the caller.
+device rows and by `ObjectEvents` for host rows, and returns run_inference's preds.  `step_alerts` goes on to decide the
+camera's alerts (clearcam_b200/alerts.py: the adds of :612-620, the object counter and the firing loop of :465-499), on
+the GPU right after the events (csrc/alerts_gpu.cu) for device rows and by `CameraAlerts` for host rows, and
+`describe_saves` runs the description alerts of clip_latest_img (:1289-1307) on `save_objects`' embeddings; what a fired
+alert then does (image, notification, upload) and the saving of the picked crops stay with the caller.
 
 Each camera has a pixel format (clearcam_b200/pixfmt.py): "bgr24" [H,W,3] frames (the default) or "yuv420p" [H*3/2,W]
 frames, which the detector converts on the GPU.  Groups are keyed by (H, W, dtype, format).
@@ -30,6 +33,7 @@ import numpy as np
 import torch
 
 from ._lib import CC_MAX_FRAMES
+from .alerts import Alert, CameraAlerts, local_time
 from .events import ObjectEvents
 from .ocsort_tracker import ocsort
 from .pixfmt import BGR24, check_pix_fmt, yuv420p_size
@@ -50,12 +54,22 @@ class CameraEvents(NamedTuple):
     saves: np.ndarray           # (m,6) int64 track_id, class_id, x1, y1, x2, y2: the crops save_object writes
 
 
+class CameraAlertResult(NamedTuple):
+    rows: np.ndarray            # (300,6) float32 detector output in this camera's frame coordinates
+    preds: np.ndarray           # (k,7) float64: run_inference's return value (clearcam.py:611, 622)
+    flags: np.ndarray           # (k,) uint8 per preds row: bit 0 new (object_set), bit 1 new in the zone (object_set_zone)
+    saves: np.ndarray           # (m,6) int64 track_id, class_id, x1, y1, x2, y2: the crops save_object writes
+    fired: list                 # the ids of the alerts that fired this step, in alert order (clearcam.py:485-499)
+
+
 class _Camera:
     def __init__(self, thresh, classes, max_age, pix_fmt=BGR24):
         self.thresh, self.classes, self.pix_fmt = thresh, classes, pix_fmt
         self.tracker = ocsort.OCSort(max_age=max_age)          # clearcam.py:239
         self.zone = (None, False, False)                       # settings["coords"], settings["outside"], non-zone alert
         self.events = ObjectEvents(classes=classes)            # host rows' events (pred_occs, object_set, object_set_zone)
+        self.alerts = CameraAlerts()                           # host rows' alerts and the settings of every alert
+        self.alert_ids: list = []                              # the alerts' ids, in order (alert_counters[cam]'s keys)
 
     def fresh_events(self):
         self.events = ObjectEvents(*self.zone, classes=self.classes)
@@ -77,6 +91,7 @@ class CameraBatch:
         self._cam_dev: Dict[Hashable, torch.Tensor] = {}       # camera -> its device frame buffer (merged groups)
         self._table_rows: Dict[tuple, torch.Tensor] = {}       # (net_h, net_w, chunk, bucket) -> pinned rows
         self._dev_trk: Optional[ocsort.DeviceTrackers] = None  # device trackers, made on the first step with device rows
+        self._desc: Dict[str, np.ndarray] = {}                 # description text -> its CLIP text embedding (D,) float32
 
     # -- camera set (clearcam.py:207-240 init_cam; settings threshold :584, class filter :586)
     def add_camera(self, name, thresh: float = 0.5, classes=None, pix_fmt: str = BGR24):
@@ -96,6 +111,7 @@ class CameraBatch:
         """A fresh tracker and fresh events for camera `name`, as init_cam makes them."""
         self.cams[name].tracker = ocsort.OCSort(max_age=self.max_age)
         self.cams[name].fresh_events()
+        self.cams[name].alerts.reset()                         # init_cam: a fresh object counter and warm-up
         if self._dev_trk is not None and name in self._dev_trk:
             self._dev_trk.reset(name)
         self._seen.pop(name, None)
@@ -103,12 +119,106 @@ class CameraBatch:
     def set_zone(self, name, zone=None, outside: bool = False, non_zone_alert: bool = False):
         """Camera `name`'s zone for `step_events`: settings["coords"] (fractions of the frame; None for no zone),
         settings["outside"] and whether any of its alerts has no zone (clearcam.py:599-610).  Its event state (which ids
-        were saved, counted and alerted on) starts afresh."""
+        were saved, counted and alerted on) starts afresh.  non_zone_alert replaces what `set_alerts` derived, so pass
+        the current value (any(not a.zone for a in alerts)) when the camera has alerts."""
         cam = self.cams[name]
         cam.zone = (zone, outside, non_zone_alert)
         cam.fresh_events()                                     # checks the arguments
         if self._dev_trk is not None and name in self._dev_trk:
             self._dev_trk.events(name, zone, outside, non_zone_alert, cam.classes)
+
+    # -- alerts (clearcam.py RollingClassCounter :47-103, alert_counters[cam], alerts_on[cam])
+    def set_alerts(self, name, alerts, finder=None):
+        """Camera `name`'s alerts: {id: alert} in order (alert_counters[cam]), each an alerts.Alert or a reference
+        RollingClassCounter (Alert.from_counter).  Descriptions not seen before are encoded in one
+        `encode_text_batch` call of the finder's CLIP model (finder: an ObjectFinder with CLIP initialised).  Alerts whose id and settings are unchanged keep their counts
+        and last_det; new or changed ones start empty at their own last_det.  The camera's non_zone_alert (set_zone)
+        becomes whether any alert has no zone, without starting its event state afresh (a later `set_zone` sets it
+        again from its own argument).  The object counter and the warm-up stay."""
+        cam = self.cams[name]
+        items = list(alerts.items())
+        al = [a if isinstance(a, Alert) else Alert.from_counter(a) for _, a in items]
+        ids = [k for k, _ in items]
+        new = sorted({a.desc for a in al if a.desc is not None and a.desc not in self._desc})
+        if new:
+            clip = getattr(finder, "model", finder)           # an ObjectFinder's CLIP model, or a CLIP model itself
+            if clip is None:
+                raise ValueError("description alerts need a finder with CLIP initialised to encode their text")
+            t = clip.encode_text_batch(new)
+            t = getattr(t, "tensor", t)
+            t = t.detach().cpu().numpy() if hasattr(t, "detach") else np.asarray(t)
+            for text, row in zip(new, np.asarray(t, np.float32)):
+                self._desc[text] = row
+        desc_emb = None
+        if any(a.desc is not None for a in al):
+            D = len(next(self._desc[a.desc] for a in al if a.desc is not None))
+            desc_emb = np.stack([self._desc[a.desc] if a.desc is not None else np.zeros(D, np.float32) for a in al])
+        old = {k: i for i, k in enumerate(cam.alert_ids)}
+        keep = [old[k] if k in old and cam.alerts.alerts[old[k]].settings() == a.settings() else -1 for k, a in zip(ids, al)]
+        cam.alerts.replace(al, desc_emb, keep)
+        dev = self._dev_trk is not None and name in self._dev_trk
+        if dev and self._dev_trk.has_alerts(name):
+            self._dev_trk.alerts(name, al, desc_emb, keep)
+        cam.alert_ids = ids
+        nza = any(not a.zone for a in al)
+        cam.zone = cam.zone[:2] + (nza,)
+        cam.events.non_zone_alert = nza
+        if dev and self._dev_trk.has_events(name):
+            self._dev_trk.set_non_zone_alert(name, nza)
+
+    def set_alerts_on(self, name, on: bool):
+        """The reference's alerts_on[cam]: False makes every alert of the camera inactive."""
+        cam = self.cams[name]
+        cam.alerts.alerts_on = bool(on)
+        if self._dev_trk is not None and self._dev_trk.has_alerts(name):
+            self._dev_trk.set_alerts_on(name, bool(on))
+
+    def alerting(self, now: Optional[float] = None, local=None) -> List[Hashable]:
+        """The cameras process_frame runs the detector for (clearcam.py:447): those with an active alert at local time
+        `local` ((seconds of day, weekday); time.localtime(now) when None)."""
+        if local is None:
+            local = local_time(time.time() if now is None else float(now))
+        return [name for name, cam in self.cams.items() if cam.alerts.active(local).any()]
+
+    def object_counts(self, name) -> np.ndarray:
+        """Camera `name`'s object counter (self.counter[cam], /get_counts): int64 [80], the new ids per class id."""
+        if self._dev_trk is not None and self._dev_trk.has_alerts(name):
+            return self._dev_trk.counts(name)
+        return self.cams[name].alerts.counter.copy()
+
+    def reset_object_counts(self, name):
+        """/reset_counts (clearcam.py:512-517)."""
+        self.cams[name].alerts.counter[:] = 0
+        if self._dev_trk is not None and self._dev_trk.has_alerts(name):
+            self._dev_trk.reset_counts(name)
+
+    def describe_saves(self, saved: Dict[Hashable, tuple], now: Optional[float] = None, local=None) -> Dict[Hashable, list]:
+        """clip_latest_img's description alerts (clearcam.py:1289-1307) on what `save_objects` returned, in save order,
+        at clock `now` (time.time() when None) and local time `local` (time.localtime(now) when None) ->
+        {camera: [(save index, alert id, similarity)]} of the alerts that fired.  Cameras stepped on the GPU are matched in
+        one launch per CC_MAX_FRAMES cameras on the device embeddings, the others by CameraAlerts."""
+        now = time.time() if now is None else float(now)
+        if local is None:
+            local = local_time(now)
+        out = {name: [] for name in saved}
+        dev, host = [], []
+        for name, (saves, _, emb) in saved.items():
+            if emb is None or len(saves) == 0 or not self.cams[name].alerts.alerts:
+                continue
+            t = getattr(emb, "tensor", emb)
+            on_dev = isinstance(t, torch.Tensor) and t.is_cuda and self._dev_trk is not None and self._dev_trk.has_alerts(name)
+            (dev if on_dev else host).append((name, t))
+        if dev:
+            emb = torch.cat([t.float() for _, t in dev]).contiguous()
+            res = self._dev_trk.describe([(name, t.shape[0]) for name, t in dev], emb, [now] * len(dev), [local] * len(dev))
+            for (name, _), (hit, sim) in zip(dev, res):
+                ids = self.cams[name].alert_ids
+                out[name] = [(s, ids[a], float(sim[s, a])) for s, a in enumerate(hit.tolist()) if a >= 0]
+        for name, t in host:
+            e = t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
+            ids = self.cams[name].alert_ids
+            out[name] = [(s, ids[a], v) for s, a, v in self.cams[name].alerts.describe(e, now, local)]
+        return out
 
     bucket = staticmethod(batch_bucket)   # group sizes are padded to a small set of batch sizes (bounded plan count)
 
@@ -271,6 +381,21 @@ class CameraBatch:
         frames = self._from_mailboxes(mailboxes)
         return self.step_events(frames, now) if frames else {}
 
+    def step_alerts_mailboxes(self, mailboxes: Dict[Hashable, "FrameMailbox"], now: Optional[float] = None, local=None
+                              ) -> Dict[Hashable, CameraAlertResult]:
+        """`step_alerts` on the cameras whose mailboxes hold a new frame (as `step_mailboxes`)."""
+        frames = self._from_mailboxes(mailboxes)
+        return self.step_alerts(frames, now, local) if frames else {}
+
+    def step_alerts(self, frames: Dict[Hashable, np.ndarray], now: Optional[float] = None, local=None
+                    ) -> Dict[Hashable, CameraAlertResult]:
+        """`step_events`, then each camera's alerts (clearcam_b200/alerts.py) at clock `now` and local time `local`
+        ((seconds of day, weekday with 0 = Monday); time.localtime(now) when None) -> {camera: CameraAlertResult}.
+        Device rows run the alerts on the GPU right after the events, before the step's one wait; host rows run
+        `CameraAlerts`.  Which cameras to step is the caller's (`alerting`, the gate of clearcam.py:447)."""
+        now = time.time() if now is None else float(now)
+        return self._step(frames, now, local_time(now) if local is None else (float(local[0]), int(local[1])))
+
     def _from_mailboxes(self, mailboxes):
         frames = {}
         for name, mb in mailboxes.items():
@@ -297,7 +422,7 @@ class CameraBatch:
         H, W = yuv420p_size(f.shape)
         return W, H
 
-    def _step(self, frames, now):
+    def _step(self, frames, now, local=None):
         for name in frames:
             if name not in self.cams:
                 self.add_camera(name)
@@ -312,9 +437,15 @@ class CameraBatch:
                         self._dev_trk.add(n, max_age=self.max_age)
                     if now is not None and not self._dev_trk.has_events(n):
                         self._dev_trk.events(n, *self.cams[n].zone, self.cams[n].classes)
+                    if local is not None and not self._dev_trk.has_alerts(n):
+                        al = self.cams[n].alerts
+                        self._dev_trk.alerts(n, [a._replace(last_det=t) for a, t in zip(al.alerts, al.last_det)], al.desc_emb)
+                        if not al.alerts_on:
+                            self._dev_trk.set_alerts_on(n, False)
             jobs = [(n, out[i], self.cams[n].thresh) for names, _, out in pending for i, n in enumerate(names)]
             launched = self._dev_trk.launch(jobs, None if now is None else
-                                            [self._picture_size(n, frames[n]) + (now,) for n, _, _ in jobs])
+                                            [self._picture_size(n, frames[n]) + (now,) for n, _, _ in jobs],
+                                            None if local is None else [local] * len(jobs))
         if self._pin:
             torch.cuda.current_stream().synchronize()
         det = {name: rows[i].numpy().copy() for names, rows, _ in pending for i, name in enumerate(names)}
@@ -322,6 +453,9 @@ class CameraBatch:
         if not names:
             return {}
         if on_device:
+            if local is not None:
+                return {name: CameraAlertResult(det[name], p, f, s, [self.cams[name].alert_ids[i] for i in fired.tolist()])
+                        for name, (p, f, s, fired) in zip(names, self._dev_trk.finish_alerts(launched))}
             if now is not None:
                 return {name: CameraEvents(det[name], *e) for name, e in zip(names, self._dev_trk.finish_events(launched))}
             targets = self._dev_trk.finish(launched)
@@ -332,7 +466,12 @@ class CameraBatch:
         for name, tg in zip(names, targets):
             cam = self.cams[name]
             if now is not None:
-                res[name] = CameraEvents(det[name], *cam.events.update(tg, *self._picture_size(name, frames[name]), now))
+                ev = cam.events.update(tg, *self._picture_size(name, frames[name]), now)
+                if local is not None:
+                    fired = cam.alerts.step(ev[0], ev[1], now, local)
+                    res[name] = CameraAlertResult(det[name], *ev, [cam.alert_ids[i] for i in fired])
+                else:
+                    res[name] = CameraEvents(det[name], *ev)
                 continue
             if cam.classes is not None:
                 tg = [t for t in tg if int(t.class_id) in cam.classes]                       # clearcam.py:586

@@ -435,6 +435,13 @@ int cc_ocsort_gpu_events_grow(cc_ocsort_gpu* h, int slot, int capacity, void* st
   return push_events(h, slot, st);
 }
 
+int cc_ocsort_gpu_events_set_non_zone_alert(cc_ocsort_gpu* h, int slot, int non_zone_alert, void* stream) {
+  CC_REQUIRE(h && slot >= 0 && slot < h->S, "cc_ocsort_gpu_events_set_non_zone_alert: bad handle or slot %d", slot);
+  CC_REQUIRE(events_active(h, slot), "cc_ocsort_gpu_events_set_non_zone_alert: slot %d is not configured for events", slot);
+  h->ev->cfg[slot].nza = non_zone_alert ? 1 : 0;
+  return push_events(h, slot, static_cast<cudaStream_t>(stream));
+}
+
 int cc_ocsort_gpu_events(cc_ocsort_gpu* h, const cc_track_job* jobs, int B, const int* frame_wh, const double* now,
                          const double* d_trk_out, int trk_cap, const int* d_trk_count, const int* d_trk_status, double* d_preds,
                          uint8_t* d_flags, int64_t* d_saves, int cap, int* d_counts, int* d_status, void* stream) {

@@ -714,6 +714,7 @@ int cc_ocsort_gpu_destroy(cc_ocsort_gpu* h) {
   if (!h) return CC_OK;
   cudaDeviceSynchronize();            // slot storage is freed stream-ordered elsewhere; here nothing may still use it
   cc_events_destroy(h);
+  cc_alerts_destroy(h);
   for (auto& c : h->cfg)
     if (c.active) cudaFree(c.dl);
   cudaFree(h->d_cfg);
@@ -746,7 +747,9 @@ int cc_ocsort_gpu_configure(cc_ocsort_gpu* h, int slot, int max_age, int min_hit
   c.iou_threshold = iou_threshold;
   c.inertia = inertia;
   CC_CHECK_CUDA(cudaMemsetAsync(h->d_cnt + slot, 0, sizeof(SlotCnt), st));
-  const int r = cc_events_slot_clear(h, slot, st);   // a restarted tracker reuses ids: its events start afresh too
+  int r = cc_events_slot_clear(h, slot, st);   // a restarted tracker reuses ids: its events start afresh too
+  if (r != CC_OK) return r;
+  r = cc_alerts_slot_clear(h, slot, st);       // and, as init_cam, its object counter and alert warm-up
   if (r != CC_OK) return r;
   return push_cfg(h, slot, st);
 }
@@ -756,7 +759,9 @@ int cc_ocsort_gpu_free(cc_ocsort_gpu* h, int slot, void* stream) {
   SlotCfg& c = h->cfg[slot];
   if (!c.active) return CC_OK;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int r = cc_events_slot_free(h, slot, st);
+  int r = cc_events_slot_free(h, slot, st);
+  if (r != CC_OK) return r;
+  r = cc_alerts_slot_free(h, slot, st);
   if (r != CC_OK) return r;
   CC_CHECK_CUDA(cudaFreeAsync(c.dl, st));
   c = SlotCfg{};

@@ -6,14 +6,16 @@ C++ tracker of libclearcam_b200 (csrc/ocsort.cu) instead of per-frame numpy.
 
 `update_many` steps the trackers of several cameras on one batched detector result in a single library call;
 `DeviceTrackers` does the same on the GPU for rows that stay on the device, and can run each camera's object events
-(clearcam_b200/events.py, csrc/events_gpu.cu) right after its tracker."""
+(clearcam_b200/events.py, csrc/events_gpu.cu) right after its tracker, and its alerts (clearcam_b200/alerts.py,
+csrc/alerts_gpu.cu) right after those."""
 import ctypes
 from typing import List, Optional, Sequence
 
 import numpy as np
 
-from .._lib import (CC_EVENT_BAD_BOX, CC_EVENT_BAD_ORDER, CC_EVENT_NEEDS_ROOM, CC_EVENT_OK, CC_TRACK_BAD_CLASS,
-                    CC_TRACK_NEEDS_ROOM, CC_TRACK_OVERFLOW, CCError, check, lib)
+from .._lib import (CC_ALERT_DESC, CC_ALERT_MAX_ALERTS, CC_ALERT_OK, CC_ALERT_ON, CC_ALERT_SCHED, CC_ALERT_ZONE, CC_EVENT_BAD_BOX,
+                    CC_EVENT_BAD_ORDER, CC_EVENT_NEEDS_ROOM, CC_EVENT_OK, CC_TRACK_BAD_CLASS, CC_TRACK_NEEDS_ROOM, CC_TRACK_OVERFLOW,
+                    CCError, cc_alert, check, lib)
 from .STrack import STrack
 
 _CAP = 1024          # rows of the result buffer (the detector emits at most 300 boxes per frame)
@@ -33,8 +35,30 @@ def _tracks(buf: np.ndarray, n: int) -> List[STrack]:
 
 
 class _Launched(list):
-    """The jobs of one DeviceTrackers.launch; `events` holds each job's (W, H, now) when the events ran with them."""
+    """The jobs of one DeviceTrackers.launch; `events` holds each job's (W, H, now) when the events ran with them, and
+    `alerts` each job's local time (seconds of day, weekday) when the alerts ran after the events."""
     events = None
+    alerts = None
+
+
+def _cc_alert(a) -> cc_alert:
+    """alerts.Alert -> the library's cc_alert."""
+    words = [0xffffffff, 0xffffffff, 0xffff] if a.classes is None else [0, 0, 0]
+    if a.classes is not None:
+        for c in a.classes:
+            if 0 <= c < 80:
+                words[c >> 5] |= 1 << (c & 31)
+    flags = ((CC_ALERT_ON if a.is_on else 0) | (CC_ALERT_ZONE if a.zone else 0) | (CC_ALERT_DESC if a.desc is not None else 0)
+             | (CC_ALERT_SCHED if a.sched is not None else 0))
+    days = 0 if a.sched is None else sum(1 << d for d in range(7) if a.sched[1][d])
+    start, end = (0.0, 0.0) if a.sched is None else a.sched[0]
+    r = cc_alert()
+    r.classes[:] = words
+    r.max, r.flags, r.days = a.max, flags, days
+    r.window, r.start, r.end = a.span, start, end
+    r.threshold = float("inf") if a.threshold is None else a.threshold
+    r.last_det = a.last_det
+    return r
 
 
 class _EventBuffers:
@@ -52,6 +76,11 @@ class _EventBuffers:
         self.host = tuple(torch.empty(tuple(t.shape), dtype=t.dtype, pin_memory=True) for t in self.head)
         self.hcs = torch.empty((3, B), dtype=torch.int32, pin_memory=True)
         self.trk, self.B = None, 0
+        self.fired = torch.empty((B, CC_ALERT_MAX_ALERTS), dtype=torch.int32, **dev)   # alerts: fired indices, then
+        self.ares = torch.empty((2, B), dtype=torch.int32, **dev)                      # their count and status
+        self.hfired = torch.empty((B, CC_ALERT_MAX_ALERTS), dtype=torch.int32, pin_memory=True)
+        self.hares = torch.empty((2, B), dtype=torch.int32, pin_memory=True)
+        self.alerts = False                                                           # whether the alerts ran
 
 
 class OCSort:
@@ -132,6 +161,8 @@ class DeviceTrackers:
         self._bufs = []                                        # per launch of one update: device and pinned results
         self._ev, self._ecap, self._event_capacity = {}, {}, int(event_capacity)   # events: settings and room per camera
         self._ebufs, self._rbufs = [], []                      # events outputs: per launch, and for reruns after growth
+        self._al = set()                                       # cameras with alerts configured
+        self._n_alerts = {}                                    # camera -> its number of alerts
 
     def __del__(self):
         try:
@@ -207,12 +238,120 @@ class DeviceTrackers:
                                                    int(nza), mask, self._ecap[cam], self._stream()),
               f"cc_ocsort_gpu_events_configure (camera {cam!r})")
 
+    def set_non_zone_alert(self, cam, non_zone_alert: bool):
+        """Change camera `cam`'s non_zone_alert (events()) without starting its event state afresh: the reference reads it
+        from the alerts at every target (clearcam.py:604-609)."""
+        if cam not in self._ev:
+            raise KeyError(f"camera {cam!r} has no events: events() it first")
+        if not isinstance(non_zone_alert, (bool, np.bool_)):
+            raise TypeError("non_zone_alert must be a bool")
+        z, outside, _, classes = self._ev[cam]
+        self._ev[cam] = (z, outside, bool(non_zone_alert), classes)
+        check(lib().cc_ocsort_gpu_events_set_non_zone_alert(self._h, self._slot[cam], int(bool(non_zone_alert)), self._stream()),
+              f"cc_ocsort_gpu_events_set_non_zone_alert (camera {cam!r})")
+
+    def alerts(self, cam, alerts, desc_emb=None, keep=None):
+        """Run camera `cam`'s alerts (a list of alerts.Alert, in order) after its events.  desc_emb: [len(alerts), D]
+        float32 description embeddings (rows of alerts without a description are not read), None when none has one.
+        keep[i]: the index of the camera's current alert whose counts and last_det alert i keeps (equal settings), or -1.
+        The object counter, the warm-up count and alerts_on stay."""
+        from ..alerts import MAX_ALERTS, Alert
+        if cam not in self._slot:
+            raise KeyError(f"camera {cam!r} has no tracker: add() it first")
+        alerts = list(alerts)
+        if len(alerts) > MAX_ALERTS or not all(isinstance(a, Alert) for a in alerts):
+            raise ValueError(f"alerts must be at most {MAX_ALERTS} alerts.Alert")
+        table = (cc_alert * max(1, len(alerts)))(*[_cc_alert(a) for a in alerts])
+        emb, dim = None, 0
+        if any(a.desc is not None for a in alerts):
+            if desc_emb is None:
+                raise ValueError("description alerts need their embeddings")
+            t = desc_emb.detach().cpu().numpy() if hasattr(desc_emb, "detach") else desc_emb
+            emb = np.ascontiguousarray(t, np.float32)
+            if emb.ndim != 2 or emb.shape[0] != len(alerts):
+                raise ValueError(f"desc_emb must be [{len(alerts)}, D], got {emb.shape}")
+            dim = emb.shape[1]
+        kp = None if keep is None else np.ascontiguousarray(keep, np.int32)
+        if kp is not None and kp.shape != (len(alerts),):
+            raise ValueError("one keep entry per alert")
+        check(lib().cc_ocsort_gpu_alerts_configure(self._h, self._slot[cam], table, len(alerts), None if emb is None else emb.ctypes.data,
+                                                   dim, None if kp is None else kp.ctypes.data, self._stream()),
+              f"cc_ocsort_gpu_alerts_configure (camera {cam!r})")
+        self._al.add(cam)
+        self._n_alerts[cam] = len(alerts)
+
+    def has_alerts(self, cam) -> bool:
+        return cam in self._al
+
+    def set_alerts_on(self, cam, on: bool):
+        """The reference's alerts_on[cam] (is_active's first test); True after the first alerts()."""
+        self._need_alerts(cam)
+        check(lib().cc_ocsort_gpu_alerts_set_on(self._h, self._slot[cam], int(bool(on)), self._stream()),
+              f"cc_ocsort_gpu_alerts_set_on (camera {cam!r})")
+
+    def counts(self, cam) -> np.ndarray:
+        """Camera `cam`'s object counter (self.counter[cam]): int64 [80], new ids per class id.  Waits for the stream."""
+        self._need_alerts(cam)
+        out = np.zeros(80, np.int64)
+        check(lib().cc_ocsort_gpu_alerts_counts(self._h, self._slot[cam], out.ctypes.data, self._stream()),
+              f"cc_ocsort_gpu_alerts_counts (camera {cam!r})")
+        return out
+
+    def reset_counts(self, cam):
+        """Zero camera `cam`'s object counter (/reset_counts, clearcam.py:512-517)."""
+        self._need_alerts(cam)
+        check(lib().cc_ocsort_gpu_alerts_reset_counts(self._h, self._slot[cam], self._stream()),
+              f"cc_ocsort_gpu_alerts_reset_counts (camera {cam!r})")
+
+    def _need_alerts(self, cam):
+        if cam not in self._al:
+            raise KeyError(f"camera {cam!r} has no alerts: alerts() it first")
+
+    def describe(self, jobs, emb, now, local):
+        """clip_latest_img's description alerts on the device.  jobs: [(camera, rows)], the cameras' consecutive rows of
+        emb (a CUDA float32 [N,D] tensor, e.g. the embeddings of save_objects), each camera at most once; now and local
+        (seconds of day, weekday) per job.  One launch per CC_MAX_FRAMES cameras, one wait -> per job (hits (rows,) int32:
+        the index of the alert that fired per row or -1, similarities (rows, alerts) float32, NaN for alerts without a
+        description)."""
+        torch = self._torch
+        if len(jobs) != len(now) or len(jobs) != len(local):
+            raise ValueError("one clock and one local time per job")
+        if not (isinstance(emb, torch.Tensor) and emb.is_cuda and emb.dtype == torch.float32 and emb.dim() == 2 and emb.is_contiguous()):
+            raise ValueError("emb must be a contiguous CUDA float32 [N, D] tensor")
+        n = sum(int(r) for _, r in jobs)
+        if n != emb.shape[0]:
+            raise ValueError(f"the jobs cover {n} rows, emb has {emb.shape[0]}")
+        for cam, _ in jobs:
+            self._need_alerts(cam)
+        hit = torch.empty(max(n, 1), dtype=torch.int32, device="cuda")
+        sim = torch.empty((max(n, 1), CC_ALERT_MAX_ALERTS), dtype=torch.float32, device="cuda")
+        r0 = 0
+        for c0 in range(0, len(jobs), self._B):
+            chunk = jobs[c0:c0 + self._B]
+            rows = np.array([int(r) for _, r in chunk], np.int32)
+            slots = np.array([self._slot[cam] for cam, _ in chunk], np.int32)
+            t = np.array([float(x) for x in now[c0:c0 + self._B]], np.float64)
+            loc = np.array([(float(a), float(b)) for a, b in local[c0:c0 + self._B]], np.float64).reshape(-1)
+            check(lib().cc_ocsort_gpu_describe(self._h, slots.ctypes.data, rows.ctypes.data, len(chunk), t.ctypes.data, loc.ctypes.data,
+                                               emb[r0:].data_ptr() if r0 < n else emb.data_ptr(), emb.shape[1], hit[r0:].data_ptr(),
+                                               sim[r0:].data_ptr(), self._stream()), "cc_ocsort_gpu_describe")
+            r0 += int(rows.sum())
+        h, s = hit.cpu().numpy(), sim.cpu().numpy()
+        out, r0 = [], 0
+        for cam, r in jobs:
+            A = self._n_alerts[cam]
+            out.append((h[r0:r0 + r].copy(), s[r0:r0 + r, :A].copy()))
+            r0 += r
+        return out
+
     def remove(self, cam):
         slot = self._slot.pop(cam, None)
         if slot is None:
             return
         del self._args[cam], self._cap[cam]
         self._ev.pop(cam, None)
+        self._al.discard(cam)
+        self._n_alerts.pop(cam, None)
         self._ecap.pop(cam, None)
         check(lib().cc_ocsort_gpu_free(self._h, slot, self._stream()), "cc_ocsort_gpu_free")   # frees its events too
         self._free.append(slot)
@@ -234,9 +373,10 @@ class DeviceTrackers:
                                torch.empty((2, self._B), dtype=torch.int32, pin_memory=True)))
         return self._bufs[i]
 
-    def _launch(self, jobs, i, events=None):
+    def _launch(self, jobs, i, events=None, alerts=None):
         """Enqueue one launch for <= CC_MAX_FRAMES jobs into buffer set i and the copy of its results to the host; with
-        `events` ((W, H, now) per job), the events launch on its outputs follows."""
+        `events` ((W, H, now) per job), the events launch on its outputs follows, and with `alerts` (local time per job)
+        the alerts launch after that."""
         from .._lib import cc_track_job
         table = (cc_track_job * len(jobs))()
         for b, (cam, rows, thr) in enumerate(jobs):
@@ -255,13 +395,16 @@ class DeviceTrackers:
         if events is not None:
             while len(self._ebufs) <= i:
                 self._ebufs.append(_EventBuffers(self._torch, self._B))
-            self._launch_events(table, [j[0] for j in jobs], events, (out, cs[0], cs[1]), self._ebufs[i])
+            self._launch_events(table, [j[0] for j in jobs], events, (out, cs[0], cs[1]), self._ebufs[i], alerts)
 
-    def _launch_events(self, table, cams, events, trk, eb):
-        """Enqueue the events of `cams` (slots in `table`) on tracker outputs `trk` into event buffers `eb`."""
+    def _launch_events(self, table, cams, events, trk, eb, alerts=None):
+        """Enqueue the events of `cams` (slots in `table`) on tracker outputs `trk` into event buffers `eb`, and with
+        `alerts` (local time per camera) the alerts on the events' outputs."""
         for cam in cams:
             if cam not in self._ev:
                 raise KeyError(f"camera {cam!r} has no events: events() it first")
+            if alerts is not None:
+                self._need_alerts(cam)
         B = len(cams)
         wh = np.array([(int(W), int(H)) for W, H, _ in events], np.int32).reshape(-1)
         now = np.array([float(t) for _, _, t in events], np.float64)
@@ -275,18 +418,39 @@ class DeviceTrackers:
         eb.hcs.view(-1)[:3 * B].copy_(cs, non_blocking=True)
         for h, d in zip(eb.head, eb.host):
             d[:B].copy_(h[:B], non_blocking=True)
+        eb.alerts = alerts is not None
+        if eb.alerts:
+            loc = np.array([(float(t), float(d)) for t, d in alerts], np.float64).reshape(-1)
+            ares = eb.ares.view(-1)[:2 * B]
+            check(lib().cc_ocsort_gpu_alerts(self._h, table, B, now.ctypes.data, loc.ctypes.data, eb.preds.data_ptr(), eb.flags.data_ptr(),
+                                             _CAP, cs.data_ptr(), cs[2 * B:].data_ptr(), eb.fired.data_ptr(), ares.data_ptr(),
+                                             self._stream()), "cc_ocsort_gpu_alerts")
+            eb.hfired[:B].copy_(eb.fired[:B], non_blocking=True)
+            eb.hares.view(-1)[:2 * B].copy_(ares, non_blocking=True)
 
-    def launch(self, jobs, events=None):
+    def launch(self, jobs, events=None, alerts=None):
         """Enqueue `update(jobs)` without waiting; pass the result to `finish` after the stream is synchronised.
         events: (W, H, now) per job — the frame's picture size and the step's clock — to run each camera's object events
-        right after its tracker (`finish_events` then returns them)."""
+        right after its tracker (`finish_events` then returns them).  alerts: (seconds of day, weekday) per job — the
+        step's local time — to run each camera's alerts right after its events (`finish_alerts` then returns them)."""
         jobs = _Launched(jobs)
         if events is not None:
             jobs.events = list(events)
             if len(jobs.events) != len(jobs):
                 raise ValueError("one (W, H, now) per job")
+        if alerts is not None:
+            if events is None:
+                raise ValueError("alerts run on the events' outputs: pass events= too")
+            jobs.alerts = [(float(t), int(d)) for t, d in alerts]
+            if len(jobs.alerts) != len(jobs):
+                raise ValueError("one (seconds of day, weekday) per job")
+            if not all(np.isfinite(t) and 0 <= d <= 6 for t, d in jobs.alerts):    # checked before the tracker launches
+                raise ValueError("local time: a finite time of day and a weekday in 0..6")
+            for cam, _, _ in jobs:
+                self._need_alerts(cam)
         for i, c0 in enumerate(range(0, len(jobs), self._B)):
-            self._launch(jobs[c0:c0 + self._B], i, None if jobs.events is None else jobs.events[c0:c0 + self._B])
+            self._launch(jobs[c0:c0 + self._B], i, None if jobs.events is None else jobs.events[c0:c0 + self._B],
+                         None if jobs.alerts is None else jobs.alerts[c0:c0 + self._B])
         return jobs
 
     def finish(self, jobs, targets: bool = True) -> list:
@@ -311,6 +475,20 @@ class DeviceTrackers:
         if getattr(jobs, "events", None) is None:
             raise ValueError("these jobs were launched without events")
         _, res, errors = self._collect(jobs, False)
+        res = [None if r is None else r[:3] for r in res]
+        if errors:
+            e = CCError("; ".join(errors))
+            e.results = res
+            raise e
+        return res
+
+    def finish_alerts(self, jobs) -> list:
+        """The events and alerts of `launch(jobs, events=..., alerts=...)` once the stream has been synchronised: per camera
+        (preds, flags, saves, fired) with fired the (n,) int32 indices of the alerts that fired, in alert order.  Events
+        run again after growth carry their alerts along.  Errors as finish_events."""
+        if getattr(jobs, "alerts", None) is None:
+            raise ValueError("these jobs were launched without alerts")
+        _, res, errors = self._collect(jobs, False)
         if errors:
             e = CCError("; ".join(errors))
             e.results = res
@@ -326,7 +504,13 @@ class DeviceTrackers:
                 p, f, s = (h[b, :c].numpy().copy() for h, c in zip(eb.host, (n, n, m)))
             else:
                 p, f, s = eb.preds[b, :n].cpu().numpy(), eb.flags[b, :n].cpu().numpy(), eb.saves[b, :m].cpu().numpy()
-            evr[k] = (p, f, s)
+            fired = None
+            if eb.alerts:
+                if int(eb.hares.view(-1)[eb.B + b]) != CC_ALERT_OK:
+                    errors.append(f"camera {cam!r}: its alerts did not run")
+                    return
+                fired = eb.hfired[b, :int(eb.hares.view(-1)[b])].numpy().copy()
+            evr[k] = (p, f, s, fired)
         elif st == CC_EVENT_NEEDS_ROOM:
             grow.append((k, eb, b, n))
         elif st == CC_EVENT_BAD_BOX:
@@ -340,6 +524,7 @@ class DeviceTrackers:
         from .._lib import cc_track_job
         res, evr, errors = [None] * len(jobs), [None] * len(jobs), []
         ev = getattr(jobs, "events", None)
+        al = getattr(jobs, "alerts", None)
         pend = [(k, k // self._B, k % self._B) for k in range(len(jobs))]    # (job, buffer set, row) of tracker launches
         ev_pend = []                                                            # (job, event buffers, row) of event reruns
         while pend or ev_pend:
@@ -380,7 +565,8 @@ class DeviceTrackers:
                 while len(self._rbufs) <= j:
                     self._rbufs.append(_EventBuffers(self._torch, self._B))
                 table = (cc_track_job * len(chunk))(*[cc_track_job(None, 0, self._slot[jobs[k][0]], 0.0, 0) for k, _, _, _ in chunk])
-                self._launch_events(table, [jobs[k][0] for k, _, _, _ in chunk], [ev[k] for k, _, _, _ in chunk], trk, self._rbufs[j])
+                self._launch_events(table, [jobs[k][0] for k, _, _, _ in chunk], [ev[k] for k, _, _, _ in chunk], trk, self._rbufs[j],
+                                    None if al is None else [al[k] for k, _, _, _ in chunk])
                 ev_pend += [(k, self._rbufs[j], b) for b, (k, _, _, _) in enumerate(chunk)]
             for k, need in grow:
                 cam = jobs[k][0]
@@ -392,7 +578,8 @@ class DeviceTrackers:
             if idx:
                 again = [jobs[k] for k in idx]
                 for i, c0 in enumerate(range(0, len(idx), self._B)):
-                    self._launch(again[c0:c0 + self._B], i, None if ev is None else [ev[k] for k in idx[c0:c0 + self._B]])
+                    self._launch(again[c0:c0 + self._B], i, None if ev is None else [ev[k] for k in idx[c0:c0 + self._B]],
+                                 None if al is None else [al[k] for k in idx[c0:c0 + self._B]])
                 pend = [(k, p // self._B, p % self._B) for p, k in enumerate(idx)]
             if pend or ev_pend:
                 self._torch.cuda.current_stream().synchronize()

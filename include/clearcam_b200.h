@@ -517,6 +517,70 @@ int cc_ocsort_gpu_events(cc_ocsort_gpu* h, const cc_track_job* jobs, int B, cons
                          const double* d_trk_out, int trk_cap, const int* d_trk_count, const int* d_trk_status, double* d_preds,
                          uint8_t* d_flags, int64_t* d_saves, int cap, int* d_counts, int* d_status, void* stream);
 
+int cc_ocsort_gpu_events_set_non_zone_alert(cc_ocsort_gpu* h, int slot, int non_zone_alert, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * Alerts on the tracker handle: the adds of run_inference (clearcam.py:612-620) behind the object events, the object
+ * counter, the firing loop of process_frame (:465-499) and the description alerts of clip_latest_img (:1289-1307).
+ * clearcam_b200/alerts.py is the host form and documents the choices (one clock and one local time per step; a missing
+ * weekday entry is inactive; alerts with max 0 and description alerts keep no counts; the warm-up counts steps; the
+ * similarity's fixed summation order; a camera the caller leaves out of a step — the reference's gate when none of its
+ * alerts is active — keeps its counts and its warm-up count until its next step).
+ *
+ * cc_alert: one alert.  classes: bits for the class ids 0..79 it counts; max: 0 = none (it never fires on counts);
+ * window: seconds > 0, already resolved (None -> 60 when is_notif, else 1); flags CC_ALERT_*; with CC_ALERT_SCHED the
+ * alert is active on the weekdays of `days` (bit 0 Monday) when start - window < time of day < end; threshold: the
+ * similarity a description alert must exceed (+inf: never); last_det: the clock of its last firing.
+ *
+ * cc_ocsort_gpu_alerts_configure: the n alerts of tracker slot `slot`, in order (at most CC_ALERT_MAX_ALERTS);
+ * desc_emb [n,dim] float32 host rows (only rows of CC_ALERT_DESC alerts are read; NULL when there are none); keep[i] >= 0
+ * makes alert i keep the counts and last_det of the slot's current alert keep[i] (same max, classes and CC_ALERT_DESC),
+ * rows of alerts without CC_ALERT_DESC are neither read nor checked;
+ * -1 (or keep NULL) starts it empty at its own last_det.  The object counter, the warm-up count and alerts_on stay.
+ * cc_ocsort_gpu_configure clears the counter and the warm-up (init_cam); cc_ocsort_gpu_free frees the alerts.
+ * cc_ocsort_gpu_alerts_set_on: the camera's alerts_on (1 after configure).  cc_ocsort_gpu_alerts_counts: the object
+ * counter, int64 [80] per class id (waits for `stream`); cc_ocsort_gpu_alerts_reset_counts zeroes it.
+ * cc_ocsort_gpu_events_set_non_zone_alert changes a slot's non_zone_alert without touching its event state.
+ *
+ * cc_ocsort_gpu_alerts: job b (a cc_ocsort_gpu_update job table; only .slot is read) runs the alerts of jobs[b].slot on
+ * row b of a cc_ocsort_gpu_events launch's outputs (d_preds [B,cap,7], d_flags [B,cap], its d_counts and d_status),
+ * queued after it on the same stream, at clock now[b] and local time local[2b] (seconds of day), local[2b+1] (weekday,
+ * 0 = Monday).  Outputs: d_fired [B,CC_ALERT_MAX_ALERTS] the indices of the alerts that fired, in order; d_res[b] their
+ * number and d_res[B+b] = CC_ALERT_*: OK, or NOT_RUN when the events' status was not CC_EVENT_OK (nothing changed; run
+ * the alerts again after the events).
+ *
+ * cc_ocsort_gpu_describe: job b matches rows[b] object embeddings of slot slots[b] (consecutive rows of d_emb [N,dim]
+ * float32, jobs in order) against its description alerts at clock now[b], local time local[2b..2b+1].  Outputs per row:
+ * d_hit the index of the alert that fired (-1 none), d_sim [N,CC_ALERT_MAX_ALERTS] float32 similarities (NaN for alerts
+ * without a description).
+ *
+ * Bad arguments (a slot without alerts, a repeated slot, B outside 1..CC_MAX_FRAMES, a clock or time of day that is not
+ * finite, a weekday outside 0..6, a description width that differs from the slot's, NULL pointers; for configure a
+ * bad alert or keep entry) fail with CC_ERR_INVALID before anything is launched or changed. */
+#define CC_ALERT_MAX_ALERTS 64
+#define CC_ALERT_MAX_COUNT 1024
+#define CC_ALERT_ON 1
+#define CC_ALERT_ZONE 2
+#define CC_ALERT_DESC 4
+#define CC_ALERT_SCHED 8
+#define CC_ALERT_OK 0
+#define CC_ALERT_NOT_RUN 1
+typedef struct {
+  uint32_t classes[3];
+  int max, flags, days, reserved[2];
+  double window, start, end, threshold, last_det;
+} cc_alert;
+int cc_ocsort_gpu_alerts_configure(cc_ocsort_gpu* h, int slot, const cc_alert* alerts, int n, const float* desc_emb, int dim,
+                                   const int* keep, void* stream);
+int cc_ocsort_gpu_alerts_set_on(cc_ocsort_gpu* h, int slot, int on, void* stream);
+int cc_ocsort_gpu_alerts_counts(cc_ocsort_gpu* h, int slot, int64_t* counts, void* stream);
+int cc_ocsort_gpu_alerts_reset_counts(cc_ocsort_gpu* h, int slot, void* stream);
+int cc_ocsort_gpu_alerts(cc_ocsort_gpu* h, const cc_track_job* jobs, int B, const double* now, const double* local,
+                         const double* d_preds, const uint8_t* d_flags, int cap, const int* d_ev_counts, const int* d_ev_status,
+                         int* d_fired, int* d_res, void* stream);
+int cc_ocsort_gpu_describe(cc_ocsort_gpu* h, const int* slots, const int* rows, int B, const double* now, const double* local,
+                           const float* d_emb, int dim, int* d_hit, float* d_sim, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
