@@ -31,6 +31,12 @@ class cc_track_job(ctypes.Structure):
                 ("reserved", ctypes.c_int)]
 
 
+class cc_track_run(ctypes.Structure):
+    """One row of a tracker run table (cc_ocsort_gpu_update_runs): device rows [frames,n,6], n, frames, slot, threshold."""
+    _fields_ = [("rows", ctypes.c_void_p), ("n", ctypes.c_int), ("frames", ctypes.c_int), ("slot", ctypes.c_int),
+                ("det_thresh", ctypes.c_float)]
+
+
 class cc_slice(ctypes.Structure):
     """An NHWC slice as cc_yolo_op_conv reports it: device pointer, channels per pixel, first channel, channels, N, H, W, fp32."""
     _fields_ = [("p", ctypes.c_void_p)] + [(n, ctypes.c_int) for n in ("cs", "co", "C", "N", "H", "W", "f32")]
@@ -51,7 +57,7 @@ class cc_conv_op(ctypes.Structure):
 CC_CONV_OP_NONE, CC_CONV_OP_GEMM, CC_CONV_OP_CHAIN, CC_CONV_OP_DIRECT = 0, 1, 2, 3
 
 # cc_ocsort_gpu_update statuses (CC_TRACK_* in include/clearcam_b200.h)
-CC_TRACK_OK, CC_TRACK_NEEDS_ROOM, CC_TRACK_BAD_CLASS, CC_TRACK_OVERFLOW = 0, 1, 2, 3
+CC_TRACK_OK, CC_TRACK_NEEDS_ROOM, CC_TRACK_BAD_CLASS, CC_TRACK_OVERFLOW, CC_TRACK_BAD_BOX = 0, 1, 2, 3, 4
 # cc_ocsort_gpu_events statuses (CC_EVENT_* in include/clearcam_b200.h)
 CC_EVENT_OK, CC_EVENT_NEEDS_ROOM, CC_EVENT_BAD_BOX, CC_EVENT_NOT_RUN, CC_EVENT_BAD_ORDER = 0, 1, 2, 3, 4
 CC_EVENT_MAX_VERTICES = 256
@@ -137,6 +143,11 @@ _SIGS = {
     "cc_ocsort_gpu_alerts_reset_counts": (_i, [_vp, _i, _vp]),
     "cc_ocsort_gpu_alerts": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "cc_ocsort_gpu_describe": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    "cc_ocsort_gpu_update_runs": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "cc_ocsort_gpu_events_runs": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp,
+                                       _vp]),
+    "cc_ocsort_gpu_alerts_runs": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "cc_ocsort_gpu_describe_runs": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     "cc_letterbox": (_i, [_vp, _i, _i, _i, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
     "cc_yolo_net_shape": (_i, [_i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i)]),
     "cc_yolo_forward_frames": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),

@@ -105,7 +105,14 @@ class CameraBatch:
             self._dev_trk.remove(name)
         self._where.pop(name, None)
         self._cam_dev.pop(name, None)
+        self._drop_run_frames(name, 0)
         self._seen.pop(name, None)             # a re-added camera starts a new mailbox whose frame_num restarts at 0
+
+    def _drop_run_frames(self, name, T):
+        """Forget camera `name`'s per-frame device buffers of step_video (keys (name, f)) for frames f >= T."""
+        for d in (self._where, self._cam_dev):
+            for key in [k for k in d if isinstance(k, tuple) and len(k) == 2 and k[0] == name and k[1] >= T]:
+                del d[key]
 
     def reset_tracker(self, name):
         """A fresh tracker and fresh events for camera `name`, as init_cam makes them."""
@@ -196,18 +203,49 @@ class CameraBatch:
         """clip_latest_img's description alerts (clearcam.py:1289-1307) on what `save_objects` returned, in save order,
         at clock `now` (time.time() when None) and local time `local` (time.localtime(now) when None) ->
         {camera: [(save index, alert id, similarity)]} of the alerts that fired.  Cameras stepped on the GPU are matched in
-        one launch per CC_MAX_FRAMES cameras on the device embeddings, the others by CameraAlerts."""
+        one launch per CC_MAX_FRAMES cameras on the device embeddings, the others by CameraAlerts.  A run's saves (from
+        `step_video`) are matched frame by frame, each at its own clock: pass now={camera: the run's clocks, one per frame} and
+        local=None (time.localtime of each) or {camera: one local time per frame}; with a dict `now`, cameras with a single
+        step's saves are matched at time.time()."""
+        runs_now, runs_local = now, local
+        if isinstance(now, dict):
+            now, local = None, None
         now = time.time() if now is None else float(now)
         if local is None:
             local = local_time(now)
         out = {name: [] for name in saved}
         dev, host = [], []
+        runs, hruns = [], []
         for name, (saves, _, emb) in saved.items():
             if emb is None or len(saves) == 0 or not self.cams[name].alerts.alerts:
                 continue
             t = getattr(emb, "tensor", emb)
             on_dev = isinstance(t, torch.Tensor) and t.is_cuda and self._dev_trk is not None and self._dev_trk.has_alerts(name)
+            if np.asarray(saves).shape[1] == 7:                # a run's saves: each frame at its own clock (step_video)
+                if not isinstance(runs_now, dict) or name not in runs_now:
+                    raise ValueError(f"camera {name!r}: a run's saves need now={{camera: one clock per frame of the run}}")
+                clocks = [float(t) for t in runs_now[name]]
+                locs = ([local_time(t) for t in clocks] if runs_local is None
+                        else [(float(a), int(d)) for a, d in runs_local[name]])
+                if len(locs) != len(clocks) or int(np.asarray(saves)[:, 0].max()) >= len(clocks):
+                    raise ValueError(f"camera {name!r}: one clock and one local time per frame of the run")
+                rows = np.bincount(np.asarray(saves)[:, 0], minlength=len(clocks)).tolist()
+                (runs if on_dev else hruns).append((name, t, rows, clocks, locs))
+                continue
             (dev if on_dev else host).append((name, t))
+        if runs:
+            emb = torch.cat([t.float() for _, t, _, _, _ in runs]).contiguous()
+            res = self._dev_trk.describe_runs([(name, rows) for name, _, rows, _, _ in runs], emb, [c for _, _, _, c, _ in runs],
+                                              [lc for _, _, _, _, lc in runs])
+            for (name, _, _, _, _), (hit, sim) in zip(runs, res):
+                ids = self.cams[name].alert_ids
+                out[name] = [(s, ids[a], float(sim[s, a])) for s, a in enumerate(hit.tolist()) if a >= 0]
+        for name, t, rows, clocks, locs in hruns:
+            e = t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
+            ids, r0 = self.cams[name].alert_ids, 0
+            for n, c, lc in zip(rows, clocks, locs):
+                out[name] += [(r0 + s, ids[a], v) for s, a, v in self.cams[name].alerts.describe(e[r0:r0 + n], c, lc)]
+                r0 += n
         if dev:
             emb = torch.cat([t.float() for _, t in dev]).contiguous()
             res = self._dev_trk.describe([(name, t.shape[0]) for name, t in dev], emb, [now] * len(dev), [local] * len(dev))
@@ -291,11 +329,12 @@ class CameraBatch:
             torch.cuda.current_stream().synchronize()
         return {name: rows[i].numpy().copy() for names, rows, _ in pending for i, name in enumerate(names)}
 
-    def _launch(self, frames) -> list:
+    def _launch(self, frames, fmts=None) -> list:
         """Queue every detector call of `detect` and the copies of its rows to the host: [(cameras, host rows, detector
-        output)]."""
+        output)].  fmts: each frame's pixel format when the keys of `frames` are not camera names (its camera's by default)."""
         pending = []
-        fmts = {name: cam.pix_fmt for name, cam in self.cams.items() if cam.pix_fmt != BGR24}
+        if fmts is None:
+            fmts = {name: cam.pix_fmt for name, cam in self.cams.items() if cam.pix_fmt != BGR24}
         groups = self.group_by_shape(frames, fmts)
         for net, keys in self.merge_groups(groups):
             if len(keys) > 1:
@@ -347,25 +386,40 @@ class CameraBatch:
     def save_objects(self, results: Dict[Hashable, CameraEvents], finder, quality: int = 95) -> Dict[Hashable, tuple]:
         """The thumbnails and embeddings of every camera's object saves of the last step in ONE call (`save_object` and
         `clip_latest_img`, clearcam.py:373-399, 272-279, 1278-1287): results is what `step_events` /
-        `step_events_mailboxes` returned; every camera's saves[:, 2:6] are cut from its `device_frame` in its own pixel
-        format by one `finder.encode_embed_frames` call -> {camera: (saves, files, embeddings)}, files and embedding rows
-        in saves order (embeddings None when CLIP is not initialised, or when the camera has no saves).  A step without
-        saves makes no library call.  Reads `device_frame`, so it is valid until the next step."""
-        cams = [name for name, ev in results.items() if len(ev.saves)]
-        out = {name: (ev.saves, [], None) for name, ev in results.items()}
-        if not cams:
+        `step_events_mailboxes` returned, or what `step_video` returned (a list per camera); every camera's saves[:, 2:6]
+        are cut from its `device_frame` — for a run, from the device copy of the save's own frame — in its own pixel format
+        by one `finder.encode_embed_frames` call -> {camera: (saves, files, embeddings)}, files and embedding rows in saves
+        order (embeddings None when CLIP is not initialised, or when the camera has no saves).  A run's saves are (m,7):
+        the frame index in the run, then the six save columns, frame after frame.  A step without saves makes no library
+        call.  Reads the device frames of the last step, so it is valid until the next step."""
+        # (camera, frame key, saves): a step's result is one frame; a step_video result (a list) one per frame of the run,
+        # whose saves are returned with their frame index in front
+        srcs, out = [], {}
+        for name, ev in results.items():
+            if isinstance(ev, list):
+                for f, e in enumerate(ev):
+                    if len(e.saves):
+                        srcs.append((name, (name, f), e.saves))
+                out[name] = (np.concatenate([np.concatenate([np.full((len(e.saves), 1), f, np.int64), np.asarray(e.saves, np.int64)
+                                                             .reshape(-1, 6)], 1) for f, e in enumerate(ev)]).reshape(-1, 7), [], None)
+            else:
+                if len(ev.saves):
+                    srcs.append((name, name, ev.saves))
+                out[name] = (ev.saves, [], None)
+        if not srcs:
             return out
-        frames = [self.device_frame(name) for name in cams]
-        rects = np.concatenate([np.concatenate([np.full((len(results[name].saves), 1), j, np.int64),
-                                                np.asarray(results[name].saves, np.int64)[:, 2:6]], 1)
-                                for j, name in enumerate(cams)]).astype(np.int32)
-        files, emb = finder.encode_embed_frames(frames, [self.cams[name].pix_fmt for name in cams], rects, quality)
+        frames = [self.device_frame(key) for _, key, _ in srcs]
+        rects = np.concatenate([np.concatenate([np.full((len(sv), 1), j, np.int64), np.asarray(sv, np.int64)[:, 2:6]], 1)
+                                for j, (_, _, sv) in enumerate(srcs)]).astype(np.int32)
+        files, emb = finder.encode_embed_frames(frames, [self.cams[name].pix_fmt for name, _, _ in srcs], rects, quality)
         from .detection.yolov9 import DeviceResult
-        k = 0
-        for name in cams:
-            n = len(results[name].saves)
-            out[name] = (results[name].saves, files[k:k + n], None if emb is None else DeviceResult(emb.tensor[k:k + n]))
-            k += n
+        k, first = 0, {}
+        for name, _, sv in srcs:
+            first.setdefault(name, k)
+            k += len(sv)
+        for name, k0 in first.items():
+            n = len(out[name][0])
+            out[name] = (out[name][0], files[k0:k0 + n], None if emb is None else DeviceResult(emb.tensor[k0:k0 + n]))
         return out
 
     def step_mailboxes(self, mailboxes: Dict[Hashable, "FrameMailbox"]) -> Dict[Hashable, CameraResult]:
@@ -416,11 +470,82 @@ class CameraBatch:
         size is its picture's (a yuv420p frame [H*3/2,W] is W x H)."""
         return self._step(frames, time.time() if now is None else float(now))
 
+    def step_video(self, frames: Dict[Hashable, object], clocks: Dict[Hashable, object], local=None
+                   ) -> Dict[Hashable, List[CameraAlertResult]]:
+        """`step_alerts` over runs of consecutive frames: frames {camera: [T,H,W,3] bgr24 or [T,H*3/2,W] yuv420p frames of
+        one video, in order}, clocks {camera: T clocks}, local None (time.localtime of each clock) or {camera: T (seconds
+        of day, weekday)} -> {camera: [CameraAlertResult per frame]}, what T successive `step_alerts` calls with those
+        clocks would return.  Every frame of every camera goes through the detector grouping of `step` (one detect_batch
+        per shape, or frame tables of at most CC_MAX_FRAMES frames per net shape); device rows then run one launch per stage
+        (tracker, events, alerts) for all cameras and one wait, host rows the host objects frame by frame.  A video camera
+        is a normal camera: `step` and `step_video` may alternate on it."""
+        flat, runs = {}, {}
+        for name, fr in frames.items():
+            if name not in self.cams:
+                self.add_camera(name)
+            T = len(fr)
+            if not 1 <= T <= CC_MAX_FRAMES:
+                raise ValueError(f"camera {name!r}: {T} frames (1..{CC_MAX_FRAMES} per run)")
+            c = [float(t) for t in clocks[name]]
+            if len(c) != T or not all(np.isfinite(c)):
+                raise ValueError(f"camera {name!r}: one finite clock per frame")
+            lc = [local_time(t) for t in c] if local is None else [(float(a), int(d)) for a, d in local[name]]
+            if len(lc) != T:
+                raise ValueError(f"camera {name!r}: one local time per frame")
+            runs[name] = (T, c, lc)
+            for f in range(T):
+                flat[(name, f)] = fr[f]
+        fmts = {(name, f): self.cams[name].pix_fmt for name, (T, _, _) in runs.items() for f in range(T)}
+        pending = self._launch(flat, fmts)
+        for name, (T, _, _) in runs.items():
+            self._drop_run_frames(name, T)     # buffers of a longer earlier run
+        size = {name: self._picture_size(name, frames[name][0]) for name in runs}
+        on_device = bool(pending) and all(isinstance(out, torch.Tensor) and out.is_cuda for _, _, out in pending)
+        if on_device:
+            if self._dev_trk is None:
+                self._dev_trk = ocsort.DeviceTrackers()
+            for n in runs:
+                self._device_camera(n, True, True)
+            where = {key: (out, i) for keys, _, out in pending for i, key in enumerate(keys)}
+            jobs = [(n, torch.stack([where[(n, f)][0][where[(n, f)][1]] for f in range(T)]), self.cams[n].thresh)
+                    for n, (T, _, _) in runs.items()]
+            launched = self._dev_trk.launch_runs(jobs, [[size[n] + (t,) for t in c] for n, (_, c, _) in runs.items()],
+                                                 [lc for _, _, lc in runs.values()])
+        if self._pin:
+            torch.cuda.current_stream().synchronize()
+        det = {key: rows[i].numpy().copy() for keys, rows, _ in pending for i, key in enumerate(keys)}
+        res = {}
+        if on_device:
+            for n, per in zip(runs, self._dev_trk.finish_runs(launched)):
+                ids = self.cams[n].alert_ids
+                res[n] = [CameraAlertResult(det[(n, f)], p, fl, s, [ids[i] for i in fired.tolist()]) for f, (p, fl, s, fired) in enumerate(per)]
+            return res
+        for n, (T, c, lc) in runs.items():
+            cam, res[n] = self.cams[n], []
+            for f in range(T):
+                [tg] = ocsort.update_many([cam.tracker], det[(n, f)][None], [cam.thresh])
+                ev = cam.events.update(tg, *size[n], c[f])
+                fired = cam.alerts.step(ev[0], ev[1], c[f], lc[f])
+                res[n].append(CameraAlertResult(det[(n, f)], *ev, [cam.alert_ids[i] for i in fired]))
+        return res
+
     def _picture_size(self, name, f):
         if self.cams[name].pix_fmt == BGR24:
             return int(f.shape[1]), int(f.shape[0])
         H, W = yuv420p_size(f.shape)
         return W, H
+
+    def _device_camera(self, n, events: bool, alerts: bool):
+        """Camera n's device tracker, and its device events and alerts when the step runs them, made on first use."""
+        if n not in self._dev_trk:
+            self._dev_trk.add(n, max_age=self.max_age)
+        if events and not self._dev_trk.has_events(n):
+            self._dev_trk.events(n, *self.cams[n].zone, self.cams[n].classes)
+        if alerts and not self._dev_trk.has_alerts(n):
+            al = self.cams[n].alerts
+            self._dev_trk.alerts(n, [a._replace(last_det=t) for a, t in zip(al.alerts, al.last_det)], al.desc_emb)
+            if not al.alerts_on:
+                self._dev_trk.set_alerts_on(n, False)
 
     def _step(self, frames, now, local=None):
         for name in frames:
@@ -433,15 +558,7 @@ class CameraBatch:
                 self._dev_trk = ocsort.DeviceTrackers()
             for names, _, _ in pending:
                 for n in names:
-                    if n not in self._dev_trk:
-                        self._dev_trk.add(n, max_age=self.max_age)
-                    if now is not None and not self._dev_trk.has_events(n):
-                        self._dev_trk.events(n, *self.cams[n].zone, self.cams[n].classes)
-                    if local is not None and not self._dev_trk.has_alerts(n):
-                        al = self.cams[n].alerts
-                        self._dev_trk.alerts(n, [a._replace(last_det=t) for a, t in zip(al.alerts, al.last_det)], al.desc_emb)
-                        if not al.alerts_on:
-                            self._dev_trk.set_alerts_on(n, False)
+                    self._device_camera(n, now is not None, local is not None)
             jobs = [(n, out[i], self.cams[n].thresh) for names, _, out in pending for i, n in enumerate(names)]
             launched = self._dev_trk.launch(jobs, None if now is None else
                                             [self._picture_size(n, frames[n]) + (now,) for n, _, _ in jobs],

@@ -118,25 +118,11 @@ __device__ __forceinline__ bool prune(const AlSlot& s, int a, double now) {
   return __any_sync(0xffffffffu, full);
 }
 
-__global__ void __launch_bounds__(kThreads) alerts_kernel(const __grid_constant__ AlJobs jt, const AlSlot* __restrict__ slots,
-                                                          const double* __restrict__ preds, const uint8_t* __restrict__ flags,
-                                                          int cap, const int* __restrict__ ev_counts,
-                                                          const int* __restrict__ ev_status, int* __restrict__ fired,
-                                                          int* __restrict__ res, int B) {
-  __shared__ int fire[kMaxA];
-  const int b = blockIdx.x;
-  if (ev_status[b] != CC_EVENT_OK) {
-    if (threadIdx.x == 0) {
-      res[b] = 0;
-      res[B + b] = CC_ALERT_NOT_RUN;
-    }
-    return;
-  }
-  const AlJob job = jt.j[b];
+// One step of slot job.slot's alerts (the whole CTA) on one frame's events: n preds rows pr [n,7] with their flags fl.
+// The indices of the alerts that fired go to fired[]; returns their number (in thread 0).
+__device__ __forceinline__ int alerts_frame(int* fire, const AlJob job, const AlSlot* slots, const double* __restrict__ pr,
+                                            const uint8_t* __restrict__ fl, int n, int* __restrict__ fired) {
   const AlSlot& s = slots[job.slot];
-  const int n = ev_counts[b];
-  const double* pr = preds + static_cast<size_t>(b) * cap * 7;
-  const uint8_t* fl = flags + static_cast<size_t>(b) * cap;
   const int warm = *s.warm;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
 
@@ -208,17 +194,113 @@ __global__ void __launch_bounds__(kThreads) alerts_kernel(const __grid_constant_
     __syncwarp();
   }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    int k = 0;
+  int k = 0;
+  if (threadIdx.x == 0)
     for (int a = 0; a < s.A; ++a)
-      if (fire[a]) fired[static_cast<size_t>(b) * kMaxA + k++] = a;
+      if (fire[a]) fired[k++] = a;
+  return k;
+}
+
+__global__ void __launch_bounds__(kThreads) alerts_kernel(const __grid_constant__ AlJobs jt, const AlSlot* __restrict__ slots,
+                                                          const double* __restrict__ preds, const uint8_t* __restrict__ flags,
+                                                          int cap, const int* __restrict__ ev_counts,
+                                                          const int* __restrict__ ev_status, int* __restrict__ fired,
+                                                          int* __restrict__ res, int B) {
+  __shared__ int fire[kMaxA];
+  const int b = blockIdx.x;
+  if (ev_status[b] != CC_EVENT_OK) {
+    if (threadIdx.x == 0) {
+      res[b] = 0;
+      res[B + b] = CC_ALERT_NOT_RUN;
+    }
+    return;
+  }
+  const int k = alerts_frame(fire, jt.j[b], slots, preds + static_cast<size_t>(b) * cap * 7, flags + static_cast<size_t>(b) * cap,
+                             ev_counts[b], fired + static_cast<size_t>(b) * kMaxA);
+  if (threadIdx.x == 0) {
     res[b] = k;
     res[B + b] = CC_ALERT_OK;
   }
 }
 
+// Runs (cc_ocsort_gpu_alerts_runs): job b's CTA applies the frames its events run completed, in order.  Per-frame clocks
+// and local times travel in the parameter block; a call with more frames is split into launches of at most kRunFrames.
+constexpr int kRunFrames = 1024;
+struct RunJob { int slot, frames, f0, row0; };
+struct AlRuns {
+  RunJob r[CC_MAX_FRAMES];
+  AlJob f[kRunFrames];                 // per frame: weekday, clock, time of day (slot unused)
+  int b0;                              // first job of this launch
+};
+
+// The slot state is read back frame after frame: no __restrict__ on `slots`, so none of it is loaded through the read-only
+// (non-coherent) path.
+__global__ void __launch_bounds__(kThreads) alerts_run_kernel(const __grid_constant__ AlRuns rt, const AlSlot* slots,
+                                                              int tmax, const double* __restrict__ preds, const uint8_t* __restrict__ flags,
+                                                              int cap, const int* __restrict__ ev_counts, const int* __restrict__ ev_done,
+                                                              int* __restrict__ fired, int* __restrict__ nfired, int* __restrict__ done,
+                                                              int* __restrict__ status) {
+  __shared__ int fire[kMaxA];
+  const RunJob run = rt.r[blockIdx.x];
+  const int b = rt.b0 + blockIdx.x;
+  const int frames = min(run.frames, ev_done[b]);
+  for (int f = 0; f < frames; ++f) {
+    const size_t bf = static_cast<size_t>(b) * tmax + f;
+    AlJob job = rt.f[run.f0 + f];
+    job.slot = run.slot;
+    const int k = alerts_frame(fire, job, slots, preds + bf * cap * 7, flags + bf * cap, ev_counts[bf], fired + bf * kMaxA);
+    if (threadIdx.x == 0) nfired[bf] = k;
+    __syncthreads();                   // the slot's rings, last_det and warm-up as this frame left them, for the next
+  }
+  if (threadIdx.x == 0) {
+    done[b] = frames;
+    status[b] = frames < run.frames ? CC_ALERT_NOT_RUN : CC_ALERT_OK;
+  }
+}
+
 struct DsJob { int slot, wday, row0, n; double now, tod; };
 struct DsJobs { DsJob j[CC_MAX_FRAMES]; };
+
+// The similarities of rows row0..row0+n-1 of emb against every alert of slot s (a warp per pair, NaN for alerts without
+// a description) into sim.
+__device__ __forceinline__ void describe_sims(const AlSlot& s, const float* __restrict__ emb, int dim, int row0, int n,
+                                              float* __restrict__ sim) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int pairs = n * s.A;
+  for (int p = w; p < pairs; p += kWarps) {
+    const int r = p / s.A, a = p - r * s.A;
+    float* out = sim + static_cast<size_t>(row0 + r) * kMaxA + a;
+    if (!(s.al[a].flags & CC_ALERT_DESC)) {
+      if (lane == 0) *out = __int_as_float(0x7fc00000);                  // NaN: no description
+      continue;
+    }
+    const float* e = emb + static_cast<size_t>(row0 + r) * dim;
+    const float* q = s.desc + static_cast<size_t>(a) * dim;
+    double acc = 0.;
+    for (int k = lane; k < dim; k += 32) acc += static_cast<double>(e[k]) * static_cast<double>(q[k]);
+    for (int o = 16; o >= 1; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if (lane == 0) *out = static_cast<float>(acc);
+  }
+}
+
+// Thread 0: rows row0..row0+n-1 in order at clock `now` with act[a] = description alert a is active: the cooldown and the
+// first match per row (clip_latest_img :1293-1307) -> hit.
+__device__ __forceinline__ void describe_match(const AlSlot& s, const int* act, double now, int row0, int n, const float* __restrict__ sim,
+                                               int* __restrict__ hit) {
+  for (int r = 0; r < n; ++r) {
+    int h = -1;
+    for (int a = 0; a < s.A; ++a) {
+      if (now - s.last[a] < kDescCooldown || !act[a]) continue;
+      const double v = sim[static_cast<size_t>(row0 + r) * kMaxA + a];
+      if (v > s.al[a].threshold) {
+        s.last[a] = now;
+        h = a;
+        break;
+      }
+    }
+    hit[row0 + r] = h;
+  }
+}
 
 __global__ void __launch_bounds__(kThreads) describe_kernel(const __grid_constant__ DsJobs jt, const AlSlot* __restrict__ slots,
                                                             const float* __restrict__ emb, int dim, int* __restrict__ hit,
@@ -226,38 +308,37 @@ __global__ void __launch_bounds__(kThreads) describe_kernel(const __grid_constan
   __shared__ int act[kMaxA];
   const DsJob job = jt.j[blockIdx.x];
   const AlSlot& s = slots[job.slot];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   for (int a = threadIdx.x; a < s.A; a += kThreads)
     act[a] = (s.al[a].flags & CC_ALERT_DESC) && is_active(s.al[a], s.on, job.tod, job.wday);
-  const int pairs = job.n * s.A;
-  for (int p = w; p < pairs; p += kWarps) {
-    const int r = p / s.A, a = p - r * s.A;
-    float* out = sim + static_cast<size_t>(job.row0 + r) * kMaxA + a;
-    if (!(s.al[a].flags & CC_ALERT_DESC)) {
-      if (lane == 0) *out = __int_as_float(0x7fc00000);                  // NaN: no description
-      continue;
-    }
-    const float* e = emb + static_cast<size_t>(job.row0 + r) * dim;
-    const float* q = s.desc + static_cast<size_t>(a) * dim;
-    double acc = 0.;
-    for (int k = lane; k < dim; k += 32) acc += static_cast<double>(e[k]) * static_cast<double>(q[k]);
-    for (int o = 16; o >= 1; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if (lane == 0) *out = static_cast<float>(acc);
-  }
+  describe_sims(s, emb, dim, job.row0, job.n, sim);
+  __syncthreads();
+  if (threadIdx.x == 0) describe_match(s, act, job.now, job.row0, job.n, sim, hit);
+}
+
+// Runs (cc_ocsort_gpu_describe_runs): job b's rows are its frames' saves in frame order; after the similarities, thread
+// 0 matches frame after frame, each at its own clock and local time.
+struct DsFrame { int n, wday; double now, tod; };
+struct DsRuns {
+  RunJob r[CC_MAX_FRAMES];
+  DsFrame f[kRunFrames];
+};
+
+__global__ void __launch_bounds__(kThreads) describe_run_kernel(const __grid_constant__ DsRuns rt, const AlSlot* slots,
+                                                                const float* __restrict__ emb, int dim, int* __restrict__ hit,
+                                                                float* __restrict__ sim) {
+  __shared__ int act[kMaxA];
+  const RunJob run = rt.r[blockIdx.x];
+  const AlSlot& s = slots[run.slot];
+  int n = 0;
+  for (int f = 0; f < run.frames; ++f) n += rt.f[run.f0 + f].n;
+  describe_sims(s, emb, dim, run.row0, n, sim);
   __syncthreads();
   if (threadIdx.x != 0) return;
-  for (int r = 0; r < job.n; ++r) {
-    int h = -1;
-    for (int a = 0; a < s.A; ++a) {
-      if (job.now - s.last[a] < kDescCooldown || !act[a]) continue;
-      const double v = sim[static_cast<size_t>(job.row0 + r) * kMaxA + a];
-      if (v > s.al[a].threshold) {
-        s.last[a] = job.now;
-        h = a;
-        break;
-      }
-    }
-    hit[job.row0 + r] = h;
+  for (int f = 0, r0 = run.row0; f < run.frames; ++f) {
+    const DsFrame fr = rt.f[run.f0 + f];
+    for (int a = 0; a < s.A; ++a) act[a] = (s.al[a].flags & CC_ALERT_DESC) && is_active(s.al[a], s.on, fr.tod, fr.wday);
+    describe_match(s, act, fr.now, r0, fr.n, sim, hit);
+    r0 += fr.n;
   }
 }
 
@@ -502,6 +583,92 @@ int cc_ocsort_gpu_describe(cc_ocsort_gpu* h, const int* slots, const int* rows, 
   }
   describe_kernel<<<B, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(jt, h->al->d_slot, d_emb, dim, d_hit, d_sim);
   CC_CHECK_CUDA(cudaGetLastError());
+  return CC_OK;
+}
+
+int cc_ocsort_gpu_alerts_runs(cc_ocsort_gpu* h, const cc_track_run* runs, int B, int frames_max, const double* now, const double* local,
+                              const double* d_preds, const uint8_t* d_flags, int cap, const int* d_ev_counts, const int* d_ev_done,
+                              int* d_fired, int* d_nfired, int* d_done, int* d_status, void* stream) {
+  CC_REQUIRE(h && runs && now && local && d_preds && d_flags && d_ev_counts && d_ev_done && d_fired && d_nfired && d_done && d_status,
+             "cc_ocsort_gpu_alerts_runs: NULL argument");
+  CC_REQUIRE(B >= 1 && B <= CC_MAX_FRAMES && frames_max >= 1 && frames_max <= CC_MAX_FRAMES,
+             "cc_ocsort_gpu_alerts_runs: B %d, frames_max %d (1..%d)", B, frames_max, CC_MAX_FRAMES);
+  CC_REQUIRE(cap >= 0, "cc_ocsort_gpu_alerts_runs: capacity %d", cap);
+  static thread_local std::vector<char> seen;
+  seen.assign(h->S, 0);
+  int f0 = 0;
+  for (int b = 0; b < B; ++b) {
+    const int s = runs[b].slot, T = runs[b].frames;
+    CC_REQUIRE(s >= 0 && s < h->S && alerts_active(h, s), "cc_ocsort_gpu_alerts_runs: run %d: slot %d has no alerts configured", b, s);
+    CC_REQUIRE(!seen[s], "cc_ocsort_gpu_alerts_runs: run %d: slot %d appears twice", b, s);
+    CC_REQUIRE(T >= 1 && T <= frames_max, "cc_ocsort_gpu_alerts_runs: run %d: %d frames (1..%d)", b, T, frames_max);
+    for (int f = f0; f < f0 + T; ++f) {
+      const int r = check_local("cc_ocsort_gpu_alerts_runs", f, now, local);
+      if (r != CC_OK) return r;
+    }
+    seen[s] = 1;
+    f0 += T;
+  }
+  static thread_local AlRuns rt;
+  for (int b = 0, f = 0; b < B;) {
+    int nb = 0, nf = 0;
+    rt.b0 = b;
+    while (b + nb < B && nf + runs[b + nb].frames <= kRunFrames) {
+      const cc_track_run& r = runs[b + nb];
+      rt.r[nb] = RunJob{r.slot, r.frames, nf, 0};
+      for (int k = 0; k < r.frames; ++k, ++f) rt.f[nf + k] = AlJob{0, static_cast<int>(local[2 * f + 1]), now[f], local[2 * f]};
+      nf += r.frames;
+      ++nb;
+    }
+    alerts_run_kernel<<<nb, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(rt, h->al->d_slot, frames_max, d_preds, d_flags, cap,
+                                                                               d_ev_counts, d_ev_done, d_fired, d_nfired, d_done, d_status);
+    CC_CHECK_CUDA(cudaGetLastError());
+    b += nb;
+  }
+  return CC_OK;
+}
+
+int cc_ocsort_gpu_describe_runs(cc_ocsort_gpu* h, const int* slots, const int* frames, int B, const int* rows, const double* now,
+                                const double* local, const float* d_emb, int dim, int* d_hit, float* d_sim, void* stream) {
+  CC_REQUIRE(h && slots && frames && rows && now && local && d_emb && d_hit && d_sim, "cc_ocsort_gpu_describe_runs: NULL argument");
+  CC_REQUIRE(B >= 1 && B <= CC_MAX_FRAMES, "cc_ocsort_gpu_describe_runs: B %d (1..%d)", B, CC_MAX_FRAMES);
+  CC_REQUIRE(dim >= 1 && dim <= 4096, "cc_ocsort_gpu_describe_runs: embedding width %d (1..4096)", dim);
+  static thread_local std::vector<char> seen;
+  seen.assign(h->S, 0);
+  int f0 = 0;
+  for (int b = 0; b < B; ++b) {
+    const int s = slots[b];
+    CC_REQUIRE(s >= 0 && s < h->S && alerts_active(h, s), "cc_ocsort_gpu_describe_runs: job %d: slot %d has no alerts configured", b, s);
+    CC_REQUIRE(!seen[s], "cc_ocsort_gpu_describe_runs: job %d: slot %d appears twice", b, s);
+    CC_REQUIRE(frames[b] >= 1 && frames[b] <= CC_MAX_FRAMES, "cc_ocsort_gpu_describe_runs: job %d: %d frames (1..%d)", b, frames[b],
+               CC_MAX_FRAMES);
+    const AlSlot& al = h->al->slot[s];
+    CC_REQUIRE(al.dim == 0 || al.dim == dim, "cc_ocsort_gpu_describe_runs: job %d: embeddings of width %d, descriptions of %d", b, dim,
+               al.dim);
+    for (int f = f0; f < f0 + frames[b]; ++f) {
+      CC_REQUIRE(rows[f] >= 0 && rows[f] <= (1 << 20), "cc_ocsort_gpu_describe_runs: job %d frame %d: %d rows", b, f - f0, rows[f]);
+      const int r = check_local("cc_ocsort_gpu_describe_runs", f, now, local);
+      if (r != CC_OK) return r;
+    }
+    seen[s] = 1;
+    f0 += frames[b];
+  }
+  static thread_local DsRuns rt;
+  for (int b = 0, f = 0, row0 = 0; b < B;) {
+    int nb = 0, nf = 0;
+    while (b + nb < B && nf + frames[b + nb] <= kRunFrames) {
+      rt.r[nb] = RunJob{slots[b + nb], frames[b + nb], nf, row0};
+      for (int k = 0; k < frames[b + nb]; ++k, ++f) {
+        rt.f[nf + k] = DsFrame{rows[f], static_cast<int>(local[2 * f + 1]), now[f], local[2 * f]};
+        row0 += rows[f];
+      }
+      nf += frames[b + nb];
+      ++nb;
+    }
+    describe_run_kernel<<<nb, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(rt, h->al->d_slot, d_emb, dim, d_hit, d_sim);
+    CC_CHECK_CUDA(cudaGetLastError());
+    b += nb;
+  }
   return CC_OK;
 }
 

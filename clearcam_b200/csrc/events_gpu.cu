@@ -192,29 +192,17 @@ __device__ Decision decide(const View& v, const Smem& sm, int i, int fl0, double
   return d;
 }
 
-__global__ void __launch_bounds__(kThreads) events_kernel(const __grid_constant__ EvJobs jt, const ocsg::SlotCfg* __restrict__ tcfg,
-                                                          const ocsg::SlotCnt* __restrict__ tcnt, const EvCfg* __restrict__ ecfgs,
-                                                          EvCnt* __restrict__ ecnts, const double* __restrict__ trk_out, int trk_cap,
-                                                          const int* __restrict__ trk_count, const int* __restrict__ trk_status,
-                                                          double* __restrict__ preds, uint8_t* __restrict__ flags,
-                                                          long long* __restrict__ saves, int cap, int* __restrict__ counts,
-                                                          int* __restrict__ status, int B) {
-  __shared__ Smem sm;
-  const int b = blockIdx.x;
-  const EvJob job = jt.j[b];
-  auto finish = [&](int st, int n_preds, int n_saves) {
-    if (threadIdx.x == 0) {
-      counts[b] = n_preds;
-      counts[B + b] = n_saves;
-      status[b] = st;
-    }
-  };
-  if (trk_status[b] != CC_TRACK_OK) return finish(CC_EVENT_NOT_RUN, 0, 0);
+struct EvOut { int status, n_preds, n_saves; };
+
+// One step of slot job.slot's events (the whole CTA) on one frame's tracker rows trk [n,9], with the tracker's live ids
+// lane [T] (ascending) after that frame; outputs into po [cap,7], fo [cap], so [cap,6].  Returns (uniform) the status and
+// the row counts (for NEEDS_ROOM, n_preds = the capacity needed).
+__device__ __forceinline__ EvOut events_frame(Smem& sm, const EvJob job, const EvCfg* ecfgs, EvCnt* ecnts,
+                                              const double* __restrict__ trk, int n, const int32_t* __restrict__ lane, int T,
+                                              double* __restrict__ po, uint8_t* __restrict__ fo, long long* __restrict__ so) {
+  auto finish = [&](int st, int n_preds, int n_saves) { return EvOut{st, n_preds, n_saves}; };
   const EvCfg* cfg = ecfgs + job.slot;
-  const View v{trk_out + static_cast<size_t>(b) * trk_cap * 9, trk_count[b], cfg, job.W, job.H, job.now};
-  const int T = tcnt[job.slot].T;
-  const ocsg::SlotCfg tc = tcfg[job.slot];
-  const int32_t* lane = tc.il + static_cast<size_t>(ocsg::kLaneId) * tc.cap;
+  const View v{trk, n, cfg, job.W, job.H, job.now};
   const int nv = cfg->nv;
   for (int k = threadIdx.x; k < nv; k += kThreads) {
     sm.zx[k] = cfg->zone[2 * k] * static_cast<double>(job.W);
@@ -274,9 +262,6 @@ __global__ void __launch_bounds__(kThreads) events_kernel(const __grid_constant_
 
   // ---- outputs in target order: preds rows with their flags, and the saves
   int np_ = 0, ns_ = 0;
-  double* po = preds + static_cast<size_t>(b) * cap * 7;
-  uint8_t* fo = flags + static_cast<size_t>(b) * cap;
-  long long* so = saves + static_cast<size_t>(b) * cap * 6;
   for (int c0 = 0; c0 < v.n; c0 += kThreads) {
     const int i = c0 + threadIdx.x;
     Decision d;
@@ -308,7 +293,79 @@ __global__ void __launch_bounds__(kThreads) events_kernel(const __grid_constant_
   }
   __syncthreads();
   if (threadIdx.x == 0) ecnts[job.slot] = EvCnt{need, 1 - ec.which};
-  finish(CC_EVENT_OK, np_, ns_);
+  return finish(CC_EVENT_OK, np_, ns_);
+}
+
+__global__ void __launch_bounds__(kThreads) events_kernel(const __grid_constant__ EvJobs jt, const ocsg::SlotCfg* __restrict__ tcfg,
+                                                          const ocsg::SlotCnt* __restrict__ tcnt, const EvCfg* __restrict__ ecfgs,
+                                                          EvCnt* __restrict__ ecnts, const double* __restrict__ trk_out, int trk_cap,
+                                                          const int* __restrict__ trk_count, const int* __restrict__ trk_status,
+                                                          double* __restrict__ preds, uint8_t* __restrict__ flags,
+                                                          long long* __restrict__ saves, int cap, int* __restrict__ counts,
+                                                          int* __restrict__ status, int B) {
+  __shared__ Smem sm;
+  const int b = blockIdx.x;
+  const EvJob job = jt.j[b];
+  auto finish = [&](const EvOut& r) {
+    if (threadIdx.x == 0) {
+      counts[b] = r.n_preds;
+      counts[B + b] = r.n_saves;
+      status[b] = r.status;
+    }
+  };
+  if (trk_status[b] != CC_TRACK_OK) return finish(EvOut{CC_EVENT_NOT_RUN, 0, 0});
+  const ocsg::SlotCfg tc = tcfg[job.slot];
+  finish(events_frame(sm, job, ecfgs, ecnts, trk_out + static_cast<size_t>(b) * trk_cap * 9, trk_count[b],
+                      tc.il + static_cast<size_t>(ocsg::kLaneId) * tc.cap, tcnt[job.slot].T, preds + static_cast<size_t>(b) * cap * 7,
+                      flags + static_cast<size_t>(b) * cap, saves + static_cast<size_t>(b) * cap * 6));
+}
+
+// Runs (cc_ocsort_gpu_events_runs): job b's CTA applies the frames its tracker run completed, in order, each on that
+// frame's tracker rows and live ids, and stops at the first frame whose status is not OK.  Per-frame picture sizes and
+// clocks travel in the parameter block; a call with more frames is split into launches of at most kRunFrames.
+constexpr int kRunFrames = 1024;
+struct EvRun { int slot, frames, f0, pad; };
+struct EvFrame { int W, H; double now; };
+struct EvRuns {
+  EvRun r[CC_MAX_FRAMES];
+  EvFrame f[kRunFrames];
+  int b0;                              // first job of this launch
+};
+
+// The slot's entries are read back frame after frame: no __restrict__ on `ecfgs` / `ecnts`, so none of them is loaded
+// through the read-only (non-coherent) path.
+__global__ void __launch_bounds__(kThreads) events_run_kernel(const __grid_constant__ EvRuns rt, const EvCfg* ecfgs,
+                                                              EvCnt* ecnts, int tmax, const double* __restrict__ trk_out,
+                                                              int trk_cap, const int* __restrict__ trk_count,
+                                                              const int32_t* __restrict__ trk_ids, int id_cap,
+                                                              const int* __restrict__ trk_live, const int* __restrict__ trk_done,
+                                                              double* __restrict__ preds, uint8_t* __restrict__ flags,
+                                                              long long* __restrict__ saves, int cap, int* __restrict__ counts,
+                                                              int* __restrict__ done, int* __restrict__ status, int B) {
+  __shared__ Smem sm;
+  const EvRun run = rt.r[blockIdx.x];
+  const int b = rt.b0 + blockIdx.x;
+  const int frames = min(run.frames, trk_done[b]);
+  int f = 0, st = CC_EVENT_OK;
+  for (; f < frames; ++f) {
+    const size_t bf = static_cast<size_t>(b) * tmax + f;
+    const EvFrame fr = rt.f[run.f0 + f];
+    const EvOut r = events_frame(sm, EvJob{run.slot, fr.W, fr.H, 0, fr.now}, ecfgs, ecnts, trk_out + bf * trk_cap * 9, trk_count[bf],
+                                 trk_ids + bf * id_cap, trk_live[bf], preds + bf * cap * 7, flags + bf * cap, saves + bf * cap * 6);
+    if (threadIdx.x == 0) {
+      counts[bf] = r.n_preds;
+      counts[static_cast<size_t>(B) * tmax + bf] = r.n_saves;
+    }
+    if (r.status != CC_EVENT_OK) {
+      st = r.status;
+      break;
+    }
+    __syncthreads();                   // the slot's entries as this frame left them, for the next
+  }
+  if (threadIdx.x == 0) {
+    done[b] = f;
+    status[b] = st == CC_EVENT_OK && f < run.frames ? CC_EVENT_NOT_RUN : st;
+  }
 }
 
 }  // namespace
@@ -468,6 +525,55 @@ int cc_ocsort_gpu_events(cc_ocsort_gpu* h, const cc_track_job* jobs, int B, cons
       jt, h->d_cfg, h->d_cnt, h->ev->d_cfg, h->ev->d_cnt, d_trk_out, trk_cap, d_trk_count, d_trk_status, d_preds, d_flags,
       reinterpret_cast<long long*>(d_saves), cap, d_counts, d_status, B);
   CC_CHECK_CUDA(cudaGetLastError());
+  return CC_OK;
+}
+
+int cc_ocsort_gpu_events_runs(cc_ocsort_gpu* h, const cc_track_run* runs, int B, int frames_max, const int* frame_wh, const double* now,
+                              const double* d_trk_out, int trk_cap, const int* d_trk_count, const int32_t* d_trk_ids, int id_cap,
+                              const int* d_trk_live, const int* d_trk_done, double* d_preds, uint8_t* d_flags, int64_t* d_saves, int cap,
+                              int* d_counts, int* d_done, int* d_status, void* stream) {
+  CC_REQUIRE(h && runs && frame_wh && now && d_trk_out && d_trk_count && d_trk_ids && d_trk_live && d_trk_done && d_preds && d_flags &&
+                 d_saves && d_counts && d_done && d_status,
+             "cc_ocsort_gpu_events_runs: NULL argument");
+  CC_REQUIRE(B >= 1 && B <= CC_MAX_FRAMES && frames_max >= 1 && frames_max <= CC_MAX_FRAMES,
+             "cc_ocsort_gpu_events_runs: B %d, frames_max %d (1..%d)", B, frames_max, CC_MAX_FRAMES);
+  CC_REQUIRE(trk_cap >= 0 && cap >= trk_cap && id_cap >= 1, "cc_ocsort_gpu_events_runs: output capacity %d below the tracker's %d",
+             cap, trk_cap);
+  static thread_local std::vector<char> seen;
+  seen.assign(h->S, 0);
+  int f0 = 0;
+  for (int b = 0; b < B; ++b) {
+    const int s = runs[b].slot, T = runs[b].frames;
+    CC_REQUIRE(s >= 0 && s < h->S && h->cfg[s].active && events_active(h, s),
+               "cc_ocsort_gpu_events_runs: run %d: slot %d is not configured for tracking and events", b, s);
+    CC_REQUIRE(!seen[s], "cc_ocsort_gpu_events_runs: run %d: slot %d appears twice", b, s);
+    CC_REQUIRE(T >= 1 && T <= frames_max, "cc_ocsort_gpu_events_runs: run %d: %d frames (1..%d)", b, T, frames_max);
+    for (int f = f0; f < f0 + T; ++f) {
+      CC_REQUIRE(frame_wh[2 * f] >= 1 && frame_wh[2 * f + 1] >= 1, "cc_ocsort_gpu_events_runs: run %d frame %d: %d x %d", b, f - f0,
+                 frame_wh[2 * f], frame_wh[2 * f + 1]);
+      CC_REQUIRE(isfinite(now[f]), "cc_ocsort_gpu_events_runs: run %d frame %d: the clock is not finite", b, f - f0);
+    }
+    seen[s] = 1;
+    f0 += T;
+  }
+  // launches of consecutive runs with at most kRunFrames frames in all
+  static thread_local EvRuns rt;
+  for (int b = 0, f = 0; b < B;) {
+    int nb = 0, nf = 0;
+    rt.b0 = b;
+    while (b + nb < B && nf + runs[b + nb].frames <= kRunFrames) {
+      const cc_track_run& r = runs[b + nb];
+      rt.r[nb] = EvRun{r.slot, r.frames, nf, 0};
+      for (int k = 0; k < r.frames; ++k, ++f) rt.f[nf + k] = EvFrame{frame_wh[2 * f], frame_wh[2 * f + 1], now[f]};
+      nf += r.frames;
+      ++nb;
+    }
+    events_run_kernel<<<nb, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        rt, h->ev->d_cfg, h->ev->d_cnt, frames_max, d_trk_out, trk_cap, d_trk_count, d_trk_ids, id_cap, d_trk_live, d_trk_done, d_preds,
+        d_flags, reinterpret_cast<long long*>(d_saves), cap, d_counts, d_done, d_status, B);
+    CC_CHECK_CUDA(cudaGetLastError());
+    b += nb;
+  }
   return CC_OK;
 }
 

@@ -393,18 +393,17 @@ __device__ void compact_lanes(V* base, int cap, int lanes, const Tr& s, int firs
   }
 }
 
-// ------------------------------------------------------------------------------------------------- one camera per CTA
-__global__ void __launch_bounds__(kThreads) ocsort_step_kernel(const __grid_constant__ JobTable jt, const SlotCfg* __restrict__ cfgs,
-                                                               SlotCnt* __restrict__ cnts, int rb, double* __restrict__ out,
-                                                               int cap_out, int* __restrict__ count, int* __restrict__ status) {
-  __shared__ Smem sm;
-  const cc_track_job job = jt.j[blockIdx.x];
-  const SlotCfg cfg = cfgs[job.slot];
-  const SlotCnt cnt = cnts[job.slot];
+// ------------------------------------------------------------------------------------------------- one frame of one camera
+struct Step { int count, status; };
+
+// One frame of slot `slot` (cc_ocsort_update's step) on rows [n,6] by the whole CTA: output rows into o [cap_out,9].
+// Returns (uniform) the row count (or the capacity needed, for NEEDS_ROOM) and the status.
+__device__ __forceinline__ Step ocsort_frame(Smem& sm, const float* rows, int n, float thr, int slot, const SlotCfg* cfgs,
+                                             SlotCnt* cnts, int rb, double* __restrict__ o, int cap_out) {
+  const SlotCfg cfg = cfgs[slot];
+  const SlotCnt cnt = cnts[slot];
   const Tr s{cfg.dl, cfg.il, cfg.cap, lane_keep(rb)};
-  const int T = cnt.T, n = job.n, delta_t = cfg.delta_t;
-  const float thr = job.det_thresh;
-  const float* rows = job.d_rows;
+  const int T = cnt.T, delta_t = cfg.delta_t;
   const double th = cfg.iou_threshold;
 
   // ---- split the detections by threshold; class ids are checked before anything changes
@@ -420,14 +419,8 @@ __global__ void __launch_bounds__(kThreads) ocsort_step_kernel(const __grid_cons
     const int pl = chunk_scan(sm, lo, &NS);
     if (lo) sm.sec[pl] = i;
   }
-  if (__syncthreads_or(bad)) {
-    if (threadIdx.x == 0) { count[blockIdx.x] = 0; status[blockIdx.x] = CC_TRACK_BAD_CLASS; }
-    return;
-  }
-  if (T + D > cfg.cap) {
-    if (threadIdx.x == 0) { count[blockIdx.x] = T + D; status[blockIdx.x] = CC_TRACK_NEEDS_ROOM; }
-    return;
-  }
+  if (__syncthreads_or(bad)) return Step{0, CC_TRACK_BAD_CLASS};
+  if (T + D > cfg.cap) return Step{T + D, CC_TRACK_NEEDS_ROOM};
   const int frame_count = cnt.frame_count + 1;
 
   // ---- predict (ocsort.py:143-155); the cost's anchor and the last observation are read before any update
@@ -614,7 +607,6 @@ __global__ void __launch_bounds__(kThreads) ocsort_step_kernel(const __grid_cons
     const int t = c0 + threadIdx.x;
     E += __syncthreads_count(t < T2 && emits(t));
   }
-  double* o = out + static_cast<size_t>(blockIdx.x) * cap_out * 9;
   int e = 0, kept = 0;
   for (int c0 = 0; c0 < T2; c0 += kThreads) {
     const int t = c0 + threadIdx.x;
@@ -656,10 +648,72 @@ __global__ void __launch_bounds__(kThreads) ocsort_step_kernel(const __grid_cons
     compact_lanes(cfg.dl, cfg.cap, D_KEEP, s, first, T2);
     compact_lanes(cfg.il, cfg.cap, lane_keep(rb), s, first, T2);
   }
+  if (threadIdx.x == 0) cnts[slot] = SlotCnt{kept, frame_count, cnt.next_id + nud, 0};
+  return Step{E, E > cap_out ? CC_TRACK_OVERFLOW : CC_TRACK_OK};
+}
+
+// ------------------------------------------------------------------------------------------------- one camera per CTA
+__global__ void __launch_bounds__(kThreads) ocsort_step_kernel(const __grid_constant__ JobTable jt, const SlotCfg* __restrict__ cfgs,
+                                                               SlotCnt* __restrict__ cnts, int rb, double* __restrict__ out,
+                                                               int cap_out, int* __restrict__ count, int* __restrict__ status) {
+  __shared__ Smem sm;
+  const cc_track_job job = jt.j[blockIdx.x];
+  const Step r = ocsort_frame(sm, job.d_rows, job.n, job.det_thresh, job.slot, cfgs, cnts, rb,
+                              out + static_cast<size_t>(blockIdx.x) * cap_out * 9, cap_out);
   if (threadIdx.x == 0) {
-    cnts[job.slot] = SlotCnt{kept, frame_count, cnt.next_id + nud, 0};
-    count[blockIdx.x] = E;
-    status[blockIdx.x] = E > cap_out ? CC_TRACK_OVERFLOW : CC_TRACK_OK;
+    count[blockIdx.x] = r.count;
+    status[blockIdx.x] = r.status;
+  }
+}
+
+// A run: the CTA applies frames 0..frames-1 of its camera in order and stops at the first frame whose status is not OK.
+// Frame f of job b writes row b * tmax + f of out [B,tmax,cap_out,9], count, live [B,tmax] and ids [B,tmax,id_cap].
+struct RunTable { cc_track_run r[CC_MAX_FRAMES]; };
+
+// The slot's lanes are read back frame after frame: no __restrict__ on `cfgs` / `cnts`, so none of them is loaded through
+// the read-only (non-coherent) path.
+__global__ void __launch_bounds__(kThreads) ocsort_run_kernel(const __grid_constant__ RunTable rt, const SlotCfg* cfgs, SlotCnt* cnts, int rb, int tmax, double* __restrict__ out,
+                                                              int cap_out, int* __restrict__ count, int32_t* __restrict__ ids, int id_cap,
+                                                              int* __restrict__ live, int* __restrict__ done, int* __restrict__ status) {
+  __shared__ Smem sm;
+  const cc_track_run run = rt.r[blockIdx.x];
+  int f = 0, st = CC_TRACK_OK;
+#pragma unroll 1
+  for (; f < run.frames; ++f) {
+    const size_t bf = static_cast<size_t>(blockIdx.x) * tmax + f;
+    double* o = out + bf * cap_out * 9;
+    const Step r = ocsort_frame(sm, run.d_rows + static_cast<size_t>(f) * run.n * 6, run.n, run.det_thresh, run.slot, cfgs, cnts, rb,
+                                o, cap_out);
+    __syncthreads();                   // the slot's counters and lanes as this frame left them
+    const SlotCfg& cfg = cfgs[run.slot];
+    const int T = cnts[run.slot].T;
+    const int32_t* lane = cfg.il + static_cast<size_t>(I_ID) * cfg.cap;
+    for (int t = threadIdx.x; t < T; t += kThreads) ids[bf * id_cap + t] = lane[t];
+    if (threadIdx.x == 0) {
+      count[bf] = r.count;
+      live[bf] = T;
+    }
+    if (r.status != CC_TRACK_OK) {
+      st = r.status;
+      break;
+    }
+    // A target box the events would reject (not finite, or beyond 2^60): end the run after this frame, so that the events
+    // stop the camera exactly here, as after a single-frame step, rather than behind a tracker that went on.
+    bool bad = false;
+    for (int i = threadIdx.x; i < r.count; i += kThreads) {
+      const double* q = o + static_cast<size_t>(i) * 9;
+      const double v[6] = {q[0], q[1], q[2], q[3], q[0] + q[2], q[1] + q[3]};
+      for (int k = 0; k < 6; ++k) bad |= !(fabs(v[k]) < 1152921504606846976.);
+    }
+    if (__syncthreads_or(bad)) {
+      st = CC_TRACK_BAD_BOX;
+      ++f;
+      break;
+    }
+  }
+  if (threadIdx.x == 0) {
+    done[blockIdx.x] = f;
+    status[blockIdx.x] = st;
   }
 }
 
@@ -822,6 +876,34 @@ int cc_ocsort_gpu_update(cc_ocsort_gpu* h, const cc_track_job* jobs, int B, doub
   }
   ocsort_step_kernel<<<B, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(jt, h->d_cfg, h->d_cnt, h->rb, d_out, cap, d_count,
                                                                               d_status);
+  CC_CHECK_CUDA(cudaGetLastError());
+  return CC_OK;
+}
+
+int cc_ocsort_gpu_update_runs(cc_ocsort_gpu* h, const cc_track_run* runs, int B, int frames_max, double* d_out, int cap, int* d_count,
+                              int32_t* d_ids, int id_cap, int* d_live, int* d_done, int* d_status, void* stream) {
+  CC_REQUIRE(h && runs && d_out && d_count && d_ids && d_live && d_done && d_status, "cc_ocsort_gpu_update_runs: NULL argument");
+  CC_REQUIRE(B >= 1 && B <= CC_MAX_FRAMES && frames_max >= 1 && frames_max <= CC_MAX_FRAMES && cap >= 0 && id_cap >= 1,
+             "cc_ocsort_gpu_update_runs: bad arguments (B %d, frames_max %d, cap %d, id_cap %d)", B, frames_max, cap, id_cap);
+  static thread_local std::vector<char> seen;
+  seen.assign(h->S, 0);
+  RunTable rt;
+  for (int b = 0; b < B; ++b) {
+    const cc_track_run& r = runs[b];
+    CC_REQUIRE(r.slot >= 0 && r.slot < h->S && h->cfg[r.slot].active, "cc_ocsort_gpu_update_runs: run %d: slot %d is not configured",
+               b, r.slot);
+    CC_REQUIRE(!seen[r.slot], "cc_ocsort_gpu_update_runs: run %d: slot %d appears twice", b, r.slot);
+    CC_REQUIRE(r.n >= 0 && r.n <= CC_OCSORT_MAX_ROWS && (r.d_rows || r.n == 0),
+               "cc_ocsort_gpu_update_runs: run %d: %d rows at %p (0..%d rows, non-null)", b, r.n, static_cast<const void*>(r.d_rows),
+               CC_OCSORT_MAX_ROWS);
+    CC_REQUIRE(r.frames >= 1 && r.frames <= frames_max, "cc_ocsort_gpu_update_runs: run %d: %d frames (1..%d)", b, r.frames, frames_max);
+    CC_REQUIRE(h->cfg[r.slot].cap <= id_cap, "cc_ocsort_gpu_update_runs: run %d: slot capacity %d exceeds id_cap %d", b,
+               h->cfg[r.slot].cap, id_cap);
+    seen[r.slot] = 1;
+    rt.r[b] = r;
+  }
+  ocsort_run_kernel<<<B, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(rt, h->d_cfg, h->d_cnt, h->rb, frames_max, d_out, cap,
+                                                                             d_count, d_ids, id_cap, d_live, d_done, d_status);
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;
 }

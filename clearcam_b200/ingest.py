@@ -9,6 +9,8 @@ bytes object, wraps it in numpy, and the consumer copies it again before use (`f
   * `PipeReader`     the `frame_loop` thread: fill the mailbox from a byte stream, count short reads and reopen the stream
                      after more than five in a row (clearcam.py:407-412)
   * `CameraBatch.step_mailboxes` (cameras.py) takes every camera's unseen frame straight from its mailbox
+  * `VideoReader`    a recorded video: every frame in order (none dropped), in runs of consecutive frames for
+                     `CameraBatch.step_video`, filled on a thread into two alternating pinned run buffers
 
 Frames are bgr24 (`-pix_fmt bgr24`, H*W*3 bytes) or, with `FrameMailbox(h, w, pix_fmt="yuv420p")`, yuv420p
 (`-pix_fmt yuv420p`, H*W*3/2 bytes: half the pipe, pinned-memory and PCIe bytes, and no swscale conversion on the host;
@@ -16,9 +18,12 @@ the GPU converts them, see clearcam_b200/pixfmt.py).
 
 Spawning ffmpeg (and HLS recording, clearcam.py:310-371) stays with the caller: `PipeReader` takes any callable that
 returns a readable binary stream, e.g. `lambda: subprocess.Popen(cmd, stdout=subprocess.PIPE).stdout`."""
+import queue
 import threading
 import time
 from typing import Callable, Optional, Tuple
+
+import numpy as np
 
 import torch
 
@@ -131,3 +136,103 @@ class PipeReader(threading.Thread):
                 self._stop_evt.wait(self.retry_sleep)
         finally:
             self._close()
+
+
+class VideoReader:
+    """A recorded video read from a rawvideo byte stream (e.g. `ffmpeg -i video.mp4 -f rawvideo -pix_fmt bgr24 -`) in runs of
+    up to `run` frames.  Unlike FrameMailbox nothing is dropped: frames come in order.  With every=2 the first frame of each
+    pair is skipped and the second kept (0-based frames 1, 3, 5, ...), as the reference's `grab()` + `read()` per step
+    does (clearcam.py:431-432).  A thread fills two alternating pinned run buffers; iterating yields (frames, positions):
+    frames a pinned uint8 view [n,H,W,3] (bgr24) or [n,H*3/2,W] (yuv420p), valid until the next run is asked for, and
+    positions the (n,) int64 CAP_PROP_POS_FRAMES of each frame (its 0-based index + 1), from which the caller computes
+    video time (pos / fps) and progress (pos / frame count).  The last run may be short; reading ends at the end of the
+    stream or at a short read (a partial last frame is dropped).  An exception raised while reading is raised by the
+    iteration, after the runs read before it.  `close()` (or leaving a `with` block) ends the thread of a reader the caller
+    stops using early."""
+
+    def __init__(self, stream, height: int, width: int, pix_fmt: str = BGR24, run: int = 32, every: int = 2, pin: Optional[bool] = None):
+        if run < 1 or every < 1:
+            raise ValueError("run and every must be >= 1")
+        self.height, self.width, self.pix_fmt = int(height), int(width), check_pix_fmt(pix_fmt)
+        shape = (self.height, self.width, 3) if self.pix_fmt == BGR24 else (yuv420p_rows(self.height, self.width), self.width)
+        self.frame_bytes = int(np.prod(shape))
+        pin = torch.cuda.is_available() if pin is None else pin
+        self._bufs = [torch.empty((run,) + shape, dtype=torch.uint8, pin_memory=pin) for _ in range(2)]
+        self._skip = bytearray(self.frame_bytes)
+        self.stream, self.run, self.every = stream, int(run), int(every)
+        self._free = queue.Queue()                    # buffer indices the reader may fill
+        self._full = queue.Queue()                    # (buffer, n, positions) runs, None at the end
+        self._free.put(0)
+        self._free.put(1)
+        self._held = None                             # buffer last handed to the consumer
+        self._stop = threading.Event()
+        self.error: Optional[BaseException] = None
+        self._thread = threading.Thread(target=self._read, daemon=True, name="video-reader")
+        self._thread.start()
+
+    def _fill(self, view) -> bool:
+        got = 0
+        while got < self.frame_bytes:
+            n = self.stream.readinto(view[got:])
+            if not n:
+                return False
+            got += n
+        return True
+
+    def _read(self):
+        index = 0                                     # frames read from the stream so far
+        try:
+            while True:
+                b = self._free.get()
+                if self._stop.is_set():
+                    break
+                views = memoryview(self._bufs[b].numpy()).cast("B")
+                pos, end = [], False
+                while len(pos) < self.run and not self._stop.is_set():
+                    for _ in range(self.every - 1):   # grab(): skipped
+                        if not self._fill(memoryview(self._skip)):
+                            end = True
+                            break
+                        index += 1
+                    if end or not self._fill(views[len(pos) * self.frame_bytes:(len(pos) + 1) * self.frame_bytes]):
+                        end = True
+                        break
+                    index += 1
+                    pos.append(index)
+                if pos:
+                    self._full.put((b, np.array(pos, np.int64)))
+                if end:
+                    break
+        except BaseException as ex:                   # reported to the consumer, which then ends
+            self.error = ex
+        finally:
+            self._full.put(None)
+
+    def __iter__(self):
+        return self
+
+    def __next__(self) -> Tuple[torch.Tensor, np.ndarray]:
+        if self._held is not None:                    # the previous run's buffer may be refilled now
+            self._free.put(self._held)
+            self._held = None
+        got = self._full.get()
+        if got is None:
+            self._full.put(None)
+            if self.error is not None:
+                raise self.error
+            raise StopIteration
+        b, pos = got
+        self._held = b
+        return self._bufs[b][:len(pos)], pos
+
+    def close(self):
+        """End the reader thread (a run in progress is dropped) and wait for it."""
+        self._stop.set()
+        self._free.put(-1)                            # wakes a thread waiting for a buffer
+        self._thread.join()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()

@@ -14,8 +14,8 @@ from typing import List, Optional, Sequence
 import numpy as np
 
 from .._lib import (CC_ALERT_DESC, CC_ALERT_MAX_ALERTS, CC_ALERT_OK, CC_ALERT_ON, CC_ALERT_SCHED, CC_ALERT_ZONE, CC_EVENT_BAD_BOX,
-                    CC_EVENT_BAD_ORDER, CC_EVENT_NEEDS_ROOM, CC_EVENT_OK, CC_TRACK_BAD_CLASS, CC_TRACK_NEEDS_ROOM, CC_TRACK_OVERFLOW,
-                    CCError, cc_alert, check, lib)
+                    CC_EVENT_BAD_ORDER, CC_EVENT_NEEDS_ROOM, CC_EVENT_OK, CC_TRACK_BAD_BOX, CC_TRACK_BAD_CLASS, CC_TRACK_NEEDS_ROOM, CC_TRACK_OK,
+                    CC_TRACK_OVERFLOW, CCError, cc_alert, cc_track_run, check, lib)
 from .STrack import STrack
 
 _CAP = 1024          # rows of the result buffer (the detector emits at most 300 boxes per frame)
@@ -59,6 +59,33 @@ def _cc_alert(a) -> cc_alert:
     r.threshold = float("inf") if a.threshold is None else a.threshold
     r.last_det = a.last_det
     return r
+
+
+class _Runs(list):
+    """The jobs of one DeviceTrackers.launch_runs: per job its per-frame events and alerts arguments, the frames read so far,
+    the errors, and the launch groups whose results are still to be read."""
+
+    def __init__(self, jobs, events, alerts):
+        super().__init__(jobs)
+        self.events, self.alerts = events, alerts
+        self.res = [[] for _ in jobs]
+        self.errors = {}
+        self.pending = []
+
+
+class _RunGroup:
+    """One launch per stage over up to CC_MAX_FRAMES runs.  items[b] = (job, first frame, carry): carry is None when the
+    tracker ran in this group, else (tracker status, capacity it needs) of the tracker launch whose rows the events rerun."""
+
+    def __init__(self, items):
+        self.items = items
+
+
+def _host(t):
+    """A pinned host copy of device tensor t, enqueued on the current stream."""
+    h = t.new_empty(tuple(t.shape), device="cpu", pin_memory=True)
+    h.copy_(t, non_blocking=True)
+    return h
 
 
 class _EventBuffers:
@@ -584,6 +611,233 @@ class DeviceTrackers:
             if pend or ev_pend:
                 self._torch.cuda.current_stream().synchronize()
         return res, evr, errors
+
+    # -- runs: several consecutive frames of one camera per job (a recorded video), one launch per stage
+    def launch_runs(self, jobs, events=None, alerts=None):
+        """Enqueue runs without waiting; pass the result to `finish_runs` after the stream is synchronised.  jobs: [(camera,
+        rows, det_thresh)] with rows a contiguous CUDA float32 [T,n,6] tensor (T consecutive frames, 1 <= T <= CC_MAX_FRAMES),
+        each camera at most once.  events: per job, a list of T (W, H, now), one per frame; alerts: per job, a list of T
+        (seconds of day, weekday).  Each camera's frames are applied in order, exactly as T `launch` calls would."""
+        from .._lib import CC_MAX_FRAMES
+        jobs = [(cam, rows, float(thr)) for cam, rows, thr in jobs]
+        if len({cam for cam, _, _ in jobs}) != len(jobs):
+            raise ValueError("each camera at most once per launch_runs")
+        for cam, rows, _ in jobs:
+            if cam not in self._slot:
+                raise KeyError(f"camera {cam!r} has no tracker: add() it first")
+            if (rows.dtype != self._torch.float32 or not rows.is_cuda or rows.dim() != 3 or rows.shape[2] != 6 or not rows.is_contiguous()
+                    or not 1 <= rows.shape[0] <= CC_MAX_FRAMES):
+                raise ValueError(f"camera {cam!r}: rows must be a contiguous CUDA float32 (T, n, 6) tensor, 1 <= T <= {CC_MAX_FRAMES}")
+        ev = al = None
+        if events is not None:
+            ev = [[(int(W), int(H), float(t)) for W, H, t in e] for e in events]
+            if len(ev) != len(jobs) or any(len(e) != rows.shape[0] for e, (_, rows, _) in zip(ev, jobs)):
+                raise ValueError("one (W, H, now) per frame of every job")
+            for cam, _, _ in jobs:
+                if cam not in self._ev:
+                    raise KeyError(f"camera {cam!r} has no events: events() it first")
+        if alerts is not None:
+            if ev is None:
+                raise ValueError("alerts run on the events' outputs: pass events= too")
+            al = [[(float(t), int(d)) for t, d in a] for a in alerts]
+            if len(al) != len(jobs) or any(len(a) != rows.shape[0] for a, (_, rows, _) in zip(al, jobs)):
+                raise ValueError("one (seconds of day, weekday) per frame of every job")
+            if not all(np.isfinite(t) and 0 <= d <= 6 for a in al for t, d in a):
+                raise ValueError("local time: a finite time of day and a weekday in 0..6")
+            for cam, _, _ in jobs:
+                self._need_alerts(cam)
+        run = _Runs(jobs, ev, al)
+        for c0 in range(0, len(jobs), self._B):
+            self._launch_runs(run, [(k, 0, None) for k in range(c0, min(len(jobs), c0 + self._B))])
+        return run
+
+    def _launch_runs(self, run, items, trk=None):
+        """One group: the tracker runs of items (job, first frame) — or, with trk (tracker rows, counts, ids, live, done of
+        an earlier launch, gathered per item), only the events — then the events and alerts behind them."""
+        torch = self._torch
+        g = _RunGroup(items)
+        B = len(items)
+        frames = [run[k][1].shape[0] - f0 for k, f0, _ in items]
+        Tm = max(frames)
+        dev = dict(device="cuda")
+        table = (cc_track_run * B)()
+        for b, (k, f0, _) in enumerate(items):
+            cam, rows, thr = run[k]
+            r = rows[f0:]
+            table[b] = cc_track_run(r.data_ptr() if r.shape[1] else None, r.shape[1], frames[b], self._slot[cam], thr)
+        if trk is None:
+            cap = max(1, max(run[k][1].shape[1] for k, _, _ in items))       # a frame emits at most one target per row
+            id_cap = max(self._cap[run[k][0]] for k, _, _ in items)
+            trk = (torch.empty((B, Tm, cap, 9), dtype=torch.float64, **dev), torch.empty((B, Tm), dtype=torch.int32, **dev),
+                   torch.empty((B, Tm, id_cap), dtype=torch.int32, **dev), torch.empty((B, Tm), dtype=torch.int32, **dev),
+                   torch.empty((2, B), dtype=torch.int32, **dev))
+            out, cnt, ids, live, ds = trk
+            check(lib().cc_ocsort_gpu_update_runs(self._h, table, B, Tm, out.data_ptr(), cap, cnt.data_ptr(), ids.data_ptr(), id_cap,
+                                                  live.data_ptr(), ds[0].data_ptr(), ds[1].data_ptr(), self._stream()),
+                  "cc_ocsort_gpu_update_runs")
+            g.hcnt, g.hds = _host(cnt), _host(ds)
+            if run.events is None:
+                g.hout = _host(out)
+        else:
+            g.avail = trk[4][0].tolist()                                       # tracker frames the gathered rows hold
+        g.trk = trk
+        out, cnt, ids, live, ds = trk
+        if run.events is not None:
+            cap = out.shape[2]
+            ev = [e for k, f0, _ in items for e in run.events[k][f0:]]
+            wh = np.array([(W, H) for W, H, _ in ev], np.int32).reshape(-1)
+            now = np.array([t for _, _, t in ev], np.float64)
+            preds = torch.empty((B, Tm, cap, 7), dtype=torch.float64, **dev)
+            flags = torch.empty((B, Tm, cap), dtype=torch.uint8, **dev)
+            saves = torch.empty((B, Tm, cap, 6), dtype=torch.int64, **dev)
+            ecnt = torch.empty((2, B, Tm), dtype=torch.int32, **dev)
+            eds = torch.empty((2, B), dtype=torch.int32, **dev)
+            check(lib().cc_ocsort_gpu_events_runs(self._h, table, B, Tm, wh.ctypes.data, now.ctypes.data, out.data_ptr(), cap, cnt.data_ptr(),
+                                                  ids.data_ptr(), ids.shape[2], live.data_ptr(), ds[0].data_ptr(), preds.data_ptr(),
+                                                  flags.data_ptr(), saves.data_ptr(), cap, ecnt.data_ptr(), eds[0].data_ptr(),
+                                                  eds[1].data_ptr(), self._stream()), "cc_ocsort_gpu_events_runs")
+            g.hev = tuple(_host(t) for t in (preds, flags, saves, ecnt, eds))
+            if run.alerts is not None:
+                loc = np.array([a for k, f0, _ in items for a in run.alerts[k][f0:]], np.float64).reshape(-1)
+                fired = torch.empty((B, Tm, CC_ALERT_MAX_ALERTS), dtype=torch.int32, **dev)
+                nf = torch.empty((B, Tm), dtype=torch.int32, **dev)
+                ads = torch.empty((2, B), dtype=torch.int32, **dev)
+                check(lib().cc_ocsort_gpu_alerts_runs(self._h, table, B, Tm, now.ctypes.data, loc.ctypes.data, preds.data_ptr(),
+                                                      flags.data_ptr(), cap, ecnt.data_ptr(), eds[0].data_ptr(), fired.data_ptr(),
+                                                      nf.data_ptr(), ads[0].data_ptr(), ads[1].data_ptr(), self._stream()),
+                      "cc_ocsort_gpu_alerts_runs")
+                g.hal = (_host(fired), _host(nf))
+        run.pending.append(g)
+
+    def finish_runs(self, run) -> list:
+        """The results of `launch_runs(jobs, ...)` once the stream has been synchronised: per camera a list with one entry
+        per frame — its targets, or with events (preds, flags, saves) as `finish_events` gives them, or with alerts (preds,
+        flags, saves, fired) as `finish_alerts`.  Trackers or event storage that lacked room are grown here and the run goes
+        on from the frame that stopped (more launches and waits).  A camera whose frame k failed (as `finish_events`
+        describes) keeps frames 0..k-1; after every other camera has finished its run, one CCError names every failed camera
+        and frame, and its `results` holds what each camera completed."""
+        from .._lib import CC_EVENT_NOT_RUN
+        torch = self._torch
+        while run.pending:
+            torch.cuda.current_stream().synchronize()
+            groups, run.pending = run.pending, []
+            full, again = [], []                     # (job, first frame): rerun everything / only the events from there
+            for g in groups:
+                for b, (k, f0, carry) in enumerate(g.items):
+                    cam, T = run[k][0], run[k][1].shape[0] - f0
+                    if carry is None:
+                        td, ts = int(g.hds[0, b]), int(g.hds[1, b])
+                        need = int(g.hcnt[b, td]) if td < T else 0
+                    else:
+                        td, (ts, need) = g.avail[b], carry
+                    if run.events is None:
+                        for f in range(td):
+                            n = int(g.hcnt[b, f])
+                            run.res[k].append(_tracks(g.hout[b, f, :n].numpy().copy(), n))
+                        stop = td
+                    else:
+                        p, fl, sv, ecnt, eds = g.hev
+                        ed, es = int(eds[0, b]), int(eds[1, b])
+                        for f in range(ed):
+                            n, m = int(ecnt[0, b, f]), int(ecnt[1, b, f])
+                            r = (p[b, f, :n].numpy().copy(), fl[b, f, :n].numpy().copy(), sv[b, f, :m].numpy().copy())
+                            if run.alerts is not None:
+                                r += (g.hal[0][b, f, :int(g.hal[1][b, f])].numpy().copy(),)
+                            run.res[k].append(r)
+                        stop = ed
+                        if es == CC_EVENT_NEEDS_ROOM:
+                            c = max(2 * self._ecap[cam], int(ecnt[0, b, ed]))
+                            check(lib().cc_ocsort_gpu_events_grow(self._h, self._slot[cam], c, self._stream()),
+                                  f"cc_ocsort_gpu_events_grow (camera {cam!r})")
+                            self._ecap[cam] = c
+                            again.append((k, f0 + ed, (g, b, ed, td, ts, need)))
+                            continue
+                        # the tracker run ends right after a frame with such a box (CC_TRACK_BAD_BOX), so here it has applied
+                        # exactly frames ..f0 + ed, as after a failing single-frame step
+                        if es == CC_EVENT_BAD_BOX:
+                            run.errors[k] = (f"camera {cam!r} frame {f0 + ed}: a target's box is not finite or beyond 2**60 (its events "
+                                             f"are unchanged; its tracker applied frame {f0 + td - 1} and stopped)")
+                            continue
+                        if es == CC_EVENT_BAD_ORDER:
+                            run.errors[k] = (f"camera {cam!r} frame {f0 + ed}: the tracker's ids are out of order (its events are "
+                                             f"unchanged; its tracker applied frame {f0 + td - 1} and stopped)")
+                            continue
+                        assert es in (CC_EVENT_OK, CC_EVENT_NOT_RUN)
+                    if ts == CC_TRACK_BAD_BOX:        # the events of that frame ran and passed: the run goes on
+                        full.append((k, f0 + stop, None))
+                    elif ts == CC_TRACK_NEEDS_ROOM:
+                        c = max(2 * self._cap[cam], need)
+                        check(lib().cc_ocsort_gpu_grow(self._h, self._slot[cam], c, self._stream()), f"cc_ocsort_gpu_grow (camera {cam!r})")
+                        self._cap[cam] = c
+                        full.append((k, f0 + stop, None))
+                    elif ts == CC_TRACK_BAD_CLASS:
+                        run.errors[k] = f"camera {cam!r} frame {f0 + stop}: a detection's class id is not an integer in 0..79 (its tracker is unchanged)"
+                    elif ts == CC_TRACK_OVERFLOW:
+                        run.errors[k] = f"camera {cam!r} frame {f0 + stop}: {need} tracks do not fit the output capacity (the frame was applied)"
+            # events that lacked room run again on the tracker rows of their frames (gathered before anything reuses them)
+            for c0 in range(0, len(again), self._B):
+                chunk = again[c0:c0 + self._B]
+                Tm = max(run[k][1].shape[0] - f for k, f, _ in chunk)
+                cap = max(src[0].trk[0].shape[2] for _, _, src in chunk)
+                id_cap = max(src[0].trk[2].shape[2] for _, _, src in chunk)
+                B = len(chunk)
+                trk = (torch.zeros((B, Tm, cap, 9), dtype=torch.float64, device="cuda"), torch.zeros((B, Tm), dtype=torch.int32, device="cuda"),
+                       torch.zeros((B, Tm, id_cap), dtype=torch.int32, device="cuda"), torch.zeros((B, Tm), dtype=torch.int32, device="cuda"))
+                for i, (_, _, (g, b, ed, td, _, _)) in enumerate(chunk):
+                    out, cnt, ids, live = g.trk[:4]
+                    trk[0][i, :td - ed, :out.shape[2]] = out[b, ed:td]
+                    trk[1][i, :td - ed] = cnt[b, ed:td]
+                    trk[2][i, :td - ed, :ids.shape[2]] = ids[b, ed:td]
+                    trk[3][i, :td - ed] = live[b, ed:td]
+                done = torch.tensor([[td - ed for _, _, (_, _, ed, td, _, _) in chunk], [0] * B], dtype=torch.int32)
+                self._launch_runs(run, [(k, f, (ts, need)) for k, f, (_, _, _, _, ts, need) in chunk], trk + (done.cuda(),))
+            for c0 in range(0, len(full), self._B):
+                self._launch_runs(run, full[c0:c0 + self._B])
+        if run.errors:
+            e = CCError("; ".join(run.errors[k] for k in sorted(run.errors)))
+            e.results = run.res
+            raise e
+        return run.res
+
+    def describe_runs(self, jobs, emb, now, local):
+        """`describe` for the saves of runs: jobs [(camera, rows per frame)], the rows of each job consecutive in emb (frame
+        after frame, job after job); now and local: per job, one clock and one (seconds of day, weekday) per frame.  Each
+        camera's frames are matched in order, each at its own clock -> per job (hits, similarities) over all its rows."""
+        torch = self._torch
+        if len(jobs) != len(now) or len(jobs) != len(local):
+            raise ValueError("one list of clocks and one of local times per job")
+        if not (isinstance(emb, torch.Tensor) and emb.is_cuda and emb.dtype == torch.float32 and emb.dim() == 2 and emb.is_contiguous()):
+            raise ValueError("emb must be a contiguous CUDA float32 [N, D] tensor")
+        counts = [[int(r) for r in rows] for _, rows in jobs]
+        if any(len(c) != len(t) or len(c) != len(l) for c, t, l in zip(counts, now, local)):
+            raise ValueError("one clock and one local time per frame")
+        n = sum(sum(c) for c in counts)
+        if n != emb.shape[0]:
+            raise ValueError(f"the jobs cover {n} rows, emb has {emb.shape[0]}")
+        for cam, _ in jobs:
+            self._need_alerts(cam)
+        hit = torch.empty(max(n, 1), dtype=torch.int32, device="cuda")
+        sim = torch.empty((max(n, 1), CC_ALERT_MAX_ALERTS), dtype=torch.float32, device="cuda")
+        r0 = 0
+        for c0 in range(0, len(jobs), self._B):
+            sl = slice(c0, c0 + self._B)
+            slots = np.array([self._slot[cam] for cam, _ in jobs[sl]], np.int32)
+            frames = np.array([len(c) for c in counts[sl]], np.int32)
+            rows = np.array([r for c in counts[sl] for r in c], np.int32)
+            t = np.array([float(x) for ts in now[sl] for x in ts], np.float64)
+            loc = np.array([(float(a), float(d)) for ls in local[sl] for a, d in ls], np.float64).reshape(-1)
+            check(lib().cc_ocsort_gpu_describe_runs(self._h, slots.ctypes.data, frames.ctypes.data, len(slots), rows.ctypes.data,
+                                                    t.ctypes.data, loc.ctypes.data, emb[r0:].data_ptr() if r0 < n else emb.data_ptr(),
+                                                    emb.shape[1], hit[r0:].data_ptr(), sim[r0:].data_ptr(), self._stream()),
+                  "cc_ocsort_gpu_describe_runs")
+            r0 += int(rows.sum())
+        h, s = hit.cpu().numpy(), sim.cpu().numpy()
+        out, r0 = [], 0
+        for (cam, _), c in zip(jobs, counts):
+            A, r = self._n_alerts[cam], sum(c)
+            out.append((h[r0:r0 + r].copy(), s[r0:r0 + r, :A].copy()))
+            r0 += r
+        return out
 
     def update(self, jobs) -> List[List[STrack]]:
         """jobs: [(camera, rows, det_thresh)] with rows a CUDA float32 (n,6) tensor; one camera at most once.  Returns each

@@ -466,6 +466,7 @@ typedef struct { const float* d_rows; int n; int slot; float det_thresh; int res
 #define CC_TRACK_NEEDS_ROOM 1
 #define CC_TRACK_BAD_CLASS 2
 #define CC_TRACK_OVERFLOW 3
+#define CC_TRACK_BAD_BOX 4              /* cc_ocsort_gpu_update_runs only */
 int cc_ocsort_gpu_create(int slots, int max_delta_t, cc_ocsort_gpu** out);
 int cc_ocsort_gpu_destroy(cc_ocsort_gpu* h);
 int cc_ocsort_gpu_configure(cc_ocsort_gpu* h, int slot, int max_age, int min_hits, double iou_threshold, int delta_t,
@@ -476,6 +477,26 @@ int cc_ocsort_gpu_capacity(cc_ocsort_gpu* h, int slot, int* capacity);
 int cc_ocsort_gpu_num_tracks(cc_ocsort_gpu* h, int slot, int* n, void* stream);
 int cc_ocsort_gpu_update(cc_ocsort_gpu* h, const cc_track_job* jobs, int B, double* d_out, int cap, int* d_count,
                          int* d_status, void* stream);
+
+/* Runs: several consecutive frames of one camera per job, e.g. a run of a recorded video, in one launch per stage.  Each
+ * job's CTA applies frames 0..frames-1 in order, exactly as that many cc_ocsort_gpu_update calls would, and stops at the
+ * first frame whose status is not CC_TRACK_OK.
+ * cc_track_run: device rows [frames,n,6] (frame f at d_rows + f*n*6; n <= CC_OCSORT_MAX_ROWS), frames 1..frames_max
+ * (frames_max <= CC_MAX_FRAMES), slot, det_thresh.
+ * cc_ocsort_gpu_update_runs: per job b and frame f, row b*frames_max + f of d_out [B,frames_max,cap,9], d_count
+ * [B,frames_max] (as cc_ocsort_gpu_update's d_out and d_count), d_live [B,frames_max] the live tracks after the frame and
+ * d_ids [B,frames_max,id_cap] their ids (slot order; what the events of that frame read), id_cap >= every job's slot
+ * capacity.  d_done[b] = frames applied with status OK, d_status[b] = the status of frame d_done[b] (CC_TRACK_OK when
+ * every frame was); its count, live and ids are written too.  NEEDS_ROOM and BAD_CLASS leave the slot as frame
+ * d_done[b] - 1 left it (grow, then run the rest from there); OVERFLOW applied that frame.  BAD_BOX: frame d_done[b] - 1
+ * was applied (status OK, counted in d_done) but one of its target boxes is not finite or beyond 2^60, which the
+ * events reject; the run stops after it so that its events run before the tracker goes on (run the rest from d_done[b]
+ * once they have).  Nothing is written past a
+ * job's last frame.  Bad arguments (as cc_ocsort_gpu_update, frames outside 1..frames_max, id_cap below a slot's
+ * capacity) fail with CC_ERR_INVALID before the launch.  A one-frame run gives what cc_ocsort_gpu_update gives. */
+typedef struct { const float* d_rows; int n; int frames; int slot; float det_thresh; } cc_track_run;
+int cc_ocsort_gpu_update_runs(cc_ocsort_gpu* h, const cc_track_run* runs, int B, int frames_max, double* d_out, int cap, int* d_count,
+                              int32_t* d_ids, int id_cap, int* d_live, int* d_done, int* d_status, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Object events on the tracker handle: what run_inference does with the targets (clearcam.py:586-621), per camera on the
@@ -518,6 +539,20 @@ int cc_ocsort_gpu_events(cc_ocsort_gpu* h, const cc_track_job* jobs, int B, cons
                          uint8_t* d_flags, int64_t* d_saves, int cap, int* d_counts, int* d_status, void* stream);
 
 int cc_ocsort_gpu_events_set_non_zone_alert(cc_ocsort_gpu* h, int slot, int non_zone_alert, void* stream);
+
+/* cc_ocsort_gpu_events_runs: the events of a cc_ocsort_gpu_update_runs call (same runs and frames_max; only .slot and
+ * .frames are read), queued after it: job b applies frames 0..d_trk_done[b]-1 in order, frame f on row b*frames_max+f of
+ * d_trk_out / d_trk_count / d_trk_ids / d_trk_live, for a picture of frame_wh[2i] x frame_wh[2i+1] at clock now[i], i the
+ * frame's index in the job-major list of every job's frames.  Outputs per frame at row b*frames_max+f: d_preds
+ * [B,frames_max,cap,7], d_flags [B,frames_max,cap], d_saves [B,frames_max,cap,6], d_counts [2,B,frames_max] (preds rows,
+ * save rows) as cc_ocsort_gpu_events writes them; d_done[b] frames applied, d_status[b] the CC_EVENT_* of frame d_done[b]
+ * (NOT_RUN when the tracker stopped there, OK when every frame was applied).  NEEDS_ROOM leaves the slot's entries as
+ * frame d_done[b]-1 left them: grow, then run the events again from that frame on the same tracker rows.  Bad arguments
+ * fail with CC_ERR_INVALID before anything is launched. */
+int cc_ocsort_gpu_events_runs(cc_ocsort_gpu* h, const cc_track_run* runs, int B, int frames_max, const int* frame_wh, const double* now,
+                              const double* d_trk_out, int trk_cap, const int* d_trk_count, const int32_t* d_trk_ids, int id_cap,
+                              const int* d_trk_live, const int* d_trk_done, double* d_preds, uint8_t* d_flags, int64_t* d_saves, int cap,
+                              int* d_counts, int* d_done, int* d_status, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Alerts on the tracker handle: the adds of run_inference (clearcam.py:612-620) behind the object events, the object
@@ -580,6 +615,21 @@ int cc_ocsort_gpu_alerts(cc_ocsort_gpu* h, const cc_track_job* jobs, int B, cons
                          int* d_fired, int* d_res, void* stream);
 int cc_ocsort_gpu_describe(cc_ocsort_gpu* h, const int* slots, const int* rows, int B, const double* now, const double* local,
                            const float* d_emb, int dim, int* d_hit, float* d_sim, void* stream);
+
+/* Runs.  cc_ocsort_gpu_alerts_runs: the alerts of a cc_ocsort_gpu_events_runs call (same runs and frames_max), queued
+ * after it: job b applies frames 0..d_ev_done[b]-1 in order, frame f on row b*frames_max+f of d_preds, d_flags and
+ * d_ev_counts [2,B,frames_max], at clock now[i] and local time local[2i..2i+1], i the frame's index in the job-major list.
+ * Outputs: d_fired [B,frames_max,CC_ALERT_MAX_ALERTS] and d_nfired [B,frames_max] per frame, d_done[b] frames applied,
+ * d_status[b] OK, or NOT_RUN when the events stopped before the last frame.
+ * cc_ocsort_gpu_describe_runs: job b matches the saves of frames[b] frames of slot slots[b]: rows[i] rows of d_emb for
+ * frame i of the job-major list (consecutive, frame after frame, job after job), frame i at clock now[i] and local time
+ * local[2i..2i+1].  The frames are matched in order, each row as cc_ocsort_gpu_describe would at its frame's clock; outputs
+ * per row as there.  Bad arguments fail with CC_ERR_INVALID before anything is launched. */
+int cc_ocsort_gpu_alerts_runs(cc_ocsort_gpu* h, const cc_track_run* runs, int B, int frames_max, const double* now, const double* local,
+                              const double* d_preds, const uint8_t* d_flags, int cap, const int* d_ev_counts, const int* d_ev_done,
+                              int* d_fired, int* d_nfired, int* d_done, int* d_status, void* stream);
+int cc_ocsort_gpu_describe_runs(cc_ocsort_gpu* h, const int* slots, const int* frames, int B, const int* rows, const double* now,
+                                const double* local, const float* d_emb, int dim, int* d_hit, float* d_sim, void* stream);
 
 #ifdef __cplusplus
 }
