@@ -25,6 +25,11 @@ class cc_frame(ctypes.Structure):
     _fields_ = [("data", ctypes.c_void_p), ("fmt", ctypes.c_int), ("h", ctypes.c_int), ("w", ctypes.c_int)]
 
 
+class cc_jpeg_dest(ctypes.Structure):
+    """One destination of cc_jpeg_decode_frames: device pointer, row pitch in bytes, height, width in pixels."""
+    _fields_ = [("data", ctypes.c_void_p), ("pitch", ctypes.c_int64), ("h", ctypes.c_int32), ("w", ctypes.c_int32)]
+
+
 class cc_track_job(ctypes.Structure):
     """One row of a tracker job table (cc_ocsort_gpu_update): device rows [n,6], their count, slot, threshold."""
     _fields_ = [("rows", ctypes.c_void_p), ("n", ctypes.c_int), ("slot", ctypes.c_int), ("det_thresh", ctypes.c_float),
@@ -179,6 +184,7 @@ _SIGS = {
     "cc_jpeg_table_bytes": (ctypes.c_size_t, []),
     "cc_jpeg_parse": (_i, [_vp, ctypes.c_int64, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "cc_jpeg_decode": (_i, [_vp, _vp, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t), _vp]),
+    "cc_jpeg_decode_frames": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t), _vp]),
     "cc_jpeg_crops_decoded": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, ctypes.c_size_t,
                                    ctypes.POINTER(ctypes.c_size_t), _vp]),
     "cc_jpeg_crops_decoded_frames": (_i, [_vp, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, ctypes.c_size_t,

@@ -18,7 +18,18 @@ the GPU right after the events (csrc/alerts_gpu.cu) for device rows and by `Came
 alert then does (image, notification, upload) and the saving of the picked crops stay with the caller.
 
 Each camera has a pixel format (clearcam_b200/pixfmt.py): "bgr24" [H,W,3] frames (the default) or "yuv420p" [H*3/2,W]
-frames, which the detector converts on the GPU.  Groups are keyed by (H, W, dtype, format).
+frames, which the detector converts on the GPU, or "mjpeg": one JPEG file per frame (bytes-like, e.g. a JpegMailbox
+view).  Groups are keyed by (H, W, dtype, format).
+
+An MJPEG camera's device frame is always cv2.imdecode of the file received, as bgr24, whichever side decodes it.  Each
+step has one decode stage ahead of the detector: every MJPEG frame of the step is gathered, with the Huffman tables its
+scan lacks (ingest.default_tables), into one pinned staging buffer and parsed in one call; the sizes place each picture
+in the step's shape and net-shape groups like any bgr24 frame; one host-to-device copy and one decode call
+(cc_jpeg_decode_frames) write the pixels straight into the buffers the detector reads (a camera's own buffer or a row
+of a uniform batch); the step then waits for the statuses.  Frames the parse or the device leaves to the host are
+decoded by cv2.imdecode and uploaded into their place; a frame cv2 also rejects is dropped for the step (the camera is
+not stepped and gets no result, its batch row is padding, `dropped_frames` counts it).  With host rows (no CUDA) every
+MJPEG frame is decoded by cv2.imdecode.
 
 With the detector's frame tables (a model with `net_shape` and `detect_frames`), uint8 groups whose frames letterbox to
 the same net input are merged: a fleet of 720p, 1080p, 1440p and 2160p cameras, bgr24 and yuv420p alike, runs as ONE
@@ -36,7 +47,7 @@ from ._lib import CC_MAX_FRAMES
 from .alerts import Alert, CameraAlerts, local_time
 from .events import ObjectEvents
 from .ocsort_tracker import ocsort
-from .pixfmt import BGR24, check_pix_fmt, yuv420p_size
+from .pixfmt import BGR24, MJPEG, check_camera_pix_fmt, yuv420p_size
 from .utils.helpers import batch_bucket
 from .ocsort_tracker.STrack import STrack
 
@@ -92,12 +103,15 @@ class CameraBatch:
         self._table_rows: Dict[tuple, torch.Tensor] = {}       # (net_h, net_w, chunk, bucket) -> pinned rows
         self._dev_trk: Optional[ocsort.DeviceTrackers] = None  # device trackers, made on the first step with device rows
         self._desc: Dict[str, np.ndarray] = {}                 # description text -> its CLIP text embedding (D,) float32
+        self._jpeg = None                                      # ops.JpegDecoder of the MJPEG cameras, made on first use
+        self.dropped_frames: Dict[Hashable, int] = {}          # MJPEG frames neither the GPU nor cv2 could decode, per camera
 
     # -- camera set (clearcam.py:207-240 init_cam; settings threshold :584, class filter :586)
     def add_camera(self, name, thresh: float = 0.5, classes=None, pix_fmt: str = BGR24):
-        """pix_fmt: the format of this camera's frames, "bgr24" [H,W,3] or "yuv420p" [H*3/2,W] (clearcam_b200/pixfmt.py)."""
+        """pix_fmt: the format of this camera's frames, "bgr24" [H,W,3], "yuv420p" [H*3/2,W] or "mjpeg" (one JPEG file per
+        frame) (clearcam_b200/pixfmt.py)."""
         self.cams[name] = _Camera(thresh or 0.5, None if classes is None else {int(c) for c in classes}, self.max_age,
-                                  check_pix_fmt(pix_fmt))
+                                  check_camera_pix_fmt(pix_fmt))
 
     def remove_camera(self, name):
         self.cams.pop(name, None)
@@ -107,6 +121,7 @@ class CameraBatch:
         self._cam_dev.pop(name, None)
         self._drop_run_frames(name, 0)
         self._seen.pop(name, None)             # a re-added camera starts a new mailbox whose frame_num restarts at 0
+        self.dropped_frames.pop(name, None)
 
     def _drop_run_frames(self, name, T):
         """Forget camera `name`'s per-frame device buffers of step_video (keys (name, f)) for frames f >= T."""
@@ -271,6 +286,8 @@ class CameraBatch:
             if f is None:
                 continue
             fmt = (pix_fmts or {}).get(name, BGR24)
+            if not hasattr(f, "dtype"):
+                raise ValueError(f"camera {name!r}: a {fmt} frame must be an array, got {type(f).__name__}")
             dt = {torch.uint8: "|u1", torch.float32: "<f4"}.get(f.dtype) if isinstance(f, torch.Tensor) else \
                 (f.dtype.str if f.dtype in (np.uint8, np.float32) else None)
             if fmt == BGR24:
@@ -327,58 +344,155 @@ class CameraBatch:
         pending = self._launch(frames)
         if self._pin:
             torch.cuda.current_stream().synchronize()
-        return {name: rows[i].numpy().copy() for names, rows, _ in pending for i, name in enumerate(names)}
+        return {name: rows[i].numpy().copy() for names, rows, _ in pending for i, name in enumerate(names) if name is not None}
 
-    def _launch(self, frames, fmts=None) -> list:
+    def _launch(self, frames, fmts=None, run=False) -> list:
         """Queue every detector call of `detect` and the copies of its rows to the host: [(cameras, host rows, detector
-        output)].  fmts: each frame's pixel format when the keys of `frames` are not camera names (its camera's by default)."""
+        output)], a camera None where its MJPEG frame was dropped.  fmts: each frame's pixel format when the keys of
+        `frames` are not camera names (its camera's by default).  run: the frames are a step_video run, in which a frame
+        that cannot be decoded raises ValueError."""
         pending = []
         if fmts is None:
             fmts = {name: cam.pix_fmt for name, cam in self.cams.items() if cam.pix_fmt != BGR24}
+        frames, fmts, jpeg, staged = self._stage_jpeg(frames, fmts, run)
         groups = self.group_by_shape(frames, fmts)
+        calls = []                             # placed first, so that MJPEG frames are decoded before any detector call
         for net, keys in self.merge_groups(groups):
             if len(keys) > 1:
-                pending += self._detect_table(net, [(name, key[3]) for key in keys for name in groups[key]], frames)
+                calls += self._detect_table(net, [(name, key[3]) for key in keys for name in groups[key]], frames, jpeg)
                 continue
             key = keys[0]
             names = groups[key]
             dev, rows = self._buffers(key, len(names))
             for i, name in enumerate(names):
+                self._where[name] = (dev, i)
+                if name in jpeg:
+                    jpeg[name] = dev[i]
+                    continue
                 f = frames[name]
                 dev[i].copy_(f if isinstance(f, torch.Tensor) else torch.from_numpy(f), non_blocking=True)
-                self._where[name] = (dev, i)
-            # bgr24 groups call detect_batch exactly as before the format existed (stand-in models need not know it)
-            out = self.model.detect_batch(dev) if key[3] == BGR24 else self.model.detect_batch(dev, pix_fmt=key[3])
-            rows.copy_(out, non_blocking=True)
-            pending.append((names, rows, out))
+
+            def call(names=names, dev=dev, rows=rows, fmt=key[3], dropped=()):
+                # bgr24 groups call detect_batch exactly as before the format existed (stand-in models need not know it)
+                out = self.model.detect_batch(dev) if fmt == BGR24 else self.model.detect_batch(dev, pix_fmt=fmt)
+                rows.copy_(out, non_blocking=True)
+                return [([None if n in dropped else n for n in names], rows, out)]
+            calls.append(call)
+        dropped = self._decode_jpeg(jpeg, staged, run) if jpeg else set()
+        for c in calls:
+            pending += c(dropped=dropped)
         return pending
 
-    def _detect_table(self, net, cams, frames) -> list:
-        """One detect_frames call per CC_MAX_FRAMES cameras of one net shape; cams: [(camera, pix_fmt)]."""
-        pending = []
+    def _stage_jpeg(self, frames, fmts, run):
+        """The first half of the decode stage (module doc): gather and parse every MJPEG frame -> (frames, formats, {frame
+        key: None}, (staged frame keys, their files)): MJPEG frames the GPU decodes become meta [H,W,3] placeholders and
+        the others cv2.imdecode's host pictures, all bgr24; frames cv2 rejects are left out (in a run: ValueError, before
+        anything is queued on the device)."""
+        keys = [k for k, f in frames.items() if f is not None and fmts.get(k) == MJPEG]
+        if not keys:
+            return frames, fmts, {}, None
+        frames, fmts = dict(frames), dict(fmts)
+        files = []
+        for k in keys:
+            f = frames[k]
+            if isinstance(f, torch.Tensor):
+                ok = f.dtype == torch.uint8 and f.dim() == 1 and not f.is_cuda
+            elif isinstance(f, np.ndarray):
+                ok = f.dtype == np.uint8 and f.ndim == 1
+            else:
+                ok = isinstance(f, (bytes, bytearray, memoryview))
+            if not ok:
+                raise ValueError(f"camera {k!r}: an mjpeg frame is one JPEG file (bytes-like or a 1-D uint8 host array)")
+            files.append(f.numpy() if isinstance(f, torch.Tensor) else f)
+            fmts[k] = BGR24
+        jpeg = {}
+        if self._pin:
+            from . import ops
+            from .ingest import default_tables
+            if self._jpeg is None:
+                self._jpeg = ops.JpegDecoder()
+            ins = [default_tables(f) for f in files]
+            sizes, status = self._jpeg.stage(files, [i if i[1] else None for i in ins])
+        for i, k in enumerate(keys):
+            if self._pin and status[i] == 0:
+                frames[k] = torch.empty((int(sizes[i, 1]), int(sizes[i, 0]), 3), dtype=torch.uint8, device="meta")
+                jpeg[k] = None
+                continue
+            img = self._imdecode(files[i])
+            if img is None:
+                self._drop(k, run)
+                del frames[k]
+            else:
+                frames[k] = img
+        return frames, fmts, jpeg, (keys, files)
+
+    @staticmethod
+    def _imdecode(f):
+        import cv2
+        a = f if isinstance(f, np.ndarray) else np.frombuffer(f, np.uint8)
+        return cv2.imdecode(a, cv2.IMREAD_COLOR) if len(a) else None
+
+    def _drop(self, key, run):
+        name = key[0] if run else key
+        if run:
+            raise ValueError(f"camera {name!r}: frame {key[1]} of the run is not a JPEG file cv2 can decode")
+        self.dropped_frames[name] = self.dropped_frames.get(name, 0) + 1
+        self._where.pop(name, None)
+
+    def _decode_jpeg(self, jpeg, staged, run) -> set:
+        """The second half of the decode stage: one decode into the placed buffers, the status wait, cv2 for the frames
+        the device left -> the frame keys dropped.  In a run, a frame cv2 rejects after the device did raises ValueError
+        here: the uploads and the decode are then queued, but no detector, tracker or event state has changed."""
+        keys, files = staged
+        dests = [jpeg.get(k) for k in keys]
+        status = self._jpeg.decode(dests)
+        torch.cuda.current_stream().synchronize()
+        dropped = set()
+        for i, k in enumerate(keys):
+            if dests[i] is None or int(status[i]) == 0:
+                continue
+            img = self._imdecode(files[i])
+            if img is None or tuple(img.shape) != tuple(dests[i].shape):
+                self._drop(k, run)
+                dropped.add(k)
+                continue
+            dests[i].copy_(torch.from_numpy(img))
+        return dropped
+
+    def _detect_table(self, net, cams, frames, jpeg) -> list:
+        """Place the frames of one net shape in their cameras' buffers (an MJPEG frame's buffer goes to `jpeg` for the
+        decode) -> one call per CC_MAX_FRAMES cameras, each queueing one detect_frames call; cams: [(camera, pix_fmt)]."""
+        calls = []
         for c0 in range(0, len(cams), CC_MAX_FRAMES):
             chunk = cams[c0:c0 + CC_MAX_FRAMES]
             devs = []
             for name, _ in chunk:
                 f = frames[name]
                 buf = self._camera_buffer(name, f)
-                buf.copy_(f if isinstance(f, torch.Tensor) else torch.from_numpy(f), non_blocking=True)
+                if name in jpeg:
+                    jpeg[name] = buf
+                else:
+                    buf.copy_(f if isinstance(f, torch.Tensor) else torch.from_numpy(f), non_blocking=True)
                 self._where[name] = (buf.unsqueeze(0), 0)
                 devs.append(buf)
-            b = self.bucket(len(chunk))
-            out = self.model.detect_frames(devs + [None] * (b - len(chunk)),
-                                           pix_fmts=[fmt for _, fmt in chunk] + [BGR24] * (b - len(chunk)))
-            k = tuple(net) + (c0 // CC_MAX_FRAMES, b)
-            if k not in self._table_rows:
-                self._table_rows[k] = torch.empty((b, 300, 6), dtype=torch.float32, pin_memory=self._pin)
-            rows = self._table_rows[k]
-            rows.copy_(out, non_blocking=True)
-            pending.append(([name for name, _ in chunk], rows, out))
-        return pending
+
+            def call(chunk=chunk, devs=devs, c0=c0, dropped=()):
+                names = [None if name in dropped else name for name, _ in chunk]
+                b = self.bucket(len(chunk))
+                out = self.model.detect_frames([d if n is not None else None for d, n in zip(devs, names)] + [None] * (b - len(chunk)),
+                                               pix_fmts=[fmt for _, fmt in chunk] + [BGR24] * (b - len(chunk)))
+                k = tuple(net) + (c0 // CC_MAX_FRAMES, b)
+                if k not in self._table_rows:
+                    self._table_rows[k] = torch.empty((b, 300, 6), dtype=torch.float32, pin_memory=self._pin)
+                rows = self._table_rows[k]
+                rows.copy_(out, non_blocking=True)
+                return [(names, rows, out)]
+            calls.append(call)
+        return calls
 
     def device_frame(self, name) -> torch.Tensor:
         """The device copy of the frame camera `name` contributed to the last detect()/step(), in the camera's own format
-        ([H,W,3] bgr24 or [H*3/2,W] yuv420p) — what the object crops for CLIP are cut from
+        ([H,W,3] bgr24 or [H*3/2,W] yuv420p; an MJPEG camera's is the bgr24 [H,W,3] picture of its file) — what the object crops for CLIP are cut from
         (ObjectFinder.embed_crops(..., pix_fmt=...)) without a second upload.  Valid until the next step."""
         dev, i = self._where[name]
         return dev[i]
@@ -411,7 +525,7 @@ class CameraBatch:
         frames = [self.device_frame(key) for _, key, _ in srcs]
         rects = np.concatenate([np.concatenate([np.full((len(sv), 1), j, np.int64), np.asarray(sv, np.int64)[:, 2:6]], 1)
                                 for j, (_, _, sv) in enumerate(srcs)]).astype(np.int32)
-        files, emb = finder.encode_embed_frames(frames, [self.cams[name].pix_fmt for name, _, _ in srcs], rects, quality)
+        files, emb = finder.encode_embed_frames(frames, [self._device_fmt(name) for name, _, _ in srcs], rects, quality)
         from .detection.yolov9 import DeviceResult
         k, first = 0, {}
         for name, _, sv in srcs:
@@ -478,7 +592,9 @@ class CameraBatch:
         clocks would return.  Every frame of every camera goes through the detector grouping of `step` (one detect_batch
         per shape, or frame tables of at most CC_MAX_FRAMES frames per net shape); device rows then run one launch per stage
         (tracker, events, alerts) for all cameras and one wait, host rows the host objects frame by frame.  A video camera
-        is a normal camera: `step` and `step_video` may alternate on it."""
+        is a normal camera: `step` and `step_video` may alternate on it.  An "mjpeg" camera's run is a list of JPEG files;
+        a file neither the GPU nor cv2 can decode raises ValueError before any detector call and leaves every camera's
+        tracker, events and alerts as they were (when the device found the fault, the decode had already been queued)."""
         flat, runs = {}, {}
         for name, fr in frames.items():
             if name not in self.cams:
@@ -496,10 +612,10 @@ class CameraBatch:
             for f in range(T):
                 flat[(name, f)] = fr[f]
         fmts = {(name, f): self.cams[name].pix_fmt for name, (T, _, _) in runs.items() for f in range(T)}
-        pending = self._launch(flat, fmts)
+        pending = self._launch(flat, fmts, run=True)
         for name, (T, _, _) in runs.items():
             self._drop_run_frames(name, T)     # buffers of a longer earlier run
-        size = {name: self._picture_size(name, frames[name][0]) for name in runs}
+        size = {name: self._picture_size(name, frames[name][0], (name, 0)) for name in runs}
         on_device = bool(pending) and all(isinstance(out, torch.Tensor) and out.is_cuda for _, _, out in pending)
         if on_device:
             if self._dev_trk is None:
@@ -513,7 +629,7 @@ class CameraBatch:
                                                  [lc for _, _, lc in runs.values()])
         if self._pin:
             torch.cuda.current_stream().synchronize()
-        det = {key: rows[i].numpy().copy() for keys, rows, _ in pending for i, key in enumerate(keys)}
+        det = {key: rows[i].numpy().copy() for keys, rows, _ in pending for i, key in enumerate(keys) if key is not None}
         res = {}
         if on_device:
             for n, per in zip(runs, self._dev_trk.finish_runs(launched)):
@@ -529,8 +645,14 @@ class CameraBatch:
                 res[n].append(CameraAlertResult(det[(n, f)], *ev, [cam.alert_ids[i] for i in fired]))
         return res
 
-    def _picture_size(self, name, f):
-        if self.cams[name].pix_fmt == BGR24:
+    def _device_fmt(self, name):
+        fmt = self.cams[name].pix_fmt
+        return BGR24 if fmt == MJPEG else fmt
+
+    def _picture_size(self, name, f, key=None):
+        if self.cams[name].pix_fmt == MJPEG:
+            f = self.device_frame(name if key is None else key)
+        if self._device_fmt(name) == BGR24:
             return int(f.shape[1]), int(f.shape[0])
         H, W = yuv420p_size(f.shape)
         return W, H
@@ -558,14 +680,15 @@ class CameraBatch:
                 self._dev_trk = ocsort.DeviceTrackers()
             for names, _, _ in pending:
                 for n in names:
-                    self._device_camera(n, now is not None, local is not None)
-            jobs = [(n, out[i], self.cams[n].thresh) for names, _, out in pending for i, n in enumerate(names)]
+                    if n is not None:
+                        self._device_camera(n, now is not None, local is not None)
+            jobs = [(n, out[i], self.cams[n].thresh) for names, _, out in pending for i, n in enumerate(names) if n is not None]
             launched = self._dev_trk.launch(jobs, None if now is None else
                                             [self._picture_size(n, frames[n]) + (now,) for n, _, _ in jobs],
                                             None if local is None else [local] * len(jobs))
         if self._pin:
             torch.cuda.current_stream().synchronize()
-        det = {name: rows[i].numpy().copy() for names, rows, _ in pending for i, name in enumerate(names)}
+        det = {name: rows[i].numpy().copy() for names, rows, _ in pending for i, name in enumerate(names) if name is not None}
         names = list(det)
         if not names:
             return {}

@@ -24,7 +24,8 @@
 //                 exclusive scan of the blocks completed per subsequence -> each subsequence's first block; too few blocks
 //                 -> corrupt
 //   9. write      from the synchronised states, every coefficient to its block (int16, zigzag; DC as a difference)
-//  10. dc         per interval (a warp): DC differences -> values per component
+//  10. dc         DC differences -> values per component: per chunk of 256 MCUs (a warp) the sums, then each chunk adds
+//                 the sums before it in its interval and scans its MCUs
 //  11. idct       per block: dequantise, islow IDCT, range limit -> the component's sample plane
 //  12. pixels     per output pixel: fancy upsampling of the chroma planes, YCbCr -> BGR into the padded batch
 // Kernels 11 and 12 also turn the encoder's quantised coefficients of object crops into the pixels of their JPEG files
@@ -52,6 +53,7 @@ constexpr int kChunk = 1024;            // scan bytes per CTA of the destuffing 
 constexpr int kSubBits = 256;           // bits per self-synchronising subsequence
 constexpr int kSyncCta = 128;           // subsequences per CTA of the sync kernels
 constexpr int kReconPerLaunch = 128;    // images per launch of the reconstruction kernels
+constexpr int kDcChunk = 256;           // MCUs per warp of the DC passes
 
 struct HuffDev {
   uint16_t look[512];                   // next 9 bits -> (length << 8) | symbol; length 0: the code is longer
@@ -91,8 +93,10 @@ struct JdecParams {
   unsigned long long* edge;             // [2][tiles] end state of each sync tile's last subsequence, by pass parity
   int32_t* flag;                        // [3] "a tile changed" per pass, by pass mod 3
   int32_t* bbase;                       // [slots] first block (relative to the image)
+  int32_t* dcsum;                       // [intervals][dc_chunks][3] DC difference sums per chunk of kDcChunk MCUs
   int16_t* coef;
   long long n_chunk, n_iv, n_slot;
+  int dc_chunks;                        // chunks of the longest interval
 };
 
 template <typename F>
@@ -476,23 +480,61 @@ __global__ void __launch_bounds__(kSyncCta) jdec_write_kernel(const __grid_const
   run<true>(im, b, nbytes, p.st[g], s.hi, s.end, done, err, p.coef + (im.blk0 + first) * 64, limit);
 }
 
-// warp per interval: DC differences -> values, per component; lane = MCU within a group of 32
-__global__ void jdec_dc_kernel(const __grid_constant__ JdecParams p) {
-  const long long gi = static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (gi >= p.n_iv) return;
-  const int k = find_image(p, gi, [](const JpegImage& t) { return t.iv0; });
+// DC differences -> values, per component, in two passes over chunks of kDcChunk MCUs of each interval (a warp per chunk,
+// grid x = interval, y * 8 + warp = chunk): the sums of each chunk's differences, then every chunk adds the sums of the
+// chunks before it in its interval and scans its own MCUs.  Integer sums: the values are those of one sequential walk.
+__device__ __forceinline__ bool dc_chunk(const JdecParams& p, int& k, int& j, int& m0, int& m1) {
+  const long long gi = blockIdx.x;
+  const int c = blockIdx.y * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (gi >= p.n_iv) return false;
+  k = find_image(p, gi, [](const JpegImage& t) { return t.iv0; });
   const JpegImage& im = p.tab[k];
-  const int j = static_cast<int>(gi - im.iv0);
-  if (j >= im.nint || p.status[k] != CC_JPEG_OK) return;
-  const int ri = im.ri ? im.ri : im.mcux * im.mcuy;
+  j = static_cast<int>(gi - im.iv0);
+  if (j >= im.nint || p.status[k] != CC_JPEG_OK) return false;
   const int nm = interval_blocks(im, j) / im.bpm;
-  int16_t* c0 = p.coef + (im.blk0 + static_cast<long long>(j) * ri * im.bpm) * 64;
+  m0 = c * kDcChunk;
+  m1 = min(nm, m0 + kDcChunk);
+  return m0 < nm;
+}
+
+__device__ __forceinline__ int16_t* dc_base(const JdecParams& p, const JpegImage& im, int j) {
+  const int ri = im.ri ? im.ri : im.mcux * im.mcuy;
+  return p.coef + (im.blk0 + static_cast<long long>(j) * ri * im.bpm) * 64;
+}
+
+__global__ void jdec_dc_sum_kernel(const __grid_constant__ JdecParams p) {
+  int k, j, m0, m1;
+  if (!dc_chunk(p, k, j, m0, m1)) return;
+  const JpegImage& im = p.tab[k];
+  const int16_t* c0 = dc_base(p, im, j);
+  const int lane = threadIdx.x & 31;
+  int sum[3] = {0, 0, 0};
+  for (int m = m0 + lane; m < m1; m += 32)
+    for (int bl = 0; bl < im.bpm; ++bl) sum[im.blk_comp[bl]] += c0[(static_cast<long long>(m) * im.bpm + bl) * 64];
+  for (int c = 0; c < 3; ++c)
+    for (int o = 16; o; o >>= 1) sum[c] += __shfl_xor_sync(~0u, sum[c], o);
+  if (lane == 0) {
+    int32_t* d = p.dcsum + (static_cast<long long>(blockIdx.x) * p.dc_chunks + m0 / kDcChunk) * 3;
+    d[0] = sum[0]; d[1] = sum[1]; d[2] = sum[2];
+  }
+}
+
+__global__ void jdec_dc_apply_kernel(const __grid_constant__ JdecParams p) {
+  int k, j, m0, m1;
+  if (!dc_chunk(p, k, j, m0, m1)) return;
+  const JpegImage& im = p.tab[k];
+  int16_t* c0 = dc_base(p, im, j);
+  const int lane = threadIdx.x & 31;
   int carry[3] = {0, 0, 0};
-  for (int m0 = 0; m0 < nm; m0 += 32) {
-    const int m = m0 + lane;
+  const int32_t* s = p.dcsum + static_cast<long long>(blockIdx.x) * p.dc_chunks * 3;
+  for (int q = lane; q < m0 / kDcChunk; q += 32)
+    for (int c = 0; c < 3; ++c) carry[c] += s[q * 3 + c];
+  for (int c = 0; c < 3; ++c)
+    for (int o = 16; o; o >>= 1) carry[c] += __shfl_xor_sync(~0u, carry[c], o);
+  for (int mb = m0; mb < m1; mb += 32) {
+    const int m = mb + lane;
     int sum[3] = {0, 0, 0};
-    if (m < nm)
+    if (m < m1)
       for (int bl = 0; bl < im.bpm; ++bl) sum[im.blk_comp[bl]] += c0[(static_cast<long long>(m) * im.bpm + bl) * 64];
     int ex[3];
     for (int c = 0; c < 3; ++c) {
@@ -500,7 +542,7 @@ __global__ void jdec_dc_kernel(const __grid_constant__ JdecParams p) {
       ex[c] = warp_excl(sum[c], lane, tot) + carry[c];
       carry[c] += tot;
     }
-    if (m < nm) {
+    if (m < m1) {
       for (int bl = 0; bl < im.bpm && bl < 6; ++bl) {
         int16_t* d = c0 + (static_cast<long long>(m) * im.bpm + bl) * 64;
         ex[im.blk_comp[bl]] += *d;
@@ -515,15 +557,16 @@ struct ReconImg {
   int k, w, h, ncomp, hs, vs, mcux, mcuy;
   long long blk0, plane0, bfirst;       // first block in the coefficients; plane bytes; first block of the launch group
   int qt[3];                            // element offset of each component's table in qbase
+  uint8_t* dst;                         // BGR pixel (0, 0) of the image's destination
+  long long pitch;                      // bytes between its rows
 };
 
 struct ReconParams {
   const int16_t* coef;
   uint8_t* planes;
-  uint8_t* out;
   int32_t* status;                      // per output slot; images not OK are skipped, the IDCT marks out-of-range ones
   const uint16_t* qbase;
-  int Hmax, Wmax, n;
+  int n;
   long long nblk;
   ReconImg img[kReconPerLaunch];
 };
@@ -632,7 +675,7 @@ __global__ void __launch_bounds__(256) jdec_pixels_kernel(const __grid_constant_
   long long off;
   plane_dims(r, 0, pw, ph, off);
   const int Y = p.planes[off + static_cast<long long>(y) * pw + x];
-  uint8_t* o = p.out + ((static_cast<long long>(r.k) * p.Hmax + y) * p.Wmax + x) * 3;
+  uint8_t* o = r.dst + static_cast<long long>(y) * r.pitch + x * 3;
   if (r.ncomp == 1) { o[0] = o[1] = o[2] = static_cast<uint8_t>(Y); return; }
   int ch[2];
   const int dw = (r.w + r.hs - 1) / r.hs, dh = (r.h + r.vs - 1) / r.vs;
@@ -912,7 +955,8 @@ void parse_one(const uint8_t* b, long long n, JpegImage& im) {
 // where each image's intermediates live in the workspace
 struct Layout {
   long long n_chunk = 0, n_iv = 0, n_slot = 0, n_blk = 0, dst = 0, planes = 0;
-  size_t chunk_kept, chunk_rst, dlen, dbuf, ivstart, subbase, st, en, cnt, err, edge, flag, bbase, coef, planesb, total;
+  int dc_chunks = 1;
+  size_t chunk_kept, chunk_rst, dlen, dbuf, ivstart, subbase, st, en, cnt, err, edge, flag, bbase, dcsum, coef, planesb, total;
 };
 
 Layout layout(const JpegImage* tab, int K, bool with_coef) {
@@ -926,6 +970,8 @@ Layout layout(const JpegImage* tab, int K, bool with_coef) {
     L.n_blk = std::max(L.n_blk, im.blk0 + static_cast<long long>(im.mcux) * im.mcuy * im.bpm);
     L.dst = std::max(L.dst, im.dst0 + im.scan_len);
     L.planes = std::max(L.planes, im.plane0 + plane_bytes(im.ncomp, im.hs, im.vs, im.mcux, im.mcuy));
+    const long long nmcu = static_cast<long long>(im.mcux) * im.mcuy, per_iv = im.ri ? std::min<long long>(im.ri, nmcu) : nmcu;
+    L.dc_chunks = std::max(L.dc_chunks, static_cast<int>((per_iv + kDcChunk - 1) / kDcChunk));
   }
   size_t off = 0;
   auto take = [&](size_t bytes) { const size_t o = off; off += align256(bytes); return o; };
@@ -936,6 +982,7 @@ Layout layout(const JpegImage* tab, int K, bool with_coef) {
   L.st = take(L.n_slot * 8); L.en = take(L.n_slot * 8);
   L.cnt = take(L.n_slot * 4); L.err = take(L.n_slot * 4); L.bbase = take(L.n_slot * 4);
   L.edge = take(2 * ((L.n_slot + kSyncCta - 1) / kSyncCta) * 8); L.flag = take(3 * 4);
+  L.dcsum = take(static_cast<size_t>(L.n_iv) * L.dc_chunks * 12);
   L.coef = with_coef ? take(L.n_blk * 128) : 0;
   L.planesb = take(L.planes);
   L.total = off;
@@ -988,28 +1035,11 @@ extern "C" int cc_jpeg_parse(const uint8_t* h_data, int64_t data_bytes, const in
   return CC_OK;
 }
 
-extern "C" int cc_jpeg_decode(const uint8_t* d_data, const void* h_table, const void* d_table, int K, uint8_t* d_out, int Hmax,
-                              int Wmax, int32_t* d_status, int16_t* d_coef, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
-                              void* stream) {
-  const char* who = "cc_jpeg_decode";
-  CC_REQUIRE(K >= 0 && (K == 0 || h_table), "%s: null table or K=%d < 0", who, K);
-  const JpegImage* tab = static_cast<const JpegImage*>(h_table);
-  const Layout L = layout(tab, K, d_coef == nullptr);
-  if (ws_needed) *ws_needed = L.total;
-  if (!d_out) return CC_OK;                           // workspace size query
-  CC_REQUIRE(d_data && d_table && d_status, "%s: d_data, d_table and d_status must not be NULL", who);
-  CC_REQUIRE(Hmax > 0 && Wmax > 0, "%s: bad batch size %dx%d", who, Hmax, Wmax);
-  CC_REQUIRE(d_workspace && ws_bytes >= L.total, "%s: workspace of %zu bytes too small (%zu needed)", who,
-             d_workspace ? ws_bytes : size_t(0), L.total);
-  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0 && (reinterpret_cast<uintptr_t>(d_table) & 15) == 0 &&
-                 (reinterpret_cast<uintptr_t>(d_coef) & 15) == 0,
-             "%s: d_workspace must be 256-byte aligned, d_table and d_coef 16-byte aligned", who);
-  for (int k = 0; k < K; ++k) {
-    CC_REQUIRE(tab[k].status >= CC_JPEG_OK && tab[k].status <= CC_JPEG_CORRUPT, "%s: table entry %d is not from cc_jpeg_parse", who,
-               k);
-    CC_REQUIRE(tab[k].status != CC_JPEG_OK || (tab[k].w <= Wmax && tab[k].h <= Hmax),
-               "%s: image %d (%dx%d) does not fit the %dx%d batch", who, k, tab[k].w, tab[k].h, Wmax, Hmax);
-  }
+// cc_jpeg_decode and cc_jpeg_decode_frames once their arguments are checked: image k (status OK) goes to dst[k], rows
+// pitch[k] bytes apart
+static int decode_checked(const uint8_t* d_data, const JpegImage* tab, const void* d_table, int K, const Layout& L,
+                          uint8_t* const* dst, const long long* pitch, int32_t* d_status, int16_t* d_coef, void* d_workspace,
+                          void* stream) {
   if (K == 0) return CC_OK;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
@@ -1028,6 +1058,8 @@ extern "C" int cc_jpeg_decode(const uint8_t* d_data, const void* h_table, const 
   p.edge = reinterpret_cast<unsigned long long*>(ws + L.edge);
   p.flag = reinterpret_cast<int32_t*>(ws + L.flag);
   p.bbase = reinterpret_cast<int32_t*>(ws + L.bbase);
+  p.dcsum = reinterpret_cast<int32_t*>(ws + L.dcsum);
+  p.dc_chunks = L.dc_chunks;
   p.coef = d_coef ? d_coef : reinterpret_cast<int16_t*>(ws + L.coef);
   p.n_chunk = L.n_chunk; p.n_iv = L.n_iv; p.n_slot = L.n_slot;
   jdec_status_kernel<<<(K + 255) / 256, 256, 0, st>>>(p);
@@ -1043,22 +1075,88 @@ extern "C" int cc_jpeg_decode(const uint8_t* d_data, const void* h_table, const 
     const unsigned giv = static_cast<unsigned>((L.n_iv + 7) / 8);
     jdec_counts_kernel<<<giv, 256, 0, st>>>(p);
     jdec_write_kernel<<<g, kSyncCta, 0, st>>>(p);
-    jdec_dc_kernel<<<giv, 256, 0, st>>>(p);
+    const dim3 gdc(static_cast<unsigned>(L.n_iv), static_cast<unsigned>((L.dc_chunks + 7) / 8));
+    jdec_dc_sum_kernel<<<gdc, 256, 0, st>>>(p);
+    jdec_dc_apply_kernel<<<gdc, 256, 0, st>>>(p);
   }
   CC_CHECK_CUDA(cudaGetLastError());
   static thread_local ReconParams rp;
-  rp.coef = p.coef; rp.planes = ws + L.planesb; rp.out = d_out; rp.status = d_status;
-  rp.qbase = reinterpret_cast<const uint16_t*>(d_table); rp.Hmax = Hmax; rp.Wmax = Wmax;
+  rp.coef = p.coef; rp.planes = ws + L.planesb; rp.status = d_status;
+  rp.qbase = reinterpret_cast<const uint16_t*>(d_table);
   std::vector<ReconImg> imgs;
   for (int k = 0; k < K; ++k) {
     const JpegImage& im = tab[k];
     if (im.status != CC_JPEG_OK) continue;
-    ReconImg r{k, im.w, im.h, im.ncomp, im.hs, im.vs, im.mcux, im.mcuy, im.blk0, im.plane0, 0, {0, 0, 0}};
+    ReconImg r{k, im.w, im.h, im.ncomp, im.hs, im.vs, im.mcux, im.mcuy, im.blk0, im.plane0, 0, {0, 0, 0}, dst[k], pitch[k]};
     for (int c = 0; c < 3; ++c)
       r.qt[c] = static_cast<int>((k * sizeof(JpegImage) + offsetof(JpegImage, qt) + c * 128) / 2);
     imgs.push_back(r);
   }
   return launch_recon(rp, imgs, st);
+}
+
+static int check_tables(const char* who, const JpegImage* tab, int K, const void* d_data, const void* d_table, const int32_t* d_status,
+                        const Layout& L, const void* d_workspace, size_t ws_bytes) {
+  CC_REQUIRE(d_data && d_table && d_status, "%s: d_data, d_table and d_status must not be NULL", who);
+  CC_REQUIRE(d_workspace && ws_bytes >= L.total, "%s: workspace of %zu bytes too small (%zu needed)", who,
+             d_workspace ? ws_bytes : size_t(0), L.total);
+  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0 && (reinterpret_cast<uintptr_t>(d_table) & 15) == 0,
+             "%s: d_workspace must be 256-byte aligned, d_table 16-byte aligned", who);
+  for (int k = 0; k < K; ++k)
+    CC_REQUIRE(tab[k].status >= CC_JPEG_OK && tab[k].status <= CC_JPEG_CORRUPT, "%s: table entry %d is not from cc_jpeg_parse", who,
+               k);
+  return CC_OK;
+}
+
+extern "C" int cc_jpeg_decode(const uint8_t* d_data, const void* h_table, const void* d_table, int K, uint8_t* d_out, int Hmax,
+                              int Wmax, int32_t* d_status, int16_t* d_coef, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
+                              void* stream) {
+  const char* who = "cc_jpeg_decode";
+  CC_REQUIRE(K >= 0 && (K == 0 || h_table), "%s: null table or K=%d < 0", who, K);
+  const JpegImage* tab = static_cast<const JpegImage*>(h_table);
+  const Layout L = layout(tab, K, d_coef == nullptr);
+  if (ws_needed) *ws_needed = L.total;
+  if (!d_out) return CC_OK;                           // workspace size query
+  CC_REQUIRE(Hmax > 0 && Wmax > 0, "%s: bad batch size %dx%d", who, Hmax, Wmax);
+  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_coef) & 15) == 0, "%s: d_coef must be 16-byte aligned", who);
+  if (int rc = check_tables(who, tab, K, d_data, d_table, d_status, L, d_workspace, ws_bytes)) return rc;
+  std::vector<uint8_t*> dst(K);
+  std::vector<long long> pitch(K, 3ll * Wmax);
+  for (int k = 0; k < K; ++k) {
+    CC_REQUIRE(tab[k].status != CC_JPEG_OK || (tab[k].w <= Wmax && tab[k].h <= Hmax),
+               "%s: image %d (%dx%d) does not fit the %dx%d batch", who, k, tab[k].w, tab[k].h, Wmax, Hmax);
+    dst[k] = d_out + static_cast<long long>(k) * Hmax * Wmax * 3;
+  }
+  return decode_checked(d_data, tab, d_table, K, L, dst.data(), pitch.data(), d_status, d_coef, d_workspace, stream);
+}
+
+extern "C" int cc_jpeg_decode_frames(const uint8_t* d_data, const void* h_table, const void* d_table, int K, const cc_jpeg_dest* outs,
+                                     int32_t* d_status, void* d_workspace, size_t ws_bytes, size_t* ws_needed, void* stream) {
+  const char* who = "cc_jpeg_decode_frames";
+  CC_REQUIRE(K >= 0 && (K == 0 || h_table), "%s: null table or K=%d < 0", who, K);
+  const JpegImage* tab = static_cast<const JpegImage*>(h_table);
+  const Layout L = layout(tab, K, true);
+  if (ws_needed) *ws_needed = L.total;
+  if (!outs) return CC_OK;                            // workspace size query
+  if (int rc = check_tables(who, tab, K, d_data, d_table, d_status, L, d_workspace, ws_bytes)) return rc;
+  std::vector<uint8_t*> dst(K);
+  std::vector<long long> pitch(K);
+  std::vector<std::pair<uintptr_t, uintptr_t>> spans;  // [first byte, end) of every destination the decode may write
+  for (int k = 0; k < K; ++k) {
+    const cc_jpeg_dest& o = outs[k];
+    dst[k] = static_cast<uint8_t*>(o.data); pitch[k] = o.pitch;
+    if (tab[k].status != CC_JPEG_OK) continue;
+    CC_REQUIRE(o.data && o.h == tab[k].h && o.w == tab[k].w, "%s: destination %d is %dx%d%s, the image %dx%d", who, k, o.w, o.h,
+               o.data ? "" : " at NULL", tab[k].w, tab[k].h);
+    CC_REQUIRE(o.pitch >= 3ll * o.w, "%s: destination %d has a pitch of %lld bytes, below 3 x %d", who, k,
+               static_cast<long long>(o.pitch), o.w);
+    const uintptr_t a = reinterpret_cast<uintptr_t>(o.data);
+    spans.emplace_back(a, a + static_cast<uintptr_t>((o.h - 1) * o.pitch + 3ll * o.w));
+  }
+  std::sort(spans.begin(), spans.end());
+  for (size_t i = 1; i < spans.size(); ++i)
+    CC_REQUIRE(spans[i].first >= spans[i - 1].second, "%s: two destinations overlap", who);
+  return decode_checked(d_data, tab, d_table, K, L, dst.data(), pitch.data(), d_status, nullptr, d_workspace, stream);
 }
 
 // cc_jpeg_crops_decoded from the point where the crops' sources, rects and quality are checked
@@ -1073,7 +1171,7 @@ static int crops_decoded_sources(const char* who, const CropSource* src, const i
     const int* r = rects + 5 * k;
     const int w = r[3] - r[1], h = r[4] - r[2];
     ReconImg& x = imgs[k];
-    x = ReconImg{k, w, h, 3, 2, 2, (w + 15) / 16, (h + 15) / 16, blk, plane, 0, {0, 64, 64}};
+    x = ReconImg{k, w, h, 3, 2, 2, (w + 15) / 16, (h + 15) / 16, blk, plane, 0, {0, 64, 64}, nullptr, 3ll * Wmax};
     blk += 6ll * x.mcux * x.mcuy;
     plane += static_cast<long long>(align256(plane_bytes(3, 2, 2, x.mcux, x.mcuy)));
   }
@@ -1090,6 +1188,7 @@ static int crops_decoded_sources(const char* who, const CropSource* src, const i
              d_workspace ? ws_bytes : size_t(0), need);
   CC_REQUIRE((reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0, "%s: d_workspace must be 256-byte aligned", who);
   if (K == 0) return CC_OK;
+  for (int k = 0; k < K; ++k) imgs[k].dst = d_out + static_cast<long long>(k) * Hmax * Wmax * 3;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
   // the quantisation tables travel at the head of the workspace: a kernel argument writes them, no host copy
@@ -1099,8 +1198,8 @@ static int crops_decoded_sources(const char* who, const CropSource* src, const i
   int16_t* coef = reinterpret_cast<int16_t*>(ws + 256);
   if (int rc = jpeg_coeffs_sources(src, rects, K, quality, coef, nullptr, st)) return rc;
   jdec_ok_kernel<<<(K + 255) / 256, 256, 0, st>>>(d_status, K);
-  rp.coef = coef; rp.planes = ws + 256 + coef_bytes; rp.out = d_out; rp.status = d_status;
-  rp.qbase = reinterpret_cast<const uint16_t*>(ws); rp.Hmax = Hmax; rp.Wmax = Wmax;
+  rp.coef = coef; rp.planes = ws + 256 + coef_bytes; rp.status = d_status;
+  rp.qbase = reinterpret_cast<const uint16_t*>(ws);
   QtArg qa;
   std::memcpy(qa.q, qt, sizeof(qt));
   jdec_put_qt_kernel<<<1, 128, 0, st>>>(qa, reinterpret_cast<uint16_t*>(ws));

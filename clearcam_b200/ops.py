@@ -463,6 +463,109 @@ class JpegBatch:
         return out, status[:self.K]
 
 
+class JpegDecoder:
+    """A reusable decode context for JPEG files that go to caller-given device destinations (cc_jpeg_decode_frames), e.g.
+    the frames of MJPEG cameras.  It owns a pinned staging buffer (the files' bytes, then the parse table), its device
+    copy, the device workspace and the statuses; each grows when a call needs more and is otherwise reused, so the steady
+    state allocates nothing.  One call sequence per batch: `stage` (host: gather and parse) -> `decode` (queued: one
+    host-to-device copy, the decode, the statuses back to pinned memory).  The staging buffer is rewritten by the next
+    `stage`, so the caller waits for the stream between batches."""
+
+    def __init__(self, device="cuda"):
+        import numpy as np
+        self.device = torch.device(device)
+        self._pin = self.device.type == "cuda"
+        self._tb = int(lib().cc_jpeg_table_bytes())
+        self._host = torch.empty(0, dtype=torch.uint8)
+        self._dev = self._ws = None
+        self._st_dev = self._st_host = None
+        self.K = 0
+        self.sizes = np.zeros((0, 2), np.int32)
+        self.status = np.zeros(0, np.int32)
+        self._nbytes = 0
+
+    @staticmethod
+    def _grow(t, n, **kw):
+        if t is not None and t.numel() >= n:
+            return t
+        return torch.empty(max(n, 256, 0 if t is None else t.numel() * 3 // 2), dtype=kw.pop("dtype", torch.uint8), **kw)
+
+    def stage(self, files, inserts=None):
+        """files: K JPEG files (bytes-like, or uint8 CPU tensors / arrays); inserts: None, or per file None or (offset,
+        bytes) to insert at that offset while gathering (ingest.default_tables).  Gathers them into the staging buffer
+        and parses them -> (sizes int32 [K,2] width, height; parse status int32 [K]), valid until the next `stage`."""
+        import numpy as np
+        arrs = []
+        for f in files:
+            if isinstance(f, torch.Tensor):
+                arrs.append(f.reshape(-1).numpy())
+            else:
+                arrs.append(f if isinstance(f, np.ndarray) else np.frombuffer(f, np.uint8))
+        inserts = inserts or [None] * len(arrs)
+        lengths = np.array([len(a) + (len(i[1]) if i else 0) for a, i in zip(arrs, inserts)], np.int64)
+        K = self.K = len(arrs)
+        offsets = np.zeros(K, np.int64)
+        if K:
+            offsets[1:] = np.cumsum(lengths)[:-1]
+        nbytes = int(lengths.sum())
+        self._table_off = (nbytes + 255) & ~255
+        self._nbytes = self._table_off + K * self._tb
+        self._host = self._grow(self._host, self._nbytes, pin_memory=self._pin)
+        h = self._host.numpy()
+        for a, ins, o in zip(arrs, inserts, offsets.tolist()):
+            if ins:
+                at, seg = ins
+                h[o:o + at] = a[:at]
+                h[o + at:o + at + len(seg)] = np.frombuffer(seg, np.uint8)
+                h[o + at + len(seg):o + len(a) + len(seg)] = a[at:]
+            else:
+                h[o:o + len(a)] = a
+        self.sizes = np.zeros((K, 2), np.int32)
+        self.status = np.zeros(K, np.int32)
+        blocks = np.zeros(K, np.int64)
+        base = self._host.data_ptr()
+        check(lib().cc_jpeg_parse(ctypes.c_void_p(base), nbytes, offsets.ctypes.data, lengths.ctypes.data, K,
+                                  ctypes.c_void_p(base + self._table_off), self.sizes.ctypes.data, self.status.ctypes.data,
+                                  blocks.ctypes.data), "cc_jpeg_parse")
+        self._files = (offsets, lengths)
+        return self.sizes, self.status
+
+    def file(self, k) -> memoryview:
+        """The bytes of staged file k as parsed (default tables inserted)."""
+        o, n = (int(x[k]) for x in self._files)
+        return memoryview(self._host.numpy()[o:o + n])
+
+    def decode(self, dests, stream=None) -> torch.Tensor:
+        """Queue the decode of the staged files: dests[k] is a device uint8 [h,w,3] tensor whose rows are contiguous
+        (a frame buffer, or a row of a batch), or None for a file the parse did not accept.  -> pinned int32 [K] statuses,
+        filled when the stream reaches this point (JPEG_OK: dests[k] holds cv2.imdecode of file k; otherwise dests[k] is
+        as it was)."""
+        from ._lib import cc_jpeg_dest
+        K = self.K
+        outs = (cc_jpeg_dest * max(K, 1))()
+        for k, d in enumerate(dests):
+            if d is None:
+                continue
+            assert d.is_cuda and d.dtype == torch.uint8 and d.dim() == 3 and d.shape[2] == 3 and d.stride(2) == 1 \
+                and d.stride(1) == 3, "a destination is a device uint8 [h, w, 3] tensor with contiguous rows"
+            outs[k] = cc_jpeg_dest(d.data_ptr(), d.stride(0), d.shape[0], d.shape[1])
+        self._dev = self._grow(self._dev, self._nbytes, device=self.device)
+        self._st_dev = self._grow(self._st_dev, K, dtype=torch.int32, device=self.device)
+        self._st_host = self._grow(self._st_host, K, dtype=torch.int32, pin_memory=self._pin)
+        base = self._dev.data_ptr()
+        h_table = ctypes.c_void_p(self._host.data_ptr() + self._table_off)
+        args = (ctypes.c_void_p(base), h_table, ctypes.c_void_p(base + self._table_off), K)
+        need = ctypes.c_size_t(0)
+        check(lib().cc_jpeg_decode_frames(*args, None, None, None, 0, ctypes.byref(need), None), "cc_jpeg_decode_frames")
+        self._ws = self._grow(self._ws, need.value, device=self.device)
+        self._dev[:self._nbytes].copy_(self._host[:self._nbytes], non_blocking=True)
+        check(lib().cc_jpeg_decode_frames(*args, outs, ptr(self._st_dev), ptr(self._ws), self._ws.numel(), None,
+                                          stream_ptr(stream)), "cc_jpeg_decode_frames")
+        st = self._st_host[:K]
+        st.copy_(self._st_dev[:K], non_blocking=True)
+        return st
+
+
 def jpeg_decode(files, out=None, stream=None):
     """files: list of `bytes` -> (out uint8 CUDA [K, Hmax, Wmax, 3] BGR, sizes int32 numpy [K, 2] (width, height), device int32
     status [K]).  Where status is JPEG_OK, out[k, :h, :w] is exactly cv2.imdecode(file, IMREAD_COLOR); JPEG_UNSUPPORTED and

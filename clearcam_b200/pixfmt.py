@@ -5,12 +5,17 @@
   * "yuv420p"  planar YUV 4:2:0 uint8 [H*3/2,W] per frame: the Y plane (H rows), then U and V ((H/2) x (W/2) each),
                contiguous.  H and W must be even.  What a camera's H.264/HEVC decodes to, half the bytes of bgr24; the
                GPU converts it exactly as cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_I420) does.
+  * "mjpeg"    a camera input format only (`CameraBatch.add_camera`, `ingest.JpegMailbox`, `ingest.VideoReader`): each
+               frame is one JPEG file (`-c:v copy -f mjpeg`).  The camera's device frame is the bgr24 [H,W,3] picture
+               cv2.imdecode gives for it, decoded on the GPU where it can be; the detector and the object crops see that
+               bgr24 frame.
 
 The format of a frame is always passed explicitly (`pix_fmt=`), never inferred from its shape."""
 from typing import Sequence, Tuple
 
-BGR24, YUV420P = "bgr24", "yuv420p"
+BGR24, YUV420P, MJPEG = "bgr24", "yuv420p", "mjpeg"
 PIX_FMTS = (BGR24, YUV420P)
+CAMERA_PIX_FMTS = PIX_FMTS + (MJPEG,)
 
 # frame_fmt codes of the C-ABI (include/clearcam_b200.h)
 CC_FRAME_BGR_U8, CC_FRAME_BGR_F32, CC_FRAME_I420_U8 = 0, 1, 2
@@ -19,6 +24,12 @@ CC_FRAME_BGR_U8, CC_FRAME_BGR_F32, CC_FRAME_I420_U8 = 0, 1, 2
 def check_pix_fmt(pix_fmt) -> str:
     if pix_fmt not in PIX_FMTS:
         raise ValueError(f"pix_fmt must be one of {PIX_FMTS}, got {pix_fmt!r}")
+    return pix_fmt
+
+
+def check_camera_pix_fmt(pix_fmt) -> str:
+    if pix_fmt not in CAMERA_PIX_FMTS:
+        raise ValueError(f"pix_fmt must be one of {CAMERA_PIX_FMTS}, got {pix_fmt!r}")
     return pix_fmt
 
 

@@ -408,6 +408,16 @@ int cc_jpeg_parse(const uint8_t* h_data, int64_t data_bytes, const int64_t* offs
                   int32_t* h_sizes, int32_t* h_status, int64_t* h_blocks);
 int cc_jpeg_decode(const uint8_t* d_data, const void* h_table, const void* d_table, int K, uint8_t* d_out, int Hmax, int Wmax,
                    int32_t* d_status, int16_t* d_coef, void* d_workspace, size_t ws_bytes, size_t* ws_needed, void* stream);
+/* cc_jpeg_decode_frames: cc_jpeg_decode into caller-given destinations rather than one padded batch, e.g. the device
+ * frame buffers a detector call reads.  outs (HOST [K], read during the call only): image k, when its status is OK, is
+ * written as BGR uint8 [h, w, 3] at outs[k].data (device), rows outs[k].pitch bytes apart; nothing else is written, and an
+ * image that fails on the device leaves its destination as it was.  Fails with CC_ERR_INVALID before any launch when the
+ * destination of a parsed image is NULL, its h x w is not the image's, its pitch is below 3 w, or two such destinations
+ * overlap; the destinations of images the parse did not accept are not read.  outs == NULL only writes *ws_needed.
+ * Statuses, workspace and stream as for cc_jpeg_decode. */
+typedef struct { void* data; int64_t pitch; int32_t h; int32_t w; } cc_jpeg_dest;
+int cc_jpeg_decode_frames(const uint8_t* d_data, const void* h_table, const void* d_table, int K, const cc_jpeg_dest* outs,
+                          int32_t* d_status, void* d_workspace, size_t ws_bytes, size_t* ws_needed, void* stream);
 int cc_jpeg_crops_decoded(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K, int quality,
                           uint8_t* d_out, int Hmax, int Wmax, int32_t* d_status, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
                           void* stream);
