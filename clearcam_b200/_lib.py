@@ -121,6 +121,14 @@ _SIGS = {
     "cc_clip_encode_text": (_i, [_vp, _vp, _i, _vp, ctypes.c_longlong, _vp]),
     "cc_clip_profile": (_i, [_vp, _i, _vp, _i, _vp, _i, ctypes.POINTER(_f), ctypes.POINTER(ctypes.c_double),
                              ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_i), ctypes.POINTER(ctypes.c_double), _vp]),
+    "cc_conv2d_prelu": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _i, _vp]),
+    "cc_face_create": (_i, [_i, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_vp), ctypes.POINTER(ctypes.c_int64),
+                            ctypes.POINTER(_vp)]),
+    "cc_face_destroy": (_i, [_vp]),
+    "cc_face_embed": (_i, [_vp, _vp, _i, _vp, ctypes.c_longlong, _vp]),
+    "cc_face_workspace_bytes": (_i, [_vp, _i, ctypes.POINTER(ctypes.c_size_t)]),
+    "cc_face_set_workspace": (_i, [_vp, _vp, ctypes.c_size_t]),
+    "cc_face_layer_output": (_i, [_vp, _vp, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
     "cc_search_scores": (_i, [_vp, _i, _i, _vp, _i, _vp, _vp]),
     "cc_search_topk": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "cc_clip_preprocess": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp]),

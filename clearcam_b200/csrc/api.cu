@@ -58,6 +58,24 @@ int cc_conv2d_chain(const void* d_in, int N, int Hin, int Win, int in_cs, int in
   return conv_gemm_launch(L, static_cast<cudaStream_t>(stream));
 }
 
+int cc_conv2d_prelu(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const void* d_w, const float* d_bias_cls,
+                    const float* d_slope, int Cout, int k, int stride, void* d_out, int out_cs, int out_co, const void* d_res,
+                    int res_cs, int res_co, int bn, void* stream) {
+  CC_REQUIRE(d_in && d_w && d_bias_cls && d_slope && d_out, "cc_conv2d_prelu: d_in, d_w, d_bias_cls, d_slope and d_out must not be NULL");
+  CC_REQUIRE(N >= 1 && Hin >= 1 && Win >= 1, "cc_conv2d_prelu: bad shape N=%d Hin=%d Win=%d", N, Hin, Win);
+  const TSlice res = nhwc_slice(d_res, res_cs, res_co, Cout);
+  ConvDesc d = conv_desc(nhwc_slice(d_in, in_cs, in_co, Cin, 0, N, Hin, Win), d_w, d_bias_cls, k, stride,
+                         nhwc_slice(d_out, out_cs, out_co, Cout), ACT_PRELU, d_res ? &res : nullptr);
+  d.slope = d_slope;
+  d.bn_override = bn;
+  CC_REQUIRE(conv_gemm_supported(d), "cc_conv2d_prelu: shape not supported by the wgmma conv (Cin=%d Cout=%d k=%d stride=%d)", Cin, Cout, k, stride);
+  const int sms = device_sm_count();
+  CC_REQUIRE(sms > 0, "cc_conv2d_prelu: no sm_90 (H100) device");
+  GemmLaunch L;
+  if (int rc = conv_gemm_build(d, sms, &L)) return rc;
+  return conv_gemm_launch(L, static_cast<cudaStream_t>(stream));
+}
+
 int cc_attention(const void* d_qkv, int B, int L, int H, int causal, int impl, void* d_ws, size_t ws_bytes, void* d_ctx,
                  size_t* ws_needed, void* stream) {
   CC_REQUIRE(impl == 1 || impl == 2, "cc_attention: unknown impl %d (1 = mma.sync, 2 = wgmma)", impl);

@@ -50,6 +50,10 @@ __device__ __forceinline__ float tanh_approx(float x) {
 //   ACT_SILU       : x*sigmoid(x) = h + h*tanh(h), h = x/2 (|abs err| <= 2^-11 on tanh, i.e. <= |x| * 2.4e-4 on the
 //                    result, below the bf16 rounding of the stored value for x > -2)
 //   ACT_GELU_TANH  : 0.5x(1+tanh(sqrt(2/pi)(x+0.044715x^3)))  (models/objects.py:125 gelu())
+// ACT_PRELU (the face embedder's conv -> BN -> PReLU, models/adaface.py:54,86) is applied in the epilogue itself: its bias
+// is a [9][Cout] table indexed by the output pixel's border class, 3 * (top 0 / interior 1 / bottom 2) + (left 0 / interior 1
+// / right 2), so that an affine map folded in front of a zero-padded 3x3 conv stays exact at the borders; then
+// x > 0 ? x : slope[c] * x.
 template <int ACT>
 __device__ __forceinline__ float act_apply(float x) {
   if (ACT == ACT_SILU) {
@@ -124,6 +128,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
   // a chained launch takes no pre-activation addend, and one with a 128-channel tile no residual: next to 128 accumulator
   // registers their epilogue code would spill (conv_gemm_chain_build refuses them)
   constexpr bool kPre = !CHAIN, kRes = !(CHAIN && BN == 128);
+  constexpr bool kPrelu = ACT == ACT_PRELU;
+  static_assert(!kPrelu || (!F32 && !CHAIN), "ACT_PRELU writes bf16 and chains nothing");
+  constexpr int kBiasRows = kPrelu ? 10 : 1;                  // ACT_PRELU: 9 border-class bias rows, then the slopes
 
   const int wg = threadIdx.x >> 7;
   const uint32_t row_bytes = p.BK * 2;
@@ -139,7 +146,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
   uint8_t* sB = sA + S * a_bytes;
   // resident-B mode: sB holds ALL k-blocks of the weights (loaded once); the ring then carries A only
   float* sBias = reinterpret_cast<float*>(sB + (p.b_res ? num_kb : S) * b_bytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + p.cout + N2);   // chained: the 1x1's bias follows
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + kBiasRows * p.cout + N2);   // chained: the 1x1's bias follows
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + S;
   uint64_t* bres_bar = bars + 2 * S;
@@ -169,7 +176,12 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     fence_mbar_init();
   }
   if (wg > 0) {  // bias -> smem once per CTA
-    for (int i = threadIdx.x - 128; i < p.cout; i += kEpiThreads) sBias[i] = p.bias ? __ldg(p.bias + i) : 0.f;
+    if constexpr (kPrelu) {
+      for (int i = threadIdx.x - 128; i < 9 * p.cout; i += kEpiThreads) sBias[i] = __ldg(p.bias + i);
+      for (int i = threadIdx.x - 128; i < p.cout; i += kEpiThreads) sBias[9 * p.cout + i] = __ldg(p.slope + i);
+    } else {
+      for (int i = threadIdx.x - 128; i < p.cout; i += kEpiThreads) sBias[i] = p.bias ? __ldg(p.bias + i) : 0.f;
+    }
     if constexpr (CHAIN)
       for (int i = threadIdx.x - 128; i < N2; i += kEpiThreads) sBias[p.cout + i] = p.bias2 ? __ldg(p.bias2 + i) : 0.f;
   }
@@ -310,13 +322,22 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             if ((pw < p.W) && (ph < p.H) && (pn < p.N))
               pre_row = p.pre + ((static_cast<long long>(pn) * p.pre_h + (ph >> 1)) * p.pre_w + (pw >> 1)) * p.cout + nb * BN;
           }
+          // ACT_PRELU: this row's bias row (its border class) and the slopes
+          uint32_t bias_q = bias_t;
+          [[maybe_unused]] uint32_t slope_q = 0;
+          if constexpr (kPrelu) {
+            const int pw = tx.w0 + (row & TWm), ph = tx.h0 + ((row >> p.lTW) & THm);
+            const int cls = 3 * (ph == 0 ? 0 : (ph == p.H - 1 ? 2 : 1)) + (pw == 0 ? 0 : (pw == p.W - 1 ? 2 : 1));
+            bias_q = bias_t + cls * p.cout * 4;
+            slope_q = bias_t + 9 * p.cout * 4;
+          }
           // staging address of (row, column): the TMA box swizzle XORs the 16-B chunk index with bits of the row offset
           const uint32_t roff = static_cast<uint32_t>(row * kBoxBytes), rxor = (roff >> 3) & kSwz;
           const uint32_t rbase = stg + roff;
 #pragma unroll
           for (int i = pass * kPassCols / 8; i < (pass + 1) * kPassCols / 8; ++i) {
             const int col = 8 * i + 2 * (lane & 3);
-            const float2 bb = lds_f2(bias_t + 32 * i);
+            const float2 bb = lds_f2(bias_q + 32 * i);
             const int pc = col - pass * kPassCols;
             float b0 = bb.x, b1 = bb.y;
             if (pre_row != nullptr) {
@@ -326,6 +347,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             const int k = 4 * i + 2 * (q & 1);
             float f0 = act_apply<ACT>(((q >> 1) ? acc1[k] : acc0[k]) + b0);
             float f1 = act_apply<ACT>(((q >> 1) ? acc1[k + 1] : acc0[k + 1]) + b1);
+            if constexpr (kPrelu) {
+              const float2 sl = lds_f2(slope_q + 32 * i);
+              f0 = f0 > 0.f ? f0 : sl.x * f0;
+              f1 = f1 > 0.f ? f1 : sl.y * f1;
+            }
             const uint32_t addr = rbase + (pc / kBoxCols) * kBoxTile + (((pc % kBoxCols) * es) ^ rxor);
             if (F32) {
               if (kRes && p.res != nullptr) {
@@ -618,7 +644,10 @@ static int gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L, bool with_o
 
   // ---- epilogue
   p.out = d.out.p; p.out_cs = d.out.cs; p.out_co = d.out.co; p.out_f32 = d.out.f32;
-  p.bias = d.bias; p.act = d.act;
+  p.bias = d.bias; p.act = d.act; p.slope = d.slope;
+  const bool prelu = d.act == ACT_PRELU;
+  if (prelu)
+    CC_REQUIRE(d.bias && d.slope && !d.out.f32 && !d.pre, "conv_gemm: ACT_PRELU needs its [9][Cout] bias table and slopes, and writes bf16");
   p.res = d.res.p; p.res_cs = d.res.cs; p.res_co = d.res.co;
   p.out_ns = d.out_ns > 0 ? d.out_ns : Hout * Wout;
   p.pre = d.pre; p.pre_h = d.pre_h; p.pre_w = d.pre_w;
@@ -642,7 +671,7 @@ static int gemm_build(const ConvDesc& d, int num_sms, GemmLaunch* L, bool with_o
   }
 
   // ---- smem budget -> pipeline depth.  Fixed part: alignment slack, one output staging tile per consumer, bias, barriers.
-  const int S = set_smem_budget(L, 1024 + kConsumers * epi_stage_bytes(BN, es) + Cout * 4 + 8 * kBarriers);
+  const int S = set_smem_budget(L, 1024 + kConsumers * epi_stage_bytes(BN, es) + Cout * 4 * (prelu ? 10 : 1) + 8 * kBarriers);
   CC_REQUIRE(S >= 2, "conv_gemm: tile does not fit shared memory (BN=%d BK=%d)", BN, p.BK);
   L->grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
   L->flops = 2.0 * double(N) * Hout * Wout * Cout * d.k * d.k * Cin;
@@ -788,6 +817,9 @@ int conv_gemm_launch(const GemmLaunch& L, cudaStream_t stream) {
     case ACT_SILU: return f32 ? launch_variant<ACT_SILU, true>(L, stream) : launch_variant<ACT_SILU, false>(L, stream);
     case ACT_GELU_TANH:
       return f32 ? launch_variant<ACT_GELU_TANH, true>(L, stream) : launch_variant<ACT_GELU_TANH, false>(L, stream);
+    case ACT_PRELU:
+      if (!f32) return launch_variant<ACT_PRELU, false>(L, stream);
+      break;
   }
   set_error("conv_gemm: unknown activation %d", L.p.act);
   return CC_ERR_INVALID;

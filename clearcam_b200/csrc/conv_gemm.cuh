@@ -5,6 +5,7 @@
 //   * bare nn.Conv2d head/CBLinear convs (no act)       (detection/yolov9.py:173,186,224)
 //   * RepNBottleneck residual  x + cv2(cv1(x))          (detection/yolov9.py:82-89)  -> residual fused in epilogue
 //   * CLIP linears: QKV / out-proj / MLP (+tanh-GELU)   (models/objects.py:107-127,157-179)
+//   * AdaFace conv -> BN -> PReLU, shortcuts, linear   (models/adaface.py:45-57,84-92) -> ACT_PRELU epilogue (csrc/adaface.cu)
 // Activations are NHWC bf16 (a channel *slice* of a wider buffer is addressed in place, so Tensor.cat /
 // chunk in the reference cost nothing here); weights are [Cout][kh][kw][Cin] bf16 (K-major); accumulation fp32
 // in registers; bias + activation + residual in the epilogue.
@@ -16,7 +17,7 @@
 
 namespace cc {
 
-enum Act : int32_t { ACT_NONE = 0, ACT_SILU = 1, ACT_GELU_TANH = 2 };
+enum Act : int32_t { ACT_NONE = 0, ACT_SILU = 1, ACT_GELU_TANH = 2, ACT_PRELU = 3 };
 
 struct GemmParams {
   CUtensorMap tmA;  // 5-D view of the NHWC activation (see conv_gemm.cu)
@@ -35,7 +36,7 @@ struct GemmParams {
   // epilogue
   void* out;
   int32_t out_cs, out_co, out_f32;    // channel stride of the out buffer, channel offset, fp32 output flag
-  const float* bias;                  // [Cout] or nullptr
+  const float* bias;                  // [Cout] or nullptr; ACT_PRELU: [9][Cout], row = the output pixel's border class
   int32_t act;
   const void* res;                    // residual (same dtype as out) or nullptr; may be the output slice itself (in place)
   int32_t res_cs, res_co;
@@ -59,6 +60,7 @@ struct GemmParams {
   int32_t ch_stage;                   // bytes of one consumer's staging region (staging + partner box, or the 1x1's output tile)
   int32_t act2, out2_f32;
   const float* bias2;                 // [Cout2] or nullptr
+  const float* slope;                 // ACT_PRELU: [Cout] negative-side slopes
 };
 
 // One conv / linear as the host describes it.  The slices carry pointer, row pitch, channel offset and width; the output
@@ -66,7 +68,8 @@ struct GemmParams {
 struct ConvDesc {
   TSlice in;                               // bf16 input slice; N, H, W: stored input dims (even for stride 2)
   const void* w;                           // bf16 [Cout][k*k*Cin]
-  const float* bias;
+  const float* bias;                       // ACT_PRELU: fp32 [9][Cout] (see GemmParams::bias), bf16 output only
+  const float* slope;                      // ACT_PRELU: fp32 [Cout]
   int k, stride;                           // k in {1,3}; pad = k/2; stride in {1,2}
   TSlice out;                              // output slice, C = Cout, bf16 or fp32 (f32); p == nullptr: none (a chain that drops it)
   int act;

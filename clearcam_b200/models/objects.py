@@ -7,8 +7,9 @@
     hits = finder.search("ferrari f40", top_k=10)                  # [(path, score)]          (models/objects.py:356)
 
 Mirrors class OpenCLIP (/root/reference/models/objects.py:21-143), encode_text (:145-186) and ObjectFinder's CLIP
-methods (:189-206, :237-251, :356-421).  The face pipeline (BlazeFace/AdaFace, :207-354) is out of scope
-(SURVEY.md §2).  All arithmetic runs in libclearcam_b200.so; there is no CPU fallback.
+methods (:189-206, :237-251, :356-421), and the face embedder's (`init_face`, `turn_off_face`, `adaface`,
+`preprocess_face` for 112x112 faces, face search; :207-217, :253-261).  Face detection and alignment (BlazeFace,
+`img_to_face`, :263-354) are not built yet.  All arithmetic runs in libclearcam_b200.so; there is no CPU fallback.
 
 Additions: `arch=` (the reference hard-codes ViT-L/14; "ViT-B/32" runs the same kernels), explicit `weights=`
 (the reference downloads from HuggingFace, :91), `encode_text_batch`, a contiguous device index for search, and
@@ -215,9 +216,12 @@ class ObjectFinder:
         self.clip = False
         self.face = False
         self.jit_cache = {}
-        self._index = None            # (paths, device tensor [N,D], per-row search metadata) cache of image_embeddings
-        self._index_fp = ()           # identities of the cached values
+        # is_face -> (paths, device tensor [N,D], per-row search metadata, identities of the cached values): the device
+        # copies of image_embeddings and face_embeddings
+        self._index = {}
         self.model: Optional[OpenCLIP] = None
+        self.blazeface = None
+        self.adaface = None           # ADAFACE once init_face ran: adaface(img) -> (1,512), as the reference calls it
 
     def init_clip(self, weights=None, arch: str = "ViT-L/14"):
         if self.clip:
@@ -233,8 +237,39 @@ class ObjectFinder:
         self.clip = False
         self.model = None
 
-    def init_face(self):
-        raise CCError("the face pipeline (BlazeFace/AdaFace) is outside the hot path built here (SURVEY.md §2)")
+    def init_face(self, weights=None):
+        """models/objects.py:211-215 without BlazeFace (face detection is not built yet): the AdaFace embedder, from the
+        reference's state dict / safetensors path, or the reference's file when None."""
+        if self.face:
+            return
+        from .adaface import ADAFACE
+        self.adaface = ADAFACE(weights)
+        self.face = True
+
+    def turn_off_face(self):
+        self.face = False
+        self.blazeface = None
+        self.adaface = None
+
+    def embed_faces(self, faces):
+        """uint8 [B,112,112,3] faces (host or device) -> device (B,512): row b is `adaface(faces[b])`, in one batched call."""
+        if self.adaface is None:
+            raise CCError("the face embedder is off: call init_face() first")
+        return self.adaface.embed(faces)
+
+    def preprocess_face(self, img):
+        """models/objects.py:253-261: an uploaded file (bytes) or a stored path under data/cameras -> the RGB image when it is
+        already a 112x112 face.  Other sizes need face detection and alignment (`img_to_face`), which is not built yet."""
+        import cv2
+        if type(img) == bytes:
+            img = cv2.imdecode(np.frombuffer(img, np.uint8), cv2.IMREAD_COLOR)
+        else:
+            img = cv2.imread(f"data/cameras{img}")
+        img = cv2.cvtColor(img, cv2.COLOR_BGR2RGB)
+        if img.shape != (112, 112, 3):
+            raise CCError(f"preprocess_face: a {img.shape[1]}x{img.shape[0]} image needs face detection and alignment "
+                          "(img_to_face), which is not built yet; only 112x112 faces are accepted")
+        return img
 
     def preprocess(self, img):
         """models/objects.py:237-242 (host, cv2): RGB HWC uint8 -> (3,S,S) float32 in [-1,1]."""
@@ -417,15 +452,17 @@ class ObjectFinder:
             emb = self.model.precompute_embedding(x).tensor
         return files, DeviceResult(emb[:K])
 
-    def _device_index(self):
-        """Contiguous device copy of `image_embeddings` plus, per row, what `search` filters and groups on — rebuilt
-        whenever a key OR the array stored under a key changes (the fingerprint holds the identity of every value, so an
-        embedding replaced under an existing path is seen).  Returns (paths, device [N,D], meta)."""
-        keys = [k for k, v in self.image_embeddings.items() if v is not None]
-        fp = tuple(id(self.image_embeddings[k]) for k in keys)
-        if self._index is None or self._index[0] != keys or self._index_fp != fp:
-            self._index_fp = fp
-            mat = np.concatenate([np.asarray(self.image_embeddings[k], np.float32).reshape(1, -1) for k in keys]) if keys \
+    def _device_index(self, is_face=False):
+        """Contiguous device copy of `image_embeddings` (`face_embeddings` when is_face) plus, per row, what `search`
+        filters and groups on — rebuilt whenever a key OR the array stored under a key changes (the fingerprint holds the
+        identity of every value, so an embedding replaced under an existing path is seen).  Returns (paths, device [N,D],
+        meta)."""
+        embeddings = self.face_embeddings if is_face else self.image_embeddings
+        keys = [k for k, v in embeddings.items() if v is not None]
+        fp = tuple(id(embeddings[k]) for k in keys)
+        cached = self._index.get(is_face)
+        if cached is None or cached[0] != keys or cached[3] != fp:
+            mat = np.concatenate([np.asarray(embeddings[k], np.float32).reshape(1, -1) for k in keys]) if keys \
                 else np.zeros((0, self.model.embed_dim if self.model else 1), np.float32)
             n = len(keys)
             norm = np.array([k.replace("\\", "/") for k in keys], dtype=str) if n else np.zeros(0, dtype=str)
@@ -445,21 +482,21 @@ class ObjectFinder:
             meta = {"norm": norm, "jpg": jpg, "truthy": truthy, "group": torch.from_numpy(group).cuda(),
                     "ident": torch.arange(n, dtype=torch.int32, device="cuda"),
                     "work": torch.empty(max(n, 1), dtype=torch.int64, device="cuda")}
-            self._index = (keys, torch.from_numpy(mat).cuda(), meta)
-        return self._index
+            self._index[is_face] = (keys, torch.from_numpy(mat).cuda(), meta, fp)
+        return self._index[is_face][:3]
 
     def search(self, query=None, top_k=10, cam_name=None, timestamp=None, text_embedding=None, is_face=False):
         """models/objects.py:356-390 — same filtering, best score per object id, descending order, top_k — with the N dot
         products, the per-object maximum and the top-k selection in one device pass over the contiguous index
-        (cc_search_topk): only the k winners come back over PCIe.  (An exact score tie goes to the earlier index row.)"""
-        if is_face:
-            raise CCError("face search is outside the hot path built here")
-        if not self.image_embeddings:
+        (cc_search_topk): only the k winners come back over PCIe.  (An exact score tie goes to the earlier index row.)
+        is_face=True searches `face_embeddings` with the embedding given (`adaface(img).numpy()` in run_clip), under the
+        same filters; as in the reference, its date filter looks for "/objects/<date>/" in the stored path."""
+        if not (self.face_embeddings if is_face else self.image_embeddings):
             print("No embeddings available.")
             return []
         if text_embedding is None:
             text_embedding = self.model._encode_text(query).numpy()
-        keys, index, meta = self._device_index()
+        keys, index, meta = self._device_index(is_face)
         n = len(keys)
         if n == 0 or top_k <= 0:
             return []
@@ -499,4 +536,4 @@ class ObjectFinder:
                 target.update(emb)
         for k in set(target.keys()) - valid:
             del target[k]
-        self._index = None
+        self._index.pop(face, None)

@@ -7,12 +7,19 @@ from ._lib import lib, check, ptr, stream_ptr
 
 
 def conv2d(xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, Cout, act=0, res=None, res_co=0, groups=1, impl=0, bn=0,
-           stream=None):
-    """xbuf: [N,H,W,in_cs] bf16 CUDA; w: [Cout,k,k,Cin/groups] bf16; obuf: [N,Ho,Wo,out_cs] bf16|fp32."""
+           stream=None, slope=None):
+    """xbuf: [N,H,W,in_cs] bf16 CUDA; w: [Cout,k,k,Cin/groups] bf16; obuf: [N,Ho,Wo,out_cs] bf16|fp32.
+    act = 3 (CC_ACT_PRELU, cc_conv2d_prelu): bias is the fp32 [9,Cout] border-class table and slope the fp32 [Cout] PReLU
+    slopes; the wgmma kernel, bf16 out."""
     assert xbuf.is_cuda and xbuf.dtype == torch.bfloat16 and xbuf.is_contiguous()
     assert w.dtype == torch.bfloat16 and w.is_contiguous() and obuf.is_contiguous()
     N, H, W, in_cs = xbuf.shape
     out_cs = obuf.shape[-1]
+    if act == 3:
+        rc = lib().cc_conv2d_prelu(ptr(xbuf), N, H, W, in_cs, in_co, Cin, ptr(w), ptr(bias), ptr(slope), Cout, k, stride, ptr(obuf),
+                                   out_cs, out_co, ptr(res), 0 if res is None else res.shape[-1], res_co, bn, stream_ptr(stream))
+        check(rc, "cc_conv2d_prelu")
+        return obuf
     out_f32 = 1 if obuf.dtype == torch.float32 else 0
     rc = lib().cc_conv2d(ptr(xbuf), N, H, W, in_cs, in_co, Cin, ptr(w), ptr(bias), Cout, k, stride, groups, ptr(obuf),
                          out_cs, out_co, out_f32, act, ptr(res), 0 if res is None else res.shape[-1], res_co, impl, bn,

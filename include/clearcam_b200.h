@@ -32,6 +32,7 @@ int cc_device_check(void);
 #define CC_ACT_NONE 0
 #define CC_ACT_SILU 1      /* x*sigmoid(x): detection/yolov9.py:38 */
 #define CC_ACT_GELU_TANH 2 /* tinygrad Tensor.gelu(): models/objects.py:125,179 */
+#define CC_ACT_PRELU 3     /* where(x > 0, x, slope * x): models/adaface.py:54,86 (cc_conv2d_prelu, the face embedder) */
 
 /* ---- kernel-level ops (used by the graphs below and exposed for the parity tests) ---- */
 
@@ -57,6 +58,15 @@ int cc_conv2d_chain(const void* d_in, int N, int Hin, int Win, int in_cs, int in
                     const void* d_w2, const float* d_bias2, int Cout2, int act2, int k0,
                     const void* d_part, int part_cs, int part_co, int part_C,
                     void* d_out2, int out2_cs, int out2_co, int out2_f32, void* stream);
+
+/* cc_conv2d on the wgmma kernel with the face embedder's epilogue (CC_ACT_PRELU), bf16 out:
+ *   out = where(y > 0, y, d_slope[c] * y) (+ res),  y = conv(x) + d_bias_cls[cls][c]
+ * where cls = 3 * (h == 0 ? 0 : h == Ho-1 ? 2 : 1) + (w == 0 ? 0 : w == Wo-1 ? 2 : 1) is the output pixel's border class.
+ * d_bias_cls: fp32 [9][Cout]; d_slope: fp32 [Cout].  A per-channel affine map applied before a zero-padded 3x3 conv folds into
+ * the weights and this table exactly (the shift summed over the taps inside the map). */
+int cc_conv2d_prelu(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const void* d_w, const float* d_bias_cls,
+                    const float* d_slope, int Cout, int k, int stride, void* d_out, int out_cs, int out_co, const void* d_res,
+                    int res_cs, int res_co, int bn, void* stream);
 
 /* ---- YOLOv9 detector (replaces detection/yolov9.py: class YOLOv9, :298-458) ---- */
 typedef struct cc_yolo cc_yolo;
@@ -318,6 +328,29 @@ int cc_clip_set_workspace(cc_clip* h, void* d_workspace, size_t bytes);
 /* per-op device timing of one encode (text != 0: text tower). */
 int cc_clip_profile(cc_clip* h, int text, const void* d_in, int B, float* d_out, int cap, float* ms, double* flops,
                     const char** names, int* n_ops, double* total_flops, void* stream);
+/* ---- AdaFace IR-50 face embedder (replaces class ADAFACE, models/adaface.py:24-96) ---- */
+typedef struct cc_face cc_face;
+/* Weights: host fp32 tensors of the folded network that clearcam_b200/models/adaface.py `fold_state_dict` makes from the
+ * reference's state dict (every BatchNorm and the input normalisation folded in float64):
+ *   "stem.w" [64][3][3][3] (input channels in the uint8 image's order), "stem.cls" [9][64], "stem.slope" [64];
+ *   "body.<i>.c0.w" [D][3][3][Cin], "body.<i>.c0.cls" [9][D], "body.<i>.c0.slope" [D], "body.<i>.c1.w" [D][3][3][D],
+ *   "body.<i>.c1.b" [D], and for a block with a stride or a width change "body.<i>.sc.w" [D][Cin], "body.<i>.sc.b" [D];
+ *   "linear.w" [512][7*7*512] (columns in NHWC order), "linear.b" [512].
+ * They are rounded to bf16 and uploaded once; the host pointers are not retained. */
+int cc_face_create(int n_tensors, const char* const* names, const float* const* h_data, const int64_t* numels, cc_face** out);
+int cc_face_destroy(cc_face* h);
+/* ADAFACE.__call__ (models/adaface.py:79-96) for B faces: d_faces uint8 [B,112,112,3] (the image as the reference receives
+ * it; the channel flip of :81 happens inside) -> L2-normalised embeddings at d_out[b*out_row_stride .. +512) (0 = 512).
+ * Face b's row is what the reference's call on face b alone returns (its norm is over its own row). */
+int cc_face_embed(cc_face* h, const uint8_t* d_faces, int B, float* d_out, long long out_row_stride, void* stream);
+/* Workspace of the face plans, same contract as cc_clip_workspace_bytes / cc_clip_set_workspace. */
+int cc_face_workspace_bytes(cc_face* h, int B, size_t* bytes);
+int cc_face_set_workspace(cc_face* h, void* d_workspace, size_t bytes);
+/* Parity tap: runs the plan of batch B up to `layer` (0: conv0 -> bn0 -> PReLU, 1..24: the output of block layer-1, 25: the
+ * linear -> bn2 output before the L2 norm) and writes that map as dense fp32 NHWC [B,H,W,C] to d_dst.  d_dst = NULL only
+ * reports C, H, W. */
+int cc_face_layer_output(cc_face* h, const uint8_t* d_faces, int B, int layer, float* d_dst, int* C, int* H, int* W, void* stream);
+
 /* ObjectFinder.search inner loop (models/objects.py:365-376): d_scores[q*N + n] = <d_index[n,:], d_q[q,:]>, fp32. */
 int cc_search_scores(const float* d_index, int N, int D, const float* d_q, int Q, float* d_scores, void* stream);
 
