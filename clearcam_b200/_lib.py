@@ -55,7 +55,8 @@ class cc_conv_op(ctypes.Structure):
                 + [("pre", ctypes.c_void_p), ("pre_h", ctypes.c_int), ("pre_w", ctypes.c_int), ("w2", ctypes.c_void_p),
                    ("bias2", ctypes.c_void_p), ("act2", ctypes.c_int), ("k0", ctypes.c_int), ("part", cc_slice), ("out2", cc_slice),
                    ("store1", ctypes.c_int)]
-                + [(n, ctypes.c_int) for n in ("BN", "BK", "lTW", "lTH", "lTN", "s2", "stages", "b_res", "grid", "num_tiles")])
+                + [(n, ctypes.c_int) for n in ("BN", "BK", "lTW", "lTH", "lTN", "s2", "stages", "b_res", "grid", "num_tiles",
+                                               "BNn", "narrow_tiles")])
 
 
 # cc_conv_op kinds (CC_CONV_OP_* in include/clearcam_b200.h)

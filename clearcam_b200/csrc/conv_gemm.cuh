@@ -61,6 +61,13 @@ struct GemmParams {
   int32_t act2, out2_f32;
   const float* bias2;                 // [Cout2] or nullptr
   const float* slope;                 // ACT_PRELU: [Cout] negative-side slopes
+  // mixed tile widths (the tile plan, conv_gemm.cu plan_tiles; BNn == 0: every tile is BN wide).  Tiles [0, num_wide) are
+  // BN wide, n_blocks per m tile.  The next n_split tiles are BNn wide: the wide tiles num_wide, num_wide + 1, ... of the
+  // last (partial) wave, each cut into 2^l_split channel blocks.  When Cout is not a multiple of BN, one BNn-wide remainder
+  // block per m tile (channels [n_blocks * BN, Cout)) follows, in m order.
+  int32_t BNn, num_wide, n_split, l_split;
+  CUtensorMap tmBn;                   // the weights with box BK x BNn
+  CUtensorMap tmOn, tmRn;             // the output / residual slices with the narrow width's column box
 };
 
 // One conv / linear as the host describes it.  The slices carry pointer, row pitch, channel offset and width; the output

@@ -1433,7 +1433,7 @@ int cc_yolo_op_conv(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, i
     o.store1 = c.store1 ? 1 : 0;
   }
   o.BN = g.BN; o.BK = g.BK; o.lTW = g.lTW; o.lTH = g.lTH; o.lTN = g.lTN; o.s2 = g.s2; o.stages = g.stages; o.b_res = g.b_res;
-  o.grid = op.gemm.grid; o.num_tiles = g.num_tiles;
+  o.grid = op.gemm.grid; o.num_tiles = g.num_tiles; o.BNn = g.BNn; o.narrow_tiles = g.num_tiles - g.num_wide;
   return n;
 }
 

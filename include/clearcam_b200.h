@@ -168,7 +168,8 @@ int cc_yolo_trace(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf
  * bias2, act2, over output channels [k0, k0 + Cout2 - part.C) followed by the partner slice `part`, into out2; store1 = 0:
  * the first output is not written.  For the tensor-core launches, the tiling as built: N tile BN, K block BK, the 128-pixel
  * tile box 2^lTW x 2^lTH x 2^lTN (w, h, images), the stride-2 pair view s2, the pipeline stages, resident weights b_res,
- * the persistent grid and the tile count.
+ * the persistent grid and the tile count; BNn, the narrow tile width (0: every tile is BN wide), and how many of the tiles
+ * are that narrow (the last wave's tiles split along N, and the remainder channel block when BN does not divide Cout).
  * cc_yolo_run_ops launches ops [first, last) of that plan on `stream` exactly as a forward launches them, without a CUDA
  * graph; d_frames, d_out and d_raw are a cc_yolo_forward call's.  Nothing synchronises. */
 #define CC_CONV_OP_NONE 0
@@ -184,6 +185,7 @@ typedef struct {
   const float* pre; int pre_h, pre_w;
   const void* w2; const float* bias2; int act2, k0; cc_slice part, out2; int store1;
   int BN, BK, lTW, lTH, lTN, s2, stages, b_res, grid, num_tiles;
+  int BNn, narrow_tiles;
 } cc_conv_op;
 int cc_yolo_op_conv(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int i, cc_conv_op* out);
 int cc_yolo_run_ops(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, int first, int last,
