@@ -30,6 +30,14 @@ class cc_jpeg_dest(ctypes.Structure):
     _fields_ = [("data", ctypes.c_void_p), ("pitch", ctypes.c_int64), ("h", ctypes.c_int32), ("w", ctypes.c_int32)]
 
 
+class cc_face_warp(ctypes.Structure):
+    """One face of cc_face_align: device image, its height and width, the crop (x1, y1, x2, y2), the rotated image's size,
+    the rotation matrix and the final transform (row-major 2x3, float64)."""
+    _fields_ = [("src", ctypes.c_void_p), ("h", ctypes.c_int), ("w", ctypes.c_int)] + \
+        [(n, ctypes.c_int) for n in ("x1", "y1", "x2", "y2", "rot_w", "rot_h")] + \
+        [("rot", ctypes.c_double * 6), ("transform", ctypes.c_double * 6)]
+
+
 class cc_track_job(ctypes.Structure):
     """One row of a tracker job table (cc_ocsort_gpu_update): device rows [n,6], their count, slot, threshold."""
     _fields_ = [("rows", ctypes.c_void_p), ("n", ctypes.c_int), ("slot", ctypes.c_int), ("det_thresh", ctypes.c_float),
@@ -130,6 +138,15 @@ _SIGS = {
     "cc_face_workspace_bytes": (_i, [_vp, _i, ctypes.POINTER(ctypes.c_size_t)]),
     "cc_face_set_workspace": (_i, [_vp, _vp, ctypes.c_size_t]),
     "cc_face_layer_output": (_i, [_vp, _vp, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
+    "cc_blazeface_create": (_i, [_i, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_vp), ctypes.POINTER(ctypes.c_int64),
+                                 ctypes.POINTER(_vp)]),
+    "cc_blazeface_destroy": (_i, [_vp]),
+    "cc_blazeface_workspace_bytes": (_i, [_vp, _i, ctypes.POINTER(ctypes.c_size_t)]),
+    "cc_blazeface_set_workspace": (_i, [_vp, _vp, ctypes.c_size_t]),
+    "cc_blazeface_forward": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "cc_blazeface_decode": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    "cc_face_canvas": (_i, [_vp, _i, _vp, _vp]),
+    "cc_face_align": (_i, [_vp, _i, _vp, _vp]),
     "cc_search_scores": (_i, [_vp, _i, _i, _vp, _i, _vp, _vp]),
     "cc_search_topk": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "cc_clip_preprocess": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp]),

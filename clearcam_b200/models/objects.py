@@ -8,8 +8,9 @@
 
 Mirrors class OpenCLIP (/root/reference/models/objects.py:21-143), encode_text (:145-186) and ObjectFinder's CLIP
 methods (:189-206, :237-251, :356-421), and the face embedder's (`init_face`, `turn_off_face`, `adaface`,
-`preprocess_face` for 112x112 faces, face search; :207-217, :253-261).  Face detection and alignment (BlazeFace,
-`img_to_face`, :263-354) are not built yet.  All arithmetic runs in libclearcam_b200.so; there is no CPU fallback.
+`preprocess_face` for 112x112 faces, face search; :207-217, :253-261) and the BlazeFace face detector (`blazeface`,
+models/blazeface.py) with face alignment (`img_to_face`, :263-354, and the batched `faces_from_images`).  All
+arithmetic runs in libclearcam_b200.so; there is no CPU fallback.
 
 Additions: `arch=` (the reference hard-codes ViT-L/14; "ViT-B/32" runs the same kernels), explicit `weights=`
 (the reference downloads from HuggingFace, :91), `encode_text_batch`, a contiguous device index for search, and
@@ -237,13 +238,18 @@ class ObjectFinder:
         self.clip = False
         self.model = None
 
-    def init_face(self, weights=None):
-        """models/objects.py:211-215 without BlazeFace (face detection is not built yet): the AdaFace embedder, from the
-        reference's state dict / safetensors path, or the reference's file when None."""
+    def init_face(self, weights=None, detector=None):
+        """models/objects.py:211-215: the AdaFace embedder, from the reference's state dict / safetensors path, or the
+        reference's file when None; and the BlazeFace detector (`blazeface(img)` -> (896,17)) from `detector` (a state dict
+        or safetensors path), or from the reference's models/blazeface.safetensors when that file exists.  Without either,
+        `blazeface` stays None."""
         if self.face:
             return
         from .adaface import ADAFACE
+        from .blazeface import WEIGHTS_PATH, BlazeFace
         self.adaface = ADAFACE(weights)
+        if detector is not None or os.path.exists(WEIGHTS_PATH):
+            self.blazeface = BlazeFace(detector)
         self.face = True
 
     def turn_off_face(self):
@@ -259,7 +265,8 @@ class ObjectFinder:
 
     def preprocess_face(self, img):
         """models/objects.py:253-261: an uploaded file (bytes) or a stored path under data/cameras -> the RGB image when it is
-        already a 112x112 face.  Other sizes need face detection and alignment (`img_to_face`), which is not built yet."""
+        already a 112x112 face.  Other sizes raise: the reference routes them through `img_to_face` (see that method), which
+        this does not do yet."""
         import cv2
         if type(img) == bytes:
             img = cv2.imdecode(np.frombuffer(img, np.uint8), cv2.IMREAD_COLOR)
@@ -268,8 +275,34 @@ class ObjectFinder:
         img = cv2.cvtColor(img, cv2.COLOR_BGR2RGB)
         if img.shape != (112, 112, 3):
             raise CCError(f"preprocess_face: a {img.shape[1]}x{img.shape[0]} image needs face detection and alignment "
-                          "(img_to_face), which is not built yet; only 112x112 faces are accepted")
+                          "(img_to_face), which uploads do not go through yet; only 112x112 faces are accepted")
         return img
+
+    def faces_from_images(self, images):
+        """`img_to_face` for many images at once: images are uint8 [h,w,3] (host or device, any sizes, as the reference's
+        call receives them) -> (device uint8 [K,112,112,3], rows): rows[i] is the index of image i's face in the batch, or
+        None where `img_to_face(images[i])` returns None.  One canvas launch, one BlazeFace forward, one read of the
+        detections for the host geometry, one alignment launch; the faces go to `embed_faces` without leaving the device."""
+        from .blazeface import _images, align_faces, face_canvas, face_geometry
+        if self.blazeface is None:
+            raise CCError("face detection is off: init_face(detector=...) builds BlazeFace from its weights, or from the "
+                          "reference's models/blazeface.safetensors when that file exists")
+        ims = _images(images)
+        canvas = face_canvas(ims)
+        dets = self.blazeface.detect(canvas).cpu().numpy()                # the host geometry needs the rows
+        jobs, rows = [], []
+        for i, t in enumerate(ims):
+            g = face_geometry(dets[i], t.shape[0], t.shape[1])
+            rows.append(None if g is None else len(jobs))
+            if g is not None:
+                jobs.append((t, g))
+        return align_faces(jobs), rows
+
+    def img_to_face(self, orig):
+        """models/objects.py:263-354: an HWC uint8 image -> the aligned 112x112 face (numpy uint8, BGR order as the
+        reference returns it), or None.  Raises CCError when BlazeFace is not built."""
+        faces, rows = self.faces_from_images([orig])
+        return None if rows[0] is None else faces[rows[0]].cpu().numpy()
 
     def preprocess(self, img):
         """models/objects.py:237-242 (host, cv2): RGB HWC uint8 -> (3,S,S) float32 in [-1,1]."""

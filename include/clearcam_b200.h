@@ -353,6 +353,49 @@ int cc_face_set_workspace(cc_face* h, void* d_workspace, size_t bytes);
  * reports C, H, W. */
 int cc_face_layer_output(cc_face* h, const uint8_t* d_faces, int B, int layer, float* d_dst, int* C, int* H, int* W, void* stream);
 
+/* ---- BlazeFace face detector (replaces class BlazeFace, models/blazeface.py:62-232), fp32 ---- */
+typedef struct cc_blazeface cc_blazeface;
+/* Weights: the reference's own host fp32 tensors under its key names (models/blazeface.safetensors): "conv_tiny.weight"
+ * [24][3][5][5], "backbone_tiny.list.<i>.conv0_tiny.weight" [C][1][3][3] / ".conv1_tiny.weight" [Cout][Cin][1][1] (i = 0..30)
+ * and their biases, "final.conv{0,1}_tiny.*", "{classifier,regressor}_{8,16}_tiny.*" and "anchors" [896][4].  Uploaded
+ * once; the host pointers are not retained. */
+int cc_blazeface_create(int n_tensors, const char* const* names, const float* const* h_data, const int64_t* numels,
+                        cc_blazeface** out);
+int cc_blazeface_destroy(cc_blazeface* h);
+/* The workspace a forward of B images needs, and the caller-owned buffer (256-byte aligned) that every later forward uses.
+ * cc_blazeface_forward allocates nothing: a missing or smaller workspace fails with CC_ERR_INVALID. */
+int cc_blazeface_workspace_bytes(cc_blazeface* h, int B, size_t* bytes);
+int cc_blazeface_set_workspace(cc_blazeface* h, void* d_workspace, size_t bytes);
+/* BlazeFace.__call__ (:153-175) for B images at once.  frames[b]: a device uint8 [h,w,3] image (format CC_FRAME_BGR_U8; its
+ * channels are used in the order given, as the reference does), any size, any number of images.  Writes the forward's raw
+ * outputs d_boxes [B,896,16] (16-byte aligned) and d_scores [B,896], and d_dets [B,896,17]: row b is exactly what the
+ * reference's call on image b alone returns, every anchor in score order, rows under 0.85 or suppressed zeroed, then *256,
+ * the pads off the box columns and everything divided by the scale.  No allocation and no host synchronisation. */
+int cc_blazeface_forward(cc_blazeface* h, const cc_frame* frames, int B, float* d_boxes, float* d_scores, float* d_dets,
+                         void* stream);
+/* The decode, order, suppression and scaling of cc_blazeface_forward alone, on given head outputs d_boxes [B,896,16] and
+ * d_scores [B,896]; h_sizes: host int32 [B][2] (height, width) of the images they stand for. */
+int cc_blazeface_decode(cc_blazeface* h, const float* d_boxes, const float* d_scores, int B, const int32_t* h_sizes, float* d_dets,
+                        void* stream);
+
+/* ---- img_to_face's image arithmetic (models/objects.py:263-354), byte for byte with cv2 ---- */
+/* The pre-resize of B images: frames[b] a device uint8 [h,w,3] image (CC_FRAME_BGR_U8, channels used as given) ->
+ * d_out [B,640,640,3]: cv2.resize(INTER_LINEAR) to a long side of 640, then cv2.copyMakeBorder's centred zero border. */
+int cc_face_canvas(const cc_frame* frames, int B, uint8_t* d_out, void* stream);
+/* One face of cc_face_align: the original device image src [h,w,3], the crop [y1:y2, x1:x2], the size of the rotated image
+ * and the two forward matrices as the reference computes them (rot: cv2.getRotationMatrix2D with the canvas growth;
+ * transform: the float32 eye transform, given as its float32 values). */
+typedef struct {
+  const void* src; int h, w;
+  int x1, y1, x2, y2;
+  int rot_w, rot_h;
+  double rot[6], transform[6];
+} cc_face_warp;
+/* d_out [K,112,112,3]: face k is cv2.cvtColor(cv2.warpAffine(cv2.warpAffine(src[y1:y2, x1:x2], rot, (rot_w, rot_h)),
+ * transform, (112, 112)), COLOR_RGB2BGR), pixel for pixel.  A crop outside its image fails with CC_ERR_INVALID before
+ * anything is launched. */
+int cc_face_align(const cc_face_warp* faces, int K, uint8_t* d_out, void* stream);
+
 /* ObjectFinder.search inner loop (models/objects.py:365-376): d_scores[q*N + n] = <d_index[n,:], d_q[q,:]>, fp32. */
 int cc_search_scores(const float* d_index, int N, int D, const float* d_q, int Q, float* d_scores, void* stream);
 
