@@ -6,6 +6,8 @@ The product path has NO fallback: if the shared library is missing or a call fai
 import ctypes
 import os
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # CC_LIB: developer override used for same-box A/B runs of two builds (tools/ab.py); production loads the in-tree library
 LIB_PATH = os.environ.get("CC_LIB") or os.path.join(_HERE, "libclearcam_b200.so")
@@ -243,6 +245,53 @@ def check(rc, what=""):
     if rc != 0:
         msg = lib().cc_last_error()
         raise CCError(f"{what} failed ({rc}): {msg.decode() if msg else '?'}")
+
+
+def _to_host_fp32(v) -> np.ndarray:
+    import torch
+    if isinstance(v, torch.Tensor):
+        return np.ascontiguousarray(v.detach().to("cpu", torch.float32).numpy())
+    if hasattr(v, "numpy") and not isinstance(v, np.ndarray):
+        v = v.numpy()
+    return np.ascontiguousarray(np.asarray(v, dtype=np.float32))
+
+
+def create(fn: str, tensors, *leading) -> ctypes.c_void_p:
+    """A new library handle from the create entry point `fn`: fn(*leading, n, names, data, numels, &handle) over the
+    {name: array or tensor} that `tensors()` returns, passed as contiguous host float32.  Without an sm_90 device it raises
+    CCError before `tensors` is called, so no weights are prepared for nothing."""
+    L = lib()
+    if L.cc_device_check() <= 0:
+        raise CCError("clearcam_b200 needs an H100 (sm_90) GPU: " + L.cc_last_error().decode())
+    items = [(k, _to_host_fp32(v)) for k, v in tensors().items()]
+    names = (ctypes.c_char_p * len(items))(*[k.encode() for k, _ in items])
+    ptrs = (ctypes.c_void_p * len(items))(*[a.ctypes.data for _, a in items])
+    nums = (ctypes.c_int64 * len(items))(*[a.size for _, a in items])
+    h = ctypes.c_void_p()
+    check(getattr(L, fn)(*leading, len(items), names, ptrs, nums, ctypes.byref(h)), fn)
+    return h
+
+
+class Handle:
+    """Owner of one library handle `_h` (a ctypes.c_void_p, passed as it is to the entry points), destroyed with the
+    object by the entry point a subclass names in `_destroy`."""
+    _h = None
+    _destroy = ""
+
+    def _adopt(self, h) -> None:
+        """Own `h` and destroy the handle it replaces.  The caller creates `h` first, so a failed create leaves the old
+        handle in place."""
+        old, self._h = self._h, h
+        if old:
+            getattr(lib(), self._destroy)(old)
+
+    def __del__(self):
+        try:
+            if self._h:
+                getattr(lib(), self._destroy)(self._h)
+                self._h = None
+        except Exception:
+            pass
 
 
 def declared_symbols():

@@ -23,10 +23,6 @@
 #include "cc_common.h"
 #include "conv_gemm.cuh"
 #include "ops.cuh"
-#include <map>
-#include <memory>
-#include <string>
-#include <vector>
 
 namespace cc {
 
@@ -75,50 +71,26 @@ struct FacePlan {
   int B = 0;
   std::vector<FOp> ops;
   std::vector<FaceLayer> layers;     // 0: stem, 1..24: blocks, 25: the linear's output before the L2 norm
-  uint64_t gen = 0, last_use = 0;
 };
 
 struct FaceModel {
   int sms = 0;
-  std::map<std::string, std::pair<const float*, long long>> host;
-  std::vector<void*> allocs;
+  DeviceWeights weights;
   __nv_bfloat16* stem_w = nullptr; float *stem_cls = nullptr, *stem_slope = nullptr;
   FaceBlockW blk[kFaceBlocks];
   __nv_bfloat16* lin_w = nullptr; float* lin_b = nullptr;
-  std::map<int, std::unique_ptr<FacePlan>> plans;
-  Arena arena;
-  uint64_t tick = 0;
-  ~FaceModel() { plans.clear(); for (void* p : allocs) cudaFree(p); }
-
-  int get(const std::string& name, long long n, const float** out) {
-    auto it = host.find(name);
-    CC_REQUIRE(it != host.end(), "cc_face_create: missing tensor '%s'", name.c_str());
-    CC_REQUIRE(it->second.second == n, "cc_face_create: '%s' has %lld elements, expected %lld", name.c_str(), it->second.second, n);
-    *out = it->second.first;
-    return CC_OK;
-  }
-  int up(const void* h, size_t bytes, void** d) {
-    CC_CHECK_CUDA(cudaMalloc(d, bytes));
-    allocs.push_back(*d);
-    CC_CHECK_CUDA(cudaMemcpy(*d, h, bytes, cudaMemcpyHostToDevice));
-    return CC_OK;
-  }
-  int up_f32(const std::string& name, long long n, float** d) {
-    const float* h;
-    if (int rc = get(name, n, &h)) return rc;
-    return up(h, n * 4, reinterpret_cast<void**>(d));
-  }
+  PlanCache<int, FacePlan> plans{"face"};   // by batch size
   // [cout][taps][cin] fp32 -> bf16 [cout][3][3][cin_pad]; taps = 1 puts the tap at the centre of the 3x3
   int up_conv(const std::string& name, int cout, int taps, int cin, int cin_pad, __nv_bfloat16** d) {
     const float* h;
-    if (int rc = get(name, static_cast<long long>(cout) * taps * cin, &h)) return rc;
+    if (int rc = weights.host.get(name, static_cast<long long>(cout) * taps * cin, &h)) return rc;
     std::vector<__nv_bfloat16> w(static_cast<size_t>(cout) * 9 * cin_pad, __float2bfloat16_rn(0.f));
     for (int o = 0; o < cout; ++o)
       for (int t = 0; t < taps; ++t)
         for (int c = 0; c < cin; ++c)
           w[(static_cast<size_t>(o) * 9 + (taps == 1 ? 4 : t)) * cin_pad + c] =
               __float2bfloat16_rn(h[(static_cast<size_t>(o) * taps + t) * cin + c]);
-    return up(w.data(), w.size() * 2, reinterpret_cast<void**>(d));
+    return weights.upload(w, d);
   }
 };
 
@@ -214,84 +186,68 @@ using namespace cc;
 
 struct cc_face { FaceModel m; };
 
-static constexpr size_t kMaxFacePlans = 16;
-
-// the plan of batch B (built against the current workspace, the least recently used dropped past kMaxFacePlans)
-static int face_plan(cc_face* h, int B, FacePlan** out) {
-  FaceModel& M = h->m;
-  auto it = M.plans.find(B);
-  if (it != M.plans.end() && it->second->gen == M.arena.gen) {
-    it->second->last_use = ++M.tick;
-    *out = it->second.get();
-    return CC_OK;
-  }
+// workspace bytes the plan of batch B addresses (measuring pass of the builder: no device work)
+static int face_plan_bytes(cc_face* h, int B, size_t* bytes) {
   FacePlan tmp;
-  FacePlanBuilder dry(M, tmp);
+  FacePlanBuilder dry(h->m, tmp);
   dry.bump.dry = true;
-  dry.build(B);
-  if (int rc = M.arena.reserve(dry.bump.off + 1024)) return rc;
-  for (auto p = M.plans.begin(); p != M.plans.end();)
-    p = (p->second->gen != M.arena.gen) ? M.plans.erase(p) : std::next(p);
-  std::unique_ptr<FacePlan> P(new FacePlan());
-  P->B = B;
-  FacePlanBuilder b(M, *P);
-  b.bump.base = static_cast<uint8_t*>(M.arena.base);
-  if (int rc = b.build(B)) return rc;
-  CC_REQUIRE(b.bump.off <= M.arena.cap, "face plan: workspace overrun (%zu > %zu)", b.bump.off, M.arena.cap);
-  P->gen = M.arena.gen;
-  P->last_use = ++M.tick;
-  if (M.plans.size() >= kMaxFacePlans) {
-    auto lru = M.plans.begin();
-    for (auto p = M.plans.begin(); p != M.plans.end(); ++p)
-      if (p->second->last_use < lru->second->last_use) lru = p;
-    M.plans.erase(lru);
-  }
-  *out = (M.plans[B] = std::move(P)).get();
+  if (int rc = dry.build(B)) return rc;
+  *bytes = dry.bump.off + 1024;
   return CC_OK;
+}
+static int face_plan(cc_face* h, int B, FacePlan** out) {
+  return h->m.plans.get(
+      B, [&](size_t* bytes) { return face_plan_bytes(h, B, bytes); },
+      [&](FacePlan& P, uint8_t* base, size_t* used) {
+        P.B = B;
+        FacePlanBuilder b(h->m, P);
+        b.bump.base = base;
+        const int rc = b.build(B);
+        *used = b.bump.off;
+        return rc;
+      },
+      out);
 }
 
 extern "C" {
 
 int cc_face_create(int n_tensors, const char* const* names, const float* const* h_data, const int64_t* numels, cc_face** out) {
-  CC_REQUIRE(out && n_tensors >= 0 && (n_tensors == 0 || (names && h_data && numels)), "cc_face_create: null argument");
+  CC_REQUIRE(out, "cc_face_create: null argument");
   const int sms = device_sm_count();
   CC_REQUIRE(sms > 0, "cc_face_create: no sm_90 (H100) device");
   std::unique_ptr<cc_face> h(new cc_face());
   FaceModel& M = h->m;
   M.sms = sms;
-  for (int i = 0; i < n_tensors; ++i) {
-    CC_REQUIRE(names[i] && h_data[i], "cc_face_create: tensor %d is NULL", i);
-    M.host[names[i]] = {h_data[i], static_cast<long long>(numels[i])};
-  }
   int rc = 0;
+  if ((rc = M.weights.host.fill("cc_face_create", n_tensors, names, h_data, numels))) return rc;
   if ((rc = M.up_conv("stem.w", 64, 9, 3, kFacePackC, &M.stem_w))) return rc;
-  if ((rc = M.up_f32("stem.cls", 9 * 64, &M.stem_cls))) return rc;
-  if ((rc = M.up_f32("stem.slope", 64, &M.stem_slope))) return rc;
+  if ((rc = M.weights.up_f32("stem.cls", 9 * 64, &M.stem_cls))) return rc;
+  if ((rc = M.weights.up_f32("stem.slope", 64, &M.stem_slope))) return rc;
   for (int i = 0; i < kFaceBlocks; ++i) {
     const int cin = kFaceSizes[i][0], D = kFaceSizes[i][1];
     const bool proj = cin != D || kFaceSizes[i][2] != 1;
     const std::string p = "body." + std::to_string(i);
     FaceBlockW& b = M.blk[i];
     if ((rc = M.up_conv(p + ".c0.w", D, 9, cin, cin, &b.w0))) return rc;
-    if ((rc = M.up_f32(p + ".c0.cls", 9 * D, &b.cls0))) return rc;
-    if ((rc = M.up_f32(p + ".c0.slope", D, &b.slope0))) return rc;
+    if ((rc = M.weights.up_f32(p + ".c0.cls", 9 * D, &b.cls0))) return rc;
+    if ((rc = M.weights.up_f32(p + ".c0.slope", D, &b.slope0))) return rc;
     if ((rc = M.up_conv(p + ".c1.w", D, 9, D, D, &b.w1))) return rc;
-    if ((rc = M.up_f32(p + ".c1.b", D, &b.b1))) return rc;
+    if ((rc = M.weights.up_f32(p + ".c1.b", D, &b.b1))) return rc;
     if (proj) {
       if ((rc = M.up_conv(p + ".sc.w", D, 1, cin, cin, &b.wsc))) return rc;
-      if ((rc = M.up_f32(p + ".sc.b", D, &b.bsc))) return rc;
+      if ((rc = M.weights.up_f32(p + ".sc.b", D, &b.bsc))) return rc;
     }
   }
   const int K = 7 * 7 * kFaceDim;
   {
     const float* w;
-    if ((rc = M.get("linear.w", static_cast<long long>(kFaceDim) * K, &w))) return rc;
+    if ((rc = M.weights.host.get("linear.w", static_cast<long long>(kFaceDim) * K, &w))) return rc;
     std::vector<__nv_bfloat16> wb(static_cast<size_t>(kFaceDim) * K);
     for (size_t i = 0; i < wb.size(); ++i) wb[i] = __float2bfloat16_rn(w[i]);
-    if ((rc = M.up(wb.data(), wb.size() * 2, reinterpret_cast<void**>(&M.lin_w)))) return rc;
+    if ((rc = M.weights.upload(wb, &M.lin_w))) return rc;
   }
-  if ((rc = M.up_f32("linear.b", kFaceDim, &M.lin_b))) return rc;
-  M.host.clear();
+  if ((rc = M.weights.up_f32("linear.b", kFaceDim, &M.lin_b))) return rc;
+  M.weights.host.clear();
   *out = h.release();
   return CC_OK;
 }
@@ -303,20 +259,12 @@ int cc_face_destroy(cc_face* h) {
 
 int cc_face_workspace_bytes(cc_face* h, int B, size_t* bytes) {
   CC_REQUIRE(h && bytes && B > 0, "cc_face_workspace_bytes: bad argument");
-  FacePlan tmp;
-  FacePlanBuilder dry(h->m, tmp);
-  dry.bump.dry = true;
-  dry.build(B);
-  *bytes = dry.bump.off + 1024;
-  return CC_OK;
+  return face_plan_bytes(h, B, bytes);
 }
 
 int cc_face_set_workspace(cc_face* h, void* d_workspace, size_t bytes) {
-  CC_REQUIRE(h, "cc_face_set_workspace: null handle");
-  CC_REQUIRE(d_workspace == nullptr || (reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0,
-             "cc_face_set_workspace: the workspace must be 256-byte aligned");
-  h->m.plans.clear();
-  return h->m.arena.adopt(d_workspace, bytes);
+  if (int rc = check_workspace("cc_face_set_workspace", h, d_workspace)) return rc;
+  return h->m.plans.adopt(d_workspace, bytes);
 }
 
 int cc_face_embed(cc_face* h, const uint8_t* d_faces, int B, float* d_out, long long out_row_stride, void* stream) {

@@ -17,10 +17,6 @@
 #include "clearcam_b200.h"
 #include "cc_common.h"
 #include "ops.cuh"
-#include <map>
-#include <memory>
-#include <string>
-#include <vector>
 
 namespace cc {
 
@@ -287,7 +283,7 @@ static int decode_launch(const float* anchors, const float* boxes, const float* 
 struct BlazeW { const float *dw, *dwb, *pw, *pwb; };
 
 struct BlazeModel {
-  std::map<std::string, std::pair<const float*, long long>> host;
+  HostTensors host;                               // the create call's tensors; emptied before it returns
   float* dev = nullptr;                           // every tensor, one allocation
   std::vector<float> pack;
   const float *stem_w = nullptr, *stem_b = nullptr, *anchors = nullptr;
@@ -301,12 +297,9 @@ struct BlazeModel {
   std::vector<std::pair<const float**, size_t>> fix;
   // rows > 0: a [rows][n / rows] matrix stored transposed, [n / rows][rows]
   int take(const std::string& name, long long n, const float** out, int rows = 0) {
-    auto it = host.find(name);
-    CC_REQUIRE(it != host.end(), "cc_blazeface_create: missing tensor '%s'", name.c_str());
-    CC_REQUIRE(it->second.second == n, "cc_blazeface_create: '%s' has %lld elements, expected %lld", name.c_str(),
-               it->second.second, n);
+    const float* h;
+    if (int rc = host.get(name, n, &h)) return rc;
     fix.push_back({out, pack.size()});
-    const float* h = it->second.first;
     if (rows > 0) {
       const long long cols = n / rows;
       for (long long c = 0; c < cols; ++c)
@@ -341,15 +334,12 @@ extern "C" {
 
 int cc_blazeface_create(int n_tensors, const char* const* names, const float* const* h_data, const int64_t* numels,
                         cc_blazeface** out) {
-  CC_REQUIRE(out && n_tensors >= 0 && (n_tensors == 0 || (names && h_data && numels)), "cc_blazeface_create: null argument");
+  CC_REQUIRE(out, "cc_blazeface_create: null argument");
   CC_REQUIRE(device_sm_count() > 0, "cc_blazeface_create: no sm_90 (H100) device");
   std::unique_ptr<cc_blazeface> h(new cc_blazeface());
   BlazeModel& M = h->m;
-  for (int i = 0; i < n_tensors; ++i) {
-    CC_REQUIRE(names[i] && h_data[i], "cc_blazeface_create: tensor %d is NULL", i);
-    M.host[names[i]] = {h_data[i], static_cast<long long>(numels[i])};
-  }
   int rc = 0;
+  if ((rc = M.host.fill("cc_blazeface_create", n_tensors, names, h_data, numels))) return rc;
   if ((rc = M.take("conv_tiny.weight", 24 * 3 * 25, &M.stem_w)) || (rc = M.take("conv_tiny.bias", 24, &M.stem_b)) ||
       (rc = M.take("anchors", kAnchors * 4, &M.anchors)) ||
       (rc = M.take("classifier_8_tiny.weight", 2 * 96, &M.c8w)) || (rc = M.take("classifier_8_tiny.bias", 2, &M.c8b)) ||
@@ -392,9 +382,7 @@ int cc_blazeface_workspace_bytes(cc_blazeface* h, int B, size_t* bytes) {
 }
 
 int cc_blazeface_set_workspace(cc_blazeface* h, void* d_workspace, size_t bytes) {
-  CC_REQUIRE(h, "cc_blazeface_set_workspace: null handle");
-  CC_REQUIRE(d_workspace == nullptr || (reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0,
-             "cc_blazeface_set_workspace: the workspace must be 256-byte aligned");
+  if (int rc = check_workspace("cc_blazeface_set_workspace", h, d_workspace)) return rc;
   h->m.ws = d_workspace;
   h->m.ws_bytes = d_workspace ? bytes : 0;
   return CC_OK;

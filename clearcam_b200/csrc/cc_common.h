@@ -5,6 +5,11 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <map>
+#include <memory>
+#include <string>
+#include <utility>
+#include <vector>
 
 namespace cc {
 
@@ -71,6 +76,82 @@ struct Bump {
     off += bytes;
     return p;
   }
+};
+
+
+// The plans of one handle, keyed by input shape, all addressing one Arena.  At most kMaxPlans are kept (host metadata only:
+// plans own no device memory); the least recently used goes first.  A plan built against an older workspace generation is
+// stale: it is dropped when the next plan is built and rebuilt on its next use.
+template <class Key, class Plan>
+struct PlanCache {
+  static constexpr size_t kMaxPlans = 16;
+  struct Entry { std::unique_ptr<Plan> plan; uint64_t gen = 0, last_use = 0; };
+  const char* who;             // names the network in refusals ("yolo" -> "yolo plan: ...")
+  Arena arena;                 // declared before `plans`, so the plans (and the CUDA graphs they hold) go first
+  std::map<Key, Entry> plans;
+  uint64_t tick = 0;
+  explicit PlanCache(const char* w) : who(w) {}
+
+  // The plan of `key`.  On a miss, measure(size_t* bytes) sizes the workspace with a dry pass, then build(Plan&, uint8_t*
+  // base, size_t* used) builds the plan against the reserved workspace and reports the bytes it addresses.
+  template <class Measure, class Build>
+  int get(const Key& key, Measure&& measure, Build&& build, Plan** out) {
+    auto it = plans.find(key);
+    if (it != plans.end() && it->second.gen == arena.gen) {
+      it->second.last_use = ++tick;
+      *out = it->second.plan.get();
+      return CC_OK;
+    }
+    size_t bytes = 0, used = 0;
+    if (int rc = measure(&bytes)) return rc;
+    if (int rc = arena.reserve(bytes)) return rc;
+    for (auto p = plans.begin(); p != plans.end();)
+      p = p->second.gen != arena.gen ? plans.erase(p) : std::next(p);
+    std::unique_ptr<Plan> P(new Plan());
+    if (int rc = build(*P, static_cast<uint8_t*>(arena.base), &used)) return rc;
+    CC_REQUIRE(used <= arena.cap, "%s plan: workspace overrun (%zu > %zu)", who, used, arena.cap);
+    if (plans.size() >= kMaxPlans) {
+      auto lru = plans.begin();
+      for (auto p = plans.begin(); p != plans.end(); ++p)
+        if (p->second.last_use < lru->second.last_use) lru = p;
+      plans.erase(lru);
+    }
+    Entry& e = plans[key];
+    e.plan = std::move(P);
+    e.gen = arena.gen;
+    e.last_use = ++tick;
+    *out = e.plan.get();
+    return CC_OK;
+  }
+  // cc_*_set_workspace after check_workspace: every plan is rebuilt against the new workspace
+  int adopt(void* d_ws, size_t bytes) {
+    plans.clear();
+    return arena.adopt(d_ws, bytes);
+  }
+};
+
+// The checks every cc_*_set_workspace makes: a handle, and a workspace that is NULL or 256-byte aligned.
+int check_workspace(const char* who, const void* handle, const void* d_ws);
+
+// The host tensors a cc_*_create call receives, by name.  The pointers are borrowed: valid only during that call.
+struct HostTensors {
+  int fill(const char* who, int n, const char* const* names, const float* const* data, const int64_t* numels);
+  int get(const std::string& name, long long n, const float** out) const;   // tensor `name`, which must have n elements
+  void clear() { map.clear(); }  // before the create call returns: the pointers are the caller's
+ private:
+  const char* who = "";        // the entry point, named in refusals
+  std::map<std::string, std::pair<const float*, long long>> map;
+};
+
+// A model's weights on the device: one allocation per upload, all freed with the model.
+struct DeviceWeights {
+  HostTensors host;            // the create call's tensors; emptied before it returns
+  std::vector<void*> allocs;
+  ~DeviceWeights() { for (void* p : allocs) cudaFree(p); }
+  int upload(const void* h, size_t bytes, void** d);
+  template <class E>
+  int upload(const std::vector<E>& v, E** d) { return upload(v.data(), v.size() * sizeof(E), reinterpret_cast<void**>(d)); }
+  int up_f32(const std::string& name, long long n, float** d);   // host tensor `name` of n elements, as it is
 };
 
 }  // namespace cc

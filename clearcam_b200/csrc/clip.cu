@@ -13,10 +13,6 @@
 #include "cc_common.h"
 #include "conv_gemm.cuh"
 #include "ops.cuh"
-#include <map>
-#include <memory>
-#include <string>
-#include <vector>
 
 namespace cc {
 
@@ -46,7 +42,6 @@ struct ClipPlan {
   int B = 0; bool text = false;
   std::vector<VOp> ops;
   size_t alloc_bytes = 0;      // bytes of the handle's shared workspace this plan addresses
-  uint64_t gen = 0, last_use = 0;
   double flops = 0;
 };
 
@@ -54,8 +49,7 @@ struct ClipModel {
   cc_clip_config cfg{};
   Tower v{}, t{};
   int kpad = 0, sms = 0;
-  std::map<std::string, std::pair<const float*, long long>> host;
-  std::vector<void*> allocs;
+  DeviceWeights weights;
   // image tower
   __nv_bfloat16* patch_w = nullptr; float *cls = nullptr, *pos = nullptr, *lnpre_g = nullptr, *lnpre_b = nullptr,
                  *lnpost_g = nullptr, *lnpost_b = nullptr;
@@ -64,41 +58,19 @@ struct ClipModel {
   // text tower
   float *tok = nullptr, *pos_t = nullptr, *lnf_g = nullptr, *lnf_b = nullptr;
   __nv_bfloat16* tprojT = nullptr;
-  std::map<std::string, std::unique_ptr<ClipPlan>> plans;   // bounded, least recently used goes first
-  Arena arena;                 // activation workspace shared by all plans (size of the largest)
-  uint64_t tick = 0;
-  ~ClipModel() { plans.clear(); for (void* p : allocs) cudaFree(p); }
+  PlanCache<std::string, ClipPlan> plans{"clip"};   // activation workspace shared by all plans (size of the largest)
 
-  int get(const std::string& name, long long n, const float** out) {
-    auto it = host.find(name);
-    CC_REQUIRE(it != host.end(), "clip: missing weight '%s'", name.c_str());
-    CC_REQUIRE(it->second.second == n, "clip: '%s' has %lld elements, expected %lld", name.c_str(), it->second.second, n);
-    *out = it->second.first;
-    return CC_OK;
-  }
-  int up(const void* h, size_t bytes, void** d) {
-    CC_CHECK_CUDA(cudaMalloc(d, bytes));
-    allocs.push_back(*d);
-    CC_CHECK_CUDA(cudaMemcpy(*d, h, bytes, cudaMemcpyHostToDevice));
-    return CC_OK;
-  }
-  int up_f32(const std::string& name, long long n, float** d) {
-    const float* h;
-    int rc = get(name, n, &h);
-    if (rc) return rc;
-    return up(h, n * 4, reinterpret_cast<void**>(d));
-  }
   // [rows][cols] fp32 -> bf16 [rows][cols_pad] (zero padded) ; transpose=true reads the source as [cols][rows]
   int up_bf16(const std::string& name, int rows, int cols, int cols_pad, bool transpose, __nv_bfloat16** d) {
     const float* h;
-    int rc = get(name, static_cast<long long>(rows) * cols, &h);
+    int rc = weights.host.get(name, static_cast<long long>(rows) * cols, &h);
     if (rc) return rc;
     std::vector<__nv_bfloat16> w(static_cast<size_t>(rows) * cols_pad, __float2bfloat16_rn(0.f));
     for (int r = 0; r < rows; ++r)
       for (int c = 0; c < cols; ++c)
         w[static_cast<size_t>(r) * cols_pad + c] =
             __float2bfloat16_rn(transpose ? h[static_cast<size_t>(c) * rows + r] : h[static_cast<size_t>(r) * cols + c]);
-    return up(w.data(), w.size() * 2, reinterpret_cast<void**>(d));
+    return weights.upload(w, d);
   }
   int load_blocks(const std::string& prefix, const Tower& tw, const char* outw, const char* outb, std::vector<BlockW>* dst) {
     const int W = tw.width, M = tw.mlp;
@@ -106,18 +78,18 @@ struct ClipModel {
       const std::string p = prefix + "." + std::to_string(i);
       BlockW b{};
       int rc = 0;
-      if ((rc = up_f32(p + ".ln_1.weight", W, &b.ln1_g))) return rc;
-      if ((rc = up_f32(p + ".ln_1.bias", W, &b.ln1_b))) return rc;
-      if ((rc = up_f32(p + ".ln_2.weight", W, &b.ln2_g))) return rc;
-      if ((rc = up_f32(p + ".ln_2.bias", W, &b.ln2_b))) return rc;
+      if ((rc = weights.up_f32(p + ".ln_1.weight", W, &b.ln1_g))) return rc;
+      if ((rc = weights.up_f32(p + ".ln_1.bias", W, &b.ln1_b))) return rc;
+      if ((rc = weights.up_f32(p + ".ln_2.weight", W, &b.ln2_g))) return rc;
+      if ((rc = weights.up_f32(p + ".ln_2.bias", W, &b.ln2_b))) return rc;
       if ((rc = up_bf16(p + ".in_proj_weight", 3 * W, W, W, false, &b.w_in))) return rc;
-      if ((rc = up_f32(p + ".in_proj_bias", 3 * W, &b.b_in))) return rc;
+      if ((rc = weights.up_f32(p + ".in_proj_bias", 3 * W, &b.b_in))) return rc;
       if ((rc = up_bf16(p + outw, W, W, W, false, &b.w_out))) return rc;
-      if ((rc = up_f32(p + outb, W, &b.b_out))) return rc;
+      if ((rc = weights.up_f32(p + outb, W, &b.b_out))) return rc;
       if ((rc = up_bf16(p + ".mlp_c_fc.weight", M, W, W, false, &b.w_fc))) return rc;
-      if ((rc = up_f32(p + ".mlp_c_fc.bias", M, &b.b_fc))) return rc;
+      if ((rc = weights.up_f32(p + ".mlp_c_fc.bias", M, &b.b_fc))) return rc;
       if ((rc = up_bf16(p + ".mlp_c_proj.weight", W, M, M, false, &b.w_proj))) return rc;
-      if ((rc = up_f32(p + ".mlp_c_proj.bias", W, &b.b_proj))) return rc;
+      if ((rc = weights.up_f32(p + ".mlp_c_proj.bias", W, &b.b_proj))) return rc;
       dst->push_back(b);
     }
     return CC_OK;
@@ -256,25 +228,25 @@ int cc_clip_create(const cc_clip_config* cfg, int n_tensors, const char* const* 
   M.t = Tower{cfg->t_width, cfg->t_layers, cfg->t_heads, cfg->t_mlp, cfg->ctx};
   const int K = 3 * cfg->patch * cfg->patch;
   M.kpad = (K + 63) / 64 * 64;
-  for (int i = 0; i < n_tensors; ++i) M.host[names[i]] = {h_data[i], static_cast<long long>(numels[i])};
   const int W = M.v.width, Wt = M.t.width, D = cfg->embed_dim;
   int rc = 0;
+  if ((rc = M.weights.host.fill("cc_clip_create", n_tensors, names, h_data, numels))) return rc;
   if ((rc = M.up_bf16("visual_conv1.weight", W, K, M.kpad, false, &M.patch_w))) return rc;
-  if ((rc = M.up_f32("class_embedding", W, &M.cls))) return rc;
-  if ((rc = M.up_f32("positional_embedding", static_cast<long long>(M.v.tokens) * W, &M.pos))) return rc;
-  if ((rc = M.up_f32("ln_pre.weight", W, &M.lnpre_g))) return rc;
-  if ((rc = M.up_f32("ln_pre.bias", W, &M.lnpre_b))) return rc;
-  if ((rc = M.up_f32("ln_post.weight", W, &M.lnpost_g))) return rc;
-  if ((rc = M.up_f32("ln_post.bias", W, &M.lnpost_b))) return rc;
+  if ((rc = M.weights.up_f32("class_embedding", W, &M.cls))) return rc;
+  if ((rc = M.weights.up_f32("positional_embedding", static_cast<long long>(M.v.tokens) * W, &M.pos))) return rc;
+  if ((rc = M.weights.up_f32("ln_pre.weight", W, &M.lnpre_g))) return rc;
+  if ((rc = M.weights.up_f32("ln_pre.bias", W, &M.lnpre_b))) return rc;
+  if ((rc = M.weights.up_f32("ln_post.weight", W, &M.lnpost_g))) return rc;
+  if ((rc = M.weights.up_f32("ln_post.bias", W, &M.lnpost_b))) return rc;
   if ((rc = M.up_bf16("proj", D, W, W, true, &M.projT))) return rc;          // stored (W, D) -> [D][W]
   if ((rc = M.load_blocks("resblocks_img", M.v, ".out_proj_weight", ".out_proj_bias", &M.vb))) return rc;
-  if ((rc = M.up_f32("token_embedding.weight", static_cast<long long>(cfg->vocab) * Wt, &M.tok))) return rc;
-  if ((rc = M.up_f32("positional_embedding_text", static_cast<long long>(cfg->ctx) * Wt, &M.pos_t))) return rc;
-  if ((rc = M.up_f32("ln_final.weight", Wt, &M.lnf_g))) return rc;
-  if ((rc = M.up_f32("ln_final.bias", Wt, &M.lnf_b))) return rc;
+  if ((rc = M.weights.up_f32("token_embedding.weight", static_cast<long long>(cfg->vocab) * Wt, &M.tok))) return rc;
+  if ((rc = M.weights.up_f32("positional_embedding_text", static_cast<long long>(cfg->ctx) * Wt, &M.pos_t))) return rc;
+  if ((rc = M.weights.up_f32("ln_final.weight", Wt, &M.lnf_g))) return rc;
+  if ((rc = M.weights.up_f32("ln_final.bias", Wt, &M.lnf_b))) return rc;
   if ((rc = M.up_bf16("text_projection", D, Wt, Wt, true, &M.tprojT))) return rc;
   if ((rc = M.load_blocks("resblocks", M.t, ".attn_out_proj_weight", ".attn_out_proj_bias", &M.tb))) return rc;
-  M.host.clear();
+  M.weights.host.clear();
   *out = h.release();
   return CC_OK;
 }
@@ -283,8 +255,6 @@ int cc_clip_destroy(cc_clip* h) {
   delete h;
   return CC_OK;
 }
-
-static constexpr size_t kMaxClipPlans = 16;
 
 static int clip_plan_bytes(cc_clip* h, bool text, int B, size_t* bytes) {
   ClipPlan tmp;
@@ -297,37 +267,17 @@ static int clip_plan_bytes(cc_clip* h, bool text, int B, size_t* bytes) {
   return CC_OK;
 }
 static int clip_plan(cc_clip* h, bool text, int B, ClipPlan** out) {
-  ClipModel& M = h->m;
-  const std::string key = std::string(text ? "t" : "i") + std::to_string(B);
-  auto it = M.plans.find(key);
-  if (it != M.plans.end() && it->second->gen == M.arena.gen) {
-    it->second->last_use = ++M.tick;
-    *out = it->second.get();
-    return CC_OK;
-  }
-  size_t bytes = 0;
-  int rc = clip_plan_bytes(h, text, B, &bytes);
-  if (rc) return rc;
-  if ((rc = M.arena.reserve(bytes))) return rc;
-  for (auto p = M.plans.begin(); p != M.plans.end();)
-    p = (p->second->gen != M.arena.gen) ? M.plans.erase(p) : std::next(p);
-  std::unique_ptr<ClipPlan> P(new ClipPlan());
-  P->B = B; P->text = text;
-  PlanBuilder b(M, *P);
-  b.bump.base = static_cast<uint8_t*>(M.arena.base);
-  rc = text ? b.build_text(B) : b.build_image(B);
-  if (rc) return rc;
-  CC_REQUIRE(b.bump.off <= M.arena.cap, "clip plan: workspace overrun (%zu > %zu)", b.bump.off, M.arena.cap);
-  P->gen = M.arena.gen;
-  P->last_use = ++M.tick;
-  if (M.plans.size() >= kMaxClipPlans) {
-    auto lru = M.plans.begin();
-    for (auto p = M.plans.begin(); p != M.plans.end(); ++p)
-      if (p->second->last_use < lru->second->last_use) lru = p;
-    M.plans.erase(lru);
-  }
-  *out = (M.plans[key] = std::move(P)).get();
-  return CC_OK;
+  return h->m.plans.get(
+      std::string(text ? "t" : "i") + std::to_string(B), [&](size_t* bytes) { return clip_plan_bytes(h, text, B, bytes); },
+      [&](ClipPlan& P, uint8_t* base, size_t* used) {
+        P.B = B; P.text = text;
+        PlanBuilder b(h->m, P);
+        b.bump.base = base;
+        const int rc = text ? b.build_text(B) : b.build_image(B);
+        *used = b.bump.off;
+        return rc;
+      },
+      out);
 }
 
 int cc_clip_workspace_bytes(cc_clip* h, int text, int B, size_t* bytes) {
@@ -336,11 +286,8 @@ int cc_clip_workspace_bytes(cc_clip* h, int text, int B, size_t* bytes) {
 }
 
 int cc_clip_set_workspace(cc_clip* h, void* d_workspace, size_t bytes) {
-  CC_REQUIRE(h, "cc_clip_set_workspace: null handle");
-  CC_REQUIRE(d_workspace == nullptr || (reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0,
-             "cc_clip_set_workspace: the workspace must be 256-byte aligned");
-  h->m.plans.clear();
-  return h->m.arena.adopt(d_workspace, bytes);
+  if (int rc = check_workspace("cc_clip_set_workspace", h, d_workspace)) return rc;
+  return h->m.plans.adopt(d_workspace, bytes);
 }
 
 int cc_clip_encode_image(cc_clip* h, const float* d_x, int B, float* d_out, long long out_row_stride, void* stream) {

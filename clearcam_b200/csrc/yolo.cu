@@ -18,10 +18,6 @@
 #include "conv_gemm.cuh"
 #include "ops.cuh"
 #include <cmath>
-#include <map>
-#include <memory>
-#include <string>
-#include <vector>
 
 namespace cc {
 
@@ -139,7 +135,6 @@ static bool build_spec(const std::string& size, std::vector<Layer>* out) {
 }
 
 // ------------------------------------------------------------------------------------------------ weights
-struct HostT { const float* p; long long n; };
 struct ConvW {           // device-resident, kernel layout
   __nv_bfloat16* w = nullptr;   // [Cout][k][k][Cin_eff]  (Cin_eff = Cin when dense, Cin/groups when grouped)
   float* wf32 = nullptr;        // stem only: fp32 [Cout][3][3][3]
@@ -281,8 +276,6 @@ struct YoloPlan {
   bool table = false;
   std::vector<Op> ops;
   size_t alloc_bytes = 0;      // bytes of the handle's shared workspace this plan addresses
-  uint64_t gen = 0;            // workspace generation the pointers / TMA descriptors were built against
-  uint64_t last_use = 0;       // LRU stamp
   float* pred = nullptr;   // [B,A,6]
   float* raw = nullptr;    // [B,84,A] (allocated lazily when a tap is requested)
   void* lb_out = nullptr;  // letterboxed BGR frames (float32 for float frames, else uint8) or nullptr when identity
@@ -302,26 +295,17 @@ struct YoloPlan {
 struct YoloModel {
   std::string size;
   std::vector<Layer> spec;
-  std::map<std::string, HostT> host;     // borrowed pointers, valid only during create
+  DeviceWeights weights;
   std::map<std::string, ConvW> convs;
-  std::vector<void*> allocs;
-  std::map<std::string, std::unique_ptr<YoloPlan>> plans;   // bounded (kMaxPlans, least recently used goes first)
-  Arena arena;                 // activation workspace shared by all plans (size of the largest)
-  uint64_t tick = 0;
+  PlanCache<std::string, YoloPlan> plans{"yolo"};   // activation workspace shared by all plans (size of the largest)
   int sms = 0;
   cudaStream_t cap_stream = nullptr;   // private stream the graphs are captured on (the caller's may be the legacy default stream)
   // fp32-accurate mode (CC_YOLO_FP32_ACCURATE): activations are stored in fp32 and every conv runs on the same wgmma kernel
   // over a 3-way bf16 split of both operands (six plane products, fp32 accumulation): the result carries fp32-level error
   // instead of bf16's 2^-9, at ~6x the tensor work and 2x the activation bytes.  The mode the 1e-3 parity bar is checked in.
   bool precise = false;
-  ~YoloModel() { plans.clear(); if (cap_stream) cudaStreamDestroy(cap_stream); for (void* p : allocs) cudaFree(p); }
-
-  int upload(const void* h, size_t bytes, void** d) {
-    CC_CHECK_CUDA(cudaMalloc(d, bytes));
-    allocs.push_back(*d);
-    CC_CHECK_CUDA(cudaMemcpy(*d, h, bytes, cudaMemcpyHostToDevice));
-    return CC_OK;
-  }
+  // the plans' CUDA graph execs go before the capture stream and the workspace
+  ~YoloModel() { plans.plans.clear(); if (cap_stream) cudaStreamDestroy(cap_stream); }
 
   // Load conv `name` (PyTorch layout [Cout][Cin/g][k][k]) -> [Cout][k][k][Cin] bf16, optionally expanding groups
   // to block-diagonal dense, optionally stacking a second conv's output channels under it (fused 1x1 pair).
@@ -341,15 +325,14 @@ struct YoloModel {
     else if (precise) wf.assign(w.size(), 0.f);   // fp32-accurate mode: w's layout in fp32 (split into bf16 planes below)
     int co_base = 0;
     for (size_t t = 0; t < names.size(); ++t) {
-      auto iw = host.find(names[t] + ".weight"), ib = host.find(names[t] + ".bias");
-      CC_REQUIRE(iw != host.end() && ib != host.end(), "yolo: missing weight '%s'", names[t].c_str());
       const int cout = couts[t];
       const int src_cin_g = ci_total / groups;
-      CC_REQUIRE(iw->second.n == static_cast<long long>(cout) * src_cin_g * k * k && ib->second.n == cout,
-                 "yolo: '%s' has %lld weight / %lld bias elements, expected %lld / %d", names[t].c_str(), iw->second.n,
-                 ib->second.n, static_cast<long long>(cout) * src_cin_g * k * k, cout);
+      const float *src, *bsrc;
+      int rc;
+      if ((rc = weights.host.get(names[t] + ".weight", static_cast<long long>(cout) * src_cin_g * k * k, &src)) ||
+          (rc = weights.host.get(names[t] + ".bias", cout, &bsrc)))
+        return rc;
       CC_REQUIRE(ci_total == cin || groups == 1, "yolo: '%s': an input-channel sub-range of a grouped conv", names[t].c_str());
-      const float* src = iw->second.p;
       const int cpg_out = cout / groups;
       if (stem) {
         CC_REQUIRE(k == 3 && cin == 3 && groups == 1 && ci_total == 3, "yolo: stem '%s' is not a 3x3 conv over 3 channels", names[t].c_str());
@@ -366,7 +349,7 @@ struct YoloModel {
               w[o] = f2bf(v);
               if (precise) wf[o] = v;
             }
-        bias[co_base + co] = with_bias ? ib->second.p[co] : 0.f;
+        bias[co_base + co] = with_bias ? bsrc[co] : 0.f;
       }
       co_base += cout;
     }
@@ -374,24 +357,23 @@ struct YoloModel {
     cw.cin = cin; cw.cout = cout_total; cw.k = k; cw.groups = dense ? 1 : groups;
     int rc;
     if (stem) {
-      if ((rc = upload(wf.data(), wf.size() * 4, reinterpret_cast<void**>(&cw.wf32)))) return rc;
-      const std::vector<__nv_bfloat16> wt = stem_tc_weights(wf.data(), cout_total);
-      if ((rc = upload(wt.data(), wt.size() * 2, reinterpret_cast<void**>(&cw.wtc)))) return rc;
+      if ((rc = weights.upload(wf, &cw.wf32))) return rc;
+      if ((rc = weights.upload(stem_tc_weights(wf.data(), cout_total), &cw.wtc))) return rc;
     }
-    else if (!precise) { if ((rc = upload(w.data(), w.size() * 2, reinterpret_cast<void**>(&cw.w)))) return rc; }
+    else if (!precise) { if ((rc = weights.upload(w, &cw.w))) return rc; }
     else {
       hi_segments(cin_eff, k, &cw.seg_off, &cw.seg_c);
       std::vector<__nv_bfloat16> w5;
       std::vector<std::vector<__nv_bfloat16>> whi;
       split_weight_planes(wf.data(), static_cast<size_t>(cout_total) * k * k, cin_eff, cw.seg_off, cw.seg_c, &w5, &whi);
-      if ((rc = upload(w5.data(), w5.size() * 2, reinterpret_cast<void**>(&cw.w5)))) return rc;
+      if ((rc = weights.upload(w5, &cw.w5))) return rc;
       for (const std::vector<__nv_bfloat16>& ws : whi) {
         __nv_bfloat16* dptr = nullptr;
-        if ((rc = upload(ws.data(), ws.size() * 2, reinterpret_cast<void**>(&dptr)))) return rc;
+        if ((rc = weights.upload(ws, &dptr))) return rc;
         cw.whi.push_back(dptr);
       }
     }
-    if ((rc = upload(bias.data(), bias.size() * 4, reinterpret_cast<void**>(&cw.bias)))) return rc;
+    if ((rc = weights.upload(bias, &cw.bias))) return rc;
     convs[key] = cw;
     return CC_OK;
   }
@@ -1009,9 +991,7 @@ int cc_yolo_create_ex(const char* size, int flags, int n_tensors, const char* co
   M.sms = sms;
   M.precise = (flags & CC_YOLO_FP32_ACCURATE) != 0;
   CC_REQUIRE(build_spec(M.size, &M.spec), "cc_yolo_create: unknown size '%s' (t|s|m|c|e)", size);
-  for (int i = 0; i < n_tensors; ++i) M.host[names[i]] = HostT{h_data[i], static_cast<long long>(numels[i])};
-
-  int rc = CC_OK;
+  int rc = M.weights.host.fill("cc_yolo_create", n_tensors, names, h_data, numels);
   auto L = [&](const std::string& key, std::vector<std::string> nm, int cin, std::vector<int> couts, int k, int g = 1,
                bool stem = false, int ci_begin = 0, int ci_total = 0, bool with_bias = true) {
     if (rc) return;
@@ -1090,7 +1070,7 @@ int cc_yolo_create_ex(const char* size, int flags, int n_tensors, const char* co
       default: break;
     }
   }
-  M.host.clear();
+  M.weights.host.clear();
   if (rc) return rc;
   *out = h.release();
   return CC_OK;
@@ -1100,8 +1080,6 @@ int cc_yolo_destroy(cc_yolo* h) {
   delete h;
   return CC_OK;
 }
-
-static constexpr size_t kMaxPlans = 16;   // cached plans per handle (host metadata only: plans own no device memory)
 
 // frame_fmt is a CC_FRAME_* code; I420 needs even sides (4:2:0 chroma covers 2x2 blocks)
 static int check_frame_fmt(const char* who, int fmt, int Hf, int Wf) {
@@ -1133,40 +1111,21 @@ static int plan_bytes(cc_yolo* h, int fmt, int B, int Hf, int Wf, int res, size_
   return CC_OK;
 }
 static int get_plan(cc_yolo* h, int fmt, int B, int Hf, int Wf, int res, YoloPlan** out, bool table = false) {
-  YoloModel& M = h->m;
-  const std::string key = plan_key(fmt, B, Hf, Wf, res, table);
-  auto it = M.plans.find(key);
-  if (it != M.plans.end() && it->second->gen == M.arena.gen) {
-    it->second->last_use = ++M.tick;
-    *out = it->second.get();
-    return CC_OK;
-  }
-  size_t bytes = 0, scratch = 0, accb = 0;
-  int rc = plan_bytes(h, fmt, B, Hf, Wf, res, &bytes, &scratch, &accb, table);
-  if (rc) return rc;
-  if ((rc = M.arena.reserve(bytes))) return rc;
-  // plans built against an older workspace are stale (they are rebuilt on their next use)
-  for (auto p = M.plans.begin(); p != M.plans.end();)
-    p = (p->second->gen != M.arena.gen) ? M.plans.erase(p) : std::next(p);
-  std::unique_ptr<YoloPlan> P(new YoloPlan());
-  P->B = B; P->Hf = Hf; P->Wf = Wf; P->res = res; P->fmt = fmt; P->table = table;
-  Builder bld(M, *P);
-  bld.bump.base = static_cast<uint8_t*>(M.arena.base);
-  bld.scratch_bytes = scratch;
-  bld.acc_bytes = accb;
-  rc = bld.build();
-  if (rc) return rc;
-  CC_REQUIRE(bld.bump.off <= M.arena.cap, "yolo plan: workspace overrun (%zu > %zu)", bld.bump.off, M.arena.cap);
-  P->gen = M.arena.gen;
-  P->last_use = ++M.tick;
-  if (M.plans.size() >= kMaxPlans) {
-    auto lru = M.plans.begin();
-    for (auto p = M.plans.begin(); p != M.plans.end(); ++p)
-      if (p->second->last_use < lru->second->last_use) lru = p;
-    M.plans.erase(lru);
-  }
-  *out = (M.plans[key] = std::move(P)).get();
-  return CC_OK;
+  size_t scratch = 0, accb = 0;   // the measuring pass's fp32-accurate buffer sizes, carved by the real build
+  return h->m.plans.get(
+      plan_key(fmt, B, Hf, Wf, res, table),
+      [&](size_t* bytes) { return plan_bytes(h, fmt, B, Hf, Wf, res, bytes, &scratch, &accb, table); },
+      [&](YoloPlan& P, uint8_t* base, size_t* used) {
+        P.B = B; P.Hf = Hf; P.Wf = Wf; P.res = res; P.fmt = fmt; P.table = table;
+        Builder bld(h->m, P);
+        bld.bump.base = base;
+        bld.scratch_bytes = scratch;
+        bld.acc_bytes = accb;
+        const int rc = bld.build();
+        *used = bld.bump.off;
+        return rc;
+      },
+      out);
 }
 
 int cc_yolo_workspace_bytes(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, size_t* bytes) {
@@ -1176,11 +1135,8 @@ int cc_yolo_workspace_bytes(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, in
 }
 
 int cc_yolo_set_workspace(cc_yolo* h, void* d_workspace, size_t bytes) {
-  CC_REQUIRE(h, "cc_yolo_set_workspace: null handle");
-  CC_REQUIRE(d_workspace == nullptr || (reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0,
-             "cc_yolo_set_workspace: the workspace must be 256-byte aligned");
-  h->m.plans.clear();
-  return h->m.arena.adopt(d_workspace, bytes);
+  if (int rc = check_workspace("cc_yolo_set_workspace", h, d_workspace)) return rc;
+  return h->m.plans.adopt(d_workspace, bytes);
 }
 
 // Runs ops [first, last) of the plan on `st`: from its CUDA graph once the caller has passed the same (frames, out, raw)

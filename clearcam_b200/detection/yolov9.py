@@ -25,7 +25,7 @@ import numpy as np
 import torch
 
 from . import padding
-from .._lib import CC_MAX_FRAMES, CCError, check, lib, ptr, stream_ptr
+from .._lib import CC_MAX_FRAMES, CCError, Handle, _to_host_fp32, check, create, lib, ptr, stream_ptr
 from ..pixfmt import BGR24, CC_FRAME_BGR_F32, CC_FRAME_BGR_U8, CC_FRAME_I420_U8, check_pix_fmt, yuv420p_rows, yuv420p_size
 
 
@@ -46,14 +46,6 @@ class DeviceResult:
     def __array__(self, dtype=None):
         a = self.numpy()
         return a if dtype is None else a.astype(dtype)
-
-
-def _to_host_fp32(v) -> np.ndarray:
-    if isinstance(v, torch.Tensor):
-        return np.ascontiguousarray(v.detach().to("cpu", torch.float32).numpy())
-    if hasattr(v, "numpy") and not isinstance(v, np.ndarray):
-        v = v.numpy()
-    return np.ascontiguousarray(np.asarray(v, dtype=np.float32))
 
 
 def _as_tensor(v) -> torch.Tensor:
@@ -134,6 +126,19 @@ def fetch(url: str) -> str:
     raise CCError(f"cannot fetch {url}: no network; put the file under $CLEARCAM_B200_WEIGHTS or pass weights=")
 
 
+def load_weights_arg(weights, default: str):
+    """A model's `weights` argument -> its state dict: a state dict as it is, a path through safe_load, None the model's
+    own file at `default`, a URL (found through `fetch`) or a local path."""
+    if weights is None:
+        if "://" in default:
+            weights = fetch(default)
+        elif not os.path.exists(default):
+            raise CCError(f"weights not found at {default} (the reference's path); pass weights=")
+        else:
+            weights = default
+    return safe_load(weights) if isinstance(weights, (str, os.PathLike)) else weights
+
+
 def load_state_dict(model: "YOLOv9", state_dict) -> None:
     """tinygrad.nn.state.load_state_dict equivalent for this model (detection/yolov9.py:373)."""
     model.load_weights(state_dict)
@@ -190,8 +195,9 @@ def postprocess(output, max_det=300, conf_threshold=0.25, iou_threshold=0.45):
 
 
 # ----------------------------------------------------------------------------------------------- model
-class YOLOv9:
+class YOLOv9(Handle):
     """YOLOv9(size, res) — same constructor/call contract as the reference (detection/yolov9.py:298-388)."""
+    _destroy = "cc_yolo_destroy"
 
     def __init__(self, size: str = "t", res: int = 1280, weights=None, pad: bool = True, precise: bool = False):
         """pad=False keeps a size with odd widths (t) on its literal graph, whose narrow convs then take the generic
@@ -200,54 +206,23 @@ class YOLOv9:
         products on the tensor cores with fp32 accumulation, exact SiLU.  The reference is fp32 end to end; this is the
         mode that reproduces its boxes / scores at the north-star tolerance (the default stores activations in bf16)."""
         self.size, self.res, self.pad, self.precise = size, res, pad, bool(precise)
-        self._h = None
-        if weights is None:
-            weights = safe_load(fetch(f"https://huggingface.co/roryclear/yolov9/resolve/main/yolov9-{size}.safetensors"))
-        elif isinstance(weights, (str, os.PathLike)):
-            weights = safe_load(weights)
-        self.load_weights(weights)
+        self.load_weights(load_weights_arg(weights, f"https://huggingface.co/roryclear/yolov9/resolve/main/yolov9-{size}.safetensors"))
 
     # -- weights
     def load_weights(self, state_dict) -> None:
-        L = lib()
-        n = L.cc_device_check()
-        if n <= 0:
-            raise CCError("clearcam_b200 needs an H100 (sm_90) GPU: " + L.cc_last_error().decode())
-        sd = {k.replace(".list.", "."): _to_host_fp32(v) for k, v in state_dict.items() if not k.endswith(("anchors", "strides"))}
-        lib_size = self.size
-        if self.pad and padding.padded_size(self.size):
-            # t and m have widths that are not multiples of 16: run their zero-padded equivalents (same function,
-            # every conv on the tensor-core kernel) — see detection/padding.py
-            sd, lib_size = padding.pad_state_dict(self.size, sd), padding.padded_size(self.size)
-        items = list(sd.items())
-        names = (ctypes.c_char_p * len(items))(*[k.encode() for k, _ in items])
-        ptrs = (ctypes.c_void_p * len(items))(*[a.ctypes.data for _, a in items])
-        nums = (ctypes.c_int64 * len(items))(*[a.size for _, a in items])
-        h = ctypes.c_void_p()
-        check(L.cc_yolo_create_ex(lib_size.encode(), 1 if self.precise else 0, len(items), names, ptrs, nums, ctypes.byref(h)),
-              "cc_yolo_create_ex")
-        if self._h is not None:
-            L.cc_yolo_destroy(self._h)
-        self._h = h
+        # t and m have widths that are not multiples of 16: run their zero-padded equivalents (same function, every conv
+        # on the tensor-core kernel) — see detection/padding.py
+        lib_size = padding.padded_size(self.size) if self.pad and padding.padded_size(self.size) else self.size
 
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None) is not None:
-                lib().cc_yolo_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+        def tensors():
+            sd = {k.replace(".list.", "."): _to_host_fp32(v) for k, v in state_dict.items() if not k.endswith(("anchors", "strides"))}
+            return padding.pad_state_dict(self.size, sd) if lib_size != self.size else sd
+        self._adopt(create("cc_yolo_create_ex", tensors, lib_size.encode(), 1 if self.precise else 0))
 
     # -- inference
     @staticmethod
     def _as_device_frames(frames) -> torch.Tensor:
-        t = frames
-        if isinstance(t, DeviceResult):
-            t = t.tensor
-        if not isinstance(t, torch.Tensor):
-            if hasattr(t, "numpy") and not isinstance(t, np.ndarray):
-                t = t.numpy()                      # tinygrad Tensor & friends
-            t = torch.from_numpy(np.ascontiguousarray(t))
+        t = _as_tensor(frames)
         if t.dtype not in (torch.uint8, torch.float32):
             t = t.to(torch.float32)
         return t.to("cuda", non_blocking=True).contiguous()

@@ -11,14 +11,13 @@ libclearcam_b200.so (csrc/adaface.cu); there is no CPU fallback.
 from __future__ import annotations
 
 import ctypes
-import os
 from typing import Dict, List
 
 import numpy as np
 import torch
 
-from .._lib import CCError, check, lib, ptr, stream_ptr
-from ..detection.yolov9 import DeviceResult, fetch, safe_load
+from .._lib import CCError, Handle, check, create, lib, ptr, stream_ptr
+from ..detection.yolov9 import DeviceResult, _as_tensor, load_weights_arg
 from ..utils.helpers import batch_bucket
 
 SIDE, DIM = 112, 512
@@ -117,44 +116,20 @@ def fold_state_dict(sd) -> Dict[str, np.ndarray]:
 
 
 def _face_batch(faces) -> torch.Tensor:
-    t = faces.tensor if isinstance(faces, DeviceResult) else faces
-    if not isinstance(t, torch.Tensor):
-        if hasattr(t, "numpy") and not isinstance(t, np.ndarray):
-            t = t.numpy()
-        t = torch.from_numpy(np.ascontiguousarray(t))
+    t = _as_tensor(faces)
     if t.dtype != torch.uint8 or t.dim() != 4 or tuple(t.shape[1:]) != (SIDE, SIDE, 3) or t.shape[0] < 1:
         raise ValueError(f"faces must be uint8 [B,{SIDE},{SIDE},3] with B >= 1, got {t.dtype} {tuple(t.shape)}")
     return t.to("cuda", non_blocking=True).contiguous()
 
 
-class ADAFACE:
+class ADAFACE(Handle):
     """models/adaface.py:63-96.  `weights`: the reference's state dict (tensors or arrays under its key names), a
     .safetensors path, or None for the reference's file (found through `fetch`)."""
+    _destroy = "cc_face_destroy"
 
     def __init__(self, weights=None):
-        self._h = None
-        if weights is None:
-            weights = safe_load(fetch(WEIGHTS_URL))
-        elif isinstance(weights, (str, os.PathLike)):
-            weights = safe_load(weights)
-        L = lib()
-        if L.cc_device_check() <= 0:
-            raise CCError("clearcam_b200 needs an H100 (sm_90) GPU: " + L.cc_last_error().decode())
-        items = [(k, np.ascontiguousarray(v, np.float32)) for k, v in fold_state_dict(weights).items()]
-        names = (ctypes.c_char_p * len(items))(*[k.encode() for k, _ in items])
-        ptrs = (ctypes.c_void_p * len(items))(*[a.ctypes.data for _, a in items])
-        nums = (ctypes.c_int64 * len(items))(*[a.size for _, a in items])
-        h = ctypes.c_void_p()
-        check(L.cc_face_create(len(items), names, ptrs, nums, ctypes.byref(h)), "cc_face_create")
-        self._h = h
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None) is not None:
-                lib().cc_face_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+        weights = load_weights_arg(weights, WEIGHTS_URL)
+        self._adopt(create("cc_face_create", lambda: fold_state_dict(weights)))
 
     def embed(self, faces) -> torch.Tensor:
         """faces uint8 [B,112,112,3] (host or device, each as the reference's call receives it) -> device (B,512) fp32; row b
@@ -170,11 +145,7 @@ class ADAFACE:
 
     def __call__(self, x) -> DeviceResult:
         """ADAFACE.__call__: one HWC uint8 (112,112,3) image -> DeviceResult (1,512)."""
-        t = x.tensor if isinstance(x, DeviceResult) else x
-        if not isinstance(t, torch.Tensor):
-            if hasattr(t, "numpy") and not isinstance(t, np.ndarray):
-                t = t.numpy()
-            t = torch.from_numpy(np.ascontiguousarray(t))
+        t = _as_tensor(x)
         if tuple(t.shape) != (SIDE, SIDE, 3):
             raise ValueError(f"ADAFACE takes one ({SIDE},{SIDE},3) image, got {tuple(t.shape)}")
         return DeviceResult(self.embed(t.unsqueeze(0)))

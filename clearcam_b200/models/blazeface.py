@@ -11,17 +11,16 @@ fallback.
 from __future__ import annotations
 
 import ctypes
-import os
 
 import numpy as np
 import torch
 
-from .._lib import CCError, cc_face_warp, cc_frame, check, lib, ptr, stream_ptr
-from ..detection.yolov9 import DeviceResult, _to_host_fp32, safe_load
+from .._lib import Handle, cc_face_warp, cc_frame, check, create, lib, ptr, stream_ptr
+from ..detection.yolov9 import DeviceResult, _as_tensor, load_weights_arg
+from ..pixfmt import CC_FRAME_BGR_U8
 
 ANCHORS, COORDS = 896, 16
 WEIGHTS_PATH = "models/blazeface.safetensors"          # models/blazeface.py:134, relative to the reference's working directory
-CC_FRAME_BGR_U8 = 0
 FACE = 112
 TARGET_LEFT_EYE = np.array([38, 51])
 TARGET_RIGHT_EYE = np.array([73, 51])
@@ -50,37 +49,15 @@ def _images(images):
     return out
 
 
-class BlazeFace:
+class BlazeFace(Handle):
     """models/blazeface.py:62-232.  `weights`: the reference's state dict (tensors or arrays under its key names, the
     anchors included), a .safetensors path, or None for the reference's relative path models/blazeface.safetensors."""
+    _destroy = "cc_blazeface_destroy"
 
     def __init__(self, weights=None):
-        self._h = None
-        if weights is None:
-            if not os.path.exists(WEIGHTS_PATH):
-                raise CCError(f"BlazeFace weights not found at {WEIGHTS_PATH} (the reference's path); pass weights=")
-            weights = WEIGHTS_PATH
-        if isinstance(weights, (str, os.PathLike)):
-            weights = safe_load(weights)
-        L = lib()
-        if L.cc_device_check() <= 0:
-            raise CCError("clearcam_b200 needs an H100 (sm_90) GPU: " + L.cc_last_error().decode())
-        items = [(k, _to_host_fp32(v)) for k, v in weights.items()]
-        names = (ctypes.c_char_p * len(items))(*[k.encode() for k, _ in items])
-        ptrs = (ctypes.c_void_p * len(items))(*[a.ctypes.data for _, a in items])
-        nums = (ctypes.c_int64 * len(items))(*[a.size for _, a in items])
-        h = ctypes.c_void_p()
-        check(L.cc_blazeface_create(len(items), names, ptrs, nums, ctypes.byref(h)), "cc_blazeface_create")
-        self._h = h
+        weights = load_weights_arg(weights, WEIGHTS_PATH)
+        self._adopt(create("cc_blazeface_create", lambda: weights))
         self._ws = None
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None) is not None:
-                lib().cc_blazeface_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
 
     def _workspace(self, B: int) -> None:
         need = ctypes.c_size_t()
@@ -96,7 +73,7 @@ class BlazeFace:
         ims = _images(images)
         B = len(ims)
         self._workspace(B)
-        table = (cc_frame * B)(*[cc_frame(t.data_ptr(), CC_FRAME_BGR_U8, t.shape[0], t.shape[1]) for t in ims])
+        table = frame_table(ims)
         boxes = torch.empty(B, ANCHORS, COORDS, device="cuda", dtype=torch.float32)
         scores = torch.empty(B, ANCHORS, device="cuda", dtype=torch.float32)
         dets = torch.empty(B, ANCHORS, COORDS + 1, device="cuda", dtype=torch.float32)
@@ -124,10 +101,7 @@ class BlazeFace:
 
     def __call__(self, img) -> DeviceResult:
         """BlazeFace.__call__: one HWC uint8 image -> DeviceResult (896,17)."""
-        t = img.tensor if isinstance(img, DeviceResult) else img
-        if hasattr(t, "numpy") and not isinstance(t, (np.ndarray, torch.Tensor)):
-            t = t.numpy()
-        return DeviceResult(self.detect([t])[0])
+        return DeviceResult(self.detect([_as_tensor(img)])[0])
 
 
 def frame_table(ims):

@@ -26,8 +26,8 @@ from typing import Dict, List, Optional
 import numpy as np
 import torch
 
-from .._lib import CCError, check, lib, ptr, stream_ptr
-from ..detection.yolov9 import DeviceResult, _to_host_fp32, fetch, safe_load
+from .._lib import CCError, Handle, check, create, lib, ptr, stream_ptr
+from ..detection.yolov9 import DeviceResult, _as_tensor, load_weights_arg
 from ..pixfmt import BGR24, check_pix_fmt, yuv420p_size
 from ..utils.clip_tokenizer import SimpleTokenizer
 from ..utils.helpers import batch_bucket
@@ -51,7 +51,9 @@ def event_img_info(name: str) -> dict:
     return {"ts": parts[0], "object_id": parts[1] if len(parts) > 1 else None, "class": parts[2] if len(parts) > 2 else None}
 
 
-class OpenCLIP:
+class OpenCLIP(Handle):
+    _destroy = "cc_clip_destroy"
+
     def __init__(self, base_path="data/cameras", weights=None, arch: str = "ViT-L/14"):
         self.base_path = base_path
         self.arch = arch
@@ -60,47 +62,17 @@ class OpenCLIP:
         self.image_size = self.cfg[0]
         self.ctx = self.cfg[12]
         self.tokenizer = SimpleTokenizer()
-        self._h = None
-        if weights is None:
-            weights = safe_load(fetch("https://huggingface.co/roryclear/CLIP-ViT-L-14-laion2B-s32B-b82K/resolve/main/"
-                                      "CLIP-ViT-L-14-laion2B-s32B-b82K.safetensors"))
-        elif isinstance(weights, (str, os.PathLike)):
-            weights = safe_load(weights)
-        self.load_weights(weights)
+        self.load_weights(load_weights_arg(weights, "https://huggingface.co/roryclear/CLIP-ViT-L-14-laion2B-s32B-b82K/resolve/main/"
+                                                    "CLIP-ViT-L-14-laion2B-s32B-b82K.safetensors"))
 
     def load_weights(self, state_dict) -> None:
-        L = lib()
-        if L.cc_device_check() <= 0:
-            raise CCError("clearcam_b200 needs an H100 (sm_90) GPU: " + L.cc_last_error().decode())
-        items = [(k, _to_host_fp32(v)) for k, v in state_dict.items() if k != "attn_mask"]
-        names = (ctypes.c_char_p * len(items))(*[k.encode() for k, _ in items])
-        ptrs = (ctypes.c_void_p * len(items))(*[a.ctypes.data for _, a in items])
-        nums = (ctypes.c_int64 * len(items))(*[a.size for _, a in items])
-        cfg = _ClipConfig(*self.cfg)
-        h = ctypes.c_void_p()
-        check(L.cc_clip_create(ctypes.byref(cfg), len(items), names, ptrs, nums, ctypes.byref(h)), "cc_clip_create")
-        if self._h is not None:
-            L.cc_clip_destroy(self._h)
-        self._h = h
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None) is not None:
-                lib().cc_clip_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+        tensors = lambda: {k: v for k, v in state_dict.items() if k != "attn_mask"}     # noqa: E731
+        self._adopt(create("cc_clip_create", tensors, ctypes.byref(_ClipConfig(*self.cfg))))
 
     # ---- image tower
     @staticmethod
     def _as_device(x, dtype) -> torch.Tensor:
-        if isinstance(x, DeviceResult):
-            x = x.tensor
-        if not isinstance(x, torch.Tensor):
-            if hasattr(x, "numpy") and not isinstance(x, np.ndarray):
-                x = x.numpy()
-            x = torch.from_numpy(np.ascontiguousarray(x))
-        return x.to("cuda", dtype, non_blocking=True).contiguous()
+        return _as_tensor(x).to("cuda", dtype, non_blocking=True).contiguous()
 
     def embed_into(self, x, out: torch.Tensor, row0: int = 0, stream=None) -> None:
         """precompute_embedding writing rows [row0, row0+B) of `out` ([N, embed_dim] fp32 CUDA) in place."""
@@ -183,9 +155,7 @@ def _device_crops(frames, rects, bgr: bool, pix_fmt: str):
     """The frame / rect conventions of `ObjectFinder.preprocess_device` and `encode_crops`: frames uint8 [n,H,W,3] / [H,W,3]
     (bgr24) or [n,H*3/2,W] / [H*3/2,W] (yuv420p), host or device; rects K rows of (frame, x1, y1, x2, y2) or (x1, y1, x2,
     y2).  -> (contiguous device frames [n,...], H, W, the C-ABI src_fmt (0 RGB, 1 BGR, 2 I420), int32 rects [K,5])."""
-    t = frames.tensor if isinstance(frames, DeviceResult) else frames
-    if not isinstance(t, torch.Tensor):
-        t = torch.from_numpy(np.ascontiguousarray(t))
+    t = _as_tensor(frames)
     if check_pix_fmt(pix_fmt) == BGR24:
         if t.dim() == 3:
             t = t.unsqueeze(0)

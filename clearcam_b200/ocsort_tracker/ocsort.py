@@ -15,7 +15,7 @@ import numpy as np
 
 from .._lib import (CC_ALERT_DESC, CC_ALERT_MAX_ALERTS, CC_ALERT_OK, CC_ALERT_ON, CC_ALERT_SCHED, CC_ALERT_ZONE, CC_EVENT_BAD_BOX,
                     CC_EVENT_BAD_ORDER, CC_EVENT_NEEDS_ROOM, CC_EVENT_OK, CC_TRACK_BAD_BOX, CC_TRACK_BAD_CLASS, CC_TRACK_NEEDS_ROOM, CC_TRACK_OK,
-                    CC_TRACK_OVERFLOW, CCError, cc_alert, cc_track_run, check, lib)
+                    CC_TRACK_OVERFLOW, CCError, Handle, cc_alert, cc_track_run, check, lib)
 from .STrack import STrack
 
 _CAP = 1024          # rows of the result buffer (the detector emits at most 300 boxes per frame)
@@ -110,7 +110,9 @@ class _EventBuffers:
         self.alerts = False                                                           # whether the alerts ran
 
 
-class OCSort:
+class OCSort(Handle):
+    _destroy = "cc_ocsort_destroy"
+
     def __init__(self, det_thresh=0.25, max_age=30, min_hits=3, iou_threshold=0.3, delta_t=3, asso_func="iou", inertia=0.2,
                  use_byte=False):
         if asso_func != "iou":
@@ -122,14 +124,6 @@ class OCSort:
         check(lib().cc_ocsort_create(int(max_age), int(min_hits), float(iou_threshold), int(delta_t), float(inertia),
                                      int(bool(use_byte)), ctypes.byref(self._h)), "cc_ocsort_create")
         self._out = np.empty((_CAP, 9), np.float64)
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                lib().cc_ocsort_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
 
     def __len__(self):
         return lib().cc_ocsort_num_tracks(self._h)
@@ -165,7 +159,7 @@ def update_many(trackers: Sequence[Optional[OCSort]], results, det_thresh) -> Li
     return [_tracks(out[b], int(n[b])) if trackers[b] is not None else [] for b in range(B)]
 
 
-class DeviceTrackers:
+class DeviceTrackers(Handle):
     """One `OCSort` per camera, all on the GPU (csrc/ocsort_gpu.cu): `update` steps every camera of a list of jobs in one
     launch per CC_MAX_FRAMES cameras, on detector rows that never leave the device, and returns what `update_many` returns
     for the same rows, bit for bit (track ids included).
@@ -175,6 +169,7 @@ class DeviceTrackers:
         [targets] = trk.update([("cam0", rows, 0.5)])       # rows: CUDA float32 (n,6), e.g. one row of detect_batch's output
 
     `launch` / `finish` split `update` around a synchronisation the caller does anyway (CameraBatch.step)."""
+    _destroy = "cc_ocsort_gpu_destroy"
 
     def __init__(self, slots: int = 1024, max_delta_t: int = 8, capacity: int = 64, event_capacity: int = 64):
         import torch
@@ -190,14 +185,6 @@ class DeviceTrackers:
         self._ebufs, self._rbufs = [], []                      # events outputs: per launch, and for reruns after growth
         self._al = set()                                       # cameras with alerts configured
         self._n_alerts = {}                                    # camera -> its number of alerts
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                lib().cc_ocsort_gpu_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
 
     def __contains__(self, cam):
         return cam in self._slot

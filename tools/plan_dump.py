@@ -4,19 +4,26 @@ forward returns on seeded frames.  A host-side change to how convs are described
 
 usage:  python tools/plan_dump.py OUT.txt
 Covers the sizes bench.py runs (c at B=32 and e at B=16, 640x640; c on 1080p frames), small t / s / m plans, the default
-and the fp32-accurate mode, a frame-table call over frames of two shapes, and both CLIP towers (ViT-B/32, ViT-L/14)."""
+and the fp32-accurate mode, a frame-table call over frames of two shapes, both CLIP towers (ViT-B/32, ViT-L/14), AdaFace
+embeddings on synthetic weights and BlazeFace detections on the reference's weights (tests/golden/blazeface_ref.npz)."""
 import hashlib
 import os
 import sys
+
+import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
+from oracle import adaface as oa  # noqa: E402
+from oracle import blazeface as obf  # noqa: E402
 from oracle import clip as oc  # noqa: E402
 from oracle import yolov9 as o  # noqa: E402
 from clearcam_b200.detection.yolov9 import YOLOv9  # noqa: E402
+from clearcam_b200.models.adaface import ADAFACE  # noqa: E402
+from clearcam_b200.models.blazeface import BlazeFace  # noqa: E402
 from clearcam_b200.models.objects import OpenCLIP  # noqa: E402
 
 #        size res  B   H     W     modes (False: bf16 storage, True: fp32-accurate)
@@ -67,6 +74,17 @@ def main():
                 say("clip", arch, tower, r["name"], repr(r["flops"]))
         say("clip", arch, "outputs", sha(cm.precompute_embedding(x).tensor, cm.encode_token_ids(ids).tensor))
         del cm
+    fm = ADAFACE(oa.synthetic_weights(seed=5))
+    for B in (1, 3, 16, 64, 200):
+        say("adaface", f"B{B}", "outputs", sha(fm.embed(oa.synthetic_faces(B, seed=B))))
+    del fm
+    det = BlazeFace({k: v.numpy() for k, v in obf.load_weights(os.path.join(ROOT, "tests", "golden", "blazeface_ref.npz")).items()})
+    sizes = [(256, 256), (640, 640), (480, 640), (97, 300), (333, 129), (720, 1280), (1080, 1920)]
+    for B in (1, 7, 64):
+        g = np.random.default_rng(B)
+        ims = [g.integers(0, 256, (*sizes[i % len(sizes)], 3), dtype=np.uint8) for i in range(B)]
+        say("blazeface", f"B{B}", "outputs", sha(*det.forward(ims)))
+    del det
     out.close()
 
 
