@@ -53,17 +53,17 @@ class cc_track_run(ctypes.Structure):
 
 
 class cc_slice(ctypes.Structure):
-    """An NHWC slice as cc_yolo_op_conv reports it: device pointer, channels per pixel, first channel, channels, N, H, W, fp32."""
+    """An NHWC slice of a conv launch: device pointer, channels per pixel, first channel, channels, N, H, W, fp32."""
     _fields_ = [("p", ctypes.c_void_p)] + [(n, ctypes.c_int) for n in ("cs", "co", "C", "N", "H", "W", "f32")]
 
 
 class cc_conv_op(ctypes.Structure):
-    """One op of a detector plan as cc_yolo_op_conv describes it (include/clearcam_b200.h); `in_` is the header's `in`."""
+    """One conv launch as cc_conv takes it and cc_yolo_op_conv reports it (include/clearcam_b200.h); `in_` is the header's `in`."""
     _fields_ = ([("kind", ctypes.c_int), ("name", ctypes.c_char * 128), ("in_", cc_slice), ("out", cc_slice), ("res", cc_slice),
                  ("w", ctypes.c_void_p), ("bias", ctypes.c_void_p)]
                 + [(n, ctypes.c_int) for n in ("k", "stride", "groups", "act")]
-                + [("pre", ctypes.c_void_p), ("pre_h", ctypes.c_int), ("pre_w", ctypes.c_int), ("w2", ctypes.c_void_p),
-                   ("bias2", ctypes.c_void_p), ("act2", ctypes.c_int), ("k0", ctypes.c_int), ("part", cc_slice), ("out2", cc_slice),
+                + [("slope", ctypes.c_void_p), ("pre", ctypes.c_void_p), ("pre_h", ctypes.c_int), ("pre_w", ctypes.c_int),
+                   ("w2", ctypes.c_void_p), ("bias2", ctypes.c_void_p), ("act2", ctypes.c_int), ("k0", ctypes.c_int), ("part", cc_slice), ("out2", cc_slice),
                    ("store1", ctypes.c_int)]
                 + [(n, ctypes.c_int) for n in ("BN", "BK", "lTW", "lTH", "lTN", "s2", "stages", "b_res", "grid", "num_tiles",
                                                "BNn", "narrow_tiles")])
@@ -98,9 +98,7 @@ _SIGS = {
     "cc_version": (_i, []),
     "cc_last_error": (ctypes.c_char_p, []),
     "cc_device_check": (_i, []),
-    "cc_conv2d": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp]),
-    "cc_conv2d_chain": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _i, _i, _i,
-                             _vp, _i, _i, _i, _vp, _i, _i, _i, _vp]),
+    "cc_conv": (_i, [ctypes.POINTER(cc_conv_op), _vp]),
     "cc_yolo_create": (_i, [ctypes.c_char_p, _i, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_vp),
                             ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(_vp)]),
     "cc_yolo_create_ex": (_i, [ctypes.c_char_p, _i, _i, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_vp),
@@ -132,7 +130,6 @@ _SIGS = {
     "cc_clip_encode_text": (_i, [_vp, _vp, _i, _vp, ctypes.c_longlong, _vp]),
     "cc_clip_profile": (_i, [_vp, _i, _vp, _i, _vp, _i, ctypes.POINTER(_f), ctypes.POINTER(ctypes.c_double),
                              ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_i), ctypes.POINTER(ctypes.c_double), _vp]),
-    "cc_conv2d_prelu": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _i, _vp]),
     "cc_face_create": (_i, [_i, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_vp), ctypes.POINTER(ctypes.c_int64),
                             ctypes.POINTER(_vp)]),
     "cc_face_destroy": (_i, [_vp]),
@@ -195,7 +192,6 @@ _SIGS = {
     "cc_finish_f32": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp]),
     "cc_stem": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, ctypes.c_size_t,
                      ctypes.POINTER(ctypes.c_size_t), _vp]),
-    "cc_conv2d_pre": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _i, _vp]),
     "cc_conv2d_fp32_accurate": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp,
                                      ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t), _vp]),
     "cc_patchify": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),

@@ -1,10 +1,71 @@
 // C-ABI entry points (include/clearcam_b200.h).
+#include <utility>
 #include "clearcam_b200.h"
 #include "cc_common.h"
 #include "conv_gemm.cuh"
 #include "ops.cuh"
 
 using namespace cc;
+
+// ---- one conv launch: the public cc_conv_op and the descriptors the conv kernels are built from, both ways
+static TSlice conv_slice(const cc_slice& s) { return nhwc_slice(s.p, s.cs, s.co, s.C, s.f32, s.N, s.H, s.W); }
+
+static cc_slice op_slice(const TSlice& t, int N, int H, int W) {
+  cc_slice s{};
+  s.p = t.p; s.cs = t.cs; s.co = t.co; s.C = t.C; s.N = N; s.H = H; s.W = W; s.f32 = t.f32;
+  return s;
+}
+
+namespace cc {
+
+ConvDesc conv_desc_of(const cc_conv_op& o, ChainDesc* c) {
+  const TSlice res = conv_slice(o.res);
+  ConvDesc d = conv_desc(conv_slice(o.in), o.w, o.bias, o.k, o.stride, conv_slice(o.out), o.act, o.res.p ? &res : nullptr);
+  d.slope = o.slope;
+  d.bn_override = o.BN;
+  d.pre = o.pre; d.pre_h = o.pre_h; d.pre_w = o.pre_w;
+  *c = ChainDesc{};
+  if (o.kind == CC_CONV_OP_CHAIN) {
+    c->w = o.w2; c->bias = o.bias2; c->act = o.act2; c->k0 = o.k0;
+    if (o.part.p) c->part = conv_slice(o.part);
+    c->out = conv_slice(o.out2);
+    c->store1 = o.store1 != 0;
+  }
+  return d;
+}
+
+cc_conv_op conv_op_of(const ConvDesc& d, const ChainDesc& c, const GemmLaunch& L) {
+  const GemmParams& g = L.p;
+  const int N = d.in.N, Ho = conv_out(d.in.H, d.stride), Wo = conv_out(d.in.W, d.stride);
+  cc_conv_op o{};
+  o.kind = c.out.p ? CC_CONV_OP_CHAIN : CC_CONV_OP_GEMM;
+  o.in = op_slice(d.in, N, d.in.H, d.in.W);
+  o.out = op_slice(d.out, N, Ho, Wo);
+  if (d.res.p) o.res = op_slice(d.res, N, Ho, Wo);
+  o.w = d.w; o.bias = d.bias; o.k = d.k; o.stride = d.stride; o.groups = 1; o.act = d.act; o.slope = d.slope;
+  o.pre = d.pre; o.pre_h = d.pre_h; o.pre_w = d.pre_w;
+  if (c.out.p) {
+    o.w2 = c.w; o.bias2 = c.bias; o.act2 = c.act; o.k0 = c.k0;
+    if (c.part.p) o.part = op_slice(c.part, N, Ho, Wo);
+    o.out2 = op_slice(c.out, N, Ho, Wo);
+    o.store1 = c.store1 ? 1 : 0;
+  }
+  o.BN = g.BN; o.BK = g.BK; o.lTW = g.lTW; o.lTH = g.lTH; o.lTN = g.lTN; o.s2 = g.s2; o.stages = g.stages; o.b_res = g.b_res;
+  o.grid = L.grid; o.num_tiles = g.num_tiles; o.BNn = g.BNn; o.narrow_tiles = g.num_tiles - g.num_wide;
+  return o;
+}
+
+cc_conv_op conv_op_of(const DirectConvParams& p) {
+  cc_conv_op o{};
+  o.kind = CC_CONV_OP_DIRECT;
+  o.in = op_slice(nhwc_slice(p.in, p.in_cs, p.in_co, p.Cin), p.N, p.Hin, p.Win);
+  o.out = op_slice(nhwc_slice(p.out, p.out_cs, p.out_co, p.Cout, p.out_f32), p.N, p.Hout, p.Wout);
+  if (p.res) o.res = op_slice(nhwc_slice(p.res, p.res_cs, p.res_co, p.Cout, p.out_f32), p.N, p.Hout, p.Wout);
+  o.w = p.w; o.bias = p.bias; o.k = p.k; o.stride = p.stride; o.groups = p.groups; o.act = p.act;
+  return o;
+}
+
+}  // namespace cc
 
 extern "C" {
 
@@ -16,64 +77,59 @@ int cc_device_check(void) {
   return n;
 }
 
-int cc_conv2d(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const void* d_w,
-              const float* d_bias, int Cout, int k, int stride, int groups, void* d_out, int out_cs, int out_co,
-              int out_f32, int act, const void* d_res, int res_cs, int res_co, int impl, int bn, void* stream) {
-  const int sms = device_sm_count();
-  CC_REQUIRE(sms > 0, "cc_conv2d: no sm_90 (H100) device");
-  const TSlice res = nhwc_slice(d_res, res_cs, res_co, Cout, out_f32);
-  ConvDesc d = conv_desc(nhwc_slice(d_in, in_cs, in_co, Cin, 0, N, Hin, Win), d_w, d_bias, k, stride,
-                         nhwc_slice(d_out, out_cs, out_co, Cout, out_f32), act, d_res ? &res : nullptr);
-  d.bn_override = bn;
-  const bool gemm_ok = groups == 1 && conv_gemm_supported(d);
-  CC_REQUIRE(impl != 1 || gemm_ok, "cc_conv2d: shape not supported by the wgmma path");
-  if (impl != 2 && gemm_ok) {
-    GemmLaunch L;
-    int rc = conv_gemm_build(d, sms, &L);
-    if (rc) return rc;
-    return conv_gemm_launch(L, static_cast<cudaStream_t>(stream));
+int cc_conv(const cc_conv_op* op, void* stream) {
+  CC_REQUIRE(op != nullptr, "cc_conv: op is NULL");
+  const cc_conv_op& o = *op;
+  const bool chain = o.kind == CC_CONV_OP_CHAIN, direct = o.kind == CC_CONV_OP_DIRECT;
+  CC_REQUIRE(o.kind == CC_CONV_OP_GEMM || chain || direct, "cc_conv: unknown kind %d (%d GEMM, %d CHAIN, %d DIRECT)", o.kind,
+             CC_CONV_OP_GEMM, CC_CONV_OP_CHAIN, CC_CONV_OP_DIRECT);
+  CC_REQUIRE(o.in.p != nullptr, "cc_conv: in.p is NULL");
+  CC_REQUIRE(o.w != nullptr, "cc_conv: w is NULL");
+  CC_REQUIRE(o.out.p != nullptr || (chain && !o.store1), "cc_conv: out.p is NULL (only a CHAIN with store1 = 0 drops its output)");
+  CC_REQUIRE(!chain || (o.w2 && o.out2.p), "cc_conv: a CHAIN needs w2 and out2.p (w2=%p out2.p=%p)", o.w2, o.out2.p);
+  CC_REQUIRE(o.in.N >= 1 && o.in.H >= 1 && o.in.W >= 1 && o.in.C >= 1 && o.out.C >= 1 && (o.k == 1 || o.k == 3) &&
+             (o.stride == 1 || o.stride == 2),
+             "cc_conv: bad shape N=%d H=%d W=%d Cin=%d Cout=%d k=%d stride=%d (k 1 or 3, stride 1 or 2)", o.in.N, o.in.H, o.in.W,
+             o.in.C, o.out.C, o.k, o.stride);
+  CC_REQUIRE(!o.in.f32 && (!o.res.p || o.res.f32 == o.out.f32), "cc_conv: in is bf16 and res has out's dtype (in.f32=%d res.f32=%d "
+             "out.f32=%d)", o.in.f32, o.res.f32, o.out.f32);
+  // pad = k/2 with k odd: the direct kernel's extent, and conv_out() of every shape the wgmma kernel takes
+  const int N = o.in.N, Ho = (o.in.H - 1) / o.stride + 1, Wo = (o.in.W - 1) / o.stride + 1;
+  const std::pair<const char*, const cc_slice*> outs[] = {{"out", &o.out}, {"res", &o.res}, {"part", &o.part}, {"out2", &o.out2}};
+  for (const auto& [what, s] : outs) {
+    if (!s->p) continue;
+    CC_REQUIRE(s->N == N && s->H == Ho && s->W == Wo, "cc_conv: %s is %dx%dx%d, the output %dx%dx%d (N x H x W)", what, s->N, s->H,
+               s->W, N, Ho, Wo);
+    CC_REQUIRE(s->C > 0 && s->co >= 0 && s->co + s->C <= s->cs, "cc_conv: %s slice cs=%d co=%d C=%d outside its row", what, s->cs,
+               s->co, s->C);
   }
-  return conv_direct_launch(direct_conv_params(d, groups), static_cast<cudaStream_t>(stream));
-}
-
-int cc_conv2d_chain(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const void* d_w, const float* d_bias,
-                    int Cout, int k, int stride, void* d_out, int out_cs, int out_co, int store1, const void* d_res, int res_cs,
-                    int res_co, const void* d_w2, const float* d_bias2, int Cout2, int act2, int k0, const void* d_part, int part_cs,
-                    int part_co, int part_C, void* d_out2, int out2_cs, int out2_co, int out2_f32, void* stream) {
+  if (o.pre) {
+    CC_REQUIRE((reinterpret_cast<uintptr_t>(o.pre) & 15) == 0, "cc_conv: pre=%p must be 16-byte aligned", o.pre);
+    CC_REQUIRE(Ho % 2 == 0 && Wo % 2 == 0, "cc_conv: the output %dx%d must have even sides (pre is its half-resolution map)", Ho, Wo);
+    CC_REQUIRE(o.pre_h == Ho / 2 && o.pre_w == Wo / 2, "cc_conv: pre is %dx%d, the output's half resolution %dx%d", o.pre_h, o.pre_w,
+               Ho / 2, Wo / 2);
+  }
+  if (o.act == CC_ACT_PRELU) {
+    CC_REQUIRE(o.bias && o.slope, "cc_conv: CC_ACT_PRELU needs its [9][Cout] bias table and slope (bias=%p slope=%p)", o.bias, o.slope);
+    CC_REQUIRE(!o.out.f32, "cc_conv: CC_ACT_PRELU writes bf16, got out.f32=%d", o.out.f32);
+  }
+  ChainDesc c;
+  const ConvDesc d = conv_desc_of(o, &c);
+  if (direct) {
+    CC_REQUIRE(!o.pre && o.act != CC_ACT_PRELU && !o.out2.p, "cc_conv: the direct kernel takes no pre, PReLU or chained output "
+               "(pre=%p act=%d out2.p=%p)", o.pre, o.act, o.out2.p);
+  } else {
+    CC_REQUIRE(o.groups == 1, "cc_conv: the wgmma kernel takes groups = 1, got %d", o.groups);
+    CC_REQUIRE(conv_gemm_supported(d), "cc_conv: shape not supported by the wgmma conv (Cin=%d in_cs=%d in_co=%d Cout=%d k=%d "
+               "stride=%d H=%d W=%d)", o.in.C, o.in.cs, o.in.co, o.out.C, o.k, o.stride, o.in.H, o.in.W);
+  }
   const int sms = device_sm_count();
-  CC_REQUIRE(sms > 0, "cc_conv2d_chain: no sm_90 (H100) device");
-  CC_REQUIRE(d_in && (d_out || !store1) && d_w2 && d_out2 && (!d_part || part_C > 0), "cc_conv2d_chain: NULL argument");
-  CC_REQUIRE(!d_part || (part_co >= 0 && part_co + part_C <= part_cs), "cc_conv2d_chain: partner slice outside its row");
-  const TSlice res = nhwc_slice(d_res, res_cs, res_co, Cout);
-  const ConvDesc d = conv_desc(nhwc_slice(d_in, in_cs, in_co, Cin, 0, N, Hin, Win), d_w, d_bias, k, stride,
-                               nhwc_slice(d_out, out_cs, out_co, Cout), CC_ACT_SILU, d_res ? &res : nullptr);
-  ChainDesc c{};
-  c.w = d_w2; c.bias = d_bias2; c.act = act2; c.k0 = k0;
-  if (d_part) c.part = nhwc_slice(d_part, part_cs, part_co, part_C);
-  c.out = nhwc_slice(d_out2, out2_cs, out2_co, Cout2, out2_f32);
-  c.store1 = store1 != 0;
-  CC_REQUIRE(out2_co >= 0 && out2_co + Cout2 <= out2_cs, "cc_conv2d_chain: second output slice outside its row");
+  CC_REQUIRE(sms > 0, "cc_conv: no sm_90 (H100) device");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (direct) return conv_direct_launch(direct_conv_params(d, o.groups), st);
   GemmLaunch L;
-  if (int rc = conv_gemm_chain_build(d, c, sms, &L)) return rc;
-  return conv_gemm_launch(L, static_cast<cudaStream_t>(stream));
-}
-
-int cc_conv2d_prelu(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const void* d_w, const float* d_bias_cls,
-                    const float* d_slope, int Cout, int k, int stride, void* d_out, int out_cs, int out_co, const void* d_res,
-                    int res_cs, int res_co, int bn, void* stream) {
-  CC_REQUIRE(d_in && d_w && d_bias_cls && d_slope && d_out, "cc_conv2d_prelu: d_in, d_w, d_bias_cls, d_slope and d_out must not be NULL");
-  CC_REQUIRE(N >= 1 && Hin >= 1 && Win >= 1, "cc_conv2d_prelu: bad shape N=%d Hin=%d Win=%d", N, Hin, Win);
-  const TSlice res = nhwc_slice(d_res, res_cs, res_co, Cout);
-  ConvDesc d = conv_desc(nhwc_slice(d_in, in_cs, in_co, Cin, 0, N, Hin, Win), d_w, d_bias_cls, k, stride,
-                         nhwc_slice(d_out, out_cs, out_co, Cout), ACT_PRELU, d_res ? &res : nullptr);
-  d.slope = d_slope;
-  d.bn_override = bn;
-  CC_REQUIRE(conv_gemm_supported(d), "cc_conv2d_prelu: shape not supported by the wgmma conv (Cin=%d Cout=%d k=%d stride=%d)", Cin, Cout, k, stride);
-  const int sms = device_sm_count();
-  CC_REQUIRE(sms > 0, "cc_conv2d_prelu: no sm_90 (H100) device");
-  GemmLaunch L;
-  if (int rc = conv_gemm_build(d, sms, &L)) return rc;
-  return conv_gemm_launch(L, static_cast<cudaStream_t>(stream));
+  if (int rc = chain ? conv_gemm_chain_build(d, c, sms, &L) : conv_gemm_build(d, sms, &L)) return rc;
+  return conv_gemm_launch(L, st);
 }
 
 int cc_attention(const void* d_qkv, int B, int L, int H, int causal, int impl, void* d_ws, size_t ws_bytes, void* d_ctx,
@@ -182,26 +238,6 @@ int cc_finish_f32(const float* d_acc, const float* d_bias, int act, int npix, in
   p.out = d_out; p.out_cs = out_cs; p.out_co = out_co;
   p.res = d_res; p.res_cs = res_cs; p.res_co = res_co;
   return finish_f32_launch(p, static_cast<cudaStream_t>(stream));
-}
-
-int cc_conv2d_pre(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const void* d_w, const float* d_bias,
-                  int Cout, int k, int stride, void* d_out, int out_cs, int out_co, int out_f32, int act, const float* d_pre, int bn,
-                  void* stream) {
-  CC_REQUIRE(d_in && d_w && d_out && d_pre, "cc_conv2d_pre: d_in, d_w, d_out and d_pre must not be NULL");
-  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_pre) & 15) == 0, "cc_conv2d_pre: d_pre must be 16-byte aligned");
-  CC_REQUIRE(N >= 1 && Hin >= 1 && Win >= 1 && (stride == 1 || stride == 2), "cc_conv2d_pre: bad shape N=%d Hin=%d Win=%d stride=%d", N, Hin, Win, stride);
-  const int Ho = conv_out(Hin, stride), Wo = conv_out(Win, stride);
-  CC_REQUIRE(Ho % 2 == 0 && Wo % 2 == 0, "cc_conv2d_pre: the output %dx%d must have even sides (pre is its half-resolution map)", Ho, Wo);
-  ConvDesc d = conv_desc(nhwc_slice(d_in, in_cs, in_co, Cin, 0, N, Hin, Win), d_w, d_bias, k, stride,
-                         nhwc_slice(d_out, out_cs, out_co, Cout, out_f32), act);
-  d.bn_override = bn;
-  d.pre = d_pre; d.pre_h = Ho / 2; d.pre_w = Wo / 2;
-  CC_REQUIRE(conv_gemm_supported(d), "cc_conv2d_pre: shape not supported by the wgmma conv (Cin=%d Cout=%d k=%d stride=%d)", Cin, Cout, k, stride);
-  const int sms = device_sm_count();
-  CC_REQUIRE(sms > 0, "cc_conv2d_pre: no sm_90 (H100) device");
-  GemmLaunch L;
-  if (int rc = conv_gemm_build(d, sms, &L)) return rc;
-  return conv_gemm_launch(L, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

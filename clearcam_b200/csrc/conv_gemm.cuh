@@ -124,4 +124,10 @@ int conv_gemm_chain_build(const ConvDesc& d, const ChainDesc& c, int num_sms, Ge
 int conv_gemm_launch(const GemmLaunch& L, cudaStream_t stream);
 bool conv_gemm_supported(const ConvDesc& d);
 
+// The public description of one conv launch (cc_conv_op) and the descriptors above, both ways (api.cu): what cc_conv launches
+// (c is set for CC_CONV_OP_CHAIN only), and what cc_yolo_op_conv reports of a plan's GEMM or direct launch (name left empty).
+ConvDesc conv_desc_of(const cc_conv_op& o, ChainDesc* c);
+cc_conv_op conv_op_of(const ConvDesc& d, const ChainDesc& c, const GemmLaunch& L);
+cc_conv_op conv_op_of(const DirectConvParams& p);
+
 }  // namespace cc

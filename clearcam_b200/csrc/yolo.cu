@@ -1344,12 +1344,6 @@ int cc_yolo_trace(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf
 }
 
 // conv op taps: what each conv launch of the cached plan computes, and the plan run one range of ops at a time
-static cc_slice op_slice(const TSlice& t, int N, int H, int W) {
-  cc_slice s{};
-  s.p = t.p; s.cs = t.cs; s.co = t.co; s.C = t.C; s.N = N; s.H = H; s.W = W; s.f32 = t.f32;
-  return s;
-}
-
 int cc_yolo_op_conv(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int i, cc_conv_op* out) {
   CC_REQUIRE(h, "cc_yolo_op_conv: null handle");
   if (int rc = check_frame_fmt("cc_yolo_op_conv", frame_fmt, Hf, Wf)) return rc;
@@ -1359,37 +1353,8 @@ int cc_yolo_op_conv(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, i
   if (!out) return n;
   CC_REQUIRE(i >= 0 && i < n, "cc_yolo_op_conv: op %d of a plan of %d ops", i, n);
   const Op& op = P->ops[i];
-  cc_conv_op& o = *out;
-  o = cc_conv_op{};
-  snprintf(o.name, sizeof(o.name), "%s", op.name.c_str());
-  if (op.kind == Op::DIRECT) {
-    const DirectConvParams& p = op.direct;
-    o.kind = CC_CONV_OP_DIRECT;
-    o.in = op_slice(nhwc_slice(p.in, p.in_cs, p.in_co, p.Cin), p.N, p.Hin, p.Win);
-    o.out = op_slice(nhwc_slice(p.out, p.out_cs, p.out_co, p.Cout, p.out_f32), p.N, p.Hout, p.Wout);
-    if (p.res) o.res = op_slice(nhwc_slice(p.res, p.res_cs, p.res_co, p.Cout, p.out_f32), p.N, p.Hout, p.Wout);
-    o.w = p.w; o.bias = p.bias; o.k = p.k; o.stride = p.stride; o.groups = p.groups; o.act = p.act;
-    return n;
-  }
-  if (op.kind != Op::GEMM) return n;
-  const ConvDesc& d = op.conv;
-  const GemmParams& g = op.gemm.p;
-  const int N = d.in.N, Ho = conv_out(d.in.H, d.stride), Wo = conv_out(d.in.W, d.stride);
-  o.kind = op.chain.out.p ? CC_CONV_OP_CHAIN : CC_CONV_OP_GEMM;
-  o.in = op_slice(d.in, N, d.in.H, d.in.W);
-  o.out = op_slice(d.out, N, Ho, Wo);
-  if (d.res.p) o.res = op_slice(d.res, N, Ho, Wo);
-  o.w = d.w; o.bias = d.bias; o.k = d.k; o.stride = d.stride; o.groups = 1; o.act = d.act;
-  o.pre = d.pre; o.pre_h = d.pre_h; o.pre_w = d.pre_w;
-  if (op.chain.out.p) {
-    const ChainDesc& c = op.chain;
-    o.w2 = c.w; o.bias2 = c.bias; o.act2 = c.act; o.k0 = c.k0;
-    if (c.part.p) o.part = op_slice(c.part, N, Ho, Wo);
-    o.out2 = op_slice(c.out, N, Ho, Wo);
-    o.store1 = c.store1 ? 1 : 0;
-  }
-  o.BN = g.BN; o.BK = g.BK; o.lTW = g.lTW; o.lTH = g.lTH; o.lTN = g.lTN; o.s2 = g.s2; o.stages = g.stages; o.b_res = g.b_res;
-  o.grid = op.gemm.grid; o.num_tiles = g.num_tiles; o.BNn = g.BNn; o.narrow_tiles = g.num_tiles - g.num_wide;
+  *out = op.kind == Op::DIRECT ? conv_op_of(op.direct) : op.kind == Op::GEMM ? conv_op_of(op.conv, op.chain, op.gemm) : cc_conv_op{};
+  snprintf(out->name, sizeof(out->name), "%s", op.name.c_str());
   return n;
 }
 

@@ -3,29 +3,19 @@ import ctypes
 
 import torch
 
-from ._lib import lib, check, ptr, stream_ptr
+from ._lib import CC_CONV_OP_CHAIN, CC_CONV_OP_DIRECT, CC_CONV_OP_GEMM, cc_conv_op, cc_slice, lib, check, ptr, stream_ptr
 
 
-def conv2d(xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, Cout, act=0, res=None, res_co=0, groups=1, impl=0, bn=0,
-           stream=None, slope=None):
-    """xbuf: [N,H,W,in_cs] bf16 CUDA; w: [Cout,k,k,Cin/groups] bf16; obuf: [N,Ho,Wo,out_cs] bf16|fp32.
-    act = 3 (CC_ACT_PRELU, cc_conv2d_prelu): bias is the fp32 [9,Cout] border-class table and slope the fp32 [Cout] PReLU
-    slopes; the wgmma kernel, bf16 out."""
-    assert xbuf.is_cuda and xbuf.dtype == torch.bfloat16 and xbuf.is_contiguous()
-    assert w.dtype == torch.bfloat16 and w.is_contiguous() and obuf.is_contiguous()
-    N, H, W, in_cs = xbuf.shape
-    out_cs = obuf.shape[-1]
-    if act == 3:
-        rc = lib().cc_conv2d_prelu(ptr(xbuf), N, H, W, in_cs, in_co, Cin, ptr(w), ptr(bias), ptr(slope), Cout, k, stride, ptr(obuf),
-                                   out_cs, out_co, ptr(res), 0 if res is None else res.shape[-1], res_co, bn, stream_ptr(stream))
-        check(rc, "cc_conv2d_prelu")
-        return obuf
-    out_f32 = 1 if obuf.dtype == torch.float32 else 0
-    rc = lib().cc_conv2d(ptr(xbuf), N, H, W, in_cs, in_co, Cin, ptr(w), ptr(bias), Cout, k, stride, groups, ptr(obuf),
-                         out_cs, out_co, out_f32, act, ptr(res), 0 if res is None else res.shape[-1], res_co, impl, bn,
-                         stream_ptr(stream))
-    check(rc, "cc_conv2d")
-    return obuf
+def conv2d(xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, Cout, act=0, res=None, res_co=0, groups=1, impl=1, bn=0,
+           stream=None, slope=None, pre=None):
+    """xbuf: [N,H,W,in_cs] bf16 CUDA; w: [Cout,k,k,Cin/groups] bf16; obuf: [N,Ho,Wo,out_cs] bf16|fp32.  impl 1 = the wgmma
+    kernel, 2 = the direct kernel.  act = 3 (CC_ACT_PRELU): bias is the fp32 [9,Cout] border-class table and slope the fp32
+    [Cout] PReLU slopes, bf16 out.  pre: the fp32 [N,Ho/2,Wo/2,Cout] addend before the activation."""
+    assert impl in (1, 2), "impl 1 = wgmma, 2 = direct"
+    assert pre is None or (pre.dtype == torch.float32 and pre.is_contiguous() and pre.dim() == 4)
+    return _conv(CC_CONV_OP_GEMM if impl == 1 else CC_CONV_OP_DIRECT, xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, Cout,
+                 act, res, res_co, stream, groups=groups, BN=bn, slope=ptr(slope), pre=ptr(pre),
+                 pre_h=0 if pre is None else pre.shape[1], pre_w=0 if pre is None else pre.shape[2])
 
 
 def conv2d_chain(xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, w2, bias2, k0, o2buf, out2_co, act2=1, part=None,
@@ -33,16 +23,29 @@ def conv2d_chain(xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, w2, bias2, 
     """A SiLU conv of w (bf16 [Cout,k,k,Cin]) into obuf[..., out_co:] and, in its epilogue, the square 1x1 conv w2 (bf16
     [Cout2,1,1,Cout2]) over [its output channels k0.. | part[..., part_co:part_co + part_C]] into o2buf[..., out2_co:] (bf16 with
     act2 = 1 SiLU, or fp32 with act2 = 0).  store1=False drops the first output (obuf may be None)."""
-    assert xbuf.is_cuda and xbuf.dtype == torch.bfloat16 and xbuf.is_contiguous() and w.is_contiguous() and w2.is_contiguous()
-    N, H, W, in_cs = xbuf.shape
-    Cout, Cout2 = w.shape[0], w2.shape[0]
-    rc = lib().cc_conv2d_chain(ptr(xbuf), N, H, W, in_cs, in_co, Cin, ptr(w), ptr(bias), Cout, k, stride, ptr(obuf),
-                               0 if obuf is None else obuf.shape[-1], out_co, int(store1), ptr(res),
-                               0 if res is None else res.shape[-1], res_co, ptr(w2), ptr(bias2), Cout2, act2, k0, ptr(part),
-                               0 if part is None else part.shape[-1], part_co, part_C, ptr(o2buf), o2buf.shape[-1], out2_co,
-                               int(o2buf.dtype == torch.float32), stream_ptr(stream))
-    check(rc, "cc_conv2d_chain")
+    assert w2.is_contiguous()
+    _conv(CC_CONV_OP_CHAIN, xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, w.shape[0], 1, res, res_co, stream, w2=ptr(w2),
+          bias2=ptr(bias2), act2=act2, k0=k0, part=_slice(part, part_co, part_C), out2=_slice(o2buf, out2_co, w2.shape[0]),
+          store1=int(store1))
     return o2buf
+
+
+def _slice(t, co, C):
+    """Channels [co, co + C) of the NHWC tensor t as a cc_slice (t None: no buffer)."""
+    if t is None:
+        return cc_slice(None, 0, co, C)
+    N, H, W, cs = t.shape
+    return cc_slice(t.data_ptr(), cs, co, C, N, H, W, int(t.dtype == torch.float32))
+
+
+def _conv(kind, xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, Cout, act, res, res_co, stream, **fields):
+    """One cc_conv launch of the given kind; `fields` sets the rest of the cc_conv_op."""
+    assert xbuf.is_cuda and xbuf.dtype == torch.bfloat16 and xbuf.is_contiguous()
+    assert w.dtype == torch.bfloat16 and w.is_contiguous() and (obuf is None or obuf.is_contiguous())
+    op = cc_conv_op(kind=kind, in_=_slice(xbuf, in_co, Cin), out=_slice(obuf, out_co, Cout), res=_slice(res, res_co, Cout),
+                    w=ptr(w), bias=ptr(bias), k=k, stride=stride, act=act, **{"groups": 1, **fields})
+    check(lib().cc_conv(ctypes.byref(op), stream_ptr(stream)), "cc_conv")
+    return obuf
 
 
 def attention(qkv, L, H, causal, impl, ctx=None, stream=None):
@@ -63,7 +66,7 @@ def attention(qkv, L, H, causal, impl, ctx=None, stream=None):
     return ctx
 
 
-# ---- the detector's non-GEMM kernels and its two special conv forms, as the plan runs them (include/clearcam_b200.h)
+# ---- the detector's non-GEMM kernels and its fp32-accurate conv, as the plan runs them (include/clearcam_b200.h)
 POOL_OPS = {"avg2_pad": 0, "avgmax": 1, "max5": 2, "upsample2": 3}
 
 
@@ -135,16 +138,6 @@ def stem(frames, w, b, obuf, out_co, impl, stream=None):
     ws = torch.empty(need.value, dtype=torch.uint8, device=frames.device)
     check(lib().cc_stem(*args, ptr(obuf), obuf.shape[-1], out_co, int(obuf.dtype == torch.float32), impl, ptr(ws), need.value,
                         None, stream_ptr(stream)), "cc_stem")
-    return obuf
-
-
-def conv2d_pre(xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, Cout, act, pre, bn=0, stream=None):
-    """conv2d on the wgmma kernel plus the half-resolution addend pre (fp32 [N,Ho/2,Wo/2,Cout]) before the activation."""
-    N, H, W, in_cs = _nhwc(xbuf)
-    assert w.dtype == torch.bfloat16 and w.is_contiguous() and pre.dtype == torch.float32 and pre.is_contiguous()
-    check(lib().cc_conv2d_pre(ptr(xbuf), N, H, W, in_cs, in_co, Cin, ptr(w), ptr(bias), Cout, k, stride, ptr(obuf),
-                              obuf.shape[-1], out_co, int(obuf.dtype == torch.float32), act, ptr(pre), bn, stream_ptr(stream)),
-          "cc_conv2d_pre")
     return obuf
 
 

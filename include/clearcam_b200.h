@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define CC_ABI_VERSION 1
+#define CC_ABI_VERSION 2
 
 int cc_version(void);
 const char* cc_last_error(void);
@@ -32,41 +32,61 @@ int cc_device_check(void);
 #define CC_ACT_NONE 0
 #define CC_ACT_SILU 1      /* x*sigmoid(x): detection/yolov9.py:38 */
 #define CC_ACT_GELU_TANH 2 /* tinygrad Tensor.gelu(): models/objects.py:125,179 */
-#define CC_ACT_PRELU 3     /* where(x > 0, x, slope * x): models/adaface.py:54,86 (cc_conv2d_prelu, the face embedder) */
+#define CC_ACT_PRELU 3     /* where(x > 0, x, slope * x): models/adaface.py:54,86 (the face embedder; see cc_conv_op) */
 
 /* ---- kernel-level ops (used by the graphs below and exposed for the parity tests) ---- */
 
-/* Conv2d(bias) [+act] [+residual], k in {1,3}, stride in {1,2}, pad = k/2, NHWC bf16 in, bf16|fp32 out.
- * Replaces nn.Conv2d + .silu() of detection/yolov9.py:33-38 (and the bare nn.Conv2d of :173,:186,:224).
- * d_w: bf16 [Cout][k][k][Cin/groups]; d_bias: fp32 [Cout] or NULL; d_res: same dtype/shape class as out or NULL.
- * impl: 0 = auto (wgmma implicit GEMM when the shape allows, else direct), 1 = force wgmma, 2 = force direct.
- * bn: wgmma N-tile upper bound (0 = heuristic). */
-int cc_conv2d(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin,
-              const void* d_w, const float* d_bias, int Cout, int k, int stride, int groups,
-              void* d_out, int out_cs, int out_co, int out_f32, int act,
-              const void* d_res, int res_cs, int res_co, int impl, int bn, void* stream);
-
-/* One launch of two convs: a SiLU conv as cc_conv2d (wgmma, bf16 out) and a square 1x1 conv (d_w2: bf16 [Cout2][Cout2]) whose
- * input is the channel run [k0, k0 + Cout2 - part_C) of the first conv's output followed by the partner slice (d_part, part_C
- * channels at part_co of a buffer of part_cs channels, same pixels; or NULL), run in the first conv's epilogue.  act2 is
- * CC_ACT_SILU with a bf16 second output or CC_ACT_NONE with fp32 (out2_f32).  store1 = 0 drops the first output (d_out may
- * be NULL).  The results equal two cc_conv2d calls bit for bit.  A pair the kernel cannot chain (see conv_gemm.cu
+/* One conv launch, as cc_conv takes it and as cc_yolo_op_conv reports a plan's launch: Conv2d(bias) [+act] [+residual], k in
+ * {1,3}, stride in {1,2}, pad = k/2, NHWC bf16 in, bf16|fp32 out.  Replaces nn.Conv2d + .silu() of detection/yolov9.py:33-38
+ * (and the bare nn.Conv2d of :173,:186,:224).
+ *   kind     CC_CONV_OP_GEMM: the wgmma implicit-GEMM kernel; CC_CONV_OP_CHAIN: the same with a 1x1 conv in its epilogue;
+ *            CC_CONV_OP_DIRECT: the CUDA-core direct kernel, the only one that takes groups != 1.  cc_yolo_op_conv reports
+ *            CC_CONV_OP_NONE for an op that is not a conv (the rest is then zero), and name: the op's name (cc_yolo_profile's).
+ *   in, out, res  NHWC slices (cc_slice: buffer p, channels per pixel cs, first channel co, channels C, extent N x H x W,
+ *            f32: float elements, else bf16).  in is bf16, Cin = in.C; Cout = out.C; res (res.p == NULL: none) has out's
+ *            dtype, is added after the activation and may be the output slice itself.  out and res have the output extent
+ *            N x Ho x Wo of in's N x H x W: Ho = (H - 1) / stride + 1, Wo likewise.
+ *   w, bias  bf16 [Cout][k][k][Cin/groups]; fp32 [Cout] or NULL.
+ *   act      CC_ACT_*.  CC_ACT_PRELU is the face embedder's epilogue (wgmma, bf16 out only):
+ *              out = where(y > 0, y, slope[c] * y) (+ res),  y = conv(x) + bias[cls][c]
+ *            where cls = 3 * (h == 0 ? 0 : h == Ho-1 ? 2 : 1) + (w == 0 ? 0 : w == Wo-1 ? 2 : 1) is the output pixel's border
+ *            class; bias is then the fp32 [9][Cout] table and slope fp32 [Cout] (NULL for the other activations).  A
+ *            per-channel affine map applied before a zero-padded 3x3 conv folds into the weights and this table exactly (the
+ *            shift summed over the taps inside the map).
+ *   pre      NULL, or the fused Upsample -> Concat addend (wgmma only): out = act(conv(x) + bias + pre[n, h/2, w/2, :]) [the
+ *            first conv of a RepNCSPELAN4 after an upsample].  pre: dense fp32 [N][pre_h][pre_w][Cout], 16-byte aligned; Ho
+ *            and Wo even, pre_h = Ho/2, pre_w = Wo/2.
+ *   CHAIN    a SiLU conv into bf16 and the square 1x1 conv w2 (bf16 [Cout2][Cout2], Cout2 = out2.C), bias2, act2 whose input
+ *            is the first conv's output channels [k0, k0 + Cout2 - part.C) followed by the partner slice `part` (bf16, same
+ *            pixels; part.p == NULL: none), into out2: CC_ACT_SILU into bf16 or CC_ACT_NONE into fp32.  store1 = 0 drops
+ *            the first output (out.p may then be NULL; out.C still gives Cout).  The results equal the two convs launched
+ *            one after the other bit for bit.
+ *   BN       an upper bound on the wgmma N tile that also keeps every tile that wide; 0 = the planner chooses.  Reported:
+ *            the N tile as built.
+ *   BK .. narrow_tiles  reported only (cc_conv ignores them), the tiling of a tensor-core launch as built: K block BK, the
+ *            128-pixel tile box 2^lTW x 2^lTH x 2^lTN (w, h, images), the stride-2 pair view s2, the pipeline stages,
+ *            resident weights b_res, the persistent grid and the tile count; BNn, the narrow tile width (0: every tile is BN
+ *            wide), and how many of the tiles are that narrow (the last wave's tiles split along N, and the remainder channel
+ *            block when BN does not divide Cout). */
+#define CC_CONV_OP_NONE 0
+#define CC_CONV_OP_GEMM 1
+#define CC_CONV_OP_CHAIN 2
+#define CC_CONV_OP_DIRECT 3
+typedef struct { void* p; int cs, co, C, N, H, W, f32; } cc_slice;
+typedef struct {
+  int kind;
+  char name[128];
+  cc_slice in, out, res;
+  const void* w; const float* bias; int k, stride, groups, act; const float* slope;
+  const float* pre; int pre_h, pre_w;
+  const void* w2; const float* bias2; int act2, k0; cc_slice part, out2; int store1;
+  int BN, BK, lTW, lTH, lTN, s2, stages, b_res, grid, num_tiles;
+  int BNn, narrow_tiles;
+} cc_conv_op;
+/* Launches the conv *op describes.  A kind other than GEMM, CHAIN or DIRECT, a NULL input, weight or output pointer, a slice
+ * whose extent is not the conv's, a shape the chosen kernel does not take or a pair the kernel cannot chain (see conv_gemm.cu
  * conv_gemm_chain_build) fails with CC_ERR_INVALID before anything is launched. */
-int cc_conv2d_chain(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin,
-                    const void* d_w, const float* d_bias, int Cout, int k, int stride,
-                    void* d_out, int out_cs, int out_co, int store1, const void* d_res, int res_cs, int res_co,
-                    const void* d_w2, const float* d_bias2, int Cout2, int act2, int k0,
-                    const void* d_part, int part_cs, int part_co, int part_C,
-                    void* d_out2, int out2_cs, int out2_co, int out2_f32, void* stream);
-
-/* cc_conv2d on the wgmma kernel with the face embedder's epilogue (CC_ACT_PRELU), bf16 out:
- *   out = where(y > 0, y, d_slope[c] * y) (+ res),  y = conv(x) + d_bias_cls[cls][c]
- * where cls = 3 * (h == 0 ? 0 : h == Ho-1 ? 2 : 1) + (w == 0 ? 0 : w == Wo-1 ? 2 : 1) is the output pixel's border class.
- * d_bias_cls: fp32 [9][Cout]; d_slope: fp32 [Cout].  A per-channel affine map applied before a zero-padded 3x3 conv folds into
- * the weights and this table exactly (the shift summed over the taps inside the map). */
-int cc_conv2d_prelu(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const void* d_w, const float* d_bias_cls,
-                    const float* d_slope, int Cout, int k, int stride, void* d_out, int out_cs, int out_co, const void* d_res,
-                    int res_cs, int res_co, int bn, void* stream);
+int cc_conv(const cc_conv_op* op, void* stream);
 
 /* ---- YOLOv9 detector (replaces detection/yolov9.py: class YOLOv9, :298-458) ---- */
 typedef struct cc_yolo cc_yolo;
@@ -160,33 +180,10 @@ int cc_yolo_trace(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf
 
 /* Conv op taps, for tests that check every conv launch of a plan in place, one op at a time.
  * cc_yolo_op_conv describes op i of the cached plan of this shape (built on first use, as cc_yolo_forward would) and returns
- * the plan's op count; out == NULL only returns the count, an i outside [0, count) fails with CC_ERR_INVALID.  out->name is
- * the op's name (the names cc_yolo_profile reports); out->kind is CC_CONV_OP_NONE for an op that is not a conv (the rest is
- * then zero).  For a conv: the input, output and residual slices (res.p == NULL: none) with the extents the launch covers;
- * bf16 weights w [Cout][k][k][Cin/groups], bias [Cout] or NULL, act; the half-resolution fp32 pre-activation addend pre
- * ([N][pre_h][pre_w][Cout] dense, or NULL).  CC_CONV_OP_CHAIN: the square 1x1 run in the conv's epilogue, w2 [Cout2][Cout2],
- * bias2, act2, over output channels [k0, k0 + Cout2 - part.C) followed by the partner slice `part`, into out2; store1 = 0:
- * the first output is not written.  For the tensor-core launches, the tiling as built: N tile BN, K block BK, the 128-pixel
- * tile box 2^lTW x 2^lTH x 2^lTN (w, h, images), the stride-2 pair view s2, the pipeline stages, resident weights b_res,
- * the persistent grid and the tile count; BNn, the narrow tile width (0: every tile is BN wide), and how many of the tiles
- * are that narrow (the last wave's tiles split along N, and the remainder channel block when BN does not divide Cout).
+ * the plan's op count (a cc_conv_op, see above, with the tiling as built); out == NULL only returns the count, an i outside
+ * [0, count) fails with CC_ERR_INVALID.
  * cc_yolo_run_ops launches ops [first, last) of that plan on `stream` exactly as a forward launches them, without a CUDA
  * graph; d_frames, d_out and d_raw are a cc_yolo_forward call's.  Nothing synchronises. */
-#define CC_CONV_OP_NONE 0
-#define CC_CONV_OP_GEMM 1
-#define CC_CONV_OP_CHAIN 2
-#define CC_CONV_OP_DIRECT 3
-typedef struct { void* p; int cs, co, C, N, H, W, f32; } cc_slice;   /* NHWC slice; f32: float elements, else bf16 */
-typedef struct {
-  int kind;
-  char name[128];
-  cc_slice in, out, res;
-  const void* w; const float* bias; int k, stride, groups, act;
-  const float* pre; int pre_h, pre_w;
-  const void* w2; const float* bias2; int act2, k0; cc_slice part, out2; int store1;
-  int BN, BK, lTW, lTH, lTN, s2, stages, b_res, grid, num_tiles;
-  int BNn, narrow_tiles;
-} cc_conv_op;
 int cc_yolo_op_conv(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int i, cc_conv_op* out);
 int cc_yolo_run_ops(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, int first, int last,
                     float* d_out, float* d_raw, void* stream);
@@ -263,11 +260,6 @@ int cc_finish_f32(const float* d_acc, const float* d_bias, int act, int npix, in
  * weights (16-byte aligned); d_out == NULL only writes *ws_needed. */
 int cc_stem(const void* d_frames, int frame_f32, int B, int H, int W, const float* h_w, const float* h_bias, int Cout, void* d_out,
             int out_cs, int out_co, int out_f32, int impl, void* d_ws, size_t ws_bytes, size_t* ws_needed, void* stream);
-/* cc_conv2d on the wgmma kernel with the fused Upsample -> Concat addend: out = act(conv(x) + bias + pre[n, h/2, w/2, :]) [the
- * first conv of a RepNCSPELAN4 after an upsample].  d_pre: dense fp32 [N][Ho/2][Wo/2][Cout]; Ho and Wo even. */
-int cc_conv2d_pre(const void* d_in, int N, int Hin, int Win, int in_cs, int in_co, int Cin, const void* d_w, const float* d_bias,
-                  int Cout, int k, int stride, void* d_out, int out_cs, int out_co, int out_f32, int act, const float* d_pre, int bn,
-                  void* stream);
 /* One conv of the fp32-accurate mode, as the detector runs it: the six-plane split of the fp32 input slice, one GEMM per hi x hi
  * input-channel segment (at most 48 k16 steps each) accumulated in fp32, the cross-product GEMM, then [res +] act(acc + bias).
  * h_w: HOST fp32 [Cout][Cin][k][k], h_bias: HOST fp32 [Cout] or NULL; k 1 (stride 1) or 3 (stride 1 or 2); act 0 or 1; Cin and Cout

@@ -1,8 +1,10 @@
-"""cc_conv2d_chain (a conv with a square 1x1 conv run in its epilogue) against the same two convs as two cc_conv2d calls:
+"""cc_conv's CHAIN launch (a conv with a square 1x1 conv run in its epilogue) against the same two convs as two GEMM launches:
 the results must be equal bit for bit.  The shapes are the chains the detector's plans build (layer 1's 3x3/s2 conv -> ELAN
 cv1, RepNCSP's last bottleneck cv2 -> cv3 over [x1 | x3], ELAN cv1 -> cv2.0 cv1+cv2 on y1, ELAN cv2.1 -> cv3.0 cv1+cv2 on y2,
 the head's cv2.j.1 -> cv2.j.2 logits) at the map sizes of 640x640 and 384x640 inputs, plus maps whose edge tiles are
 clipped."""
+import re
+
 import pytest
 import torch
 
@@ -151,7 +153,7 @@ def test_head_box_logits_fp32():
         assert torch.equal(got, ref), (N, H, W)
 
 
-def test_rejects_pairs_that_do_not_chain():
+def test_cc_conv_refuses_pairs_that_do_not_chain():
     g = torch.Generator().manual_seed(5)
     x = _rand((1, 40, 40, 128), 1.0, g)
     o = torch.zeros(1, 40, 40, 256, dtype=torch.bfloat16, device="cuda")
@@ -162,23 +164,23 @@ def test_rejects_pairs_that_do_not_chain():
     sq = {c: _conv_w(c, 1, c, g) for c in (32, 64, 128, 256)}
     bad = [
         # the 1x1 has more than 128 channels
-        dict(w=w128, bias=b128, w2=sq[256], k0=0, o2=o2),
+        dict(w=w128, bias=b128, w2=sq[256], k0=0, o2=o2, why="the 1x1 has 256 channels"),
         # on this small map the standalone 1x1 would tile its 128 channels as two 64-channel blocks
-        dict(w=w128, bias=b128, w2=sq[128], k0=0, o2=o2),
+        dict(w=w128, bias=b128, w2=sq[128], k0=0, o2=o2, why="would tile its 128 channels in blocks"),
         # the input run [32, 96) crosses the end of the 64-channel output
-        dict(w=w64, bias=b64, w2=sq[64], k0=32, o2=o2),
+        dict(w=w64, bias=b64, w2=sq[64], k0=32, o2=o2, why="input run [32, 96) is not inside one"),
         # fp32 output of more than 64 channels
-        dict(w=w128, bias=b128, w2=sq[128], k0=0, o2=o2f, act2=0),
+        dict(w=w128, bias=b128, w2=sq[128], k0=0, o2=o2f, act2=0, why="no activation into fp32 (<= 64 channels)"),
         # SiLU into an fp32 output
-        dict(w=w64, bias=b64, w2=sq[64], k0=0, o2=o2f, act2=1),
+        dict(w=w64, bias=b64, w2=sq[64], k0=0, o2=o2f, act2=1, why="SiLU into bf16 or no activation into fp32"),
         # a partner that is not one staging box wide (64 channels here)
-        dict(w=w64, bias=b64, w2=sq[64], k0=0, o2=o2, part=x, part_C=32),
+        dict(w=w64, bias=b64, w2=sq[64], k0=0, o2=o2, part=x, part_C=32, why="partner slice must be one staging box"),
         # a k0 that is not on a k16 step
-        dict(w=w64, bias=b64, w2=sq[32], k0=8, o2=o2),
+        dict(w=w64, bias=b64, w2=sq[32], k0=8, o2=o2, why="input run [8, 40) is not inside one"),
     ]
     for a in bad:
         w2, bias2 = a["w2"]
-        with pytest.raises(CCError, match="cc_conv2d_chain"):
+        with pytest.raises(CCError, match="cc_conv .*" + re.escape(a["why"])):
             ops.conv2d_chain(x, 0, 128, a["w"], a["bias"], 3, 1, o, 0, w2, bias2, a["k0"], a["o2"], 0, act2=a.get("act2", 1),
                              part=a.get("part"), part_co=0, part_C=a.get("part_C", 0))
     torch.cuda.synchronize()
@@ -192,7 +194,7 @@ def test_rejects_residual_on_a_128_channel_tile():
     o2 = torch.zeros_like(o)
     w, bias = _conv_w(128, 3, 128, g)
     w2, bias2 = _conv_w(128, 1, 128, g)
-    with pytest.raises(CCError, match="takes no residual"):
+    with pytest.raises(CCError, match="cc_conv .*a 128-channel tile takes no residual"):
         ops.conv2d_chain(x, 0, 128, w, bias, 3, 1, o, 0, w2, bias2, 0, o2, 0, act2=1, res=o, res_co=0)
     torch.cuda.synchronize()
     assert not o.any() and not o2.any()

@@ -20,7 +20,7 @@ import torch
 import torch.nn.functional as F
 
 from clearcam_b200 import ops
-from clearcam_b200._lib import lib
+from clearcam_b200._lib import CC_CONV_OP_DIRECT, CC_CONV_OP_GEMM, CC_CONV_OP_NONE, cc_conv_op, cc_slice, lib
 
 SENT = -7.0
 F32_BAR = 2.0 ** -18          # fp32 conv GEMM outputs (tests/test_conv_gpu.py): per element, x (sum|x.w| + |bias| + |pre|)
@@ -457,14 +457,14 @@ def pre_bar(z, y, mag, out_f32):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", PRE_CASES, ids=[f"{c[0]}x{c[1]}x{c[2]}-{c[3]}to{c[4]}-{'f32' if c[5] else 'bf16'}-bn{c[7]}" for c in PRE_CASES])
-def test_conv_pre_addend_matches_float64(case):
+def test_cc_conv_pre_addend_matches_float64(case):
     """act(conv(x) + b + up2(pre)) of the fused Upsample -> Concat -> RepNCSPELAN4 first conv, into the lower half of its
     concat buffer; at B = 32 the 128-pixel tiles span several images."""
     N, Ho, Wo, Cin, Cout, out_f32, act, bn = case
     x, w, b, pre = pre_inputs(case)
     dt = torch.float32 if out_f32 else torch.bfloat16
     obuf = _sentinel_buf(N, Ho, Wo, 2 * Cout, dt)
-    ops.conv2d_pre(x.cuda(), 0, Cin, w.cuda(), b.cuda(), 1, 1, obuf, 0, Cout, act, pre.cuda(), bn=bn)
+    ops.conv2d(x.cuda(), 0, Cin, w.cuda(), b.cuda(), 1, 1, obuf, 0, Cout, act=act, bn=bn, pre=pre.cuda())
     torch.cuda.synchronize()
     _assert_outside_untouched(obuf, 0, Cout)
     z, y, mag = pre_ref(x, w, b, pre, act, "cuda")
@@ -553,7 +553,7 @@ def test_bars_see_detector_bugs():
         assert r >= 4.0, f"'{name}' moves the result by only {r:.2f}x the bar"
 
 
-def test_detector_taps_reject_bad_arguments():
+def test_detector_taps_and_cc_conv_reject_bad_arguments():
     """Every check of the taps runs before anything is launched (no GPU needed): the pointers below are never dereferenced."""
     h = lib()
     fake = ctypes.c_void_p(1 << 20)
@@ -619,15 +619,31 @@ def test_detector_taps_reject_bad_arguments():
     refused(stem(ws=None), "cc_stem", "too small")
     refused(stem(out=odd), "cc_stem", "16-byte aligned")
     refused(stem(hw=None), "cc_stem", "NULL")
-    # cc_conv2d_pre(in, N, Hin, Win, in_cs, in_co, Cin, w, bias, Cout, k, stride, out, out_cs, out_co, out_f32, act, pre, bn)
-    pre = lambda Hin=40, Cin=64, k=1, s=1, p=fake: h.cc_conv2d_pre(fake, 1, Hin, 40, Cin, 0, Cin, fake, fake, 64, k, s, fake, 64, 0,
-                                                                   0, 1, p, 0, None)
-    refused(pre(p=None), "cc_conv2d_pre", "NULL")
-    refused(pre(p=odd), "cc_conv2d_pre", "d_pre must be 16-byte aligned")
-    refused(pre(Hin=41), "cc_conv2d_pre", "even sides")
-    refused(pre(Hin=42, s=2, k=3), "cc_conv2d_pre", "even sides")
-    refused(pre(Cin=24), "cc_conv2d_pre", "not supported")
-    refused(pre(s=2), "cc_conv2d_pre", "not supported")
+    # cc_conv(op, stream): a 1x1 SiLU conv 64 -> 64 over a 40-wide map with the pre addend, the slices and pre_h / pre_w at the
+    # extent its input and stride give, then the fields set by `kw`
+    def conv(Hin=40, Cin=64, k=1, s=1, p=fake.value, out_f32=0, **kw):
+        Ho, Wo = (Hin - 1) // s + 1, (40 - 1) // s + 1
+        op = cc_conv_op(kind=CC_CONV_OP_GEMM, in_=cc_slice(fake.value, Cin, 0, Cin, 1, Hin, 40, 0), w=fake.value, bias=fake.value,
+                        out=cc_slice(fake.value, 64, 0, 64, 1, Ho, Wo, out_f32), k=k, stride=s, groups=1, act=1, pre=p,
+                        pre_h=Ho // 2, pre_w=Wo // 2)
+        for name, v in kw.items():
+            setattr(op, name, v)
+        return h.cc_conv(ctypes.byref(op), None)
+    refused(conv(p=odd.value), "cc_conv:", f"pre={hex(odd.value)} must be 16-byte aligned")
+    refused(conv(Hin=41), "cc_conv:", "output 41x40 must have even sides")
+    refused(conv(Hin=42, s=2, k=3), "cc_conv:", "output 21x20 must have even sides")
+    refused(conv(Cin=24), "cc_conv:", "not supported", "Cin=24")
+    refused(conv(s=2), "cc_conv:", "not supported", "k=1 stride=2")
+    refused(conv(kind=CC_CONV_OP_NONE), "cc_conv:", "unknown kind 0")
+    refused(conv(kind=4), "cc_conv:", "unknown kind 4")
+    refused(conv(in_=cc_slice(None, 64, 0, 64, 1, 40, 40, 0)), "cc_conv:", "in.p is NULL")
+    refused(conv(w=None), "cc_conv:", "w is NULL")
+    refused(conv(out=cc_slice(None, 64, 0, 64, 1, 40, 40, 0)), "cc_conv:", "out.p is NULL")
+    refused(conv(out=cc_slice(fake.value, 64, 0, 64, 1, 39, 40, 0)), "cc_conv:", "out is 1x39x40, the output 1x40x40")
+    refused(conv(pre_h=19), "cc_conv:", "pre is 19x20, the output's half resolution 20x20")
+    refused(conv(act=3, p=None), "cc_conv:", "CC_ACT_PRELU needs", "slope", f"bias={hex(fake.value)}")
+    refused(conv(act=3, p=None, slope=fake.value, out_f32=1), "cc_conv:", "CC_ACT_PRELU writes bf16", "out.f32=1")
+    refused(conv(kind=CC_CONV_OP_DIRECT), "cc_conv:", "direct kernel takes no pre", f"pre={hex(fake.value)}")
     # cc_conv2d_fp32_accurate(in, N, Hin, Win, in_cs, in_co, Cin, h_w, h_bias, Cout, k, stride, act, res, res_cs, res_co,
     #                         out, out_cs, out_co, ws, ws_bytes, ws_needed, stream)
     wp = torch.zeros(64 * 256 * 9)

@@ -203,7 +203,7 @@ def test_face_search_matches_reference_loop(finder):
         f.face_embeddings[f"data/cameras/back/objects/video/{1800000000 + rep}_77_0.jpg"] = emb[5:6] * 0.5   # the index follows
 
 
-def test_argument_errors_before_launch(finder):
+def test_embed_and_cc_conv_argument_errors_before_launch(finder):
     L = lib()
     h = finder.adaface._h
     faces = oa.synthetic_faces(2, seed=1).cuda()
@@ -223,7 +223,7 @@ def test_argument_errors_before_launch(finder):
     x = torch.zeros(1, 8, 8, 64, dtype=torch.bfloat16, device="cuda")
     w = torch.zeros(64, 3, 3, 64, dtype=torch.bfloat16, device="cuda")
     o = torch.zeros(1, 8, 8, 64, dtype=torch.bfloat16, device="cuda")
-    with pytest.raises(CCError, match="cc_conv2d_prelu"):
+    with pytest.raises(CCError, match="cc_conv: .*slope"):
         ops.conv2d(x, 0, 64, w, torch.zeros(9, 64, device="cuda"), 3, 1, o, 0, 64, act=3, slope=None)
     with pytest.raises(CCError):
         ca.ADAFACE({k: v for k, v in oa.synthetic_weights(0).items() if k != "linear.bias"})

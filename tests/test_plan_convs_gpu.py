@@ -7,13 +7,13 @@ slice that is also the op's residual); the op then runs alone, and:
   (a) images 0..REPS-1 of its output match a float64 conv of the operands as stored: the saved input, residual and
       pre-activation addend, and the weights and bias read through their device pointers.  The bars are those of
       tests/test_conv_gpu.py (bf16_bar, F32_BAR, the round-to-nearest bias of activation-free bf16 outputs) and, for a conv with
-      the fused-upsample addend, that of tests/test_detector_ops_gpu.py::test_conv_pre_addend_matches_float64;
+      the fused-upsample addend, that of tests/test_detector_ops_gpu.py::test_cc_conv_pre_addend_matches_float64;
   (b) the batch holds copies of REPS distinct frames, so image b of every output must equal image b % REPS bit for bit: a
       pixel's arithmetic does not depend on which tile or CTA computes it, so a wrong tile anywhere in the batch shows;
   (c) every output is finite;
   (d) every workspace byte the op changed lies in its declared outputs (the first output when stored, the chained output);
   (e) a chained launch: its first conv is checked as in (a) (recomputed unchained when the launch drops it), and the chained
-      1x1's output equals the unchained pair (two cc_conv2d launches over the same channels) bit for bit and is checked as
+      1x1's output equals the unchained pair (two cc_conv launches over the same channels) bit for bit and is checked as
       in (a) itself.
 
 Then the whole forward: the first cc_yolo_forward call (plain launches, with programmatic dependent launch), the second
@@ -181,7 +181,7 @@ def check_op(op, snap, ws, worst):
                act=op.act, res=rbuf, res_co=0 if op.res is None else op.res.co)
     first = buf1[..., op.out.co:op.out.co + op.out.C]
     if op.store1:
-        assert torch.equal(bits(sview(ws, op.out)), bits(first)), f"{tag}: (e) the chained launch's first output differs from cc_conv2d"
+        assert torch.equal(bits(sview(ws, op.out)), bits(first)), f"{tag}: (e) the chained launch's first output differs from cc_conv"
     check_values(tag + " [first conv]", first, x, op.w, op.bias, op.k, op.stride, 1, op.act, res, None, False, worst)
     N2 = op.out2.C
     run = N2 - (op.part.C if op.part is not None else 0)

@@ -1,4 +1,4 @@
-"""Run single conv shapes through cc_conv2d (for ncu / timing). usage: one_conv.py [iters]"""
+"""Run single conv shapes through cc_conv (for ncu / timing). usage: one_conv.py [iters]"""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
