@@ -58,7 +58,8 @@ class cc_slice(ctypes.Structure):
 
 
 class cc_conv_op(ctypes.Structure):
-    """One conv launch as cc_conv takes it and cc_yolo_op_conv reports it (include/clearcam_b200.h); `in_` is the header's `in`."""
+    """One conv launch as cc_conv takes it and the plan taps (cc_yolo_op_conv, cc_clip_op_conv, cc_face_op_conv) report it
+    (include/clearcam_b200.h); `in_` is the header's `in`."""
     _fields_ = ([("kind", ctypes.c_int), ("name", ctypes.c_char * 128), ("in_", cc_slice), ("out", cc_slice), ("res", cc_slice),
                  ("w", ctypes.c_void_p), ("bias", ctypes.c_void_p)]
                 + [(n, ctypes.c_int) for n in ("k", "stride", "groups", "act")]
@@ -66,7 +67,7 @@ class cc_conv_op(ctypes.Structure):
                    ("w2", ctypes.c_void_p), ("bias2", ctypes.c_void_p), ("act2", ctypes.c_int), ("k0", ctypes.c_int), ("part", cc_slice), ("out2", cc_slice),
                    ("store1", ctypes.c_int)]
                 + [(n, ctypes.c_int) for n in ("BN", "BK", "lTW", "lTH", "lTN", "s2", "stages", "b_res", "grid", "num_tiles",
-                                               "BNn", "narrow_tiles")])
+                                               "BNn", "narrow_tiles", "out_ns")])
 
 
 # cc_conv_op kinds (CC_CONV_OP_* in include/clearcam_b200.h)
@@ -130,6 +131,8 @@ _SIGS = {
     "cc_clip_encode_text": (_i, [_vp, _vp, _i, _vp, ctypes.c_longlong, _vp]),
     "cc_clip_profile": (_i, [_vp, _i, _vp, _i, _vp, _i, ctypes.POINTER(_f), ctypes.POINTER(ctypes.c_double),
                              ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_i), ctypes.POINTER(ctypes.c_double), _vp]),
+    "cc_clip_op_conv": (_i, [_vp, _i, _i, _i, ctypes.POINTER(cc_conv_op)]),
+    "cc_clip_run_ops": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, ctypes.c_longlong, _vp]),
     "cc_face_create": (_i, [_i, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_vp), ctypes.POINTER(ctypes.c_int64),
                             ctypes.POINTER(_vp)]),
     "cc_face_destroy": (_i, [_vp]),
@@ -137,6 +140,8 @@ _SIGS = {
     "cc_face_workspace_bytes": (_i, [_vp, _i, ctypes.POINTER(ctypes.c_size_t)]),
     "cc_face_set_workspace": (_i, [_vp, _vp, ctypes.c_size_t]),
     "cc_face_layer_output": (_i, [_vp, _vp, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
+    "cc_face_op_conv": (_i, [_vp, _i, _i, ctypes.POINTER(cc_conv_op)]),
+    "cc_face_run_ops": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "cc_blazeface_create": (_i, [_i, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_vp), ctypes.POINTER(ctypes.c_int64),
                                  ctypes.POINTER(_vp)]),
     "cc_blazeface_destroy": (_i, [_vp]),

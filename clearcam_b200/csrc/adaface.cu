@@ -60,7 +60,9 @@ struct FaceBlockW {
 
 struct FOp {
   enum Kind { PACK, GEMM, L2NORM } kind;
+  std::string name;          // pack, stem, body.<i>.c0 | sc | c1, linear, l2norm
   GemmLaunch gemm;
+  ConvDesc conv{};           // GEMM: the descriptor its launch was built from (cc_face_op_conv reports it)
   __nv_bfloat16* packed = nullptr;
   float* feat = nullptr;
 };
@@ -99,15 +101,18 @@ struct FacePlanBuilder {
   Bump bump;
   FacePlanBuilder(FaceModel& m, FacePlan& p) : M(m), P(p) {}
   void* dalloc(size_t bytes) { return bump.take(bytes); }
-  void conv(const TSlice& in, const __nv_bfloat16* w, const float* bias, const float* slope, int stride, const TSlice& out,
-            int act, const TSlice* res) {
+  void gemm(std::string name, const ConvDesc& d) {
     if (rc || bump.dry) return;
-    ConvDesc d = conv_desc(in, w, bias, 3, stride, out, act, res);
-    d.slope = slope;
-    FOp op; op.kind = FOp::GEMM;
+    FOp op; op.kind = FOp::GEMM; op.name = std::move(name); op.conv = d;
     rc = conv_gemm_build(d, M.sms, &op.gemm);
     if (rc) return;
     P.ops.push_back(op);
+  }
+  void conv(std::string name, const TSlice& in, const __nv_bfloat16* w, const float* bias, const float* slope, int stride,
+            const TSlice& out, int act, const TSlice* res) {
+    ConvDesc d = conv_desc(in, w, bias, 3, stride, out, act, res);
+    d.slope = slope;
+    gemm(std::move(name), d);
   }
   void layer(const void* p, int f32, int C, int H, int W) { P.layers.push_back(FaceLayer{p, f32, C, H, W, P.ops.size() - 1}); }
   int build(int B) {
@@ -118,22 +123,23 @@ struct FacePlanBuilder {
     __nv_bfloat16* S = static_cast<__nv_bfloat16*>(dalloc(big));
     float* feat = static_cast<float*>(dalloc(static_cast<size_t>(B) * kFaceDim * 4));
     if (bump.dry) return CC_OK;
-    { FOp op; op.kind = FOp::PACK; op.packed = packed; P.ops.push_back(op); }
+    { FOp op; op.kind = FOp::PACK; op.name = "pack"; op.packed = packed; P.ops.push_back(op); }
     int H = kFaceSide;
-    conv(nhwc_slice(packed, kFacePackC, 0, kFacePackC, 0, B, H, H), M.stem_w, M.stem_cls, M.stem_slope, 1,
+    conv("stem", nhwc_slice(packed, kFacePackC, 0, kFacePackC, 0, B, H, H), M.stem_w, M.stem_cls, M.stem_slope, 1,
          nhwc_slice(X, 64, 0, 64), ACT_PRELU, nullptr);
     layer(X, 0, 64, H, H);
     for (int i = 0; i < kFaceBlocks && !rc; ++i) {
       const int cin = kFaceSizes[i][0], D = kFaceSizes[i][1], s = kFaceSizes[i][2], Ho = H / s;
       const FaceBlockW& b = M.blk[i];
-      conv(nhwc_slice(X, cin, 0, cin, 0, B, H, H), b.w0, b.cls0, b.slope0, 1, nhwc_slice(T, D, 0, D), ACT_PRELU, nullptr);
+      const std::string name = "body." + std::to_string(i);
+      conv(name + ".c0", nhwc_slice(X, cin, 0, cin, 0, B, H, H), b.w0, b.cls0, b.slope0, 1, nhwc_slice(T, D, 0, D), ACT_PRELU, nullptr);
       if (!b.wsc) {          // identity shortcut: conv_layer1 adds x in place
         const TSlice o = nhwc_slice(X, D, 0, D);
-        conv(nhwc_slice(T, D, 0, D, 0, B, H, H), b.w1, b.b1, nullptr, 1, o, ACT_NONE, &o);
+        conv(name + ".c1", nhwc_slice(T, D, 0, D, 0, B, H, H), b.w1, b.b1, nullptr, 1, o, ACT_NONE, &o);
       } else {               // shortcut conv into S, then conv_layer1 adds onto it in place
         const TSlice o = nhwc_slice(S, D, 0, D);
-        conv(nhwc_slice(X, cin, 0, cin, 0, B, H, H), b.wsc, b.bsc, nullptr, s, o, ACT_NONE, nullptr);
-        conv(nhwc_slice(T, D, 0, D, 0, B, H, H), b.w1, b.b1, nullptr, s, o, ACT_NONE, &o);
+        conv(name + ".sc", nhwc_slice(X, cin, 0, cin, 0, B, H, H), b.wsc, b.bsc, nullptr, s, o, ACT_NONE, nullptr);
+        conv(name + ".c1", nhwc_slice(T, D, 0, D, 0, B, H, H), b.w1, b.b1, nullptr, s, o, ACT_NONE, &o);
         std::swap(X, S);
       }
       H = Ho;
@@ -146,27 +152,24 @@ struct FacePlanBuilder {
       ConvDesc d = conv_desc(nhwc_slice(X, K, 0, K, 0, 1, 1, B), M.lin_w, M.lin_b, 1, 1, o, ACT_NONE);
       // 512 outputs in 16 n blocks of 32: at small B the 25.7 MB of weights are streamed by 16 x ceil(B / 128) CTAs
       d.bn_override = 32;
-      FOp op; op.kind = FOp::GEMM;
-      if ((rc = conv_gemm_build(d, M.sms, &op.gemm))) return rc;
-        P.ops.push_back(op);
+      gemm("linear", d);
+      if (rc) return rc;
       layer(feat, 1, kFaceDim, 1, 1);
     }
-    { FOp op; op.kind = FOp::L2NORM; op.feat = feat; P.ops.push_back(op); }
+    { FOp op; op.kind = FOp::L2NORM; op.name = "l2norm"; op.feat = feat; P.ops.push_back(op); }
     return rc;
   }
 };
 
-// ops [0, end) of the plan; rows >= B of the batch are zero input
-static int run_face_plan(FacePlan& P, const uint8_t* d_faces, int B, size_t end, float* d_out, long long out_stride, cudaStream_t st) {
-  for (size_t i = 0; i < end; ++i) {
+// ops [first, last) of the plan of batch B
+static int run_face_plan(FacePlan& P, const uint8_t* d_faces, int B, size_t first, size_t last, float* d_out, long long out_stride,
+                         cudaStream_t st) {
+  for (size_t i = first; i < last; ++i) {
     FOp& op = P.ops[i];
     int rc = CC_OK;
     switch (op.kind) {
       case FOp::PACK: {
-        const size_t plane = static_cast<size_t>(kFaceSide) * kFaceSide;
-        if (P.B > B)
-          CC_CHECK_CUDA(cudaMemsetAsync(op.packed + plane * kFacePackC * B, 0, plane * kFacePackC * 2 * (P.B - B), st));
-        const long long npix = static_cast<long long>(B) * plane;
+        const long long npix = static_cast<long long>(B) * kFaceSide * kFaceSide;
         const long long blocks = (npix + 255) / 256;
         face_pack_kernel<<<blocks < 132 * 16 ? static_cast<int>(blocks) : 132 * 16, 256, 0, st>>>(d_faces, op.packed, npix);
         CC_CHECK_CUDA(cudaGetLastError());
@@ -274,7 +277,7 @@ int cc_face_embed(cc_face* h, const uint8_t* d_faces, int B, float* d_out, long 
   CC_REQUIRE((reinterpret_cast<uintptr_t>(d_out) & 3) == 0, "cc_face_embed: d_out must be 4-byte aligned");
   FacePlan* P = nullptr;
   if (int rc = face_plan(h, B, &P)) return rc;
-  return run_face_plan(*P, d_faces, B, P->ops.size(), d_out, out_row_stride > 0 ? out_row_stride : kFaceDim,
+  return run_face_plan(*P, d_faces, B, 0, P->ops.size(), d_out, out_row_stride > 0 ? out_row_stride : kFaceDim,
                        static_cast<cudaStream_t>(stream));
 }
 
@@ -290,10 +293,34 @@ int cc_face_layer_output(cc_face* h, const uint8_t* d_faces, int B, int layer, f
   if (!d_dst) return CC_OK;
   CC_REQUIRE(d_faces, "cc_face_layer_output: d_faces is NULL");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = run_face_plan(*P, d_faces, B, t.last_op + 1, nullptr, kFaceDim, st)) return rc;
+  if (int rc = run_face_plan(*P, d_faces, B, 0, t.last_op + 1, nullptr, kFaceDim, st)) return rc;
   face_tap_kernel<<<132 * 8, 256, 0, st>>>(t.p, t.f32, t.C, static_cast<long long>(B) * t.H * t.W * t.C, d_dst);
   CC_CHECK_CUDA(cudaGetLastError());
   return CC_OK;
+}
+
+// conv op taps: what each GEMM launch of the cached plan computes, and the plan run one range of ops at a time
+int cc_face_op_conv(cc_face* h, int B, int i, cc_conv_op* out) {
+  CC_REQUIRE(h && B > 0, "cc_face_op_conv: bad argument");
+  FacePlan* P = nullptr;
+  if (int rc = face_plan(h, B, &P)) return rc;
+  const int n = static_cast<int>(P->ops.size());
+  if (!out) return n;
+  CC_REQUIRE(i >= 0 && i < n, "cc_face_op_conv: op %d of a plan of %d ops", i, n);
+  const FOp& op = P->ops[i];
+  *out = op.kind == FOp::GEMM ? conv_op_of(op.conv, ChainDesc{}, op.gemm) : cc_conv_op{};
+  snprintf(out->name, sizeof(out->name), "%s", op.name.c_str());
+  return n;
+}
+
+int cc_face_run_ops(cc_face* h, const uint8_t* d_faces, int B, int first, int last, float* d_out, void* stream) {
+  CC_REQUIRE(h && d_faces && d_out && B > 0, "cc_face_run_ops: bad argument");
+  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_out) & 3) == 0, "cc_face_run_ops: d_out must be 4-byte aligned");
+  FacePlan* P = nullptr;
+  if (int rc = face_plan(h, B, &P)) return rc;
+  const int n = static_cast<int>(P->ops.size());
+  CC_REQUIRE(0 <= first && first <= last && last <= n, "cc_face_run_ops: ops [%d, %d) of a plan of %d ops", first, last, n);
+  return run_face_plan(*P, d_faces, B, first, last, d_out, kFaceDim, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -23,6 +23,7 @@ ConvDesc conv_desc_of(const cc_conv_op& o, ChainDesc* c) {
   ConvDesc d = conv_desc(conv_slice(o.in), o.w, o.bias, o.k, o.stride, conv_slice(o.out), o.act, o.res.p ? &res : nullptr);
   d.slope = o.slope;
   d.bn_override = o.BN;
+  d.out_ns = o.out_ns;
   d.pre = o.pre; d.pre_h = o.pre_h; d.pre_w = o.pre_w;
   *c = ChainDesc{};
   if (o.kind == CC_CONV_OP_CHAIN) {
@@ -44,6 +45,7 @@ cc_conv_op conv_op_of(const ConvDesc& d, const ChainDesc& c, const GemmLaunch& L
   if (d.res.p) o.res = op_slice(d.res, N, Ho, Wo);
   o.w = d.w; o.bias = d.bias; o.k = d.k; o.stride = d.stride; o.groups = 1; o.act = d.act; o.slope = d.slope;
   o.pre = d.pre; o.pre_h = d.pre_h; o.pre_w = d.pre_w;
+  o.out_ns = d.out_ns;
   if (c.out.p) {
     o.w2 = c.w; o.bias2 = c.bias; o.act2 = c.act; o.k0 = c.k0;
     if (c.part.p) o.part = op_slice(c.part, N, Ho, Wo);
@@ -102,6 +104,10 @@ int cc_conv(const cc_conv_op* op, void* stream) {
                s->W, N, Ho, Wo);
     CC_REQUIRE(s->C > 0 && s->co >= 0 && s->co + s->C <= s->cs, "cc_conv: %s slice cs=%d co=%d C=%d outside its row", what, s->cs,
                s->co, s->C);
+  }
+  if (o.out_ns != 0) {
+    CC_REQUIRE(o.kind == CC_CONV_OP_GEMM, "cc_conv: out_ns=%d needs kind GEMM, got %d", o.out_ns, o.kind);
+    CC_REQUIRE(o.out_ns >= Ho * Wo, "cc_conv: out_ns=%d pixels per image is less than the output's %dx%d", o.out_ns, Ho, Wo);
   }
   if (o.pre) {
     CC_REQUIRE((reinterpret_cast<uintptr_t>(o.pre) & 15) == 0, "cc_conv: pre=%p must be 16-byte aligned", o.pre);

@@ -26,6 +26,7 @@ struct BlockW {
 struct VOp {
   enum Kind { PATCHIFY, GEMM, EMBED_LN, LN, ATTN, TEXT_EMBED, L2NORM } kind;
   GemmLaunch gemm;
+  ConvDesc conv{};           // GEMM: the descriptor its launch was built from (cc_clip_op_conv reports it)
   // generic slots
   const float* f0 = nullptr; const float* f1 = nullptr; const float* f2 = nullptr; const float* f3 = nullptr;
   float* fo = nullptr;
@@ -114,7 +115,7 @@ struct PlanBuilder {
     const TSlice o = nhwc_slice(out, ldc, 0, N, f32 ? 1 : 0), r = nhwc_slice(res, ldc, 0, N, f32 ? 1 : 0);
     ConvDesc d = conv_desc(nhwc_slice(A, lda, 0, K, 0, n_img, 1, rows_per_img ? rows_per_img : Mrows), Wt, bias, 1, 1, o, act, res ? &r : nullptr);
     d.out_ns = out_ns;
-    VOp op; op.kind = VOp::GEMM; op.name = name;
+    VOp op; op.kind = VOp::GEMM; op.name = name; op.conv = d;
     rc = conv_gemm_build(d, M.sms, &op.gemm);
     if (rc) return;
     op.flops = op.gemm.flops;
@@ -174,10 +175,12 @@ struct PlanBuilder {
   }
 };
 
-static int run_plan(ClipPlan& P, const void* d_in, float* d_out, long long out_stride, cudaStream_t st,
+// ops [first, last) of the plan; ev: one event before each op and one after the last
+static int run_plan(ClipPlan& P, const void* d_in, float* d_out, long long out_stride, cudaStream_t st, size_t first, size_t last,
                     std::vector<cudaEvent_t>* ev = nullptr) {
   size_t oi = 0;
-  for (VOp& op : P.ops) {
+  for (size_t i = first; i < last; ++i) {
+    VOp& op = P.ops[i];
     int rc = CC_OK;
     if (ev) cudaEventRecord((*ev)[oi++], st);
     switch (op.kind) {
@@ -295,7 +298,8 @@ int cc_clip_encode_image(cc_clip* h, const float* d_x, int B, float* d_out, long
   ClipPlan* P = nullptr;
   int rc = clip_plan(h, false, B, &P);
   if (rc) return rc;
-  return run_plan(*P, d_x, d_out, out_row_stride > 0 ? out_row_stride : h->m.cfg.embed_dim, static_cast<cudaStream_t>(stream));
+  return run_plan(*P, d_x, d_out, out_row_stride > 0 ? out_row_stride : h->m.cfg.embed_dim, static_cast<cudaStream_t>(stream), 0,
+                  P->ops.size());
 }
 
 int cc_clip_encode_text(cc_clip* h, const int32_t* d_ids, int B, float* d_out, long long out_row_stride, void* stream) {
@@ -303,7 +307,8 @@ int cc_clip_encode_text(cc_clip* h, const int32_t* d_ids, int B, float* d_out, l
   ClipPlan* P = nullptr;
   int rc = clip_plan(h, true, B, &P);
   if (rc) return rc;
-  return run_plan(*P, d_ids, d_out, out_row_stride > 0 ? out_row_stride : h->m.cfg.embed_dim, static_cast<cudaStream_t>(stream));
+  return run_plan(*P, d_ids, d_out, out_row_stride > 0 ? out_row_stride : h->m.cfg.embed_dim, static_cast<cudaStream_t>(stream), 0,
+                  P->ops.size());
 }
 
 int cc_clip_profile(cc_clip* h, int text, const void* d_in, int B, float* d_out, int cap, float* ms, double* flops,
@@ -316,7 +321,7 @@ int cc_clip_profile(cc_clip* h, int text, const void* d_in, int B, float* d_out,
   std::vector<cudaEvent_t> ev(n + 1);
   for (auto& e : ev) CC_CHECK_CUDA(cudaEventCreate(&e));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  rc = run_plan(*P, d_in, d_out, h->m.cfg.embed_dim, st, &ev);
+  rc = run_plan(*P, d_in, d_out, h->m.cfg.embed_dim, st, 0, n, &ev);
   if (!rc) {
     CC_CHECK_CUDA(cudaStreamSynchronize(st));
     for (size_t i = 0; i < n && static_cast<int>(i) < cap; ++i) {
@@ -331,6 +336,31 @@ int cc_clip_profile(cc_clip* h, int text, const void* d_in, int B, float* d_out,
   if (n_ops) *n_ops = static_cast<int>(n);
   if (total_flops) *total_flops = P->flops;
   return rc;
+}
+
+// conv op taps: what each GEMM launch of the cached plan computes, and the plan run one range of ops at a time
+int cc_clip_op_conv(cc_clip* h, int text, int B, int i, cc_conv_op* out) {
+  CC_REQUIRE(h && B > 0, "cc_clip_op_conv: bad argument");
+  ClipPlan* P = nullptr;
+  if (int rc = clip_plan(h, text != 0, B, &P)) return rc;
+  const int n = static_cast<int>(P->ops.size());
+  if (!out) return n;
+  CC_REQUIRE(i >= 0 && i < n, "cc_clip_op_conv: op %d of a plan of %d ops", i, n);
+  const VOp& op = P->ops[i];
+  *out = op.kind == VOp::GEMM ? conv_op_of(op.conv, ChainDesc{}, op.gemm) : cc_conv_op{};
+  snprintf(out->name, sizeof(out->name), "%s", op.name);
+  return n;
+}
+
+int cc_clip_run_ops(cc_clip* h, int text, const void* d_in, int B, int first, int last, float* d_out, long long out_row_stride,
+                    void* stream) {
+  CC_REQUIRE(h && d_in && d_out && B > 0, "cc_clip_run_ops: bad argument");
+  ClipPlan* P = nullptr;
+  if (int rc = clip_plan(h, text != 0, B, &P)) return rc;
+  const int n = static_cast<int>(P->ops.size());
+  CC_REQUIRE(0 <= first && first <= last && last <= n, "cc_clip_run_ops: ops [%d, %d) of a plan of %d ops", first, last, n);
+  return run_plan(*P, d_in, d_out, out_row_stride > 0 ? out_row_stride : h->m.cfg.embed_dim, static_cast<cudaStream_t>(stream),
+                  first, last);
 }
 
 int cc_search_scores(const float* d_index, int N, int D, const float* d_q, int Q, float* d_scores, void* stream) {

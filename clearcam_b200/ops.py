@@ -7,15 +7,17 @@ from ._lib import CC_CONV_OP_CHAIN, CC_CONV_OP_DIRECT, CC_CONV_OP_GEMM, cc_conv_
 
 
 def conv2d(xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, Cout, act=0, res=None, res_co=0, groups=1, impl=1, bn=0,
-           stream=None, slope=None, pre=None):
+           stream=None, slope=None, pre=None, out_ns=0):
     """xbuf: [N,H,W,in_cs] bf16 CUDA; w: [Cout,k,k,Cin/groups] bf16; obuf: [N,Ho,Wo,out_cs] bf16|fp32.  impl 1 = the wgmma
     kernel, 2 = the direct kernel.  act = 3 (CC_ACT_PRELU): bias is the fp32 [9,Cout] border-class table and slope the fp32
-    [Cout] PReLU slopes, bf16 out.  pre: the fp32 [N,Ho/2,Wo/2,Cout] addend before the activation."""
+    [Cout] PReLU slopes, bf16 out.  pre: the fp32 [N,Ho/2,Wo/2,Cout] addend before the activation.  out_ns: pixels per image
+    in obuf's and res's buffers (0 = dense); obuf and res are then [N,Ho,Wo,cs] views with an image stride of out_ns * cs
+    elements, e.g. x.view(N, L, cs)[:, 1:].unsqueeze(1) for tokens 1.. of an L-token stream."""
     assert impl in (1, 2), "impl 1 = wgmma, 2 = direct"
     assert pre is None or (pre.dtype == torch.float32 and pre.is_contiguous() and pre.dim() == 4)
     return _conv(CC_CONV_OP_GEMM if impl == 1 else CC_CONV_OP_DIRECT, xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, Cout,
                  act, res, res_co, stream, groups=groups, BN=bn, slope=ptr(slope), pre=ptr(pre),
-                 pre_h=0 if pre is None else pre.shape[1], pre_w=0 if pre is None else pre.shape[2])
+                 pre_h=0 if pre is None else pre.shape[1], pre_w=0 if pre is None else pre.shape[2], out_ns=out_ns)
 
 
 def conv2d_chain(xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, w2, bias2, k0, o2buf, out2_co, act2=1, part=None,
@@ -38,10 +40,19 @@ def _slice(t, co, C):
     return cc_slice(t.data_ptr(), cs, co, C, N, H, W, int(t.dtype == torch.float32))
 
 
+def _dense_or_pitched(t, ns):
+    """t is contiguous, or (ns > 0) a [N,H,W,cs] view whose images are ns pixels apart and dense within."""
+    if t is None or ns == 0:
+        return t is None or t.is_contiguous()
+    N, H, W, cs = t.shape
+    return t.stride()[1:] == (W * cs, cs, 1) and (N == 1 or t.stride(0) == ns * cs)
+
+
 def _conv(kind, xbuf, in_co, Cin, w, bias, k, stride, obuf, out_co, Cout, act, res, res_co, stream, **fields):
     """One cc_conv launch of the given kind; `fields` sets the rest of the cc_conv_op."""
     assert xbuf.is_cuda and xbuf.dtype == torch.bfloat16 and xbuf.is_contiguous()
-    assert w.dtype == torch.bfloat16 and w.is_contiguous() and (obuf is None or obuf.is_contiguous())
+    ns = fields.get("out_ns", 0)
+    assert w.dtype == torch.bfloat16 and w.is_contiguous() and _dense_or_pitched(obuf, ns) and (ns == 0 or _dense_or_pitched(res, ns))
     op = cc_conv_op(kind=kind, in_=_slice(xbuf, in_co, Cin), out=_slice(obuf, out_co, Cout), res=_slice(res, res_co, Cout),
                     w=ptr(w), bias=ptr(bias), k=k, stride=stride, act=act, **{"groups": 1, **fields})
     check(lib().cc_conv(ctypes.byref(op), stream_ptr(stream)), "cc_conv")

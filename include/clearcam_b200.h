@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define CC_ABI_VERSION 2
+#define CC_ABI_VERSION 3
 
 int cc_version(void);
 const char* cc_last_error(void);
@@ -36,12 +36,12 @@ int cc_device_check(void);
 
 /* ---- kernel-level ops (used by the graphs below and exposed for the parity tests) ---- */
 
-/* One conv launch, as cc_conv takes it and as cc_yolo_op_conv reports a plan's launch: Conv2d(bias) [+act] [+residual], k in
+/* One conv launch, as cc_conv takes it and as cc_yolo_op_conv / cc_clip_op_conv / cc_face_op_conv report a plan's launch: Conv2d(bias) [+act] [+residual], k in
  * {1,3}, stride in {1,2}, pad = k/2, NHWC bf16 in, bf16|fp32 out.  Replaces nn.Conv2d + .silu() of detection/yolov9.py:33-38
  * (and the bare nn.Conv2d of :173,:186,:224).
  *   kind     CC_CONV_OP_GEMM: the wgmma implicit-GEMM kernel; CC_CONV_OP_CHAIN: the same with a 1x1 conv in its epilogue;
- *            CC_CONV_OP_DIRECT: the CUDA-core direct kernel, the only one that takes groups != 1.  cc_yolo_op_conv reports
- *            CC_CONV_OP_NONE for an op that is not a conv (the rest is then zero), and name: the op's name (cc_yolo_profile's).
+ *            CC_CONV_OP_DIRECT: the CUDA-core direct kernel, the only one that takes groups != 1.  The plan taps report
+ *            CC_CONV_OP_NONE for an op that is not a conv (the rest is then zero), and name: the op's name.
  *   in, out, res  NHWC slices (cc_slice: buffer p, channels per pixel cs, first channel co, channels C, extent N x H x W,
  *            f32: float elements, else bf16).  in is bf16, Cin = in.C; Cout = out.C; res (res.p == NULL: none) has out's
  *            dtype, is added after the activation and may be the output slice itself.  out and res have the output extent
@@ -67,7 +67,10 @@ int cc_device_check(void);
  *            128-pixel tile box 2^lTW x 2^lTH x 2^lTN (w, h, images), the stride-2 pair view s2, the pipeline stages,
  *            resident weights b_res, the persistent grid and the tile count; BNn, the narrow tile width (0: every tile is BN
  *            wide), and how many of the tiles are that narrow (the last wave's tiles split along N, and the remainder channel
- *            block when BN does not divide Cout). */
+ *            block when BN does not divide Cout).
+ *   out_ns   pixels per image in the out and res buffers, 0 = dense (Ho * Wo).  A larger pitch leaves the pixels past Ho * Wo
+ *            of each image untouched (the CLIP patch embedding writes tokens 1..L-1 of each image's L-row stream this way:
+ *            out.p one row past the buffer's start, Ho * Wo = L - 1, out_ns = L).  GEMM kind only; out_ns < Ho * Wo fails. */
 #define CC_CONV_OP_NONE 0
 #define CC_CONV_OP_GEMM 1
 #define CC_CONV_OP_CHAIN 2
@@ -82,6 +85,7 @@ typedef struct {
   const void* w2; const float* bias2; int act2, k0; cc_slice part, out2; int store1;
   int BN, BK, lTW, lTH, lTN, s2, stages, b_res, grid, num_tiles;
   int BNn, narrow_tiles;
+  int out_ns;
 } cc_conv_op;
 /* Launches the conv *op describes.  A kind other than GEMM, CHAIN or DIRECT, a NULL input, weight or output pointer, a slice
  * whose extent is not the conv's, a shape the chosen kernel does not take or a pair the kernel cannot chain (see conv_gemm.cu
@@ -322,6 +326,15 @@ int cc_clip_set_workspace(cc_clip* h, void* d_workspace, size_t bytes);
 /* per-op device timing of one encode (text != 0: text tower). */
 int cc_clip_profile(cc_clip* h, int text, const void* d_in, int B, float* d_out, int cap, float* ms, double* flops,
                     const char** names, int* n_ops, double* total_flops, void* stream);
+/* Conv op taps of the CLIP plans (text != 0: text tower), with cc_yolo_op_conv's contract: cc_clip_op_conv describes op i of
+ * the cached plan of batch B and returns the op count (out == NULL only counts; an i outside [0, count) fails); a GEMM is
+ * reported as CC_CONV_OP_GEMM (a linear over R rows as a 1x1 conv of N = 1, H = 1, W = R; the patch embedding with out_ns),
+ * any other op as CC_CONV_OP_NONE, both with cc_clip_profile's op name.  cc_clip_run_ops launches ops [first, last) exactly
+ * as an encode launches them; d_in, d_out and out_row_stride are those of cc_clip_encode_image / cc_clip_encode_text.
+ * Nothing synchronises. */
+int cc_clip_op_conv(cc_clip* h, int text, int B, int i, cc_conv_op* out);
+int cc_clip_run_ops(cc_clip* h, int text, const void* d_in, int B, int first, int last, float* d_out, long long out_row_stride,
+                    void* stream);
 /* ---- AdaFace IR-50 face embedder (replaces class ADAFACE, models/adaface.py:24-96) ---- */
 typedef struct cc_face cc_face;
 /* Weights: host fp32 tensors of the folded network that clearcam_b200/models/adaface.py `fold_state_dict` makes from the
@@ -344,6 +357,12 @@ int cc_face_set_workspace(cc_face* h, void* d_workspace, size_t bytes);
  * linear -> bn2 output before the L2 norm) and writes that map as dense fp32 NHWC [B,H,W,C] to d_dst.  d_dst = NULL only
  * reports C, H, W. */
 int cc_face_layer_output(cc_face* h, const uint8_t* d_faces, int B, int layer, float* d_dst, int* C, int* H, int* W, void* stream);
+/* Conv op taps of the face plans, as cc_clip_op_conv / cc_clip_run_ops: op names "pack", "stem", "body.<i>.c0", "body.<i>.sc"
+ * (the 1x1 shortcut, run as a 3x3 whose only nonzero tap is the centre), "body.<i>.c1", "linear" (a 1x1 conv of N = 1,
+ * H = 1, W = B over the 7x7x512 map as one row per face) and "l2norm".  d_faces and d_out are those of cc_face_embed
+ * (d_out rows of 512 floats). */
+int cc_face_op_conv(cc_face* h, int B, int i, cc_conv_op* out);
+int cc_face_run_ops(cc_face* h, const uint8_t* d_faces, int B, int first, int last, float* d_out, void* stream);
 
 /* ---- BlazeFace face detector (replaces class BlazeFace, models/blazeface.py:62-232), fp32 ---- */
 typedef struct cc_blazeface cc_blazeface;

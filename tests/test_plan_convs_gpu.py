@@ -42,11 +42,13 @@ pytestmark = pytest.mark.gpu
 
 REPS = 3      # distinct frames per batch: image b is a copy of image b % REPS, at a different offset within its tile group
 BF16, F32 = torch.bfloat16, torch.float32
-ACT_NAMES = {0: "NONE", 1: "SILU", 2: "GELU_TANH"}
+ACT_NAMES = {0: "NONE", 1: "SILU", 2: "GELU_TANH", 3: "PRELU"}
+ACT_PRELU = 3
 
 
 class Slice(NamedTuple):
-    """An NHWC slice of the workspace: byte offset of the buffer, channels per pixel, first channel, channels, N, H, W, fp32."""
+    """An NHWC slice of the workspace: byte offset of the buffer, channels per pixel, first channel, channels, N, H, W, fp32,
+    and the pixels from one image to the next (0: H * W, dense)."""
     off: int
     cs: int
     co: int
@@ -55,6 +57,7 @@ class Slice(NamedTuple):
     H: int
     W: int
     f32: int
+    ns: int = 0
 
 
 def sview(ws, s):
@@ -62,7 +65,7 @@ def sview(ws, s):
     es = 4 if s.f32 else 2
     assert s.off >= 0 and s.off % es == 0, s
     flat = ws.view(F32 if s.f32 else BF16)
-    return flat.as_strided((s.N, s.H, s.W, s.C), (s.H * s.W * s.cs, s.W * s.cs, s.cs, 1), s.off // es + s.co)
+    return flat.as_strided((s.N, s.H, s.W, s.C), ((s.ns or s.H * s.W) * s.cs, s.W * s.cs, s.cs, 1), s.off // es + s.co)
 
 
 def sbuf(ws, s):
@@ -78,19 +81,28 @@ def bits(t):
     return t.view(torch.int32 if t.dtype == F32 else torch.int16)
 
 
-def ref64(x, w, b, k, s, groups, act, res=None, pre=None):
+def ref64(x, w, b, k, s, groups, act, res=None, pre=None, slope=None):
     """float64 (z, y = [res +] act(z), sum|x.w| + |b| + |pre| + |res|) of a conv, z = conv(x, w) + b [+ up2(pre)].  x: [n, H, W,
-    Cin]; w: [Cout, k, k, Cin / groups]; pre: [n, Ho / 2, Wo / 2, Cout] added before the activation (nearest upsampling)."""
+    Cin]; w: [Cout, k, k, Cin / groups]; pre: [n, Ho / 2, Wo / 2, Cout] added before the activation (nearest upsampling).
+    act = ACT_PRELU: b is the [9, Cout] table indexed by the output pixel's border class, and act(z) = where(z > 0, z,
+    slope * z)."""
     xd, wd = x.double().permute(0, 3, 1, 2), w.double().permute(0, 3, 1, 2)
     z = F.conv2d(xd, wd, None, s, k // 2, 1, groups).permute(0, 2, 3, 1)
     mag = F.conv2d(xd.abs(), wd.abs(), None, s, k // 2, 1, groups).permute(0, 2, 3, 1)
     if b is not None:
-        z, mag = z + b.double(), mag + b.double().abs()
+        bd = b.double()
+        if act == ACT_PRELU:
+            from oracle.adaface import class_map
+            bd = bd[class_map(*z.shape[1:3]).to(bd.device)]
+        z, mag = z + bd, mag + bd.abs()
     if pre is not None:
         Ho, Wo = z.shape[1:3]
         up = pre.double()[:, torch.arange(Ho, device=pre.device) // 2][:, :, torch.arange(Wo, device=pre.device) // 2]
         z, mag = z + up, mag + up.abs()
-    y = F.silu(z) if act == 1 else F.gelu(z, approximate="tanh") if act == 2 else z
+    if act == ACT_PRELU:
+        y = torch.where(z > 0, z, slope.double() * z)
+    else:
+        y = F.silu(z) if act == 1 else F.gelu(z, approximate="tanh") if act == 2 else z
     if res is not None:
         y, mag = y + res.double(), mag + res.double().abs()
     return z, y, mag
@@ -100,9 +112,9 @@ def _first(mask):
     return tuple(int(v) for v in mask.nonzero()[0])
 
 
-def check_values(tag, got, x, w, b, k, s, groups, act, res, pre, f32, worst):
+def check_values(tag, got, x, w, b, k, s, groups, act, res, pre, f32, worst, slope=None):
     """(c), (b) and (a) of one output: got [B, Ho, Wo, C] is the whole batch as the op wrote it; x, res and pre are images
-    0..REPS-1 of the operands as stored before the op."""
+    0..REPS-1 of the operands as stored before the op; slope: the PReLU slopes of act = ACT_PRELU."""
     fin = torch.isfinite(got)
     assert fin.all(), f"{tag}: (c) output not finite at {_first(~fin)}"
     gb = bits(got)
@@ -111,7 +123,7 @@ def check_values(tag, got, x, w, b, k, s, groups, act, res, pre, f32, worst):
             raise AssertionError(f"{tag}: (b) image {i} differs from its copy, image {i % REPS}, at "
                                  f"{_first(gb[i] != gb[i % REPS])}")
     n = x.shape[0]
-    z, y, mag = ref64(x, w, b, k, s, groups, act, res, pre)
+    z, y, mag = ref64(x, w, b, k, s, groups, act, res, pre, slope)
     g = got[:n].double()
     if f32:
         # F32_BAR holds per tc.F32_STEPS k16 steps into one accumulator (see test_conv_gpu.py): the fp32-accurate mode's
@@ -120,6 +132,9 @@ def check_values(tag, got, x, w, b, k, s, groups, act, res, pre, f32, worst):
         bar, key = tc.F32_BAR * max(1.0, steps / tc.F32_STEPS) * mag, "fp32 |err|/bar"
     elif pre is not None:
         bar, key = td.pre_bar(z, y, mag, False), "bf16 + pre |err|/bar"
+    elif act == ACT_PRELU:
+        # the negative side scales z, and so z's fp32 error, by the slope
+        bar, key = 2.0 ** -7 * y.abs() + tc.F32_BAR * mag * slope.double().abs().clamp(min=1.0), "PReLU |err|/bar"
     else:
         bar, key = tc.bf16_bar(z, y, mag, act), "bf16 |err|/bar"
     err = (g - y).abs()
@@ -161,16 +176,25 @@ def op_outputs(op):
     return ([op.out] if not chained or op.store1 else []) + ([op.out2] if chained else [])
 
 
-def check_op(op, snap, ws, worst):
-    """(a)-(e) of one conv op that ran on ws, whose contents before the op were snap."""
+def images(t, rows):
+    """t [1, 1, R, C], the R rows of a row GEMM (a linear as a 1x1 conv), as [R / rows, 1, rows, C]: one image per block of
+    `rows` rows.  rows = 0: t as it is."""
+    return t if not rows else t.reshape(-1, 1, rows, t.shape[-1])
+
+
+def check_op(op, snap, ws, worst, rows=0):
+    """(a)-(e) of one conv op that ran on ws, whose contents before the op were snap.  rows: the op is a row GEMM whose images
+    are blocks of that many rows (see `images`)."""
     tag = op.name
     check_stray(tag, snap, ws, op_outputs(op))
-    n = min(REPS, op.in_.N)
-    x = sview(snap, op.in_)[:n]
-    res = None if op.res is None else sview(snap, op.res)[:n]
+    xs = images(sview(snap, op.in_), rows)
+    n = min(REPS, xs.shape[0])
+    x = xs[:n]
+    res = None if op.res is None else images(sview(snap, op.res), rows)[:n]
     pre = None if op.pre is None else sview(snap, op.pre)[:n]
     if op.kind != CC_CONV_OP_CHAIN:
-        check_values(tag, sview(ws, op.out), x, op.w, op.bias, op.k, op.stride, op.groups, op.act, res, pre, op.out.f32, worst)
+        check_values(tag, images(sview(ws, op.out), rows), x, op.w, op.bias, op.k, op.stride, op.groups, op.act, res, pre,
+                     op.out.f32, worst, op.slope)
         return
     # (e) the same two convs unchained, on the operands as stored: the first into a copy of its buffer
     buf1 = sbuf(snap, op.out).clone()
@@ -293,18 +317,20 @@ def _plan_op(d, ws):
     """The conv op d (a cc_conv_op) with its slices as workspace offsets and its weights copied out."""
     wp, nbytes = ws.data_ptr(), ws.numel()
 
-    def sl(s):
+    def sl(s, ns=0):
         if not s.p:
             return None
         assert wp <= s.p < wp + nbytes, f"{d.name.decode()}: a slice outside the workspace"
-        return Slice(s.p - wp, s.cs, s.co, s.C, s.N, s.H, s.W, s.f32)
+        return Slice(s.p - wp, s.cs, s.co, s.C, s.N, s.H, s.W, s.f32, ns)
 
     Cout = d.out.C
-    op = types.SimpleNamespace(kind=d.kind, name=d.name.decode(), in_=sl(d.in_), out=sl(d.out), res=sl(d.res), k=d.k,
-                               stride=d.stride, groups=d.groups, act=d.act, store1=d.store1, k0=d.k0, act2=d.act2,
-                               part=sl(d.part), out2=sl(d.out2), pre=None, w2=None, bias2=None)
+    op = types.SimpleNamespace(kind=d.kind, name=d.name.decode(), in_=sl(d.in_), out=sl(d.out, d.out_ns), res=sl(d.res, d.out_ns),
+                               k=d.k, stride=d.stride, groups=d.groups, act=d.act, store1=d.store1, k0=d.k0, act2=d.act2,
+                               part=sl(d.part), out2=sl(d.out2), pre=None, w2=None, bias2=None, slope=None)
     op.w = _device(d.w, (Cout, d.k, d.k, d.in_.C // d.groups), BF16)
-    op.bias = _device(d.bias, (Cout,), F32) if d.bias else None
+    op.bias = _device(d.bias, (9, Cout) if d.act == ACT_PRELU else (Cout,), F32) if d.bias else None
+    if d.act == ACT_PRELU:
+        op.slope = _device(d.slope, (Cout,), F32)
     if d.pre:
         assert wp <= d.pre < wp + nbytes
         op.pre = Slice(d.pre - wp, Cout, 0, Cout, d.out.N, d.pre_h, d.pre_w, 1)
