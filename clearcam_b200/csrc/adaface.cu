@@ -23,6 +23,7 @@
 #include "cc_common.h"
 #include "conv_gemm.cuh"
 #include "ops.cuh"
+#include "plan.h"
 
 namespace cc {
 
@@ -46,32 +47,16 @@ __global__ void face_pack_kernel(const uint8_t* __restrict__ in, __nv_bfloat16* 
   }
 }
 
-// one NHWC slice -> dense fp32 (the layer taps)
-__global__ void face_tap_kernel(const void* __restrict__ src, int f32, int C, long long n, float* __restrict__ dst) {
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<long long>(gridDim.x) * blockDim.x)
-    dst[i] = f32 ? static_cast<const float*>(src)[i] : __bfloat162float(static_cast<const __nv_bfloat16*>(src)[i]);
-}
-
 struct FaceBlockW {
   __nv_bfloat16 *w0 = nullptr, *w1 = nullptr, *wsc = nullptr;   // wsc == nullptr: identity shortcut at stride 1
   float *cls0 = nullptr, *slope0 = nullptr, *b1 = nullptr, *bsc = nullptr;
 };
 
-struct FOp {
-  enum Kind { PACK, GEMM, L2NORM } kind;
-  std::string name;          // pack, stem, body.<i>.c0 | sc | c1, linear, l2norm
-  GemmLaunch gemm;
-  ConvDesc conv{};           // GEMM: the descriptor its launch was built from (cc_face_op_conv reports it)
-  __nv_bfloat16* packed = nullptr;
-  float* feat = nullptr;
-};
-
-struct FaceLayer { const void* p; int f32, C, H, W; size_t last_op; };
+struct FaceLayer { TSlice out; size_t last_op; };   // a layer's output and the op that completes it
 
 struct FacePlan {
   int B = 0;
-  std::vector<FOp> ops;
+  std::vector<PlanOp> ops;   // pack, stem, body.<i>.c0 | sc | c1, linear, l2norm
   std::vector<FaceLayer> layers;     // 0: stem, 1..24: blocks, 25: the linear's output before the L2 norm
 };
 
@@ -101,20 +86,20 @@ struct FacePlanBuilder {
   Bump bump;
   FacePlanBuilder(FaceModel& m, FacePlan& p) : M(m), P(p) {}
   void* dalloc(size_t bytes) { return bump.take(bytes); }
-  void gemm(std::string name, const ConvDesc& d) {
+  void gemm(const std::string& name, const ConvDesc& d) {
     if (rc || bump.dry) return;
-    FOp op; op.kind = FOp::GEMM; op.name = std::move(name); op.conv = d;
-    rc = conv_gemm_build(d, M.sms, &op.gemm);
+    GemmLaunch L;
+    rc = conv_gemm_build(d, M.sms, &L);
     if (rc) return;
-    P.ops.push_back(op);
+    P.ops.push_back(gemm_op(name, d, ChainDesc{}, L));
   }
-  void conv(std::string name, const TSlice& in, const __nv_bfloat16* w, const float* bias, const float* slope, int stride,
+  void conv(const std::string& name, const TSlice& in, const __nv_bfloat16* w, const float* bias, const float* slope, int stride,
             const TSlice& out, int act, const TSlice* res) {
     ConvDesc d = conv_desc(in, w, bias, 3, stride, out, act, res);
     d.slope = slope;
-    gemm(std::move(name), d);
+    gemm(name, d);
   }
-  void layer(const void* p, int f32, int C, int H, int W) { P.layers.push_back(FaceLayer{p, f32, C, H, W, P.ops.size() - 1}); }
+  void layer(const TSlice& out) { P.layers.push_back(FaceLayer{out, P.ops.size() - 1}); }
   int build(int B) {
     const size_t big = static_cast<size_t>(B) * kFaceSide * kFaceSide * 64 * 2;
     __nv_bfloat16* packed = static_cast<__nv_bfloat16*>(dalloc(static_cast<size_t>(B) * kFaceSide * kFaceSide * kFacePackC * 2));
@@ -123,11 +108,18 @@ struct FacePlanBuilder {
     __nv_bfloat16* S = static_cast<__nv_bfloat16*>(dalloc(big));
     float* feat = static_cast<float*>(dalloc(static_cast<size_t>(B) * kFaceDim * 4));
     if (bump.dry) return CC_OK;
-    { FOp op; op.kind = FOp::PACK; op.name = "pack"; op.packed = packed; P.ops.push_back(op); }
+    P.ops.push_back(plan_op("pack", "face_pack", [packed, B](const PlanIO& io, cudaStream_t st) {
+      const long long npix = static_cast<long long>(B) * kFaceSide * kFaceSide;
+      const long long blocks = (npix + 255) / 256;
+      face_pack_kernel<<<blocks < 132 * 16 ? static_cast<int>(blocks) : 132 * 16, 256, 0, st>>>(static_cast<const uint8_t*>(io.in),
+                                                                                              packed, npix);
+      CC_CHECK_CUDA(cudaGetLastError());
+      return CC_OK;
+    }));
     int H = kFaceSide;
     conv("stem", nhwc_slice(packed, kFacePackC, 0, kFacePackC, 0, B, H, H), M.stem_w, M.stem_cls, M.stem_slope, 1,
          nhwc_slice(X, 64, 0, 64), ACT_PRELU, nullptr);
-    layer(X, 0, 64, H, H);
+    layer(nhwc_slice(X, 64, 0, 64, 0, B, H, H));
     for (int i = 0; i < kFaceBlocks && !rc; ++i) {
       const int cin = kFaceSizes[i][0], D = kFaceSizes[i][1], s = kFaceSizes[i][2], Ho = H / s;
       const FaceBlockW& b = M.blk[i];
@@ -143,7 +135,7 @@ struct FacePlanBuilder {
         std::swap(X, S);
       }
       H = Ho;
-      layer(X, 0, D, H, H);
+      layer(nhwc_slice(X, D, 0, D, 0, B, H, H));
     }
     if (rc) return rc;
     {  // bn -> flatten -> linear -> bn2: [B, 7*7*512] . W^T + b, fp32
@@ -154,34 +146,14 @@ struct FacePlanBuilder {
       d.bn_override = 32;
       gemm("linear", d);
       if (rc) return rc;
-      layer(feat, 1, kFaceDim, 1, 1);
+      layer(nhwc_slice(feat, kFaceDim, 0, kFaceDim, 1, B, 1, 1));
     }
-    { FOp op; op.kind = FOp::L2NORM; op.name = "l2norm"; op.feat = feat; P.ops.push_back(op); }
+    P.ops.push_back(plan_op("l2norm", "l2norm", [feat, B](const PlanIO& io, cudaStream_t st) {
+      return l2norm_launch(feat, io.out, B, kFaceDim, io.out_stride, 0.f, st);
+    }));
     return rc;
   }
 };
-
-// ops [first, last) of the plan of batch B
-static int run_face_plan(FacePlan& P, const uint8_t* d_faces, int B, size_t first, size_t last, float* d_out, long long out_stride,
-                         cudaStream_t st) {
-  for (size_t i = first; i < last; ++i) {
-    FOp& op = P.ops[i];
-    int rc = CC_OK;
-    switch (op.kind) {
-      case FOp::PACK: {
-        const long long npix = static_cast<long long>(B) * kFaceSide * kFaceSide;
-        const long long blocks = (npix + 255) / 256;
-        face_pack_kernel<<<blocks < 132 * 16 ? static_cast<int>(blocks) : 132 * 16, 256, 0, st>>>(d_faces, op.packed, npix);
-        CC_CHECK_CUDA(cudaGetLastError());
-        break;
-      }
-      case FOp::GEMM: rc = conv_gemm_launch(op.gemm, st); break;
-      case FOp::L2NORM: rc = l2norm_launch(op.feat, d_out, B, kFaceDim, out_stride, 0.f, st); break;
-    }
-    if (rc) return rc;
-  }
-  return CC_OK;
-}
 
 }  // namespace cc
 
@@ -277,8 +249,7 @@ int cc_face_embed(cc_face* h, const uint8_t* d_faces, int B, float* d_out, long 
   CC_REQUIRE((reinterpret_cast<uintptr_t>(d_out) & 3) == 0, "cc_face_embed: d_out must be 4-byte aligned");
   FacePlan* P = nullptr;
   if (int rc = face_plan(h, B, &P)) return rc;
-  return run_face_plan(*P, d_faces, B, 0, P->ops.size(), d_out, out_row_stride > 0 ? out_row_stride : kFaceDim,
-                       static_cast<cudaStream_t>(stream));
+  return run_ops(P->ops, PlanIO{d_faces, d_out, out_row_stride > 0 ? out_row_stride : kFaceDim}, static_cast<cudaStream_t>(stream));
 }
 
 int cc_face_layer_output(cc_face* h, const uint8_t* d_faces, int B, int layer, float* d_dst, int* C, int* H, int* W, void* stream) {
@@ -286,17 +257,15 @@ int cc_face_layer_output(cc_face* h, const uint8_t* d_faces, int B, int layer, f
   CC_REQUIRE(layer >= 0 && layer <= kFaceBlocks + 1, "cc_face_layer_output: bad layer %d (0 stem, 1..24 blocks, 25 linear)", layer);
   FacePlan* P = nullptr;
   if (int rc = face_plan(h, B, &P)) return rc;
-  const FaceLayer& t = P->layers[layer];
+  const TSlice& t = P->layers[layer].out;
   if (C) *C = t.C;
   if (H) *H = t.H;
   if (W) *W = t.W;
   if (!d_dst) return CC_OK;
   CC_REQUIRE(d_faces, "cc_face_layer_output: d_faces is NULL");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = run_face_plan(*P, d_faces, B, 0, t.last_op + 1, nullptr, kFaceDim, st)) return rc;
-  face_tap_kernel<<<132 * 8, 256, 0, st>>>(t.p, t.f32, t.C, static_cast<long long>(B) * t.H * t.W * t.C, d_dst);
-  CC_CHECK_CUDA(cudaGetLastError());
-  return CC_OK;
+  if (int rc = run_ops(P->ops, PlanIO{d_faces, nullptr, kFaceDim}, st, 0, P->layers[layer].last_op + 1)) return rc;
+  return slice_to_f32_launch(t, d_dst, st);
 }
 
 // conv op taps: what each GEMM launch of the cached plan computes, and the plan run one range of ops at a time
@@ -304,13 +273,7 @@ int cc_face_op_conv(cc_face* h, int B, int i, cc_conv_op* out) {
   CC_REQUIRE(h && B > 0, "cc_face_op_conv: bad argument");
   FacePlan* P = nullptr;
   if (int rc = face_plan(h, B, &P)) return rc;
-  const int n = static_cast<int>(P->ops.size());
-  if (!out) return n;
-  CC_REQUIRE(i >= 0 && i < n, "cc_face_op_conv: op %d of a plan of %d ops", i, n);
-  const FOp& op = P->ops[i];
-  *out = op.kind == FOp::GEMM ? conv_op_of(op.conv, ChainDesc{}, op.gemm) : cc_conv_op{};
-  snprintf(out->name, sizeof(out->name), "%s", op.name.c_str());
-  return n;
+  return op_conv_tap("cc_face_op_conv", P->ops, i, out);
 }
 
 int cc_face_run_ops(cc_face* h, const uint8_t* d_faces, int B, int first, int last, float* d_out, void* stream) {
@@ -318,9 +281,8 @@ int cc_face_run_ops(cc_face* h, const uint8_t* d_faces, int B, int first, int la
   CC_REQUIRE((reinterpret_cast<uintptr_t>(d_out) & 3) == 0, "cc_face_run_ops: d_out must be 4-byte aligned");
   FacePlan* P = nullptr;
   if (int rc = face_plan(h, B, &P)) return rc;
-  const int n = static_cast<int>(P->ops.size());
-  CC_REQUIRE(0 <= first && first <= last && last <= n, "cc_face_run_ops: ops [%d, %d) of a plan of %d ops", first, last, n);
-  return run_face_plan(*P, d_faces, B, first, last, d_out, kFaceDim, static_cast<cudaStream_t>(stream));
+  if (int rc = check_range("cc_face_run_ops", first, last, static_cast<int>(P->ops.size()))) return rc;
+  return run_ops(P->ops, PlanIO{d_faces, d_out, kFaceDim}, static_cast<cudaStream_t>(stream), first, last);
 }
 
 }  // extern "C"

@@ -13,6 +13,7 @@
 #include "cc_common.h"
 #include "conv_gemm.cuh"
 #include "ops.cuh"
+#include "plan.h"
 
 namespace cc {
 
@@ -23,25 +24,9 @@ struct BlockW {
   float *b_in, *b_out, *b_fc, *b_proj;
 };
 
-struct VOp {
-  enum Kind { PATCHIFY, GEMM, EMBED_LN, LN, ATTN, TEXT_EMBED, L2NORM } kind;
-  GemmLaunch gemm;
-  ConvDesc conv{};           // GEMM: the descriptor its launch was built from (cc_clip_op_conv reports it)
-  // generic slots
-  const float* f0 = nullptr; const float* f1 = nullptr; const float* f2 = nullptr; const float* f3 = nullptr;
-  float* fo = nullptr;
-  __nv_bfloat16* bo = nullptr; const __nv_bfloat16* bi = nullptr; __nv_bfloat16* bw = nullptr;
-  const int* idx = nullptr; int* io = nullptr;
-  int i0 = 0, i1 = 0, i2 = 0, i3 = 0, i4 = 0;
-  long long l0 = 0;
-  float eps = 0.f;
-  const char* name = "";
-  double flops = 0;
-};
-
 struct ClipPlan {
   int B = 0; bool text = false;
-  std::vector<VOp> ops;
+  std::vector<PlanOp> ops;
   size_t alloc_bytes = 0;      // bytes of the handle's shared workspace this plan addresses
   double flops = 0;
 };
@@ -107,6 +92,10 @@ struct PlanBuilder {
     P.alloc_bytes = bump.off;
     return d;
   }
+  void push(PlanOp op) {
+    P.flops += op.flops;
+    P.ops.push_back(std::move(op));
+  }
   // out[M,N] = act(A[M,K] . Wt[N,K]^T + bias) (+res)
   void gemm(const char* name, const __nv_bfloat16* A, int lda, int Mrows, int K, const __nv_bfloat16* Wt, const float* bias,
             int N, void* out, int ldc, bool f32, int act, const void* res, int n_img = 1, int rows_per_img = 0, int out_ns = 0) {
@@ -115,12 +104,23 @@ struct PlanBuilder {
     const TSlice o = nhwc_slice(out, ldc, 0, N, f32 ? 1 : 0), r = nhwc_slice(res, ldc, 0, N, f32 ? 1 : 0);
     ConvDesc d = conv_desc(nhwc_slice(A, lda, 0, K, 0, n_img, 1, rows_per_img ? rows_per_img : Mrows), Wt, bias, 1, 1, o, act, res ? &r : nullptr);
     d.out_ns = out_ns;
-    VOp op; op.kind = VOp::GEMM; op.name = name; op.conv = d;
-    rc = conv_gemm_build(d, M.sms, &op.gemm);
+    GemmLaunch L;
+    rc = conv_gemm_build(d, M.sms, &L);
     if (rc) return;
-    op.flops = op.gemm.flops;
-    P.flops += op.flops;
-    P.ops.push_back(op);
+    push(gemm_op(name, d, ChainDesc{}, L));
+  }
+  // LayerNorm of `rows` fp32 rows of x (row_stride rows apart, or the rows row_idx names) into bf16
+  void layernorm(const char* name, const float* x, __nv_bfloat16* out, const float* g, const float* b, int rows, int W,
+                 long long row_stride, const int* row_idx) {
+    push(plan_op(name, "layernorm", [=](const PlanIO&, cudaStream_t st) {
+      return layernorm_bf16_launch(x, out, g, b, rows, W, row_stride, row_idx, st);
+    }));
+  }
+  // the embeddings, L2-normalised into the call's output rows
+  void l2norm(const float* emb, int B, int D, float eps) {
+    push(plan_op("l2norm", "l2norm", [=](const PlanIO& io, cudaStream_t st) {
+      return l2norm_launch(emb, io.out, B, D, io.out_stride, eps, st);
+    }));
   }
   void blocks(const Tower& tw, const std::vector<BlockW>& bw, int B, float* x, bool causal) {
     const int W = tw.width, L = tw.tokens, rows = B * L;
@@ -131,12 +131,14 @@ struct PlanBuilder {
     __nv_bfloat16* vt = attention_tc_supported(L) ? static_cast<__nv_bfloat16*>(dalloc(attention_tc_workspace_bytes(B, L, tw.heads))) : nullptr;
     for (int i = 0; i < tw.layers && !rc; ++i) {
       const BlockW& b = bw[i];
-      { VOp op; op.kind = VOp::LN; op.name = "ln_1"; op.f0 = x; op.bo = h; op.f1 = b.ln1_g; op.f2 = b.ln1_b; op.i0 = rows; op.i1 = W; op.l0 = 1; P.ops.push_back(op); }
+      layernorm("ln_1", x, h, b.ln1_g, b.ln1_b, rows, W, 1, nullptr);
       gemm("qkv", h, W, rows, W, b.w_in, b.b_in, 3 * W, qkv, 3 * W, false, CC_ACT_NONE, nullptr);
-      { VOp op; op.kind = VOp::ATTN; op.name = "attention"; op.bi = qkv; op.bo = ctx; op.bw = vt; op.i0 = B; op.i1 = L; op.i2 = tw.heads; op.i3 = causal ? 1 : 0;
-        op.flops = 4.0 * B * tw.heads * double(L) * L * 64; P.flops += op.flops; P.ops.push_back(op); }
+      const int heads = tw.heads, c = causal ? 1 : 0;
+      push(plan_op("attention", "attention", [=](const PlanIO&, cudaStream_t st) {
+        return vt ? attention_tc_launch(qkv, ctx, vt, B, L, heads, c, st) : attention_launch(qkv, ctx, B, L, heads, c, st);
+      }, 4.0 * B * tw.heads * double(L) * L * 64));
       gemm("out_proj", ctx, W, rows, W, b.w_out, b.b_out, W, x, W, true, CC_ACT_NONE, x);
-      { VOp op; op.kind = VOp::LN; op.name = "ln_2"; op.f0 = x; op.bo = h; op.f1 = b.ln2_g; op.f2 = b.ln2_b; op.i0 = rows; op.i1 = W; op.l0 = 1; P.ops.push_back(op); }
+      layernorm("ln_2", x, h, b.ln2_g, b.ln2_b, rows, W, 1, nullptr);
       gemm("mlp_fc", h, W, rows, W, b.w_fc, b.b_fc, tw.mlp, hid, tw.mlp, false, CC_ACT_GELU_TANH, nullptr);
       gemm("mlp_proj", hid, tw.mlp, rows, tw.mlp, b.w_proj, b.b_proj, W, x, W, true, CC_ACT_NONE, x);
     }
@@ -146,17 +148,22 @@ struct PlanBuilder {
     const int W = tw.width, L = tw.tokens, Pn = L - 1, S = M.cfg.image_size, p = M.cfg.patch, D = M.cfg.embed_dim;
     __nv_bfloat16* patches = static_cast<__nv_bfloat16*>(dalloc(static_cast<size_t>(B) * Pn * M.kpad * 2));
     float* x = static_cast<float*>(dalloc(static_cast<size_t>(B) * L * W * 4));
-    { VOp op; op.kind = VOp::PATCHIFY; op.name = "patchify"; op.bo = patches; op.i0 = B; op.i1 = S; op.i2 = p; op.i3 = M.kpad; P.ops.push_back(op); }
+    const int kpad = M.kpad;
+    push(plan_op("patchify", "patchify", [=](const PlanIO& io, cudaStream_t st) {
+      return patchify_launch(static_cast<const float*>(io.in), patches, B, S, p, kpad, st);
+    }));
     // conv14x14/s14 (no bias) == GEMM over patches; rows land at token 1.. of each image (out_ns = L, +1 row offset)
     gemm("patch_embed", patches, M.kpad, B * Pn, M.kpad, M.patch_w, nullptr, W, x + W, W, true, CC_ACT_NONE, nullptr, B, Pn, L);
-    { VOp op; op.kind = VOp::EMBED_LN; op.name = "cls+pos+ln_pre"; op.fo = x; op.f0 = M.cls; op.f1 = M.pos; op.f2 = M.lnpre_g; op.f3 = M.lnpre_b;
-      op.i0 = B * L; op.i1 = L; op.i2 = W; P.ops.push_back(op); }
+    const float *cls = M.cls, *pos = M.pos, *g = M.lnpre_g, *b = M.lnpre_b;
+    push(plan_op("cls+pos+ln_pre", "embed_ln_pre", [=](const PlanIO&, cudaStream_t st) {
+      return embed_ln_pre_launch(x, cls, pos, g, b, B * L, L, W, st);
+    }));
     blocks(tw, M.vb, B, x, false);
     __nv_bfloat16* pooled = static_cast<__nv_bfloat16*>(dalloc(static_cast<size_t>(B) * W * 2));
     float* emb = static_cast<float*>(dalloc(static_cast<size_t>(B) * D * 4));
-    { VOp op; op.kind = VOp::LN; op.name = "ln_post(token 0)"; op.f0 = x; op.bo = pooled; op.f1 = M.lnpost_g; op.f2 = M.lnpost_b; op.i0 = B; op.i1 = W; op.l0 = L; P.ops.push_back(op); }
+    layernorm("ln_post(token 0)", x, pooled, M.lnpost_g, M.lnpost_b, B, W, L, nullptr);
     gemm("proj", pooled, W, B, W, M.projT, nullptr, D, emb, D, true, CC_ACT_NONE, nullptr);
-    { VOp op; op.kind = VOp::L2NORM; op.name = "l2norm"; op.f0 = emb; op.i0 = B; op.i1 = D; op.eps = 1e-8f; P.ops.push_back(op); }
+    l2norm(emb, B, D, 1e-8f);
     return rc;
   }
   int build_text(int B) {
@@ -164,42 +171,20 @@ struct PlanBuilder {
     const int W = tw.width, L = tw.tokens, D = M.cfg.embed_dim;
     float* x = static_cast<float*>(dalloc(static_cast<size_t>(B) * L * W * 4));
     int* eot = static_cast<int*>(dalloc(static_cast<size_t>(B) * 4));
-    { VOp op; op.kind = VOp::TEXT_EMBED; op.name = "tok+pos"; op.f0 = M.tok; op.f1 = M.pos_t; op.fo = x; op.io = eot; op.i0 = B; op.i1 = L; op.i2 = W; op.i3 = M.cfg.vocab; P.ops.push_back(op); }
+    const float *tok = M.tok, *pos = M.pos_t;
+    const int vocab = M.cfg.vocab;
+    push(plan_op("tok+pos", "text_embed", [=](const PlanIO& io, cudaStream_t st) {
+      return text_embed_launch(static_cast<const int*>(io.in), tok, pos, x, eot, B, L, W, vocab, st);
+    }));
     blocks(tw, M.tb, B, x, true);
     __nv_bfloat16* pooled = static_cast<__nv_bfloat16*>(dalloc(static_cast<size_t>(B) * W * 2));
     float* emb = static_cast<float*>(dalloc(static_cast<size_t>(B) * D * 4));
-    { VOp op; op.kind = VOp::LN; op.name = "ln_final(EOT row)"; op.f0 = x; op.bo = pooled; op.f1 = M.lnf_g; op.f2 = M.lnf_b; op.i0 = B; op.i1 = W; op.idx = eot; P.ops.push_back(op); }
+    layernorm("ln_final(EOT row)", x, pooled, M.lnf_g, M.lnf_b, B, W, 0, eot);
     gemm("text_projection", pooled, W, B, W, M.tprojT, nullptr, D, emb, D, true, CC_ACT_NONE, nullptr);
-    { VOp op; op.kind = VOp::L2NORM; op.name = "l2norm"; op.f0 = emb; op.i0 = B; op.i1 = D; op.eps = 0.f; P.ops.push_back(op); }
+    l2norm(emb, B, D, 0.f);
     return rc;
   }
 };
-
-// ops [first, last) of the plan; ev: one event before each op and one after the last
-static int run_plan(ClipPlan& P, const void* d_in, float* d_out, long long out_stride, cudaStream_t st, size_t first, size_t last,
-                    std::vector<cudaEvent_t>* ev = nullptr) {
-  size_t oi = 0;
-  for (size_t i = first; i < last; ++i) {
-    VOp& op = P.ops[i];
-    int rc = CC_OK;
-    if (ev) cudaEventRecord((*ev)[oi++], st);
-    switch (op.kind) {
-      case VOp::PATCHIFY: rc = patchify_launch(static_cast<const float*>(d_in), op.bo, op.i0, op.i1, op.i2, op.i3, st); break;
-      case VOp::GEMM: rc = conv_gemm_launch(op.gemm, st); break;
-      case VOp::EMBED_LN: rc = embed_ln_pre_launch(op.fo, op.f0, op.f1, op.f2, op.f3, op.i0, op.i1, op.i2, st); break;
-      case VOp::LN: rc = layernorm_bf16_launch(op.f0, op.bo, op.f1, op.f2, op.i0, op.i1, op.l0, op.idx, st); break;
-      case VOp::ATTN:
-        rc = op.bw ? attention_tc_launch(op.bi, op.bo, op.bw, op.i0, op.i1, op.i2, op.i3, st)
-                   : attention_launch(op.bi, op.bo, op.i0, op.i1, op.i2, op.i3, st);
-        break;
-      case VOp::TEXT_EMBED: rc = text_embed_launch(static_cast<const int*>(d_in), op.f0, op.f1, op.fo, op.io, op.i0, op.i1, op.i2, op.i3, st); break;
-      case VOp::L2NORM: rc = l2norm_launch(op.f0, d_out, op.i0, op.i1, out_stride, op.eps, st); break;
-    }
-    if (rc) return rc;
-  }
-  if (ev) cudaEventRecord((*ev)[oi], st);
-  return CC_OK;
-}
 
 }  // namespace cc
 
@@ -298,8 +283,7 @@ int cc_clip_encode_image(cc_clip* h, const float* d_x, int B, float* d_out, long
   ClipPlan* P = nullptr;
   int rc = clip_plan(h, false, B, &P);
   if (rc) return rc;
-  return run_plan(*P, d_x, d_out, out_row_stride > 0 ? out_row_stride : h->m.cfg.embed_dim, static_cast<cudaStream_t>(stream), 0,
-                  P->ops.size());
+  return run_ops(P->ops, PlanIO{d_x, d_out, out_row_stride > 0 ? out_row_stride : h->m.cfg.embed_dim}, static_cast<cudaStream_t>(stream));
 }
 
 int cc_clip_encode_text(cc_clip* h, const int32_t* d_ids, int B, float* d_out, long long out_row_stride, void* stream) {
@@ -307,8 +291,7 @@ int cc_clip_encode_text(cc_clip* h, const int32_t* d_ids, int B, float* d_out, l
   ClipPlan* P = nullptr;
   int rc = clip_plan(h, true, B, &P);
   if (rc) return rc;
-  return run_plan(*P, d_ids, d_out, out_row_stride > 0 ? out_row_stride : h->m.cfg.embed_dim, static_cast<cudaStream_t>(stream), 0,
-                  P->ops.size());
+  return run_ops(P->ops, PlanIO{d_ids, d_out, out_row_stride > 0 ? out_row_stride : h->m.cfg.embed_dim}, static_cast<cudaStream_t>(stream));
 }
 
 int cc_clip_profile(cc_clip* h, int text, const void* d_in, int B, float* d_out, int cap, float* ms, double* flops,
@@ -317,23 +300,9 @@ int cc_clip_profile(cc_clip* h, int text, const void* d_in, int B, float* d_out,
   ClipPlan* P = nullptr;
   int rc = clip_plan(h, text != 0, B, &P);
   if (rc) return rc;
-  const size_t n = P->ops.size();
-  std::vector<cudaEvent_t> ev(n + 1);
-  for (auto& e : ev) CC_CHECK_CUDA(cudaEventCreate(&e));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  rc = run_plan(*P, d_in, d_out, h->m.cfg.embed_dim, st, 0, n, &ev);
-  if (!rc) {
-    CC_CHECK_CUDA(cudaStreamSynchronize(st));
-    for (size_t i = 0; i < n && static_cast<int>(i) < cap; ++i) {
-      float t = 0.f;
-      cudaEventElapsedTime(&t, ev[i], ev[i + 1]);
-      if (ms) ms[i] = t;
-      if (flops) flops[i] = P->ops[i].flops;
-      if (names) names[i] = P->ops[i].name;
-    }
-  }
-  for (auto& e : ev) cudaEventDestroy(e);
-  if (n_ops) *n_ops = static_cast<int>(n);
+  rc = profile_ops(P->ops, PlanIO{d_in, d_out, h->m.cfg.embed_dim}, static_cast<cudaStream_t>(stream), cap, ms, flops, nullptr, nullptr,
+                   names);
+  if (n_ops) *n_ops = static_cast<int>(P->ops.size());
   if (total_flops) *total_flops = P->flops;
   return rc;
 }
@@ -343,13 +312,7 @@ int cc_clip_op_conv(cc_clip* h, int text, int B, int i, cc_conv_op* out) {
   CC_REQUIRE(h && B > 0, "cc_clip_op_conv: bad argument");
   ClipPlan* P = nullptr;
   if (int rc = clip_plan(h, text != 0, B, &P)) return rc;
-  const int n = static_cast<int>(P->ops.size());
-  if (!out) return n;
-  CC_REQUIRE(i >= 0 && i < n, "cc_clip_op_conv: op %d of a plan of %d ops", i, n);
-  const VOp& op = P->ops[i];
-  *out = op.kind == VOp::GEMM ? conv_op_of(op.conv, ChainDesc{}, op.gemm) : cc_conv_op{};
-  snprintf(out->name, sizeof(out->name), "%s", op.name);
-  return n;
+  return op_conv_tap("cc_clip_op_conv", P->ops, i, out);
 }
 
 int cc_clip_run_ops(cc_clip* h, int text, const void* d_in, int B, int first, int last, float* d_out, long long out_row_stride,
@@ -357,10 +320,9 @@ int cc_clip_run_ops(cc_clip* h, int text, const void* d_in, int B, int first, in
   CC_REQUIRE(h && d_in && d_out && B > 0, "cc_clip_run_ops: bad argument");
   ClipPlan* P = nullptr;
   if (int rc = clip_plan(h, text != 0, B, &P)) return rc;
-  const int n = static_cast<int>(P->ops.size());
-  CC_REQUIRE(0 <= first && first <= last && last <= n, "cc_clip_run_ops: ops [%d, %d) of a plan of %d ops", first, last, n);
-  return run_plan(*P, d_in, d_out, out_row_stride > 0 ? out_row_stride : h->m.cfg.embed_dim, static_cast<cudaStream_t>(stream),
-                  first, last);
+  if (int rc = check_range("cc_clip_run_ops", first, last, static_cast<int>(P->ops.size()))) return rc;
+  return run_ops(P->ops, PlanIO{d_in, d_out, out_row_stride > 0 ? out_row_stride : h->m.cfg.embed_dim}, static_cast<cudaStream_t>(stream),
+                 first, last);
 }
 
 int cc_search_scores(const float* d_index, int N, int D, const float* d_q, int Q, float* d_scores, void* stream) {

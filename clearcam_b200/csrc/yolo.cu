@@ -17,6 +17,7 @@
 #include "cc_common.h"
 #include "conv_gemm.cuh"
 #include "ops.cuh"
+#include "plan.h"
 #include <cmath>
 
 namespace cc {
@@ -249,24 +250,6 @@ static int require_net(const LbGeom& g, int Hf, int Wf, int res) {
 // A tensor of the plan: a slice, or the input frames (`image`, no buffer of the plan's own)
 struct T : TSlice { bool image = false; T() : TSlice{} {} };
 
-struct Op {
-  enum Kind { GEMM, DIRECT, AVGPAD, AVGMAX, MAXPOOL5, UPSAMPLE, CBFUSE, LETTERBOX, STEM, STEM_TC, DECODE, POST, SPLIT, FINISH, SPP3 } kind;
-  GemmLaunch gemm;
-  ConvDesc conv{};           // GEMM: the conv its launch was built from (cc_yolo_op_conv reports it; the launch never reads it)
-  ChainDesc chain{};         //   ... and the 1x1 chained in its epilogue (chain.out.p != nullptr)
-  DirectConvParams direct;
-  TSlice s_in, s_out;
-  CBFuseParams cbf;
-  LetterboxParams lb;
-  StemParams stem;
-  StemTcParams stem_tc;
-  FinishParams fin;
-  double flops = 0;          // algorithmic FLOPs of a non-GEMM conv op (stem)
-  DecodeParams dec;
-  PostParams post;
-  std::string name;
-};
-
 struct YoloPlan {
   int B = 0, Hf = 0, Wf = 0, res = 0, fmt = 0, H = 0, W = 0, A = 0;    // fmt: CC_FRAME_* of the frames
   int Hr = 0, Wr = 0;          // the reference's letterboxed extent (H, W are it rounded up to a multiple of 32)
@@ -274,7 +257,8 @@ struct YoloPlan {
   // has no letterbox (launched by the caller with the call's table into lb_out) and ends with the postprocess (launched with
   // the call's per-image scales); in between it is the op list of a uniform plan of the net shape.
   bool table = false;
-  std::vector<Op> ops;
+  std::vector<PlanOp> ops;
+  PostParams post{};          // the postprocess op's parameters (a frame-table call launches it with per-image scales)
   size_t alloc_bytes = 0;      // bytes of the handle's shared workspace this plan addresses
   float* pred = nullptr;   // [B,A,6]
   float* raw = nullptr;    // [B,84,A] (allocated lazily when a tap is requested)
@@ -380,6 +364,8 @@ struct YoloModel {
 };
 
 static bool tc_ok(int cin, int cout) { return cin % 16 == 0 && cout % 16 == 0; }
+// algorithmic HBM bytes of a slice, for the bytes a memory-bound op reports (inputs once + outputs once)
+static double slice_bytes(const TSlice& t) { return double(t.N) * t.H * t.W * t.C * (t.f32 ? 4 : 2); }
 
 // The fp32-accurate conv as ops, shared by the plan builder and cc_conv2d_fp32_accurate: fp32 slice -> six bf16 planes
 // [lo|mid|hi|mid|hi|hi] in `scratch`; then on the same wgmma conv kernel, all with fp32 output into the dense partial-sum buffer
@@ -387,9 +373,10 @@ static bool tc_ok(int cin, int cout) { return cin % 16 == 0 && cout % 16 == 0; }
 // in-place fp32 residual of the epilogue (one round-to-nearest add), one GEMM for the five cross products (planes 0..4 against
 // the weight planes hi|mid|lo|hi|mid); a last pass applies bias, the exact SiLU and the residual and writes the output slice.
 static int precise_conv_ops(const std::string& key, const ConvW& cw, const TSlice& in, int stride, int act, __nv_bfloat16* scratch,
-                            float* accbuf, const TSlice& out, const TSlice* res, int sms, std::vector<Op>* ops, double* conv_flops) {
-  Op sp; sp.kind = Op::SPLIT; sp.name = key + ".split"; sp.s_in = in; sp.s_out = TSlice{}; sp.s_out.p = scratch;
-  ops->push_back(std::move(sp));
+                            float* accbuf, const TSlice& out, const TSlice* res, int sms, std::vector<PlanOp>* ops, double* conv_flops) {
+  ops->push_back(plan_op(key + ".split", "split_planes", [in, scratch](const PlanIO&, cudaStream_t st) {
+    return split_planes_launch(in, scratch, st);
+  }));
   const int Ho = conv_out(in.H, stride), Wo = conv_out(in.W, stride);
   const int nseg = static_cast<int>(cw.seg_off.size());
   const TSlice acc = dense_f32(accbuf, cw.cout);
@@ -397,20 +384,17 @@ static int precise_conv_ops(const std::string& key, const ConvW& cw, const TSlic
     const TSlice planes = g < nseg ? nhwc_slice(scratch, 6 * in.C, 5 * in.C + cw.seg_off[g], cw.seg_c[g], 0, in.N, in.H, in.W)
                                    : nhwc_slice(scratch, 6 * in.C, 0, 5 * in.C, 0, in.N, in.H, in.W);
     const ConvDesc d = conv_desc(planes, g < nseg ? cw.whi[g] : cw.w5, nullptr, cw.k, stride, acc, CC_ACT_NONE, g > 0 ? &acc : nullptr);
-    Op gop; gop.kind = Op::GEMM; gop.name = key + (g < nseg ? ".hi" + std::to_string(g) : ".cross");
-    gop.conv = d;
-    if (int rc = conv_gemm_build(d, sms, &gop.gemm)) return rc;
-    gop.gemm.flops = g == 0 ? 2.0 * in.N * Ho * Wo * double(cw.cout) * cw.k * cw.k * cw.cin : 0.0;   // algorithmic FLOPs once
-    *conv_flops += gop.gemm.flops;
-    ops->push_back(std::move(gop));
+    GemmLaunch L;
+    if (int rc = conv_gemm_build(d, sms, &L)) return rc;
+    L.flops = g == 0 ? 2.0 * in.N * Ho * Wo * double(cw.cout) * cw.k * cw.k * cw.cin : 0.0;   // algorithmic FLOPs once
+    *conv_flops += L.flops;
+    ops->push_back(gemm_op(key + (g < nseg ? ".hi" + std::to_string(g) : ".cross"), d, ChainDesc{}, L));
   }
-  Op op; op.kind = Op::FINISH; op.name = key;
-  FinishParams& f = op.fin;
-  f = FinishParams{};
+  FinishParams f{};
   f.acc = accbuf; f.bias = cw.bias; f.act = act; f.npix = static_cast<long long>(in.N) * Ho * Wo; f.C = cw.cout;
   f.out = reinterpret_cast<float*>(out.p); f.out_cs = out.cs; f.out_co = out.co;
   if (res) { f.res = reinterpret_cast<const float*>(res->p); f.res_cs = res->cs; f.res_co = res->co; }
-  ops->push_back(std::move(op));
+  ops->push_back(plan_op(key, "finish_f32", [f](const PlanIO&, cudaStream_t st) { return finish_f32_launch(f, st); }));
   return CC_OK;
 }
 // The two first convs of a detect-head scale read the same input and are fused into one conv of 64 + d output channels —
@@ -487,20 +471,19 @@ struct Builder {
     }
     ConvDesc d = conv_desc(in, cw.w, cw.bias, cw.k, stride, out, act, res);
     d.pre = pre; d.pre_h = pre_h; d.pre_w = pre_w;
-    Op op;
-    op.name = key;
     if (cw.groups == 1 && tc_ok(cw.cin, cw.cout)) {
-      op.kind = Op::GEMM;
-      op.conv = d;
-      rc = conv_gemm_build(d, M.sms, &op.gemm);
+      GemmLaunch L;
+      rc = conv_gemm_build(d, M.sms, &L);
       if (rc) return;
-      P.conv_flops += op.gemm.flops;
-    } else {
-      op.kind = Op::DIRECT;
-      op.direct = direct_conv_params(d, cw.groups);
-      P.conv_flops += 2.0 * P.B * op.direct.Hout * op.direct.Wout * cw.cout * (cw.cin / cw.groups) * cw.k * cw.k;
+      P.conv_flops += L.flops;
+      P.ops.push_back(gemm_op(key, d, ChainDesc{}, L));
+    } else {   // the direct kernel's FLOPs count in conv_flops; its op reports none
+      const DirectConvParams p = direct_conv_params(d, cw.groups);
+      P.conv_flops += 2.0 * P.B * p.Hout * p.Wout * cw.cout * (cw.cin / cw.groups) * cw.k * cw.k;
+      PlanOp op = plan_op(key, "conv_direct", [p](const PlanIO&, cudaStream_t st) { return conv_direct_launch(p, st); });
+      op.conv = conv_op_of(p);
+      P.ops.push_back(std::move(op));
     }
-    P.ops.push_back(std::move(op));
   }
   // conv key1 (in -> out1) followed by the 1x1 conv key2 over in2, a slice of out1's buffer that starts inside out1 and may
   // run past its end (the partner: channels another conv wrote), into out2 (a tensor or a dense fp32 map).  One chained
@@ -523,14 +506,10 @@ struct Builder {
         if (part_c > 0) c.part = nhwc_slice(in2.p, in2.cs, out1.co + out1.C, part_c);
         c.out = out2;
         c.store1 = keep1;
-        Op op;
-        op.kind = Op::GEMM;
-        op.name = key1 + "+" + key2;
-        op.conv = d;
-        op.chain = c;
-        if (conv_gemm_chain_build(d, c, M.sms, &op.gemm) == CC_OK) {
-          P.conv_flops += op.gemm.flops;
-          P.ops.push_back(std::move(op));
+        GemmLaunch L;
+        if (conv_gemm_chain_build(d, c, M.sms, &L) == CC_OK) {
+          P.conv_flops += L.flops;
+          P.ops.push_back(gemm_op(key1 + "+" + key2, d, c, L));
           return true;
         }
       }
@@ -539,10 +518,12 @@ struct Builder {
     conv(key2, in2, out2, 1, act2);
     return false;
   }
-  void simple(Op::Kind kind, const T& in, const T& out, const char* name) {
+  // a pool or upsample kernel from slice `in` to slice `out`
+  void simple(const char* kind, int (*launch)(const TSlice&, const TSlice&, cudaStream_t), const TSlice& in, const TSlice& out,
+              const char* name) {
     if (rc || bump.dry) return;
-    Op op; op.kind = kind; op.s_in = in; op.s_out = out; op.name = name;
-    P.ops.push_back(std::move(op));
+    P.ops.push_back(plan_op(name, kind, [launch, in, out](const PlanIO&, cudaStream_t st) { return launch(in, out, st); }, 0,
+                            slice_bytes(in) + slice_bytes(out)));
   }
 
   // destination of layer i's output: a slice of a later concat buffer, or a fresh buffer
@@ -659,13 +640,18 @@ int Builder::build() {
     P.lb_out = dalloc(static_cast<size_t>(P.B) * P.H * P.W * 3 * es);
     net_in = P.lb_out;
     if (!bump.dry && !P.table) {
-    Op op; op.kind = Op::LETTERBOX; op.name = "letterbox";
-    op.lb = LetterboxParams{};
-    op.lb.in = nullptr; op.lb.out = P.lb_out; op.lb.fmt = P.fmt;
-    op.lb.B = P.B; op.lb.Hin = P.Hf; op.lb.Win = P.Wf; op.lb.Hr = g.new_h; op.lb.Wr = g.new_w;
-    op.lb.pad_y = g.py; op.lb.pad_x = g.px; op.lb.Hout = P.H; op.lb.Wout = P.W;
-    op.lb.sx = g.sx; op.lb.sy = g.sy;
-    P.ops.push_back(std::move(op));
+      LetterboxParams lb{};
+      lb.in = nullptr; lb.out = P.lb_out; lb.fmt = P.fmt;
+      lb.B = P.B; lb.Hin = P.Hf; lb.Win = P.Wf; lb.Hr = g.new_h; lb.Wr = g.new_w;
+      lb.pad_y = g.py; lb.pad_x = g.px; lb.Hout = P.H; lb.Wout = P.W;
+      lb.sx = g.sx; lb.sy = g.sy;
+      const double in_px = lb.fmt == CC_FRAME_BGR_F32 ? 12.0 : lb.fmt == CC_FRAME_I420_U8 ? 1.5 : 3.0;   // bytes per pixel
+      const double bytes = double(lb.B) * (double(lb.Hin) * lb.Win * in_px + double(lb.Hout) * lb.Wout * 3 * (lb.fmt == CC_FRAME_BGR_F32 ? 4 : 1));
+      P.ops.push_back(plan_op("letterbox", "letterbox", [lb](const PlanIO& io, cudaStream_t st) {
+        LetterboxParams q = lb;
+        q.in = io.in;
+        return letterbox_launch(q, st);
+      }, 0, bytes));
     }
   }
 
@@ -694,20 +680,26 @@ int Builder::build() {
           if (!f32 && !M.precise && (cw.cout == 16 || cw.cout == 32 || cw.cout == 64)) {
             // uint8 frames: raw pixel values are exact in bf16, weights bf16(w/255); stem_tc_kernel gathers the A tile from
             // the frame itself
-            Op op; op.kind = Op::STEM_TC; op.name = pfx; op.stem = StemParams{}; op.stem.in = net_in;
-            rc = stem_tc_build(P.B, P.H, P.W, cw.wtc, cw.bias, cw.cout, out, &op.stem_tc);
+            StemTcParams tc;
+            rc = stem_tc_build(P.B, P.H, P.W, cw.wtc, cw.bias, cw.cout, out, &tc);
             if (rc) break;
-            op.flops = 2.0 * P.B * (P.H / 2) * (P.W / 2) * cw.cout * 27;
-            P.conv_flops += op.flops;
-            P.ops.push_back(std::move(op));
+            const double flops = 2.0 * P.B * (P.H / 2) * (P.W / 2) * cw.cout * 27;
+            P.conv_flops += flops;
+            P.ops.push_back(plan_op(pfx, "stem_tc", [tc, net_in](const PlanIO& io, cudaStream_t st) {
+              return stem_tc_launch(tc, static_cast<const uint8_t*>(net_in ? net_in : io.in), st);
+            }, flops, double(tc.B) * tc.H * tc.W * 3 + double(tc.Mrows) * tc.Cout * 2));
             break;
           }
-          Op op; op.kind = Op::STEM; op.name = pfx;
-          op.stem = StemParams{};
-          op.stem.in = net_in; op.stem.is_f32 = f32; op.stem.B = P.B; op.stem.H = P.H; op.stem.W = P.W;
-          op.stem.w = cw.wf32; op.stem.bias = cw.bias; op.stem.Cout = cw.cout; op.stem.out = out;
+          // the CUDA-core stem's FLOPs count in conv_flops; its op reports none
+          StemParams sp{};
+          sp.in = net_in; sp.is_f32 = f32; sp.B = P.B; sp.H = P.H; sp.W = P.W;
+          sp.w = cw.wf32; sp.bias = cw.bias; sp.Cout = cw.cout; sp.out = out;
           P.conv_flops += 2.0 * P.B * (P.H / 2) * (P.W / 2) * cw.cout * 27;
-          P.ops.push_back(std::move(op));
+          P.ops.push_back(plan_op(pfx, "stem", [sp](const PlanIO& io, cudaStream_t st) {
+            StemParams q = sp;
+            if (!q.in) q.in = io.in;
+            return stem_launch(q, st);
+          }));
         } else {
           out = out_for(i, l.b, conv_out(in.H, l.s), conv_out(in.W, l.s));
           if (!place.count(i) && conv_feeds_only_elan(S, outC, i, M.precise)) deferred = {pfx, in, out, l.s, i};
@@ -740,12 +732,12 @@ int Builder::build() {
           if (!rc && !bump.dry && P.ops.size() >= 2) {
             // algorithmic FLOPs: the pair replaces ONE 1x1 conv over all input channels at full resolution (what the reference
             // computes and SURVEY 8(d) counts); booked on the full-resolution launch, the half-resolution one carries none
-            GemmLaunch& g_hi = P.ops[P.ops.size() - 1].gemm;
-            GemmLaunch& g_lo = P.ops[P.ops.size() - 2].gemm;
+            PlanOp& op_hi = P.ops[P.ops.size() - 1];
+            PlanOp& op_lo = P.ops[P.ops.size() - 2];
             const double full = 2.0 * P.B * in.H * in.W * double(4 * b) * in.C;
-            P.conv_flops += full - g_hi.flops - g_lo.flops;
-            g_hi.flops = full;
-            g_lo.flops = 0.0;
+            P.conv_flops += full - op_hi.flops - op_lo.flops;
+            op_hi.flops = full;
+            op_lo.flops = 0.0;
           }
           conv(pfx + ".cv2.0.cv1+cv2", slice(cat, 2 * b, 2 * b), t1, 1, CC_ACT_SILU);
         } else if (deferred.layer == i - 1) {   // the previous Conv with cv1 chained in its epilogue; its output is not stored
@@ -774,18 +766,18 @@ int Builder::build() {
         const int ch = l.a;
         CC_REQUIRE(in.C == 2 * ch, "yolo: ADown(%d) fed %d channels", ch, in.C);
         T t1 = talloc(ch, in.H, in.W);
-        simple(Op::AVGPAD, slice(in, 0, ch), t1, "adown.avg");
+        simple("avgpool2_pad", avgpool2_pad_launch, slice(in, 0, ch), t1, "adown.avg");
         out = out_for(i, 2 * ch, in.H / 2, in.W / 2);
         conv(pfx + ".cv1", t1, slice(out, 0, ch), 2, CC_ACT_SILU);
         T t2 = talloc(ch, in.H / 2, in.W / 2);
-        simple(Op::AVGMAX, slice(in, ch, ch), t2, "adown.avgmax");
+        simple("avgmax_pool", avgmax_pool_launch, slice(in, ch, ch), t2, "adown.avgmax");
         conv(pfx + ".cv2", t2, slice(out, ch, ch), 1, CC_ACT_SILU);
         break;
       }
       case L_ACONV: {
         // detection/yolov9.py:54-63
         T t1 = talloc(in.C, in.H, in.W);
-        simple(Op::AVGPAD, in, t1, "aconv.avg");
+        simple("avgpool2_pad", avgpool2_pad_launch, in, t1, "aconv.avg");
         out = out_for(i, l.b, in.H / 2, in.W / 2);
         conv(pfx + ".cv1", t1, out, 2, CC_ACT_SILU);
         break;
@@ -796,9 +788,11 @@ int Builder::build() {
         T cat = talloc(4 * c1, in.H, in.W);
         conv(pfx + ".cv1", in, slice(cat, 0, c1), 1, CC_ACT_SILU);
         if (spp3_supported(cat, c1)) {
-          if (!rc && !bump.dry) { Op op; op.kind = Op::SPP3; op.s_in = cat; op.s_out = cat; op.s_out.C = c1; op.name = "spp.max5x3"; P.ops.push_back(std::move(op)); }
+          if (!rc && !bump.dry)
+            P.ops.push_back(plan_op("spp.max5x3", "spp3", [cat, c1](const PlanIO&, cudaStream_t st) { return spp3_launch(cat, c1, st); }, 0,
+                                    4.0 * cat.N * cat.H * cat.W * c1 * 2));
         } else {
-          for (int q = 0; q < 3; ++q) simple(Op::MAXPOOL5, slice(cat, q * c1, c1), slice(cat, (q + 1) * c1, c1), "spp.max5");
+          for (int q = 0; q < 3; ++q) simple("maxpool5", maxpool5_launch, slice(cat, q * c1, c1), slice(cat, (q + 1) * c1, c1), "spp.max5");
         }
         out = out_for(i, l.c, in.H, in.W);
         conv(pfx + ".cv5", cat, out, 1, CC_ACT_SILU);
@@ -810,7 +804,7 @@ int Builder::build() {
           break;
         }
         out = out_for(i, in.C, in.H * 2, in.W * 2);
-        simple(Op::UPSAMPLE, in, out, "upsample");
+        simple("upsample2", upsample2_launch, in, out, "upsample");
         break;
       }
       case L_CONCAT: {
@@ -838,23 +832,23 @@ int Builder::build() {
         const T& last = src(l.f.back());
         out = out_for(i, last.C, last.H, last.W);
         if (bump.dry) break;
-        Op op; op.kind = Op::CBFUSE; op.name = pfx;
-        op.cbf = CBFuseParams{};
-        op.cbf.nsrc = static_cast<int>(l.f.size()) - 1;
-        for (int q = 0; q < op.cbf.nsrc; ++q) {
+        CBFuseParams cbf{};
+        cbf.nsrc = static_cast<int>(l.f.size()) - 1;
+        for (int q = 0; q < cbf.nsrc; ++q) {
           const T& ch = cbl_chunks[l.f[q]][l.list[q]];
           CC_REQUIRE(ch.C == last.C, "yolo: CBFuse chunk has %d channels, target %d", ch.C, last.C);
-          op.cbf.src[q] = ch;
+          cbf.src[q] = ch;
         }
-        op.cbf.last = last; op.cbf.out = out;
-        P.ops.push_back(std::move(op));
+        cbf.last = last; cbf.out = out;
+        double bytes = slice_bytes(cbf.last) + slice_bytes(cbf.out);
+        for (int q = 0; q < cbf.nsrc; ++q) bytes += slice_bytes(cbf.src[q]);
+        P.ops.push_back(plan_op(pfx, "cbfuse", [cbf](const PlanIO&, cudaStream_t st) { return cbfuse_launch(cbf, st); }, 0, bytes));
         break;
       }
       case L_DETECT: {
         // detection/yolov9.py:157-220 + postprocess :439-458 + scale_boxes :406-421
         const int d = l.a;
-        Op dec; dec.kind = Op::DECODE; dec.name = "decode";
-        dec.dec = DecodeParams{};
+        DecodeParams dec{};
         int A = 0;
         for (int q = 0; q < 3; ++q) {
           const T& x = src(l.f[q]);
@@ -874,21 +868,29 @@ int Builder::build() {
           conv_pair(hp + ".cv2." + sq + ".1", slice(t0, 0, 64), tb, 1, nullptr, hp + ".cv2." + sq + ".2", tb, dense_f32(bl, 64), CC_ACT_NONE, false);
           conv(hp + ".cv3." + sq + ".1", slice(t0, 64, d), tc, 1, CC_ACT_SILU);
           conv(hp + ".cv3." + sq + ".2", tc, dense_f32(cl, 80), 1, CC_ACT_NONE);
-          dec.dec.box[q] = bl; dec.dec.cls[q] = cl; dec.dec.h[q] = x.H; dec.dec.w[q] = x.W;
-          dec.dec.stride[q] = float(P.H / x.H);
+          dec.box[q] = bl; dec.cls[q] = cl; dec.h[q] = x.H; dec.w[q] = x.W;
+          dec.stride[q] = float(P.H / x.H);
           A += x.H * x.W;
         }
         P.A = A;
         P.pred = static_cast<float*>(dalloc(static_cast<size_t>(P.B) * A * 6 * 4));
-        dec.dec.B = P.B; dec.dec.A = A; dec.dec.conf_thr = 0.25f; dec.dec.pred = P.pred; dec.dec.raw = nullptr;
+        dec.B = P.B; dec.A = A; dec.conf_thr = 0.25f; dec.pred = P.pred; dec.raw = nullptr;
         if (bump.dry) break;
-        P.ops.push_back(std::move(dec));
-        Op po; po.kind = Op::POST; po.name = "postprocess";
-        po.post = PostParams{};
-        po.post.pred = P.pred; po.post.B = P.B; po.post.A = A; po.post.max_det = 300; po.post.iou_thr = 0.45f;
-        po.post.scale = g.scale; po.post.do_scale = 1;
-        po.post.out = nullptr;
-        P.ops.push_back(std::move(po));
+        P.ops.push_back(plan_op("decode", "decode", [dec](const PlanIO& io, cudaStream_t st) {
+          DecodeParams q = dec;
+          q.raw = io.raw;
+          return decode_launch(q, st);
+        }, 0, double(dec.B) * dec.A * ((64 + 80) * 4 + 6 * 4)));
+        PostParams& post = P.post;
+        post = PostParams{};
+        post.pred = P.pred; post.B = P.B; post.A = A; post.max_det = 300; post.iou_thr = 0.45f;
+        post.scale = g.scale; post.do_scale = 1;
+        post.out = nullptr;
+        P.ops.push_back(plan_op("postprocess", "postprocess", [post](const PlanIO& io, cudaStream_t st) {
+          PostParams q = post;
+          q.out = io.out;
+          return postprocess_launch(q, st);
+        }));
         break;
       }
     }
@@ -898,72 +900,6 @@ int Builder::build() {
   P.layer_outs = outs;
   for (int f : folded) P.layer_outs[f].p = nullptr;   // reported as a folded layer (a shape, no tensor)
   return rc;
-}
-
-// ops [first, last) of the plan (all of them by default)
-static int plan_run(YoloPlan& P, const void* d_frames, float* d_out, float* d_raw, cudaStream_t st,
-                    std::vector<cudaEvent_t>* ev = nullptr, unsigned long long* d_trace = nullptr, size_t first = 0,
-                    size_t last = SIZE_MAX) {
-  size_t oi = 0, ti = 0;
-  if (last > P.ops.size()) last = P.ops.size();
-  for (size_t k = first; k < last; ++k) {
-    Op& op = P.ops[k];
-    int rc = CC_OK;
-    if (ev) cudaEventRecord((*ev)[oi++], st);
-    switch (op.kind) {
-      case Op::GEMM:
-        if (d_trace) { GemmLaunch g = op.gemm; g.p.trace = d_trace + 12 * ti; rc = conv_gemm_launch(g, st); }
-        else rc = conv_gemm_launch(op.gemm, st);
-        break;
-      case Op::DIRECT: rc = conv_direct_launch(op.direct, st); break;
-      case Op::AVGPAD: rc = avgpool2_pad_launch(op.s_in, op.s_out, st); break;
-      case Op::AVGMAX: rc = avgmax_pool_launch(op.s_in, op.s_out, st); break;
-      case Op::MAXPOOL5: rc = maxpool5_launch(op.s_in, op.s_out, st); break;
-      case Op::UPSAMPLE: rc = upsample2_launch(op.s_in, op.s_out, st); break;
-      case Op::SPP3: rc = spp3_launch(op.s_in, op.s_out.C, st); break;
-      case Op::CBFUSE: rc = cbfuse_launch(op.cbf, st); break;
-      case Op::LETTERBOX: { LetterboxParams q = op.lb; q.in = d_frames; rc = letterbox_launch(q, st); break; }
-      case Op::STEM: { StemParams q = op.stem; if (!q.in) q.in = d_frames; rc = stem_launch(q, st); break; }
-      case Op::STEM_TC:
-        rc = stem_tc_launch(op.stem_tc, static_cast<const uint8_t*>(op.stem.in ? op.stem.in : d_frames), st);
-        break;
-      case Op::DECODE: { DecodeParams q = op.dec; q.raw = d_raw; rc = decode_launch(q, st); break; }
-      case Op::POST: { PostParams q = op.post; q.out = d_out; rc = postprocess_launch(q, st); break; }
-      case Op::SPLIT: rc = split_planes_launch(op.s_in, op.s_out.p, st); break;
-      case Op::FINISH: rc = finish_f32_launch(op.fin, st); break;
-    }
-    if (rc) return rc;
-    ++ti;
-  }
-  if (ev) cudaEventRecord((*ev)[oi], st);
-  return CC_OK;
-}
-
-// algorithmic HBM bytes of a memory-bound op (inputs once + outputs once), for the achieved-GB/s figures of the bench line
-static double op_bytes(const Op& op) {
-  auto sl = [](const TSlice& t) { return double(t.N) * t.H * t.W * t.C * (t.f32 ? 4 : 2); };
-  switch (op.kind) {
-    case Op::AVGPAD: case Op::AVGMAX: case Op::MAXPOOL5: case Op::UPSAMPLE: return sl(op.s_in) + sl(op.s_out);
-    case Op::SPP3: return 4.0 * op.s_in.N * op.s_in.H * op.s_in.W * op.s_out.C * 2;
-    case Op::CBFUSE: { double b = sl(op.cbf.last) + sl(op.cbf.out); for (int k = 0; k < op.cbf.nsrc; ++k) b += sl(op.cbf.src[k]); return b; }
-    case Op::STEM_TC: return double(op.stem_tc.B) * op.stem_tc.H * op.stem_tc.W * 3 + double(op.stem_tc.Mrows) * op.stem_tc.Cout * 2;
-    case Op::LETTERBOX: {
-      const double in_px = op.lb.fmt == CC_FRAME_BGR_F32 ? 12.0 : op.lb.fmt == CC_FRAME_I420_U8 ? 1.5 : 3.0;   // bytes per pixel
-      return double(op.lb.B) * (double(op.lb.Hin) * op.lb.Win * in_px + double(op.lb.Hout) * op.lb.Wout * 3 * (op.lb.fmt == CC_FRAME_BGR_F32 ? 4 : 1));
-    }
-    case Op::DECODE: return double(op.dec.B) * op.dec.A * ((64 + 80) * 4 + 6 * 4);
-    default: return 0.0;
-  }
-}
-
-static const char* op_kind_name(Op::Kind k) {
-  switch (k) {
-    case Op::GEMM: return "conv_gemm"; case Op::DIRECT: return "conv_direct"; case Op::AVGPAD: return "avgpool2_pad";
-    case Op::AVGMAX: return "avgmax_pool"; case Op::MAXPOOL5: return "maxpool5"; case Op::UPSAMPLE: return "upsample2";
-    case Op::CBFUSE: return "cbfuse"; case Op::LETTERBOX: return "letterbox"; case Op::STEM: return "stem"; case Op::STEM_TC: return "stem_tc";
-    case Op::DECODE: return "decode"; case Op::POST: return "postprocess"; case Op::SPLIT: return "split_planes"; case Op::FINISH: return "finish_f32"; case Op::SPP3: return "spp3";
-  }
-  return "?";
 }
 
 }  // namespace cc
@@ -1139,6 +1075,13 @@ int cc_yolo_set_workspace(cc_yolo* h, void* d_workspace, size_t bytes) {
   return h->m.plans.adopt(d_workspace, bytes);
 }
 
+// What a detector call supplies to its plan's ops
+static PlanIO frames_io(const void* d_frames, float* d_out, float* d_raw) {
+  PlanIO io;
+  io.in = d_frames; io.out = d_out; io.raw = d_raw;
+  return io;
+}
+
 // Runs ops [first, last) of the plan on `st`: from its CUDA graph once the caller has passed the same (frames, out, raw)
 // pointers twice in a row, else launch by launch.
 static int run_graphed(cc_yolo* h, YoloPlan* P, const void* d_frames, float* d_out, float* d_raw, cudaStream_t st, size_t first = 0,
@@ -1149,6 +1092,7 @@ static int run_graphed(cc_yolo* h, YoloPlan* P, const void* d_frames, float* d_o
   }
   const bool stable = P->ran && P->l_frames == d_frames && P->l_out == d_out && P->l_raw == d_raw;
   P->l_frames = d_frames; P->l_out = d_out; P->l_raw = d_raw; P->ran = true;
+  const PlanIO io = frames_io(d_frames, d_out, d_raw);
   if (stable) {
     // second call in a row with these pointers: capture the launch list (on a private stream: nothing executes) and replay
     if (!h->m.cap_stream) CC_CHECK_CUDA(cudaStreamCreateWithFlags(&h->m.cap_stream, cudaStreamNonBlocking));
@@ -1156,7 +1100,7 @@ static int run_graphed(cc_yolo* h, YoloPlan* P, const void* d_frames, float* d_o
     cudaGraph_t g = nullptr;
     bool ok = cudaStreamBeginCapture(h->m.cap_stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
     if (ok) {
-      const int rc = plan_run(*P, d_frames, d_out, d_raw, h->m.cap_stream, nullptr, nullptr, first, last);
+      const int rc = run_ops(P->ops, io, h->m.cap_stream, first, last);
       ok = cudaStreamEndCapture(h->m.cap_stream, &g) == cudaSuccess && rc == CC_OK && g != nullptr;
     }
     if (ok) ok = cudaGraphInstantiate(&P->gexec, g, 0) == cudaSuccess;
@@ -1169,7 +1113,7 @@ static int run_graphed(cc_yolo* h, YoloPlan* P, const void* d_frames, float* d_o
     cudaGetLastError();            // capture is an optimisation: fall through to plain launches
     P->gexec = nullptr;
   }
-  return plan_run(*P, d_frames, d_out, d_raw, st, nullptr, nullptr, first, last);
+  return run_ops(P->ops, io, st, first, last);
 }
 
 int cc_yolo_forward(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, float* d_out,
@@ -1243,7 +1187,7 @@ int cc_yolo_forward_frames(cc_yolo* h, const cc_frame* frames, int B, int res, f
   if (int rc = table_geometry("cc_yolo_forward_frames", frames, B, res, &geo, &H, &W)) return rc;
   YoloPlan* P = nullptr;
   if (int rc = get_plan(h, CC_FRAME_BGR_U8, B, H, W, res, &P, true)) return rc;
-  CC_REQUIRE(!P->ops.empty() && P->ops.back().kind == Op::POST && P->lb_out, "cc_yolo_forward_frames: plan without postprocess");
+  CC_REQUIRE(!P->ops.empty() && P->post.pred && P->lb_out, "cc_yolo_forward_frames: plan without postprocess");
   LetterboxTable t;
   table_letterbox(frames, B, geo, H, W, P->lb_out, &t);
   std::vector<PostScale> scales(B);
@@ -1255,7 +1199,7 @@ int cc_yolo_forward_frames(cc_yolo* h, const cc_frame* frames, int B, int res, f
   // the workspace (and d_raw), so their graph does not depend on the table
   if (int rc = letterbox_frames_launch(t, st)) return rc;
   if (int rc = run_graphed(h, P, nullptr, nullptr, d_raw, st, 0, P->ops.size() - 1)) return rc;
-  PostParams q = P->ops.back().post;
+  PostParams q = P->post;
   q.out = d_out;
   return postprocess_launch(q, st, scales.data());
 }
@@ -1278,7 +1222,7 @@ int cc_yolo_plan_info(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res,
 
 /* Per-op device timing of one forward (CUDA events between launches on `stream`; synchronises at the end).
  * Fills up to `cap` entries: ms[i], flops[i] (algorithmic, 0 for non-conv ops) and a name pointer valid for the
- * life of the handle.  Returns the op count through n_ops. */
+ * life of the process.  Returns the op count through n_ops. */
 int cc_yolo_profile(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, float* d_out, int cap,
                     float* ms, double* flops, double* bytes, const char** kinds, const char** names, int* n_ops, void* stream) {
   CC_REQUIRE(h && d_frames && d_out, "cc_yolo_profile: bad argument");
@@ -1286,25 +1230,8 @@ int cc_yolo_profile(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int 
   if (int rc = check_frame_fmt("cc_yolo_profile", frame_fmt, Hf, Wf)) return rc;
   int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P);
   if (rc) return rc;
-  const size_t n = P->ops.size();
-  std::vector<cudaEvent_t> ev(n + 1);
-  for (auto& e : ev) CC_CHECK_CUDA(cudaEventCreate(&e));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  rc = plan_run(*P, d_frames, d_out, nullptr, st, &ev);
-  if (!rc) {
-    CC_CHECK_CUDA(cudaStreamSynchronize(st));
-    for (size_t i = 0; i < n && static_cast<int>(i) < cap; ++i) {
-      float t = 0.f;
-      cudaEventElapsedTime(&t, ev[i], ev[i + 1]);
-      if (ms) ms[i] = t;
-      if (flops) flops[i] = P->ops[i].kind == Op::GEMM ? P->ops[i].gemm.flops : P->ops[i].flops;
-      if (bytes) bytes[i] = P->ops[i].kind == Op::GEMM ? P->ops[i].gemm.bytes : op_bytes(P->ops[i]);
-      if (kinds) kinds[i] = op_kind_name(P->ops[i].kind);
-      if (names) names[i] = P->ops[i].name.c_str();
-    }
-  }
-  for (auto& e : ev) cudaEventDestroy(e);
-  if (n_ops) *n_ops = static_cast<int>(n);
+  rc = profile_ops(P->ops, frames_io(d_frames, d_out, nullptr), static_cast<cudaStream_t>(stream), cap, ms, flops, bytes, kinds, names);
+  if (n_ops) *n_ops = static_cast<int>(P->ops.size());
   return rc;
 }
 
@@ -1324,16 +1251,20 @@ int cc_yolo_trace(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf
   CC_CHECK_CUDA(cudaMalloc(&d_trace, n * 12 * sizeof(unsigned long long)));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   cudaMemsetAsync(d_trace, 0, n * 12 * sizeof(unsigned long long), st);
-  rc = plan_run(*P, d_frames, d_out, nullptr, st, nullptr, d_trace);
+  PlanIO io = frames_io(d_frames, d_out, nullptr);
+  io.trace = d_trace;
+  rc = run_ops(P->ops, io, st);
   if (!rc) {
     cudaError_t e = cudaStreamSynchronize(st);
     if (e == cudaSuccess) {
       const size_t m = n < static_cast<size_t>(cap) ? n : static_cast<size_t>(cap);
       e = cudaMemcpy(host_ns, d_trace, m * 12 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
       for (size_t i = 0; i < m; ++i) {
-        if (kinds) kinds[i] = op_kind_name(P->ops[i].kind);
-        if (names) names[i] = P->ops[i].name.c_str();
-        if (flops) flops[i] = P->ops[i].kind == Op::GEMM ? P->ops[i].gemm.flops : 0.0;
+        const PlanOp& op = P->ops[i];
+        const bool gemm = op.conv.kind == CC_CONV_OP_GEMM || op.conv.kind == CC_CONV_OP_CHAIN;
+        if (kinds) kinds[i] = op.kind;
+        if (names) names[i] = op.name;
+        if (flops) flops[i] = gemm ? op.flops : 0.0;
       }
     }
     if (e != cudaSuccess) { set_error("cc_yolo_trace: %s", cudaGetErrorString(e)); rc = CC_ERR_CUDA; }
@@ -1349,13 +1280,7 @@ int cc_yolo_op_conv(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, i
   if (int rc = check_frame_fmt("cc_yolo_op_conv", frame_fmt, Hf, Wf)) return rc;
   YoloPlan* P = nullptr;
   if (int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P)) return rc;
-  const int n = static_cast<int>(P->ops.size());
-  if (!out) return n;
-  CC_REQUIRE(i >= 0 && i < n, "cc_yolo_op_conv: op %d of a plan of %d ops", i, n);
-  const Op& op = P->ops[i];
-  *out = op.kind == Op::DIRECT ? conv_op_of(op.direct) : op.kind == Op::GEMM ? conv_op_of(op.conv, op.chain, op.gemm) : cc_conv_op{};
-  snprintf(out->name, sizeof(out->name), "%s", op.name.c_str());
-  return n;
+  return op_conv_tap("cc_yolo_op_conv", P->ops, i, out);
 }
 
 int cc_yolo_run_ops(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, int first, int last,
@@ -1364,22 +1289,11 @@ int cc_yolo_run_ops(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int 
   if (int rc = check_frame_fmt("cc_yolo_run_ops", frame_fmt, Hf, Wf)) return rc;
   YoloPlan* P = nullptr;
   if (int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P)) return rc;
-  const int n = static_cast<int>(P->ops.size());
-  CC_REQUIRE(0 <= first && first <= last && last <= n, "cc_yolo_run_ops: ops [%d, %d) of a plan of %d ops", first, last, n);
-  return plan_run(*P, d_frames, d_out, d_raw, static_cast<cudaStream_t>(stream), nullptr, nullptr, first, last);
+  if (int rc = check_range("cc_yolo_run_ops", first, last, static_cast<int>(P->ops.size()))) return rc;
+  return run_ops(P->ops, frames_io(d_frames, d_out, d_raw), static_cast<cudaStream_t>(stream), first, last);
 }
 
 // parity tap: copy the output of spec layer `layer` of the cached plan (after a forward) to dense fp32 NHWC
-__global__ void tap_kernel(const __nv_bfloat16* src, int f32, int cs, int co, int C, long long npix, float* dst) {
-  const long long total = npix * C;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const long long pix = i / C;
-    const int c = static_cast<int>(i % C);
-    dst[i] = f32 ? reinterpret_cast<const float*>(src)[pix * cs + co + c] : __bfloat162float(src[pix * cs + co + c]);
-  }
-}
-
 int cc_yolo_layer_output(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int layer, float* d_dst, int* C,
                          int* H, int* W, void* stream) {
   CC_REQUIRE(h, "cc_yolo_layer_output: null handle");
@@ -1393,10 +1307,7 @@ int cc_yolo_layer_output(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int r
   if (H) *H = t.H;
   if (W) *W = t.W;
   if (!d_dst || t.image || !t.p) return CC_OK;
-  const long long npix = static_cast<long long>(B) * t.H * t.W;
-  tap_kernel<<<132 * 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(t.p, t.f32 ? 1 : 0, t.cs, t.co, t.C, npix, d_dst);
-  CC_CHECK_CUDA(cudaGetLastError());
-  return CC_OK;
+  return slice_to_f32_launch(t, d_dst, static_cast<cudaStream_t>(stream));
 }
 
 // kernel-level taps for the parity tests
@@ -1539,17 +1450,17 @@ int cc_conv2d_fp32_accurate(const float* d_in, int N, int Hin, int Win, int in_c
   cw.bias = h_bias ? reinterpret_cast<float*>(ws) : nullptr;     ws += bias_b;
   for (size_t i = 0; i < seg_c.size(); ++i) { cw.whi.push_back(reinterpret_cast<__nv_bfloat16*>(ws)); ws += al256(rows * seg_c[i] * 2); }
   const TSlice in = nhwc_slice(d_in, in_cs, in_co, Cin, 1, N, Hin, Win), res = nhwc_slice(d_res, res_cs, res_co, Cout, 1);
-  YoloPlan run;
+  std::vector<PlanOp> ops;
   double flops = 0;
   if (int rc = precise_conv_ops("conv", cw, in, stride, act, planes, acc, nhwc_slice(d_out, out_cs, out_co, Cout, 1), d_res ? &res : nullptr, sms,
-                                &run.ops, &flops))
+                                &ops, &flops))
     return rc;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   CC_CHECK_CUDA(cudaMemcpyAsync(cw.w5, w5.data(), w5.size() * 2, cudaMemcpyHostToDevice, st));
   if (h_bias) CC_CHECK_CUDA(cudaMemcpyAsync(cw.bias, h_bias, size_t(Cout) * 4, cudaMemcpyHostToDevice, st));
   for (size_t i = 0; i < whi.size(); ++i)
     CC_CHECK_CUDA(cudaMemcpyAsync(cw.whi[i], whi[i].data(), whi[i].size() * 2, cudaMemcpyHostToDevice, st));
-  return plan_run(run, nullptr, nullptr, nullptr, st);
+  return run_ops(ops, PlanIO{}, st);
 }
 
 }  // extern "C"

@@ -1,11 +1,14 @@
-"""What the detector and CLIP plans of this build are made of, as text two builds can be diffed on (CC_LIB selects the
-library, as in tools/ab.py): per op its kind, name, algorithmic FLOPs and bytes; the plan facts; and a SHA-256 of what a
-forward returns on seeded frames.  A host-side change to how convs are described must leave every line as it was.
+"""What the detector, CLIP and face plans of this build are made of, as text two builds can be diffed on (CC_LIB selects the
+library, as in tools/ab.py): per op its kind, name, algorithmic FLOPs and bytes; the detector trace's kind, name and FLOPs per
+op; every op's conv descriptor (cc_*_op_conv: each non-pointer field, and whether each pointer is NULL); the plan facts; and
+a SHA-256 of what a forward returns on seeded frames.  A host-side change to how plans are built or run must leave every
+line as it was.
 
 usage:  python tools/plan_dump.py OUT.txt
 Covers the sizes bench.py runs (c at B=32 and e at B=16, 640x640; c on 1080p frames), small t / s / m plans, the default
 and the fp32-accurate mode, a frame-table call over frames of two shapes, both CLIP towers (ViT-B/32, ViT-L/14), AdaFace
 embeddings on synthetic weights and BlazeFace detections on the reference's weights (tests/golden/blazeface_ref.npz)."""
+import ctypes
 import hashlib
 import os
 import sys
@@ -21,10 +24,12 @@ from oracle import adaface as oa  # noqa: E402
 from oracle import blazeface as obf  # noqa: E402
 from oracle import clip as oc  # noqa: E402
 from oracle import yolov9 as o  # noqa: E402
+from clearcam_b200._lib import cc_conv_op, check, lib  # noqa: E402
 from clearcam_b200.detection.yolov9 import YOLOv9  # noqa: E402
 from clearcam_b200.models.adaface import ADAFACE  # noqa: E402
 from clearcam_b200.models.blazeface import BlazeFace  # noqa: E402
 from clearcam_b200.models.objects import OpenCLIP  # noqa: E402
+from clearcam_b200.utils.helpers import batch_bucket  # noqa: E402
 
 #        size res  B   H     W     modes (False: bf16 storage, True: fp32-accurate)
 CASES = [("c", 640, 32, 640, 640, (False,)), ("e", 640, 16, 640, 640, (False,)), ("c", 640, 8, 1080, 1920, (False, True)),
@@ -36,6 +41,30 @@ def sha(*ts):
     for t in ts:
         h.update(t.detach().cpu().contiguous().numpy().tobytes())
     return h.hexdigest()
+
+
+def fields(s):
+    """A ctypes struct as text: every non-pointer field's value, and for a pointer only whether it is NULL."""
+    out = []
+    for name, typ in s._fields_:
+        v = getattr(s, name)
+        if isinstance(v, ctypes.Structure):
+            out.append(f"{name}({fields(v)})")
+        elif typ is ctypes.c_void_p:
+            out.append(f"{name}={'NULL' if v is None else 'set'}")
+        else:
+            out.append(f"{name}={v.decode() if isinstance(v, bytes) else v}")
+    return " ".join(out)
+
+
+def op_convs(say, tag, op_conv):
+    """Every op's cc_conv_op of a plan; op_conv(i, out) is the cc_*_op_conv call with the plan's arguments bound."""
+    n = op_conv(0, None)
+    check(min(n, 0), "op_conv")
+    for i in range(n):
+        d = cc_conv_op()
+        check(min(op_conv(i, ctypes.byref(d)), 0), "op_conv")
+        say(tag, "conv", i, fields(d))
 
 
 def main():
@@ -52,6 +81,9 @@ def main():
             say(tag, "plan", sorted(m.plan_info(B, H, W).items()))
             for r in m.profile(fr):
                 say(tag, r["kind"], r["name"], repr(r["flops"]), repr(r["bytes"]))
+            for r in m.trace(fr):
+                say(tag, "trace", r["kind"], r["name"], repr(r["flops"]))
+            op_convs(say, tag, lambda i, d: lib().cc_yolo_op_conv(m._h, 0, B, H, W, m.res, i, d))
             det, raw = m.detect_batch(fr, raw=True)
             say(tag, "outputs", sha(det, raw))
             if size == "c" and H == 1080 and not precise:       # frame-table plan: bgr24 1080p and yuv420p 720p share a net shape
@@ -72,11 +104,15 @@ def main():
             say("clip", arch, tower, "total flops", repr(total))
             for r in ops:
                 say("clip", arch, tower, r["name"], repr(r["flops"]))
+            nb = B if tower == "image" else ids.shape[0]
+            op_convs(say, f"clip {arch} {tower} B{nb}",
+                     lambda i, d: lib().cc_clip_op_conv(cm._h, int(tower == "text"), nb, i, d))
         say("clip", arch, "outputs", sha(cm.precompute_embedding(x).tensor, cm.encode_token_ids(ids).tensor))
         del cm
     fm = ADAFACE(oa.synthetic_weights(seed=5))
     for B in (1, 3, 16, 64, 200):
         say("adaface", f"B{B}", "outputs", sha(fm.embed(oa.synthetic_faces(B, seed=B))))
+        op_convs(say, f"adaface B{batch_bucket(B)}", lambda i, d: lib().cc_face_op_conv(fm._h, batch_bucket(B), i, d))
     del fm
     det = BlazeFace({k: v.numpy() for k, v in obf.load_weights(os.path.join(ROOT, "tests", "golden", "blazeface_ref.npz")).items()})
     sizes = [(256, 256), (640, 640), (480, 640), (97, 300), (333, 129), (720, 1280), (1080, 1920)]
