@@ -18,7 +18,8 @@ class CCError(RuntimeError):
 
 
 # frames per cc_yolo_forward_frames / cc_letterbox_frames call (CC_MAX_FRAMES in include/clearcam_b200.h); the crop entry
-# points' tables (cc_*_frames of the JPEG encoder and the CLIP preprocess) have no such limit
+# points' tables (the cc_*_frames of the CLIP preprocess and of the JPEG encoder, coefficients and crops-decoded) have no
+# such limit
 CC_MAX_FRAMES = 128
 
 
@@ -153,7 +154,6 @@ _SIGS = {
     "cc_face_align": (_i, [_vp, _i, _vp, _vp]),
     "cc_search_scores": (_i, [_vp, _i, _i, _vp, _i, _vp, _vp]),
     "cc_search_topk": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
-    "cc_clip_preprocess": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp]),
     "cc_clip_preprocess_frames": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp]),
     "cc_ocsort_create": (_i, [_i, _i, ctypes.c_double, _i, ctypes.c_double, _i, ctypes.POINTER(_vp)]),
     "cc_ocsort_destroy": (_i, [_vp]),
@@ -205,17 +205,12 @@ _SIGS = {
     "cc_text_embed": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "cc_l2norm": (_i, [_vp, _i, _i, _f, _vp, ctypes.c_longlong, _vp]),
     "cc_jpeg_bound": (_i, [_i, _i, ctypes.POINTER(ctypes.c_int64)]),
-    "cc_jpeg_encode_crops": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, ctypes.c_int64, _vp, _vp, _vp, ctypes.c_size_t,
-                                  ctypes.POINTER(ctypes.c_size_t), _vp]),
     "cc_jpeg_encode_crops_frames": (_i, [_vp, _i, _vp, _i, _i, _vp, ctypes.c_int64, _vp, _vp, _vp, ctypes.c_size_t,
                                          ctypes.POINTER(ctypes.c_size_t), _vp]),
-    "cc_jpeg_coeffs": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, ctypes.POINTER(ctypes.c_int64), _vp]),
+    "cc_jpeg_coeffs_frames": (_i, [_vp, _i, _vp, _i, _i, _vp, ctypes.POINTER(ctypes.c_int64), _vp]),
     "cc_jpeg_table_bytes": (ctypes.c_size_t, []),
     "cc_jpeg_parse": (_i, [_vp, ctypes.c_int64, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
-    "cc_jpeg_decode": (_i, [_vp, _vp, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t), _vp]),
-    "cc_jpeg_decode_frames": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t), _vp]),
-    "cc_jpeg_crops_decoded": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, ctypes.c_size_t,
-                                   ctypes.POINTER(ctypes.c_size_t), _vp]),
+    "cc_jpeg_decode_frames": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t), _vp]),
     "cc_jpeg_crops_decoded_frames": (_i, [_vp, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, ctypes.c_size_t,
                                           ctypes.POINTER(ctypes.c_size_t), _vp]),
 }

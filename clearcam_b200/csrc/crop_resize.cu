@@ -10,8 +10,7 @@
 //
 // HBM-bound and tiny next to the encoder (K x 224 x 224 outputs, 48 byte reads each, served from L1/L2): one thread per
 // output pixel, three channels, coalesced plane writes.  Each rect carries its own source (frame pointer, extent, format),
-// so one call takes crops of frames of any shapes and formats (cc_clip_preprocess_frames); cc_clip_preprocess fills the
-// same table from one frame batch.
+// so one call takes crops of frames of any shapes and formats (cc_clip_preprocess_frames).
 #include <cstdint>
 #include <vector>
 
@@ -143,25 +142,6 @@ int crop_resize_sources(const CropSource* src, const int32_t* rects, int K, int 
 
 }  // namespace
 }  // namespace cc
-
-extern "C" int cc_clip_preprocess(const uint8_t* d_frames, int n_frames, int H, int W, const int32_t* rects, int K, int size,
-                                  int src_fmt, float* d_out, void* stream) {
-  using namespace cc;
-  CC_REQUIRE(d_frames && d_out && (rects || K == 0), "cc_clip_preprocess: null pointer");
-  CC_REQUIRE(n_frames > 0 && H > 0 && W > 0 && K >= 0 && size >= 1 && size <= 4096, "cc_clip_preprocess: bad sizes");
-  CC_REQUIRE(src_fmt >= 0 && src_fmt <= 2, "cc_clip_preprocess: unknown source format %d (0 = RGB, 1 = BGR, 2 = I420)", src_fmt);
-  CC_REQUIRE(src_fmt != 2 || (H % 2 == 0 && W % 2 == 0), "cc_clip_preprocess: an I420 frame needs an even height and width, got %dx%d",
-             H, W);
-  for (int k = 0; k < K; ++k) {
-    const int32_t* r = rects + 5 * k;
-    CC_REQUIRE(r[0] >= 0 && r[0] < n_frames && r[1] >= 0 && r[2] >= 0 && r[3] > r[1] && r[4] > r[2] && r[3] <= W && r[4] <= H,
-               "cc_clip_preprocess: rect %d (frame %d, %d,%d-%d,%d) is empty or outside the %dx%d frame", k, r[0], r[1], r[2],
-               r[3], r[4], W, H);
-  }
-  std::vector<CropSource> src(K);
-  uniform_crop_sources(d_frames, H, W, src_fmt, rects, K, src.data());
-  return crop_resize_sources(src.data(), rects, K, size, d_out, static_cast<cudaStream_t>(stream));
-}
 
 extern "C" int cc_clip_preprocess_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int size, float* d_out,
                                          void* stream) {

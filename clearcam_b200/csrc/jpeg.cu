@@ -8,8 +8,7 @@
 // One call, per group of up to kCropsPerLaunch crops (the crop table travels as a kernel parameter, so there is no copy,
 // no allocation and no host sync), runs eight stream-ordered launches over all of its crops.  In the transform's table
 // every crop carries its own source (frame pointer, extent, RGB / BGR / I420), so the crops of one call may come from
-// frames of any shapes and formats (cc_jpeg_encode_crops_frames); the uniform entry points fill the same table from one
-// frame batch.
+// frames of any shapes and formats (cc_jpeg_encode_crops_frames).
 //   1. transform  one CTA per MCU (16x16 pixels): gather with libjpeg's edge replication, YCbCr, h2v2 downsampling,
 //                 8x8 integer DCT, quantisation -> int16 zigzag coefficients of the 6 blocks, dummy blocks included
 //   2. lengths    one CTA per tile of kTileMcus MCUs, a warp per block: the bit length of every block's Huffman codes
@@ -657,23 +656,6 @@ Layout layout(const int32_t* rects, int k0, int n, bool with_coef) {
   return L;
 }
 
-int check_common(const char* who, const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K,
-                 int quality) {
-  CC_REQUIRE(d_frames && (rects || K == 0), "%s: null pointer", who);
-  CC_REQUIRE(n_frames > 0 && H > 0 && W > 0 && K >= 0, "%s: bad sizes n_frames=%d H=%d W=%d K=%d", who, n_frames, H, W, K);
-  CC_REQUIRE(src_fmt >= 0 && src_fmt <= 2, "%s: unknown source format %d (0 = RGB, 1 = BGR, 2 = I420)", who, src_fmt);
-  CC_REQUIRE(src_fmt != 2 || (H % 2 == 0 && W % 2 == 0), "%s: an I420 frame needs an even height and width, got %dx%d", who, H, W);
-  CC_REQUIRE(quality >= 0 && quality <= 100, "%s: quality %d outside 0..100", who, quality);
-  for (int k = 0; k < K; ++k) {
-    const int32_t* r = rects + 5 * k;
-    CC_REQUIRE(r[0] >= 0 && r[0] < n_frames && r[1] >= 0 && r[2] >= 0 && r[3] > r[1] && r[4] > r[2] && r[3] <= W && r[4] <= H,
-               "%s: rect %d (frame %d, %d,%d-%d,%d) is empty or outside the %dx%d frame", who, k, r[0], r[1], r[2], r[3], r[4],
-               W, H);
-    CC_REQUIRE(r[3] - r[1] <= kMaxSide && r[4] - r[2] <= kMaxSide, "%s: rect %d is larger than %d pixels", who, k, kMaxSide);
-  }
-  return CC_OK;
-}
-
 // the crop table of crops [k0, k0 + n); with_coef: coefficients at d_coef (the tap) instead of the workspace
 void fill_params(JpegParams& p, TransformParams& t, const CropSource* src, const int32_t* rects, int k0, int n, uint8_t* ws,
                  const Layout& L, int16_t* d_coef, uint8_t* d_out, const int64_t* out_offsets, int64_t* d_lengths) {
@@ -712,7 +694,7 @@ int total_zero_ctas(const JpegParams& p) {
   return c.zero0 + static_cast<int>((w + kZeroWords - 1) / kZeroWords);
 }
 
-// cc_jpeg_encode_crops from the point where the crops' sources and rects are checked
+// cc_jpeg_encode_crops_frames from the point where the crops' sources and rects are checked
 int encode_sources(const char* who, const CropSource* src, const int32_t* rects, int K, int quality, uint8_t* d_out,
                    int64_t out_bytes, const int64_t* out_offsets, int64_t* d_lengths, void* d_workspace, size_t ws_bytes,
                    size_t* ws_needed, void* stream) {
@@ -765,19 +747,15 @@ int encode_sources(const char* who, const CropSource* src, const int32_t* rects,
 
 }  // namespace
 
-void uniform_crop_sources(const uint8_t* d_frames, int H, int W, int src_fmt, const int32_t* rects, int K, CropSource* src) {
-  const size_t frame_bytes = src_fmt == 2 ? static_cast<size_t>(H) * W * 3 / 2 : static_cast<size_t>(H) * W * 3;
-  for (int k = 0; k < K; ++k) src[k] = CropSource{d_frames + static_cast<size_t>(rects[5 * k]) * frame_bytes, H, W, src_fmt};
-}
-
 int table_crop_sources(const char* who, const cc_frame* frames, int n_frames, const int32_t* rects, int K, CropSource* src) {
   CC_REQUIRE(frames && (rects || K == 0), "%s: null pointer", who);
   CC_REQUIRE(n_frames > 0 && K >= 0, "%s: bad sizes n_frames=%d K=%d", who, n_frames, K);
   for (int i = 0; i < n_frames; ++i) {
     const cc_frame& f = frames[i];
     CC_REQUIRE(f.data, "%s: frame %d is NULL", who, i);
-    CC_REQUIRE(f.fmt == CC_FRAME_BGR_U8 || f.fmt == CC_FRAME_I420_U8,
-               "%s: frame %d has format %d; crops take CC_FRAME_BGR_U8 (0) or CC_FRAME_I420_U8 (2) frames", who, i, f.fmt);
+    CC_REQUIRE(f.fmt == CC_FRAME_BGR_U8 || f.fmt == CC_FRAME_I420_U8 || f.fmt == CC_FRAME_RGB_U8,
+               "%s: frame %d has format %d: unknown source format %d for a crop (CC_FRAME_BGR_U8 0, CC_FRAME_I420_U8 2 or "
+               "CC_FRAME_RGB_U8 3)", who, i, f.fmt, f.fmt);
     CC_REQUIRE(f.h > 0 && f.w > 0, "%s: frame %d has a bad size %dx%d", who, i, f.w, f.h);
     CC_REQUIRE(f.fmt != CC_FRAME_I420_U8 || (f.h % 2 == 0 && f.w % 2 == 0),
                "%s: frame %d: an I420 frame needs an even height and width, got %dx%d", who, i, f.w, f.h);
@@ -789,7 +767,8 @@ int table_crop_sources(const char* who, const cc_frame* frames, int n_frames, co
     CC_REQUIRE(r[1] >= 0 && r[2] >= 0 && r[3] > r[1] && r[4] > r[2] && r[3] <= f.w && r[4] <= f.h,
                "%s: rect %d (frame %d, %d,%d-%d,%d) is empty or outside its %dx%d frame", who, k, r[0], r[1], r[2], r[3], r[4],
                f.w, f.h);
-    src[k] = CropSource{static_cast<const uint8_t*>(f.data), f.h, f.w, f.fmt == CC_FRAME_BGR_U8 ? 1 : 2};
+    const int fmt = f.fmt == CC_FRAME_RGB_U8 ? 0 : f.fmt == CC_FRAME_BGR_U8 ? 1 : 2;
+    src[k] = CropSource{static_cast<const uint8_t*>(f.data), f.h, f.w, fmt};
   }
   return CC_OK;
 }
@@ -842,17 +821,6 @@ extern "C" int cc_jpeg_bound(int w, int h, int64_t* bytes) {
   return CC_OK;
 }
 
-extern "C" int cc_jpeg_encode_crops(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K,
-                                    int quality, uint8_t* d_out, int64_t out_bytes, const int64_t* out_offsets, int64_t* d_lengths,
-                                    void* d_workspace, size_t ws_bytes, size_t* ws_needed, void* stream) {
-  const char* who = "cc_jpeg_encode_crops";
-  if (int rc = check_common(who, d_frames, n_frames, H, W, src_fmt, rects, K, quality)) return rc;
-  std::vector<CropSource> src(K);
-  uniform_crop_sources(d_frames, H, W, src_fmt, rects, K, src.data());
-  return encode_sources(who, src.data(), rects, K, quality, d_out, out_bytes, out_offsets, d_lengths, d_workspace, ws_bytes,
-                        ws_needed, stream);
-}
-
 extern "C" int cc_jpeg_encode_crops_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int quality,
                                            uint8_t* d_out, int64_t out_bytes, const int64_t* out_offsets, int64_t* d_lengths,
                                            void* d_workspace, size_t ws_bytes, size_t* ws_needed, void* stream) {
@@ -864,12 +832,12 @@ extern "C" int cc_jpeg_encode_crops_frames(const cc_frame* frames, int n_frames,
                         ws_needed, stream);
 }
 
-extern "C" int cc_jpeg_coeffs(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K,
-                              int quality, int16_t* d_coef, int64_t* n_blocks, void* stream) {
-  const char* who = "cc_jpeg_coeffs";
-  if (int rc = check_common(who, d_frames, n_frames, H, W, src_fmt, rects, K, quality)) return rc;
-  std::vector<CropSource> src(K);
-  uniform_crop_sources(d_frames, H, W, src_fmt, rects, K, src.data());
+extern "C" int cc_jpeg_coeffs_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int quality,
+                                     int16_t* d_coef, int64_t* n_blocks, void* stream) {
+  const char* who = "cc_jpeg_coeffs_frames";
+  std::vector<CropSource> src(std::max(K, 0));
+  if (int rc = table_crop_sources(who, frames, n_frames, rects, K, src.data())) return rc;
+  if (int rc = check_table_jpeg(who, rects, K, quality)) return rc;
   jpeg_coeffs_sources(src.data(), rects, K, quality, nullptr, n_blocks, nullptr);
   if (!d_coef) return CC_OK;                     // size query
   CC_REQUIRE((reinterpret_cast<uintptr_t>(d_coef) & 3) == 0, "%s: d_coef must be 4-byte aligned", who);

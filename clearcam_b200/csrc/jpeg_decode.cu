@@ -8,7 +8,7 @@
 // cc_jpeg_parse (host) reads the markers of K files into a per-image table: sizes, sampling, quantisation tables, Huffman
 // lookup tables, restart interval, the scan's place in the data, and where each image's intermediates go in the workspace.
 // Files the device does not decode get a status (unsupported or corrupt) there and are left to the caller.
-// cc_jpeg_decode then runs, on the caller's stream, with no allocation and no host sync:
+// cc_jpeg_decode_frames then runs, on the caller's stream, with no allocation and no host sync:
 //   1. status     the table's status per image into d_status
 //   2. count      per 1 KB chunk of scan data: bytes kept after removing FF 00 stuffing, fill bytes and RSTn markers
 //   3. scan       per image (a warp): chunk offsets; interval bounds; wrong RSTn count -> corrupt
@@ -27,9 +27,9 @@
 //  10. dc         DC differences -> values per component: per chunk of 256 MCUs (a warp) the sums, then each chunk adds
 //                 the sums before it in its interval and scans its MCUs
 //  11. idct       per block: dequantise, islow IDCT, range limit -> the component's sample plane
-//  12. pixels     per output pixel: fancy upsampling of the chroma planes, YCbCr -> BGR into the padded batch
+//  12. pixels     per output pixel: fancy upsampling of the chroma planes, YCbCr -> BGR into the destinations
 // Kernels 11 and 12 also turn the encoder's quantised coefficients of object crops into the pixels of their JPEG files
-// (cc_jpeg_crops_decoded), with no entropy coding in between.
+// (cc_jpeg_crops_decoded_frames), with no entropy coding in between.
 #include <cstddef>
 #include <cstdint>
 #include <cstring>
@@ -1035,7 +1035,7 @@ extern "C" int cc_jpeg_parse(const uint8_t* h_data, int64_t data_bytes, const in
   return CC_OK;
 }
 
-// cc_jpeg_decode and cc_jpeg_decode_frames once their arguments are checked: image k (status OK) goes to dst[k], rows
+// cc_jpeg_decode_frames once its arguments are checked: image k (status OK) goes to dst[k], rows
 // pitch[k] bytes apart
 static int decode_checked(const uint8_t* d_data, const JpegImage* tab, const void* d_table, int K, const Layout& L,
                           uint8_t* const* dst, const long long* pitch, int32_t* d_status, int16_t* d_coef, void* d_workspace,
@@ -1108,36 +1108,16 @@ static int check_tables(const char* who, const JpegImage* tab, int K, const void
   return CC_OK;
 }
 
-extern "C" int cc_jpeg_decode(const uint8_t* d_data, const void* h_table, const void* d_table, int K, uint8_t* d_out, int Hmax,
-                              int Wmax, int32_t* d_status, int16_t* d_coef, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
-                              void* stream) {
-  const char* who = "cc_jpeg_decode";
+extern "C" int cc_jpeg_decode_frames(const uint8_t* d_data, const void* h_table, const void* d_table, int K, const cc_jpeg_dest* outs,
+                                     int32_t* d_status, int16_t* d_coef, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
+                                     void* stream) {
+  const char* who = "cc_jpeg_decode_frames";
   CC_REQUIRE(K >= 0 && (K == 0 || h_table), "%s: null table or K=%d < 0", who, K);
   const JpegImage* tab = static_cast<const JpegImage*>(h_table);
   const Layout L = layout(tab, K, d_coef == nullptr);
   if (ws_needed) *ws_needed = L.total;
-  if (!d_out) return CC_OK;                           // workspace size query
-  CC_REQUIRE(Hmax > 0 && Wmax > 0, "%s: bad batch size %dx%d", who, Hmax, Wmax);
-  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_coef) & 15) == 0, "%s: d_coef must be 16-byte aligned", who);
-  if (int rc = check_tables(who, tab, K, d_data, d_table, d_status, L, d_workspace, ws_bytes)) return rc;
-  std::vector<uint8_t*> dst(K);
-  std::vector<long long> pitch(K, 3ll * Wmax);
-  for (int k = 0; k < K; ++k) {
-    CC_REQUIRE(tab[k].status != CC_JPEG_OK || (tab[k].w <= Wmax && tab[k].h <= Hmax),
-               "%s: image %d (%dx%d) does not fit the %dx%d batch", who, k, tab[k].w, tab[k].h, Wmax, Hmax);
-    dst[k] = d_out + static_cast<long long>(k) * Hmax * Wmax * 3;
-  }
-  return decode_checked(d_data, tab, d_table, K, L, dst.data(), pitch.data(), d_status, d_coef, d_workspace, stream);
-}
-
-extern "C" int cc_jpeg_decode_frames(const uint8_t* d_data, const void* h_table, const void* d_table, int K, const cc_jpeg_dest* outs,
-                                     int32_t* d_status, void* d_workspace, size_t ws_bytes, size_t* ws_needed, void* stream) {
-  const char* who = "cc_jpeg_decode_frames";
-  CC_REQUIRE(K >= 0 && (K == 0 || h_table), "%s: null table or K=%d < 0", who, K);
-  const JpegImage* tab = static_cast<const JpegImage*>(h_table);
-  const Layout L = layout(tab, K, true);
-  if (ws_needed) *ws_needed = L.total;
   if (!outs) return CC_OK;                            // workspace size query
+  CC_REQUIRE((reinterpret_cast<uintptr_t>(d_coef) & 15) == 0, "%s: d_coef must be 16-byte aligned", who);
   if (int rc = check_tables(who, tab, K, d_data, d_table, d_status, L, d_workspace, ws_bytes)) return rc;
   std::vector<uint8_t*> dst(K);
   std::vector<long long> pitch(K);
@@ -1156,10 +1136,10 @@ extern "C" int cc_jpeg_decode_frames(const uint8_t* d_data, const void* h_table,
   std::sort(spans.begin(), spans.end());
   for (size_t i = 1; i < spans.size(); ++i)
     CC_REQUIRE(spans[i].first >= spans[i - 1].second, "%s: two destinations overlap", who);
-  return decode_checked(d_data, tab, d_table, K, L, dst.data(), pitch.data(), d_status, nullptr, d_workspace, stream);
+  return decode_checked(d_data, tab, d_table, K, L, dst.data(), pitch.data(), d_status, d_coef, d_workspace, stream);
 }
 
-// cc_jpeg_crops_decoded from the point where the crops' sources, rects and quality are checked
+// cc_jpeg_crops_decoded_frames from the point where the crops' sources, rects and quality are checked
 static int crops_decoded_sources(const char* who, const CropSource* src, const int32_t* rects, int K, int quality, uint8_t* d_out,
                                  int Hmax, int Wmax, int32_t* d_status, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
                                  void* stream) {
@@ -1204,17 +1184,6 @@ static int crops_decoded_sources(const char* who, const CropSource* src, const i
   std::memcpy(qa.q, qt, sizeof(qt));
   jdec_put_qt_kernel<<<1, 128, 0, st>>>(qa, reinterpret_cast<uint16_t*>(ws));
   return launch_recon(rp, imgs, st);
-}
-
-extern "C" int cc_jpeg_crops_decoded(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K,
-                                     int quality, uint8_t* d_out, int Hmax, int Wmax, int32_t* d_status, void* d_workspace,
-                                     size_t ws_bytes, size_t* ws_needed, void* stream) {
-  // validates the frames, rects and quality exactly as the encoder does
-  if (int rc = cc_jpeg_coeffs(d_frames, n_frames, H, W, src_fmt, rects, K, quality, nullptr, nullptr, nullptr)) return rc;
-  std::vector<CropSource> src(K);
-  uniform_crop_sources(d_frames, H, W, src_fmt, rects, K, src.data());
-  return crops_decoded_sources("cc_jpeg_crops_decoded", src.data(), rects, K, quality, d_out, Hmax, Wmax, d_status, d_workspace,
-                               ws_bytes, ws_needed, stream);
 }
 
 extern "C" int cc_jpeg_crops_decoded_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int quality,

@@ -28,7 +28,8 @@ import torch
 
 from .._lib import CCError, Handle, check, create, lib, ptr, stream_ptr
 from ..detection.yolov9 import DeviceResult, _as_tensor, load_weights_arg
-from ..pixfmt import BGR24, check_pix_fmt, yuv420p_size
+from .. import ops
+from ..pixfmt import BGR24, CC_FRAME_BGR_U8, CC_FRAME_I420_U8, CC_FRAME_RGB_U8, check_pix_fmt, yuv420p_size
 from ..utils.clip_tokenizer import SimpleTokenizer
 from ..utils.helpers import batch_bucket
 
@@ -153,26 +154,28 @@ def search_scores(index, queries) -> torch.Tensor:
 
 def _device_crops(frames, rects, bgr: bool, pix_fmt: str):
     """The frame / rect conventions of `ObjectFinder.preprocess_device` and `encode_crops`: frames uint8 [n,H,W,3] / [H,W,3]
-    (bgr24) or [n,H*3/2,W] / [H*3/2,W] (yuv420p), host or device; rects K rows of (frame, x1, y1, x2, y2) or (x1, y1, x2,
-    y2).  -> (contiguous device frames [n,...], H, W, the C-ABI src_fmt (0 RGB, 1 BGR, 2 I420), int32 rects [K,5])."""
+    (bgr24, or RGB when not `bgr`) or [n,H*3/2,W] / [H*3/2,W] (yuv420p), host or device; rects K rows of (frame, x1, y1,
+    x2, y2) or (x1, y1, x2, y2).  -> (contiguous device frames [n,...], their frame table, int32 rects [K,5]); the table
+    points into the frames, so it is used while they live."""
     t = _as_tensor(frames)
     if check_pix_fmt(pix_fmt) == BGR24:
         if t.dim() == 3:
             t = t.unsqueeze(0)
         if t.dtype != torch.uint8 or t.dim() != 4 or t.shape[-1] != 3:
             raise ValueError("frames must be uint8 [n,H,W,3]")
-        H, W, src_fmt = t.shape[1], t.shape[2], 1 if bgr else 0
+        fmt = CC_FRAME_BGR_U8 if bgr else CC_FRAME_RGB_U8
     else:
         if t.dim() == 2:
             t = t.unsqueeze(0)
         if t.dtype != torch.uint8 or t.dim() != 3:
             raise ValueError(f"yuv420p frames must be uint8 [n,H*3/2,W], got {t.dtype} {tuple(t.shape)}")
-        (H, W), src_fmt = yuv420p_size(t.shape), 2
+        yuv420p_size(t.shape)
+        fmt = CC_FRAME_I420_U8
     t = t.to("cuda", non_blocking=True).contiguous()
     r = np.asarray(rects, np.int32).reshape(-1, np.shape(rects)[-1] if len(rects) else 5)
     if r.shape[1] == 4:
         r = np.concatenate([np.zeros((len(r), 1), np.int32), r], 1)
-    return t, H, W, src_fmt, np.ascontiguousarray(r, np.int32)
+    return t, ops.batch_table(t, fmt), np.ascontiguousarray(r, np.int32)
 
 
 class ObjectFinder:
@@ -313,13 +316,13 @@ class ObjectFinder:
         `preprocess(cv2.cvtColor(frame[y1:y2, x1:x2], BGR2RGB))` with OpenCV's own bicubic — without leaving the GPU.
         pix_fmt="yuv420p": frames are uint8 [n,H*3/2,W] or [H*3/2,W] (H, W even; rects in pixels), and the result is
         bit-identical to the same crop of `cv2.cvtColor(frame, COLOR_YUV2RGB_I420)` (`bgr` does not apply)."""
-        t, H, W, src_fmt, r = _device_crops(frames, rects, bgr, pix_fmt)
+        t, table, r = _device_crops(frames, rects, bgr, pix_fmt)
         s = size or (self.model.image_size if self.model is not None else 224)
         # rows > K: the result is allocated with `rows` images, the first K filled and the rest zero (batch padding)
         out = torch.empty(len(r), 3, s, s, device="cuda", dtype=torch.float32) if not rows or rows <= len(r) else \
             torch.zeros(rows, 3, s, s, device="cuda", dtype=torch.float32)
-        check(lib().cc_clip_preprocess(ptr(t), t.shape[0], H, W, r.ctypes.data, len(r), s, src_fmt, ptr(out), stream_ptr(None)),
-              "cc_clip_preprocess")
+        check(lib().cc_clip_preprocess_frames(table, len(table), r.ctypes.data, len(r), s, ptr(out), stream_ptr(None)),
+              "cc_clip_preprocess_frames")
         return DeviceResult(out)
 
     def embed_crops(self, frames, rects, bgr: bool = True, pix_fmt: str = BGR24):
@@ -339,21 +342,19 @@ class ObjectFinder:
         `cv2.imwrite(path, frame[y1:y2, x1:x2])` writes at IMWRITE_JPEG_QUALITY `quality` (`save_object`,
         clearcam.py:373-399).  frames / rects / bgr / pix_fmt as in `preprocess_device`; a yuv420p frame gives the file of
         the same crop of `cv2.cvtColor(frame, COLOR_YUV2BGR_I420)`.  Only the encoded bytes cross PCIe."""
-        from .. import ops
         if not 0 <= int(quality) <= 100:
             raise ValueError(f"quality must be in 0..100 (cv2's range), got {quality}")
-        t, _, _, src_fmt, r = _device_crops(frames, rects, bgr, pix_fmt)
-        return ops.jpeg_encode_crops(t, r, quality, src_fmt)
+        t, table, r = _device_crops(frames, rects, bgr, pix_fmt)
+        return ops.jpeg_collect(*ops.jpeg_encode_crops_frames(table, r, quality)) if len(r) else []
 
     def embed_images(self, items):
         """The batched device form of `run_clip`'s `preprocess_clip` + `precompute_embedding` (clearcam.py:671-678,
         models/objects.py:244-251): items are `bytes` (an uploaded file) or the reference's paths relative to data/cameras
         (stored thumbnails) -> DeviceResult (K, embed_dim).  The files are decoded on the device (ops.jpeg_decode), then
-        cropped, resized and normalised by cc_clip_preprocess and embedded in one batch.  A file the device reports as
+        cropped, resized and normalised by cc_clip_preprocess_frames and embedded in one batch.  A file the device reports as
         unsupported or corrupt is decoded by cv2 on the host and joins the same batch; where cv2 returns None this raises as
         the reference's cvtColor does."""
         import cv2
-        from .. import ops
         k = len(items)
         if k == 0:
             return DeviceResult(torch.empty(0, self.model.embed_dim, device="cuda", dtype=torch.float32))
@@ -395,23 +396,13 @@ class ObjectFinder:
         """Detector frame -> (the JPEG file of each object crop, exactly as `encode_crops` returns them, and DeviceResult
         (K, embed_dim): the embeddings `clip_latest_img` stores for those files).  The reference writes the crop with
         cv2.imwrite, reads the file back and embeds the decoded pixels (clearcam.py:272-279, 1278-1287); here the decoded
-        pixels come from the encoder's quantised coefficients on the device (ops.jpeg_crops_decoded), with no host round
-        trip, and are embedded in one batch (a crop whose coefficients the device leaves to cv2 is decoded from its file on
-        the host)."""
-        from .. import ops
-        files = self.encode_crops(frames, rects, quality, bgr, pix_fmt)
-        k = len(files)
-        if k == 0:
-            return files, DeviceResult(torch.empty(0, self.model.embed_dim, device="cuda", dtype=torch.float32))
-        t, _, _, src_fmt, r = _device_crops(frames, rects, bgr, pix_fmt)
-        pix, status = ops.jpeg_crops_decoded(t, r, quality, src_fmt)
-        for i in np.flatnonzero(status.cpu().numpy() != ops.JPEG_OK):
-            import cv2                                  # coefficients outside the range every libjpeg-turbo IDCT agrees on
-            img = cv2.imdecode(np.frombuffer(files[i], np.uint8), cv2.IMREAD_COLOR)
-            pix[i, :img.shape[0], :img.shape[1]] = torch.from_numpy(img).to(pix.device)
-        crops = [(i, 0, 0, int(x2 - x1), int(y2 - y1)) for i, (_, x1, y1, x2, y2) in enumerate(r)]
-        x = self.preprocess_device(pix, crops, bgr=True, rows=batch_bucket(k))
-        return files, DeviceResult(self.model.precompute_embedding(x).tensor[:k])
+        pixels come from the encoder's quantised coefficients on the device (ops.jpeg_crops_decoded_frames), with no host
+        round trip, and are embedded in one batch (a crop whose coefficients the device leaves to cv2 is decoded from its
+        file on the host).  `encode_embed_frames` over the table of this batch."""
+        if not 0 <= int(quality) <= 100:
+            raise ValueError(f"quality must be in 0..100 (cv2's range), got {quality}")
+        t, table, r = _device_crops(frames, rects, bgr, pix_fmt)
+        return self._encode_embed(table, r, quality)
 
     def encode_embed_frames(self, frames, pix_fmts, rects, quality: int = 95):
         """`encode_embed_crops` for the objects of many frames of different shapes and formats in one call (the saves of
@@ -426,25 +417,25 @@ class ObjectFinder:
         and the decoded crops' statuses together, once for the files' bytes.  A crop whose coefficients the device leaves
         to cv2 (CC_JPEG_UNSUPPORTED, which only very low qualities reach) is decoded from its file on the host; the
         preprocess then runs again over those crops only, and the CLIP forward is repeated on the same padded batch."""
-        from .. import ops
         if not 0 <= int(quality) <= 100:
             raise ValueError(f"quality must be in 0..100 (cv2's range), got {quality}")
-        frames = list(frames)
         table, sizes = ops.frame_table(frames, pix_fmts)
-        r = ops.table_rects(rects, sizes)
+        return self._encode_embed(table, ops.table_rects(rects, sizes), quality)
+
+    def _encode_embed(self, table, r, quality):
         K = len(r)
         if K == 0:
             return [], (None if self.model is None else
                         DeviceResult(torch.empty(0, self.model.embed_dim, device="cuda", dtype=torch.float32)))
-        out, lengths, offsets = ops.jpeg_encode_launch_frames(table, len(frames), r, quality, frames[0].device)
+        out, lengths, offsets = ops.jpeg_encode_crops_frames(table, r, quality)
         if self.model is None:
-            return ops.jpeg_collect(out, lengths, lengths.cpu().numpy(), offsets), None
-        pix, status = ops.jpeg_crops_decoded_frames(frames, pix_fmts, r, quality, table=(table, r))
+            return ops.jpeg_collect(out, lengths, offsets), None
+        pix, status = ops.jpeg_crops_decoded_frames(table, r, quality)
         crops = [(i, 0, 0, int(x2 - x1), int(y2 - y1)) for i, (_, x1, y1, x2, y2) in enumerate(r)]
         x = self.preprocess_device(pix, crops, bgr=True, rows=batch_bucket(K)).tensor
         emb = self.model.precompute_embedding(x).tensor
         got = torch.cat([lengths, status.long()]).cpu().numpy()                 # host wait 1
-        files = ops.jpeg_collect(out, lengths, got[:K], offsets)                # host wait 2
+        files = ops.jpeg_collect(out, lengths, offsets, got[:K])                # host wait 2
         bad = [int(i) for i in np.flatnonzero(got[K:] != ops.JPEG_OK)]
         if bad:
             import cv2                                  # coefficients outside the range every libjpeg-turbo IDCT agrees on

@@ -240,31 +240,6 @@ def l2norm(x, eps, out=None, out_stride=None, stream=None):
     return out
 
 
-# ---- JPEG of frame crops (object thumbnails), byte-identical to cv2.imwrite
-JPEG_SRC_FMTS = {"rgb": 0, "bgr": 1, "i420": 2}
-
-
-def jpeg_bound(w, h):
-    """Worst-case bytes of one encoded w x h crop."""
-    b = ctypes.c_int64(0)
-    check(lib().cc_jpeg_bound(int(w), int(h), ctypes.byref(b)), "cc_jpeg_bound")
-    return b.value
-
-
-def _jpeg_frames(frames, src_fmt):
-    assert frames.is_cuda and frames.dtype == torch.uint8 and frames.is_contiguous()
-    if src_fmt == 2:
-        n, rows, W = frames.shape
-        return n, rows * 2 // 3, W
-    n, H, W, _ = frames.shape
-    return n, H, W
-
-
-def _rects_i32(rects):
-    import numpy as np
-    return np.ascontiguousarray(np.asarray(rects, np.int32).reshape(-1, 5))
-
-
 # ---- frame tables: device frames of different shapes and formats in one call
 def frame_table(frames, pix_fmts, padding=False):
     """Validate a list of device frames with per-frame formats -> (ctypes cc_frame array, [(H, W) or None per frame]).
@@ -277,7 +252,7 @@ def frame_table(frames, pix_fmts, padding=False):
     fmts = [pix_fmts] * B if isinstance(pix_fmts, str) else list(pix_fmts)
     if len(fmts) != B:
         raise ValueError(f"{B} frames but {len(fmts)} pixel formats")
-    table = (cc_frame * max(B, 1))()
+    table = (cc_frame * B)()
     sizes = []
     for i, (f, fmt) in enumerate(zip(frames, fmts)):
         check_pix_fmt(fmt)
@@ -300,6 +275,34 @@ def frame_table(frames, pix_fmts, padding=False):
     return table, sizes
 
 
+# the numpy layout of one cc_frame row (include/clearcam_b200.h): pointer, format, height, width
+_FRAME_ROW = {"names": ["data", "fmt", "h", "w"], "formats": ["<u8", "<i4", "<i4", "<i4"], "offsets": [0, 8, 12, 16],
+              "itemsize": 24}
+# ... and of one cc_jpeg_dest: pointer, row pitch, height, width
+_DEST_ROW = {"names": ["data", "pitch", "h", "w"], "formats": ["<u8", "<i8", "<i4", "<i4"], "offsets": [0, 8, 16, 20],
+             "itemsize": 24}
+
+
+def batch_table(frames, fmt):
+    """The frame table of a contiguous uint8 CUDA batch of n frames of one format (a CC_FRAME_* code): [n,H,W,3] for
+    CC_FRAME_BGR_U8 / CC_FRAME_RGB_U8, [n,H*3/2,W] for CC_FRAME_I420_U8 -> ctypes cc_frame [n], row i at the batch's
+    pointer + i frames.  The library checks the rows (and the rects against them) when a call reads the table."""
+    import numpy as np
+    from ._lib import cc_frame
+    from .pixfmt import CC_FRAME_I420_U8
+    assert frames.is_cuda and frames.dtype == torch.uint8 and frames.is_contiguous()
+    n, rows, W = frames.shape[:3]
+    t = np.zeros(n, _FRAME_ROW)                         # filled as one array: a fraction of the cost of n ctypes rows
+    t["data"] = frames.data_ptr() + frames.stride(0) * np.arange(n, dtype=np.uint64)
+    t["fmt"], t["h"], t["w"] = fmt, rows * 2 // 3 if fmt == CC_FRAME_I420_U8 else rows, W
+    return (cc_frame * n).from_buffer(t)
+
+
+def _rects_i32(rects):
+    import numpy as np
+    return np.ascontiguousarray(np.asarray(rects, np.int32).reshape(-1, 5))
+
+
 def table_rects(rects, sizes):
     """rects: K rows (frame, x1, y1, x2, y2) against a frame table's sizes -> contiguous int32 [K,5]; ValueError for a
     frame index outside the table or a rect that is empty or leaves its own frame."""
@@ -314,27 +317,43 @@ def table_rects(rects, sizes):
     return np.ascontiguousarray(r)
 
 
-def _jpeg_encode_launch(fn, args, r, dev, stream):
-    """Queue one encoder call (uniform or table form: fn(*args, d_out, ...)) -> (out, device lengths, offsets)."""
+# ---- JPEG of frame crops (object thumbnails), byte-identical to cv2.imwrite.  table: a frame_table or batch_table;
+# rects: K rows (frame index into the table, x1, y1, x2, y2)
+def jpeg_bound(w, h):
+    """Worst-case bytes of one encoded w x h crop."""
+    b = ctypes.c_int64(0)
+    check(lib().cc_jpeg_bound(int(w), int(h), ctypes.byref(b)), "cc_jpeg_bound")
+    return b.value
+
+
+def jpeg_encode_crops_frames(table, rects, quality=95, stream=None):
+    """Queue the encoding of K crops -> (out, device lengths, offsets); nothing waits.  The crops go into one device
+    buffer at offsets given by the prefix sum of their bounds; `jpeg_collect` brings the files back, file k being the one
+    cv2.imwrite writes for crop k at `quality`."""
     import numpy as np
+    r = _rects_i32(rects)
     K = len(r)
+    args = (table, len(table), r.ctypes.data, K, int(quality))
     bounds = np.array([jpeg_bound(x2 - x1, y2 - y1) if x2 > x1 and y2 > y1 else 0 for _, x1, y1, x2, y2 in r], np.int64)
     offsets = np.ascontiguousarray(np.concatenate([[0], np.cumsum(bounds)[:-1]]).astype(np.int64))
     need = ctypes.c_size_t(0)
-    check(getattr(lib(), fn)(*args, None, 0, None, None, None, 0, ctypes.byref(need), None), fn)
-    out = torch.empty(int(bounds.sum()), dtype=torch.uint8, device=dev)
-    lengths = torch.empty(K, dtype=torch.int64, device=dev)
-    ws = torch.empty(max(need.value, 1), dtype=torch.uint8, device=dev)
-    check(getattr(lib(), fn)(*args, ptr(out), out.numel(), offsets.ctypes.data, ptr(lengths), ptr(ws), need.value, None,
-                             stream_ptr(stream)), fn)
+    check(lib().cc_jpeg_encode_crops_frames(*args, None, 0, None, None, None, 0, ctypes.byref(need), None),
+          "cc_jpeg_encode_crops_frames")
+    out = torch.empty(int(bounds.sum()), dtype=torch.uint8, device="cuda")
+    lengths = torch.empty(K, dtype=torch.int64, device="cuda")
+    ws = torch.empty(max(need.value, 1), dtype=torch.uint8, device="cuda")
+    check(lib().cc_jpeg_encode_crops_frames(*args, ptr(out), out.numel(), offsets.ctypes.data, ptr(lengths), ptr(ws), need.value,
+                                            None, stream_ptr(stream)), "cc_jpeg_encode_crops_frames")
     return out, lengths, offsets
 
 
-def jpeg_collect(out, lengths, lens, offsets):
-    """The encoded files: the used bytes of every crop gathered into one device run, one copy to the host (one wait).
-    lens: the lengths already on the host."""
+def jpeg_collect(out, lengths, offsets, lens=None):
+    """The files of `jpeg_encode_crops_frames`' (out, lengths, offsets) as a list of K `bytes`: the used bytes of every crop
+    gathered into one device run, one copy to the host.  lens: the lengths already on the host, or None to fetch them
+    (a second host wait)."""
     import numpy as np
     dev = out.device
+    lens = lengths.cpu().numpy() if lens is None else lens
     total = int(lens.sum())
     starts = torch.cumsum(lengths, 0) - lengths
     idx = torch.arange(total, device=dev) + torch.repeat_interleave(torch.from_numpy(offsets).to(dev) - starts, lengths,
@@ -344,79 +363,38 @@ def jpeg_collect(out, lengths, lens, offsets):
     return [flat[e - l:e] for e, l in zip(ends, lens)]
 
 
-def jpeg_encode_crops_frames(frames, pix_fmts, rects, quality=95, stream=None):
-    """jpeg_encode_crops over frames of different shapes and formats in one call: frames / pix_fmts as in `frame_table`,
-    rects: K rows (frame index into `frames`, x1, y1, x2, y2) -> list of K `bytes`, file k being exactly what
-    jpeg_encode_crops gives for that crop of its frame alone.  Two host waits: the lengths, then the bytes."""
-    table, sizes = frame_table(frames, pix_fmts)
-    if not sizes:
-        raise ValueError("a frame table needs at least one frame")
-    r = table_rects(rects, sizes)
-    if len(r) == 0:
-        return []
-    out, lengths, offsets = jpeg_encode_launch_frames(table, len(sizes), r, quality, frames[0].device, stream)
-    return jpeg_collect(out, lengths, lengths.cpu().numpy(), offsets)
+def jpeg_coeffs_frames(table, rects, quality=95, stream=None):
+    """The quantised coefficients of every block of every crop: int16 CUDA [n_blocks, 64], zigzag order, crop by crop, MCU
+    by MCU (Y0 Y1 Y2 Y3 Cb Cr), dummy blocks included (oracle.jpeg.blocks of each crop, concatenated)."""
+    r = _rects_i32(rects)
+    nb = ctypes.c_int64(0)
+    args = (table, len(table), r.ctypes.data, len(r), int(quality))
+    check(lib().cc_jpeg_coeffs_frames(*args, None, ctypes.byref(nb), None), "cc_jpeg_coeffs_frames")
+    coef = torch.empty(nb.value, 64, dtype=torch.int16, device="cuda")
+    check(lib().cc_jpeg_coeffs_frames(*args, ptr(coef), ctypes.byref(nb), stream_ptr(stream)), "cc_jpeg_coeffs_frames")
+    return coef
 
 
-def jpeg_encode_launch_frames(table, n_frames, r, quality, dev, stream=None):
-    """Queue cc_jpeg_encode_crops_frames for a checked table and rects -> (out, device lengths, offsets); nothing waits."""
-    return _jpeg_encode_launch("cc_jpeg_encode_crops_frames", (table, n_frames, r.ctypes.data, len(r), int(quality)), r, dev,
-                               stream)
-
-
-def jpeg_crops_decoded_frames(frames, pix_fmts, rects, quality=95, out=None, stream=None, table=None):
-    """jpeg_crops_decoded over frames of different shapes and formats in one call (frames / pix_fmts / rects as in
-    jpeg_encode_crops_frames) -> (uint8 CUDA [K, Hmax, Wmax, 3], device int32 status [K]); crop k's slot and status are what
-    jpeg_crops_decoded gives for that crop of its frame alone.  Nothing waits.  table: a checked (frame_table, rects) pair
-    to reuse instead of checking again."""
-    if table is None:
-        t, sizes = frame_table(frames, pix_fmts)
-        if not sizes:
-            raise ValueError("a frame table needs at least one frame")
-        table = (t, table_rects(rects, sizes))
-    t, r = table
+def jpeg_crops_decoded_frames(table, rects, quality=95, out=None, stream=None):
+    """-> (uint8 CUDA [K, Hmax, Wmax, 3], device int32 status [K]): where the status is JPEG_OK, crop k's slot holds, in its
+    h x w corner, the pixels cv2.imdecode gives for the file jpeg_encode_crops_frames writes for it; JPEG_UNSUPPORTED
+    (coefficients outside the range where every libjpeg-turbo IDCT agrees) leaves the slot unwritten, for the caller to
+    decode that file with cv2.  Nothing waits."""
+    r = _rects_i32(rects)
     K = len(r)
-    dev = frames[0].device
     if out is None:
         hmax = max([int(y2 - y1) for _, _, y1, _, y2 in r] + [1])
         wmax = max([int(x2 - x1) for _, x1, _, x2, _ in r] + [1])
-        out = torch.zeros(K, hmax, wmax, 3, dtype=torch.uint8, device=dev)
-    args = (t, len(frames), r.ctypes.data, K, int(quality))
+        out = torch.zeros(K, hmax, wmax, 3, dtype=torch.uint8, device="cuda")
+    args = (table, len(table), r.ctypes.data, K, int(quality))
     need = ctypes.c_size_t(0)
     check(lib().cc_jpeg_crops_decoded_frames(*args, None, 0, 0, None, None, 0, ctypes.byref(need), None),
           "cc_jpeg_crops_decoded_frames")
-    ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=dev)
-    status = torch.empty(max(K, 1), dtype=torch.int32, device=dev)
+    ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=out.device)
+    status = torch.empty(max(K, 1), dtype=torch.int32, device=out.device)
     check(lib().cc_jpeg_crops_decoded_frames(*args, ptr(out), out.shape[1], out.shape[2], ptr(status), ptr(ws), ws.numel(), None,
                                              stream_ptr(stream)), "cc_jpeg_crops_decoded_frames")
     return out, status[:K]
-
-
-def jpeg_encode_crops(frames, rects, quality=95, src_fmt=1, stream=None):
-    """frames: uint8 CUDA [n,H,W,3] (src_fmt 0 RGB, 1 BGR) or [n,H*3/2,W] (2 I420); rects: K rows (frame, x1, y1, x2, y2)
-    -> list of K `bytes`, each the file cv2.imwrite writes for that crop at `quality`.  The crops go into one device buffer
-    at offsets given by the prefix sum of their bounds; only the lengths and then the used bytes come back to the host."""
-    n, H, W = _jpeg_frames(frames, src_fmt)
-    r = _rects_i32(rects)
-    K = len(r)
-    if K == 0:
-        return []
-    out, lengths, offsets = _jpeg_encode_launch("cc_jpeg_encode_crops", (ptr(frames), n, H, W, src_fmt, r.ctypes.data, K,
-                                                                         int(quality)), r, frames.device, stream)
-    return jpeg_collect(out, lengths, lengths.cpu().numpy(), offsets)
-
-
-def jpeg_coeffs(frames, rects, quality=95, src_fmt=1, stream=None):
-    """The quantised coefficients of every block of every crop: int16 CUDA [n_blocks, 64], zigzag order, crop by crop, MCU
-    by MCU (Y0 Y1 Y2 Y3 Cb Cr), dummy blocks included (oracle.jpeg.blocks of each crop, concatenated)."""
-    n, H, W = _jpeg_frames(frames, src_fmt)
-    r = _rects_i32(rects)
-    nb = ctypes.c_int64(0)
-    args = (ptr(frames), n, H, W, src_fmt, r.ctypes.data, len(r), int(quality))
-    check(lib().cc_jpeg_coeffs(*args, None, ctypes.byref(nb), None), "cc_jpeg_coeffs")
-    coef = torch.empty(nb.value, 64, dtype=torch.int16, device=frames.device)
-    check(lib().cc_jpeg_coeffs(*args, ptr(coef), ctypes.byref(nb), stream_ptr(stream)), "cc_jpeg_coeffs")
-    return coef
 
 
 # ---- JPEG files -> BGR pixels, pixel for pixel cv2.imdecode(buf, IMREAD_COLOR)
@@ -462,16 +440,31 @@ class JpegBatch:
             hmax = hmax or max([int(v) for v in self.sizes[ok, 1]] + [1])
             wmax = wmax or max([int(v) for v in self.sizes[ok, 0]] + [1])
             out = torch.zeros(self.K, hmax, wmax, 3, dtype=torch.uint8, device=self.dev.device)
-        assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.dim() == 4 and out.shape[0] >= self.K
         status = torch.empty(max(self.K, 1), dtype=torch.int32, device=self.dev.device)
-        d_data, h_table, d_table = self._ptrs()
+        args = (*self._ptrs(), self.K)
         need = ctypes.c_size_t(0)
-        check(lib().cc_jpeg_decode(d_data, h_table, d_table, self.K, None, 0, 0, None, ptr(coef), None, 0, ctypes.byref(need),
-                                   None), "cc_jpeg_decode")
+        check(lib().cc_jpeg_decode_frames(*args, None, None, ptr(coef), None, 0, ctypes.byref(need), None), "cc_jpeg_decode_frames")
         ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=self.dev.device)
-        check(lib().cc_jpeg_decode(d_data, h_table, d_table, self.K, ptr(out), out.shape[1], out.shape[2], ptr(status), ptr(coef),
-                                   ptr(ws), ws.numel(), None, stream_ptr(stream)), "cc_jpeg_decode")
+        check(lib().cc_jpeg_decode_frames(*args, self.dests(out), ptr(status), ptr(coef), ptr(ws), ws.numel(), None,
+                                          stream_ptr(stream)), "cc_jpeg_decode_frames")
         return out, status[:self.K]
+
+    def dests(self, out):
+        """The decode destinations of a padded batch out uint8 CUDA [>= K, Hmax, Wmax, 3]: image k (parse status OK) to
+        the h x w corner of slot k.  ValueError when an image does not fit its slot."""
+        import numpy as np
+        from ._lib import cc_jpeg_dest
+        assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.dim() == 4 and out.shape[0] >= self.K
+        K, (w, h) = self.K, self.sizes.T
+        ok = self.status == JPEG_OK                     # the other files' rows stay zero: the library does not read them
+        big = np.flatnonzero(ok & ((h > out.shape[1]) | (w > out.shape[2])))
+        if len(big):
+            k = big[0]
+            raise ValueError(f"image {k} ({w[k]}x{h[k]}) does not fit the {out.shape[2]}x{out.shape[1]} batch")
+        d = np.zeros(max(K, 1), _DEST_ROW)              # filled as one array, like batch_table
+        d["data"][:K] = np.where(ok, out.data_ptr() + out.stride(0) * np.arange(K, dtype=np.uint64), 0)
+        d["pitch"][:K], d["h"][:K], d["w"][:K] = out.stride(1), h, w
+        return (cc_jpeg_dest * len(d)).from_buffer(d)
 
 
 class JpegDecoder:
@@ -567,10 +560,10 @@ class JpegDecoder:
         h_table = ctypes.c_void_p(self._host.data_ptr() + self._table_off)
         args = (ctypes.c_void_p(base), h_table, ctypes.c_void_p(base + self._table_off), K)
         need = ctypes.c_size_t(0)
-        check(lib().cc_jpeg_decode_frames(*args, None, None, None, 0, ctypes.byref(need), None), "cc_jpeg_decode_frames")
+        check(lib().cc_jpeg_decode_frames(*args, None, None, None, None, 0, ctypes.byref(need), None), "cc_jpeg_decode_frames")
         self._ws = self._grow(self._ws, need.value, device=self.device)
         self._dev[:self._nbytes].copy_(self._host[:self._nbytes], non_blocking=True)
-        check(lib().cc_jpeg_decode_frames(*args, outs, ptr(self._st_dev), ptr(self._ws), self._ws.numel(), None,
+        check(lib().cc_jpeg_decode_frames(*args, outs, ptr(self._st_dev), None, ptr(self._ws), self._ws.numel(), None,
                                           stream_ptr(stream)), "cc_jpeg_decode_frames")
         st = self._st_host[:K]
         st.copy_(self._st_dev[:K], non_blocking=True)
@@ -593,25 +586,3 @@ def jpeg_decode_coeffs(files, stream=None):
     coef = torch.zeros(max(int(b.blocks.sum()), 1), 64, dtype=torch.int16, device=b.dev.device)
     _, st = b.decode(coef=coef, stream=stream)
     return coef[:int(b.blocks.sum())], st
-
-
-def jpeg_crops_decoded(frames, rects, quality=95, src_fmt=1, out=None, stream=None):
-    """frames / rects / quality / src_fmt as in jpeg_encode_crops -> (uint8 CUDA [K, Hmax, Wmax, 3], device int32 status [K]):
-    where the status is JPEG_OK, crop k's slot holds, in its h x w corner, the pixels cv2.imdecode gives for the file
-    jpeg_encode_crops writes for it; JPEG_UNSUPPORTED (coefficients outside the range where every libjpeg-turbo IDCT agrees)
-    leaves the slot unwritten, for the caller to decode that file with cv2."""
-    n, H, W = _jpeg_frames(frames, src_fmt)
-    r = _rects_i32(rects)
-    K = len(r)
-    if out is None:
-        hmax = max([int(y2 - y1) for _, _, y1, _, y2 in r] + [1])
-        wmax = max([int(x2 - x1) for _, x1, _, x2, _ in r] + [1])
-        out = torch.zeros(K, hmax, wmax, 3, dtype=torch.uint8, device=frames.device)
-    args = (ptr(frames), n, H, W, src_fmt, r.ctypes.data, K, int(quality))
-    need = ctypes.c_size_t(0)
-    check(lib().cc_jpeg_crops_decoded(*args, None, 0, 0, None, None, 0, ctypes.byref(need), None), "cc_jpeg_crops_decoded")
-    ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=frames.device)
-    status = torch.empty(max(K, 1), dtype=torch.int32, device=frames.device)
-    check(lib().cc_jpeg_crops_decoded(*args, ptr(out), out.shape[1], out.shape[2], ptr(status), ptr(ws), ws.numel(), None,
-                                      stream_ptr(stream)), "cc_jpeg_crops_decoded")
-    return out, status[:K]

@@ -17,8 +17,8 @@ BGR24, YUV420P, MJPEG = "bgr24", "yuv420p", "mjpeg"
 PIX_FMTS = (BGR24, YUV420P)
 CAMERA_PIX_FMTS = PIX_FMTS + (MJPEG,)
 
-# frame_fmt codes of the C-ABI (include/clearcam_b200.h)
-CC_FRAME_BGR_U8, CC_FRAME_BGR_F32, CC_FRAME_I420_U8 = 0, 1, 2
+# frame_fmt codes of the C-ABI (include/clearcam_b200.h); RGB frames are taken by the crop entry points only
+CC_FRAME_BGR_U8, CC_FRAME_BGR_F32, CC_FRAME_I420_U8, CC_FRAME_RGB_U8 = 0, 1, 2, 3
 
 
 def check_pix_fmt(pix_fmt) -> str:

@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define CC_ABI_VERSION 3
+#define CC_ABI_VERSION 4
 
 int cc_version(void);
 const char* cc_last_error(void);
@@ -120,11 +120,15 @@ int cc_yolo_destroy(cc_yolo* h);
  *   CC_FRAME_BGR_F32 [B,Hf,Wf,3] HWC BGR float32 (test/run_mot.py:33);
  *   CC_FRAME_I420_U8 [B,Hf*3/2,Wf] uint8 planar YUV 4:2:0 (ffmpeg -pix_fmt yuv420p, OpenCV I420): the Y plane Hf x Wf, then
  *                    U and V, each (Hf/2) x (Wf/2); Hf and Wf must be even.  Converted to BGR on the device exactly as
- *                    cv2.cvtColor(yuv, COLOR_YUV2BGR_I420) does (BT.601 limited range, 20-bit fixed point, nearest chroma).
+ *                    cv2.cvtColor(yuv, COLOR_YUV2BGR_I420) does (BT.601 limited range, 20-bit fixed point, nearest chroma);
+ *   CC_FRAME_RGB_U8  [h,w,3] HWC RGB uint8, in the frame tables of the crop entry points only (cc_clip_preprocess_frames,
+ *                    cc_jpeg_encode_crops_frames, cc_jpeg_coeffs_frames, cc_jpeg_crops_decoded_frames); every other entry
+ *                    point refuses it.
  * Any other code, or an odd Hf / Wf with I420, fails with CC_ERR_INVALID before anything is launched. */
 #define CC_FRAME_BGR_U8 0
 #define CC_FRAME_BGR_F32 1
 #define CC_FRAME_I420_U8 2
+#define CC_FRAME_RGB_U8 3
 
 /* YOLOv9.__call__ (detection/yolov9.py:375-388) for a batch of same-shape frames.
  * d_frames: B frames of format frame_fmt, Hf x Wf pixels each.
@@ -146,8 +150,8 @@ typedef struct { const void* data; int fmt; int h; int w; } cc_frame;
 int cc_yolo_net_shape(int frame_fmt, int Hf, int Wf, int res, int* net_h, int* net_w);
 /* cc_yolo_forward over a table of B frames (HOST array, read during the call only) that share one net shape; row b of
  * d_out [B,300,6] is frame b's detections in its own pixels, as cc_yolo_forward of a batch of frames of its shape and
- * format would give it at that row.  d_raw: optional [B,84,A] head tap.  Mixed net shapes, CC_FRAME_BGR_F32 frames, odd
- * I420 sides, no frame at all or B > CC_MAX_FRAMES fail with CC_ERR_INVALID before anything is launched.  Plans are
+ * format would give it at that row.  d_raw: optional [B,84,A] head tap.  Mixed net shapes, CC_FRAME_BGR_F32 or
+ * CC_FRAME_RGB_U8 frames, odd I420 sides, no frame at all or B > CC_MAX_FRAMES fail with CC_ERR_INVALID before anything is launched.  Plans are
  * cached per (B, net shape, res); the letterbox and the postprocess take the table as a kernel parameter on every call and
  * the CUDA graph covers the launches between them, so a different table every call still replays the graph. */
 int cc_yolo_forward_frames(cc_yolo* h, const cc_frame* frames, int B, int res, float* d_out, float* d_raw, void* stream);
@@ -418,47 +422,41 @@ int cc_search_scores(const float* d_index, int N, int D, const float* d_q, int Q
 int cc_search_topk(const float* d_index, int N, int D, const float* d_q, const int32_t* d_group, const uint8_t* d_mask, int G, int k,
                    void* d_workspace, int32_t* d_rows, float* d_scores, void* stream);
 
-/* Crop + ObjectFinder.preprocess on the device, for objects cut out of frames already resident for the detector:
+/* Object crops of device frames.  frames: HOST array of n_frames cc_frame rows (read during the call only) of any shapes,
+ * CC_FRAME_BGR_U8, CC_FRAME_RGB_U8 or CC_FRAME_I420_U8 (h, w even); rects: HOST int32 [K,5] = frame, x1, y1, x2, y2 in
+ * pixels, r[0] indexing the table and the rect lying inside its own frame (validated, passed as kernel arguments: no copy,
+ * no sync).  A batch of n frames of one shape and format is n rows.  Crop k of any output is what the same call gives for
+ * that crop alone.  A NULL frame, another format, an odd I420 side or a rect that is empty or outside its own frame fails
+ * with CC_ERR_INVALID before anything is launched.
+ *
+ * Crop + ObjectFinder.preprocess on the device, for objects cut out of frames already resident for the detector:
  * frame[y1:y2, x1:x2] (clearcam.py:396) -> RGB (models/objects.py:249) -> cv2.resize((size,size), INTER_CUBIC) -> /255 ->
- * (x-0.5)/0.5 -> CHW (models/objects.py:237-242).  src_fmt: 0 = d_frames is uint8 RGB [n_frames,H,W,3], taken as is;
- * 1 = uint8 BGR [n_frames,H,W,3], channels swapped; 2 = I420 [n_frames,H*3/2,W] (H, W even), converted as
- * cv2.cvtColor(frame, COLOR_YUV2RGB_I420) and then cropped.  rects: HOST int32 [K,5] = frame, x1, y1, x2, y2 in pixels
- * (validated, passed as kernel arguments: no copy, no sync); d_out: device float32 [K,3,size,size] — the tensor
- * cc_clip_encode_image takes. */
-int cc_clip_preprocess(const uint8_t* d_frames, int n_frames, int H, int W, const int32_t* rects, int K, int size,
-                       int src_fmt, float* d_out, void* stream);
-/* The same over a frame table: frames (HOST array of n_frames cc_frame rows, read during the call only) of any shapes,
- * CC_FRAME_BGR_U8 or CC_FRAME_I420_U8 (h, w even); rect r[0] indexes the table and must lie inside its own frame.  Crop k
- * of the output is what cc_clip_preprocess gives for that crop called on its frame alone.  A NULL frame, another format,
- * an odd I420 side or a rect outside its own frame fails with CC_ERR_INVALID before anything is launched. */
+ * (x-0.5)/0.5 -> CHW (models/objects.py:237-242).  An RGB frame is taken as is, a BGR frame has its channels swapped, an
+ * I420 frame is converted as cv2.cvtColor(frame, COLOR_YUV2RGB_I420) and then cropped.  d_out: device float32
+ * [K,3,size,size] — the tensor cc_clip_encode_image takes. */
 int cc_clip_preprocess_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int size, float* d_out,
                               void* stream);
 
 /* Object thumbnails on the device: baseline JPEG of frame crops, byte for byte the file cv2.imwrite(path, crop) writes at
  * IMWRITE_JPEG_QUALITY `quality` (`VideoCapture.save_object`, clearcam.py:373-399): 4:2:0, integer DCT, Annex K tables,
- * JFIF 1.01 header; oracle/jpeg.py states the arithmetic.  d_frames, n_frames, H, W, src_fmt and the HOST rects [K,5]
- * (frame, x1, y1, x2, y2) are as in cc_clip_preprocess; the crop is encoded as the BGR image cv2 would see (RGB frames are
- * swapped, I420 frames converted as cv2.cvtColor(COLOR_YUV2BGR_I420) and then cropped).  quality: 0..100 (0 acts as 1).
+ * JFIF 1.01 header; oracle/jpeg.py states the arithmetic.  frames and rects as above; the crop is encoded as the BGR image
+ * cv2 would see (RGB frames are swapped, I420 frames converted as cv2.cvtColor(COLOR_YUV2BGR_I420) and then cropped).
+ * quality: 0..100 (0 acts as 1); a crop side over 65535 fails.
  * cc_jpeg_bound: worst-case bytes of one encoded w x h crop (every code at its longest, every byte stuffed, headers, EOI).
- * cc_jpeg_encode_crops: crop k is written to d_out + out_offsets[k] (HOST int64 [K]; each region [offset, offset +
+ * cc_jpeg_encode_crops_frames: crop k is written to d_out + out_offsets[k] (HOST int64 [K]; each region [offset, offset +
  * cc_jpeg_bound) inside the out_bytes of d_out, none overlapping: the prefix sum of the bounds needs no sync) and its
  * length to d_lengths[k] (device int64 [K]).  d_workspace: *ws_needed bytes of device scratch, 256-byte aligned.
  * d_out == NULL only writes *ws_needed.  Nothing is allocated and nothing synchronises; a bad argument fails with
  * CC_ERR_INVALID before anything is launched.
- * cc_jpeg_coeffs (parity tap): the quantised coefficients of every 8x8 block of every crop, int16 [n_blocks][64] in zigzag
- * order: crop by crop, MCU by MCU (Y0 Y1 Y2 Y3 Cb Cr), dummy blocks included.  d_coef == NULL only writes *n_blocks. */
+ * cc_jpeg_coeffs_frames (parity tap): the quantised coefficients of every 8x8 block of every crop, int16 [n_blocks][64]
+ * in zigzag order: crop by crop, MCU by MCU (Y0 Y1 Y2 Y3 Cb Cr), dummy blocks included.  d_coef == NULL only writes
+ * *n_blocks; otherwise d_coef is 4-byte aligned. */
 int cc_jpeg_bound(int w, int h, int64_t* bytes);
-int cc_jpeg_encode_crops(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K, int quality,
-                         uint8_t* d_out, int64_t out_bytes, const int64_t* out_offsets, int64_t* d_lengths, void* d_workspace,
-                         size_t ws_bytes, size_t* ws_needed, void* stream);
-int cc_jpeg_coeffs(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K, int quality,
-                   int16_t* d_coef, int64_t* n_blocks, void* stream);
-/* cc_jpeg_encode_crops over a frame table (cc_clip_preprocess_frames' rules for frames and rects): one call encodes the
- * crops of frames of different shapes and formats, crop k's bytes and length being what cc_jpeg_encode_crops gives for
- * that crop called on its frame alone. */
 int cc_jpeg_encode_crops_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int quality, uint8_t* d_out,
                                 int64_t out_bytes, const int64_t* out_offsets, int64_t* d_lengths, void* d_workspace,
                                 size_t ws_bytes, size_t* ws_needed, void* stream);
+int cc_jpeg_coeffs_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int quality, int16_t* d_coef,
+                          int64_t* n_blocks, void* stream);
 
 /* JPEG files -> BGR uint8 on the device, pixel for pixel what cv2.imdecode(buf, IMREAD_COLOR) returns (libjpeg-turbo 3.1:
  * islow IDCT, fancy upsampling, table-driven YCbCr -> BGR); oracle/jpeg_decode.py states the arithmetic.  Replaces the host
@@ -475,43 +473,33 @@ int cc_jpeg_encode_crops_frames(const cc_frame* frames, int n_frames, const int3
  * h_table (K entries, 16-byte aligned), h_sizes [K,2] = width, height (0 where the header did not say), h_status [K] and
  * h_blocks [K] (8x8 blocks of each decoded image, 0 for the others).  A file never makes it fail; the entries also place
  * each image's intermediates in the workspace, so a table belongs to its own set of K files.
- * cc_jpeg_decode: d_data holds the same bytes as h_data and d_table the same bytes as h_table.  Image k (status OK) is
- * written to d_out [K, Hmax, Wmax, 3] rows 0..h-1, columns 0..w-1 of slot k; no other byte of d_out is written.  d_status
- * [K] (device int32) receives the final status: the parse status, or CC_JPEG_CORRUPT / CC_JPEG_UNSUPPORTED found on the
- * device, in which case that image's region is left as it was and the other images are unaffected.  d_coef: NULL, or
- * device int16 [sum of h_blocks][64] that receives the dequantisation input (zigzag order, block by block in scan order,
- * image after image): the coefficient tap.  d_workspace: *ws_needed bytes of device scratch, 256-byte aligned; d_out ==
- * NULL only writes *ws_needed.  Nothing is allocated and nothing synchronises; a bad argument fails with CC_ERR_INVALID
- * before anything is launched.
- * cc_jpeg_crops_decoded: for the crops of cc_jpeg_encode_crops (same frames, rects and quality), the pixels
+ * cc_jpeg_decode_frames: d_data holds the same bytes as h_data and d_table the same bytes as h_table.  outs (HOST [K],
+ * read during the call only): image k, when its status is OK, is written as BGR uint8 [h, w, 3] at outs[k].data (device),
+ * rows outs[k].pitch bytes apart, e.g. a device frame buffer a detector call reads, or slot k of a padded batch [K, Hmax,
+ * Wmax, 3] (pitch 3 Wmax); nothing else is written.  d_status [K] (device int32) receives the final status: the parse
+ * status, or CC_JPEG_CORRUPT / CC_JPEG_UNSUPPORTED found on the device, in which case that image's destination is left as
+ * it was and the other images are unaffected.  d_coef: NULL, or device int16 [sum of h_blocks][64], 16-byte aligned, that
+ * receives the dequantisation input (zigzag order, block by block in scan order, image after image): the coefficient tap.
+ * d_workspace: *ws_needed bytes of device scratch, 256-byte aligned; outs == NULL only writes *ws_needed (which depends
+ * on whether d_coef is NULL).  Nothing is allocated and nothing synchronises; a bad argument fails with CC_ERR_INVALID
+ * before anything is launched, among them a parsed image whose destination is NULL, is not the image's h x w, has a pitch
+ * below 3 w or overlaps another such destination; the destinations of images the parse did not accept are not read.
+ * cc_jpeg_crops_decoded_frames: for the crops of cc_jpeg_encode_crops_frames (same frames, rects and quality), the pixels
  * cv2.imdecode(cv2.imencode(".jpg", crop, quality)) gives: the encoder's transform, then the decoder's reconstruction, with
- * no entropy coding between them (the coefficients are the file's content).  Crop k goes to slot k of d_out [K, Hmax,
- * Wmax, 3] as above, and d_status [K] (device int32) gets CC_JPEG_OK, or CC_JPEG_UNSUPPORTED where the coefficients leave
- * the range in which every libjpeg-turbo IDCT agrees (that slot is then not written; decode the file with cv2).
- * Workspace as above. */
+ * no entropy coding between them (the coefficients are the file's content).  Crop k goes to rows 0..h-1, columns 0..w-1 of
+ * slot k of d_out [K, Hmax, Wmax, 3], and d_status [K] (device int32) gets CC_JPEG_OK, or CC_JPEG_UNSUPPORTED where the
+ * coefficients leave the range in which every libjpeg-turbo IDCT agrees (that slot is then not written; decode the file
+ * with cv2).  d_out == NULL only writes *ws_needed; workspace as above. */
 #define CC_JPEG_OK 0
 #define CC_JPEG_UNSUPPORTED 1
 #define CC_JPEG_CORRUPT 2
 size_t cc_jpeg_table_bytes(void);
 int cc_jpeg_parse(const uint8_t* h_data, int64_t data_bytes, const int64_t* offsets, const int64_t* lengths, int K, void* h_table,
                   int32_t* h_sizes, int32_t* h_status, int64_t* h_blocks);
-int cc_jpeg_decode(const uint8_t* d_data, const void* h_table, const void* d_table, int K, uint8_t* d_out, int Hmax, int Wmax,
-                   int32_t* d_status, int16_t* d_coef, void* d_workspace, size_t ws_bytes, size_t* ws_needed, void* stream);
-/* cc_jpeg_decode_frames: cc_jpeg_decode into caller-given destinations rather than one padded batch, e.g. the device
- * frame buffers a detector call reads.  outs (HOST [K], read during the call only): image k, when its status is OK, is
- * written as BGR uint8 [h, w, 3] at outs[k].data (device), rows outs[k].pitch bytes apart; nothing else is written, and an
- * image that fails on the device leaves its destination as it was.  Fails with CC_ERR_INVALID before any launch when the
- * destination of a parsed image is NULL, its h x w is not the image's, its pitch is below 3 w, or two such destinations
- * overlap; the destinations of images the parse did not accept are not read.  outs == NULL only writes *ws_needed.
- * Statuses, workspace and stream as for cc_jpeg_decode. */
 typedef struct { void* data; int64_t pitch; int32_t h; int32_t w; } cc_jpeg_dest;
 int cc_jpeg_decode_frames(const uint8_t* d_data, const void* h_table, const void* d_table, int K, const cc_jpeg_dest* outs,
-                          int32_t* d_status, void* d_workspace, size_t ws_bytes, size_t* ws_needed, void* stream);
-int cc_jpeg_crops_decoded(const uint8_t* d_frames, int n_frames, int H, int W, int src_fmt, const int32_t* rects, int K, int quality,
-                          uint8_t* d_out, int Hmax, int Wmax, int32_t* d_status, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
+                          int32_t* d_status, int16_t* d_coef, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
                           void* stream);
-/* cc_jpeg_crops_decoded over a frame table (cc_clip_preprocess_frames' rules): crop k's pixels and status are what
- * cc_jpeg_crops_decoded gives for that crop called on its frame alone. */
 int cc_jpeg_crops_decoded_frames(const cc_frame* frames, int n_frames, const int32_t* rects, int K, int quality, uint8_t* d_out,
                                  int Hmax, int Wmax, int32_t* d_status, void* d_workspace, size_t ws_bytes, size_t* ws_needed,
                                  void* stream);

@@ -167,7 +167,7 @@ def test_device_topk_search_equals_the_reference_loop(tmp_path):
 
 # ------------------------------------------------------------------------------------------------ crop -> CLIP input
 def test_device_crop_preprocess_bit_exact():
-    """cc_clip_preprocess == crop + cvtColor + ObjectFinder.preprocess with OpenCV's bicubic (oracle pinned to cv2)."""
+    """cc_clip_preprocess_frames == crop + cvtColor + ObjectFinder.preprocess with OpenCV's bicubic (oracle pinned to cv2)."""
     from pathlib import Path
     from oracle import clip_preprocess as cp
     g = np.load(Path(__file__).parent / "golden" / "clip_preprocess.npz")

@@ -175,6 +175,8 @@ def test_argument_errors(det, P):
     out = torch.empty(2 * 896 * 17, device="cuda")
     t1 = (cc_frame * 1)(cc_frame(img.data_ptr(), 2, 64, 64))                 # I420 is not taken
     assert L.cc_blazeface_forward(det._h, t1, 1, ptr(out), ptr(out), ptr(out), stream_ptr()) != 0
+    t3 = (cc_frame * 1)(cc_frame(img.data_ptr(), 3, 64, 64))                 # nor RGB, which only the crops take
+    assert L.cc_blazeface_forward(det._h, t3, 1, ptr(out), ptr(out), ptr(out), stream_ptr()) != 0
     t0 = (cc_frame * 1)(cc_frame(None, 0, 64, 64))
     assert L.cc_blazeface_forward(det._h, t0, 1, ptr(out), ptr(out), ptr(out), stream_ptr()) != 0
     fresh = BlazeFace({k: v.numpy() for k, v in P.items()})                 # no workspace set

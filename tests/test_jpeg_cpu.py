@@ -123,9 +123,9 @@ def test_each_usual_mistake_changes_some_bytes(variant):
 
 
 # ------------------------------------------------------------------------------------------------ argument checks
-def test_jpeg_entry_points_reject_bad_arguments():
+def test_jpeg_table_entry_points_reject_bad_arguments():
     """Every check runs before anything is launched: the device pointers below are never dereferenced."""
-    from clearcam_b200._lib import lib
+    from clearcam_b200._lib import cc_frame, lib
     h = lib()
     fake = ctypes.c_void_p(1 << 20)
     b = ctypes.c_int64(0)
@@ -145,21 +145,30 @@ def test_jpeg_entry_points_reject_bad_arguments():
     offs = np.array([0, bounds[0]], np.int64)
     cap = sum(bounds)
 
-    def enc(frames=fake, n=2, H=240, W=320, fmt=1, r=rects, K=2, q=95, out=fake, cap=cap, offsets=offs, lengths=fake, ws=fake,
+    def table(n, H, W, fmt):
+        step = H * 3 // 2 * W if fmt == 2 else H * W * 3
+        return (cc_frame * max(n, 1))(*[cc_frame(fake.value + i * step, fmt, H, W) for i in range(n)])
+
+    def enc(frames=fake, n=2, H=240, W=320, fmt=0, r=rects, K=2, q=95, out=fake, cap=cap, offsets=offs, lengths=fake, ws=fake,
             wsb=1 << 30, need=ctypes.byref(need)):
-        return h.cc_jpeg_encode_crops(frames, n, H, W, fmt, None if r is None else r.ctypes.data, K, q, out, cap,
-                                      None if offsets is None else offsets.ctypes.data, lengths, ws, wsb, need, None)
+        return h.cc_jpeg_encode_crops_frames(frames and table(n, H, W, fmt), n, None if r is None else r.ctypes.data, K, q, out,
+                                             cap, None if offsets is None else offsets.ctypes.data, lengths, ws, wsb, need, None)
 
     assert enc(out=None) == 0 and need.value > 0
-    refused(enc(frames=None), "cc_jpeg_encode_crops", "null pointer")
-    refused(enc(r=None), "cc_jpeg_encode_crops", "null pointer")
-    refused(enc(n=0), "cc_jpeg_encode_crops", "bad sizes")
-    refused(enc(fmt=3), "cc_jpeg_encode_crops", "unknown source format 3")
-    refused(enc(fmt=-1), "cc_jpeg_encode_crops", "unknown source format")
-    refused(enc(fmt=2, H=241), "cc_jpeg_encode_crops", "even height and width")
-    refused(enc(fmt=2, W=321), "cc_jpeg_encode_crops", "even height and width")
-    refused(enc(q=-1), "cc_jpeg_encode_crops", "quality -1")
-    refused(enc(q=101), "cc_jpeg_encode_crops", "quality 101")
+    for fmt in (0, 2, 3):                                             # BGR, I420 and RGB frames
+        assert enc(fmt=fmt, out=None) == 0
+    refused(enc(frames=None), "cc_jpeg_encode_crops_frames", "null pointer")
+    refused(enc(r=None), "cc_jpeg_encode_crops_frames", "null pointer")
+    refused(enc(n=0), "cc_jpeg_encode_crops_frames", "bad sizes")
+    refused(enc(K=-1), "cc_jpeg_encode_crops_frames", "bad sizes")
+    refused(enc(fmt=4), "cc_jpeg_encode_crops_frames", "unknown source format 4")
+    refused(enc(fmt=1), "cc_jpeg_encode_crops_frames", "unknown source format 1")      # CC_FRAME_BGR_F32
+    refused(enc(fmt=-1), "cc_jpeg_encode_crops_frames", "unknown source format")
+    refused(enc(H=0), "cc_jpeg_encode_crops_frames", "bad size")
+    refused(enc(fmt=2, H=241), "cc_jpeg_encode_crops_frames", "even height and width")
+    refused(enc(fmt=2, W=321), "cc_jpeg_encode_crops_frames", "even height and width")
+    refused(enc(q=-1), "cc_jpeg_encode_crops_frames", "quality -1")
+    refused(enc(q=101), "cc_jpeg_encode_crops_frames", "quality 101")
     refused(enc(r=np.array([[0, 5, 5, 5, 9], [1, 10, 10, 50, 50]], np.int32)), "rect 0", "empty or outside")
     refused(enc(r=np.array([[0, 0, 0, 100, 80], [1, 10, 10, 321, 50]], np.int32)), "rect 1", "empty or outside")
     refused(enc(r=np.array([[0, 0, 0, 100, 80], [2, 10, 10, 50, 50]], np.int32)), "rect 1", "frame 2")
@@ -175,13 +184,15 @@ def test_jpeg_entry_points_reject_bad_arguments():
     refused(enc(offsets=np.array([-1, bounds[0]], np.int64)), "crop 0", "exceeds")
     assert enc(offsets=np.array([bounds[1], 0], np.int64), cap=cap, out=None) == 0      # query ignores the offsets
 
-    def coef(fmt=1, H=240, q=95, d=fake, nb=ctypes.byref(b)):
-        return h.cc_jpeg_coeffs(fake, 2, H, 320, fmt, rects.ctypes.data, 2, q, d, nb, None)
+    def coef(fmt=0, H=240, q=95, r=rects, d=fake, nb=ctypes.byref(b)):
+        return h.cc_jpeg_coeffs_frames(table(2, H, 320, fmt), 2, r.ctypes.data, len(r), q, d, nb, None)
 
     assert coef(d=None) == 0
     g = [oj.geometry(100, 80), oj.geometry(40, 40)]
     assert b.value == sum(6 * x["mw"] * x["mh"] for x in g)
-    refused(coef(fmt=7), "cc_jpeg_coeffs", "unknown source format 7")
-    refused(coef(fmt=2, H=239), "cc_jpeg_coeffs", "even height")
-    refused(coef(q=200), "cc_jpeg_coeffs", "quality 200")
-    refused(coef(d=ctypes.c_void_p((1 << 20) + 2)), "cc_jpeg_coeffs", "4-byte aligned")
+    assert coef(fmt=3, d=None) == 0 and b.value == sum(6 * x["mw"] * x["mh"] for x in g)
+    refused(coef(fmt=7), "cc_jpeg_coeffs_frames", "unknown source format 7")
+    refused(coef(fmt=2, H=239), "cc_jpeg_coeffs_frames", "even height")
+    refused(coef(q=200), "cc_jpeg_coeffs_frames", "quality 200")
+    refused(coef(r=np.array([[0, 0, 0, 321, 80]], np.int32)), "cc_jpeg_coeffs_frames", "rect 0", "empty or outside")
+    refused(coef(d=ctypes.c_void_p((1 << 20) + 2)), "cc_jpeg_coeffs_frames", "4-byte aligned")

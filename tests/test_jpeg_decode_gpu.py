@@ -11,7 +11,8 @@ import torch
 
 from oracle import jpeg_decode as od
 from clearcam_b200 import ops
-from clearcam_b200._lib import lib, ptr, stream_ptr
+from clearcam_b200._lib import cc_jpeg_dest, lib, ptr, stream_ptr
+from clearcam_b200.pixfmt import CC_FRAME_BGR_U8 as BGR, CC_FRAME_I420_U8 as I420, CC_FRAME_RGB_U8 as RGB
 
 pytestmark = pytest.mark.gpu
 
@@ -142,16 +143,17 @@ def test_unsupported_and_corrupt_are_reported_and_do_not_disturb_the_others():
         assert od.decode(f)[0] == s
 
 
-def test_coefficient_tap_equals_the_encoders_coefficients():
+def test_decode_coefficient_tap_equals_the_table_encoders_coefficients():
     cv2 = _cv2()
     fr = _img(240, 320, 12)
     rects = [(0, 0, 0, 320, 240), (0, 3, 5, 40, 22), (0, 311, 231, 320, 240), (0, 17, 1, 18, 2), (0, 100, 50, 250, 200)]
     dev = torch.from_numpy(fr[None]).cuda()
+    table = ops.batch_table(dev, BGR)
     for q in (95, 20):
-        files = ops.jpeg_encode_crops(dev, rects, q, 1)
+        files = ops.jpeg_collect(*ops.jpeg_encode_crops_frames(table, rects, q))
         got, st = ops.jpeg_decode_coeffs(files)
         assert (st.cpu().numpy() == 0).all()
-        assert torch.equal(got, ops.jpeg_coeffs(dev, rects, q, 1)), q
+        assert torch.equal(got, ops.jpeg_coeffs_frames(table, rects, q)), q
         assert np.array_equal(got.cpu().numpy(), np.concatenate([od.coeffs(f) for f in files]))
     del cv2
 
@@ -161,15 +163,16 @@ _RECTS = [(0, 1, 3, 201, 157), (1, 1719, 881, 1920, 1080), (0, 0, 0, 1920, 1080)
 
 
 @pytest.mark.parametrize("q", [95, 60, 2])
-def test_crops_decoded_equal_imdecode_of_encode_crops(q):
+def test_table_crops_decoded_equal_imdecode_of_table_encoder(q):
     cv2 = _cv2()
     bgr = np.stack([_img(1080, 1920, 20), _img(1080, 1920, 21)])
     rgb = np.ascontiguousarray(bgr[..., ::-1])
     yuv = np.stack([cv2.cvtColor(f, cv2.COLOR_BGR2YUV_I420) for f in bgr])
-    for src, fmt in ((bgr, 1), (rgb, 0), (yuv, 2)):
+    for src, fmt in ((bgr, BGR), (rgb, RGB), (yuv, I420)):
         dev = torch.from_numpy(src).cuda()
-        files = ops.jpeg_encode_crops(dev, _RECTS, q, fmt)
-        pix, st = ops.jpeg_crops_decoded(dev, _RECTS, q, fmt)
+        table = ops.batch_table(dev, fmt)
+        files = ops.jpeg_collect(*ops.jpeg_encode_crops_frames(table, _RECTS, q))
+        pix, st = ops.jpeg_crops_decoded_frames(table, _RECTS, q)
         pix, st = pix.cpu().numpy(), st.cpu().numpy()
         for k, (f, x1, y1, x2, y2) in enumerate(_RECTS):
             # a crop is left to cv2 exactly where the decoder of its file would leave it (the IDCT range check)
@@ -178,7 +181,7 @@ def test_crops_decoded_equal_imdecode_of_encode_crops(q):
                 assert np.array_equal(pix[k, :y2 - y1, :x2 - x1], _imdecode(files[k])), (fmt, k)
 
 
-def test_crops_decoded_200_in_one_call():
+def test_table_crops_decoded_200_in_one_call():
     fr = np.stack([_img(540, 960, 30 + i) for i in range(4)])
     rng = np.random.default_rng(31)
     rects = []
@@ -187,8 +190,9 @@ def test_crops_decoded_200_in_one_call():
         x, y = int(rng.integers(0, 960 - w + 1)), int(rng.integers(0, 540 - h + 1))
         rects.append((int(rng.integers(0, 4)), x, y, x + w, y + h))
     dev = torch.from_numpy(fr).cuda()
-    files = ops.jpeg_encode_crops(dev, rects, 95, 1)
-    pix, st = ops.jpeg_crops_decoded(dev, rects, 95, 1)
+    table = ops.batch_table(dev, BGR)
+    files = ops.jpeg_collect(*ops.jpeg_encode_crops_frames(table, rects, 95))
+    pix, st = ops.jpeg_crops_decoded_frames(table, rects, 95)
     assert (st.cpu().numpy() == 0).all()
     pix = pix.cpu().numpy()
     for k, (f, x1, y1, x2, y2) in enumerate(rects):
@@ -246,7 +250,7 @@ def test_embed_images_equals_preprocess_clip(tmp_path, monkeypatch):
         of.embed_images(["/cam/objects/missing.jpg"])
 
 
-def test_bad_arguments_fail_before_any_launch():
+def test_decode_and_crops_decoded_tables_refuse_bad_arguments_before_any_launch():
     L = lib()
     f = _enc(_img(20, 30, 60), 90)
     b = ops.JpegBatch([f])
@@ -254,28 +258,35 @@ def test_bad_arguments_fail_before_any_launch():
     out = torch.zeros(1, 20, 30, 3, dtype=torch.uint8, device="cuda")
     st = torch.zeros(1, dtype=torch.int32, device="cuda")
     need = ctypes.c_size_t(0)
-    assert L.cc_jpeg_decode(d_data, h_table, d_table, 1, None, 0, 0, None, None, None, 0, ctypes.byref(need), None) == 0
+    assert L.cc_jpeg_decode_frames(d_data, h_table, d_table, 1, None, None, None, None, 0, ctypes.byref(need), None) == 0
     ws = torch.empty(need.value, dtype=torch.uint8, device="cuda")
-    args = lambda **k: [k.get("data", d_data), h_table, k.get("table", d_table), 1, ptr(k.get("out", out)), k.get("H", 20),
-                        k.get("W", 30), ptr(st), None, ptr(ws), k.get("ws", need.value), None, stream_ptr()]   # noqa: E731
-    assert L.cc_jpeg_decode(*args()) == 0
-    assert L.cc_jpeg_decode(*args(H=19)) == -1                      # the image does not fit the batch
-    assert L.cc_jpeg_decode(*args(ws=need.value - 1)) == -1         # workspace too small
-    assert L.cc_jpeg_decode(*args(data=None)) == -1
-    assert L.cc_jpeg_decode(*args(W=0)) == -1
+
+    def args(H=20, W=30, data=d_data, coef=None, ws_bytes=need.value):     # slot 0 of an H x W batch
+        dest = (cc_jpeg_dest * 1)(cc_jpeg_dest(out.data_ptr(), 3 * W, H, W))
+        return [data, h_table, d_table, 1, dest, ptr(st), coef, ptr(ws), ws_bytes, None, stream_ptr()]
+    assert L.cc_jpeg_decode_frames(*args()) == 0
+    assert L.cc_jpeg_decode_frames(*args(H=19)) == -1                # the image does not fit the batch
+    assert L.cc_jpeg_decode_frames(*args(ws_bytes=need.value - 1)) == -1          # workspace too small
+    assert L.cc_jpeg_decode_frames(*args(data=None)) == -1
+    assert L.cc_jpeg_decode_frames(*args(W=0)) == -1
+    assert L.cc_jpeg_decode_frames(*args(coef=ctypes.c_void_p(ws.data_ptr() + 8))) == -1     # coefficient tap not 16-byte aligned
+    with pytest.raises(ValueError):
+        b.decode(hmax=19)
     data = np.frombuffer(f, np.uint8).copy()
     assert L.cc_jpeg_parse(data.ctypes.data, len(f) - 1, np.array([0], np.int64).ctypes.data,
                            np.array([len(f)], np.int64).ctypes.data, 1, ctypes.c_void_p(b.host.data_ptr() + b.table_off),
                            np.zeros(2, np.int32).ctypes.data, np.zeros(1, np.int32).ctypes.data,
                            np.zeros(1, np.int64).ctypes.data) == -1   # file outside the data
     dev = torch.from_numpy(_img(40, 40, 61)[None]).cuda()
+    t = ops.batch_table(dev, BGR)
     r = np.array([(0, 0, 0, 40, 40)], np.int32)
-    assert L.cc_jpeg_crops_decoded(ptr(dev), 1, 40, 40, 1, r.ctypes.data, 1, 95, ptr(out), 20, 30, ptr(st), ptr(ws), 1 << 30, None,
-                                   stream_ptr()) == -1               # the crop does not fit the batch
+    assert L.cc_jpeg_crops_decoded_frames(t, 1, r.ctypes.data, 1, 95, ptr(out), 20, 30, ptr(st), ptr(ws), 1 << 30, None,
+                                          stream_ptr()) == -1        # the crop does not fit the batch
     big = torch.zeros(1, 40, 40, 3, dtype=torch.uint8, device="cuda")
-    assert L.cc_jpeg_crops_decoded(ptr(dev), 1, 40, 40, 1, r.ctypes.data, 1, 95, ptr(big), 40, 40, None, ptr(ws), 1 << 30, None,
-                                   stream_ptr()) == -1               # no status array
-    assert L.cc_jpeg_crops_decoded(ptr(dev), 1, 40, 40, 7, r.ctypes.data, 1, 95, None, 0, 0, None, None, 0, ctypes.byref(need),
-                                   None) == -1                       # unknown source format
+    assert L.cc_jpeg_crops_decoded_frames(t, 1, r.ctypes.data, 1, 95, ptr(big), 40, 40, None, ptr(ws), 1 << 30, None,
+                                          stream_ptr()) == -1        # no status array
+    t7 = ops.batch_table(dev, 7)
+    assert L.cc_jpeg_crops_decoded_frames(t7, 1, r.ctypes.data, 1, 95, None, 0, 0, None, None, 0, ctypes.byref(need),
+                                          None) == -1                # unknown source format
     torch.cuda.synchronize()
     assert st.cpu().item() == 0

@@ -11,6 +11,7 @@ from oracle import jpeg as oj
 from oracle.yuv import i420_to_bgr
 from clearcam_b200 import ops
 from clearcam_b200._lib import lib, ptr, stream_ptr
+from clearcam_b200.pixfmt import CC_FRAME_BGR_U8 as BGR, CC_FRAME_I420_U8 as I420, CC_FRAME_RGB_U8 as RGB
 
 pytestmark = pytest.mark.gpu
 
@@ -38,11 +39,15 @@ def _frames(n, H, W, seed):
     return np.stack(out)
 
 
-def _encode(frames, rects, q, src_fmt=1):
-    return ops.jpeg_encode_crops(torch.from_numpy(np.ascontiguousarray(frames)).cuda(), rects, q, src_fmt)
+def _encode_dev(dev, rects, q, fmt=BGR):
+    return ops.jpeg_collect(*ops.jpeg_encode_crops_frames(ops.batch_table(dev, fmt), rects, q))
 
 
-def test_fixture():
+def _encode(frames, rects, q, fmt=BGR):
+    return _encode_dev(torch.from_numpy(np.ascontiguousarray(frames)).cuda(), rects, q, fmt)
+
+
+def test_table_encoder_fixture():
     g = np.load(GOLDEN)
     k = 0
     while f"img{k}" in g:
@@ -50,7 +55,7 @@ def test_fixture():
             want = g[f"jpg{k}_{q}"].tobytes()
             if f"yuv{k}" in g:
                 x1, y1, x2, y2 = (int(v) for v in g[f"rect{k}"])
-                got = _encode(g[f"yuv{k}"][None], [(0, x1, y1, x2, y2)], q, 2)[0]
+                got = _encode(g[f"yuv{k}"][None], [(0, x1, y1, x2, y2)], q, I420)[0]
             else:
                 img = g[f"img{k}"]
                 got = _encode(img[None], [(0, 0, 0, img.shape[1], img.shape[0])], q)[0]
@@ -59,7 +64,7 @@ def test_fixture():
     assert k >= 17
 
 
-def test_every_size_up_to_33_in_one_call():
+def test_table_encoder_every_size_up_to_33_in_one_call():
     fr = _frames(2, 70, 70, seed=1)
     rects = [((w + h) % 2, (3 * w) % 5, (7 * h) % 3, (3 * w) % 5 + w, (7 * h) % 3 + h) for w in range(1, 34) for h in range(1, 34)]
     for q in (95, 50):
@@ -78,13 +83,13 @@ _RECTS_1080 = [(0, 1, 3, 201, 157), (1, 1719, 881, 1920, 1080), (0, 0, 0, 1920, 
 
 
 @pytest.mark.parametrize("q", [95, 85])
-def test_source_formats(q):
+def test_table_encoder_source_formats(q):
     cv2 = _cv2()
     bgr = _frames(2, 1080, 1920, seed=2)
     rgb = np.ascontiguousarray(bgr[..., ::-1])
     yuv = np.stack([cv2.cvtColor(f, cv2.COLOR_BGR2YUV_I420) for f in bgr])
     conv = i420_to_bgr(yuv)
-    got_b, got_r, got_y = _encode(bgr, _RECTS_1080, q, 1), _encode(rgb, _RECTS_1080, q, 0), _encode(yuv, _RECTS_1080, q, 2)
+    got_b, got_r, got_y = _encode(bgr, _RECTS_1080, q, BGR), _encode(rgb, _RECTS_1080, q, RGB), _encode(yuv, _RECTS_1080, q, I420)
     for i, (f, x1, y1, x2, y2) in enumerate(_RECTS_1080):
         want = _imencode(bgr[f, y1:y2, x1:x2], q)
         assert got_b[i] == want, ("bgr", i)
@@ -94,14 +99,14 @@ def test_source_formats(q):
         assert np.array_equal(conv[f, y1:y2, x1:x2], cv2.cvtColor(yuv[f], cv2.COLOR_YUV2BGR_I420)[y1:y2, x1:x2])
 
 
-def test_full_frame_q85_matches_oracle():
+def test_table_encoder_full_frame_q85_matches_oracle():
     fr = _frames(1, 1080, 1920, seed=3)
     got = _encode(fr, [(0, 0, 0, 1920, 1080)], 85)[0]
     assert got == _imencode(fr[0], 85)
     assert got == oj.encode(fr[0], 85)
 
 
-def test_many_crops_in_one_call_equal_single_calls():
+def test_table_encoder_many_crops_in_one_call_equal_single_calls():
     fr = _frames(8, 540, 960, seed=4)
     rng = np.random.default_rng(5)
     rects = []
@@ -112,13 +117,13 @@ def test_many_crops_in_one_call_equal_single_calls():
     got = _encode(fr, rects, 95)
     dev = torch.from_numpy(fr).cuda()
     for i, r in enumerate(rects):
-        assert got[i] == ops.jpeg_encode_crops(dev, [r], 95, 1)[0], i
+        assert got[i] == _encode_dev(dev, [r], 95)[0], i
         if i % 20 == 0:
             f, x1, y1, x2, y2 = r
             assert got[i] == _imencode(fr[f, y1:y2, x1:x2], 95), i
 
 
-def test_bytes_past_each_length_stay_untouched_and_noise_fits_the_bound():
+def test_table_encoder_bytes_past_each_length_stay_untouched_and_noise_fits_the_bound():
     rng = np.random.default_rng(6)
     fr = rng.integers(0, 256, (2, 300, 400, 3), dtype=np.uint8)
     rects = np.array([(0, 0, 0, 400, 300), (1, 7, 9, 240, 263), (0, 399, 299, 400, 300), (1, 100, 100, 133, 117)], np.int32)
@@ -132,11 +137,11 @@ def test_bytes_past_each_length_stay_untouched_and_noise_fits_the_bound():
         out = torch.full((cap,), 0xA5, dtype=torch.uint8, device="cuda")
         lengths = torch.zeros(len(rects), dtype=torch.int64, device="cuda")
         need = ctypes.c_size_t(0)
-        args = (ptr(dev), 2, 300, 400, 1, rects.ctypes.data, len(rects), q)
-        assert L.cc_jpeg_encode_crops(*args, None, 0, None, None, None, 0, ctypes.byref(need), None) == 0
+        args = (ops.batch_table(dev, BGR), 2, rects.ctypes.data, len(rects), q)
+        assert L.cc_jpeg_encode_crops_frames(*args, None, 0, None, None, None, 0, ctypes.byref(need), None) == 0
         ws = torch.empty(need.value, dtype=torch.uint8, device="cuda")
-        assert L.cc_jpeg_encode_crops(*args, ptr(out), cap, offsets.ctypes.data, ptr(lengths), ptr(ws), need.value, None,
-                                      stream_ptr()) == 0
+        assert L.cc_jpeg_encode_crops_frames(*args, ptr(out), cap, offsets.ctypes.data, ptr(lengths), ptr(ws), need.value, None,
+                                             stream_ptr()) == 0
         o, n = out.cpu().numpy(), lengths.cpu().numpy()
         used = np.zeros(cap, bool)
         for k, r in enumerate(rects):
@@ -147,15 +152,16 @@ def test_bytes_past_each_length_stay_untouched_and_noise_fits_the_bound():
         assert (o[~used] == 0xA5).all(), q
 
 
-def test_coefficient_tap_equals_the_oracle_blocks():
+def test_table_coefficient_tap_equals_the_oracle_blocks():
     cv2 = _cv2()
     fr = _frames(2, 240, 320, seed=7)
     rects = [(0, 0, 0, 320, 240), (1, 3, 5, 40, 22), (1, 311, 231, 320, 240), (0, 17, 1, 18, 2), (1, 100, 50, 250, 200)]
-    for q, fmt in ((95, 1), (10, 0), (100, 2)):
-        src = fr if fmt == 1 else np.ascontiguousarray(fr[..., ::-1]) if fmt == 0 else \
+    for q, fmt in ((95, BGR), (10, RGB), (100, I420)):
+        src = fr if fmt == BGR else np.ascontiguousarray(fr[..., ::-1]) if fmt == RGB else \
             np.stack([cv2.cvtColor(f, cv2.COLOR_BGR2YUV_I420) for f in fr])
-        img = fr if fmt != 2 else i420_to_bgr(src)
-        got = ops.jpeg_coeffs(torch.from_numpy(src).cuda(), rects, q, fmt).cpu().numpy()
+        img = fr if fmt != I420 else i420_to_bgr(src)
+        dev = torch.from_numpy(src).cuda()
+        got = ops.jpeg_coeffs_frames(ops.batch_table(dev, fmt), rects, q).cpu().numpy()
         want = np.concatenate([oj.blocks(img[f, y1:y2, x1:x2], q) for f, x1, y1, x2, y2 in rects])
         assert got.shape == want.shape and np.array_equal(got, want), (q, fmt)
 

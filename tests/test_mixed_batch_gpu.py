@@ -235,6 +235,7 @@ def test_bad_tables_fail_and_leave_the_output_untouched():
     bad = {
         "mixed net shapes": [cc_frame(b180.data_ptr(), 0, 180, 320), cc_frame(square.data_ptr(), 0, 320, 320)],
         "float32 frame": [cc_frame(b180.data_ptr(), 0, 180, 320), cc_frame(f32.data_ptr(), 1, 180, 320)],
+        "RGB frame": [cc_frame(b180.data_ptr(), 0, 180, 320), cc_frame(b180.data_ptr(), 3, 180, 320)],
         "odd I420 side": [cc_frame(b360.data_ptr(), 0, 360, 640), cc_frame(odd.data_ptr(), 2, 181, 320)],
         "too many frames": [cc_frame(b180.data_ptr(), 0, 180, 320)] * (CC_MAX_FRAMES + 1),
         "only padding": [cc_frame(None, 0, 0, 0)] * 2,
@@ -247,6 +248,8 @@ def test_bad_tables_fail_and_leave_the_output_untouched():
         torch.cuda.synchronize()
         assert rc != 0 and lib().cc_last_error(), what
         assert bool((out == -7.0).all()), f"{what}: d_out was written"
+        sz = ctypes.c_size_t(0)
+        assert lib().cc_yolo_workspace_bytes_frames(m._h, ctypes.cast(table, ctypes.c_void_p), B, RES, ctypes.byref(sz)) != 0, what
     for frames, fmts in [([b180, square], "bgr24"), ([b180, f32], "bgr24"), ([b180.cpu()], "bgr24"),
                          ([b360, b180[None]], "bgr24"), ([b180] * (CC_MAX_FRAMES + 1), "bgr24"), ([None, None], "bgr24"),
                          ([b180, b180], ["bgr24"]), ([b180], "nv12")]:

@@ -98,7 +98,7 @@ def test_decode_frames_into_pitched_rows_and_buffers_touches_nothing_else():
     assert (b[~written] == 0xA5).all()
 
 
-def test_decode_frames_argument_refusals_before_launch():
+def test_decode_frames_refuses_bad_destinations_before_launch():
     f = _enc(_img(20, 30, 60), 90)
     dec = ops.JpegDecoder()
     dec.stage([f, f])
@@ -112,14 +112,14 @@ def test_decode_frames_argument_refusals_before_launch():
 
     def call(*d):
         outs = (cc_jpeg_dest * 2)(*d)
-        return L.cc_jpeg_decode_frames(*args, outs, ptr(dec._st_dev), ptr(dec._ws), dec._ws.numel(), None, stream_ptr())
+        return L.cc_jpeg_decode_frames(*args, outs, ptr(dec._st_dev), None, ptr(dec._ws), dec._ws.numel(), None, stream_ptr())
     ok = cc_jpeg_dest(out[0].data_ptr(), 90, 20, 30), cc_jpeg_dest(out[1].data_ptr(), 90, 20, 30)
     assert call(*ok) == 0
     assert call(ok[0], cc_jpeg_dest(big.data_ptr(), 120, 21, 30)) == -1              # not the image's size
     assert call(ok[0], cc_jpeg_dest(big.data_ptr(), 89, 20, 30)) == -1               # pitch below 3 w
     assert call(ok[0], cc_jpeg_dest(out[0].data_ptr() + 90 * 19, 90, 20, 30)) == -1  # overlaps the first
     assert call(ok[0], cc_jpeg_dest(None, 90, 20, 30)) == -1
-    assert L.cc_jpeg_decode_frames(*args, (cc_jpeg_dest * 2)(*ok), ptr(dec._st_dev), ptr(dec._ws), 1, None, stream_ptr()) == -1
+    assert L.cc_jpeg_decode_frames(*args, (cc_jpeg_dest * 2)(*ok), ptr(dec._st_dev), None, ptr(dec._ws), 1, None, stream_ptr()) == -1
     out.fill_(3)
     big.fill_(3)
     for bad in ((ok[0], cc_jpeg_dest(big.data_ptr(), 120, 21, 30)), (ok[0], cc_jpeg_dest(big.data_ptr(), 89, 20, 30))):

@@ -146,9 +146,7 @@ def test_table_checks_raise_before_any_library_call(no_library):
             of.encode_embed_frames(frames, fmts, rects)
             pytest.fail(what)
         with pytest.raises(ValueError):
-            ops.jpeg_encode_crops_frames(frames, fmts, rects)
-        with pytest.raises(ValueError):
-            ops.jpeg_crops_decoded_frames(frames, fmts, rects)
+            ops.table_rects(rects, ops.frame_table(frames, fmts)[1])
     with pytest.raises(ValueError):
         of.encode_embed_frames([big], "bgr24", [(0, 0, 0, 8, 8)], quality=101)
 
@@ -166,7 +164,7 @@ def test_detector_frame_table_keeps_its_checks():
 
 
 # ------------------------------------------------------------------------------------------------ C-ABI argument checks
-def test_table_entry_points_reject_bad_arguments():
+def test_crop_tables_reject_bad_arguments_and_take_rgb():
     """Every check runs before anything is launched: the device pointers below are never dereferenced."""
     from clearcam_b200._lib import cc_frame, lib
     h = lib()
@@ -202,11 +200,13 @@ def test_table_entry_points_reject_bad_arguments():
 
     assert enc(out=None) == 0 and need.value > 0
     assert dec() == 0 and need.value > 0
+    rgb = [cc_frame(f.data, 3 if f.fmt == 0 else f.fmt, f.h, f.w) for f in good]      # CC_FRAME_RGB_U8: the crops take it
+    assert enc(frames=rgb, out=None) == 0 and dec(frames=rgb) == 0
     odd_i420 = [good[0], cc_frame(fake, 2, 481, 640), good[2]]
     cases = [
         (dict(frames=[good[0], cc_frame(None, 0, 480, 640), good[2]]), ["frame 1 is NULL"]),
         (dict(frames=[good[0], cc_frame(fake, 1, 480, 640), good[2]]), ["frame 1 has format 1"]),
-        (dict(frames=[good[0], cc_frame(fake, 3, 480, 640), good[2]]), ["frame 1 has format 3"]),
+        (dict(frames=[good[0], cc_frame(fake, 4, 480, 640), good[2]]), ["frame 1 has format 4"]),
         (dict(frames=odd_i420), ["frame 1", "even height and width"]),
         (dict(frames=[good[0], cc_frame(fake, 2, 480, 639), good[2]]), ["frame 1", "even height and width"]),
         (dict(frames=[good[0], good[1], cc_frame(fake, 0, 0, 17)]), ["frame 2 has a bad size"]),
@@ -238,3 +238,9 @@ def test_table_entry_points_reject_bad_arguments():
     big = np.array([[0, 0, 0, 320, 240]], np.int32)
     refused(enc(frames=[cc_frame(fake, 0, 70000, 70000)], r=np.array([[0, 0, 0, 65536, 8]], np.int32)), "larger than 65535")
     assert enc(r=big, out=None) == 0
+    # RGB frames are for the crops only: the letterbox and the face canvas refuse them before any device query
+    oh, ow = ctypes.c_int(), ctypes.c_int()
+    refused(h.cc_letterbox_frames((cc_frame * 1)(rgb[0]), 1, 640, None, ctypes.byref(oh), ctypes.byref(ow), None),
+            "cc_letterbox_frames", "frame 0 has format 3")
+    assert h.cc_letterbox_frames((cc_frame * 1)(good[0]), 1, 640, None, ctypes.byref(oh), ctypes.byref(ow), None) == 0
+    refused(h.cc_face_canvas((cc_frame * 1)(rgb[0]), 1, fake, None), "cc_face_canvas", "format 3")

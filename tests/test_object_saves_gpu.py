@@ -1,5 +1,6 @@
-"""Every camera's object saves in one call on the GPU: the frame-table forms of the JPEG encoder, the crops-decoded tap and
-the CLIP preprocess against the uniform entry points on each frame alone and against cv2, ObjectFinder.encode_embed_frames
+"""Every camera's object saves in one call on the GPU: the JPEG encoder, the crops-decoded tap and the CLIP preprocess over
+a mixed table against the same entry points called with each frame alone (a "uniform call": a one-frame table, so crops of
+different sources in one call, over more than one launch, do not affect each other) and against cv2, ObjectFinder.encode_embed_frames
 against the reference's host chain, CameraBatch.save_objects end to end on a mixed fleet, and bad tables."""
 import ctypes
 
@@ -75,8 +76,12 @@ def _rects(seed=7, n_random=300):
 
 
 def _solo(frames, fmts, j):
-    """Frame j alone as a uniform batch of one: (tensor, src_fmt of the uniform entry points)."""
-    return frames[j][None], 1 if fmts[j] == "bgr24" else 2
+    """Frame j alone: a one-frame table."""
+    return ops.frame_table([frames[j]], fmts[j])[0]
+
+
+def _files(table, rects, q):
+    return ops.jpeg_collect(*ops.jpeg_encode_crops_frames(table, rects, q))
 
 
 @pytest.fixture(scope="module")
@@ -84,20 +89,20 @@ def fleet():
     return _fleet()
 
 
-def test_table_encoder_equals_the_uniform_encoder_and_cv2(fleet):
+def test_table_encoder_equals_one_frame_tables_and_cv2(fleet):
     cv2 = _cv2()
     frames, fmts, host = fleet
     rects = _rects()
     assert len(rects) > 256
+    table, _ = ops.frame_table(frames, fmts)
     for q in (95, 50):
-        files = ops.jpeg_encode_crops_frames(frames, fmts, rects, q)
+        files = _files(table, rects, q)
         assert len(files) == len(rects)
         for j in range(len(FLEET)):
             ks = np.flatnonzero(rects[:, 0] == j)
             sub = rects[ks].copy()
             sub[:, 0] = 0
-            t, src_fmt = _solo(frames, fmts, j)
-            solo = ops.jpeg_encode_crops(t, sub, q, src_fmt)
+            solo = _files(_solo(frames, fmts, j), sub, q)
             for k, f in zip(ks, solo):
                 assert files[k] == f, (q, j, k)
         for k, (j, x1, y1, x2, y2) in enumerate(rects):
@@ -105,7 +110,7 @@ def test_table_encoder_equals_the_uniform_encoder_and_cv2(fleet):
             assert files[k] == want.tobytes(), (q, k)
 
 
-def test_table_encoder_leaves_the_bytes_past_each_length(fleet):
+def test_table_encoder_leaves_the_bytes_past_each_crop_length(fleet):
     frames, fmts, _ = fleet
     rects = _rects(seed=8, n_random=40)
     table, sizes = ops.frame_table(frames, fmts)
@@ -120,25 +125,25 @@ def test_table_encoder_leaves_the_bytes_past_each_length(fleet):
     assert lib().cc_jpeg_encode_crops_frames(*args, ptr(out), out.numel(), offs.ctypes.data, ptr(lengths), ptr(ws), need.value,
                                              None, stream_ptr()) == 0
     lens, host = lengths.cpu().numpy(), out.cpu().numpy()
-    files = ops.jpeg_encode_crops_frames(frames, fmts, rects, 95)
+    files = _files(table, rects, 95)
     for k in range(len(rects)):
         assert host[offs[k]:offs[k] + lens[k]].tobytes() == files[k]
         assert (host[offs[k] + lens[k]:offs[k] + bounds[k]] == 0xA5).all(), k
 
 
 @pytest.mark.parametrize("q", [95, 2])
-def test_table_crops_decoded_equal_the_uniform_call(fleet, q):
+def test_table_crops_decoded_equal_one_frame_tables(fleet, q):
     cv2 = _cv2()
     frames, fmts, _ = fleet
     rects = _rects(seed=9, n_random=60)
-    pix, st = ops.jpeg_crops_decoded_frames(frames, fmts, rects, q)
+    table, _ = ops.frame_table(frames, fmts)
+    pix, st = ops.jpeg_crops_decoded_frames(table, rects, q)
     pix, st = pix.cpu().numpy(), st.cpu().numpy()
     for j in range(len(FLEET)):
         ks = np.flatnonzero(rects[:, 0] == j)
         sub = rects[ks].copy()
         sub[:, 0] = 0
-        t, src_fmt = _solo(frames, fmts, j)
-        want, wst = ops.jpeg_crops_decoded(t, sub, q, src_fmt)
+        want, wst = ops.jpeg_crops_decoded_frames(_solo(frames, fmts, j), sub, q)
         want, wst = want.cpu().numpy(), wst.cpu().numpy()
         for i, k in enumerate(ks):
             assert st[k] == wst[i], (q, j, k)
@@ -147,7 +152,7 @@ def test_table_crops_decoded_equal_the_uniform_call(fleet, q):
                 assert np.array_equal(pix[k, :h, :w], want[i, :h, :w]), (q, j, k)
     if q == 2:
         assert (st == ops.JPEG_UNSUPPORTED).any()
-        files = ops.jpeg_encode_crops_frames(frames, fmts, rects, q)
+        files = _files(table, rects, q)
         from oracle import jpeg_decode as od
         for k in np.flatnonzero(st == ops.JPEG_UNSUPPORTED):
             assert od.decode(files[k])[0] == ops.JPEG_UNSUPPORTED
@@ -156,7 +161,7 @@ def test_table_crops_decoded_equal_the_uniform_call(fleet, q):
     del cv2
 
 
-def test_table_clip_preprocess_equals_the_uniform_call(fleet):
+def test_table_clip_preprocess_equals_one_frame_tables(fleet):
     frames, fmts, _ = fleet
     rects = _rects(seed=10, n_random=80)
     assert len(rects) > 64
@@ -169,10 +174,8 @@ def test_table_clip_preprocess_equals_the_uniform_call(fleet):
         ks = np.flatnonzero(rects[:, 0] == j)
         sub = np.ascontiguousarray(rects[ks].copy())
         sub[:, 0] = 0
-        t, src_fmt = _solo(frames, fmts, j)
-        H, W = FLEET[j][0]
         want = torch.empty(len(sub), 3, S, S, device="cuda")
-        assert lib().cc_clip_preprocess(ptr(t), 1, H, W, sub.ctypes.data, len(sub), S, src_fmt, ptr(want), stream_ptr()) == 0
+        assert lib().cc_clip_preprocess_frames(_solo(frames, fmts, j), 1, sub.ctypes.data, len(sub), S, ptr(want), stream_ptr()) == 0
         assert torch.equal(got[torch.from_numpy(ks).cuda()], want), j
 
 
@@ -195,7 +198,7 @@ def _host_chain(of, files):
 
 
 @pytest.mark.parametrize("q", [95, 2])
-def test_encode_embed_frames_equals_encode_crops_and_the_host_chain(fleet, q):
+def test_encode_embed_frames_equals_per_frame_encode_crops_and_the_host_chain(fleet, q):
     cv2 = _cv2()
     cv2.ipp.setUseIPP(False)
     frames, fmts, _ = fleet
@@ -206,11 +209,10 @@ def test_encode_embed_frames_equals_encode_crops_and_the_host_chain(fleet, q):
     of = _finder()
     files, emb = of.encode_embed_frames(frames, fmts, rects, q)
     for k, (j, *r) in enumerate(rects.tolist()):
-        t, _ = _solo(frames, fmts, j)
-        assert files[k] == of.encode_crops(t, [(0, *r)], q, pix_fmt=fmts[j])[0], k
+        assert files[k] == of.encode_crops(frames[j][None], [(0, *r)], q, pix_fmt=fmts[j])[0], k
     assert torch.equal(emb.tensor, _host_chain(of, files))
     if q == 2:
-        _, st = ops.jpeg_crops_decoded_frames(frames, fmts, rects, q)
+        _, st = ops.jpeg_crops_decoded_frames(ops.frame_table(frames, fmts)[0], rects, q)
         assert (st.cpu().numpy() == ops.JPEG_UNSUPPORTED).any()         # the cv2 fallback ran
     of.model = None
     files2, none = of.encode_embed_frames(frames, fmts, rects, q)

@@ -10,7 +10,7 @@ import torch
 
 from oracle import yolov9 as o
 from oracle.yuv import i420_to_bgr
-from clearcam_b200._lib import lib, ptr, stream_ptr
+from clearcam_b200._lib import cc_frame, lib, ptr, stream_ptr
 from clearcam_b200.detection.yolov9 import YOLOv9
 
 pytestmark = pytest.mark.gpu
@@ -167,7 +167,7 @@ def test_bad_frames_raise_value_error_in_python():
         m(torch.zeros(1621, 1920, dtype=torch.uint8), pix_fmt="yuv420p")
 
 
-def test_library_rejects_odd_i420_sizes_and_unknown_formats():
+def test_library_and_crop_tables_reject_odd_i420_sizes_and_unknown_formats():
     L = lib()
     m = _model(False)
     buf = torch.zeros(2 * 1622 * 1921, dtype=torch.uint8, device="cuda")
@@ -180,7 +180,8 @@ def test_library_rejects_odd_i420_sizes_and_unknown_formats():
         assert rc < 0 and words in L.cc_last_error().decode(), (fmt, H, W)
     rects = np.array([[0, 0, 0, 8, 8]], np.int32)
     crops = torch.empty(1, 3, 224, 224, device="cuda")
-    for fmt, H, W, words in [(2, 1081, 1920, "even"), (2, 1080, 1921, "even"), (3, 1080, 1920, "unknown source format")]:
-        rc = L.cc_clip_preprocess(ptr(buf), 1, H, W, rects.ctypes.data, 1, 224, fmt, ptr(crops), stream_ptr())
+    for fmt, H, W, words in [(2, 1081, 1920, "even"), (2, 1080, 1921, "even"), (4, 1080, 1920, "unknown source format")]:
+        table = (cc_frame * 1)(cc_frame(buf.data_ptr(), fmt, H, W))
+        rc = L.cc_clip_preprocess_frames(table, 1, rects.ctypes.data, 1, 224, ptr(crops), stream_ptr())
         assert rc < 0 and words in L.cc_last_error().decode(), (fmt, H, W)
     torch.cuda.synchronize()

@@ -6,7 +6,7 @@ Prints the card's name and power limit, then for two workloads, alternated `reps
   * crops: K = 64 crops of 150-600 px sides from 8 1080p BGR frames at quality 95 (the object thumbnails of
     `save_object`); also from the same frames as yuv420p;
   * frames: the 8 whole 1080p frames at quality 85;
-the device time of one cc_jpeg_encode_crops call (CUDA events around `calls` back-to-back calls, buffers allocated once),
+the device time of one cc_jpeg_encode_crops_frames call (CUDA events around `calls` back-to-back calls, buffers allocated once),
 the wall time of `ObjectFinder.encode_crops` (launch, lengths back, used bytes back, split into `bytes`), the device time
 per kernel from one torch.profiler pass (which stage dominates), the bytes that cross PCIe against the raw crops, and
 single-thread cv2.imencode of the same crops on this host.  Every GPU file is checked against cv2's bytes first.
@@ -61,18 +61,18 @@ def crop_rects(k=64, seed=1):
 
 
 class Call:
-    """One cc_jpeg_encode_crops call with its buffers allocated up front."""
+    """One cc_jpeg_encode_crops_frames call with its frame table and buffers made up front."""
 
-    def __init__(self, dev, rects, q, src_fmt):
+    def __init__(self, dev, rects, q, fmt):
         from clearcam_b200 import ops
         from clearcam_b200._lib import lib, ptr
-        self.lib, n = lib(), dev.shape[0]
+        self.lib, self.table = lib(), ops.batch_table(dev, fmt)
         self.rects = np.ascontiguousarray(rects, np.int32)
         bounds = np.array([ops.jpeg_bound(r[3] - r[1], r[4] - r[2]) for r in self.rects], np.int64)
         self.offsets = np.ascontiguousarray(np.concatenate([[0], np.cumsum(bounds)[:-1]]).astype(np.int64))
         need = ctypes.c_size_t(0)
-        self.args = (ptr(dev), n, H, W, src_fmt, self.rects.ctypes.data, len(self.rects), q)
-        assert self.lib.cc_jpeg_encode_crops(*self.args, None, 0, None, None, None, 0, ctypes.byref(need), None) == 0
+        self.args = (self.table, len(self.table), self.rects.ctypes.data, len(self.rects), q)
+        assert self.lib.cc_jpeg_encode_crops_frames(*self.args, None, 0, None, None, None, 0, ctypes.byref(need), None) == 0
         self.out = torch.empty(int(bounds.sum()), dtype=torch.uint8, device="cuda")
         self.lengths = torch.empty(len(self.rects), dtype=torch.int64, device="cuda")
         self.ws = torch.empty(need.value, dtype=torch.uint8, device="cuda")
@@ -81,8 +81,8 @@ class Call:
 
     def __call__(self):
         s = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        rc = self.lib.cc_jpeg_encode_crops(*self.args, self.ptr(self.out), self.out.numel(), self.offsets.ctypes.data,
-                                           self.ptr(self.lengths), self.ptr(self.ws), self.need, None, s)
+        rc = self.lib.cc_jpeg_encode_crops_frames(*self.args, self.ptr(self.out), self.out.numel(), self.offsets.ctypes.data,
+                                                  self.ptr(self.lengths), self.ptr(self.ws), self.need, None, s)
         assert rc == 0, self.lib.cc_last_error()
 
 
@@ -137,6 +137,7 @@ def main():
         sys.exit("needs a GPU")
     import cv2
     from clearcam_b200.models.objects import ObjectFinder
+    from clearcam_b200.pixfmt import CC_FRAME_BGR_U8, CC_FRAME_I420_U8
     info = card()
     print("card:", info, flush=True)
     fr = frames()
@@ -145,8 +146,9 @@ def main():
     dev, dev_y = torch.from_numpy(fr).cuda(), torch.from_numpy(yuv).cuda()
     rects = crop_rects()
     full = np.array([(i, 0, 0, W, H) for i in range(NF)], np.int32)
-    work = {"crops_q95_bgr24": (dev, rects, 95, 1, "bgr24", fr), "crops_q95_yuv420p": (dev_y, rects, 95, 2, "yuv420p", conv),
-            "frames_q85_bgr24": (dev, full, 85, 1, "bgr24", fr)}
+    work = {"crops_q95_bgr24": (dev, rects, 95, CC_FRAME_BGR_U8, "bgr24", fr),
+            "crops_q95_yuv420p": (dev_y, rects, 95, CC_FRAME_I420_U8, "yuv420p", conv),
+            "frames_q85_bgr24": (dev, full, 85, CC_FRAME_BGR_U8, "bgr24", fr)}
     finder = ObjectFinder()
     result = {"metric": "jpeg_encode_crops", "card": info, "frames": [NF, H, W], "calls": a.calls, "reps": a.reps, "by_workload": {}}
     rows = {}

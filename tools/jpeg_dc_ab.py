@@ -1,4 +1,4 @@
-"""Per-kernel device time of cc_jpeg_decode on one large file without restart markers, for several library builds
+"""Per-kernel device time of cc_jpeg_decode_frames on one large file without restart markers, for several library builds
 alternated in fresh processes (the DC pass walks such a file's single restart interval).
 
     python tools/jpeg_dc_ab.py [--reps 3] [--calls 30] -- base "CC_LIB=/path/to/other/libclearcam_b200.so" ...

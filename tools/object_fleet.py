@@ -1,6 +1,6 @@
 """What saving and embedding every camera's objects in one call buys over one call per camera.
 
-    python tools/object_fleet.py [--steps 100] [--runs 3] [--archs ViT-B/32 ViT-L/14] [--parent-lib PATH] [--out FILE]
+    python tools/object_fleet.py [--steps 100] [--runs 3] [--archs ViT-B/32 ViT-L/14] [--out FILE]
 
 Prints the card's name and power limit, then, for each CLIP architecture (synthetic weights) and each fleet:
   * a: 8 cameras each of 720p, 1080p, 1440p and 2160p, alternately bgr24 and yuv420p (32 cameras);
@@ -10,12 +10,8 @@ a seeded sequence of steps in which a seeded subset of cameras (about half) has 
 It first checks, over the first steps, that `CameraBatch.save_objects`'s way (one `encode_embed_frames` call) gives the
 same files as the per-camera `encode_embed_crops` loop, and reports how far the embeddings are apart (bit-equal, or the
 largest difference).  Then it alternates the two ways in `runs` runs of `steps` steps each and records, per step, the
-device time between CUDA events around the step's calls and the wall time of the step (ending in a synchronise).
-
-With --parent-lib (a libclearcam_b200.so built from the parent commit) it also re-times the uniform crop workloads of
-tools/jpeg_crops.py and tools/jpeg_decode.py (64 crops of 150-600 px from 8 1080p frames, bgr24 and yuv420p, quality 95)
-and the uniform cc_clip_preprocess of the same crops, on the parent library and on this tree's, alternated in fresh
-processes, because the crop kernels changed.  One JSON line at the end."""
+device time between CUDA events around the step's calls and the wall time of the step (ending in a synchronise).  One
+JSON line at the end."""
 import argparse
 import json
 import os
@@ -160,67 +156,17 @@ def fleet_bench(arch, steps_n, runs):
     return out
 
 
-# ---- the uniform crop workloads (run in a fresh process per library)
-def uniform_workloads(calls=50):
-    import ctypes
-    from tools.jpeg_crops import Call, crop_rects, device_ms, frames
-    from tools.jpeg_decode import Chain
-    from clearcam_b200._lib import lib, ptr
-    import cv2
-    fr = frames()
-    rects = crop_rects()
-    bgr = torch.from_numpy(fr).cuda()
-    yuv = torch.from_numpy(np.stack([cv2.cvtColor(f, cv2.COLOR_BGR2YUV_I420) for f in fr])).cuda()
-    res = {}
-    for name, dev, fmt in (("bgr24", bgr, 1), ("yuv420p", yuv, 2)):
-        res[f"encode_{name}_ms"] = device_ms(Call(dev, rects, 95, fmt), calls)
-    res["crops_decoded_bgr24_ms"] = device_ms(Chain(bgr, rects, 95), calls)
-    H, W = fr.shape[1], fr.shape[2]
-    r = np.ascontiguousarray(rects, np.int32)
-    out = torch.empty(len(r), 3, 224, 224, device="cuda")
-    for name, dev, fmt in (("bgr24", bgr, 1), ("yuv420p", yuv, 2)):
-        def pre(dev=dev, fmt=fmt):
-            s = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-            assert lib().cc_clip_preprocess(ptr(dev), dev.shape[0], H, W, r.ctypes.data, len(r), 224, fmt, ptr(out), s) == 0
-        res[f"clip_preprocess_{name}_ms"] = device_ms(pre, calls)
-    return {k: round(v, 4) for k, v in res.items()}
-
-
-def uniform_ab(parent_lib, reps):
-    rows = {"parent": [], "this": []}
-    for _ in range(reps):
-        for key in ("parent", "this"):
-            env = dict(os.environ)
-            env.pop("CC_LIB", None)
-            if key == "parent":
-                env["CC_LIB"] = parent_lib
-            p = subprocess.run([sys.executable, os.path.abspath(__file__), "--uniform-only"], env=env, capture_output=True,
-                               text=True, cwd=ROOT)
-            if p.returncode != 0:
-                raise RuntimeError(p.stderr[-3000:])
-            rows[key].append(json.loads(p.stdout.strip().splitlines()[-1]))
-            print(key, rows[key][-1], flush=True)
-    return rows
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--archs", nargs="+", default=["ViT-B/32", "ViT-L/14"])
-    ap.add_argument("--parent-lib", default=None)
-    ap.add_argument("--uniform-only", action="store_true")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("needs a GPU")
-    if a.uniform_only:
-        print(json.dumps(uniform_workloads()))
-        return
     result = {"card": card()}
     print(json.dumps(result["card"]), flush=True)
-    if a.parent_lib:
-        result["uniform_crops"] = uniform_ab(a.parent_lib, a.runs)
     for arch in a.archs:
         result[arch] = fleet_bench(arch, a.steps, a.runs)
     line = json.dumps(result)
