@@ -74,6 +74,26 @@ class cc_conv_op(ctypes.Structure):
 # cc_conv_op kinds (CC_CONV_OP_* in include/clearcam_b200.h)
 CC_CONV_OP_NONE, CC_CONV_OP_GEMM, CC_CONV_OP_CHAIN, CC_CONV_OP_DIRECT = 0, 1, 2, 3
 
+# cc_operand element types (CC_OP_* in include/clearcam_b200.h)
+CC_OP_U8, CC_OP_BF16, CC_OP_F32, CC_OP_I32 = 0, 1, 2, 3
+CC_OP_IO_MAX = 8
+
+
+class cc_operand(ctypes.Structure):
+    """One operand of a plan op: its slice, CC_OP_* element type and elements from one image to the next (0: dense)."""
+    _fields_ = [("s", cc_slice), ("type", ctypes.c_int), ("ns", ctypes.c_int)]
+
+
+class cc_op_io(ctypes.Structure):
+    """What op i of a plan reads (`in_`, the header's `in`) and writes (`out`), as the cc_*_op_io taps report it, with the
+    scalars a reference needs (include/clearcam_b200.h documents the operand order of each kind)."""
+    _fields_ = ([("kind", ctypes.c_char * 32), ("name", ctypes.c_char * 128), ("n_in", ctypes.c_int), ("n_out", ctypes.c_int),
+                 ("in_", cc_operand * CC_OP_IO_MAX), ("out", cc_operand * CC_OP_IO_MAX),
+                 ("causal", ctypes.c_int), ("eps", ctypes.c_float), ("conf_thr", ctypes.c_float), ("max_det", ctypes.c_int),
+                 ("iou_thr", ctypes.c_float), ("do_scale", ctypes.c_int)]
+                + [(n, ctypes.c_float) for n in ("pad_x", "pad_y", "gain", "clip_w", "clip_h")]
+                + [("act", ctypes.c_int), ("patch", ctypes.c_int)])
+
 # cc_ocsort_gpu_update statuses (CC_TRACK_* in include/clearcam_b200.h)
 CC_TRACK_OK, CC_TRACK_NEEDS_ROOM, CC_TRACK_BAD_CLASS, CC_TRACK_OVERFLOW, CC_TRACK_BAD_BOX = 0, 1, 2, 3, 4
 # cc_ocsort_gpu_events statuses (CC_EVENT_* in include/clearcam_b200.h)
@@ -118,6 +138,7 @@ _SIGS = {
     "cc_yolo_trace": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _i, ctypes.POINTER(ctypes.c_ulonglong), ctypes.POINTER(ctypes.c_char_p),
                            ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_double), ctypes.POINTER(_i), _vp]),
     "cc_yolo_op_conv": (_i, [_vp, _i, _i, _i, _i, _i, _i, ctypes.POINTER(cc_conv_op)]),
+    "cc_yolo_op_io": (_i, [_vp, _i, _i, _i, _i, _i, _i, ctypes.POINTER(cc_op_io)]),
     "cc_yolo_run_ops": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "cc_yolo_layer_output": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i),
                                   ctypes.POINTER(_i), _vp]),
@@ -133,6 +154,7 @@ _SIGS = {
     "cc_clip_profile": (_i, [_vp, _i, _vp, _i, _vp, _i, ctypes.POINTER(_f), ctypes.POINTER(ctypes.c_double),
                              ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_i), ctypes.POINTER(ctypes.c_double), _vp]),
     "cc_clip_op_conv": (_i, [_vp, _i, _i, _i, ctypes.POINTER(cc_conv_op)]),
+    "cc_clip_op_io": (_i, [_vp, _i, _i, _i, ctypes.POINTER(cc_op_io)]),
     "cc_clip_run_ops": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, ctypes.c_longlong, _vp]),
     "cc_face_create": (_i, [_i, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_vp), ctypes.POINTER(ctypes.c_int64),
                             ctypes.POINTER(_vp)]),
@@ -142,6 +164,7 @@ _SIGS = {
     "cc_face_set_workspace": (_i, [_vp, _vp, ctypes.c_size_t]),
     "cc_face_layer_output": (_i, [_vp, _vp, _i, _i, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
     "cc_face_op_conv": (_i, [_vp, _i, _i, ctypes.POINTER(cc_conv_op)]),
+    "cc_face_op_io": (_i, [_vp, _i, _i, ctypes.POINTER(cc_op_io)]),
     "cc_face_run_ops": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "cc_blazeface_create": (_i, [_i, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_vp), ctypes.POINTER(ctypes.c_int64),
                                  ctypes.POINTER(_vp)]),

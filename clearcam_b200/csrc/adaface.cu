@@ -108,7 +108,10 @@ struct FacePlanBuilder {
     __nv_bfloat16* S = static_cast<__nv_bfloat16*>(dalloc(big));
     float* feat = static_cast<float*>(dalloc(static_cast<size_t>(B) * kFaceDim * 4));
     if (bump.dry) return CC_OK;
-    P.ops.push_back(plan_op("pack", "face_pack", [packed, B](const PlanIO& io, cudaStream_t st) {
+    P.ops.push_back(plan_op("pack", "face_pack",
+                            op_io({operand(nullptr, CC_OP_U8, B, kFaceSide, kFaceSide, 3)},
+                                  {operand(packed, CC_OP_BF16, B, kFaceSide, kFaceSide, kFacePackC)}),
+                            [packed, B](const PlanIO& io, cudaStream_t st) {
       const long long npix = static_cast<long long>(B) * kFaceSide * kFaceSide;
       const long long blocks = (npix + 255) / 256;
       face_pack_kernel<<<blocks < 132 * 16 ? static_cast<int>(blocks) : 132 * 16, 256, 0, st>>>(static_cast<const uint8_t*>(io.in),
@@ -148,7 +151,8 @@ struct FacePlanBuilder {
       if (rc) return rc;
       layer(nhwc_slice(feat, kFaceDim, 0, kFaceDim, 1, B, 1, 1));
     }
-    P.ops.push_back(plan_op("l2norm", "l2norm", [feat, B](const PlanIO& io, cudaStream_t st) {
+    P.ops.push_back(plan_op("l2norm", "l2norm", op_io({operand(feat, CC_OP_F32, B, 1, 1, kFaceDim)}, {operand(nullptr, CC_OP_F32, B, 1, 1, kFaceDim)}),
+                            [feat, B](const PlanIO& io, cudaStream_t st) {
       return l2norm_launch(feat, io.out, B, kFaceDim, io.out_stride, 0.f, st);
     }));
     return rc;
@@ -274,6 +278,13 @@ int cc_face_op_conv(cc_face* h, int B, int i, cc_conv_op* out) {
   FacePlan* P = nullptr;
   if (int rc = face_plan(h, B, &P)) return rc;
   return op_conv_tap("cc_face_op_conv", P->ops, i, out);
+}
+
+int cc_face_op_io(cc_face* h, int B, int i, cc_op_io* out) {
+  CC_REQUIRE(h && B > 0, "cc_face_op_io: bad argument");
+  FacePlan* P = nullptr;
+  if (int rc = face_plan(h, B, &P)) return rc;
+  return op_io_tap("cc_face_op_io", P->ops, i, out);
 }
 
 int cc_face_run_ops(cc_face* h, const uint8_t* d_faces, int B, int first, int last, float* d_out, void* stream) {

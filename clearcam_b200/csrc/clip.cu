@@ -109,16 +109,24 @@ struct PlanBuilder {
     if (rc) return;
     push(gemm_op(name, d, ChainDesc{}, L));
   }
-  // LayerNorm of `rows` fp32 rows of x (row_stride rows apart, or the rows row_idx names) into bf16
+  // LayerNorm of `rows` fp32 rows of x (row_stride rows apart, or the rows row_idx names) into bf16; x is a stream of B images
+  // of L rows
   void layernorm(const char* name, const float* x, __nv_bfloat16* out, const float* g, const float* b, int rows, int W,
-                 long long row_stride, const int* row_idx) {
-    push(plan_op(name, "layernorm", [=](const PlanIO&, cudaStream_t st) {
+                 long long row_stride, const int* row_idx, int B, int L) {
+    const int per = rows / B;   // output rows per image
+    cc_op_io io = op_io({row_idx || row_stride == 1 ? operand(x, CC_OP_F32, B, 1, L, W) : operand(x, CC_OP_F32, B, 1, 1, W, 0, 0, L),
+                         operand(g, CC_OP_F32, 1, 1, 1, W), operand(b, CC_OP_F32, 1, 1, 1, W)},
+                        {operand(out, CC_OP_BF16, B, 1, per, W)});
+    if (row_idx) io.in[io.n_in++] = operand(row_idx, CC_OP_I32, B, 1, 1, 1);
+    push(plan_op(name, "layernorm", io, [=](const PlanIO&, cudaStream_t st) {
       return layernorm_bf16_launch(x, out, g, b, rows, W, row_stride, row_idx, st);
     }));
   }
   // the embeddings, L2-normalised into the call's output rows
   void l2norm(const float* emb, int B, int D, float eps) {
-    push(plan_op("l2norm", "l2norm", [=](const PlanIO& io, cudaStream_t st) {
+    cc_op_io io = op_io({operand(emb, CC_OP_F32, B, 1, 1, D)}, {operand(nullptr, CC_OP_F32, B, 1, 1, D)});
+    io.eps = eps;
+    push(plan_op("l2norm", "l2norm", io, [=](const PlanIO& io, cudaStream_t st) {
       return l2norm_launch(emb, io.out, B, D, io.out_stride, eps, st);
     }));
   }
@@ -131,14 +139,17 @@ struct PlanBuilder {
     __nv_bfloat16* vt = attention_tc_supported(L) ? static_cast<__nv_bfloat16*>(dalloc(attention_tc_workspace_bytes(B, L, tw.heads))) : nullptr;
     for (int i = 0; i < tw.layers && !rc; ++i) {
       const BlockW& b = bw[i];
-      layernorm("ln_1", x, h, b.ln1_g, b.ln1_b, rows, W, 1, nullptr);
+      layernorm("ln_1", x, h, b.ln1_g, b.ln1_b, rows, W, 1, nullptr, B, L);
       gemm("qkv", h, W, rows, W, b.w_in, b.b_in, 3 * W, qkv, 3 * W, false, CC_ACT_NONE, nullptr);
       const int heads = tw.heads, c = causal ? 1 : 0;
-      push(plan_op("attention", "attention", [=](const PlanIO&, cudaStream_t st) {
+      cc_op_io io = op_io({operand(qkv, CC_OP_BF16, B, 1, L, 3 * W)}, {operand(ctx, CC_OP_BF16, B, 1, L, W)});
+      if (vt) io.out[io.n_out++] = operand(vt, CC_OP_BF16, B, heads * 64, (L + 63) / 64 * 64, 1);
+      io.causal = c;
+      push(plan_op("attention", "attention", io, [=](const PlanIO&, cudaStream_t st) {
         return vt ? attention_tc_launch(qkv, ctx, vt, B, L, heads, c, st) : attention_launch(qkv, ctx, B, L, heads, c, st);
       }, 4.0 * B * tw.heads * double(L) * L * 64));
       gemm("out_proj", ctx, W, rows, W, b.w_out, b.b_out, W, x, W, true, CC_ACT_NONE, x);
-      layernorm("ln_2", x, h, b.ln2_g, b.ln2_b, rows, W, 1, nullptr);
+      layernorm("ln_2", x, h, b.ln2_g, b.ln2_b, rows, W, 1, nullptr, B, L);
       gemm("mlp_fc", h, W, rows, W, b.w_fc, b.b_fc, tw.mlp, hid, tw.mlp, false, CC_ACT_GELU_TANH, nullptr);
       gemm("mlp_proj", hid, tw.mlp, rows, tw.mlp, b.w_proj, b.b_proj, W, x, W, true, CC_ACT_NONE, x);
     }
@@ -149,19 +160,24 @@ struct PlanBuilder {
     __nv_bfloat16* patches = static_cast<__nv_bfloat16*>(dalloc(static_cast<size_t>(B) * Pn * M.kpad * 2));
     float* x = static_cast<float*>(dalloc(static_cast<size_t>(B) * L * W * 4));
     const int kpad = M.kpad;
-    push(plan_op("patchify", "patchify", [=](const PlanIO& io, cudaStream_t st) {
+    cc_op_io pio = op_io({operand(nullptr, CC_OP_F32, B, 3 * S, S, 1)}, {operand(patches, CC_OP_BF16, B, 1, Pn, kpad)});
+    pio.patch = p;
+    push(plan_op("patchify", "patchify", pio, [=](const PlanIO& io, cudaStream_t st) {
       return patchify_launch(static_cast<const float*>(io.in), patches, B, S, p, kpad, st);
     }));
     // conv14x14/s14 (no bias) == GEMM over patches; rows land at token 1.. of each image (out_ns = L, +1 row offset)
     gemm("patch_embed", patches, M.kpad, B * Pn, M.kpad, M.patch_w, nullptr, W, x + W, W, true, CC_ACT_NONE, nullptr, B, Pn, L);
     const float *cls = M.cls, *pos = M.pos, *g = M.lnpre_g, *b = M.lnpre_b;
-    push(plan_op("cls+pos+ln_pre", "embed_ln_pre", [=](const PlanIO&, cudaStream_t st) {
+    const cc_op_io eio = op_io({operand(x, CC_OP_F32, B, 1, L, W), operand(cls, CC_OP_F32, 1, 1, 1, W), operand(pos, CC_OP_F32, 1, 1, L, W),
+                                operand(g, CC_OP_F32, 1, 1, 1, W), operand(b, CC_OP_F32, 1, 1, 1, W)},
+                               {operand(x, CC_OP_F32, B, 1, L, W)});
+    push(plan_op("cls+pos+ln_pre", "embed_ln_pre", eio, [=](const PlanIO&, cudaStream_t st) {
       return embed_ln_pre_launch(x, cls, pos, g, b, B * L, L, W, st);
     }));
     blocks(tw, M.vb, B, x, false);
     __nv_bfloat16* pooled = static_cast<__nv_bfloat16*>(dalloc(static_cast<size_t>(B) * W * 2));
     float* emb = static_cast<float*>(dalloc(static_cast<size_t>(B) * D * 4));
-    layernorm("ln_post(token 0)", x, pooled, M.lnpost_g, M.lnpost_b, B, W, L, nullptr);
+    layernorm("ln_post(token 0)", x, pooled, M.lnpost_g, M.lnpost_b, B, W, L, nullptr, B, L);
     gemm("proj", pooled, W, B, W, M.projT, nullptr, D, emb, D, true, CC_ACT_NONE, nullptr);
     l2norm(emb, B, D, 1e-8f);
     return rc;
@@ -173,13 +189,15 @@ struct PlanBuilder {
     int* eot = static_cast<int*>(dalloc(static_cast<size_t>(B) * 4));
     const float *tok = M.tok, *pos = M.pos_t;
     const int vocab = M.cfg.vocab;
-    push(plan_op("tok+pos", "text_embed", [=](const PlanIO& io, cudaStream_t st) {
+    const cc_op_io tio = op_io({operand(nullptr, CC_OP_I32, B, 1, L, 1), operand(tok, CC_OP_F32, 1, 1, vocab, W), operand(pos, CC_OP_F32, 1, 1, L, W)},
+                               {operand(x, CC_OP_F32, B, 1, L, W), operand(eot, CC_OP_I32, B, 1, 1, 1)});
+    push(plan_op("tok+pos", "text_embed", tio, [=](const PlanIO& io, cudaStream_t st) {
       return text_embed_launch(static_cast<const int*>(io.in), tok, pos, x, eot, B, L, W, vocab, st);
     }));
     blocks(tw, M.tb, B, x, true);
     __nv_bfloat16* pooled = static_cast<__nv_bfloat16*>(dalloc(static_cast<size_t>(B) * W * 2));
     float* emb = static_cast<float*>(dalloc(static_cast<size_t>(B) * D * 4));
-    layernorm("ln_final(EOT row)", x, pooled, M.lnf_g, M.lnf_b, B, W, 0, eot);
+    layernorm("ln_final(EOT row)", x, pooled, M.lnf_g, M.lnf_b, B, W, 0, eot, B, L);
     gemm("text_projection", pooled, W, B, W, M.tprojT, nullptr, D, emb, D, true, CC_ACT_NONE, nullptr);
     l2norm(emb, B, D, 0.f);
     return rc;
@@ -313,6 +331,13 @@ int cc_clip_op_conv(cc_clip* h, int text, int B, int i, cc_conv_op* out) {
   ClipPlan* P = nullptr;
   if (int rc = clip_plan(h, text != 0, B, &P)) return rc;
   return op_conv_tap("cc_clip_op_conv", P->ops, i, out);
+}
+
+int cc_clip_op_io(cc_clip* h, int text, int B, int i, cc_op_io* out) {
+  CC_REQUIRE(h && B > 0, "cc_clip_op_io: bad argument");
+  ClipPlan* P = nullptr;
+  if (int rc = clip_plan(h, text != 0, B, &P)) return rc;
+  return op_io_tap("cc_clip_op_io", P->ops, i, out);
 }
 
 int cc_clip_run_ops(cc_clip* h, int text, const void* d_in, int B, int first, int last, float* d_out, long long out_row_stride,

@@ -12,20 +12,60 @@ const char* intern(const std::string& s) {
   return pool.insert(s).first->c_str();
 }
 
-PlanOp plan_op(const std::string& name, const char* kind, PlanOp::Launch launch, double flops, double bytes) {
+cc_operand operand(const TSlice& s, int N, int H, int W, int ns) {
+  cc_operand o{};
+  o.s = cc_slice{s.p, s.cs, s.co, s.C, N, H, W, s.f32 ? 1 : 0};
+  o.type = s.f32 ? CC_OP_F32 : CC_OP_BF16;
+  o.ns = ns;
+  return o;
+}
+
+cc_operand operand(const void* p, int type, int N, int H, int W, int C, int cs, int co, int ns) {
+  cc_operand o{};
+  o.s = cc_slice{const_cast<void*>(p), cs ? cs : C, co, C, N, H, W, type == CC_OP_F32 ? 1 : 0};
+  o.type = type;
+  o.ns = ns;
+  return o;
+}
+
+cc_op_io op_io(std::initializer_list<cc_operand> in, std::initializer_list<cc_operand> out) {
+  cc_op_io io{};
+  for (const cc_operand& o : in) if (io.n_in < CC_OP_IO_MAX) io.in[io.n_in++] = o;
+  for (const cc_operand& o : out) if (io.n_out < CC_OP_IO_MAX) io.out[io.n_out++] = o;
+  return io;
+}
+
+cc_op_io conv_io(const cc_conv_op& c) {
+  auto op = [](const cc_slice& s, int ns) {
+    cc_operand o{};
+    o.s = s; o.type = s.f32 ? CC_OP_F32 : CC_OP_BF16; o.ns = ns;
+    return o;
+  };
+  cc_op_io io{};
+  io.in[io.n_in++] = op(c.in, 0);
+  if (c.res.p) io.in[io.n_in++] = op(c.res, c.out_ns);
+  if (c.pre) io.in[io.n_in++] = op(cc_slice{const_cast<float*>(c.pre), c.out.C, 0, c.out.C, c.out.N, c.pre_h, c.pre_w, 1}, 0);
+  if (c.part.p) io.in[io.n_in++] = op(c.part, 0);
+  if (c.out.p && (c.kind != CC_CONV_OP_CHAIN || c.store1)) io.out[io.n_out++] = op(c.out, c.out_ns);
+  if (c.kind == CC_CONV_OP_CHAIN) io.out[io.n_out++] = op(c.out2, 0);
+  return io;
+}
+
+PlanOp plan_op(const std::string& name, const char* kind, const cc_op_io& io, PlanOp::Launch launch, double flops, double bytes) {
   PlanOp op;
-  op.name = intern(name); op.kind = kind; op.flops = flops; op.bytes = bytes; op.launch = std::move(launch);
+  op.name = intern(name); op.kind = kind; op.io = io; op.flops = flops; op.bytes = bytes; op.launch = std::move(launch);
   return op;
 }
 
 PlanOp gemm_op(const std::string& name, const ConvDesc& d, const ChainDesc& c, const GemmLaunch& L) {
-  PlanOp op = plan_op(name, "conv_gemm", [L](const PlanIO& io, cudaStream_t st) {
+  const cc_conv_op conv = conv_op_of(d, c, L);
+  PlanOp op = plan_op(name, "conv_gemm", conv_io(conv), [L](const PlanIO& io, cudaStream_t st) {
     if (!io.trace) return conv_gemm_launch(L, st);
     GemmLaunch g = L;
     g.p.trace = io.trace;
     return conv_gemm_launch(g, st);
   }, L.flops, L.bytes);
-  op.conv = conv_op_of(d, c, L);
+  op.conv = conv;
   return op;
 }
 
@@ -69,6 +109,16 @@ int op_conv_tap(const char* who, const std::vector<PlanOp>& ops, int i, cc_conv_
   if (!out) return n;
   CC_REQUIRE(i >= 0 && i < n, "%s: op %d of a plan of %d ops", who, i, n);
   *out = ops[i].conv;
+  snprintf(out->name, sizeof(out->name), "%s", ops[i].name);
+  return n;
+}
+
+int op_io_tap(const char* who, const std::vector<PlanOp>& ops, int i, cc_op_io* out) {
+  const int n = static_cast<int>(ops.size());
+  if (!out) return n;
+  CC_REQUIRE(i >= 0 && i < n, "%s: op %d of a plan of %d ops", who, i, n);
+  *out = ops[i].io;
+  snprintf(out->kind, sizeof(out->kind), "%s", ops[i].kind);
   snprintf(out->name, sizeof(out->name), "%s", ops[i].name);
   return n;
 }

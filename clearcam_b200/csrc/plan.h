@@ -3,6 +3,7 @@
 #include "cc_common.h"
 #include "conv_gemm.cuh"
 #include <functional>
+#include <initializer_list>
 
 namespace cc {
 
@@ -22,11 +23,22 @@ struct PlanOp {
   const char* kind = "";                 // the kernel, as the profile and trace report it ("conv_gemm", "avgpool2_pad", ...)
   double flops = 0, bytes = 0;           // algorithmic FLOPs and HBM bytes the profile reports
   cc_conv_op conv{};                     // what the cc_*_op_conv taps report (name left empty); CC_CONV_OP_NONE: not a conv
+  cc_op_io io{};                         // what the cc_*_op_io taps report (kind and name left empty); the launch never reads it
   Launch launch;
 };
 
+// Operands of a cc_op_io: a slice with its extent (bf16 or f32 as s.f32 says), or a buffer of `type` elements.  ns: elements
+// from one image to the next (0: dense).
+cc_operand operand(const TSlice& s, int N, int H, int W, int ns = 0);
+inline cc_operand operand(const TSlice& s) { return operand(s, s.N, s.H, s.W); }
+cc_operand operand(const void* p, int type, int N, int H, int W, int C, int cs = 0, int co = 0, int ns = 0);
+cc_op_io op_io(std::initializer_list<cc_operand> in, std::initializer_list<cc_operand> out);
+
 const char* intern(const std::string& s);   // a copy of s that lives as long as the process
-PlanOp plan_op(const std::string& name, const char* kind, PlanOp::Launch launch, double flops = 0, double bytes = 0);
+PlanOp plan_op(const std::string& name, const char* kind, const cc_op_io& io, PlanOp::Launch launch, double flops = 0,
+               double bytes = 0);
+// The operands of a conv op (the cc_op_io of cc_conv_op c)
+cc_op_io conv_io(const cc_conv_op& c);
 // A conv GEMM launch L built from d (and the chained 1x1 c, if c.out.p): FLOPs and bytes are L's.
 PlanOp gemm_op(const std::string& name, const ConvDesc& d, const ChainDesc& c, const GemmLaunch& L);
 
@@ -39,6 +51,8 @@ int profile_ops(const std::vector<PlanOp>& ops, const PlanIO& io, cudaStream_t s
                 const char** kinds, const char** names);
 // The cc_*_op_conv taps: op i's conv with its name; returns the op count (out == NULL only counts).
 int op_conv_tap(const char* who, const std::vector<PlanOp>& ops, int i, cc_conv_op* out);
+// The cc_*_op_io taps: op i's operands with its kind and name; returns the op count (out == NULL only counts).
+int op_io_tap(const char* who, const std::vector<PlanOp>& ops, int i, cc_op_io* out);
 // The cc_*_run_ops range check.
 int check_range(const char* who, int first, int last, int n);
 // The layer taps: slice s (N x H x W pixels) -> dense fp32 [N*H*W][C].

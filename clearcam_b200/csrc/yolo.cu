@@ -374,7 +374,8 @@ static double slice_bytes(const TSlice& t) { return double(t.N) * t.H * t.W * t.
 // the weight planes hi|mid|lo|hi|mid); a last pass applies bias, the exact SiLU and the residual and writes the output slice.
 static int precise_conv_ops(const std::string& key, const ConvW& cw, const TSlice& in, int stride, int act, __nv_bfloat16* scratch,
                             float* accbuf, const TSlice& out, const TSlice* res, int sms, std::vector<PlanOp>* ops, double* conv_flops) {
-  ops->push_back(plan_op(key + ".split", "split_planes", [in, scratch](const PlanIO&, cudaStream_t st) {
+  ops->push_back(plan_op(key + ".split", "split_planes", op_io({operand(in)}, {operand(scratch, CC_OP_BF16, in.N, in.H, in.W, 6 * in.C)}),
+                         [in, scratch](const PlanIO&, cudaStream_t st) {
     return split_planes_launch(in, scratch, st);
   }));
   const int Ho = conv_out(in.H, stride), Wo = conv_out(in.W, stride);
@@ -394,7 +395,11 @@ static int precise_conv_ops(const std::string& key, const ConvW& cw, const TSlic
   f.acc = accbuf; f.bias = cw.bias; f.act = act; f.npix = static_cast<long long>(in.N) * Ho * Wo; f.C = cw.cout;
   f.out = reinterpret_cast<float*>(out.p); f.out_cs = out.cs; f.out_co = out.co;
   if (res) { f.res = reinterpret_cast<const float*>(res->p); f.res_cs = res->cs; f.res_co = res->co; }
-  ops->push_back(plan_op(key, "finish_f32", [f](const PlanIO&, cudaStream_t st) { return finish_f32_launch(f, st); }));
+  cc_op_io io = op_io({operand(accbuf, CC_OP_F32, in.N, Ho, Wo, cw.cout), operand(cw.bias, CC_OP_F32, 1, 1, 1, cw.cout)},
+                      {operand(out, in.N, Ho, Wo)});
+  if (res) io.in[io.n_in++] = operand(*res, in.N, Ho, Wo);
+  io.act = act;
+  ops->push_back(plan_op(key, "finish_f32", io, [f](const PlanIO&, cudaStream_t st) { return finish_f32_launch(f, st); }));
   return CC_OK;
 }
 // The two first convs of a detect-head scale read the same input and are fused into one conv of 64 + d output channels —
@@ -480,8 +485,9 @@ struct Builder {
     } else {   // the direct kernel's FLOPs count in conv_flops; its op reports none
       const DirectConvParams p = direct_conv_params(d, cw.groups);
       P.conv_flops += 2.0 * P.B * p.Hout * p.Wout * cw.cout * (cw.cin / cw.groups) * cw.k * cw.k;
-      PlanOp op = plan_op(key, "conv_direct", [p](const PlanIO&, cudaStream_t st) { return conv_direct_launch(p, st); });
-      op.conv = conv_op_of(p);
+      const cc_conv_op c = conv_op_of(p);
+      PlanOp op = plan_op(key, "conv_direct", conv_io(c), [p](const PlanIO&, cudaStream_t st) { return conv_direct_launch(p, st); });
+      op.conv = c;
       P.ops.push_back(std::move(op));
     }
   }
@@ -522,7 +528,7 @@ struct Builder {
   void simple(const char* kind, int (*launch)(const TSlice&, const TSlice&, cudaStream_t), const TSlice& in, const TSlice& out,
               const char* name) {
     if (rc || bump.dry) return;
-    P.ops.push_back(plan_op(name, kind, [launch, in, out](const PlanIO&, cudaStream_t st) { return launch(in, out, st); }, 0,
+    P.ops.push_back(plan_op(name, kind, op_io({operand(in)}, {operand(out)}), [launch, in, out](const PlanIO&, cudaStream_t st) { return launch(in, out, st); }, 0,
                             slice_bytes(in) + slice_bytes(out)));
   }
 
@@ -647,7 +653,10 @@ int Builder::build() {
       lb.sx = g.sx; lb.sy = g.sy;
       const double in_px = lb.fmt == CC_FRAME_BGR_F32 ? 12.0 : lb.fmt == CC_FRAME_I420_U8 ? 1.5 : 3.0;   // bytes per pixel
       const double bytes = double(lb.B) * (double(lb.Hin) * lb.Win * in_px + double(lb.Hout) * lb.Wout * 3 * (lb.fmt == CC_FRAME_BGR_F32 ? 4 : 1));
-      P.ops.push_back(plan_op("letterbox", "letterbox", [lb](const PlanIO& io, cudaStream_t st) {
+      const int in_type = lb.fmt == CC_FRAME_BGR_F32 ? CC_OP_F32 : CC_OP_U8;
+      const cc_operand frames = lb.fmt == CC_FRAME_I420_U8 ? operand(nullptr, CC_OP_U8, lb.B, lb.Hin * 3 / 2, lb.Win, 1)
+                                                           : operand(nullptr, in_type, lb.B, lb.Hin, lb.Win, 3);
+      P.ops.push_back(plan_op("letterbox", "letterbox", op_io({frames}, {operand(lb.out, in_type, lb.B, lb.Hout, lb.Wout, 3)}), [lb](const PlanIO& io, cudaStream_t st) {
         LetterboxParams q = lb;
         q.in = io.in;
         return letterbox_launch(q, st);
@@ -677,6 +686,10 @@ int Builder::build() {
           out = out_for(i, l.b, in.H / 2, in.W / 2);
           const ConvW& cw = M.convs[pfx];
           if (bump.dry) break;
+          // the stems read the letterbox's output, or the call's frames (net_in == nullptr)
+          const cc_op_io stem_io = op_io({operand(net_in, f32 ? CC_OP_F32 : CC_OP_U8, P.B, P.H, P.W, 3),
+                                          operand(cw.wf32, CC_OP_F32, 1, 1, cw.cout, 27), operand(cw.bias, CC_OP_F32, 1, 1, 1, cw.cout)},
+                                         {operand(out)});
           if (!f32 && !M.precise && (cw.cout == 16 || cw.cout == 32 || cw.cout == 64)) {
             // uint8 frames: raw pixel values are exact in bf16, weights bf16(w/255); stem_tc_kernel gathers the A tile from
             // the frame itself
@@ -685,7 +698,7 @@ int Builder::build() {
             if (rc) break;
             const double flops = 2.0 * P.B * (P.H / 2) * (P.W / 2) * cw.cout * 27;
             P.conv_flops += flops;
-            P.ops.push_back(plan_op(pfx, "stem_tc", [tc, net_in](const PlanIO& io, cudaStream_t st) {
+            P.ops.push_back(plan_op(pfx, "stem_tc", stem_io, [tc, net_in](const PlanIO& io, cudaStream_t st) {
               return stem_tc_launch(tc, static_cast<const uint8_t*>(net_in ? net_in : io.in), st);
             }, flops, double(tc.B) * tc.H * tc.W * 3 + double(tc.Mrows) * tc.Cout * 2));
             break;
@@ -695,7 +708,7 @@ int Builder::build() {
           sp.in = net_in; sp.is_f32 = f32; sp.B = P.B; sp.H = P.H; sp.W = P.W;
           sp.w = cw.wf32; sp.bias = cw.bias; sp.Cout = cw.cout; sp.out = out;
           P.conv_flops += 2.0 * P.B * (P.H / 2) * (P.W / 2) * cw.cout * 27;
-          P.ops.push_back(plan_op(pfx, "stem", [sp](const PlanIO& io, cudaStream_t st) {
+          P.ops.push_back(plan_op(pfx, "stem", stem_io, [sp](const PlanIO& io, cudaStream_t st) {
             StemParams q = sp;
             if (!q.in) q.in = io.in;
             return stem_launch(q, st);
@@ -789,7 +802,7 @@ int Builder::build() {
         conv(pfx + ".cv1", in, slice(cat, 0, c1), 1, CC_ACT_SILU);
         if (spp3_supported(cat, c1)) {
           if (!rc && !bump.dry)
-            P.ops.push_back(plan_op("spp.max5x3", "spp3", [cat, c1](const PlanIO&, cudaStream_t st) { return spp3_launch(cat, c1, st); }, 0,
+            P.ops.push_back(plan_op("spp.max5x3", "spp3", op_io({operand(slice(cat, 0, c1))}, {operand(slice(cat, c1, 3 * c1))}), [cat, c1](const PlanIO&, cudaStream_t st) { return spp3_launch(cat, c1, st); }, 0,
                                     4.0 * cat.N * cat.H * cat.W * c1 * 2));
         } else {
           for (int q = 0; q < 3; ++q) simple("maxpool5", maxpool5_launch, slice(cat, q * c1, c1), slice(cat, (q + 1) * c1, c1), "spp.max5");
@@ -842,7 +855,10 @@ int Builder::build() {
         cbf.last = last; cbf.out = out;
         double bytes = slice_bytes(cbf.last) + slice_bytes(cbf.out);
         for (int q = 0; q < cbf.nsrc; ++q) bytes += slice_bytes(cbf.src[q]);
-        P.ops.push_back(plan_op(pfx, "cbfuse", [cbf](const PlanIO&, cudaStream_t st) { return cbfuse_launch(cbf, st); }, 0, bytes));
+        cc_op_io io = op_io({}, {operand(cbf.out)});
+        for (int q = 0; q < cbf.nsrc; ++q) io.in[io.n_in++] = operand(cbf.src[q]);
+        io.in[io.n_in++] = operand(cbf.last);
+        P.ops.push_back(plan_op(pfx, "cbfuse", io, [cbf](const PlanIO&, cudaStream_t st) { return cbfuse_launch(cbf, st); }, 0, bytes));
         break;
       }
       case L_DETECT: {
@@ -876,7 +892,11 @@ int Builder::build() {
         P.pred = static_cast<float*>(dalloc(static_cast<size_t>(P.B) * A * 6 * 4));
         dec.B = P.B; dec.A = A; dec.conf_thr = 0.25f; dec.pred = P.pred; dec.raw = nullptr;
         if (bump.dry) break;
-        P.ops.push_back(plan_op("decode", "decode", [dec](const PlanIO& io, cudaStream_t st) {
+        cc_op_io dio = op_io({}, {operand(P.pred, CC_OP_F32, P.B, 1, A, 6), operand(nullptr, CC_OP_F32, P.B, 84, A, 1)});
+        for (int q = 0; q < 3; ++q) dio.in[dio.n_in++] = operand(dec.box[q], CC_OP_F32, P.B, dec.h[q], dec.w[q], 64);
+        for (int q = 0; q < 3; ++q) dio.in[dio.n_in++] = operand(dec.cls[q], CC_OP_F32, P.B, dec.h[q], dec.w[q], 80);
+        dio.conf_thr = dec.conf_thr;
+        P.ops.push_back(plan_op("decode", "decode", dio, [dec](const PlanIO& io, cudaStream_t st) {
           DecodeParams q = dec;
           q.raw = io.raw;
           return decode_launch(q, st);
@@ -886,7 +906,11 @@ int Builder::build() {
         post.pred = P.pred; post.B = P.B; post.A = A; post.max_det = 300; post.iou_thr = 0.45f;
         post.scale = g.scale; post.do_scale = 1;
         post.out = nullptr;
-        P.ops.push_back(plan_op("postprocess", "postprocess", [post](const PlanIO& io, cudaStream_t st) {
+        cc_op_io pio = op_io({operand(P.pred, CC_OP_F32, P.B, 1, A, 6)}, {operand(nullptr, CC_OP_F32, P.B, 1, post.max_det, 6)});
+        pio.max_det = post.max_det; pio.iou_thr = post.iou_thr; pio.do_scale = post.do_scale;
+        pio.pad_x = post.scale.pad_x; pio.pad_y = post.scale.pad_y; pio.gain = post.scale.gain;
+        pio.clip_w = post.scale.clip_w; pio.clip_h = post.scale.clip_h;
+        P.ops.push_back(plan_op("postprocess", "postprocess", pio, [post](const PlanIO& io, cudaStream_t st) {
           PostParams q = post;
           q.out = io.out;
           return postprocess_launch(q, st);
@@ -1281,6 +1305,14 @@ int cc_yolo_op_conv(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, i
   YoloPlan* P = nullptr;
   if (int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P)) return rc;
   return op_conv_tap("cc_yolo_op_conv", P->ops, i, out);
+}
+
+int cc_yolo_op_io(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int i, cc_op_io* out) {
+  CC_REQUIRE(h, "cc_yolo_op_io: null handle");
+  if (int rc = check_frame_fmt("cc_yolo_op_io", frame_fmt, Hf, Wf)) return rc;
+  YoloPlan* P = nullptr;
+  if (int rc = get_plan(h, frame_fmt, B, Hf, Wf, res, &P)) return rc;
+  return op_io_tap("cc_yolo_op_io", P->ops, i, out);
 }
 
 int cc_yolo_run_ops(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, int first, int last,

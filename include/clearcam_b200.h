@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define CC_ABI_VERSION 4
+#define CC_ABI_VERSION 5
 
 int cc_version(void);
 const char* cc_last_error(void);
@@ -193,6 +193,57 @@ int cc_yolo_trace(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf
  * cc_yolo_run_ops launches ops [first, last) of that plan on `stream` exactly as a forward launches them, without a CUDA
  * graph; d_frames, d_out and d_raw are a cc_yolo_forward call's.  Nothing synchronises. */
 int cc_yolo_op_conv(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int i, cc_conv_op* out);
+/* Operand taps, for tests that check every launch of a plan in place: what op i of a plan reads and writes, for every op,
+ * convs included.  Each operand is a slice of type cc_slice, whose f32 field mirrors type == CC_OP_F32, with an element type and ns, the
+ * elements ("pixels") from one image to the next (0: dense, H * W).  A row-major matrix of R rows of C values per image is
+ * N images of H = 1, W = R pixels of cs values.  An operand with p == NULL is the call's own input (frames, images, token ids,
+ * faces), output or raw tap, with its extent filled in (an output's cs is its row width; the call picks the row stride).
+ * Operand order per kind (in: what the op reads; out: what it writes; [x]: only when present):
+ *   conv_gemm, conv_direct  in: in, [res], [pre], [part]   out: [out] (a stored first output), [out2] (a chained 1x1)
+ *                           (the weights are in the cc_*_op_conv descriptor of the same op)
+ *   letterbox          in: frames (u8 [B,Hf,Wf,3], f32 for CC_FRAME_BGR_F32, u8 [B,Hf*3/2,Wf,1] for I420)  out: net input
+ *   stem, stem_tc      in: net input (the letterbox's output, or the call's frames), w (f32 [Cout][3][3][3], (kh, kw, RGB)
+ *                      order, before any packing), bias (f32 [Cout])   out: the first map
+ *   avgpool2_pad, avgmax_pool, maxpool5, upsample2   in: in   out: out
+ *   spp3               in: channels [co, co + c1) of the concat buffer   out: channels [co + c1, co + 4 c1)
+ *   cbfuse             in: src_0 .. src_{n-1}, last   out: out
+ *   split_planes       in: in (f32)   out: the dense bf16 planes [N,H,W][6C]
+ *   finish_f32         in: acc (dense f32), bias, [res]   out: out.  Scalar: act
+ *   decode             in: box_0..2 (f32 [B,h,w,64]), cls_0..2 (f32 [B,h,w,80])   out: pred (f32 [B,1,A,6]), raw tap
+ *                      (p NULL, f32 [B,84,A,1]).  Scalar: conf_thr
+ *   postprocess        in: pred   out: detections (p NULL, f32 [B,1,max_det,6]).  Scalars: max_det, iou_thr, scale_boxes'
+ *                      pad_x, pad_y, gain, clip_w, clip_h (do_scale = 0: none)
+ *   patchify           in: images (p NULL, f32 [B,3,S,S] as [B,3S,S,1])   out: patches (bf16 [B,1,Pn,Kpad]).  Scalar: patch
+ *   embed_ln_pre       in: stream (f32 [B,1,L,W]), cls (f32 [1,1,1,W]), pos ([1,1,L,W]), gamma, beta ([W])   out: stream
+ *   text_embed         in: ids (p NULL, i32 [B,1,L,1]), tok ([1,1,vocab,W]), pos ([1,1,L,W])   out: stream (f32 [B,1,L,W]),
+ *                      EOT rows (i32 [B,1,1,1]: b * L + the EOT's position)
+ *   layernorm          in: x, gamma, beta, [row index (i32 [B,1,1,1])]   out: bf16 rows.  x is the rows read: every row of
+ *                      the stream ([B,1,L,W]), token 0 of each image ([B,1,1,W], ns = L), or with a row index the whole stream
+ *   attention          in: qkv (bf16 [B,1,L,3*heads*64])   out: ctx (bf16 [B,1,L,heads*64]), [the wgmma kernel's V^T
+ *                      scratch (bf16 [B,heads*64,Lpad,1])].  Scalar: causal
+ *   l2norm             in: embeddings (f32 [B,1,1,D])   out: the call's output rows (p NULL, [B,1,1,D]).  Scalar: eps
+ *   face_pack          in: faces (p NULL, u8 [B,112,112,3])   out: bf16 [B,112,112,16] (channels 3..15 zero)
+ * Same contract as cc_yolo_op_conv: the op count, out == NULL only counts, an i outside [0, count) fails. */
+#define CC_OP_U8 0
+#define CC_OP_BF16 1
+#define CC_OP_F32 2
+#define CC_OP_I32 3
+#define CC_OP_IO_MAX 8
+typedef struct { cc_slice s; int type; int ns; } cc_operand;
+typedef struct {
+  char kind[32];
+  char name[128];
+  int n_in, n_out;
+  cc_operand in[CC_OP_IO_MAX], out[CC_OP_IO_MAX];
+  int causal;                                  /* attention */
+  float eps;                                   /* l2norm */
+  float conf_thr;                              /* decode */
+  int max_det; float iou_thr;                  /* postprocess */
+  int do_scale; float pad_x, pad_y, gain, clip_w, clip_h;
+  int act;                                     /* finish_f32 */
+  int patch;                                   /* patchify */
+} cc_op_io;
+int cc_yolo_op_io(cc_yolo* h, int frame_fmt, int B, int Hf, int Wf, int res, int i, cc_op_io* out);
 int cc_yolo_run_ops(cc_yolo* h, const void* d_frames, int frame_fmt, int B, int Hf, int Wf, int res, int first, int last,
                     float* d_out, float* d_raw, void* stream);
 
@@ -337,6 +388,8 @@ int cc_clip_profile(cc_clip* h, int text, const void* d_in, int B, float* d_out,
  * as an encode launches them; d_in, d_out and out_row_stride are those of cc_clip_encode_image / cc_clip_encode_text.
  * Nothing synchronises. */
 int cc_clip_op_conv(cc_clip* h, int text, int B, int i, cc_conv_op* out);
+/* The operand tap of the CLIP plans (cc_yolo_op_io). */
+int cc_clip_op_io(cc_clip* h, int text, int B, int i, cc_op_io* out);
 int cc_clip_run_ops(cc_clip* h, int text, const void* d_in, int B, int first, int last, float* d_out, long long out_row_stride,
                     void* stream);
 /* ---- AdaFace IR-50 face embedder (replaces class ADAFACE, models/adaface.py:24-96) ---- */
@@ -366,6 +419,8 @@ int cc_face_layer_output(cc_face* h, const uint8_t* d_faces, int B, int layer, f
  * H = 1, W = B over the 7x7x512 map as one row per face) and "l2norm".  d_faces and d_out are those of cc_face_embed
  * (d_out rows of 512 floats). */
 int cc_face_op_conv(cc_face* h, int B, int i, cc_conv_op* out);
+/* The operand tap of the face plans (cc_yolo_op_io). */
+int cc_face_op_io(cc_face* h, int B, int i, cc_op_io* out);
 int cc_face_run_ops(cc_face* h, const uint8_t* d_faces, int B, int first, int last, float* d_out, void* stream);
 
 /* ---- BlazeFace face detector (replaces class BlazeFace, models/blazeface.py:62-232), fp32 ---- */

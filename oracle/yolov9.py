@@ -450,8 +450,12 @@ def postprocess(output, max_det=300, conf_threshold=0.25, iou_threshold=0.45):
     probs, class_ids = cls.max(1)               # torch.max returns the first maximal index like argmax
     class_ids = cls.argmax(1)
     probs = torch.where(probs >= conf_threshold, probs, torch.zeros_like(probs))
-    boxes = torch.stack([x1, y1, x2, y2, probs, class_ids.float()], 2)
-    order = torch.sort(probs, dim=1, descending=True, stable=True)[1][:, :max_det]
+    return postprocess_boxes(torch.stack([x1, y1, x2, y2, probs, class_ids.float()], 2), max_det, iou_threshold)
+
+
+def postprocess_boxes(boxes, max_det=300, iou_threshold=0.45):
+    """The selection half of postprocess: (B,A,6) [x1,y1,x2,y2,conf (0 below the threshold),class] -> (B,max_det,6)."""
+    order = torch.sort(boxes[..., 4], dim=1, descending=True, stable=True)[1][:, :max_det]
     boxes = torch.gather(boxes, 1, order.unsqueeze(-1).expand(-1, -1, 6))
     ious = torch.triu(compute_iou_matrix(boxes[:, :, :4]), diagonal=1)
     cid = boxes[:, :, -1]

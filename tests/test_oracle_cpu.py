@@ -131,7 +131,7 @@ def test_clip_oracle_shapes_and_norms():
 
 
 # ------------------------------------------------------------------------------------------------ C-ABI surface
-def test_library_exports_every_declared_symbol_of_abi_4():
+def test_library_exports_every_declared_symbol_of_abi_5():
     from clearcam_b200._lib import lib, declared_symbols, LIB_PATH
     hdr = open(os.path.join(ROOT, "include", "clearcam_b200.h")).read()
     declared = set(re.findall(r"\b(cc_[a-z0-9_]+)\s*\(", hdr))
@@ -140,7 +140,7 @@ def test_library_exports_every_declared_symbol_of_abi_4():
     for name in sorted(declared):
         assert hasattr(h, name), f"{name} declared in include/clearcam_b200.h but not exported"
     assert declared == set(declared_symbols()), "ctypes signature table out of sync with the header"
-    assert lib().cc_version() == 4
+    assert lib().cc_version() == 5
 
 
 def test_product_path_fails_loudly_without_gpu():

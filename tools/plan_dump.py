@@ -1,6 +1,7 @@
 """What the detector, CLIP and face plans of this build are made of, as text two builds can be diffed on (CC_LIB selects the
 library, as in tools/ab.py): per op its kind, name, algorithmic FLOPs and bytes; the detector trace's kind, name and FLOPs per
-op; every op's conv descriptor (cc_*_op_conv: each non-pointer field, and whether each pointer is NULL); the plan facts; and
+op; every op's conv descriptor (cc_*_op_conv: each non-pointer field, and whether each pointer is NULL) and operands
+(cc_*_op_io, likewise; the lines of an older build without that tap are missing, the others unchanged); the plan facts; and
 a SHA-256 of what a forward returns on seeded frames.  A host-side change to how plans are built or run must leave every
 line as it was.
 
@@ -24,7 +25,7 @@ from oracle import adaface as oa  # noqa: E402
 from oracle import blazeface as obf  # noqa: E402
 from oracle import clip as oc  # noqa: E402
 from oracle import yolov9 as o  # noqa: E402
-from clearcam_b200._lib import cc_conv_op, check, lib  # noqa: E402
+from clearcam_b200._lib import cc_conv_op, cc_op_io, check, lib  # noqa: E402
 from clearcam_b200.detection.yolov9 import YOLOv9  # noqa: E402
 from clearcam_b200.models.adaface import ADAFACE  # noqa: E402
 from clearcam_b200.models.blazeface import BlazeFace  # noqa: E402
@@ -67,6 +68,27 @@ def op_convs(say, tag, op_conv):
         say(tag, "conv", i, fields(d))
 
 
+def io_fields(d):
+    """A cc_op_io as text: its scalars, then the n_in / n_out operands it reports (the unused slots left out)."""
+    head = " ".join(f"{n}={getattr(d, n).decode() if n in ('kind', 'name') else getattr(d, n)}" for n, _ in d._fields_
+                    if n not in ("in_", "out"))
+    return " ".join([head] + [f"in{k}({fields(d.in_[k])})" for k in range(d.n_in)] + [f"out{k}({fields(d.out[k])})" for k in range(d.n_out)])
+
+
+def op_ios(say, tag, op_io):
+    """Every op's cc_op_io of a plan; op_io(i, out) is the cc_*_op_io call with the plan's arguments bound (nothing from a
+    build without the tap)."""
+    try:
+        n = op_io(0, None)
+    except AttributeError:
+        return
+    check(min(n, 0), "op_io")
+    for i in range(n):
+        d = cc_op_io()
+        check(min(op_io(i, ctypes.byref(d)), 0), "op_io")
+        say(tag, "io", i, io_fields(d))
+
+
 def main():
     out = open(sys.argv[1], "w")
     say = lambda *a: print(*a, file=out, flush=True)     # noqa: E731
@@ -84,6 +106,7 @@ def main():
             for r in m.trace(fr):
                 say(tag, "trace", r["kind"], r["name"], repr(r["flops"]))
             op_convs(say, tag, lambda i, d: lib().cc_yolo_op_conv(m._h, 0, B, H, W, m.res, i, d))
+            op_ios(say, tag, lambda i, d: lib().cc_yolo_op_io(m._h, 0, B, H, W, m.res, i, d))
             det, raw = m.detect_batch(fr, raw=True)
             say(tag, "outputs", sha(det, raw))
             if size == "c" and H == 1080 and not precise:       # frame-table plan: bgr24 1080p and yuv420p 720p share a net shape
@@ -107,12 +130,14 @@ def main():
             nb = B if tower == "image" else ids.shape[0]
             op_convs(say, f"clip {arch} {tower} B{nb}",
                      lambda i, d: lib().cc_clip_op_conv(cm._h, int(tower == "text"), nb, i, d))
+            op_ios(say, f"clip {arch} {tower} B{nb}", lambda i, d: lib().cc_clip_op_io(cm._h, int(tower == "text"), nb, i, d))
         say("clip", arch, "outputs", sha(cm.precompute_embedding(x).tensor, cm.encode_token_ids(ids).tensor))
         del cm
     fm = ADAFACE(oa.synthetic_weights(seed=5))
     for B in (1, 3, 16, 64, 200):
         say("adaface", f"B{B}", "outputs", sha(fm.embed(oa.synthetic_faces(B, seed=B))))
         op_convs(say, f"adaface B{batch_bucket(B)}", lambda i, d: lib().cc_face_op_conv(fm._h, batch_bucket(B), i, d))
+        op_ios(say, f"adaface B{batch_bucket(B)}", lambda i, d: lib().cc_face_op_io(fm._h, batch_bucket(B), i, d))
     del fm
     det = BlazeFace({k: v.numpy() for k, v in obf.load_weights(os.path.join(ROOT, "tests", "golden", "blazeface_ref.npz")).items()})
     sizes = [(256, 256), (640, 640), (480, 640), (97, 300), (333, 129), (720, 1280), (1080, 1920)]
