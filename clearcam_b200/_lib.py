@@ -173,8 +173,11 @@ _SIGS = {
     "cc_blazeface_set_workspace": (_i, [_vp, _vp, ctypes.c_size_t]),
     "cc_blazeface_forward": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "cc_blazeface_decode": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    "cc_blazeface_first": (_i, [_vp, _i, _vp, _vp]),
     "cc_face_canvas": (_i, [_vp, _i, _vp, _vp]),
     "cc_face_align": (_i, [_vp, _i, _vp, _vp]),
+    "cc_face_canvas_slots": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
+    "cc_face_align_slots": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "cc_search_scores": (_i, [_vp, _i, _i, _vp, _i, _vp, _vp]),
     "cc_search_topk": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "cc_clip_preprocess_frames": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp]),

@@ -14,8 +14,9 @@ picks and new-object flags (clearcam_b200/events.py), on the GPU right after the
 device rows and by `ObjectEvents` for host rows, and returns run_inference's preds.  `step_alerts` goes on to decide the
 camera's alerts (clearcam_b200/alerts.py: the adds of :612-620, the object counter and the firing loop of :465-499), on
 the GPU right after the events (csrc/alerts_gpu.cu) for device rows and by `CameraAlerts` for host rows, and
-`describe_saves` runs the description alerts of clip_latest_img (:1289-1307) on `save_objects`' embeddings; what a fired
-alert then does (image, notification, upload) and the saving of the picked crops stay with the caller.
+`describe_saves` runs the description alerts of clip_latest_img (:1289-1307) on `save_objects`' embeddings, and
+`save_objects_and_faces` adds the faces of the person saves (process_latest_face, :1228-1241); what a fired alert then
+does (image, notification, upload) and the writing of the thumbnails, faces and embeddings stay with the caller.
 
 Each camera has a pixel format (clearcam_b200/pixfmt.py): "bgr24" [H,W,3] frames (the default) or "yuv420p" [H*3/2,W]
 frames, which the detector converts on the GPU, or "mjpeg": one JPEG file per frame (bytes-like, e.g. a JpegMailbox
@@ -506,8 +507,20 @@ class CameraBatch:
         order (embeddings None when CLIP is not initialised, or when the camera has no saves).  A run's saves are (m,7):
         the frame index in the run, then the six save columns, frame after frame.  A step without saves makes no library
         call.  Reads the device frames of the last step, so it is valid until the next step."""
+        return self._save(results, finder, quality, False)[0]
+
+    def save_objects_and_faces(self, results: Dict[Hashable, CameraEvents], finder, quality: int = 95):
+        """`save_objects` and the faces of its person saves in the same ONE call (`process_latest_face`, clearcam.py:272-279,
+        1228-1241: a save of class 0, the reference's "_0.jpg" name) -> (saved, faces): saved is exactly what save_objects
+        returns; faces is {camera: FaceSaves} (ObjectFinder.encode_embed_faces_frames) whose rows index the camera's saves
+        ((n,6) for a step, (m,7) for a run), or None per camera when the finder's face leg is off.  A camera without saves
+        gets an empty FaceSaves with embeddings None.  A step without saves makes no library call."""
+        return self._save(results, finder, quality, True)
+
+    def _save(self, results, finder, quality, faces):
         # (camera, frame key, saves): a step's result is one frame; a step_video result (a list) one per frame of the run,
         # whose saves are returned with their frame index in front
+        from .models.objects import FaceSaves
         srcs, out = [], {}
         for name, ev in results.items():
             if isinstance(ev, list):
@@ -520,12 +533,18 @@ class CameraBatch:
                 if len(ev.saves):
                     srcs.append((name, name, ev.saves))
                 out[name] = (ev.saves, [], None)
+        face = {name: (FaceSaves([], [], None) if finder.face else None) for name in out} if faces else None
         if not srcs:
-            return out
+            return out, face
         frames = [self.device_frame(key) for _, key, _ in srcs]
         rects = np.concatenate([np.concatenate([np.full((len(sv), 1), j, np.int64), np.asarray(sv, np.int64)[:, 2:6]], 1)
                                 for j, (_, _, sv) in enumerate(srcs)]).astype(np.int32)
-        files, emb = finder.encode_embed_frames(frames, [self._device_fmt(name) for name, _, _ in srcs], rects, quality)
+        fmts = [self._device_fmt(name) for name, _, _ in srcs]
+        if faces:
+            person = np.concatenate([np.asarray(sv, np.int64)[:, 1] == 0 for _, _, sv in srcs])     # class 0: a "_0.jpg" save
+            files, emb, fs = finder.encode_embed_faces_frames(frames, fmts, rects, person, quality)
+        else:
+            files, emb = finder.encode_embed_frames(frames, fmts, rects, quality)
         from .detection.yolov9 import DeviceResult
         k, first = 0, {}
         for name, _, sv in srcs:
@@ -534,7 +553,11 @@ class CameraBatch:
         for name, k0 in first.items():
             n = len(out[name][0])
             out[name] = (out[name][0], files[k0:k0 + n], None if emb is None else DeviceResult(emb.tensor[k0:k0 + n]))
-        return out
+            if faces and fs is not None:
+                j = [i for i, r in enumerate(fs.rows) if k0 <= r < k0 + n]
+                face[name] = FaceSaves([fs.rows[i] - k0 for i in j], [fs.files[i] for i in j],
+                                       DeviceResult(fs.embeddings.tensor[j[0]:j[0] + len(j)] if j else fs.embeddings.tensor[:0]))
+        return out, face
 
     def step_mailboxes(self, mailboxes: Dict[Hashable, "FrameMailbox"]) -> Dict[Hashable, CameraResult]:
         """`step` on every camera whose mailbox (clearcam_b200.ingest) holds a frame this object has not seen yet —

@@ -250,6 +250,23 @@ __global__ void __launch_bounds__(1024) blaze_decode_kernel(const float* __restr
   }
 }
 
+// One CTA per image: the first row of dets [896][17] whose column 0 != 0 as numpy compares it (-0.0 is zero, NaN is not),
+// copied bit for bit, or a zero row.  The host geometry of img_to_face reads only that row (models/objects.py:283-284).
+__global__ void __launch_bounds__(128) blaze_first_kernel(const float* __restrict__ dets, float* __restrict__ first) {
+  __shared__ int s_first;
+  if (threadIdx.x == 0) s_first = kAnchors;
+  __syncthreads();
+  const float* d = dets + static_cast<long long>(blockIdx.x) * kAnchors * kDet;
+  int mine = kAnchors;
+  for (int i = threadIdx.x; i < kAnchors; i += blockDim.x)
+    if (d[i * kDet] != 0.f) { mine = i; break; }                  // unordered !=: true for NaN
+  if (mine < kAnchors) atomicMin(&s_first, mine);
+  __syncthreads();
+  const int r = s_first;
+  if (threadIdx.x < kDet)
+    first[static_cast<long long>(blockIdx.x) * kDet + threadIdx.x] = r < kAnchors ? d[r * kDet + threadIdx.x] : 0.f;
+}
+
 // the letterbox geometry of BlazeFace.__call__ (:155-165) for an h x w image
 struct Fit { double scale; int new_w, new_h, top, left; };
 static Fit fit(int h, int w) {
@@ -396,6 +413,13 @@ int cc_blazeface_decode(cc_blazeface* h, const float* d_boxes, const float* d_sc
                h_sizes[2 * b]);
   }
   return decode_launch(h->m.anchors, d_boxes, d_scores, h_sizes, B, d_dets, static_cast<cudaStream_t>(stream));
+}
+
+int cc_blazeface_first(const float* d_dets, int B, float* d_first, void* stream) {
+  CC_REQUIRE(d_dets && d_first && B > 0, "cc_blazeface_first: bad argument (dets %p, B = %d, first %p)", d_dets, B, d_first);
+  blaze_first_kernel<<<B, 128, 0, static_cast<cudaStream_t>(stream)>>>(d_dets, d_first);
+  CC_CHECK_CUDA(cudaGetLastError());
+  return CC_OK;
 }
 
 int cc_blazeface_forward(cc_blazeface* h, const cc_frame* frames, int B, float* d_boxes, float* d_scores, float* d_dets,

@@ -4,6 +4,7 @@
     det = BlazeFace(weights)                 # state dict, .safetensors path, or None for the reference's models/blazeface.safetensors
     rows = det(img).numpy()                  # img: HWC uint8 -> (896,17) [ymin, xmin, ymax, xmax, 6 keypoints (x, y), score]
     dets = det.detect(images)                # many images of any sizes -> device [B,896,17], row b = det(images[b])
+    first = first_detections(dets)           # device [B,17]: the one row img_to_face reads per image
 
 The network, the decode and the suppression run in fp32 in libclearcam_b200.so (csrc/blazeface.cu); there is no CPU
 fallback.
@@ -178,18 +179,67 @@ def face_geometry(detections: np.ndarray, h: int, w: int):
     return x1_crop, y1_crop, x2_crop, y2_crop, rot_mat, new_w, new_h, transform_mat
 
 
+def _warps(jobs):
+    """jobs: (image pointer or None, h, w, face_geometry result) per face -> a cc_face_warp table."""
+    table = (cc_face_warp * len(jobs))()
+    for k, (src, h, w, (x1, y1, x2, y2, rot, nw, nh, tm)) in enumerate(jobs):
+        f = table[k]
+        f.src, f.h, f.w = src, h, w
+        f.x1, f.y1, f.x2, f.y2, f.rot_w, f.rot_h = x1, y1, x2, y2, nw, nh
+        f.rot[:] = [float(v) for v in np.asarray(rot, np.float64).ravel()]
+        f.transform[:] = [float(v) for v in np.asarray(tm, np.float32).astype(np.float64).ravel()]
+    return table
+
+
 def align_faces(jobs) -> torch.Tensor:
     """jobs: (device uint8 [h,w,3] image, face_geometry result) pairs -> device uint8 [K,112,112,3] in one launch: face k is
     exactly the reference's two cv2.warpAffine calls and RGB2BGR on its image."""
     out = torch.empty(len(jobs), FACE, FACE, 3, dtype=torch.uint8, device="cuda")
     if not jobs:
         return out
-    table = (cc_face_warp * len(jobs))()
-    for k, (t, (x1, y1, x2, y2, rot, nw, nh, tm)) in enumerate(jobs):
-        f = table[k]
-        f.src, f.h, f.w = t.data_ptr(), t.shape[0], t.shape[1]
-        f.x1, f.y1, f.x2, f.y2, f.rot_w, f.rot_h = x1, y1, x2, y2, nw, nh
-        f.rot[:] = [float(v) for v in np.asarray(rot, np.float64).ravel()]
-        f.transform[:] = [float(v) for v in np.asarray(tm, np.float32).astype(np.float64).ravel()]
+    table = _warps([(t.data_ptr(), t.shape[0], t.shape[1], g) for t, g in jobs])
     check(lib().cc_face_align(table, len(jobs), ptr(out), stream_ptr()), "cc_face_align")
+    return out
+
+
+# ---- the same on the images of a padded BGR batch [n,Hmax,Wmax,3] (image k in the h x w corner of its slot), as the device
+# JPEG decoders write them: each slot is read as the RGB image cv2.cvtColor(slot, BGR2RGB) that img_to_face receives
+def _slots(slots, index):
+    assert slots.is_cuda and slots.dtype == torch.uint8 and slots.is_contiguous() and slots.dim() == 4 and slots.shape[3] == 3
+    return (ptr(slots), *slots.shape[:3], np.ascontiguousarray(index, np.int32))
+
+
+def face_canvas_slots(slots, index, sizes, rows=None) -> torch.Tensor:
+    """The canvas of image b: the (height, width) = sizes[b] corner of slots[index[b]] -> device uint8 [max(rows, B),640,640,3]
+    in one launch; canvas b equals `face_canvas` of the contiguous RGB copy of that image, and rows past B are zero (batch
+    padding)."""
+    B = len(index)
+    out = torch.empty(max(rows or B, B), 640, 640, 3, dtype=torch.uint8, device="cuda")
+    out[B:].zero_()
+    p, n, H, W, idx = _slots(slots, index)
+    hw = np.ascontiguousarray(np.asarray(sizes, np.int32).reshape(-1, 2))
+    check(lib().cc_face_canvas_slots(p, n, H, W, idx.ctypes.data, hw.ctypes.data, B, ptr(out), stream_ptr()), "cc_face_canvas_slots")
+    return out
+
+
+def align_faces_slots(slots, jobs) -> torch.Tensor:
+    """jobs: (slot, (height, width), face_geometry result) -> device uint8 [K,112,112,3] in one launch: face k equals
+    `align_faces` on the contiguous RGB copy of its image."""
+    out = torch.empty(len(jobs), FACE, FACE, 3, dtype=torch.uint8, device="cuda")
+    if not jobs:
+        return out
+    p, n, H, W, idx = _slots(slots, [s for s, _, _ in jobs])
+    table = _warps([(None, h, w, g) for _, (h, w), g in jobs])
+    check(lib().cc_face_align_slots(p, n, H, W, idx.ctypes.data, table, len(jobs), ptr(out), stream_ptr()), "cc_face_align_slots")
+    return out
+
+
+def first_detections(dets) -> torch.Tensor:
+    """Device dets [B,896,17] -> device [B,17]: row b is detections[detections[:, 0] != 0][0] of image b (models/objects.py:
+    283-284), or zeros where no row is kept; `face_geometry` of that one row is that of all 896."""
+    d = dets.contiguous()
+    B = d.shape[0]
+    out = torch.empty(B, COORDS + 1, device="cuda", dtype=torch.float32)
+    if B:
+        check(lib().cc_blazeface_first(ptr(d), B, ptr(out), stream_ptr()), "cc_blazeface_first")
     return out

@@ -9,8 +9,9 @@
 Mirrors class OpenCLIP (/root/reference/models/objects.py:21-143), encode_text (:145-186) and ObjectFinder's CLIP
 methods (:189-206, :237-251, :356-421), and the face embedder's (`init_face`, `turn_off_face`, `adaface`,
 `preprocess_face` for 112x112 faces, face search; :207-217, :253-261) and the BlazeFace face detector (`blazeface`,
-models/blazeface.py) with face alignment (`img_to_face`, :263-354, and the batched `faces_from_images`).  All
-arithmetic runs in libclearcam_b200.so; there is no CPU fallback.
+models/blazeface.py) with face alignment (`img_to_face`, :263-354, and the batched `faces_from_images`), and the
+faces of object saves (`encode_embed_faces_frames`, clearcam.py:1228-1241) and of uploads (`embed_face_images`,
+clearcam.py:671-678).  All arithmetic runs in libclearcam_b200.so; there is no CPU fallback.
 
 Additions: `arch=` (the reference hard-codes ViT-L/14; "ViT-B/32" runs the same kernels), explicit `weights=`
 (the reference downloads from HuggingFace, :91), `encode_text_batch`, a contiguous device index for search, and
@@ -21,7 +22,7 @@ from __future__ import annotations
 import ctypes
 import os
 import pickle
-from typing import Dict, List, Optional
+from typing import Dict, List, NamedTuple, Optional
 
 import numpy as np
 import torch
@@ -178,6 +179,13 @@ def _device_crops(frames, rects, bgr: bool, pix_fmt: str):
     return t, ops.batch_table(t, fmt), np.ascontiguousarray(r, np.int32)
 
 
+class FaceSaves(NamedTuple):
+    """The faces of a batch of object saves (`process_latest_face`, clearcam.py:1228-1241)."""
+    rows: List[int]                         # the saves whose img_to_face found a face, in save order
+    files: List[bytes]                      # each face's JPEG, as cv2.imwrite writes the 112x112 BGR face
+    embeddings: Optional[DeviceResult]      # (f,512): row j is adaface(face j)
+
+
 class ObjectFinder:
     """CLIP half of the reference's ObjectFinder (models/objects.py:188-206, 237-251, 356-421)."""
 
@@ -238,8 +246,8 @@ class ObjectFinder:
 
     def preprocess_face(self, img):
         """models/objects.py:253-261: an uploaded file (bytes) or a stored path under data/cameras -> the RGB image when it is
-        already a 112x112 face.  Other sizes raise: the reference routes them through `img_to_face` (see that method), which
-        this does not do yet."""
+        already a 112x112 face.  Other sizes raise: the reference routes them through `img_to_face`, which
+        `embed_face_images` does for a batch of uploads."""
         import cv2
         if type(img) == bytes:
             img = cv2.imdecode(np.frombuffer(img, np.uint8), cv2.IMREAD_COLOR)
@@ -256,20 +264,44 @@ class ObjectFinder:
         call receives them) -> (device uint8 [K,112,112,3], rows): rows[i] is the index of image i's face in the batch, or
         None where `img_to_face(images[i])` returns None.  One canvas launch, one BlazeFace forward, one read of the
         detections for the host geometry, one alignment launch; the faces go to `embed_faces` without leaving the device."""
-        from .blazeface import _images, align_faces, face_canvas, face_geometry
-        if self.blazeface is None:
-            raise CCError("face detection is off: init_face(detector=...) builds BlazeFace from its weights, or from the "
-                          "reference's models/blazeface.safetensors when that file exists")
+        from .blazeface import _images, align_faces, face_canvas, face_geometry, first_detections
+        self._need_detector()
         ims = _images(images)
         canvas = face_canvas(ims)
-        dets = self.blazeface.detect(canvas).cpu().numpy()                # the host geometry needs the rows
+        first = first_detections(self.blazeface.detect(canvas)).cpu().numpy()      # the host geometry needs one row per image
         jobs, rows = [], []
         for i, t in enumerate(ims):
-            g = face_geometry(dets[i], t.shape[0], t.shape[1])
+            g = face_geometry(first[i:i + 1], t.shape[0], t.shape[1])
             rows.append(None if g is None else len(jobs))
             if g is not None:
                 jobs.append((t, g))
         return align_faces(jobs), rows
+
+    def _need_detector(self):
+        if self.blazeface is None:
+            raise CCError("face detection is off: init_face(detector=...) builds BlazeFace from its weights, or from the "
+                          "reference's models/blazeface.safetensors when that file exists")
+
+    def _queue_first(self, slots, index, sizes):
+        """Queue img_to_face's detection for the (height, width) corners of slots[index] of a padded BGR batch, each read
+        as its RGB image: canvas, BlazeFace on a batch padded to batch_bucket, first kept row -> device [len(index),17]."""
+        from .blazeface import face_canvas_slots, first_detections
+        n = len(index)
+        canvas = face_canvas_slots(slots, index, sizes, rows=batch_bucket(n))
+        return first_detections(self.blazeface.detect(canvas)[:n])
+
+    @staticmethod
+    def _align_slots(slots, index, sizes, first):
+        """The rest of img_to_face for those images, given their first rows on the host: the reference's geometry on the
+        host, then one alignment launch -> (device uint8 [f,112,112,3] BGR faces, per image its face's row or None)."""
+        from .blazeface import align_faces_slots, face_geometry
+        jobs, rows = [], []
+        for i, (slot, hw) in enumerate(zip(index, sizes)):
+            g = face_geometry(first[i:i + 1], *hw)
+            rows.append(None if g is None else len(jobs))
+            if g is not None:
+                jobs.append((slot, hw, g))
+        return align_faces_slots(slots, jobs), rows
 
     def img_to_face(self, orig):
         """models/objects.py:263-354: an HWC uint8 image -> the aligned 112x112 face (numpy uint8, BGR order as the
@@ -354,10 +386,21 @@ class ObjectFinder:
         cropped, resized and normalised by cc_clip_preprocess_frames and embedded in one batch.  A file the device reports as
         unsupported or corrupt is decoded by cv2 on the host and joins the same batch; where cv2 returns None this raises as
         the reference's cvtColor does."""
-        import cv2
         k = len(items)
         if k == 0:
             return DeviceResult(torch.empty(0, self.model.embed_dim, device="cuda", dtype=torch.float32))
+        out, sizes = self._decode_items(items)
+        rects = [(i, 0, 0, w, h) for i, (w, h) in enumerate(sizes)]
+        x = self.preprocess_device(out, rects, bgr=True, rows=batch_bucket(k))
+        return DeviceResult(self.model.precompute_embedding(x).tensor[:k])
+
+    @staticmethod
+    def _decode_items(items):
+        """Uploaded files (`bytes`) or paths relative to data/cameras -> (device uint8 [k,Hmax,Wmax,3], image i in the
+        top-left corner of slot i as cv2.imdecode gives it, [(w, h)] per image).  The device decodes what it can
+        (ops.JpegBatch); a file it reports as unsupported or corrupt is decoded by cv2 on the host and copied into its slot;
+        where cv2 returns None this raises as the reference's cvtColor does."""
+        import cv2
         files = []
         for it in items:
             if type(it) == bytes:
@@ -388,9 +431,43 @@ class ObjectFinder:
             host_decode(int(i))
         for i, img in host.items():
             out[i, :img.shape[0], :img.shape[1]] = torch.from_numpy(img).to(out.device)
-        rects = [(i, 0, 0, w, h) for i, (w, h) in enumerate(sizes)]
-        x = self.preprocess_device(out, rects, bgr=True, rows=batch_bucket(k))
-        return DeviceResult(self.model.precompute_embedding(x).tensor[:k])
+        return out, sizes
+
+    def embed_face_images(self, items):
+        """The batched `run_clip(..., is_face=True)` face embedding (clearcam.py:671-678: preprocess_face, then adaface):
+        items are `bytes` (an uploaded file) or the reference's paths relative to data/cameras -> (DeviceResult (n,512), rows):
+        rows[i] is item i's row, or None where the reference's img_to_face finds no face (run_clip then returns no hits).
+        The files are decoded as in `embed_images`.  A 112x112 image is embedded as the RGB image preprocess_face returns
+        it; any other size goes through img_to_face on the device-decoded batch (canvas, BlazeFace, one read of the first
+        detections for the host geometry, alignment), and all faces are embedded in one batch."""
+        if self.adaface is None:
+            raise CCError("the face embedder is off: call init_face() first")
+        if not len(items):
+            return DeviceResult(torch.empty(0, 512, device="cuda", dtype=torch.float32)), []
+        out, sizes = self._decode_items(items)
+        other = [i for i, wh in enumerate(sizes) if wh != (112, 112)]
+        hw = [(sizes[i][1], sizes[i][0]) for i in other]
+        aligned, arow = None, {}
+        if other:
+            self._need_detector()
+            aligned, got = self._align_slots(out, other, hw, self._queue_first(out, other, hw).cpu().numpy())
+            arow = dict(zip(other, got))
+        rows, pick = [], []                                  # pick: (aligned face row) or (-1 - slot of a 112x112 image)
+        for i in range(len(items)):
+            r = arow.get(i, -1 - i)
+            rows.append(None if r is None else len(pick))
+            if r is not None:
+                pick.append(r)
+        if not pick:
+            return DeviceResult(torch.empty(0, 512, device="cuda", dtype=torch.float32)), rows
+        faces = torch.empty(len(pick), 112, 112, 3, dtype=torch.uint8, device="cuda")
+        at = [j for j, r in enumerate(pick) if r >= 0]
+        if at:
+            faces[at] = aligned[[pick[j] for j in at]]
+        at = [j for j, r in enumerate(pick) if r < 0]
+        if at:                                               # preprocess_face's cvtColor(BGR2RGB) of a 112x112 upload
+            faces[at] = out[[-1 - pick[j] for j in at], :112, :112].flip(-1)
+        return DeviceResult(self.adaface.embed(faces)), rows
 
     def encode_embed_crops(self, frames, rects, quality: int = 95, bgr: bool = True, pix_fmt: str = BGR24):
         """Detector frame -> (the JPEG file of each object crop, exactly as `encode_crops` returns them, and DeviceResult
@@ -402,7 +479,7 @@ class ObjectFinder:
         if not 0 <= int(quality) <= 100:
             raise ValueError(f"quality must be in 0..100 (cv2's range), got {quality}")
         t, table, r = _device_crops(frames, rects, bgr, pix_fmt)
-        return self._encode_embed(table, r, quality)
+        return self._encode_embed(table, r, quality)[:2]
 
     def encode_embed_frames(self, frames, pix_fmts, rects, quality: int = 95):
         """`encode_embed_crops` for the objects of many frames of different shapes and formats in one call (the saves of
@@ -420,31 +497,85 @@ class ObjectFinder:
         if not 0 <= int(quality) <= 100:
             raise ValueError(f"quality must be in 0..100 (cv2's range), got {quality}")
         table, sizes = ops.frame_table(frames, pix_fmts)
-        return self._encode_embed(table, ops.table_rects(rects, sizes), quality)
+        return self._encode_embed(table, ops.table_rects(rects, sizes), quality)[:2]
 
-    def _encode_embed(self, table, r, quality):
+    def encode_embed_faces_frames(self, frames, pix_fmts, rects, person, quality: int = 95):
+        """`encode_embed_frames` and the faces of the person saves among the crops in the same call (`process_latest_face`,
+        clearcam.py:1228-1241, on the thumbnail that save_object wrote and the queue read back as RGB): person is one bool per
+        rect -> (files, embeddings, faces).  files and embeddings are exactly what `encode_embed_frames` returns; faces is a
+        FaceSaves: the rects whose img_to_face finds a face, each face's JPEG as cv2.imwrite writes it at `quality`, and
+        DeviceResult (f,512) of adaface(face); None when the face leg is off (`face` false).  Raises CCError before anything
+        is queued when the face leg is on without a detector.
+        The crops-decoded pixels (ops.jpeg_crops_decoded_frames) feed both legs.  Queued before the first read: the encoder,
+        the decoded pixels, the CLIP preprocess and forward, and over the person crops the face canvas, BlazeFace and the
+        first kept detection.  The host then waits once for the thumbnails' lengths, the decode statuses and the first rows
+        together, runs the reference's face geometry, and queues the alignment, the faces' encoder and the AdaFace batch;
+        it waits a second time for the thumbnails' bytes and the faces' lengths, and a third for the faces' bytes, whatever
+        the number of frames, saves or faces.  A crop whose coefficients the device leaves to cv2 is decoded from its file on
+        the host as in `encode_embed_frames`, and its face detection is run again (more waits, at very low qualities only)."""
+        if not 0 <= int(quality) <= 100:
+            raise ValueError(f"quality must be in 0..100 (cv2's range), got {quality}")
+        table, sizes = ops.frame_table(frames, pix_fmts)
+        r = ops.table_rects(rects, sizes)
+        person = np.asarray(person, bool).reshape(-1)
+        if len(person) != len(r):
+            raise ValueError(f"{len(person)} person flags for {len(r)} rects")
+        if self.face:
+            self._need_detector()
+        return self._encode_embed(table, r, quality, person if self.face else None)
+
+    def _encode_embed(self, table, r, quality, person=None):
+        """-> (files, CLIP embeddings or None, FaceSaves or None); person: None (no face leg) or one bool per rect."""
         K = len(r)
+        persons = [] if person is None else [int(i) for i in np.flatnonzero(person)]
+        none = lambda dim: DeviceResult(torch.empty(0, dim, device="cuda", dtype=torch.float32))   # noqa: E731
+        no_faces = None if person is None else FaceSaves([], [], none(512))
         if K == 0:
-            return [], (None if self.model is None else
-                        DeviceResult(torch.empty(0, self.model.embed_dim, device="cuda", dtype=torch.float32)))
+            return [], (None if self.model is None else none(self.model.embed_dim)), no_faces
         out, lengths, offsets = ops.jpeg_encode_crops_frames(table, r, quality)
-        if self.model is None:
-            return ops.jpeg_collect(out, lengths, offsets), None
+        if self.model is None and not persons:
+            return ops.jpeg_collect(out, lengths, offsets), None, no_faces
         pix, status = ops.jpeg_crops_decoded_frames(table, r, quality)
         crops = [(i, 0, 0, int(x2 - x1), int(y2 - y1)) for i, (_, x1, y1, x2, y2) in enumerate(r)]
-        x = self.preprocess_device(pix, crops, bgr=True, rows=batch_bucket(K)).tensor
-        emb = self.model.precompute_embedding(x).tensor
-        got = torch.cat([lengths, status.long()]).cpu().numpy()                 # host wait 1
-        files = ops.jpeg_collect(out, lengths, offsets, got[:K])                # host wait 2
-        bad = [int(i) for i in np.flatnonzero(got[K:] != ops.JPEG_OK)]
+        hw = [(int(y2 - y1), int(x2 - x1)) for _, x1, y1, x2, y2 in r]
+        x = emb = None
+        if self.model is not None:
+            x = self.preprocess_device(pix, crops, bgr=True, rows=batch_bucket(K)).tensor
+            emb = self.model.precompute_embedding(x).tensor
+        first = self._queue_first(pix, persons, [hw[i] for i in persons]) if persons else torch.empty(0, 17, device="cuda")
+        lens, st, first = ops.read_together(lengths, status, first)                # host wait 1
+        thumbs = ops.jpeg_gather(out, lengths, offsets, lens)
+        files = None
+        bad = [int(i) for i in np.flatnonzero(st != ops.JPEG_OK)]
         if bad:
             import cv2                                  # coefficients outside the range every libjpeg-turbo IDCT agrees on
+            files = ops.jpeg_split(thumbs.cpu().numpy(), lens)
             for i in bad:
                 img = cv2.imdecode(np.frombuffer(files[i], np.uint8), cv2.IMREAD_COLOR)
                 pix[i, :img.shape[0], :img.shape[1]] = torch.from_numpy(img).to(pix.device)
-            x[torch.tensor(bad, device=x.device)] = self.preprocess_device(pix, [crops[i] for i in bad], bgr=True).tensor
-            emb = self.model.precompute_embedding(x).tensor
-        return files, DeviceResult(emb[:K])
+            if x is not None:
+                x[torch.tensor(bad, device=x.device)] = self.preprocess_device(pix, [crops[i] for i in bad], bgr=True).tensor
+                emb = self.model.precompute_embedding(x).tensor
+            redo = [j for j, i in enumerate(persons) if i in bad]
+            if redo:
+                first[redo] = self._queue_first(pix, [persons[j] for j in redo], [hw[persons[j]] for j in redo]).cpu().numpy()
+        emb = None if emb is None else DeviceResult(emb[:K])
+        if person is None:
+            return (ops.jpeg_split(thumbs.cpu().numpy(), lens) if files is None else files), emb, None  # host wait 2
+        faces, got = self._align_slots(pix, persons, [hw[i] for i in persons], first)
+        rows = [i for i, g in zip(persons, got) if g is not None]
+        if not rows:
+            return (ops.jpeg_split(thumbs.cpu().numpy(), lens) if files is None else files), emb, no_faces
+        from ..pixfmt import CC_FRAME_BGR_U8
+        fout, flengths, foffsets = ops.jpeg_encode_crops_frames(ops.batch_table(faces, CC_FRAME_BGR_U8),
+                                                                [(j, 0, 0, 112, 112) for j in range(len(rows))], quality)
+        femb = DeviceResult(self.adaface.embed(faces))
+        if files is None:
+            flat, flens = ops.read_together(thumbs, flengths)                    # host wait 2
+            files = ops.jpeg_split(flat, lens)
+        else:
+            flens = flengths.cpu().numpy()
+        return files, emb, FaceSaves(rows, ops.jpeg_collect(fout, flengths, foffsets, flens), femb)   # host wait 3
 
     def _device_index(self, is_face=False):
         """Contiguous device copy of `image_embeddings` (`face_embeddings` when is_face) plus, per row, what `search`

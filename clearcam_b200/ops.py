@@ -351,16 +351,38 @@ def jpeg_collect(out, lengths, offsets, lens=None):
     """The files of `jpeg_encode_crops_frames`' (out, lengths, offsets) as a list of K `bytes`: the used bytes of every crop
     gathered into one device run, one copy to the host.  lens: the lengths already on the host, or None to fetch them
     (a second host wait)."""
-    import numpy as np
-    dev = out.device
     lens = lengths.cpu().numpy() if lens is None else lens
+    return jpeg_split(jpeg_gather(out, lengths, offsets, lens).cpu().numpy(), lens)
+
+
+def jpeg_gather(out, lengths, offsets, lens):
+    """Queue the gather of the used bytes of every crop (lens: the lengths on the host) into one device run; nothing
+    waits.  `jpeg_split` cuts its host copy into the files."""
+    dev = out.device
     total = int(lens.sum())
     starts = torch.cumsum(lengths, 0) - lengths
     idx = torch.arange(total, device=dev) + torch.repeat_interleave(torch.from_numpy(offsets).to(dev) - starts, lengths,
                                                                      output_size=total)
-    flat = out[idx].cpu().numpy().tobytes()
+    return out[idx]
+
+
+def jpeg_split(flat, lens):
+    """The host copy of a `jpeg_gather` run (uint8 numpy) -> the list of files."""
+    import numpy as np
+    flat = flat.tobytes()
     ends = np.cumsum(lens)
     return [flat[e - l:e] for e, l in zip(ends, lens)]
+
+
+def read_together(*tensors):
+    """Device tensors -> numpy copies of each, through one device-to-host copy (one host wait)."""
+    flat = torch.cat([t.contiguous().reshape(-1).view(torch.uint8) for t in tensors]).cpu().numpy()
+    out, o = [], 0
+    for t in tensors:
+        n = t.numel() * t.element_size()
+        out.append(flat[o:o + n].copy().view(torch.empty(0, dtype=t.dtype).numpy().dtype).reshape(t.shape))
+        o += n
+    return out
 
 
 def jpeg_coeffs_frames(table, rects, quality=95, stream=None):

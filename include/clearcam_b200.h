@@ -447,6 +447,10 @@ int cc_blazeface_forward(cc_blazeface* h, const cc_frame* frames, int B, float* 
  * d_scores [B,896]; h_sizes: host int32 [B][2] (height, width) of the images they stand for. */
 int cc_blazeface_decode(cc_blazeface* h, const float* d_boxes, const float* d_scores, int B, const int32_t* h_sizes, float* d_dets,
                         void* stream);
+/* The detection img_to_face uses (models/objects.py:283-284, detections[detections[:, 0] != 0][0]) for B images at once:
+ * d_first [B,17] gets, for each image, the first row of d_dets [B,896,17] whose column 0 != 0 as numpy compares it (-0.0
+ * counts as zero, NaN as non-zero), bit for bit, or a zero row when there is none.  Works on any B >= 1. */
+int cc_blazeface_first(const float* d_dets, int B, float* d_first, void* stream);
 
 /* ---- img_to_face's image arithmetic (models/objects.py:263-354), byte for byte with cv2 ---- */
 /* The pre-resize of B images: frames[b] a device uint8 [h,w,3] image (CC_FRAME_BGR_U8, channels used as given) ->
@@ -465,6 +469,18 @@ typedef struct {
  * transform, (112, 112)), COLOR_RGB2BGR), pixel for pixel.  A crop outside its image fails with CC_ERR_INVALID before
  * anything is launched. */
 int cc_face_align(const cc_face_warp* faces, int K, uint8_t* d_out, void* stream);
+/* The same two operations on the images of a padded batch, as the device JPEG decoders write them (cc_jpeg_decode_frames,
+ * cc_jpeg_crops_decoded_frames): d_slots uint8 [n_slots, Hmax, Wmax, 3], image k in the h x w corner of slot h_slot[k]
+ * (host int32 [K]), rows Wmax * 3 bytes apart, slots Hmax * Wmax * 3 bytes apart.  The slots hold BGR pixels (cv2.imread,
+ * cv2.imdecode); each is read as the RGB image cv2.cvtColor(slot, COLOR_BGR2RGB) that img_to_face receives
+ * (clearcam.py:1228-1241, 671-678), so result k equals cc_face_canvas / cc_face_align on that contiguous RGB copy, byte for
+ * byte.  Canvas: h_sizes host int32 [B][2] (height, width).  Align: faces[k].src is not read; faces[k].h and .w are the image's
+ * size within its slot.  Bad arguments (NULL pointers, B or K < 1, a slot index outside the batch, an image larger than a
+ * slot, a crop outside its image) fail with CC_ERR_INVALID before anything is launched. */
+int cc_face_canvas_slots(const uint8_t* d_slots, int n_slots, int Hmax, int Wmax, const int32_t* h_slot, const int32_t* h_sizes,
+                         int B, uint8_t* d_out, void* stream);
+int cc_face_align_slots(const uint8_t* d_slots, int n_slots, int Hmax, int Wmax, const int32_t* h_slot, const cc_face_warp* faces,
+                        int K, uint8_t* d_out, void* stream);
 
 /* ObjectFinder.search inner loop (models/objects.py:365-376): d_scores[q*N + n] = <d_index[n,:], d_q[q,:]>, fp32. */
 int cc_search_scores(const float* d_index, int N, int D, const float* d_q, int Q, float* d_scores, void* stream);
